@@ -1,10 +1,11 @@
 #!/usr/bin/env python
 """Benchmark of the stage-2 (SoVITS + HiFi-GAN) train step -- BASELINE.json's metric.
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path (N>1: launched by torchrun)
+  python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path (N>1: launched by torchrun)
   python bench.py --impl reference --steps K --warmup W    # the reference's algorithm on the host CPU cores (oracle port)
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's results as DIR/<name>.npy
 
-One "step" = everything in /root/reference/src/train/sovits.py:438-525 for one batch of 16 x 10 s utterances:
+One "step" = everything in the reference's src/train/sovits.py:438-525 for one batch of 16 x 10 s utterances:
 G forward, mel features + slicing, D forward/backward/AdamW, D forward again, G backward/AdamW.
 `value` is device-timed with the batch resident in HBM; `e2e` adds, every step, the pinned-host -> device copy of the
 step's inputs (wav, ssl features, phonemes, lengths), the on-GPU |X| feature extraction the reference does in CPU
@@ -36,11 +37,11 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d["hbm_gbs"], d["bf16_tflops"], d.get("bf16_tflops_sustained", d["bf16_tflops"]), "measured"
-    return 6650.0, 1590.0, 1400.0, "fallback"
+    return 3350.0, 989.0, 989.0, "H100 SXM data sheet (dense; not a measured rate)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks/throttle reasons every 200 ms during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons every 200 ms during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -128,12 +129,12 @@ def cpu_reference_step(Bc, T, threads, steps, warmup, budget_s=None):
 
 
 def torch_gpu_port_step(dev, T, amp, steps=5):
-    """The reference's algorithm through STOCK PyTorch kernels (cuDNN / cuBLAS / cuFFT / ATen) on the same B200, B = 16,
+    """The reference's algorithm through STOCK PyTorch kernels (cuDNN / cuBLAS / cuFFT / ATen) on the same GPU, B = 16,
     whole optimisation step (two torch.optim.AdamW updates): the oracle port moved to the GPU.
       amp=False: fp32 storage, TF32 allowed exactly as the reference sets it (sovits.py:172-176);
       amp=True : the reference's AS-SHIPPED regime (configs/s2.json fp16_run: true): torch.autocast(float16) around the
                  networks, losses in fp32, GradScaler on both optimizers (sovits.py:378,459-525).
-    The reference package itself cannot travel to the GPU box (see DESIGN.md: pip install of /root/reference fails), so its
+    The reference package itself is not installed next to this one, so its
     restated algorithm stands in for it; this is the 'reference 1-GPU PyTorch step' of BASELINE.json's >= 10x target."""
     import torch
     from oracle import s2_oracle, mel_oracle
@@ -196,8 +197,8 @@ def torch_gpu_port_step(dev, T, amp, steps=5):
 
 def run_reference(args):
     """`--impl reference`: the reference's CPU path for the same workload / config / metric.  The reference package cannot be
-    installed into baseline/_ref (DESIGN.md section 2), so the arm runs its restated algorithm (oracle port, kind "port") on
-    the box's host cores at the FULL benchmark batch (16 x 10 s), whole optimisation step.  Rank 0 only."""
+    installed next to this one, so the arm runs its restated algorithm (oracle port, kind "port") on
+    the host's CPU cores at the FULL benchmark batch (16 x 10 s), whole optimisation step.  Rank 0 only."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return 0
@@ -223,7 +224,7 @@ def workload_config(sr_label, world):
     T = frames_for(sr_label)
     return dict(workload=f"s2_step_B{B_PER_GPU}x{UTT_SECONDS:.0f}s_sr{sr_label}_T{T}", global_batch=world * B_PER_GPU, frames=T,
                 segment=20480, text_len=TEXT_LEN, parallelism=f"dp{world}", weights="random-init seed 1234",
-                l2="params+optimizer state+activations touched per step (>2 GB) far exceed the 126 MB L2; no explicit flush")
+                l2="params+optimizer state+activations touched per step (>2 GB) far exceed the 50 MB L2 of an H100; no explicit flush")
 
 
 # --------------------------------------------------------------------------------------------------
@@ -279,14 +280,28 @@ def kernel_table(ops, dev):
     return rows
 
 
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel`, from the ncu --set full capture committed under
-    profiles/ (tools/sum_launches.py --traffic writes the JSON); None when no capture of this build exists."""
-    p = os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")
-    try:
-        return json.load(open(p)).get(kernel, {}).get("dram_bytes_per_launch")
-    except (OSError, ValueError):
-        return None
+def dump_outputs(dirpath, arrays):
+    """--dump-outputs: one DIR/<name>.npy per array (float32 / float64 only), so that two builds run with the same arguments
+    can be compared output for output."""
+    import numpy as np
+    os.makedirs(dirpath, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        total += a.nbytes
+        np.save(os.path.join(dirpath, name + ".npy"), a)
+    assert total <= 64 * 2**20, total
+
+
+def param_sample(params, n=1 << 20, seed=0):
+    """A fixed, seeded sample of n elements of the concatenated parameters (all of them when there are fewer)."""
+    import torch
+    flat = torch.cat([p_.detach().reshape(-1).float() for p_ in params])
+    if flat.numel() <= n:
+        return flat.cpu().numpy()
+    idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(seed))[:n].sort().values
+    return flat[idx.to(flat.device)].cpu().numpy()
 
 
 def trace(msg):
@@ -383,6 +398,13 @@ def run_ours(args):
     ms = timed(step_resident, args.steps)
     trace(f"timed region done {ms:.1f} ms")
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        # the last timed step's losses and the parameters it left behind (seeded sample of each network)
+        import numpy as np
+        arrays = {f"loss_{k}": np.asarray([float(v)], dtype=np.float64) for k, v in last.items() if k != "host"}
+        arrays["net_g_params_sample"] = param_sample(net_g.parameters())
+        arrays["net_d_params_sample"] = param_sample(net_d.parameters())
+        dump_outputs(args.dump_outputs, arrays)
     for _ in range(2):
         step_e2e()
     ms_e2e = timed(step_e2e, args.steps)
@@ -415,19 +437,17 @@ def run_ours(args):
         all_fl = sum(v["flops"] for v in prof.values())
         ach = tma_fl / (tma_ms * 1e-3) / 1e12
         table = kernel_table(ops, dev)
-        traffic = ncu_traffic("gemm_tma_kernel")
         top = sorted(prof.items(), key=lambda kv: -kv[1]["ms"])[:14]
-        extra["roofline"] = dict(bound="tensor", kernel="gemm_tma_kernel (TMA-fed persistent tcgen05 TF32 GEMM / implicit-GEMM conv: forward, data-gradient, "
+        extra["roofline"] = dict(bound="tensor", kernel="gemm_tma_kernel (TMA-fed persistent wgmma TF32 GEMM / implicit-GEMM conv: forward, data-gradient, "
                                                         "ConvTranspose-phase, strided-phase and weight-gradient launches)",
-                                 achieved=ach, peak=tf_sus, unit="TFLOP/s", frac=ach / tf_sus, traffic=traffic,
+                                 achieved=ach, peak=tf_sus, unit="TFLOP/s", frac=ach / tf_sus,
                                  flops_per_step=tma_fl, ms_per_step=tma_ms, launches_per_step=sum(prof[k]["calls"] for k in tma_keys),
                                  share_of_step_time=tma_ms / all_ms, share_of_step_flops=tma_fl / all_fl,
                                  step_tflops=all_fl / (ms * 1e-3) / 1e12,
-                                 peak_source=f"{src} cuBLAS bf16 sustained; the kernel computes in TF32 whose nominal peak is half of bf16",
+                                 peak_source=f"{src} bf16; the kernel computes in TF32 whose nominal peak is half of bf16",
                                  how="achieved = analytic flops of EVERY gemm_tma launch of one training step / the sum of their CUDA-event durations "
                                      "(events recorded on the launching stream around each call of an eager step run behind a 30 ms spin kernel so the host stays ahead, single stream, same process, after the timed region); "
-                                     "share_of_step_time is against the event time of all library calls of that step (torch fill/add/copy kernels excluded); "
-                                     "traffic = dram read+write bytes per launch of the heaviest layer from the committed ncu capture (profiles/r2_ncu_traffic.json), null if absent",
+                                     "share_of_step_time is against the event time of all library calls of that step (torch fill/add/copy kernels excluded)",
                                  by_call={k: dict(calls=v["calls"], ms=round(v["ms"], 3), tflops=(round(v["flops"] / (v["ms"] * 1e-3) / 1e12, 1) if v["flops"] else None))
                                           for k, v in top},
                                  layers=[{k: (round(v, 4) if isinstance(v, float) else v) for k, v in r.items()} for r in table])
@@ -462,12 +482,11 @@ def run_ours(args):
         del bigw
         extra["mel_roofline"] = dict(bound="hbm", kernel="mel_fwd_warp_kernel (|X| + log-mel emitted)", achieved=big_gbs, peak=hbm,
                                      unit="GB/s", frac=big_gbs / hbm, frames=big_frames, ms=big_ms, peak_source=src,
-                                     traffic=ncu_traffic("mel_fwd"),
                                      how="one launch over 256 x 10 s (graph replay, 226 MB in + 408 MB out > L2)",
                                      batch16=dict(achieved=gbs, frac=gbs / hbm, frames=frames, ms=mel_ms,
                                                   how=f"{nset * reps} back-to-back launches of the training batch (16 x 10 s) over {nset} rotating buffer sets"),
                                      mel_only=dict(achieved=only_gbs, frac=only_gbs / hbm, ms=only_ms,
-                                                   note="log-mel only (3 072 B/frame): FFT-arithmetic bound on the fp32 pipe, see DESIGN.md section 6"))
+                                                   note="log-mel only (3 072 B/frame): FFT-arithmetic bound on the fp32 pipe"))
         line = dict(metric=METRIC, value=audio_s / (ms * 1e-3), unit=UNIT, n_gpus=world, steps=args.steps, warmup=args.warmup,
                     ms_per_step=ms, higher_is_better=True, scaling="weak", vs_baseline=None, dtype="tf32", data="synthetic",
                     config=workload_config(args.sr_label, world),
@@ -490,7 +509,7 @@ def run_ours(args):
         # The comparators below run LAST: the CPU arm leaves the host busy / memory-fragmented enough to slow the eager, event-timed
         # GPT profile above by 2x when it ran first (graph-replayed timings were never affected).
         extra = {}
-        # ---- the same algorithm through stock PyTorch GPU kernels, whole optimisation step, same B200: the ">= 10x the
+        # ---- the same algorithm through stock PyTorch GPU kernels, whole optimisation step, same GPU: the ">= 10x the
         #      reference's 1-GPU PyTorch step" comparator of BASELINE.json, in the reference's as-shipped fp16-autocast regime
         #      and in fp32/TF32
         if not args.no_torch_port and world == 1:
@@ -505,7 +524,7 @@ def run_ours(args):
                 except Exception as e:                      # context only: never fail the benchmark because of it
                     extra[key] = dict(error=repr(e)[:300])
                 torch.cuda.empty_cache()
-        # ---- CPU baseline on this box's host cores: the full benchmark batch, whole optimisation step, bounded in time
+        # ---- CPU baseline on the host's CPU cores: the full benchmark batch, whole optimisation step, bounded in time
         threads = cpu_threads()
         if not args.no_cpu_baseline and world == 1:                      # contract: rank 0 at N = 1 only
             Bc = args.cpu_batch if args.cpu_batch > 0 else B_PER_GPU
@@ -576,7 +595,7 @@ def gpt_section(args, dev, rank, world):
     for _ in range(max(args.warmup, 3)):
         resident()
     st.batch_idx = 1
-    steps = 8                                          # two accumulate-4 cycles: 8 micro-batches + 2 optimizer updates
+    steps = args.steps                                 # micro-batches; every 4th runs the optimizer update (accumulate 4)
     ms = timed(resident, steps)
     st.batch_idx = 1
     for _ in range(2):
@@ -601,9 +620,9 @@ def gpt_section(args, dev, rank, world):
         all_ms = sum(v["ms"] for v in prof.values())
         attn = {k: round(v["ms"], 3) for k, v in prof.items() if "flash" in k}
         roof = dict(bound="tensor", kernel="gemm_tma_kernel (six Linear layers per block: forward, data gradient, weight gradient)", achieved=g_fl / (g_ms * 1e-3) / 1e12,
-                    peak=tf_sus, unit="TFLOP/s", frac=g_fl / (g_ms * 1e-3) / 1e12 / tf_sus, traffic=ncu_traffic("gemm_tma_kernel_gpt"),
+                    peak=tf_sus, unit="TFLOP/s", frac=g_fl / (g_ms * 1e-3) / 1e12 / tf_sus,
                     share_of_step_time=g_ms / all_ms, attention_ms=attn, attention_share_of_step_time=sum(attn.values()) / all_ms,
-                    peak_source=f"{src} cuBLAS bf16 sustained (TF32 nominal = half)",
+                    peak_source=f"{src} bf16 (TF32 nominal = half)",
                     how="analytic flops of every gemm_tma launch of one micro-batch / the sum of their CUDA-event durations (eager step, events around each library call)")
         if not args.no_cpu_baseline and world == 1:
             cpu = gpt_cpu_baseline(B, X, Y)
@@ -749,6 +768,8 @@ def main():
     ap.add_argument("--gpt", type=int, default=2, help="2 (default): also time the stage-1 AR-GPT step at every N; 1: at N=1 only; 0: skip")
     ap.add_argument("--config", type=int, default=3, help="3 (default): the stage-2 step (BASELINE configs 3/4); 5: vocoder-only per-layer sweep with the MR-STFT loss")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from Python instead of replaying the captured CUDA graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's losses and a seeded sample of the updated parameters as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)

@@ -20,6 +20,54 @@ int check_launch(const char* what) {
 }
 int mel_init_tables();
 double g_disp_flops[EVK_DISPATCH_SLOTS] = {0};
+
+static cudaMemPool_t g_pool = nullptr;
+void Scratch::alloc(long long n) {
+  if (p) { cudaFreeAsync(p, st); p = nullptr; }
+  if (n <= 0 || !g_pool) return;
+  void* q = nullptr;
+  if (cudaMallocFromPoolAsync(&q, (size_t)n * sizeof(float), g_pool, st) == cudaSuccess) p = static_cast<float*>(q);
+  else cudaGetLastError();
+}
+Scratch::~Scratch() {
+  if (p) cudaFreeAsync(p, st);
+}
+
+// block (32, OS_LANES) per 32 consecutive output elements: lane ty sums the partials s = ty, ty + OS_LANES, ... (its fixed share),
+// then the OS_LANES sums are added in ty order -- the same order on every run, independent of scheduling
+constexpr int OS_LANES = 16;
+__global__ void ordered_sum_kernel(const float* __restrict__ part, int S, long long ps, int O, int R, int Cn, float* __restrict__ dst,
+                                   long long d_so, long long d_sr) {
+  __shared__ float red[OS_LANES][33];
+  const long long n = (long long)O * R * Cn;
+  for (long long i0 = (long long)blockIdx.x * 32; i0 < n; i0 += (long long)gridDim.x * 32) {
+    const long long i = i0 + threadIdx.x;
+    float acc = 0.f;
+    if (i < n)
+      for (int s = threadIdx.y; s < S; s += OS_LANES) acc += part[s * ps + i];
+    red[threadIdx.y][threadIdx.x] = acc;
+    __syncthreads();
+    if (threadIdx.y == 0 && i < n) {
+      float t = 0.f;
+#pragma unroll
+      for (int k = 0; k < OS_LANES; ++k) t += red[k][threadIdx.x];
+      const int c = (int)(i % Cn);
+      const long long orr = i / Cn;
+      const int r = (int)(orr % R), o = (int)(orr / R);
+      dst[o * d_so + r * d_sr + c] += t;
+    }
+    __syncthreads();
+  }
+}
+
+int ordered_sum(const float* part, int S, long long ps, int O, int R, int Cn, float* dst, long long d_so, long long d_sr, cudaStream_t st) {
+  const long long n = (long long)O * R * Cn;
+  if (n <= 0) return EVK_OK;
+  const long long blocks = (n + 31) / 32;
+  ordered_sum_kernel<<<(unsigned)(blocks < kNumSMs * 16 ? blocks : kNumSMs * 16), dim3(32, OS_LANES), 0, st>>>(part, S, ps, O, R, Cn, dst,
+                                                                                                               d_so, d_sr);
+  return check_launch("ordered_sum");
+}
 }  // namespace evk
 using namespace evk;
 
@@ -34,9 +82,22 @@ extern "C" int evk_init(void) {
   cudaDeviceProp prop;
   e = cudaGetDeviceProperties(&prop, dev);
   if (e != cudaSuccess) { set_error("evk_init: %s", cudaGetErrorString(e)); return EVK_ERR_CUDA; }
-  if (prop.major != 10) {
-    set_error("evk_init: device '%s' is sm_%d%d; libevk_sm100 is built for sm_100a (B200) only", prop.name, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("evk_init: device '%s' is sm_%d%d; libevk_sm90 is built for sm_90a (H100) only", prop.name, prop.major, prop.minor);
     return EVK_ERR_ARCH;
+  }
+  if (!g_pool) {                                   // scratch pool: keeps what it has reserved instead of returning it at every sync
+    cudaMemPoolProps props{};
+    props.allocType = cudaMemAllocationTypePinned;
+    props.location.type = cudaMemLocationTypeDevice;
+    props.location.id = dev;
+    uint64_t keep = UINT64_MAX;
+    if (cudaMemPoolCreate(&g_pool, &props) != cudaSuccess ||
+        cudaMemPoolSetAttribute(g_pool, cudaMemPoolAttrReleaseThreshold, &keep) != cudaSuccess) {
+      g_pool = nullptr;
+      set_error("evk_init: scratch memory pool creation failed");
+      return EVK_ERR_CUDA;
+    }
   }
   int rc = mel_init_tables();
   if (rc) { set_error("evk_init: twiddle/window table upload failed"); return rc; }

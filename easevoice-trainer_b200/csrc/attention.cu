@@ -110,7 +110,8 @@ __global__ void relk_dq_kernel(const float* __restrict__ drel, const float* __re
   }
 }
 
-// dE[r][d] += sum_{z,i} band[z][i][r] * x[b][i][h*dk+d]   (thread per (r,d), rows chunked over blocks)
+// dE[r][d] += sum_{z,i} band[z][i][r] * x[b][i][h*dk+d]   (thread per (r,d), rows chunked over blocks; this kernel writes
+// the partial of its row chunk to part[chunk][r*dk+d], ordered_sum adds the chunks in order)
 // used for both dEk (band = drel, x = q) and dEv (band = P band, x = dOut)
 __global__ void rel_dE_kernel(const float* __restrict__ band, const float* __restrict__ x, int ldx, int H, int T, int dk,
                               int W, float* __restrict__ dE, long long nrows, int rows_per_block) {
@@ -125,7 +126,7 @@ __global__ void rel_dE_kernel(const float* __restrict__ band, const float* __res
     acc = fmaf(band[(long long)zi * W + r], x[((long long)b * T + i) * ldx + h * dk + d], acc);
     if (++i == T) { i = 0; ++z; }
   }
-  atomicAdd(&dE[rd], acc);
+  dE[(long long)blockIdx.x * W * dk + rd] = acc;
 }
 
 // band[z][i][r] = P[z][i][i+r-win] (0 outside)            (to_band = 1)
@@ -159,7 +160,7 @@ __global__ void relv_out_kernel(const float* __restrict__ band, const float* __r
 
 static inline dim3 g1(long long n) {
   long long g = (n + 255) / 256;
-  if (g > 148LL * 32) g = 148LL * 32;
+  if (g > (long long)kNumSMs * 32) g = (long long)kNumSMs * 32;
   if (g < 1) g = 1;
   return dim3((unsigned)g);
 }
@@ -206,8 +207,12 @@ extern "C" int evk_relk_bwd(const float* drel, const float* q, int32_t ldq, cons
   EVK_REQUIRE(nrows < 0x7fffffffLL, EVK_ERR_ARG, "relk_bwd: too many rows");
   const int rpb = 32;
   dim3 grid(cdiv(nrows, rpb), cdiv(W * dk, 128));
-  rel_dE_kernel<<<grid, 128, 0, ST>>>(drel, q, ldq, H, T, dk, W, dE, nrows, rpb);
-  return check_launch("relk_dE");
+  Scratch part_buf((long long)grid.x * W * dk, ST);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "relk_bwd: scratch allocation failed");
+  rel_dE_kernel<<<grid, 128, 0, ST>>>(drel, q, ldq, H, T, dk, W, part, nrows, rpb);
+  if (int rc2 = check_launch("relk_dE")) return rc2;
+  return ordered_sum(part, grid.x, 1, 1, W * dk, dE, 0, 0, ST);
 }
 extern "C" int evk_attn_band(float* P, int32_t lds, float* band, int32_t Z, int32_t Tq, int32_t Tk, int32_t win, int32_t to_band,
                              evk_stream_t stream) {
@@ -238,6 +243,10 @@ extern "C" int evk_relv_bwd(const float* band, const float* dout, int32_t lddo, 
   EVK_REQUIRE(nrows < 0x7fffffffLL, EVK_ERR_ARG, "relv_bwd: too many rows");
   const int rpb = 32;
   dim3 grid(cdiv(nrows, rpb), cdiv(W * dk, 128));
-  rel_dE_kernel<<<grid, 128, 0, ST>>>(band, dout, lddo, H, T, dk, W, dE, nrows, rpb);
-  return check_launch("relv_dE");
+  Scratch part_buf((long long)grid.x * W * dk, ST);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "relv_bwd: scratch allocation failed");
+  rel_dE_kernel<<<grid, 128, 0, ST>>>(band, dout, lddo, H, T, dk, W, part, nrows, rpb);
+  if (int rc2 = check_launch("relv_dE")) return rc2;
+  return ordered_sum(part, grid.x, 1, 1, W * dk, dE, 0, 0, ST);
 }

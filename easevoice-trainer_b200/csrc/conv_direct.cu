@@ -118,8 +118,9 @@ __global__ void direct_dgrad(const __grid_constant__ DP p) {
   (const_cast<float*>(p.x) + b * p.x_sb + h * p.x_sh)[ipos * p.ldx + c] = acc;
 }
 
-// dW[q][n][cl] += sum_z sum_pos dY[orow][n] * X[irow][g*Cg+cl]; one thread per weight, positions chunked over grid.x
-__global__ void direct_wgrad(const __grid_constant__ DP p) {
+// dW[q][n][cl] += sum_z sum_pos dY[orow][n] * X[irow][g*Cg+cl]; one thread per weight, positions chunked over grid.x.
+// Each (z, chunk) writes its partial to part[(z * chunks + chunk) * nw + widx]; ordered_sum adds them in that order.
+__global__ void direct_wgrad(const __grid_constant__ DP p, float* __restrict__ part) {
   const int z = blockIdx.z, b = z / p.H, h = z - b * p.H;
   const int Cg = p.C / p.G, Ng = p.N / p.G;
   const long long nw = (long long)p.Q * p.N * Cg;
@@ -143,7 +144,7 @@ __global__ void direct_wgrad(const __grid_constant__ DP p) {
     if (ij < 0 || ij >= lim) continue;
     acc = fmaf(Yg[((long long)(p.o0 + j * p.os) * p.P + w) * p.ldy], X[((long long)ij * p.P + w) * p.ldx], acc);
   }
-  atomicAdd(p.w + b * p.w_sb + h * p.w_sh + (long long)q * p.w_sq + (long long)n * p.ldw + cl, acc);
+  part[((long long)z * gridDim.x + blockIdx.x) * nw + widx] = acc;
 }
 
 static int fill_dp(const evk_gconv_desc* d, DP& p) {
@@ -207,13 +208,26 @@ extern "C" int evk_conv_direct_wgrad(const evk_gconv_desc* d, evk_stream_t strea
   const long long npos = (long long)p.J * p.P;
   if (nw == 0 || npos == 0) return EVK_OK;
   const int wblocks = cdiv(nw, 256);
-  long long want = (148LL * 8 + (long long)wblocks * p.Z - 1) / ((long long)wblocks * p.Z);
+  long long want = ((long long)kNumSMs * 8 + (long long)wblocks * p.Z - 1) / ((long long)wblocks * p.Z);
   long long chunk = (npos + want - 1) / want;
   if (chunk < 128) chunk = 128;
   p.chunk = (int)chunk;
   dim3 grid(cdiv(npos, chunk), wblocks, p.Z);
   EVK_REQUIRE(grid.y <= 65535, EVK_ERR_ARG, "conv_direct_wgrad: too many weights");
-  direct_wgrad<<<grid, 256, 0, (cudaStream_t)stream>>>(p);
+  const int chunks = (int)grid.x, Cg = p.C / p.G;
+  Scratch part_buf(nw * chunks * p.Z, (cudaStream_t)stream);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "conv_direct_wgrad: scratch allocation failed");
+  direct_wgrad<<<grid, 256, 0, (cudaStream_t)stream>>>(p, part);
   g_disp_flops[6] += desc_flops(d);
-  return check_launch("conv_direct_wgrad");
+  if (int rc2 = check_launch("conv_direct_wgrad")) return rc2;
+  if (p.w_sb == 0 && p.w_sh == 0)                                  // one weight for every z: all partials in (z, chunk) order
+    return ordered_sum(part, p.Z * chunks, p.Q, p.N, Cg, p.w, p.w_sq, p.ldw, (cudaStream_t)stream);
+  for (int z = 0; z < p.Z; ++z) {                                  // z in order, each adding its chunks
+    const int b = z / p.H, h = z - b * p.H;
+    if (int rc2 = ordered_sum(part + (long long)z * chunks * nw, chunks, p.Q, p.N, Cg, p.w + b * p.w_sb + h * p.w_sh, p.w_sq, p.ldw,
+                              (cudaStream_t)stream))
+      return rc2;
+  }
+  return EVK_OK;
 }

@@ -7,7 +7,7 @@ namespace evk {
 
 static inline dim3 grid1d(long long n, int bs = 256) {
   long long g = (n + bs - 1) / bs;
-  if (g > 148LL * 32) g = 148LL * 32;   // grid-stride, a few waves of 148 SMs
+  if (g > (long long)kNumSMs * 32) g = (long long)kNumSMs * 32;   // grid-stride, a few waves of the SMs
   if (g < 1) g = 1;
   return dim3((unsigned)g);
 }
@@ -285,7 +285,7 @@ __global__ void transpose_rows_multi_kernel(const float* __restrict__ x, int ldx
 // backward, transpose for the TMA weight gradient, column sums for the bias -- and four trips through memory):
 //   g[t][c]    = dy[t][c] * act'(y[t][c]) * (t < len*P)        -> dpre  (normal layout, only when it differs from dy)
 //   dyt[c][t]  = g[t][c]                                        -> the K-major A operand of the weight-gradient GEMM
-//   dbias[c]  += sum_t g[t][c]                                  (atomics; one per column per block of TPB row tiles)
+//   dbias[c]  += sum_t g[t][c]                                  (one partial per column per block, summed in block order)
 constexpr int DYP_ROWS = 128;          // rows per block: 16 independent loads per thread in flight, one barrier
 __global__ void __launch_bounds__(256) dy_prep_kernel(const float* __restrict__ dy, int lddy, const float* __restrict__ yact, int ldy, int act,
                                                       float slope, float gscale, const int* __restrict__ len, int P, float* __restrict__ dpre,
@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(256) dy_prep_kernel(const float* __restrict__ 
       float sacc = 0.f;
 #pragma unroll
       for (int k = 0; k < 8; ++k) sacc += csum[k][tx];
-      atomicAdd(&dbias[c], sacc);
+      dbias[((long long)blockIdx.z * gridDim.x + blockIdx.x) * C + c] = sacc;    // partial of this block (ordered_sum)
     }
   }
 }
@@ -371,12 +371,18 @@ __global__ void embedding_kernel(const float* __restrict__ tab, int ldt, const l
   }
 }
 
+// dtab[idx[r]][c] += dy[r][c] without atomics, in two passes: thread (chunk, c) adds the rows of its EMB_CHUNK-row chunk in
+// row order into part[chunk][idx][c] (zeroed first), then ordered_sum adds the chunks in order.
+constexpr int EMB_CHUNK = 256;
 __global__ void embedding_bwd_kernel(const float* __restrict__ dy, int lddy, const long long* __restrict__ idx,
-                                     long long rows, float* __restrict__ dtab, int ldt, int C) {
-  EW_LOOP(i, rows * C) {
-    long long r = i / C;
-    int c = (int)(i - r * C);
-    atomicAdd(&dtab[idx[r] * ldt + c], dy[r * lddy + c]);
+                                     long long rows, float* __restrict__ part, int V, int C) {
+  const long long nchunks = (rows + EMB_CHUNK - 1) / EMB_CHUNK;
+  EW_LOOP(i, nchunks * C) {
+    const int c = (int)(i % C);
+    const long long k = i / C;
+    float* pk = part + k * V * (long long)C + c;
+    const long long r1 = min(rows, (k + 1) * EMB_CHUNK);
+    for (long long r = k * EMB_CHUNK; r < r1; ++r) pk[idx[r] * C] += dy[r * lddy + c];
   }
 }
 
@@ -612,8 +618,13 @@ extern "C" int evk_dy_prep(const float* dy, int32_t lddy, const float* yact, int
   if ((long long)B * T * C == 0) return EVK_OK;
   dim3 grid(cdiv(T, DYP_ROWS), cdiv(C, 32), B), block(32, 8);
   EVK_REQUIRE(grid.y <= 65535 && grid.z <= 65535, EVK_ERR_ARG, "dy_prep: grid too large");
-  dy_prep_kernel<<<grid, block, 0, ST>>>(dy, lddy, yact, ldy, act, slope, gscale, len, P, dpre, ldp, dyt, ldt, t_sb, dbias, T, C);
-  return check_launch("dy_prep");
+  const int S = (int)(grid.x * grid.z);
+  Scratch part_buf(dbias ? (long long)S * C : 0, ST);
+  float* part = part_buf.p;
+  EVK_REQUIRE(!dbias || part, EVK_ERR_CUDA, "dy_prep: scratch allocation failed");
+  dy_prep_kernel<<<grid, block, 0, ST>>>(dy, lddy, yact, ldy, act, slope, gscale, len, P, dpre, ldp, dyt, ldt, t_sb, part, T, C);
+  if (int rc = check_launch("dy_prep")) return rc;
+  return dbias ? ordered_sum(part, S, 1, 1, C, dbias, 0, 0, ST) : EVK_OK;
 }
 extern "C" int evk_phase_split(const float* x, int32_t ldx, int64_t x_sb, float* xs, int64_t xs_ps, int32_t B, int32_t T, int32_t P,
                                int32_t C, int32_t stride, int32_t Jp, evk_stream_t stream) {
@@ -632,11 +643,16 @@ extern "C" int evk_embedding(const float* table, int32_t ldt, const int64_t* idx
   return check_launch("embedding");
 }
 extern "C" int evk_embedding_bwd(const float* dy, int32_t lddy, const int64_t* idx, int64_t rows, float* dtable,
-                                 int32_t ldt, int32_t C, evk_stream_t stream) {
-  EVK_REQUIRE(dy && idx && dtable, EVK_ERR_ARG, "embedding_bwd: null tensor");
+                                 int32_t ldt, int32_t C, int32_t V, evk_stream_t stream) {
+  EVK_REQUIRE(dy && idx && dtable && V > 0, EVK_ERR_ARG, "embedding_bwd: null tensor or empty table");
   if (rows * C == 0) return EVK_OK;
-  embedding_bwd_kernel<<<grid1d(rows * C), 256, 0, ST>>>(dy, lddy, (const long long*)idx, rows, dtable, ldt, C);
-  return check_launch("embedding_bwd");
+  const long long nchunks = (rows + EMB_CHUNK - 1) / EMB_CHUNK;
+  Scratch part_buf(nchunks * V * (long long)C, ST);
+  EVK_REQUIRE(part_buf.p, EVK_ERR_CUDA, "embedding_bwd: scratch allocation failed");
+  if (cudaMemsetAsync(part_buf.p, 0, (size_t)nchunks * V * C * sizeof(float), ST) != cudaSuccess) return check_launch("embedding_bwd_zero");
+  embedding_bwd_kernel<<<grid1d(nchunks * C), 256, 0, ST>>>(dy, lddy, (const long long*)idx, rows, part_buf.p, V, C);
+  if (int rc = check_launch("embedding_bwd")) return rc;
+  return ordered_sum(part_buf.p, (int)nchunks, 1, V, C, dtable, 0, ldt, ST);
 }
 extern "C" int evk_masked_mean(const float* x, int32_t ldx, float* y, int32_t ldy, int32_t B, int32_t T, int32_t C,
                                const int32_t* len, int32_t bwd, evk_stream_t stream) {

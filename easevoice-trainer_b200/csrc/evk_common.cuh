@@ -1,4 +1,4 @@
-// Common device/host helpers for libevk_sm100.so (sm_100a only).
+// Common device/host helpers for libevk_sm90.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -27,7 +27,33 @@ static inline double desc_flops(const evk_gconv_desc* d) {
   return 2.0 * d->Z * (double)d->J * d->P * d->N * (d->C / (d->G > 0 ? d->G : 1)) * d->Q;
 }
 
+// SMs of an H100 SXM: sizes the grids of grid-stride and persistent launches (the TMA GEMM queries the device instead).
+constexpr int kNumSMs = 132;
+
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// ---- deterministic cross-block sums ------------------------------------------------------------
+// Float additions do not associate, so a result that many blocks add into with atomics changes in its last bits from run
+// to run (and a training run amplifies that).  Kernels instead write one partial per block into library scratch and
+// ordered_sum adds the partials in block order:
+//   dst[o*d_so + r*d_sr + c] += sum_{s < S} part[s*ps + (o*R + r)*Cn + c]      (ps = O*R*Cn unless given)
+// Scratch is stream-ordered device memory for those partials: allocated on stream st from the library's memory pool
+// (cudaMallocFromPoolAsync) and freed on st (cudaFreeAsync) when it goes out of scope, after the kernels that use it have
+// been enqueued.  The pool allocator orders reuse across streams itself, and under CUDA-graph capture the pair becomes the
+// graph's own allocation / free nodes.  p is null when n == 0 or the allocation failed.
+struct Scratch {
+  float* p = nullptr;
+  cudaStream_t st;
+  Scratch(long long n, cudaStream_t s) : st(s) { alloc(n); }
+  ~Scratch();
+  void alloc(long long n);
+  Scratch(const Scratch&) = delete;
+  Scratch& operator=(const Scratch&) = delete;
+};
+int ordered_sum(const float* part, int S, long long ps, int O, int R, int Cn, float* dst, long long d_so, long long d_sr, cudaStream_t st);
+static inline int ordered_sum(const float* part, int S, int O, int R, int Cn, float* dst, long long d_so, long long d_sr, cudaStream_t st) {
+  return ordered_sum(part, S, (long long)O * R * Cn, O, R, Cn, dst, d_so, d_sr, st);
+}
 
 // ---- device helpers -----------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {

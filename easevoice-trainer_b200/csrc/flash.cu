@@ -17,9 +17,9 @@ namespace {
 constexpr int BT = 64;       // tile (queries or keys)
 constexpr int LDT = 36;      // smem row pitch in floats: conflict-free for both fragment patterns
 
-// Is EVERY (query i0.., key j0..) pair of a BT x BT tile visible?  Then the per-element mask (a third of the round-1
-// kernels' instructions: ISETP/FSETP/BRA/BSSY, see profiles/r2_ncu_before_epilogue_fix.md) is skipped for the tile -- all
-// but the tiles on the causal diagonal and on the x_len / y_len / prefix boundaries.
+// Is EVERY (query i0.., key j0..) pair of a BT x BT tile visible?  Then the per-element mask (compares, selects and branches
+// for every element) is skipped for the tile -- all but the tiles on the causal diagonal and on the x_len / y_len / prefix
+// boundaries.
 __device__ __forceinline__ bool tile_full(int i0, int j0, int X, int xl, int yl) {
   const int j1 = j0 + BT - 1;
   if (j1 < X) return j1 < xl;                                         // text keys only: visible to every query
@@ -71,7 +71,7 @@ __device__ __forceinline__ void mma_p(float (&c)[4], const uint32_t (&ah)[4], co
     mma_tf32(c, ah, bh);
   } else {
     // the B operand (K / V / Q / dO tile rows from shared memory) is fed as raw fp32 bits: the tensor core ignores the low
-    // 13 mantissa bits (truncation, as the TMA-fed tcgen05 GEMMs do); 128 of the 160 cvt.rna per key tile sat on the
+    // 13 mantissa bits (truncation, as the TMA-fed wgmma GEMMs do); 128 of the 160 cvt.rna per key tile sat on the
     // critical path next to only 64 mma.  A operands (Q, dO, K, V fragments loaded once; P / dS) stay round-to-nearest.
     uint32_t bh[2] = {__float_as_uint(b0), __float_as_uint(b1)};
     mma_tf32(c, ah, bh);
@@ -220,8 +220,8 @@ __global__ void __launch_bounds__(128, 5) flash_fwd_kernel(FlashArgs a) {
 }
 
 // delta[z][i] = sum_d dO[i][d] * O[i][d].  Eight lanes per (position, head) row, heads fastest: a warp reads 4 x 128 contiguous
-// bytes of dO and of O with one float4 per lane (the one-warp-per-row version below spent 48 us per layer on index divisions and
-// five shuffle rounds per row: ncu, profiles/r2_ncu_flash.md).
+// bytes of dO and of O with one float4 per lane (the one-warp-per-row version below spends its time on index divisions and
+// five shuffle rounds per row).
 __global__ void __launch_bounds__(256) flash_delta8_kernel(FlashArgs a) {
   const long long t = (long long)blockIdx.x * 256 + threadIdx.x;
   const long long rows = (long long)a.B * a.H * a.L;
@@ -446,8 +446,6 @@ int check_common(int B, int H, int L, int X, int dk, int ld, int ldo) {
 
 }  // namespace
 extern int g_precise;
-int flash_tc_fwd_try(const FlashArgs& a, cudaStream_t st);     // flash_tc.cu: 0 launched, < 0 error, 1 not eligible
-int flash_tc_bwd_try(const FlashArgs& a, cudaStream_t st);
 }  // namespace evk
 
 using namespace evk;
@@ -462,10 +460,6 @@ extern "C" int evk_flash_attn_fwd(const float* q, const float* k, const float* v
   FlashArgs a{};
   a.q = q; a.k = k; a.v = v; a.ld = ld; a.o = o; a.ldo = ldo; a.lse = lse; a.B = B; a.H = H; a.L = L; a.X = X;
   a.xlen = (const long long*)xlen; a.ylen = (const long long*)ylen; a.scale = scale; a.p_drop = p_drop; a.rng = (const unsigned long long*)rng; a.sid = sid;
-  if (!g_precise) {                                                // tcgen05 / TMEM kernels (flash_tc.cu); 3xTF32 test mode stays on mma.sync
-    const int rc = flash_tc_fwd_try(a, st);
-    if (rc <= 0) return rc;
-  }
   dim3 grid(cdiv(L, BT), H, B);
   if (g_precise) flash_fwd_kernel<true><<<grid, 128, 0, st>>>(a);
   else flash_fwd_kernel<false><<<grid, 128, 0, st>>>(a);
@@ -488,10 +482,6 @@ extern "C" int evk_flash_attn_bwd(const float* q, const float* k, const float* v
   if (ldo % 4 == 0 && ((uintptr_t)o % 16) == 0) flash_delta8_kernel<<<cdiv((long long)rows * 8, 256), 256, 0, st>>>(a);
   else flash_delta_kernel<<<cdiv(rows, 8), 256, 0, st>>>(a);
   if (int rc = check_launch("flash_delta")) return rc;
-  if (!g_precise) {
-    const int rc = flash_tc_bwd_try(a, st);
-    if (rc <= 0) return rc;
-  }
   dim3 grid(cdiv(L, BT), H, B);
   if (g_precise) flash_dq_kernel<true><<<grid, 128, 0, st>>>(a);
   else flash_dq_kernel<false><<<grid, 128, 0, st>>>(a);

@@ -5,7 +5,7 @@
 // Forward kernel ("F"): output positions on the MMA M axis, output channels on N, input channels on K.
 // The input rows a tile needs for ALL taps are staged once per channel chunk as a shared-memory slab
 // (tap q reads the slab shifted by off[q]*P rows), so the implicit im2col never touches L2 twice.
-// Weight-gradient kernel ("W"): positions on K, (n, c) on M/N, fp32 atomics for the split-K merge.
+// Weight-gradient kernel ("W"): positions on K, (n, c) on M/N, per-CTA partials added in a fixed order for the split-K merge.
 //
 // Replaces the cuDNN / cuBLAS kernels behind the reference's Conv1d / Conv2d(k,1) / ConvTranspose1d /
 // Linear / matmul call sites (see include/evk.h for file:line).
@@ -26,6 +26,8 @@ struct GP {
   int off_min, off_max;
   int KS, TG, NG, slab_rows;   // F: k-steps/tap/chunk, taps per group, groups, slab rows
   int rch;                     // W: positions per CTA
+  float* part;                 // W: per-(z, position chunk, K warp) partials [z - zoff][S1][Q][N][C], summed by gconv_w_sum
+  int zoff;                    // W: first batch x group item of this launch (blockIdx.z counts from it)
   int off[EVK_MAX_TAPS];
 };
 
@@ -213,7 +215,7 @@ __global__ void __launch_bounds__(NT) gconv_f_kernel(const __grid_constant__ GP 
 // ============================================================================================
 // W kernel (weight gradient): dW[q][n][c] += sum_pos Yg[orow][n] * X[irow(pos,q)][c]
 // GEMM view: M = n (out channels), N = (q, c) columns (taps folded into the column space so that skinny layers
-// fill the tile), K = positions (split over CTAs, merged with fp32 atomics).
+// fill the tile), K = positions (split over CTAs and K warps; each writes a partial, ordered_sum adds them in order).
 // ============================================================================================
 template <int TN, int TC, int WARPS_N, int WARPS_C, int WARPS_K, bool PRECISE>
 __global__ void __launch_bounds__(NT) gconv_w_kernel(const __grid_constant__ GP p) {
@@ -229,7 +231,7 @@ __global__ void __launch_bounds__(NT) gconv_w_kernel(const __grid_constant__ GP 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int gid = lane >> 2, t4 = lane & 3;
   const int wk = warp % WARPS_K, wc = (warp / WARPS_K) % WARPS_C, wnn = warp / (WARPS_K * WARPS_C);
-  const int z = blockIdx.z;
+  const int z = p.zoff + blockIdx.z;
   const int b = z / p.H, h = z - b * p.H;
   const int Cq = (p.C + 3) & ~3;                      // per-tap column pitch (16-byte pieces never straddle taps)
   const int ncols = p.Q * Cq;
@@ -331,7 +333,7 @@ __global__ void __launch_bounds__(NT) gconv_w_kernel(const __grid_constant__ GP 
     __syncthreads();
   }
 
-  float* Wd = p.w + b * p.w_sb + h * p.w_sh;
+  float* Wd = p.part + (((long long)blockIdx.z * gridDim.x + blockIdx.x) * WARPS_K + wk) * ((long long)p.Q * p.N * p.C);
 #pragma unroll
   for (int nf = 0; nf < NF; ++nf)
 #pragma unroll
@@ -339,13 +341,13 @@ __global__ void __launch_bounds__(NT) gconv_w_kernel(const __grid_constant__ GP 
       const int col = col0 + wc * NF * 8 + nf * 8 + 2 * t4 + e;
       const int q = col / Cq, c = col - q * Cq;
       if (q >= p.Q || c >= p.C) continue;
-      float* wq = Wd + (long long)q * p.w_sq + c;
+      float* wq = Wd + (long long)q * p.N * p.C + c;
 #pragma unroll
       for (int mf = 0; mf < MF; ++mf)
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
           const int n = n0 + wnn * MF * 16 + mf * 16 + hf * 8 + gid;
-          if (n < p.N) atomicAdd(wq + (long long)n * p.ldw, acc[mf][nf][hf * 2 + e]);
+          if (n < p.N) wq[(long long)n * p.C] = acc[mf][nf][hf * 2 + e];
         }
     }
 }
@@ -354,7 +356,7 @@ __global__ void __launch_bounds__(NT) gconv_w_kernel(const __grid_constant__ GP 
 // host side
 // ============================================================================================
 int g_precise = 0;          // 3xTF32 products on the mma.sync kernels (parity tests)
-int g_backend_tc = 1;       // use the tcgen05/TMEM kernel for eligible (stride-1) launches
+int g_backend_tc = 1;       // use the TMA / wgmma kernels for eligible (stride-1) launches
 int gconv_tc_try(const evk_gconv_desc* d, cudaStream_t st);
 int gemm_tma_try(const evk_gconv_desc* d, cudaStream_t st);
 
@@ -437,7 +439,7 @@ using namespace evk;
 
 extern "C" int evk_set_precise(int32_t on) { g_precise = on ? 1 : 0; return EVK_OK; }
 extern "C" int evk_get_precise(void) { return g_precise; }
-extern "C" int evk_set_backend(int32_t tcgen05) { g_backend_tc = tcgen05 ? 1 : 0; return EVK_OK; }
+extern "C" int evk_set_backend(int32_t tensor_core) { g_backend_tc = tensor_core ? 1 : 0; return EVK_OK; }
 
 extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
   GP p;
@@ -448,7 +450,7 @@ extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
   EVK_REQUIRE(d->y != nullptr && d->x != nullptr && d->w != nullptr, EVK_ERR_ARG, "gconv_fwd: null tensor");
   cudaStream_t st = (cudaStream_t)stream;
   if (g_backend_tc && !g_precise && (d->ldx % 4) == 0) {
-    rc = gemm_tma_try(d, st);          // TMA-fed persistent tcgen05 GEMM / implicit-GEMM conv
+    rc = gemm_tma_try(d, st);          // TMA-fed persistent wgmma GEMM / implicit-GEMM conv
     if (rc <= 0) { if (rc == 0) g_disp_flops[0] += desc_flops(d); return rc; }
     EVK_REQUIRE(!(d->drop_rng && d->drop_p > 0.f), EVK_ERR_UNSUPPORTED, "gconv_fwd: fused dropout needs a launch the TMA kernel takes");
     rc = gconv_tc_try(d, st);
@@ -477,6 +479,24 @@ extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
 #undef EVK_F
 }
 
+// W[b'][h'][q][n][c] += sum over the batch items b of [b0, b0 + nb) (all of them when w_sb == 0, else b = b') and the groups h
+// (all when w_sh == 0, else h = h') and the S1 partials j, in that nesting order, of part[((b - b0) * H + h) * S1 + j][q][n][c]
+__global__ void gconv_w_sum_kernel(const GP p, int b0, int nb, int S1) {
+  const long long nwt = (long long)p.Q * p.N * p.C;
+  const int Bo = p.w_sb == 0 ? 1 : nb, Ho = p.w_sh == 0 ? 1 : p.H;
+  const long long total = (long long)Bo * Ho * nwt;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long e = i % nwt, bh = i / nwt;
+    const int hh = (int)(bh % Ho), bb = (int)(bh / Ho);
+    const int c = (int)(e % p.C), n = (int)((e / p.C) % p.N), q = (int)(e / ((long long)p.C * p.N));
+    float acc = 0.f;
+    for (int b = (p.w_sb == 0 ? 0 : bb); b < (p.w_sb == 0 ? nb : bb + 1); ++b)
+      for (int h = (p.w_sh == 0 ? 0 : hh); h < (p.w_sh == 0 ? p.H : hh + 1); ++h)
+        for (int j = 0; j < S1; ++j) acc += p.part[(((long long)b * p.H + h) * S1 + j) * nwt + e];
+    p.w[(long long)(b0 + bb) * p.w_sb + (long long)hh * p.w_sh + (long long)q * p.w_sq + (long long)n * p.ldw + c] += acc;
+  }
+}
+
 template <int TN, int TC, int WN, int WC, int WK, bool PRECISE>
 static int launch_w(GP& p, cudaStream_t st) {
   constexpr int RK = (WK * 8 > 32) ? WK * 8 : 32;
@@ -484,14 +504,25 @@ static int launch_w(GP& p, cudaStream_t st) {
   const long long npos = (long long)p.J * p.P;
   const int Cq = (p.C + 3) & ~3;
   const int tiles = cdiv(p.N, TN) * cdiv((long long)p.Q * Cq, TC);
-  // aim for >= ~4 waves of 148 SMs, but keep >= 256 positions per CTA
+  // aim for >= ~4 waves of the SMs, but keep >= 256 positions per CTA
   long long ctas_fixed = (long long)tiles * p.Z;
-  long long want = (148LL * 8 + ctas_fixed - 1) / ctas_fixed;
+  long long want = ((long long)kNumSMs * 8 + ctas_fixed - 1) / ctas_fixed;
   long long rch = (npos + want - 1) / want;
   rch = ((rch + 31) / 32) * 32;
   if (rch < 256) rch = 256;
+  // partials: [batch items of one launch][H][S1 = chunks * WK][Q][N][C], at most PART_CAP floats per launch
+  constexpr long long PART_CAP = 40ll << 20;            // floats of partials per launch (batch slices beyond it)
+  if (npos == 0 || p.Z == 0) return EVK_OK;
+  const long long nwt = (long long)p.Q * p.N * p.C;
+  const int B = p.Z / p.H;
+  while (rch < npos && (long long)cdiv(npos, rch) * p.H * WK * nwt > PART_CAP) rch *= 2;
   p.rch = (int)rch;
-  dim3 grid(cdiv(npos, rch), tiles, p.Z);
+  const int S1 = cdiv(npos, rch) * WK;
+  const int nb = (int)max(1ll, min((long long)B, PART_CAP / ((long long)S1 * p.H * nwt)));
+  Scratch part_buf((long long)nb * p.H * S1 * nwt, st);
+  p.part = part_buf.p;
+  EVK_REQUIRE(p.part, EVK_ERR_CUDA, "gconv_wgrad: scratch allocation failed");
+  dim3 grid(cdiv(npos, rch), tiles, nb * p.H);
   if (grid.x == 0) return EVK_OK;
   EVK_REQUIRE(grid.y <= 65535 && grid.z <= 65535, EVK_ERR_ARG, "gconv_wgrad: grid too large");
   auto kern = gconv_w_kernel<TN, TC, WN, WC, WK, PRECISE>;
@@ -500,8 +531,17 @@ static int launch_w(GP& p, cudaStream_t st) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     attr_set = true;
   }
-  kern<<<grid, NT, smem, st>>>(p);
-  return check_launch("gconv_w_kernel");
+  for (int b0 = 0; b0 < B; b0 += nb) {                             // batch slices in order, each reduced before the next
+    const int n_b = min(nb, B - b0);
+    p.zoff = b0 * p.H;
+    grid.z = n_b * p.H;
+    kern<<<grid, NT, smem, st>>>(p);
+    if (int rc = check_launch("gconv_w_kernel")) return rc;
+    const long long total = (long long)(p.w_sb == 0 ? 1 : n_b) * (p.w_sh == 0 ? 1 : p.H) * nwt;
+    gconv_w_sum_kernel<<<(unsigned)min((long long)kNumSMs * 16, (total + 255) / 256), 256, 0, st>>>(p, b0, n_b, S1);
+    if (int rc = check_launch("gconv_w_sum")) return rc;
+  }
+  return EVK_OK;
 }
 
 extern "C" int evk_gconv_wgrad(const evk_gconv_desc* d, evk_stream_t stream) {

@@ -1,17 +1,15 @@
-// tcgen05 / TMEM implicit-GEMM convolution (sm_100a): the stride-1 launches of the generalised conv
+// wgmma implicit-GEMM convolution (sm_90a): the stride-1 launches of the generalised conv
 //
 //   Y[z][pos][n] = epi( sum_q sum_c X[z][pos + off[q]*P][c] * W[z][q][n][c] ),   pos = j*P + w  (is == 1)
 //
-// Mapping: 128 output positions = the UMMA M dimension (TMEM lanes), output channels = UMMA N (TMEM columns),
-// input channels = K.  Both operands are K-major in the canonical *interleaved* (SWIZZLE_NONE) core-matrix
-// layout: for every 16-byte K-chunk a panel [rows][16 B].  A row shift is then a plain +16 B*rows start-address
-// offset, so ONE staged slab of input rows serves every tap (the smem descriptor of tap q just starts
-// off[q]*P rows further down) -- the implicit im2col costs no extra shared-memory fill.
-// tcgen05.mma is issued by one thread; accumulators live in TMEM (fp32, BN columns per 128-position tile);
-// completion is tracked with tcgen05.commit -> mbarrier; the epilogue reads TMEM with tcgen05.ld (32x32b).
+// Mapping: 128 output positions per M tile = two warpgroups x 64 rows (wgmma M), output channels = wgmma N, input
+// channels = K.  Both operands are K-major in the canonical *interleaved* (no-swizzle) core-matrix layout: for every
+// 16-byte K-chunk a panel [rows][16 B].  A row shift is then a plain +16 B*rows start-address offset, so ONE staged slab
+// of input rows serves every tap (the smem descriptor of tap q just starts off[q]*P rows further down) -- the implicit
+// im2col costs no extra shared-memory fill.  Accumulators live in registers (fp32, MT x BN / 2 per thread).
 // Activations are staged global -> registers -> cvt.rna.tf32 -> smem (round-to-nearest instead of the tensor
 // core's operand truncation, which would bias every product towards zero); weights are pre-rounded at pack time.
-#include "evk_common.cuh"
+#include "wgmma.cuh"
 
 namespace evk {
 
@@ -28,65 +26,22 @@ struct TP {
   int off[EVK_MAX_TAPS];
 };
 
-constexpr int TC_THREADS = 256;
+constexpr int TC_THREADS = 256;                       // two warpgroups
 
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\n"
-      "bra WAIT_%=;\n"
-      "DONE_%=:\n"
-      "}\n" ::"r"(smem_u32(bar)), "r"(parity));
-}
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  // SWIZZLE_NONE, K-major: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=0
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t taddr, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(taddr), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum));
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.b64 [%0];\n" ::"l"(__cvta_generic_to_shared(bar)));
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// BN: N tile (UMMA N, TMEM columns per M tile); MT: number of 128-position M tiles per CTA (weights reused MT times)
+// BN: N tile (wgmma N); MT: number of 128-position M tiles per CTA (weights reused MT times)
 template <int BN, int MT>
-__global__ void __launch_bounds__(TC_THREADS, 2) gconv_tc_kernel(const __grid_constant__ TP p) {
+__global__ void __launch_bounds__(TC_THREADS, 1) gconv_tc_kernel(const __grid_constant__ TP p) {
   constexpr int B_PITCH = BN + 4;                               // weight panel pitch (rows); == 4 (mod 8)
-  constexpr int TCOLS = (BN * MT < 32) ? 32 : BN * MT;          // power of two >= 32 for BN in {16..256}, MT in {1,2}
-  static_assert(TCOLS <= 512, "TMEM has 512 columns");
   extern __shared__ __align__(128) uint8_t tsm[];
   const int KCH = p.KCH, KC = KCH * 4;
   const int slab_bytes = KCH * p.a_pitch * 16;
   const int wt_bytes = p.TG * KCH * B_PITCH * 16;
   uint8_t* slab0 = tsm;                                         // [2][KCH][a_pitch][16 B]
   uint8_t* wt0 = tsm + 2 * slab_bytes;                          // [NW][TG][KCH][B_PITCH][16 B]
-  constexpr int NW = 2;                                         // weight-stage ring depth (3 measured slower: smaller stages, lower flop/byte)
-  __shared__ __align__(8) uint64_t mbar[NW];
-  __shared__ uint32_t tmem_base_s;
+  constexpr int NW = 2;                                         // weight-stage ring depth
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;                                     // warpgroup: rows 64 wg .. 64 wg + 63 of each M tile
   const int z = blockIdx.z, b = z / p.H, h = z - b * p.H;
   const float* X = p.x + b * p.x_sb + h * p.x_sh;
   const float* Wg = p.w + b * p.w_sb + h * p.w_sh;
@@ -97,19 +52,6 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gconv_tc_kernel(const __grid_co
   if (p.in_len) lim = min(lim, p.in_len[b]);
   const int lim_rows = lim * p.P;
 
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(&tmem_base_s)), "n"(TCOLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  if (tid == 32) {
-    for (int i = 0; i < NW; ++i) mbar_init(&mbar[i], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n");
-  const uint32_t tmem_base = tmem_base_s;
-
   const int nchunks = (p.C + KC - 1) / KC;
   const int U = nchunks * p.NG;
 
@@ -117,7 +59,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gconv_tc_kernel(const __grid_co
     uint8_t* dst = slab0 + buf * slab_bytes;
     const int c0 = ch * KC;
     const int total = p.slab_rows * KCH;
-    for (int i = tid; i < total; i += TC_THREADS) {              // (a hand-unrolled 4-loads-in-flight variant measured 8 % slower)
+    for (int i = tid; i < total; i += TC_THREADS) {
       const int r = i / KCH, kc = i - r * KCH;
       const int c = c0 + kc * 4, f = lo + r;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -140,105 +82,86 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gconv_tc_kernel(const __grid_co
     }
   };
 
-  // instruction descriptor: D=f32, A=B=tf32, both K-major, N = BN, M = 128
-  constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-
+  float acc[MT][BN / 2];
   load_slab(0, 0);
   load_w(0, 0, 0);
   cp_async_commit();
-  // Pipeline: unit u uses weight stage u % 3 and slab buffer ch % 2.  The loads of unit u+1 are issued as soon as the
-  // MMAs of unit u-2 have retired (their stage is then free), i.e. while the MMAs of unit u-1 may still be running.
-  // The slab buffer of chunk ch+1 was last read by chunk ch-1, whose last unit is <= u-NG <= u-2 when NG >= 2; for
-  // NG == 1 it is unit u-1, so that case waits for unit u-1 instead.
+  // Pipeline: unit u reads weight stage u % 2 and slab buffer ch % 2.  Its wgmmas are issued first; the loads of unit u+1
+  // (the other weight stage and, at a chunk boundary, the other slab buffer) run while they execute.  Both buffers were
+  // last read by unit u-1, whose wgmmas every thread waited for before the barrier that opens unit u.
   for (int u = 0; u < U; ++u) {
     const int ch = u / p.NG, g = u - ch * p.NG;
-    if (u + 1 < U) {
-      const int ch1 = (u + 1) / p.NG, g1 = (u + 1) - ch1 * p.NG;
-      const int need = u + 1 - NW;                               // youngest unit whose MMAs must have retired (frees stage and slab)
-      if (need >= 0) {
-        mbar_wait(&mbar[need % NW], (need / NW) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;\n");
-      }
-      if (g1 == 0) load_slab(ch1, ch1 & 1);
-      load_w(ch1, g1, (u + 1) % NW);
-      cp_async_commit();
-      cp_async_wait<1>();
-    } else {
-      cp_async_wait<0>();
-    }
+    cp_async_wait<0>();
     asm volatile("fence.proxy.async.shared::cta;\n");           // generic-proxy smem writes -> visible to the tensor core
     __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;\n");
-      const uint32_t sl = smem_u32(slab0 + (ch & 1) * slab_bytes);
+    {
+      const uint32_t sl = smem_u32(slab0 + (ch & 1) * slab_bytes) + (uint32_t)(wg * 64 * 16);
       const uint32_t wt = smem_u32(wt0 + (u % NW) * wt_bytes);
       const int ntaps = min(p.TG, p.Q - g * p.TG);
+      wgmma_fence();
       for (int tq = 0; tq < ntaps; ++tq) {
         const int toff = (p.off[g * p.TG + tq] - p.off_min) * p.P;
         for (int k2 = 0; k2 < KCH / 2; ++k2) {
-          const uint64_t bdesc = make_smem_desc(wt + ((tq * KCH + 2 * k2) * B_PITCH) * 16, B_PITCH * 16, 128);
+          const uint64_t bdesc = wg_desc_plain(wt + ((tq * KCH + 2 * k2) * B_PITCH) * 16, B_PITCH * 16, 128);
 #pragma unroll
           for (int mt = 0; mt < MT; ++mt) {
-            const uint64_t adesc = make_smem_desc(sl + ((2 * k2) * p.a_pitch + mt * 128 + toff) * 16, p.a_pitch * 16, 128);
-            umma_tf32(tmem_base + mt * BN, adesc, bdesc, IDESC, (u | tq | k2) != 0 ? 1u : 0u);
+            const uint64_t adesc = wg_desc_plain(sl + ((2 * k2) * p.a_pitch + mt * 128 + toff) * 16, p.a_pitch * 16, 128);
+            wgmma_tf32<BN>(acc[mt], adesc, bdesc, (u | tq | k2) != 0 ? 1u : 0u);
           }
         }
       }
-      umma_commit(&mbar[u % NW]);
+      wgmma_commit();
     }
+    if (u + 1 < U) {
+      const int ch1 = (u + 1) / p.NG, g1 = (u + 1) - ch1 * p.NG;
+      if (g1 == 0) load_slab(ch1, ch1 & 1);
+      load_w(ch1, g1, (u + 1) % NW);
+      cp_async_commit();
+    }
+    wgmma_wait<0>();
   }
-  // wait for the last commit (all MMAs complete), then epilogue
-  mbar_wait(&mbar[(U - 1) % NW], ((U - 1) / NW) & 1);
-  asm volatile("tcgen05.fence::after_thread_sync;\n");
 
   float* Y = p.y + b * p.y_sb + h * p.y_sh;
   const float* R = p.res ? (p.res + b * p.r_sb + h * p.r_sh) : nullptr;
   const float* bias = p.bias ? (p.bias + h * p.b_sh) : nullptr;
   const int olen = p.out_len ? p.out_len[b] : 0x7fffffff;
-  const int lq = warp & 3, chalf = warp >> 2;
-  constexpr int CW = BN / 2;                                     // columns per warp (two warps share a lane quadrant)
+  // accumulator fragment: d[4j + 2hh + e] = (row 16 (warp % 4) + lane / 4 + 8 hh, column 8 j + 2 (lane % 4) + e)
 #pragma unroll
   for (int mt = 0; mt < MT; ++mt) {
-    const int pos = p0 + mt * 128 + lq * 32 + lane;
-    const int j = pos / p.P, w = pos - j * p.P;
-    const int oj = p.o0 + j * p.os;
-    const long long orow = (long long)oj * p.P + w;
-    const bool live_row = pos < npos;
-    const bool live = oj < olen;
 #pragma unroll
-    for (int c8 = 0; c8 < CW; c8 += 8) {
-      float v[8];
-      const int col = chalf * CW + c8;
-      tmem_ld8(tmem_base + ((uint32_t)(lq * 32) << 16) + (uint32_t)(mt * BN + col), v);   // warp-collective
-      if (!live_row) continue;
-      const int n = n0 + col;
+    for (int hh = 0; hh < 2; ++hh) {
+      const int pos = p0 + mt * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * hh;
+      if (pos >= npos) continue;
+      const int j = pos / p.P, w = pos - j * p.P;
+      const int oj = p.o0 + j * p.os;
+      const long long orow = (long long)oj * p.P + w;
+      const bool live = oj < olen;
+      float* yr = Y + orow * p.ldy;
+      const float* rr = R ? R + orow * p.ldr : nullptr;
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        float t = v[e];
-        if (n + e < p.N) {
-          if (bias) t += bias[n + e];
-          if (R) t += R[orow * p.ldr + n + e];
-          if (p.act == EVK_ACT_LRELU) t = t > 0.f ? t : t * p.slope;
-          else if (p.act == EVK_ACT_RELU) t = fmaxf(t, 0.f);
-          else if (p.act == EVK_ACT_TANH) t = tanhf(t);
-          v[e] = live ? t : 0.f;
+      for (int jn = 0; jn < BN / 8; ++jn) {
+        const int n = n0 + jn * 8 + 2 * (lane & 3);
+        float v[2] = {acc[mt][4 * jn + 2 * hh], acc[mt][4 * jn + 2 * hh + 1]};
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float t = v[e];
+          if (n + e < p.N) {
+            if (bias) t += bias[n + e];
+            if (rr) t += rr[n + e];
+            if (p.act == EVK_ACT_LRELU) t = t > 0.f ? t : t * p.slope;
+            else if (p.act == EVK_ACT_RELU) t = fmaxf(t, 0.f);
+            else if (p.act == EVK_ACT_TANH) t = tanhf(t);
+            v[e] = live ? t : 0.f;
+          }
+        }
+        if (n + 2 <= p.N && ((reinterpret_cast<uintptr_t>(yr + n) & 7) == 0)) {
+          *reinterpret_cast<float2*>(yr + n) = make_float2(v[0], v[1]);
+        } else {
+          if (n < p.N) yr[n] = v[0];
+          if (n + 1 < p.N) yr[n + 1] = v[1];
         }
       }
-      float* yr = Y + orow * p.ldy + n;
-      if (n + 8 <= p.N && ((reinterpret_cast<uintptr_t>(yr) & 15) == 0)) {
-        *reinterpret_cast<float4*>(yr) = make_float4(v[0], v[1], v[2], v[3]);
-        *reinterpret_cast<float4*>(yr + 4) = make_float4(v[4], v[5], v[6], v[7]);
-      } else {
-#pragma unroll
-        for (int e = 0; e < 8; ++e)
-          if (n + e < p.N) yr[e] = v[e];
-      }
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "n"(TCOLS));
   }
 }
 
@@ -258,7 +181,7 @@ static int launch_tc(TP& p, cudaStream_t st) {
   };
   int KCH = p.C >= 32 ? 8 : (p.C >= 16 ? 4 : 2), TG = 1, NG = 1;
   long long smem = plan(KCH, TG, NG);
-  if (smem > 110 * 1024 && KCH == 8) {                            // prefer two resident CTAs per SM
+  if (smem > 110 * 1024 && KCH == 8) {                            // smaller stages when they fit 110 KB (two CTAs per SM where registers allow)
     int tg2, ng2;
     long long s2 = plan(4, tg2, ng2);
     if (s2 <= 110 * 1024) { KCH = 4; TG = tg2; NG = ng2; smem = s2; }
@@ -295,11 +218,8 @@ int gconv_tc_try(const evk_gconv_desc* d, cudaStream_t st) {
   }
   p.off_min = mn; p.off_max = mx;
   const long long npos = (long long)d->J * d->P;
-  const bool two = npos >= 4 * 128;                              // two M tiles per CTA: each weight tile is reused twice (measured: flop/byte wins over CTA count)
+  const bool two = npos >= 4 * 128;                              // two M tiles per CTA: each weight tile is reused twice (flop/byte wins over CTA count)
   const int N = d->N;
-  // 256-wide N tiles double the flops per staged byte, but only pay off when the grid still fills the chip
-  const long long ctas256 = ((npos + 255) / 256) * (N / 256) * (long long)d->Z;
-  if (N >= 256 && (N % 256) == 0 && two && ctas256 >= 2 * 148) return launch_tc<256, 2>(p, st);
   if (N > 64) return two ? launch_tc<128, 2>(p, st) : launch_tc<128, 1>(p, st);
   if (N > 32) return two ? launch_tc<64, 2>(p, st) : launch_tc<64, 1>(p, st);
   if (N > 16) return two ? launch_tc<32, 2>(p, st) : launch_tc<32, 1>(p, st);

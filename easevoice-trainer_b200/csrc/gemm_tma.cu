@@ -1,37 +1,39 @@
-// TMA-fed, warp-specialised, persistent tcgen05 GEMM (sm_100a):   D[M][N] (+)= epi( A[M][K] * B[N][K]^T )
-// fp32 storage, TF32 tensor-core math, fp32 accumulation in TMEM.  Serves every dense contraction without taps:
+// TMA-fed, warp-specialised, persistent wgmma GEMM (sm_90a):   D[M][N] (+)= epi( A[M][K] * B[N][K]^T )
+// fp32 storage, TF32 tensor-core math, fp32 accumulation in registers.  Serves every dense contraction without taps:
 // nn.Linear / 1x1 conv forward (A = activations rows, B = packed weight [N][C]), their data gradients
 // (A = dY rows, B = packed transposed weight [C][N]) and -- through evk_gemm_tf32 with split-K -- weight gradients
 // on pre-transposed operands.
 //
 //   warp 0 (one lane)  : TMA producer.  cp.async.bulk.tensor 2-D boxes [128 x 32 fl] (A) and [BN x 32 fl] (B), 128-byte
-//                        swizzle, into a STAGES-deep shared-memory ring; full[s] mbarrier with expect_tx.
-//   warp 1 (one lane)  : MMA issuer.  4 x tcgen05.mma.kind::tf32 (K = 8) per stage, descriptors advance 32 B inside the
-//                        128-byte swizzle atom; tcgen05.commit -> empty[s] releases the stage, -> acc_full[a] after
-//                        the last K block of a tile.
-//   warps 2..5         : epilogue.  tcgen05.ld 32x32b.x32 from the accumulator (each warp owns its TMEM lane quadrant),
-//                        bias / residual / activation, 128-byte row segments to global (or fp32 atomics for split-K),
-//                        then arrive on acc_empty[a].
-// Two TMEM accumulators (2 x BN columns) let the epilogue of tile i overlap the main loop of tile i+1; CTAs are
-// persistent (one per SM) and walk the tile list n-fastest so that concurrent CTAs share the A row block in L2.
+//                        swizzle, into SA / SB-deep shared-memory rings; full[s] mbarrier with expect_tx.
+//   warps 4..11        : two consumer warpgroups.  Warpgroup g owns rows 64 g .. 64 g + 63 of every 128-row block: per
+//                        stage 4 x wgmma.m64nBNk8 (K = 8) per block, descriptors advance 32 B inside the 128-byte swizzle
+//                        atom.  One wgmma group stays in flight; when the previous group has retired its stages are
+//                        released (empty[s], one arrival per consumer warp).  After the last K block of a tile the
+//                        warpgroup runs the epilogue from its registers: bias / residual / activation / dropout, 128-byte
+//                        row segments to global (split-K: to a per-split partial), while the producer already stages the next
+//                        tile.
+// CTAs are persistent (one per SM) and walk the tile list n-fastest so that concurrent CTAs share the A row block in L2.
 // Out-of-range rows / K tails are zero-filled by TMA, so no shape needs padding.
 #include <cuda.h>
-#include <cstdlib>
 
-#include "evk_common.cuh"
+#include "wgmma.cuh"
 
 namespace evk {
 namespace {
 
 constexpr int BM = 128, BK = 32;                    // 32 floats = one 128-byte swizzle row
-constexpr int GT_THREADS = 320;                     // TMA producer warp, MMA warp, eight epilogue warps
+constexpr int GT_THREADS = 384;                     // producer warpgroup (warp 0 issues TMA) + two consumer warpgroups
+constexpr int CONSUMER_WARPS = 8;
 
 struct GemmP {
   float* d; int ldd;
   const float* bias; const float* res; int ldr;
   int M, N, K, act; float slope;                     // M = output positions per batch item, K = input channels
   int tiles_m, tiles_n, splits, kb_per_split;        // kb = K blocks of 32
-  int atomic;
+  int atomic;                                        // accumulate into d: with d_ssp > 0 each K split stores its partial at
+                                                     // d + split * d_ssp (ordered_sum adds them), with d_ssp == 0 (one split) d += result
+  long long d_ssp;
   // implicit-GEMM convolution mode (stride 1): Z batch items, Q taps, period P; tap q reads input row pos + off[q]*P
   int Z, Q, P;
   int os, o0;                                        // output position of tile row pos: ((o0 + (pos / P) * os) * P + pos % P)
@@ -62,64 +64,20 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "@p bra DONE_%=;\n"
       "bra WAIT_%=;\n"
       "DONE_%=:\n"
-      "}\n" ::"r"(smem_u32(bar)), "r"(parity));
+      "}\n" ::"r"(smem_u32(bar)), "r"(parity)
+      : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(bytes));
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)));
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];\n" ::"r"(smem_u32(dst)),
                "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
                : "memory");
 }
-// K-major, SWIZZLE_128B: start>>4 | LBO(ignored)=1 | SBO = 1024 B (8 rows x 128 B) | version 1 | layout 2
-__device__ __forceinline__ uint64_t sw128_desc(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t taddr, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(taddr), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum));
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.b64 [%0];\n" ::"l"(__cvta_generic_to_shared(bar)));
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-#ifdef GT_PROFILE
-// developer build only (tools/exp/gt_profile.py): per-CTA cycle counters of the three roles.  Each role accumulates in
-// registers (prof_acc[]) and flushes once when it leaves its loop -- a global read-modify-write per wait would cost more
-// than the waits being measured.
-__device__ unsigned long long g_gt_prof[160 * 16];
-#define PROF_DECL() unsigned long long prof_acc[4] = {0ull, 0ull, 0ull, 0ull}
-#define PROF_WAIT(i, stmt) do { const long long prof_t0 = clock64(); stmt; prof_acc[i] += (unsigned long long)(clock64() - prof_t0); } while (0)
-#define PROF_INC(i) prof_acc[i] += 1ull
-#define PROF_FLUSH(i, slot) g_gt_prof[blockIdx.x * 16 + (slot)] += prof_acc[i]
-#else
-#define PROF_DECL()
-#define PROF_WAIT(i, stmt) stmt
-#define PROF_INC(i)
-#define PROF_FLUSH(i, slot)
-#endif
 
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -133,16 +91,15 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-// Fast epilogue rows of one 32 x 32 chunk: this lane owns columns nn .. nn+3 of rows i*4 + r_sub (i = 0..7).  Straight-line
-// code: the only conditionals left are single predicated loads / stores (the branchy general path cost ~4800 cycles per
-// chunk against ~500 for this one -- tools/exp/gt_profile.py -- and made the GPT Linear layers epilogue-bound).
+// Fast epilogue rows of one 16 x 32 chunk: this lane owns columns nn .. nn+3 of rows i*4 + r_sub (i = 0..3).  Straight-line
+// code: the only conditionals left are single predicated loads / stores.
 template <bool RES, bool DROP>
 __device__ __forceinline__ void epi_rows_fast(const float* __restrict__ tr, int r_sub, int c4, float4 bv, float* __restrict__ dz,
-                                              const float* __restrict__ rz, const size_t (&orow)[8], const bool (&keep)[8],
-                                              const bool (&ok)[8], int ldd, int ldr, int nn, float neg, const DropK& dropk,
+                                              const float* __restrict__ rz, const size_t (&orow)[4], const bool (&keep)[4],
+                                              const bool (&ok)[4], int ldd, int ldr, int nn, float neg, const DropK& dropk,
                                               const float* dbase) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
+  for (int i = 0; i < 4; ++i) {
     float4 t = *reinterpret_cast<const float4*>(tr + (i * 4 + r_sub) * 36 + c4);
     float* dp = dz + orow[i] * ldd + nn;
     t.x += bv.x; t.y += bv.y; t.z += bv.z; t.w += bv.w;
@@ -162,18 +119,92 @@ __device__ __forceinline__ void epi_rows_fast(const float* __restrict__ tr, int 
   }
 }
 
+// One 16-row x 32-column chunk of a warp's accumulator, staged row-major in `tr` (pitch 36), to global memory.
+// Lane owns columns c4 .. c4+3 of rows i*4 + r_sub.
+__device__ __forceinline__ void epi_chunk(const GemmP& p, const float* __restrict__ tr, int lane, int n, float* dz, const float* rz,
+                                          const size_t (&orow)[4], const bool (&keep)[4], const bool (&inside)[4], float neg,
+                                          const DropK& dropk) {
+  const int r_sub = lane >> 3, c4 = (lane & 7) * 4;
+  const int nn = n + c4;
+  if (p.fast) {
+    const bool colok = nn < p.N;                          // N % 4 == 0: the float4 is entirely inside or outside
+    float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (p.bias && colok) bv = *reinterpret_cast<const float4*>(p.bias + nn);
+    bool ok[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) ok[i] = inside[i] && colok;
+    if (dropk.thr) {
+      if (rz) epi_rows_fast<true, true>(tr, r_sub, c4, bv, dz, rz, orow, keep, ok, p.ldd, p.ldr, nn, neg, dropk, p.d);
+      else epi_rows_fast<false, true>(tr, r_sub, c4, bv, dz, rz, orow, keep, ok, p.ldd, p.ldr, nn, neg, dropk, p.d);
+    } else if (rz) {
+      epi_rows_fast<true, false>(tr, r_sub, c4, bv, dz, rz, orow, keep, ok, p.ldd, p.ldr, nn, neg, dropk, p.d);
+    } else {
+      epi_rows_fast<false, false>(tr, r_sub, c4, bv, dz, rz, orow, keep, ok, p.ldd, p.ldr, nn, neg, dropk, p.d);
+    }
+    return;
+  }
+  float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
+  const bool full4 = nn + 4 <= p.N;
+  if (p.bias && !p.atomic) {
+    if (full4 && ((reinterpret_cast<uintptr_t>(p.bias + nn) & 15) == 0)) bv = *reinterpret_cast<const float4*>(p.bias + nn);
+    else { if (nn < p.N) bv.x = p.bias[nn]; if (nn + 1 < p.N) bv.y = p.bias[nn + 1]; if (nn + 2 < p.N) bv.z = p.bias[nn + 2]; if (nn + 3 < p.N) bv.w = p.bias[nn + 3]; }
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    if (!inside[i] || nn >= p.N) continue;
+    const float4 tv = *reinterpret_cast<const float4*>(tr + (i * 4 + r_sub) * 36 + c4);
+    float t[4] = {tv.x, tv.y, tv.z, tv.w};
+    float* dp = dz + orow[i] * p.ldd + nn;
+    if (p.atomic) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        if (nn + e < p.N) dp[e] = p.d_ssp ? t[e] : dp[e] + t[e];
+      continue;
+    }
+    t[0] += bv.x; t[1] += bv.y; t[2] += bv.z; t[3] += bv.w;
+    if (rz) {
+      const float* rp = rz + orow[i] * p.ldr + nn;
+      if (full4 && ((reinterpret_cast<uintptr_t>(rp) & 15) == 0)) {
+        const float4 rv = *reinterpret_cast<const float4*>(rp);
+        t[0] += rv.x; t[1] += rv.y; t[2] += rv.z; t[3] += rv.w;
+      } else {
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (nn + e < p.N) t[e] += rp[e];
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      if (p.act == EVK_ACT_LRELU) t[e] = t[e] > 0.f ? t[e] : t[e] * p.slope;
+      else if (p.act == EVK_ACT_RELU) t[e] = fmaxf(t[e], 0.f);
+      else if (p.act == EVK_ACT_TANH) t[e] = tanhf(t[e]);
+      if (!keep[i]) t[e] = 0.f;
+    }
+    if (dropk.thr) {                                     // group index = offset of the float4 in the output tensor / 4
+      float m[4];
+      dropk_scale4(dropk, (unsigned long long)(dp - p.d) >> 2, m);
+      t[0] *= m[0]; t[1] *= m[1]; t[2] *= m[2]; t[3] *= m[3];
+    }
+    if (full4 && ((reinterpret_cast<uintptr_t>(dp) & 15) == 0)) {
+      *reinterpret_cast<float4*>(dp) = make_float4(t[0], t[1], t[2], t[3]);
+    } else {
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        if (nn + e < p.N) dp[e] = t[e];
+    }
+  }
+}
+
 struct MapB4 { CUtensorMap m[4]; };                  // B: mode 1 uses one map per delayed copy of X^T, mode 0 only m[0]
                                                      // A: mode 0 uses one map per stride phase of the input, mode 1 only m[0];
                                                      //    slab mode: m[1] = the same tensor with a `span`-row box (the slab tail)
 constexpr int MAX_RING = 8;
 
 // One CTA per SM, persistent over the tile list.  Tile = (MT x 128) output rows x BN output channels.
-//   MT = 2 : two 128-row accumulators share every weight (B) tile -> half the L2->SM weight traffic per flop.
+//   MT = 2 : two 128-row blocks share every weight (B) tile -> half the L2->SM weight traffic per flop.
 //   slab   : stride-1 tap sums stage ONE input slab of MT*128 + span rows per channel block and run every tap from it
-//            (tap q = the A descriptor advanced by (off[q] - off_min) * P rows; the 128-byte swizzle is a function of the
-//            shared-memory ADDRESS, so any row offset is a valid descriptor start -- tools/exp/slab_desc.cu measured
-//            all 24 shifts exact with base_offset = 0).  The round-1 kernel re-fetched the A box for every tap from L2
-//            (21x operand re-read on the k = 11 layers, 25 % tensor-pipe, L2->SM bandwidth bound at 46.6 B/clk/SM).
+//            (tap q = the A descriptor advanced by (off[q] - off_min) * P rows; see wg_desc_sw128) instead of re-fetching the
+//            A box of every tap from L2.
 template <int BN, int MT>
 __global__ void __launch_bounds__(GT_THREADS, 1) gemm_tma_kernel(const __grid_constant__ MapB4 mapA4,
                                                                  const __grid_constant__ MapB4 mapB4,
@@ -181,39 +212,22 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gemm_tma_kernel(const __grid_co
   const CUtensorMap& mapA = mapA4.m[0];
   const CUtensorMap& mapB = mapB4.m[0];
   constexpr int B_BYTES = BN * BK * 4;
-  constexpr int NACC = (2 * MT * BN <= 512) ? 2 : 1;
-  constexpr int TCOLS_RAW = NACC * MT * BN;
-  constexpr int TCOLS = TCOLS_RAW <= 32 ? 32 : TCOLS_RAW <= 64 ? 64 : TCOLS_RAW <= 128 ? 128 : TCOLS_RAW <= 256 ? 256 : 512;
-  static_assert(TCOLS_RAW <= 512, "TMEM columns");
   extern __shared__ uint8_t gsm_raw[];
   uint8_t* gsm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(gsm_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* gsmB = gsm + (size_t)p.SA * p.a_stage;           // B ring behind the A ring (a_stage is a multiple of 1024)
-  __shared__ __align__(8) uint64_t fullA[MAX_RING], emptyA[MAX_RING], fullB[MAX_RING], emptyB[MAX_RING], acc_full[2], acc_empty[2];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ __align__(16) float epi_s[8 * 32 * 36];            // per-epilogue-warp transpose tile (pitch 36: 128-bit conflict-free)
+  __shared__ __align__(8) uint64_t fullA[MAX_RING], emptyA[MAX_RING], fullB[MAX_RING], emptyB[MAX_RING];
+  __shared__ __align__(16) float epi_s[CONSUMER_WARPS * 16 * 36];   // per-consumer-warp transpose tile (pitch 36: 128-bit conflict-free)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#ifdef GT_PROFILE
-  const long long prof_start = clock64();
-#endif
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < MAX_RING; ++i) { mbar_init(&fullA[i], 1); mbar_init(&emptyA[i], 1); mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], BN >= 64 ? 8 : 4); }   // = participating epilogue warps
+    for (int i = 0; i < MAX_RING; ++i) {
+      mbar_init(&fullA[i], 1); mbar_init(&emptyA[i], CONSUMER_WARPS); mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], CONSUMER_WARPS);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;\n");
     asm volatile("prefetch.tensormap [%0];\n" ::"l"(reinterpret_cast<uint64_t>(&mapA4.m[0])));
     asm volatile("prefetch.tensormap [%0];\n" ::"l"(reinterpret_cast<uint64_t>(&mapB4.m[0])));
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(&tmem_base_s)), "n"(TCOLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n");
-  const uint32_t tmem_base = tmem_base_s;
-#ifdef GT_PROFILE
-  if (threadIdx.x == 0) g_gt_prof[blockIdx.x * 16 + 9] += (unsigned long long)(clock64() - prof_start);
-#endif
 
   const int tiles_mn = p.tiles_m * p.tiles_n;
   // mode 0: tile -> (outer = batch item or K split, m tile, n tile); K iterations = taps x channel blocks (splits > 1 only
@@ -227,188 +241,170 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gemm_tma_kernel(const __grid_co
   };
   const int slab = p.slab;
 
-  // Both single-thread loops below run once per (tap, channel block) step and must stay well under the 128..256 cycles the
-  // MMAs of a step take: ring positions and the (tap, block) decomposition are carried incrementally -- no integer
-  // division or modulo by run-time values inside the step loops.
+  // Both loops below run once per (tap, channel block) step: ring positions and the (tap, block) decomposition are carried
+  // incrementally -- no integer division or modulo by run-time values inside the step loops.
   const int SA = p.SA, SB = p.SB, Q = p.Q;
   if (warp == 0) {
     // The whole warp walks the tile list with warp-uniform state; only the elected lane touches the barriers' tx counts and
-    // issues the TMA.  (Running the loop under `lane == 0` made the compiler wrap every UTMALDG / UTCHMMA in a
-    // divergence "waterfall" loop with R2UR moves: ~480 cycles per 4-MMA step, twice the tensor time at BN = 128.)
-    {
-      int sA = 0, phA = 1, sB = 0, phB = 1;                      // empty barriers: the first pass over a ring passes immediately
-      PROF_DECL();
-      const bool leader = elect_one();
-      for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-        const int outer = tile / tiles_mn, mn = tile - outer * tiles_mn;
-        const int tm = mn / p.tiles_n, tn = mn - tm * p.tiles_n;
-        const int z = (p.splits > 1 || p.mode) ? 0 : outer;
-        auto next_a = [&]() -> uint8_t* {
-          PROF_WAIT(0, mbar_wait(&emptyA[sA], phA));
-          if (leader) mbar_expect_tx(&fullA[sA], (uint32_t)p.a_bytes);
-          return gsm + (size_t)sA * p.a_stage;
-        };
-        auto done_a = [&]() { if (++sA == SA) { sA = 0; phA ^= 1; } };
-        auto next_b = [&]() -> uint8_t* {
-          PROF_WAIT(1, mbar_wait(&emptyB[sB], phB));
-          if (leader) mbar_expect_tx(&fullB[sB], B_BYTES);
-          return gsmB + (size_t)sB * B_BYTES;
-        };
-        auto done_b = [&]() { if (++sB == SB) { sB = 0; phB ^= 1; } };
-        if (slab) {
-          const int row0 = tm * (MT * BM) + p.off_min * p.P;
+    // issues the TMA (a loop under `lane == 0` makes the compiler wrap every TMA issue in a divergence loop).
+    int sA = 0, phA = 1, sB = 0, phB = 1;                      // empty barriers: the first pass over a ring passes immediately
+    const bool leader = elect_one();
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+      const int outer = tile / tiles_mn, mn = tile - outer * tiles_mn;
+      const int tm = mn / p.tiles_n, tn = mn - tm * p.tiles_n;
+      const int z = (p.splits > 1 || p.mode) ? 0 : outer;
+      auto next_a = [&]() -> uint8_t* {
+        mbar_wait(&emptyA[sA], phA);
+        if (leader) mbar_expect_tx(&fullA[sA], (uint32_t)p.a_bytes);
+        return gsm + (size_t)sA * p.a_stage;
+      };
+      auto done_a = [&]() { if (++sA == SA) { sA = 0; phA ^= 1; } };
+      auto next_b = [&]() -> uint8_t* {
+        mbar_wait(&emptyB[sB], phB);
+        if (leader) mbar_expect_tx(&fullB[sB], B_BYTES);
+        return gsmB + (size_t)sB * B_BYTES;
+      };
+      auto done_b = [&]() { if (++sB == SB) { sB = 0; phB ^= 1; } };
+      if (slab) {
+        const int row0 = tm * (MT * BM) + p.off_min * p.P;
+        for (int kb = 0; kb < kb_total; ++kb) {
+          uint8_t* sa = next_a();
+          if (leader) tma_load_3d(sa, &mapA, kb * BK, row0, z, &fullA[sA]);
+          if (leader) tma_load_3d(sa + MT * BM * BK * 4, &mapA4.m[1], kb * BK, row0 + MT * BM, z, &fullA[sA]);
+          done_a();
+          for (int q = 0; q < Q; ++q) {
+            uint8_t* sb = next_b();
+            if (leader) tma_load_3d(sb, &mapB, kb * BK, tn * BN, q, &fullB[sB]);
+            done_b();
+          }
+        }
+      } else if (!p.mode && p.splits == 1) {
+        for (int q = 0; q < Q; ++q) {
+          const CUtensorMap* am = &mapA4.m[p.src[q]];
+          const int arow = tm * (MT * BM) + p.off[q] * p.P;
           for (int kb = 0; kb < kb_total; ++kb) {
             uint8_t* sa = next_a();
-            if (leader) tma_load_3d(sa, &mapA, kb * BK, row0, z, &fullA[sA]);
-            if (leader) tma_load_3d(sa + MT * BM * BK * 4, &mapA4.m[1], kb * BK, row0 + MT * BM, z, &fullA[sA]);
+            if (leader) tma_load_3d(sa, am, kb * BK, arow, z, &fullA[sA]);
             done_a();
-            for (int q = 0; q < Q; ++q) {
-              uint8_t* sb = next_b();
-              if (leader) tma_load_3d(sb, &mapB, kb * BK, tn * BN, q, &fullB[sB]);
-              done_b();
-            }
-          }
-        } else if (!p.mode && p.splits == 1) {
-          for (int q = 0; q < Q; ++q) {
-            const CUtensorMap* am = &mapA4.m[p.src[q]];
-            const int arow = tm * (MT * BM) + p.off[q] * p.P;
-            for (int kb = 0; kb < kb_total; ++kb) {
-              uint8_t* sa = next_a();
-              if (leader) tma_load_3d(sa, am, kb * BK, arow, z, &fullA[sA]);
-              done_a();
-              uint8_t* sb = next_b();
-              if (leader) tma_load_3d(sb, &mapB, kb * BK, tn * BN, q, &fullB[sB]);
-              done_b();
-            }
-          }
-        } else {
-          int k0, k1;
-          k_range(outer, k0, k1);
-          if (p.mode) {
-            const int q = outer / p.splits;
-            // TMA needs the inner coordinate 16-byte aligned: X[t + sh] is read from the copy delayed by r = (-sh) mod 4
-            // (xt_r[u] = X[u - r]) at the aligned coordinate t + sh + r
-            const int sh = p.off[q] * p.P, r = (((-sh) % 4) + 4) % 4;
-            int b = k0 / p.kbs, kk = k0 - b * p.kbs;
-            for (int ki = k0; ki < k1; ++ki) {
-              uint8_t* sa = next_a();
-              if (leader) tma_load_3d(sa, &mapA, kk * BK, tm * BM, b, &fullA[sA]);
-              done_a();
-              uint8_t* sb = next_b();
-              if (leader) tma_load_3d(sb, &mapB4.m[r], kk * BK + (sh + r), tn * BN, b, &fullB[sB]);
-              done_b();
-              if (++kk == p.kbs) { kk = 0; ++b; }
-            }
-          } else {                                               // split-K plain GEMM (Z == Q == 1)
-            for (int kb = k0; kb < k1; ++kb) {
-              uint8_t* sa = next_a();
-              if (leader) tma_load_3d(sa, &mapA, kb * BK, tm * (MT * BM), 0, &fullA[sA]);
-              done_a();
-              uint8_t* sb = next_b();
-              if (leader) tma_load_3d(sb, &mapB, kb * BK, tn * BN, 0, &fullB[sB]);
-              done_b();
-            }
+            uint8_t* sb = next_b();
+            if (leader) tma_load_3d(sb, &mapB, kb * BK, tn * BN, q, &fullB[sB]);
+            done_b();
           }
         }
-      }
-      if (leader) { PROF_FLUSH(0, 1); PROF_FLUSH(1, 2); }
-    }
-  } else if (warp == 1) {
-    {
-      PROF_DECL();
-      const bool leader = elect_one();
-      // instruction descriptor: D = f32, A = B = tf32, both K-major, N = BN, M = 128
-      constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      int sA = 0, phA = 0, sB = 0, phB = 0, tcount = 0;
-      const uint32_t a_ring = smem_u32(gsm), b_ring = smem_u32(gsmB);
-      for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++tcount) {
-        const int a = tcount % NACC;
-        PROF_WAIT(2, mbar_wait(&acc_empty[a], ((tcount / NACC) & 1) ^ 1));
-        PROF_INC(3);
-        asm volatile("tcgen05.fence::after_thread_sync;\n");
-        const uint32_t tacc = tmem_base + (uint32_t)(a * MT * BN);
-        uint32_t accum = 0;
-        // one step: MT x 4 MMAs of (128 x BN x 8) from A rows starting `a_off` bytes into the current A stage
-        auto step = [&](uint32_t a_off) {
-          PROF_WAIT(1, mbar_wait(&fullB[sB], phB));
-          asm volatile("tcgen05.fence::after_thread_sync;\n");
-          const uint32_t a_addr = a_ring + (uint32_t)sA * (uint32_t)p.a_stage + a_off;
-          const uint64_t db = sw128_desc(b_ring + (uint32_t)sB * B_BYTES);
-          if (leader) {
-#pragma unroll
-            for (int mt = 0; mt < MT; ++mt) {
-              const uint64_t da = sw128_desc(a_addr + (uint32_t)(mt * BM * BK * 4));
-#pragma unroll
-              for (int k = 0; k < BK / 8; ++k) umma_tf32(tacc + (uint32_t)(mt * BN), da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), IDESC, accum | (uint32_t)k);
-            }
-            umma_commit(&emptyB[sB]);
-          }
-          accum = 1;
-          if (++sB == SB) { sB = 0; phB ^= 1; }
-        };
-        auto wait_a = [&]() { PROF_WAIT(0, mbar_wait(&fullA[sA], phA)); };
-        auto free_a = [&]() { if (leader) umma_commit(&emptyA[sA]); if (++sA == SA) { sA = 0; phA ^= 1; } };
-        if (slab) {
-          for (int kb = 0; kb < kb_total; ++kb) {
-            wait_a();
-            for (int q = 0; q < Q; ++q) step((uint32_t)((p.off[q] - p.off_min) * p.P) * (BK * 4));
-            free_a();
-          }
-        } else {
-          int k0, k1;
-          k_range(tile / tiles_mn, k0, k1);
+      } else {
+        int k0, k1;
+        k_range(outer, k0, k1);
+        if (p.mode) {
+          const int q = outer / p.splits;
+          // TMA needs the inner coordinate 16-byte aligned: X[t + sh] is read from the copy delayed by r = (-sh) mod 4
+          // (xt_r[u] = X[u - r]) at the aligned coordinate t + sh + r
+          const int sh = p.off[q] * p.P, r = (((-sh) % 4) + 4) % 4;
+          int b = k0 / p.kbs, kk = k0 - b * p.kbs;
           for (int ki = k0; ki < k1; ++ki) {
-            wait_a();
-            step(0);
-            free_a();
+            uint8_t* sa = next_a();
+            if (leader) tma_load_3d(sa, &mapA, kk * BK, tm * BM, b, &fullA[sA]);
+            done_a();
+            uint8_t* sb = next_b();
+            if (leader) tma_load_3d(sb, &mapB4.m[r], kk * BK + (sh + r), tn * BN, b, &fullB[sB]);
+            done_b();
+            if (++kk == p.kbs) { kk = 0; ++b; }
+          }
+        } else {                                               // split-K plain GEMM (Z == Q == 1)
+          for (int kb = k0; kb < k1; ++kb) {
+            uint8_t* sa = next_a();
+            if (leader) tma_load_3d(sa, &mapA, kb * BK, tm * (MT * BM), 0, &fullA[sA]);
+            done_a();
+            uint8_t* sb = next_b();
+            if (leader) tma_load_3d(sb, &mapB, kb * BK, tn * BN, 0, &fullB[sB]);
+            done_b();
           }
         }
-        if (leader) umma_commit(&acc_full[a]);
       }
-      if (leader) { PROF_FLUSH(0, 3); PROF_FLUSH(1, 4); PROF_FLUSH(2, 5); PROF_FLUSH(3, 8); }
     }
-  } else {
-    // ---- epilogue: EIGHT warps.  ncu (profiles/r2_ncu_gemm_tma.md) showed the round-1 epilogue -- four warps, one per
-    // scheduler, scalar shared-memory transposes and two integer divisions per row -- taking ~3x the main loop of a
-    // K = 11 x 128 tile: the tensor pipe idled at 30 % waiting for acc_empty no matter how the operands were staged.
-    // Now two warps share each TMEM lane quadrant (they split the 32-column chunks), the transpose tile is float4 in and
-    // float4 out (pitch 36: conflict-free for 128-bit accesses), and the row -> output-row mapping is computed once per
-    // 128-row block (no division at all when P == 1).
-    const int ew = warp - 2;
-    const int lq = warp & 3;                                    // TMEM lane quadrant this warp may read (hardware: warp id % 4)
-    const int half = ew >> 2;
-    constexpr int CHUNKS = BN / 32;
-    constexpr int NHALF = CHUNKS >= 2 ? 2 : 1;
-    if (half < NHALF) {
-    float* tr = epi_s + ew * (32 * 36);
-    const int r_sub = lane >> 3, c4 = (lane & 7) * 4;
+  } else if (warp >= 4) {
+    const int cw = warp - 4;                                   // consumer warp 0..7
+    const int wg = cw >> 2, wq = cw & 3;                       // warpgroup (64-row half of a 128-row block), warp in it (16 rows)
+    float* tr = epi_s + cw * (16 * 36);
     const float comp = p.comp;
     const DropK dropk = dropk_make(p.drop_rng, p.drop_sid, p.drop_p);
     const float neg = p.act == EVK_ACT_LRELU ? p.slope : (p.act == EVK_ACT_RELU ? 0.f : 1.f);   // fast path: x > 0 ? x : x * neg
-    int tcount = 0;
-    PROF_DECL();
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++tcount) {
+    int sA = 0, phA = 0, sB = 0, phB = 0;
+    const uint32_t a_ring = smem_u32(gsm) + (uint32_t)(wg * 64 * BK * 4), b_ring = smem_u32(gsmB);
+    float acc[MT][BN / 2];
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+      // ---- main loop: one wgmma group per step in flight; the stages of the step before it are released once it retires
+      int relA = -1, relB = -1;
+      uint32_t accum = 0;
+      auto step = [&](uint32_t a_off) {
+        mbar_wait(&fullB[sB], phB);
+        const int ra = relA;
+        relA = -1;
+        const uint32_t a_addr = a_ring + (uint32_t)sA * (uint32_t)p.a_stage + a_off;
+        const uint64_t db = wg_desc_sw128(b_ring + (uint32_t)sB * B_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt) {
+          const uint64_t da = wg_desc_sw128(a_addr + (uint32_t)(mt * BM * BK * 4));
+#pragma unroll
+          for (int k = 0; k < BK / 8; ++k) wgmma_tf32<BN>(acc[mt], da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), accum | (uint32_t)k);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (lane == 0) {
+          if (relB >= 0) mbar_arrive(&emptyB[relB]);
+          if (ra >= 0) mbar_arrive(&emptyA[ra]);
+        }
+        relB = sB;
+        accum = 1;
+        if (++sB == SB) { sB = 0; phB ^= 1; }
+      };
+      auto wait_a = [&]() { mbar_wait(&fullA[sA], phA); };
+      auto free_a = [&]() { relA = sA; if (++sA == SA) { sA = 0; phA ^= 1; } };
+      if (slab) {
+        for (int kb = 0; kb < kb_total; ++kb) {
+          wait_a();
+          for (int q = 0; q < Q; ++q) step((uint32_t)((p.off[q] - p.off_min) * p.P) * (BK * 4));
+          free_a();
+        }
+      } else {
+        int k0, k1;
+        k_range(tile / tiles_mn, k0, k1);
+        for (int ki = k0; ki < k1; ++ki) {
+          wait_a();
+          step(0);
+          free_a();
+        }
+      }
+      wgmma_wait<0>();
+      if (lane == 0) {
+        if (relB >= 0) mbar_arrive(&emptyB[relB]);
+        if (relA >= 0) mbar_arrive(&emptyA[relA]);
+      }
+      if (!accum) {                                            // empty K range (cannot happen for a listed tile): write zeros
+#pragma unroll
+        for (int mt = 0; mt < MT; ++mt)
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[mt][i] = 0.f;
+      }
+
+      // ---- epilogue from registers
       const int outer = tile / tiles_mn, mn = tile - outer * tiles_mn;
       const int tm = mn / p.tiles_n, tn = mn - tm * p.tiles_n;
       const int z = (p.splits > 1 || p.mode) ? 0 : outer;
       float* dz = p.mode ? p.d + (size_t)(outer / p.splits) * p.d_sq : p.d + (size_t)z * p.y_sb;
+      if (p.atomic) dz += (size_t)(p.mode ? outer % p.splits : outer) * p.d_ssp;
       const float* rz = p.res ? p.res + (size_t)z * p.r_sb : nullptr;
       const int olen = p.out_len ? p.out_len[z] : 0x7fffffff;
-      const int a = tcount % NACC;
-      PROF_WAIT(0, mbar_wait(&acc_full[a], (tcount / NACC) & 1));
-#ifdef GT_PROFILE
-      const long long prof_e1 = clock64();
-#endif
-      asm volatile("tcgen05.fence::after_thread_sync;\n");
-#pragma unroll 1
-      for (int mt = 0; mt < MT; ++mt) {
-        const int row_base = tm * (MT * BM) + mt * BM + lq * 32;
-        if (row_base >= p.M) continue;                           // warp-uniform: nothing of this quadrant is inside the problem
-        // this lane's 8 rows (rl = i*4 + r_sub): output row index and length-mask flag, once per block
-        size_t orow[8];
-        bool keep[8], inside[8];
+      const int r_sub = lane >> 3;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
+      for (int mt = 0; mt < MT; ++mt) {
+        const int row_base = tm * (MT * BM) + mt * BM + wg * 64 + wq * 16;
+        if (row_base >= p.M) continue;                           // warp-uniform: nothing of this warp's rows is inside the problem
+        // this lane's 4 rows (rl = i*4 + r_sub): output row index and length-mask flag, once per block
+        size_t orow[4];
+        bool keep[4], inside[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
           const int row = row_base + i * 4 + r_sub;
           inside[i] = row < p.M;
           int jo;
@@ -416,107 +412,25 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gemm_tma_kernel(const __grid_co
           else { const int jq = row / p.P; jo = p.o0 + jq * p.os; orow[i] = (size_t)jo * p.P + (row - jq * p.P); }
           keep[i] = jo < olen;
         }
-#pragma unroll 1
-        for (int c = half; c < CHUNKS; c += NHALF) {
-          const int c0 = c * 32;
-          const int n = tn * BN + c0;
+#pragma unroll
+        for (int c = 0; c < BN / 32; ++c) {
+          const int n = tn * BN + c * 32;
           if (n >= p.N) break;                                   // warp-uniform
-          float v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(lq * 32) << 16) + (uint32_t)(a * MT * BN + mt * BN + c0), v);
-          float4* trw = reinterpret_cast<float4*>(tr + lane * 36);
+          // fragment -> row-major 16 x 32 tile: d[4j + 2h + e] = (row lane/4 + 8h, column 8j + 2(lane%4) + e)
 #pragma unroll
-          for (int e = 0; e < 8; ++e) trw[e] = make_float4(v[4 * e] * comp, v[4 * e + 1] * comp, v[4 * e + 2] * comp, v[4 * e + 3] * comp);
+          for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int j = c * 4 + jj;
+              *reinterpret_cast<float2*>(tr + ((lane >> 2) + 8 * h) * 36 + jj * 8 + 2 * (lane & 3)) =
+                  make_float2(acc[mt][4 * j + 2 * h] * comp, acc[mt][4 * j + 2 * h + 1] * comp);
+            }
           __syncwarp();
-          const int nn = n + c4;
-          if (p.fast) {
-            const bool colok = nn < p.N;                          // N % 4 == 0: the float4 is entirely inside or outside
-            float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.bias && colok) bv = *reinterpret_cast<const float4*>(p.bias + nn);
-            bool ok[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) ok[i] = inside[i] && colok;
-            if (dropk.thr) {
-              if (rz) epi_rows_fast<true, true>(tr, r_sub, c4, bv, dz, rz, orow, keep, ok, p.ldd, p.ldr, nn, neg, dropk, p.d);
-              else epi_rows_fast<false, true>(tr, r_sub, c4, bv, dz, rz, orow, keep, ok, p.ldd, p.ldr, nn, neg, dropk, p.d);
-            } else if (rz) {
-              epi_rows_fast<true, false>(tr, r_sub, c4, bv, dz, rz, orow, keep, ok, p.ldd, p.ldr, nn, neg, dropk, p.d);
-            } else {
-              epi_rows_fast<false, false>(tr, r_sub, c4, bv, dz, rz, orow, keep, ok, p.ldd, p.ldr, nn, neg, dropk, p.d);
-            }
-            __syncwarp();
-            continue;
-          }
-          float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-          const bool full4 = nn + 4 <= p.N;
-          if (p.bias && !p.atomic) {
-            if (full4 && ((reinterpret_cast<uintptr_t>(p.bias + nn) & 15) == 0)) bv = *reinterpret_cast<const float4*>(p.bias + nn);
-            else { if (nn < p.N) bv.x = p.bias[nn]; if (nn + 1 < p.N) bv.y = p.bias[nn + 1]; if (nn + 2 < p.N) bv.z = p.bias[nn + 2]; if (nn + 3 < p.N) bv.w = p.bias[nn + 3]; }
-          }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            if (!inside[i] || nn >= p.N) continue;
-            const float4 tv = *reinterpret_cast<const float4*>(tr + (i * 4 + r_sub) * 36 + c4);
-            float t[4] = {tv.x, tv.y, tv.z, tv.w};
-            float* dp = dz + orow[i] * p.ldd + nn;
-            if (p.atomic) {
-#pragma unroll
-              for (int e = 0; e < 4; ++e)
-                if (nn + e < p.N) atomicAdd(dp + e, t[e]);
-              continue;
-            }
-            t[0] += bv.x; t[1] += bv.y; t[2] += bv.z; t[3] += bv.w;
-            if (rz) {
-              const float* rp = rz + orow[i] * p.ldr + nn;
-              if (full4 && ((reinterpret_cast<uintptr_t>(rp) & 15) == 0)) {
-                const float4 rv = *reinterpret_cast<const float4*>(rp);
-                t[0] += rv.x; t[1] += rv.y; t[2] += rv.z; t[3] += rv.w;
-              } else {
-#pragma unroll
-                for (int e = 0; e < 4; ++e)
-                  if (nn + e < p.N) t[e] += rp[e];
-              }
-            }
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              if (p.act == EVK_ACT_LRELU) t[e] = t[e] > 0.f ? t[e] : t[e] * p.slope;
-              else if (p.act == EVK_ACT_RELU) t[e] = fmaxf(t[e], 0.f);
-              else if (p.act == EVK_ACT_TANH) t[e] = tanhf(t[e]);
-              if (!keep[i]) t[e] = 0.f;
-            }
-            if (dropk.thr) {                                     // group index = offset of the float4 in the output tensor / 4
-              float m[4];
-              dropk_scale4(dropk, (unsigned long long)(dp - p.d) >> 2, m);
-              t[0] *= m[0]; t[1] *= m[1]; t[2] *= m[2]; t[3] *= m[3];
-            }
-            if (full4 && ((reinterpret_cast<uintptr_t>(dp) & 15) == 0)) {
-              *reinterpret_cast<float4*>(dp) = make_float4(t[0], t[1], t[2], t[3]);
-            } else {
-#pragma unroll
-              for (int e = 0; e < 4; ++e)
-                if (nn + e < p.N) dp[e] = t[e];
-            }
-          }
+          epi_chunk(p, tr, lane, n, dz, rz, orow, keep, inside, neg, dropk);
           __syncwarp();
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;\n");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[a]);
-#ifdef GT_PROFILE
-      prof_acc[1] += (unsigned long long)(clock64() - prof_e1);
-#endif
     }
-    if (threadIdx.x == 64) { PROF_FLUSH(0, 6); PROF_FLUSH(1, 7); }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n");
-  __syncthreads();
-#ifdef GT_PROFILE
-  if (threadIdx.x == 0) g_gt_prof[blockIdx.x * 16 + 0] += (unsigned long long)(clock64() - prof_start);
-#endif
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;\n");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "n"(TCOLS));
   }
 }
 
@@ -568,7 +482,7 @@ struct Operands {
   int raw_operands;                                    // how many of the two operands are un-rounded fp32 (truncated by the MMA)
 };
 
-constexpr int SMEM_BUDGET = 184 * 1024;               // + 36.9 KB static epilogue tiles + barriers <= 227 KB
+constexpr int SMEM_BUDGET = 200 * 1024;               // + 1 KB alignment + 18.4 KB static epilogue tiles + barriers <= 227 KB
 
 template <int BN, int MT>
 int launch_gemm(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
@@ -625,16 +539,38 @@ int launch_gemm(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
   splits = max(1, min(splits, kb_total));
   p.kb_per_split = cdiv(kb_total, splits);
   p.splits = cdiv(kb_total, p.kb_per_split);
+  // split-K partials: [split][Q][M][N] in scratch (bounded: fewer splits when a large output would not fit)
+  const long long outq = (long long)(p.mode ? p.Q : 1) * p.M * p.N;
+  float* dst = p.d;
+  const long long dst_sq = p.d_sq, dst_ld = p.ldd;
+  Scratch part_buf(0, st);
+  if (p.atomic) {
+    constexpr long long PART_CAP = 32ll << 20;
+    if ((long long)p.splits * outq > PART_CAP) {
+      splits = (int)max(1ll, PART_CAP / outq);
+      p.kb_per_split = cdiv(kb_total, splits);
+      p.splits = cdiv(kb_total, p.kb_per_split);
+    }
+    p.d_ssp = 0;
+    if (p.splits > 1) {                                   // one split: every element has one writer, which adds in place
+      part_buf.alloc((long long)p.splits * outq);
+      p.d = part_buf.p;
+      EVK_REQUIRE(p.d, EVK_ERR_CUDA, "gemm_tma: scratch allocation failed");
+      p.ldd = p.N; p.d_sq = (long long)p.M * p.N; p.d_ssp = outq;
+    }
+  }
   const long long total = (long long)p.tiles_m * p.tiles_n * p.splits * (p.mode ? p.Q : p.Z);
   if (total > 0x7fffffff) return 1;
   if (total <= 0) return EVK_OK;
   const int grid = (int)(total < (long long)g_sm_count ? total : (long long)g_sm_count);
   kern<<<grid, GT_THREADS, SMEM, st>>>(ma, mb, p);
-  return check_launch("gemm_tma_kernel");
+  if (int rc = check_launch("gemm_tma_kernel")) return rc;
+  return (p.atomic && p.d_ssp) ? ordered_sum(p.d, p.splits, outq, p.mode ? p.Q : 1, p.M, p.N, dst, dst_sq, dst_ld, st) : EVK_OK;
 }
 
 // MT = 2 halves the weight-tile traffic per flop but doubles the tile: take it when the wave quantisation of the persistent
-// grid does not eat the gain (cost in units of 128-row tile-times; 0.65 = measured relative cost of a row in a 256-row tile)
+// grid does not eat the gain (cost in units of 128-row tile-times; 0.65 = relative cost of a row in a 256-row tile).  Only
+// the 32-channel layers use it: they are bound by operand traffic, the wider ones by the tensor core.
 template <int BN>
 int launch_bn(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
   if (!g_sm_count) {
@@ -642,59 +578,23 @@ int launch_bn(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
   }
-  bool mt2 = false;
-  // measured (profiles/r2_ab_tma.md): 256-row tiles pay only on the 32-channel layers (HBM-side bound, +15 %); at 64 channels they
-  // are neutral, at 128 they lose to the wave quantisation of the 148-CTA grid, at 256 they cost the second accumulator
-  if (g_opt_mt2 && BN == 32 && !p.mode && splits <= 1 && p.M >= 2 * BM) {
-    const long long per = (long long)cdiv(p.N, BN) * p.Z;
-    const long long t1 = per * cdiv(p.M, BM), t2 = per * cdiv(p.M, 2 * BM);
-    const double c1 = (double)cdiv(t1, g_sm_count), c2 = (double)cdiv(t2, g_sm_count) * 2.0 * 0.65;
-    mt2 = c2 < c1;
+  if constexpr (BN == 32) {
+    if (g_opt_mt2 && !p.mode && splits <= 1 && p.M >= 2 * BM) {
+      const long long per = (long long)cdiv(p.N, BN) * p.Z;
+      const long long t1 = per * cdiv(p.M, BM), t2 = per * cdiv(p.M, 2 * BM);
+      const double c1 = (double)cdiv(t1, g_sm_count), c2 = (double)cdiv(t2, g_sm_count) * 2.0 * 0.65;
+      if (c2 < c1) return launch_gemm<BN, 2>(o, p, splits, st);
+    }
   }
-  return mt2 ? launch_gemm<BN, 2>(o, p, splits, st) : launch_gemm<BN, 1>(o, p, splits, st);
+  return launch_gemm<BN, 1>(o, p, splits, st);
 }
 
-// Tile width.  A wide tile is the cheapest per flop (one A read per 256 columns; the TF32 shared-memory-operand MMA is bound
-// by shared-memory bandwidth, so the A re-read of narrower tiles is real cost), but most launches of the step are SMALL:
-// 5536 rows x 192..384 channels is 44..88 tiles of 128 x 256 on 148 SMs.  Pick the width that minimises
-//   waves * max(main loop, epilogue) + epilogue      (cycles; per-step and epilogue costs measured by tools/exp/gt_profile.py)
-int pick_bn(const GemmP& p, int splits) {
-  static int auto_bn = -1;
-  if (auto_bn < 0) { const char* e = getenv("EVK_TMA_AUTO_BN"); auto_bn = (e && e[0] == '1') ? 1 : 0; }   // opt-in: measured neutral on the step (53.48 vs 53.49 ms), slower in aggregate
-  int widest = p.N > 128 ? 256 : p.N > 64 ? 128 : p.N > 32 ? 64 : 32;
-  if (!auto_bn) return widest;
-  if (!g_sm_count) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
-  }
-  const int cand[4] = {256, 128, 64, 32};
-  const double step_c[4] = {560.0, 340.0, 325.0, 310.0}, epi_c[4] = {8000.0, 4300.0, 2300.0, 1500.0};
-  const int kb_total = p.mode ? p.Z * p.kbs : cdiv(p.K, BK);
-  const int sp = max(1, min(splits, kb_total));
-  const double steps = (double)cdiv(kb_total, sp) * (p.mode ? 1 : p.Q);
-  const long long outer = (long long)sp * (p.mode ? p.Q : p.Z);
-  const long long tiles_m = cdiv(p.M, BM);
-  int best = widest;
-  double best_cost = 1e30;
-  for (int i = 0; i < 4; ++i) {
-    const int bn = cand[i];
-    if (bn > widest) continue;
-    const long long tiles = tiles_m * cdiv(p.N, bn) * outer;
-    const double waves = (double)cdiv(tiles, (long long)g_sm_count);
-    const double cost = waves * fmax(steps * step_c[i], epi_c[i]) + epi_c[i];
-    if (cost < best_cost * 0.97) { best_cost = cost; best = bn; }      // ties (within 3 %) go to the wider tile
-  }
-  return best;
-}
-
+// Tile width: the widest that the output channels fill.  128 is the cap: the 64 x 128 fp32 accumulator of a consumer
+// warpgroup already takes 64 registers per thread, and a 128-row x 128-column tile reads each staged A byte for 128 columns.
 int run_gemm(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
-  switch (pick_bn(p, splits)) {
-    case 256: return launch_bn<256>(o, p, splits, st);
-    case 128: return launch_bn<128>(o, p, splits, st);
-    case 64: return launch_bn<64>(o, p, splits, st);
-    default: return launch_bn<32>(o, p, splits, st);
-  }
+  if (p.N > 64) return launch_bn<128>(o, p, splits, st);
+  if (p.N > 32) return launch_bn<64>(o, p, splits, st);
+  return launch_bn<32>(o, p, splits, st);
 }
 
 }  // namespace
@@ -734,8 +634,7 @@ int gemm_tma_run(const evk_gconv_desc* d, int phases, long long x_ps, const int*
     p.M = (int)rows; p.Z = 1; p.y_sb = 0; p.r_sb = 0;
     o.A = d->x; o.lda = d->ldx; o.a_sb = 0; o.a_rows = rows;
   } else {                                                  // stride-1 tap sum: one TMA box per (tap, channel block), OOB rows = padding
-    // 16-channel layers stay on gconv_tc_kernel: routed here (half of every 32-float K box out of range) the generator's
-    // stage-4 convs measured 56 us against 36 us there (profiles/r2_bench_history.md)
+    // 16-channel layers stay on gconv_tc_kernel: routed here, half of every 32-float K box would be out of range
     if (npos < 64 || (long long)d->Z * npos < 1024 || d->C < 32 || d->N < 32 || npos > 0x7fffffff) return 1;
     p.M = (int)npos; p.Z = d->Z; p.y_sb = d->y_sb; p.r_sb = d->r_sb;
     o.A = d->x; o.lda = d->ldx; o.a_sb = d->x_sb; o.a_rows = in_rows;
@@ -757,7 +656,7 @@ extern "C" int evk_set_tma_options(int32_t slab, int32_t mt2, float trunc_comp) 
   return EVK_OK;
 }
 
-// Strided convolution forward on the TMA/tcgen05 kernel.  d describes the conv as a STRIDE-1 tap sum over `phases` (= the
+// Strided convolution forward on the TMA/wgmma kernel.  d describes the conv as a STRIDE-1 tap sum over `phases` (= the
 // conv stride, <= 4) phase copies of the input produced by evk_phase_split: d->x = copy 0, copies x_ps floats apart, each
 // [Z][Tin * P][ldx] with d->Tin = ceil(T / stride); tap q reads copy src[q] at row shift off[q] (src, d->off: host arrays).
 // Returns EVK_ERR_UNSUPPORTED when the launch is not eligible (caller keeps the strided mma.sync kernel).
@@ -789,13 +688,14 @@ extern "C" int evk_gemm_tf32(const float* A, int32_t lda, const float* B, int32_
 }
 
 
-// Weight gradient of a stride-1 (dilated / period-folded) convolution on the TMA/tcgen05 GEMM:
+// Weight gradient of a stride-1 (dilated / period-folded) convolution on the TMA/wgmma GEMM:
 //   dW[q][n][c] += sum_b sum_pos dY[b][pos][n] * X[b][pos + off[q]*P][c]
 // with both operands pre-transposed so that the contraction index is contiguous: dyt [B][N][ld_dy] (rows = J*P valid),
 // xt [4][B][C][ld_x]: copy r is X^T delayed by r positions, xt_r[b][c][u] = X[b][u - r][c] (Tin*P + r valid; TMA box
 // coordinates along the contiguous dimension must be 16-byte aligned, so a tap shift s reads copy r = (-s) mod 4 at the
 // aligned offset s + r; only the copies that occur need to be filled).  One output tile per (tap, n tile, c tile, K split); out-of-range rows (the conv padding)
-// are zero-filled by the copy engine.  Accumulates with fp32 atomics into dW (pitch ldw, tap pitch w_sq).
+// are zero-filled by the copy engine.  Accumulates into dW (pitch ldw, tap pitch w_sq): the K splits write partials that
+// are added in split order.
 extern "C" int evk_conv_wgrad_tma(const float* dyt, int32_t ld_dy, int64_t dy_sb, const float* xt, int32_t ld_x, int64_t x_sb, int64_t x_rs, float* dW,
                                   int32_t ldw, int64_t w_sq, int32_t B, int32_t N, int32_t C, int32_t out_rows, int32_t in_rows,
                                   int32_t Q, int32_t P, const int32_t* off, int32_t splits, cudaStream_t st) {
@@ -813,11 +713,3 @@ extern "C" int evk_conv_wgrad_tma(const float* dyt, int32_t ld_dy, int64_t dy_sb
   if (rc == 0) g_disp_flops[4] += 2.0 * B * (double)out_rows * N * C * Q;
   return rc;
 }
-
-#ifdef GT_PROFILE
-extern "C" int evk_gt_prof_read(unsigned long long* host, int reset) {
-  if (host) cudaMemcpyFromSymbol(host, evk::g_gt_prof, sizeof(evk::g_gt_prof));
-  if (reset) { static unsigned long long z[160 * 16]; cudaMemcpyToSymbol(evk::g_gt_prof, z, sizeof(z)); }
-  return 0;
-}
-#endif

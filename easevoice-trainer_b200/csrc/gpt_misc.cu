@@ -37,7 +37,7 @@ __global__ void sinepos_bwd_kernel(const float* __restrict__ dy, int ldy, long l
     acc += dy[b * dy_sb + (size_t)t * ldy + d] * pe[(size_t)t * ldpe + d];
   }
   acc = block_sum(acc, red);
-  if (threadIdx.x == 0) atomicAdd(dalpha, acc);
+  if (threadIdx.x == 0) dalpha[blockIdx.x] = acc;            // per-block partial (ordered_sum adds them)
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -148,11 +148,23 @@ __global__ void sadam_reduce_kernel(const float* __restrict__ p, const float* __
   pp = block_sum(pp, red);
   pg = block_sum(pg, red);
   gg = block_sum(gg, red);
-  if (threadIdx.x == 0) {
-    atomicAdd(stats + t * 3 + 0, pp);
-    atomicAdd(stats + t * 3 + 1, pg);
-    atomicAdd(stats + t * 3 + 2, gg);
+  if (threadIdx.x == 0) {                                     // per-chunk partials; sadam_stats_sum adds them in chunk order
+    stats[blockIdx.x * 3 + 0] = pp;
+    stats[blockIdx.x * 3 + 1] = pg;
+    stats[blockIdx.x * 3 + 2] = gg;
   }
+}
+
+// stats[t][j] += sum over the chunks c of tensor t (ascending) of part[c][j]
+__global__ void sadam_stats_sum_kernel(const float* __restrict__ part, const long long* __restrict__ chunks, int nchunks, int nt,
+                                       float* __restrict__ stats) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nt * 3) return;
+  const int t = i / 3, j = i - t * 3;
+  float acc = 0.f;
+  for (int c = 0; c < nchunks; ++c)
+    if ((int)chunks[(size_t)c * 3] == t) acc += part[c * 3 + j];
+  stats[i] += acc;
 }
 
 struct SadamCfg {
@@ -425,7 +437,7 @@ extern "C" int evk_sinepos_add(const float* x, int ldx, int64_t x_sb, const floa
               "sinepos_add: D and pitches must be multiples of 4");
   if (B * T == 0) return 0;
   long long n = (long long)B * T * (D / 4);
-  sinepos_add_kernel<<<(int)min((long long)148 * 8, (n + 255) / 256), 256, 0, st>>>(x, ldx, x_sb, pe, ldpe, alpha, y, ldy, y_sb, B, T, D);
+  sinepos_add_kernel<<<(int)min((long long)kNumSMs * 8, (n + 255) / 256), 256, 0, st>>>(x, ldx, x_sb, pe, ldpe, alpha, y, ldy, y_sb, B, T, D);
   return check_launch("sinepos_add");
 }
 
@@ -433,8 +445,13 @@ extern "C" int evk_sinepos_bwd(const float* dy, int ldy, int64_t dy_sb, const fl
                                int D, cudaStream_t st) {
   if (B * T == 0) return 0;
   long long n = (long long)B * T * D;
-  sinepos_bwd_kernel<<<(int)min((long long)148 * 4, (n + 255) / 256), 256, 0, st>>>(dy, ldy, dy_sb, pe, ldpe, dalpha, B, T, D);
-  return check_launch("sinepos_bwd");
+  const int blocks = (int)min((long long)kNumSMs * 4, (n + 255) / 256);
+  Scratch part_buf(blocks, st);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "sinepos_bwd: scratch allocation failed");
+  sinepos_bwd_kernel<<<blocks, 256, 0, st>>>(dy, ldy, dy_sb, pe, ldpe, part, B, T, D);
+  if (int rc = check_launch("sinepos_bwd")) return rc;
+  return ordered_sum(part, blocks, 1, 1, 1, dalpha, 0, 0, st);
 }
 
 extern "C" int evk_ce_fwd(const float* logits, int ld, const int64_t* targets, int rows, int V, int topk, int64_t ignore_index,
@@ -457,7 +474,7 @@ extern "C" int evk_ce_bwd(const float* logits, int ld, const int64_t* targets, c
                           int rows_per_g, float* dl, int lddl, int rows, int V, cudaStream_t st) {
   EVK_REQUIRE(rows_per_g > 0, EVK_ERR_ARG, "ce_bwd: rows_per_g");
   long long n = (long long)rows * V;
-  ce_bwd_kernel<<<(int)min((long long)148 * 16, (n + 255) / 256), 256, 0, st>>>(logits, ld, (const long long*)targets, lse, gscale, rows_per_g, dl, lddl, rows, V);
+  ce_bwd_kernel<<<(int)min((long long)kNumSMs * 16, (n + 255) / 256), 256, 0, st>>>(logits, ld, (const long long*)targets, lse, gscale, rows_per_g, dl, lddl, rows, V);
   return check_launch("ce_bwd");
 }
 
@@ -473,8 +490,13 @@ extern "C" int evk_scaled_adam(float* p, float* g, float* delta, float* v, const
   EVK_REQUIRE(size_update_period >= 1 && size_update_period <= 16, EVK_ERR_UNSUPPORTED, "scaled_adam: size_update_period");
   SadamCfg c{beta1, beta2, clipping_scale, scalar_lr_scale, eps, param_min_rms, param_max_rms, clipping_update_period,
              size_update_period};
-  sadam_reduce_kernel<<<nchunks, 256, 0, st>>>(p, g, (const long long*)chunks, gscale, stats);
+  Scratch part_buf(3ll * nchunks, st);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "scaled_adam: scratch allocation failed");
+  sadam_reduce_kernel<<<nchunks, 256, 0, st>>>(p, g, (const long long*)chunks, gscale, part);
   if (int rc = check_launch("sadam_reduce")) return rc;
+  sadam_stats_sum_kernel<<<cdiv(3ll * nt, 256), 256, 0, st>>>(part, (const long long*)chunks, nchunks, nt, stats);
+  if (int rc = check_launch("sadam_stats_sum")) return rc;
   sadam_scalars_kernel<<<1, 1024, 0, st>>>(nt, (const long long*)numel, stats, rms, sv, sg, coef, hyper, (long long*)stepbuf, norms, thr, glob, c);
   if (int rc = check_launch("sadam_scalars")) return rc;
   sadam_update_kernel<<<nchunks, 256, 0, st>>>(p, g, delta, v, (const long long*)chunks, (const long long*)numel, coef, glob, gscale, beta1, beta2, eps, scalar_max,
@@ -491,7 +513,7 @@ extern "C" int evk_gemv_rows(const float* x, int32_t ldx, int32_t rows, const fl
   const int R = rows == 1 ? 1 : (rows == 2 ? 2 : 4);
   EVK_REQUIRE((size_t)R * C * 4 <= 40 * 1024, EVK_ERR_UNSUPPORTED, "gemv_rows: %d rows of %d channels exceed the staging buffer", R, C);
   int KS = 1;
-  while (KS < 8 && (long long)N * KS < 148 * 8 && C / 4 >= 64 * KS) KS *= 2;      // enough warps to cover the chip, >= 2 float4 groups per lane
+  while (KS < 8 && (long long)N * KS < kNumSMs * 8 && C / 4 >= 64 * KS) KS *= 2;      // enough warps to cover the chip, >= 2 float4 groups per lane
   const int per = 8 / KS;
   const size_t smem = ((size_t)R * C + 8 * R) * sizeof(float);
   const int grid = cdiv(N, per);

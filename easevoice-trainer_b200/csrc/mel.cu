@@ -288,7 +288,7 @@ extern "C" int evk_mel_fwd(const float* wav, const int32_t* lens, int32_t B, int
     attr_set = true;
   }
   const long long need = (nframes + MEL_WPB - 1) / MEL_WPB;
-  const unsigned grid = (unsigned)(need < 2 * 148 ? need : 2 * 148);            // persistent: two CTAs per SM
+  const unsigned grid = (unsigned)(need < 2 * kNumSMs ? need : 2 * kNumSMs);            // persistent: two CTAs per SM
   mel_fwd_warp_kernel<<<grid, MEL_WPB * 32, MEL_TAB_SMEM + MEL_WPB * MEL_WARP_SMEM, (cudaStream_t)stream>>>(
       wav, lens, L, ldw, T, nframes, hop, n_mels, fb_ptr, fb_idx, fb_val, spec, ld_spec, mel, ld_mel, cplx);
   return check_launch("mel_fwd_warp_kernel");

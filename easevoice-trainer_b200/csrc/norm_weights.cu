@@ -85,6 +85,8 @@ __global__ void layernorm_bwd_kernel(const float* __restrict__ x, int ldx, const
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
   const long long r0 = (long long)blockIdx.x * rows_per_block;
   const long long r1 = min(rows, r0 + rows_per_block);
+  float ag[LN_MAXV], ab[LN_MAXV];            // this lane's dgamma / dbeta sums over the warp's rows
+  for (int i = 0; i < LN_MAXV; ++i) { ag[i] = 0.f; ab[i] = 0.f; }
   for (long long row = r0 + wid; row < r1; row += nw) {
     const float mean = stats[row * 2], rstd = stats[row * 2 + 1];
     float xh[LN_MAXV], gd[LN_MAXV];
@@ -98,18 +100,25 @@ __global__ void layernorm_bwd_kernel(const float* __restrict__ x, int ldx, const
       const float g = d * gamma[c];
       xh[nv] = h; gd[nv] = g;
       s1 += g; s2 += g * h;
-      atomicAdd(&sg[c], d * h);
-      atomicAdd(&sb[c], d);
+      ag[nv] += d * h;
+      ab[nv] += d;
     }
     s1 = warp_sum(s1) / (float)C;
     s2 = warp_sum(s2) / (float)C;
     nv = 0;
     for (int c = lane; c < C; c += 32, ++nv) dx[row * lddx + c] = rstd * (gd[nv] - s1 - xh[nv] * s2);
   }
-  __syncthreads();
+  for (int w = 0; w < nw; ++w) {             // warps add their sums in a fixed order (reproducible)
+    if (wid == w) {
+      int nv = 0;
+      for (int c = lane; c < C; c += 32, ++nv) { sg[c] += ag[nv]; sb[c] += ab[nv]; }
+    }
+    __syncthreads();
+  }
+  // partial of this block: dgamma[blockIdx.x][c], dbeta at the same index of its own array (ordered_sum adds the blocks)
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    atomicAdd(&dgamma[c], sg[c]);
-    atomicAdd(&dbeta[c], sb[c]);
+    dgamma[(long long)blockIdx.x * 2 * C + c] = sg[c];
+    dgamma[(long long)blockIdx.x * 2 * C + C + c] = sb[c];
   }
 }
 
@@ -228,18 +237,22 @@ __global__ void __launch_bounds__(256) layernorm_drop_bwd_kernel(const float4* _
       }
     }
   }
+  for (int w = 0; w < nw; ++w) {             // warps add their sums in a fixed order (reproducible)
+    if (wid == w) {
 #pragma unroll
-  for (int i = 0; i < LND_MAXV; ++i) {
-    const int c = lane + 32 * i;
-    if (c < C4) {
-      atomicAdd(&sg[4 * c], ag[i].x); atomicAdd(&sg[4 * c + 1], ag[i].y); atomicAdd(&sg[4 * c + 2], ag[i].z); atomicAdd(&sg[4 * c + 3], ag[i].w);
-      atomicAdd(&sb[4 * c], ab[i].x); atomicAdd(&sb[4 * c + 1], ab[i].y); atomicAdd(&sb[4 * c + 2], ab[i].z); atomicAdd(&sb[4 * c + 3], ab[i].w);
+      for (int i = 0; i < LND_MAXV; ++i) {
+        const int c = lane + 32 * i;
+        if (c < C4) {
+          sg[4 * c] += ag[i].x; sg[4 * c + 1] += ag[i].y; sg[4 * c + 2] += ag[i].z; sg[4 * c + 3] += ag[i].w;
+          sb[4 * c] += ab[i].x; sb[4 * c + 1] += ab[i].y; sb[4 * c + 2] += ab[i].z; sb[4 * c + 3] += ab[i].w;
+        }
+      }
     }
+    __syncthreads();
   }
-  __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    atomicAdd(&dgamma[c], sg[c]);
-    atomicAdd(&dbeta[c], sb[c]);
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {      // partial of this block (ordered_sum adds the blocks)
+    dgamma[(long long)blockIdx.x * 2 * C + c] = sg[c];
+    dgamma[(long long)blockIdx.x * 2 * C + C + c] = sb[c];
   }
 }
 
@@ -318,7 +331,7 @@ __global__ void colsum_kernel(const float* __restrict__ x, long long rows, int n
     float s = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) s += part[k][threadIdx.x];
-    atomicAdd(&out[c], s);
+    out[(long long)blockIdx.y * n + c] = s;                      // partial of this row block (ordered_sum)
   }
 }
 
@@ -381,11 +394,16 @@ extern "C" int evk_layernorm_bwd(const float* x, int32_t ldx, const float* res, 
   EVK_REQUIRE(x && gamma && stats && dy && dx && dgamma && dbeta, EVK_ERR_ARG, "layernorm_bwd: null tensor");
   EVK_REQUIRE(C >= 1 && C <= 32 * LN_MAXV, EVK_ERR_UNSUPPORTED, "layernorm_bwd: C=%d unsupported", C);
   if (rows == 0) return EVK_OK;
-  int rpb = (int)((rows + 148 * 4 - 1) / (148 * 4));
+  int rpb = (int)((rows + kNumSMs * 4 - 1) / (kNumSMs * 4));
   if (rpb < 8) rpb = 8;
-  layernorm_bwd_kernel<<<cdiv(rows, rpb), 256, 2 * C * sizeof(float), ST>>>(x, ldx, res, ldr, gamma, stats, dy, lddy, dx,
-                                                                            lddx, dgamma, dbeta, rows, C, rpb);
-  return check_launch("layernorm_bwd");
+  const int S = cdiv(rows, rpb);
+  Scratch part_buf((long long)S * 2 * C, ST);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "layernorm_bwd: scratch allocation failed");
+  layernorm_bwd_kernel<<<S, 256, 2 * C * sizeof(float), ST>>>(x, ldx, res, ldr, gamma, stats, dy, lddy, dx, lddx, part, nullptr, rows, C, rpb);
+  if (int rc = check_launch("layernorm_bwd")) return rc;
+  if (int rc = ordered_sum(part, S, 2ll * C, 1, 1, C, dgamma, 0, 0, ST)) return rc;
+  return ordered_sum(part + C, S, 2ll * C, 1, 1, C, dbeta, 0, 0, ST);
 }
 
 extern "C" int evk_layernorm_drop_fwd(const float* x, const float* res, const float* gamma, const float* beta, float eps, float p,
@@ -407,12 +425,18 @@ extern "C" int evk_layernorm_drop_bwd(const float* x, const float* res, const fl
   EVK_REQUIRE(((((uintptr_t)x) | ((uintptr_t)res) | ((uintptr_t)dy) | ((uintptr_t)dx) | ((uintptr_t)dres)) & 15) == 0, EVK_ERR_ARG,
               "layernorm_drop_bwd: x / res / dy / dx / dres must be 16-byte aligned");
   if (rows == 0) return EVK_OK;
-  int rpb = (int)((rows + 148 * 4 - 1) / (148 * 4));
+  int rpb = (int)((rows + kNumSMs * 4 - 1) / (kNumSMs * 4));
   if (rpb < 8) rpb = 8;
-  layernorm_drop_bwd_kernel<<<cdiv(rows, rpb), 256, 2 * C * sizeof(float), ST>>>((const float4*)x, (const float4*)res, gamma, stats,
-                                                                                 (const float4*)dy, p, (const unsigned long long*)rng, sid, (float4*)dx,
-                                                                                 (float4*)dres, dgamma, dbeta, rows, C / 4, rpb);
-  return check_launch("layernorm_drop_bwd");
+  const int S = cdiv(rows, rpb);
+  Scratch part_buf((long long)S * 2 * C, ST);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "layernorm_drop_bwd: scratch allocation failed");
+  layernorm_drop_bwd_kernel<<<S, 256, 2 * C * sizeof(float), ST>>>((const float4*)x, (const float4*)res, gamma, stats, (const float4*)dy, p,
+                                                                   (const unsigned long long*)rng, sid, (float4*)dx, (float4*)dres, part, nullptr,
+                                                                   rows, C / 4, rpb);
+  if (int rc = check_launch("layernorm_drop_bwd")) return rc;
+  if (int rc = ordered_sum(part, S, 2ll * C, 1, 1, C, dgamma, 0, 0, ST)) return rc;
+  return ordered_sum(part + C, S, 2ll * C, 1, 1, C, dbeta, 0, 0, ST);
 }
 
 extern "C" int evk_weight_pack(const float* v, const float* g, int32_t D0, int32_t D1, int32_t Q, float* pa,
@@ -455,13 +479,17 @@ extern "C" int evk_colsum(const float* x, int64_t rows, int32_t n, int32_t ld, f
   }
   if (rows == 0) return EVK_OK;
   int nb = cdiv(n, 32);
-  long long want = (148LL * 8 + nb - 1) / nb;
+  long long want = ((long long)kNumSMs * 8 + nb - 1) / nb;
   int rpb = (int)((rows + want - 1) / want);
   if (rpb < 64) rpb = 64;
   dim3 grid(nb, cdiv(rows, rpb)), block(32, 8);
   EVK_REQUIRE(grid.y <= 65535, EVK_ERR_ARG, "colsum: grid too large");
-  colsum_kernel<<<grid, block, 0, ST>>>(x, rows, n, ld, out, rpb);
-  return check_launch("colsum");
+  Scratch part_buf((long long)grid.y * n, ST);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "colsum: scratch allocation failed");
+  colsum_kernel<<<grid, block, 0, ST>>>(x, rows, n, ld, part, rpb);
+  if (int rc = check_launch("colsum")) return rc;
+  return ordered_sum(part, grid.y, 1, 1, n, out, 0, 0, ST);
 }
 
 extern "C" int evk_instnorm_cl(const float* x, int32_t ldx, const float* gamma, const float* beta, float eps, int32_t act_gelu, float* y,

@@ -44,6 +44,7 @@ struct StftP {
   int n_mels; const int* fb_ptr; const int* fb_idx; const float* fb_val;
   // backward inputs
   const float* gcplx; const float* dmel; int ld_dmel; const float* mel_in; const float* cplx_in;
+  float* frbuf;              // backward: windowed adjoint of every frame [B*T][N], overlap-added by stft_ola_kernel
 };
 
 __device__ __forceinline__ int frames_of_row(int Lrow, int pad, int N, int hop) {
@@ -106,7 +107,8 @@ __global__ void __launch_bounds__(ST_THREADS) stft_fwd_kernel(const StftP p) {
   }
 }
 
-// adjoint of one frame, overlap-added (atomics) into dwav through the same reflect indexing the forward read with
+// adjoint of one frame, windowed, into frbuf; stft_ola_kernel then overlap-adds the frames into dwav through the same reflect
+// indexing the forward read with (a gather in fixed frame order: reproducible, unlike atomics)
 __global__ void __launch_bounds__(ST_THREADS) stft_bwd_kernel(const StftP p) {
   extern __shared__ __align__(16) uint8_t ssm[];
   const int NH = p.N >> 1, NB = NH + 1;
@@ -123,16 +125,21 @@ __global__ void __launch_bounds__(ST_THREADS) stft_bwd_kernel(const StftP p) {
     for (int k = tid; k < NB; k += ST_THREADS) G[k] = reinterpret_cast<const float2*>(p.gcplx)[frame * NB + k];
   } else {
     // d log(clamp(s, clip)) / ds = 1/s where s >= clip (torch.clamp passes the gradient at s >= min); s = exp(log-mel)
+    float* gm = reinterpret_cast<float*>(d1);                   // per-mel gradient (d1 is free until the FFT)
     for (int k = tid; k < NB; k += ST_THREADS) dmag[k] = 0.f;
-    __syncthreads();
     const float lclip = logf(p.clip);
     for (int m = tid; m < p.n_mels; m += ST_THREADS) {
       const float lm = p.mel_in[frame * p.ld_mel + m];
-      const float g = (lm > lclip) ? p.dmel[frame * p.ld_dmel + m] * expf(-lm) : 0.f;
-      if (g != 0.f)
-        for (int e = p.fb_ptr[m]; e < p.fb_ptr[m + 1]; ++e) atomicAdd(&dmag[p.fb_idx[e]], p.fb_val[e] * g);
+      gm[m] = (lm > lclip) ? p.dmel[frame * p.ld_dmel + m] * expf(-lm) : 0.f;
     }
     __syncthreads();
+    // filterbank transpose in mel order: the bins of one filter are distinct, so a bin receives its filters' terms in m order
+    for (int m = 0; m < p.n_mels; ++m) {
+      const float g = gm[m];
+      if (g != 0.f)
+        for (int e = p.fb_ptr[m] + tid; e < p.fb_ptr[m + 1]; e += ST_THREADS) dmag[p.fb_idx[e]] += p.fb_val[e] * g;
+      __syncthreads();
+    }
     for (int k = tid; k < NB; k += ST_THREADS) {
       const float2 x = reinterpret_cast<const float2*>(p.cplx_in)[frame * NB + k];
       const float s = dmag[k] / sqrtf(x.x * x.x + x.y * x.y + p.mag_eps);
@@ -143,14 +150,36 @@ __global__ void __launch_bounds__(ST_THREADS) stft_bwd_kernel(const StftP p) {
   stft_adjoint_pack_phase(tid, ST_THREADS, p.N, G, g_stw, d0);
   __syncthreads();
   const float2* r = run_fft(NH, d0, d1);
-  float* dw = p.dwav + (long long)b * p.ldw;
-  const int s0 = f * p.hop - p.pad;
+  float* fr = p.frbuf + frame * p.N;
   for (int m = tid; m < NH; m += ST_THREADS) {
     const float2 v = r[m];
     const int n0 = 2 * m, n1 = n0 + 1;
     const float w0 = stft_window(g_shann, n0, p.N, p.win), w1 = stft_window(g_shann, n1, p.N, p.win);
-    if (w0 != 0.f) atomicAdd(&dw[stft_reflect(s0 + n0, Lrow)], v.x * w0);
-    if (w1 != 0.f) atomicAdd(&dw[stft_reflect(s0 + n1, Lrow)], -v.y * w1);
+    fr[n0] = v.x * w0;
+    fr[n1] = -v.y * w1;
+  }
+}
+
+// dwav[b][n] += sum over the padded positions s that reflect onto n (s = n, -n, 2 (Lrow - 1) - n, in that order) and over
+// the frames f covering s (ascending) of frbuf[b*T + f][s - f*hop + pad]
+__global__ void stft_ola_kernel(const StftP p) {
+  const long long total = (long long)p.B * p.L;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int b = (int)(i / p.L), n = (int)(i - (long long)b * p.L);
+    const int Lrow = p.lens ? min(p.lens[b], p.L) : p.L;
+    if (n >= Lrow) continue;
+    const int nf = min(frames_of_row(Lrow, p.pad, p.N, p.hop), p.T);   // frbuf holds T frames per row
+    const int cand[3] = {n, -n, 2 * (Lrow - 1) - n};
+    float acc = 0.f;
+    for (int ci = 0; ci < 3; ++ci) {
+      const int s = cand[ci];
+      if ((ci == 1 && n == 0) || (ci == 2 && cand[2] == n) || stft_reflect(s, Lrow) != n) continue;
+      const int hi = (s + p.pad) >= 0 ? (s + p.pad) / p.hop : -1;                      // last frame starting at or before s
+      int lo = s + p.pad - p.N + 1;                                                      // first frame whose span reaches s
+      lo = lo <= 0 ? 0 : (lo + p.hop - 1) / p.hop;
+      for (int f = lo; f <= hi && f < nf; ++f) acc += p.frbuf[((long long)b * p.T + f) * p.N + (s - f * p.hop + p.pad)];
+    }
+    p.dwav[(long long)b * p.ldw + n] += acc;
   }
 }
 
@@ -171,7 +200,7 @@ __global__ void __launch_bounds__(256) cplx_l1_kernel(const float2* __restrict__
     }
   }
   const float tot = block_sum(acc, red);
-  if (threadIdx.x == 0) atomicAdd(loss, tot * scale);
+  if (threadIdx.x == 0) loss[blockIdx.x] = tot * scale;      // per-block partial (ordered_sum adds them)
 }
 
 int fill(StftP& p, const float* wav, const int32_t* lens, int B, int L, int ldw, int n_fft, int hop, int win, int pad, int T) {
@@ -240,14 +269,26 @@ extern "C" int evk_stft_bwd(const float* gcplx, const float* dmel, int32_t ld_dm
   EVK_REQUIRE(dwav && (gcplx || (dmel && cplx && mel && fb_ptr && fb_idx && fb_val && n_mels > 0)), EVK_ERR_ARG, "stft_bwd: missing gradient inputs");
   p.dwav = dwav; p.gcplx = gcplx; p.dmel = dmel; p.ld_dmel = ld_dmel; p.cplx_in = cplx; p.mel_in = mel; p.ld_mel = ld_mel;
   p.mag_eps = mag_eps; p.clip = clip; p.n_mels = n_mels; p.fb_ptr = fb_ptr; p.fb_idx = fb_idx; p.fb_val = fb_val;
-  return launch(stft_bwd_kernel, p, (cudaStream_t)stream, "stft_bwd_kernel");
+  EVK_REQUIRE(gcplx || n_mels <= n_fft, EVK_ERR_ARG, "stft_bwd: n_mels > n_fft");
+  Scratch fr_buf((long long)B * T * n_fft, (cudaStream_t)stream);
+  p.frbuf = fr_buf.p;
+  EVK_REQUIRE(p.frbuf, EVK_ERR_CUDA, "stft_bwd: scratch allocation failed");
+  if (int rc2 = launch(stft_bwd_kernel, p, (cudaStream_t)stream, "stft_bwd_kernel")) return rc2;
+  const long long total = (long long)B * L;
+  const long long blocks = (total + 255) / 256;
+  stft_ola_kernel<<<(unsigned)(blocks < kNumSMs * 16 ? blocks : kNumSMs * 16), 256, 0, (cudaStream_t)stream>>>(p);
+  return check_launch("stft_ola_kernel");
 }
 
 // loss[0] += scale * sum |a - b| over n complex elements; grad (nullable) = scale * (a - b) / |a - b|
 extern "C" int evk_cplx_l1(const float* a, const float* b, int64_t n, float scale, float* loss, float* grad, evk_stream_t stream) {
   EVK_REQUIRE(a && b && loss && n > 0, EVK_ERR_ARG, "cplx_l1: null argument");
-  const int blocks = (int)min((long long)148 * 8, (long long)((n + 255) / 256));
-  cplx_l1_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float2*>(a), reinterpret_cast<const float2*>(b), n, scale, loss,
+  const int blocks = (int)min((long long)kNumSMs * 8, (long long)((n + 255) / 256));
+  Scratch part_buf(blocks, (cudaStream_t)stream);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "cplx_l1: scratch allocation failed");
+  cplx_l1_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float2*>(a), reinterpret_cast<const float2*>(b), n, scale, part,
                                                           reinterpret_cast<float2*>(grad));
-  return check_launch("cplx_l1_kernel");
+  if (int rc = check_launch("cplx_l1_kernel")) return rc;
+  return ordered_sum(part, blocks, 1, 1, 1, loss, 0, 0, (cudaStream_t)stream);
 }

@@ -103,7 +103,7 @@ EVK_HD void stft_untangle_phase(int tid, int nt, int N, const float2* z, const f
 }
 
 // ---- adjoint: given G[k] = dL/dRe X[k] + i dL/dIm X[k] (k <= NH), build conj(Z'') so that ONE MORE forward FFT yields
-//      S[n] = sum_k Re(G[k] e^{+2 pi i k n / N}) = dL/d(x[n] w[n]):   S[2m] = r[m].x, S[2m+1] = -r[m].y  (see DESIGN.md) -------
+//      S[n] = sum_k Re(G[k] e^{+2 pi i k n / N}) = dL/d(x[n] w[n]):   S[2m] = r[m].x, S[2m+1] = -r[m].y -------
 EVK_HD void stft_adjoint_pack_phase(int tid, int nt, int N, const float2* G, const float2* tw, float2* d) {
   const int NH = N >> 1, step = STFT_TAB / N;
   for (int k = tid; k < NH; k += nt) {

@@ -93,7 +93,7 @@ __global__ void reduce_loss_kernel(int kind, const float* __restrict__ a, const 
     else acc += fabsf(v - b[i]);
   }
   acc = block_sum(acc, red);
-  if (threadIdx.x == 0) atomicAdd(out, acc * scale);
+  if (threadIdx.x == 0) out[blockIdx.x] = acc * scale;      // per-block partial (ordered_sum adds them)
 }
 
 __global__ void reduce_loss_bwd_kernel(int kind, const float* __restrict__ a, const float* __restrict__ b, long long n,
@@ -124,7 +124,7 @@ __global__ void kl_loss_kernel(const float* __restrict__ zp, int ldz, const floa
     acc += l - lq[r * ldq + c] - 0.5f + 0.5f * d * d * __expf(-2.f * l);
   }
   acc = block_sum(acc, red);
-  if (threadIdx.x == 0) atomicAdd(out, acc);
+  if (threadIdx.x == 0) out[blockIdx.x] = acc;             // per-block partial (ordered_sum adds them)
 }
 
 __global__ void kl_loss_bwd_kernel(const float* __restrict__ zp, int ldz, const float* __restrict__ lq, int ldq,
@@ -175,13 +175,13 @@ __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g,
   }
   if (gnorm_sq) {
     acc = block_sum(acc, red);
-    if (threadIdx.x == 0) atomicAdd(gnorm_sq, acc);
+    if (threadIdx.x == 0) gnorm_sq[blockIdx.x] = acc;         // per-block partial (ordered_sum adds them)
   }
 }
 
 static inline dim3 g1(long long n) {
   long long g = (n + 255) / 256;
-  if (g > 148LL * 16) g = 148LL * 16;
+  if (g > (long long)kNumSMs * 16) g = (long long)kNumSMs * 16;
   if (g < 1) g = 1;
   return dim3((unsigned)g);
 }
@@ -215,8 +215,13 @@ extern "C" int evk_reduce_loss(int32_t kind, const float* a, const float* b, int
                                evk_stream_t stream) {
   EVK_REQUIRE(a && out && kind >= 0 && kind <= 2 && (kind != 2 || b), EVK_ERR_ARG, "reduce_loss: bad arguments");
   if (n == 0) return EVK_OK;
-  reduce_loss_kernel<<<g1(n), 256, 0, ST>>>(kind, a, b, n, scale, out);
-  return check_launch("reduce_loss");
+  const dim3 g = g1(n);
+  Scratch part_buf(g.x, ST);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "reduce_loss: scratch allocation failed");
+  reduce_loss_kernel<<<g, 256, 0, ST>>>(kind, a, b, n, scale, part);
+  if (int rc = check_launch("reduce_loss")) return rc;
+  return ordered_sum(part, g.x, 1, 1, 1, out, 0, 0, ST);
 }
 extern "C" int evk_reduce_loss_bwd(int32_t kind, const float* a, const float* b, int64_t n, float scale,
                                    const float* gout, float* da, evk_stream_t stream) {
@@ -231,8 +236,13 @@ extern "C" int evk_kl_loss(const float* z_p, int32_t ldz, const float* logs_q, i
   EVK_REQUIRE(z_p && logs_q && m_p && logs_p && out, EVK_ERR_ARG, "kl_loss: null tensor");
   const long long rows = (long long)B * T;
   if (rows * C == 0) return EVK_OK;
-  kl_loss_kernel<<<g1(rows * C), 256, 0, ST>>>(z_p, ldz, logs_q, ldq, m_p, ldm, logs_p, ldp, rows, T, C, len, out);
-  return check_launch("kl_loss");
+  const dim3 g = g1(rows * C);
+  Scratch part_buf(g.x, ST);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "kl_loss: scratch allocation failed");
+  kl_loss_kernel<<<g, 256, 0, ST>>>(z_p, ldz, logs_q, ldq, m_p, ldm, logs_p, ldp, rows, T, C, len, part);
+  if (int rc = check_launch("kl_loss")) return rc;
+  return ordered_sum(part, g.x, 1, 1, 1, out, 0, 0, ST);
 }
 extern "C" int evk_kl_loss_bwd(const float* z_p, int32_t ldz, const float* logs_q, int32_t ldq, const float* m_p,
                                int32_t ldm, const float* logs_p, int32_t ldp, int32_t B, int32_t T, int32_t C,
@@ -259,6 +269,11 @@ extern "C" int evk_adamw_flat(float* p, const float* g, float* m, float* v, int6
                               evk_stream_t stream) {
   EVK_REQUIRE(p && g && m && v && hyper, EVK_ERR_ARG, "adamw_flat: null tensor");
   if (n == 0) return EVK_OK;
-  adamw_kernel<<<g1(n), 256, 0, ST>>>(p, g, m, v, n, hyper, lr_scale, beta1, beta2, eps, wd, grad_scale, gnorm_sq);
-  return check_launch("adamw_flat");
+  const dim3 gr = g1(n);
+  Scratch part_buf(gnorm_sq ? gr.x : 0, ST);
+  float* part = part_buf.p;
+  EVK_REQUIRE(!gnorm_sq || part, EVK_ERR_CUDA, "adamw_flat: scratch allocation failed");
+  adamw_kernel<<<gr, 256, 0, ST>>>(p, g, m, v, n, hyper, lr_scale, beta1, beta2, eps, wd, grad_scale, part);
+  if (int rc = check_launch("adamw_flat")) return rc;
+  return gnorm_sq ? ordered_sum(part, gr.x, 1, 1, 1, gnorm_sq, 0, 0, ST) : EVK_OK;
 }

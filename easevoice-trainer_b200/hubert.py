@@ -6,7 +6,7 @@ the `transformers.HubertModel` forward WITHOUT the Wav2Vec2 feature-extractor no
 model per file.  This module is that forward on the library's kernels, same state_dict keys (transformers 5.x naming, the older
 `weight_g` / `weight_v` pair of the positional conv is accepted too), same `[B, L] -> {"last_hidden_state": [B, T, 768]}` contract:
 
-  feature extractor  strided Conv1d stack on the tcgen05 / mma.sync conv kernels, GroupNorm(512, 512) + GELU in one kernel
+  feature extractor  strided Conv1d stack on the wgmma / mma.sync conv kernels, GroupNorm(512, 512) + GELU in one kernel
                      (`evk_instnorm_cl`), exact-erf GELU (`evk_unary` op 6)
   encoder            grouped k = 128 positional conv (weight-norm folded on the host once), 12 post-LN blocks: three Linear
                      launches for q / k / v, batched attention GEMMs + masked softmax (`ops.attention`), LayerNorm kernels

@@ -1,4 +1,4 @@
-"""ctypes binding of libevk_sm100.so.  Prototypes are parsed from include/evk.h so the header stays the
+"""ctypes binding of libevk_sm90.so.  Prototypes are parsed from include/evk.h so the header stays the
 single source of truth for the C ABI."""
 import ctypes
 import os
@@ -7,7 +7,7 @@ import threading
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 HEADER = os.path.join(os.path.dirname(HERE), "include", "evk.h")
-LIB_PATH = os.environ.get("EVK_LIB_PATH") or os.path.join(HERE, "libevk_sm100.so")   # override: instrumented developer builds (tools/exp)
+LIB_PATH = os.environ.get("EVK_LIB_PATH") or os.path.join(HERE, "libevk_sm90.so")   # override: instrumented developer builds (tools/exp)
 MAX_TAPS = 48
 
 
@@ -74,19 +74,17 @@ def last_error():
 
 
 def init():
-    """Load + evk_init() (requires a B200)."""
+    """Load + evk_init() (requires an H100)."""
     global _inited
     lib = load()
     if not _inited:
         rc = lib.evk_init()
         if rc != 0:
             raise RuntimeError(f"evk_init failed ({rc}): {last_error()}")
-        if os.environ.get("EVK_FLASH_TC") is not None:       # developer A/B switch: attention kernel family (csrc/flash_tc.cu)
-            lib.evk_set_flash_tc(1 if os.environ["EVK_FLASH_TC"] != "0" else 0, -1.0)
         _inited = True
     return lib
 
 
 def check(rc):
     if rc != 0:
-        raise RuntimeError(f"libevk_sm100 error {rc}: {last_error()}")
+        raise RuntimeError(f"libevk_sm90 error {rc}: {last_error()}")

@@ -1,5 +1,5 @@
 """Drop-in for /root/reference/src/easevoice/module/mel_processing.py (same function names, argument order and
-[B, F, T] results), computed by the fused sm_100a mel kernel instead of torch.stft + matmul + elementwise ops.
+[B, F, T] results), computed by the fused sm_90a mel kernel instead of torch.stft + matmul + elementwise ops.
 
 The Slaney filterbank is librosa.filters.mel (librosa 0.9.2, the reference's pinned dependency) restated here in
 float64 -> float32; librosa itself is not needed.

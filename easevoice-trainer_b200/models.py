@@ -1,7 +1,7 @@
 """Stage-2 networks: SynthesizerTrn (SoVITS acoustic model + HiFi-GAN generator) and MultiPeriodDiscriminator.
 
 Same constructor arguments, forward signatures and ``state_dict()`` keys/shapes as the reference
-(/root/reference/src/easevoice/module/models.py:803-946, 590-614), but every tensor operation is a libevk_sm100
+(the reference's src/easevoice/module/models.py:803-946, 590-614), but every tensor operation is a libevk_sm90
 kernel on channels-last activations.  ``forward`` keeps the reference's [B, C, T] contract at the API boundary;
 ``forward_cl`` is the channels-last fast path the trainer uses.
 
@@ -316,7 +316,7 @@ class SynthesizerTrn(ParamTree):
             x = ops.layernorm(x, self.P(f"{pfx}.norm_layers_1.{i}.gamma"), self.P(f"{pfx}.norm_layers_1.{i}.beta"), res=y)
             # FFN(x * mask) (attentions.py:408-416): rows past `length` never influence valid rows (keys are masked, every
             # conv input is masked), so the stream itself is masked here once and both convs run without an input mask
-            # (unmasked launches are the ones the TMA/tcgen05 kernel takes); conv_1's epilogue mask == masking conv_2's input
+            # (unmasked launches are the ones the TMA/wgmma kernel takes); conv_1's epilogue mask == masking conv_2's input
             x = ops.rowmask(x, length)
             f = f"{pfx}.ffn_layers.{i}"
             h = ops.conv(x, self.w(f + ".conv_1"), self.b(f + ".conv_1"), pad=pad, act=ops.ACT_RELU, out_len=length)
@@ -415,7 +415,7 @@ class SynthesizerTrn(ParamTree):
             x = ops.conv_transpose(x, self.w(f"dec.ups.{i}"), self.b(f"dec.ups.{i}"), stride=u, pad=(k - u) // 2)
             xa = ops.lrelu(x, LRELU_SLOPE)                 # shared first activation of the three resblocks
             outs = []
-            # the three resblocks of a stage are independent chains of six convolutions; stage 0 is 40 tiles on 148 SMs and
+            # the three resblocks of a stage are independent chains of six convolutions; stage 0 is 40 tiles on 132 SMs and
             # stage 1 is 2.16 waves of the persistent grid, so they run as three parallel branches (streams 2, 3 + current;
             # 0 and 1 may still be busy with the prior encoder and the flow)
             cur = torch.cuda.current_stream() if (SIDE_STREAMS and x.is_cuda) else None

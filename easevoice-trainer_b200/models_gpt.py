@@ -1,11 +1,11 @@
-"""Stage-1 AR semantic-token GPT on the sm_100a kernels.
+"""Stage-1 AR semantic-token GPT on the sm_90a kernels.
 
 Mirror of /root/reference/src/easevoice/soundstorm/auto_reg/models/t2s_model.py `Text2SemanticDecoder` (training
 path: forward_old :431-490) with the reference's parameter names, shapes and dtypes, so `state_dict()` is
 interchangeable (Lightning checkpoints carry these keys under a "model." prefix, t2s_lightning_module.py:26).
 
 Execution is channels-last [B, L, D] fp32 throughout:
-  bert_proj / in_proj / out_proj / linear1(+ReLU) / linear2 / ar_predict_layer  -> ops.linear (tcgen05 TF32 GEMM tiles)
+  bert_proj / in_proj / out_proj / linear1(+ReLU) / linear2 / ar_predict_layer  -> ops.linear (wgmma TF32 GEMM tiles)
   prefix-LM masked SDPA with probability dropout                               -> ops.flash_attention (fused, O(L) memory)
   residual + post-LayerNorm (transformer.py:300-315, norm_first=False)          -> ops.layernorm(res=...)
   token embeddings, alpha * sinusoid + concat                                   -> ops.embedding / ops.gpt_embed
@@ -261,7 +261,7 @@ class Text2SemanticDecoder(ParamTree):
         (exponential-race multinomial on the device).  `trace` (list) receives the [1, V] logits of every step (tests).
         Prompt-free decoding (prompts = None) is not implemented on this path."""
         if prompts is None:
-            raise NotImplementedError("infer_panel: prompt-free decoding is not implemented on the sm_100a path")
+            raise NotImplementedError("infer_panel: prompt-free decoding is not implemented on the sm_90a path")
         assert x.shape[0] == 1 and prompts.shape[0] == 1, "one utterance at a time, like infer_panel_naive"
         was_training = self.training
         self.eval()

@@ -1,4 +1,4 @@
-"""Autograd operators over channels-last tensors, each a thin wrapper around libevk_sm100 kernels.
+"""Autograd operators over channels-last tensors, each a thin wrapper around libevk_sm90 kernels.
 
 Layout: an activation is [B, T, C] fp32 with unit channel stride (row pitch = stride(-2)); column slices of a
 contiguous tensor are valid operands (no copies).  Discriminator "period" views are [B, H*P, C] with the inner
@@ -16,7 +16,7 @@ from . import lib as L
 
 ACT_NONE, ACT_LRELU, ACT_RELU, ACT_TANH = 0, 1, 2, 3
 USE_TMA_STRIDED = True   # strided conv forward: phase-split input + stride-1 multi-source tap sum on the TMA kernel
-USE_TMA_WGRAD = True     # weight gradients of tap-free layers: transposes + split-K TMA/tcgen05 GEMM
+USE_TMA_WGRAD = True     # weight gradients of tap-free layers: transposes + split-K TMA/wgmma GEMM
 UN_SCALE, UN_LRELU, UN_TANH, UN_MISH, UN_RELU, UN_TANH_FROM_OUT, UN_GELU = 0, 1, 2, 3, 4, 5, 6
 
 _launches = 0          # number of libevk kernel-launching calls (bench.py reports it)
@@ -546,7 +546,7 @@ class _ConvFn(torch.autograd.Function):
         if (USE_TMA_STRIDED and 1 < stride <= 4 and G == 1 and in_len is None and C % 4 == 0 and C >= 32 and N >= 32 and lda % 4 == 0
                 and B * J * P >= 2048 and J * P >= 64 and _aligned(x, ldx) and not _lib().evk_get_precise()):
             # strided conv = stride-1 tap sum over `stride` phase copies of the input (tap u = q*dil - pad reads phase u mod s
-            # at shift floor(u / s)): runs on the TMA/tcgen05 kernel instead of the strided mma.sync one
+            # at shift floor(u / s)): runs on the TMA/wgmma kernel instead of the strided mma.sync one
             Jp = (Tin + stride - 1) // stride
             xs = torch.empty((stride, B, Jp * P, C), device=x.device, dtype=torch.float32)
             _call("evk_phase_split", _p(x), ldx, Tin * P * ldx, _p(xs), B * Jp * P * C, B, Tin, P, C, stride, Jp)
@@ -625,7 +625,7 @@ class _ConvFn(torch.autograd.Function):
             ldx, mma = ldx_, mma_w
             if tma_w:
                 # dW[q][n][c] = sum_{b,pos} dY[b][pos][n] X[b][pos + shift_q][c]: both operands are transposed once (positions
-                # become the contiguous K dim), then the TMA-fed tcgen05 GEMM runs one output tile per (tap, n, c, K split)
+                # become the contiguous K dim), then the TMA-fed wgmma GEMM runs one output tile per (tap, n, c, K split)
                 # with the tap shift as a TMA coordinate (out-of-range rows = conv padding, zero-filled by the copy engine).
                 # A strided conv is first split into `stride` phase copies of X (as in the forward): taps u = q - pad with
                 # u mod stride == rho form a stride-1 problem on copy rho with shifts floor(u / stride).
@@ -650,9 +650,10 @@ class _ConvFn(torch.autograd.Function):
                     _call("evk_transpose_rows_multi", _p(xsrc), ldsrc, Ri * ldsrc, _p(xt), ldi, C * ldi, B * C * ldi, B, Ri, C, mask)
                     nq = len(qs)
                     qstep = (qs[1] - qs[0]) if nq > 1 else 1
-                    tiles = nq * ((N + 127) // 128) * ((C + 255) // 256 if C > 128 else 1)
+                    tiles = nq * ((N + 127) // 128) * ((C + 127) // 128)     # the TMA GEMM's tiles are at most 128 x 128
                     kblocks = B * ((Ro + 31) // 32)
-                    splits = max(1, min(64, 148 // tiles, kblocks // 8))        # one full wave of (tile, split) CTAs
+                    sms = torch.cuda.get_device_properties(dy.device).multi_processor_count
+                    splits = max(1, min(64, sms // tiles, kblocks // 8))        # one full wave of (tile, split) CTAs
                     offa = (ctypes.c_int32 * nq)(*shifts)
                     _call_f("evk_conv_wgrad_tma", 2.0 * B * Ro * N * C * nq, _p(dyt), ldo, N * ldo, _p(xt), ldi, C * ldi, B * C * ldi,
                             dpa.data_ptr() + 4 * qs[0] * N * lda, lda, qstep * N * lda, B, N, C, Ro, Ri, nq, P, offa, splits,
@@ -1264,7 +1265,7 @@ class _EmbFn(torch.autograd.Function):
         assert rep == 1
         dy = dy.contiguous()
         dt = torch.zeros(shape, device=dy.device, dtype=torch.float32)
-        _call("evk_embedding_bwd", _p(dy), shape[1], _p(idx), idx.numel(), _p(dt), shape[1], shape[1])
+        _call("evk_embedding_bwd", _p(dy), shape[1], _p(idx), idx.numel(), _p(dt), shape[1], shape[1], shape[0])
         return dt, None, None
 
 
@@ -2002,7 +2003,7 @@ def scaled_adam(st, gscale=1.0, zero_grad=True):
 
 
 def gemm_tf32(a, b, out=None, bias=None, res=None, act=ACT_NONE, slope=0.0, splits=1):
-    """out[M, N] (+)= a[M, K] @ b[N, K]^T on the TMA-fed tcgen05 GEMM (no autograd).  splits > 1 accumulates into `out`."""
+    """out[M, N] (+)= a[M, K] @ b[N, K]^T on the TMA-fed wgmma GEMM (no autograd).  splits > 1 accumulates into `out`."""
     M, K = a.shape
     N = b.shape[0]
     assert b.shape[1] == K and a.stride(1) == 1 and b.stride(1) == 1

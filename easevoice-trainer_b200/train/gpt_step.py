@@ -1,4 +1,4 @@
-"""One stage-1 (AR semantic-token GPT) optimisation step on the sm_100a kernels.
+"""One stage-1 (AR semantic-token GPT) optimisation step on the sm_90a kernels.
 
 Mirrors /root/reference/src/easevoice/soundstorm/auto_reg/models/t2s_lightning_module.py:
   training_step :41-89     manual optimisation: backward every micro-batch (loss is NOT divided), optimizer + scheduler

@@ -1,4 +1,4 @@
-"""One stage-2 (SoVITS + HiFi-GAN) optimisation step on the sm_100a kernels.
+"""One stage-2 (SoVITS + HiFi-GAN) optimisation step on the sm_90a kernels.
 
 Mirrors /root/reference/src/train/sovits.py:459-525 (G forward, mel/slice features, D step, G step, two AdamW
 updates) with these deliberate differences, none of which changes the math of the update:

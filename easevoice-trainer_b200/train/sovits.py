@@ -4,7 +4,7 @@
 
 Same parameter dataclass (field names are the REST wire format), same config file (configs/s2.json), same output
 directory scheme, checkpoint/export layouts and stdout progress protocol.  The training loop itself runs on the
-sm_100a kernels (S2Step, CUDA-graph replay per batch shape) and is data-parallel over `gpu_ids` with NCCL:
+sm_90a kernels (S2Step, CUDA-graph replay per batch shape) and is data-parallel over `gpu_ids` with NCCL:
 one process per GPU (the reference hard-codes n_gpus = 1, sovits.py:199-210).
 """
 import logging

@@ -1,9 +1,9 @@
-/* libevk_sm100.so -- C ABI of the B200-native EaseVoice stage-2 hot path.
+/* libevk_sm90.so -- C ABI of the H100-native EaseVoice stage-2 hot path.
  *
  * The reference (megaease/easevoice-trainer) is pure Python on stock PyTorch: it has NO operator /
  * FFI interface.  Every entry point below therefore replaces a *call site* of the reference that
  * lowers to a library kernel; the citation after each declaration is that call site
- * (paths relative to /root/reference/src/easevoice/module unless noted).  INTEGRATION.md shows the
+ * (paths relative to the reference's src/easevoice/module unless noted).  INTEGRATION.md shows the
  * ctypes binding a reference maintainer would add.
  *
  * Conventions
@@ -13,7 +13,7 @@
  *  - All work is enqueued on `stream`; no hidden synchronisation, no default-stream use; every
  *    entry point is CUDA-graph capturable.  Returns 0 or a negative evk_status;
  *    evk_last_error() gives the thread-local message.  Never throws, never exits.
- *  - sm_100a only: evk_init() fails on any other device.  There is no CPU fallback.
+ *  - sm_90a only: evk_init() fails on any other device.  There is no CPU fallback.
  */
 #ifndef EVK_H_
 #define EVK_H_
@@ -71,11 +71,11 @@ int evk_gconv_desc_size(void);         /* sizeof(evk_gconv_desc) as compiled: bi
  * the parity tests use it to separate indexing errors from TF32 operand rounding. Process-wide. */
 int evk_set_precise(int32_t on);
 int evk_get_precise(void);
-/* 1 (default): stride-1 launches run on the tcgen05/TMEM kernel (gconv_tc.cu); 0: mma.sync kernels only. */
-int evk_set_backend(int32_t tcgen05);
+/* 1 (default): eligible launches run on the wgmma kernels (gemm_tma.cu, gconv_tc.cu); 0: mma.sync kernels only. */
+int evk_set_backend(int32_t tensor_core);
 /* Dispatch accounting: algorithmic flops enqueued since the last reset, per kernel family (host-side counters; graph
  * replays add nothing).  out[i], i < EVK_DISPATCH_SLOTS:
- *   0 conv/linear fwd-like on gemm_tma_kernel (TMA + tcgen05)   1 ... on gconv_tc_kernel (tcgen05, staged slab)
+ *   0 conv/linear fwd-like on gemm_tma_kernel (TMA + wgmma)   1 ... on gconv_tc_kernel (wgmma, staged slab)
  *   2 ... on gconv_f_kernel (mma.sync)                          3 ... on the direct CUDA-core kernels
  *   4 weight gradients on gemm_tma_kernel                        5 ... on gconv_w_kernel (mma.sync)
  *   6 ... on the direct kernels                                  7 plain evk_gemm_tf32 calls */
@@ -87,7 +87,8 @@ int evk_set_tma_options(int32_t slab, int32_t mt2, float trunc_comp);
 int evk_dispatch_stats(double* out, int32_t n);
 int evk_dispatch_stats_reset(void);
 /* Weight gradient of the same operator:  W[z][q][n][c] += sum_{j,w} Yg[z][orow][n] * X[z][irow][c]
- * (d->y is read as the output gradient, d->w is accumulated with atomics; when w_sb == w_sh == 0 the
+ * (d->y is read as the output gradient, d->w is accumulated -- partial sums added in a fixed order, so the result is
+ * reproducible; when w_sb == w_sh == 0 the
  * sum also runs over z).  Replaces autograd's conv weight-gradient kernels for the call sites above. */
 int evk_gconv_wgrad(const evk_gconv_desc* d, evk_stream_t stream);
 /* Direct (CUDA-core) variants for skinny layers: C/G < 8 (1-channel inputs, grouped k=41 convs of
@@ -218,8 +219,9 @@ int evk_transpose_bct_btc(const float* x, float* y, int32_t B, int32_t C, int32_
  * scatter-add gradient (rep must be 1) */
 int evk_embedding(const float* table, int32_t ldt, const int64_t* idx, int64_t rows, int32_t rep, float* y,
                   int32_t ldy, int32_t C, evk_stream_t stream);
+/* dtable[idx[r]][c] += dy[r][c] for the V-row table; every entry sums its rows in row order (reproducible). */
 int evk_embedding_bwd(const float* dy, int32_t lddy, const int64_t* idx, int64_t rows, float* dtable, int32_t ldt,
-                      int32_t C, evk_stream_t stream);
+                      int32_t C, int32_t V, evk_stream_t stream);
 /* masked temporal mean (modules.py:729-737): y[b][:] = sum_{t<len[b]} x[b][t][:] / len[b]; bwd broadcast */
 int evk_masked_mean(const float* x, int32_t ldx, float* y, int32_t ldy, int32_t B, int32_t T, int32_t C,
                     const int32_t* len, int32_t bwd, evk_stream_t stream);
@@ -309,10 +311,10 @@ int evk_adamw_flat(float* p, const float* g, float* m, float* v, int64_t n,
 int evk_scalar_add(float* x, float v, evk_stream_t stream);   /* x[0] += v (device-side step counters) */
 
 /* ------------------------------------------------------------------------------------------
- * Dense TF32 GEMM on the TMA-fed persistent tcgen05 kernel: D[M][N] = epi(A[M][K] * B[N][K]^T + bias[n] + res[m][n]),
+ * Dense TF32 GEMM on the TMA-fed persistent wgmma kernel: D[M][N] = epi(A[M][K] * B[N][K]^T + bias[n] + res[m][n]),
  * fp32 storage, row pitches lda/ldb/ldd/ldr in floats (lda, ldb multiples of 4; A, B 16-byte aligned).  This is the
  * kernel evk_gconv_fwd dispatches tap-free (Linear / 1x1 conv) launches to; it is exported for weight gradients on
- * pre-transposed operands: splits > 1 partitions K across CTAs and ACCUMULATES into D with fp32 atomics (D must hold
+ * pre-transposed operands: splits > 1 partitions K across CTAs and ACCUMULATES into D, the splits' partials added in split order (D must hold
  * the value to add to, bias/res/act must be null/0).  evk_set_backend_tma(0) routes those launches back to the tap kernel.
  * ------------------------------------------------------------------------------------------ */
 int evk_gemm_tf32(const float* A, int32_t lda, const float* B, int32_t ldb, float* D, int32_t ldd, int32_t M, int32_t N,
@@ -325,7 +327,7 @@ int evk_set_backend_tma(int32_t on);
  * xt [4][B][C][ld_x] with pitch x_rs between four copies delayed by r = 0..3 positions, xt_r[b][c][u] = X[b][u - r][c]
  * (in_rows + r valid, evk_transpose_rows with shift = r).  TMA coordinates along the contiguous dimension must be 16-byte
  * aligned: a tap shift s reads copy r = (-s) mod 4 at the aligned offset s + r; only the copies that occur need filling.  Rows outside the input (the conv padding) are zero-filled by the copy engine.
- * fp32 atomics into dW (pitch ldw, tap pitch w_sq); off is a HOST array. */
+ * Accumulates the K splits' partials, added in split order, into dW (pitch ldw, tap pitch w_sq); off is a HOST array. */
 int evk_conv_wgrad_tma(const float* dyt, int32_t ld_dy, int64_t dy_sb, const float* xt, int32_t ld_x, int64_t x_sb, int64_t x_rs, float* dW,
                        int32_t ldw, int64_t w_sq, int32_t B, int32_t N, int32_t C, int32_t out_rows, int32_t in_rows,
                        int32_t Q, int32_t P, const int32_t* off, int32_t splits, evk_stream_t stream);
@@ -371,12 +373,6 @@ int evk_flash_attn_bwd(const float* q, const float* k, const float* v, int32_t l
                        const float* lse, const float* dout, int32_t lddo, float* delta, float* dq, float* dk, float* dv,
                        int32_t lddq, int32_t B, int32_t H, int32_t L, int32_t X, int32_t dkdim, const int64_t* xlen,
                        const int64_t* ylen, float scale, float p_drop, const uint64_t* rng, uint64_t sid, evk_stream_t stream);
-/* Kernel family behind evk_flash_attn_fwd / _bwd: 1 (default) = tcgen05 / TMEM kernels (csrc/flash_tc.cu), 0 = the mma.sync
- * kernels (csrc/flash.cu; always used in the 3xTF32 test mode).  trunc_comp >= 0 sets the relative compensation per raw
- * (truncated) TF32 operand, < 0 keeps it.  Forward and backward of one step must run on the same family (their S differ by the
- * compensation factor). */
-int evk_set_flash_tc(int32_t on, float trunc_comp);
-int evk_get_flash_tc(void);
 /* SinePositionalEmbedding with learnable alpha (embedding.py:36-81): y[b][t] = x[b][t] + alpha[0] * pe[t]; *_sb are batch
  * strides in floats so y can be a row range of the concatenated [B, X+Y, D] sequence.  bwd: dalpha[0] += <dy, pe>. */
 int evk_sinepos_add(const float* x, int32_t ldx, int64_t x_sb, const float* pe, int32_t ldpe, const float* alpha, float* y,

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Pin the oracle against the reference itself and (re)generate tests/golden/*.
 
-Runs ONLY in the authoring container (needs /root/reference, CPU).  It
+Needs a local checkout of the reference (EVK_REFERENCE=<its directory>), CPU only.  It
   1. stubs the one missing import of the hot-path modules (librosa.filters.mel, restated in
      oracle/mel_oracle.py and cross-checked here against torchaudio's independent Slaney filterbank),
   2. imports the reference's mel_processing / models / losses unchanged,
@@ -10,6 +10,7 @@ Runs ONLY in the authoring container (needs /root/reference, CPU).  It
 
 Usage:  python oracle/pin_against_reference.py
 """
+import hashlib
 import json
 import os
 import sys
@@ -21,7 +22,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REF = "/root/reference"
+REF = os.environ.get("EVK_REFERENCE", "")              # a local checkout of megaease/easevoice-trainer
 GOLD = os.path.join(ROOT, "tests", "golden")
 
 from oracle import mel_oracle, s2_oracle, gpt_oracle  # noqa: E402
@@ -503,6 +504,38 @@ def pin_hubert():
     return res
 
 
+def pin_ckpt_layouts(models):
+    """tests/golden/ckpt_layouts.json: the state_dict layouts the reference's checkpoint consumers build (TTS.init_vits_weights:
+    SynthesizerTrn without enc_q; TTS.init_t2s_weights: Text2SemanticLightningModule) and the named_parameters order by which
+    its G_/D_ checkpoints index AdamW state."""
+    import yaml
+    from oracle import ref_import
+    tts = ref_import.import_tts()
+    from easevoice_trainer_b200 import configs
+    from easevoice_trainer_b200.train import gpt as gpt_train
+    hps = configs.load_s2_config()
+    g = models.SynthesizerTrn(hps["data"]["filter_length"] // 2 + 1, hps["train"]["segment_size"] // hps["data"]["hop_length"],
+                              n_speakers=hps["data"]["n_speakers"], **hps["model"])
+    del g.enc_q
+    config = yaml.safe_load(open(gpt_train.GPT_CONFIG_PATH))
+    t2s = tts.Text2SemanticLightningModule(config, "****", is_train=False)
+    rg = models.SynthesizerTrn(1025, 32, n_speakers=300, **dict(s2_oracle.S2_MODEL))
+    rd = models.MultiPeriodDiscriminator(False)
+    def lay(items):          # stored as digest + length + first / last entry of the canonical JSON (tests/test_cpu_ckpt_roundtrip.py)
+        lst = [[k, list(v.shape)] for k, v in items]
+        return dict(count=len(lst), sha256=hashlib.sha256(json.dumps(lst, separators=(",", ":")).encode()).hexdigest(), first=lst[0], last=lst[-1])
+    out = dict(about="Parameter / state_dict layouts of the reference's checkpoint consumers (megaease/easevoice-trainer): the SynthesizerTrn that "
+                     "TTS.init_vits_weights builds (enc_q deleted, loaded with strict=False), the Text2SemanticLightningModule that TTS.init_t2s_weights "
+                     "loads strictly, and the named_parameters order of SynthesizerTrn(1025, 32, n_speakers=300) / MultiPeriodDiscriminator that "
+                     "utils/path/ckpt.load_checkpoint + torch.optim.AdamW index optimizer state by. Each layout is stored as the sha256 of its canonical JSON "
+                     "([[name, shape], ...] with separators (',', ':')), its length and its first and last entries.",
+               vits_state=lay(g.state_dict().items()), t2s_state=lay(t2s.state_dict().items()),
+               s2_g_params=lay(rg.named_parameters()), s2_d_params=lay(rd.named_parameters()))
+    with open(os.path.join(GOLD, "ckpt_layouts.json"), "w") as f:
+        f.write(json.dumps(out, indent=1) + "\n")
+    return {k: v["count"] for k, v in out.items() if k != "about"}
+
+
 def main():
     os.makedirs(GOLD, exist_ok=True)
     torch.manual_seed(0)
@@ -517,6 +550,9 @@ def main():
     if "--infer-panel" in sys.argv:      # only the AR decoding golden (needs the torchmetrics stub of pin_gpt: run after it)
         stub_torchmetrics()
         print(pin_infer_panel())
+        return
+    if "--ckpt-layouts" in sys.argv:     # only the checkpoint-consumer layouts (seconds)
+        print(pin_ckpt_layouts(models))
         return
     if "--decode" in sys.argv:           # only the TTS vocoder-call golden (seconds)
         print(pin_decode(models))

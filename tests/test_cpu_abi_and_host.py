@@ -34,7 +34,7 @@ def test_descriptor_struct_layout():
 
 
 def test_no_cpu_fallback():
-    """Without a B200 the product path must fail loudly, never silently compute on the CPU."""
+    """Without an H100 the product path must fail loudly, never silently compute on the CPU."""
     if torch.cuda.is_available():
         pytest.skip("GPU present")
     from easevoice_trainer_b200 import lib, ops
@@ -225,7 +225,7 @@ def test_gpt_dataset_collate_and_sampler(tmp_path):
 
 def test_bench_reference_arm_prints_one_json_line():
     """`bench.py --impl reference` (the CPU arm the driver runs next to ours) must emit exactly one JSON line on stdout with the
-    contract keys, without touching a GPU or /root/reference."""
+    contract keys, without touching a GPU or the reference checkout."""
     import json
     import subprocess
     import sys

@@ -1,73 +1,72 @@
 """Checkpoints written by this package are consumed by the UNMODIFIED reference (SURVEY 8b "Files out", 8f-2):
-  * stage-2 export  -> TTS.init_vits_weights            (inference/tts.py:265-299)
-  * stage-1 export  -> TTS.init_t2s_weights             (inference/tts.py:301-315)
+  * stage-2 export  -> TTS.init_vits_weights            (inference/tts.py:265-299: SynthesizerTrn without enc_q, strict=False)
+  * stage-1 export  -> TTS.init_t2s_weights             (inference/tts.py:301-315: Text2SemanticLightningModule, strict)
   * G_/D_ resumable -> ckpt.load_checkpoint + torch.optim.AdamW.load_state_dict + ExponentialLR (sovits.py:327-376)
-and reference-style optimizer states load back into the flat optimizers.  CPU only; needs /root/reference."""
+and reference-style optimizer states load back into the flat optimizers.  CPU only.
+
+What those consumers expect is pinned in tests/golden/ckpt_layouts.json, recorded from the reference: the state_dict
+layouts its two loaders build, and the named_parameters order by which torch.optim.AdamW indexes the optimizer state in a
+G_/D_ checkpoint (oracle/pin_against_reference.py --ckpt-layouts regenerates it)."""
+import hashlib
+import json
 import os
-import types
 
 import pytest
 import torch
 
-from tests import ref_import
-
-pytestmark = pytest.mark.skipif(not ref_import.available(), reason="/root/reference is only present in the authoring container")
+GOLD = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ckpt_layouts.json")))
 
 
-def _fake_tts():
-    cfg = types.SimpleNamespace(device="cpu", is_half=False, save_configs=lambda: None)
-    return types.SimpleNamespace(configs=cfg)
+def _layout(items):
+    return [[k, list(v.shape)] for k, v in items]
 
 
-def test_s2_export_loads_through_reference_tts(tmp_path):
+def _check_layout(items, key):
+    """items == the stored reference layout `key` (count, first / last entry, sha256 of the canonical JSON)."""
+    lst, gold = _layout(items), GOLD[key]
+    assert len(lst) == gold["count"] and lst[0] == gold["first"] and lst[-1] == gold["last"], (key, len(lst), lst[0], lst[-1])
+    assert hashlib.sha256(json.dumps(lst, separators=(",", ":")).encode()).hexdigest() == gold["sha256"], key
+
+
+def test_s2_export_matches_reference_vits_loader(tmp_path):
     from easevoice_trainer_b200 import configs, models
     from easevoice_trainer_b200.utils import ckpt
-    tts = ref_import.import_tts()
     hps = configs.load_s2_config()
     net_g = models.SynthesizerTrn(hps["data"]["filter_length"] // 2 + 1, hps["train"]["segment_size"] // hps["data"]["hop_length"],
                                   n_speakers=hps["data"]["n_speakers"], **hps["model"])
     before = set(os.listdir("."))
     path = ckpt.export_weights(net_g.state_dict(), hps, "rt_e1_s10", 1, 10, str(tmp_path))
-    fake = _fake_tts()
-    tts.TTS.init_vits_weights(fake, path)                        # the reference's own loader, unmodified
-    ref_sd = fake.vits_model.state_dict()                        # reference SynthesizerTrn without enc_q
-    ours = torch.load(path, map_location="cpu")["weight"]
-    assert set(ref_sd) == set(ours), (sorted(set(ref_sd) ^ set(ours))[:6])
-    for k, v in ref_sd.items():
-        assert torch.equal(v, ours[k].float()), k                # strict=False in the loader: prove nothing was skipped
-    assert fake.configs.sampling_rate == 32000 and fake.configs.hop_length == 640
+    d = torch.load(path, map_location="cpu")
+    ours = d["weight"]
+    # strict=False in the loader: a missing or renamed key would be skipped silently, so keys and shapes must be exactly the
+    # loader's (its model lists them in module order; the export keeps ours, which is the same order)
+    _check_layout(ours.items(), "vits_state")
+    sd = net_g.state_dict()
+    for k, v in ours.items():
+        assert torch.equal(v, sd[k].half()), k
+    assert ours["enc_p.text_embedding.weight"].shape[0] != 322           # the loader rejects v1 models by this shape
+    cfg = d["config"]
+    assert cfg["data"]["sampling_rate"] == 32000 and cfg["data"]["hop_length"] == 640
+    for k in ("filter_length", "win_length", "n_speakers"):
+        assert k in cfg["data"], k
+    assert "segment_size" in cfg["train"] and isinstance(cfg["model"], dict)
     assert set(os.listdir(".")) == before, "the temp file of save_with_torch must live next to its target, not in the CWD"
 
 
-def test_gpt_export_loads_through_reference_tts(tmp_path):
+def test_gpt_export_matches_reference_t2s_loader(tmp_path):
     import yaml
     from collections import OrderedDict
     from easevoice_trainer_b200.models_gpt import Text2SemanticDecoder
     from easevoice_trainer_b200.train import gpt as gpt_train
-    tts = ref_import.import_tts()
     config = yaml.safe_load(open(gpt_train.GPT_CONFIG_PATH))
     net = Text2SemanticDecoder(config, top_k=3)
     sd = OrderedDict(("model." + k, v.detach().clone()) for k, v in net.state_dict().items())
-    od = OrderedDict(weight=OrderedDict((k, v.half()) for k, v in sd.items()), config=config, info="GPT-e1")
-    path = os.path.join(tmp_path, "rt-e1.ckpt")
-    torch.save(od, path)
-    fake = _fake_tts()
-    tts.TTS.init_t2s_weights(fake, path)                         # strict load_state_dict inside
-    ref_sd = fake.t2s_model.state_dict()
-    for k, v in ref_sd.items():
-        assert torch.equal(v, sd[k].half().float()), k
-    assert fake.configs.max_sec == config["data"]["max_sec"]
-
-
-def _ref_nets():
-    _, models, _, _ = ref_import.import_hot_path()
-    from oracle import s2_oracle
-    net_g = models.SynthesizerTrn(1025, 32, n_speakers=300, **dict(s2_oracle.S2_MODEL))
-    net_d = models.MultiPeriodDiscriminator(False)
-    return net_g, net_d
+    _check_layout(sd.items(), "t2s_state")                               # load_state_dict(strict=True) in the loader
+    assert "max_sec" in config["data"]
 
 
 def _ref_optim_g(net_g, lr=1e-4, low=0.4):
+    """The reference's optimizer of G (sovits.py): AdamW over four lr groups, text-side modules at lr * low."""
     te = list(map(id, net_g.enc_p.text_embedding.parameters()))
     et = list(map(id, net_g.enc_p.encoder_text.parameters()))
     mr = list(map(id, net_g.enc_p.mrte.parameters()))
@@ -77,13 +76,24 @@ def _ref_optim_g(net_g, lr=1e-4, low=0.4):
                               {"params": net_g.enc_p.mrte.parameters(), "lr": lr * low}], lr, betas=(0.8, 0.99), eps=1e-9)
 
 
+def _ref_load_checkpoint(path, model, optimizer):
+    """What the reference's utils/path/ckpt.load_checkpoint does with a G_/D_ file: optimizer state first, then every key of
+    the model's own state_dict taken from the file with an equal shape, then a strict load."""
+    d = torch.load(path, map_location="cpu")
+    optimizer.load_state_dict(d["optimizer"])
+    own = model.state_dict()
+    for k, v in own.items():
+        assert k in d["model"] and d["model"][k].shape == v.shape, k
+    model.load_state_dict({k: d["model"][k] for k in own})
+    return d["learning_rate"], d["iteration"]
+
+
 def test_resumable_checkpoints_round_trip_with_reference_optimizer(tmp_path):
-    """our G_/D_ -> reference load_checkpoint + AdamW + ExponentialLR + one optimizer step; and back."""
+    """our G_/D_ -> the reference's loading recipe + AdamW + ExponentialLR + one optimizer step; and back."""
     from easevoice_trainer_b200 import models
     from easevoice_trainer_b200.train import s2_step
     from easevoice_trainer_b200.utils import ckpt
     from oracle import s2_oracle
-    from src.utils.path import ckpt as ref_ckpt                  # the reference's own reader
     og = models.SynthesizerTrn(1025, 32, n_speakers=300, **dict(s2_oracle.S2_MODEL))
     od = models.MultiPeriodDiscriminator(False)
     opt_g = s2_step.FlatAdamW(og.named_parameters(), s2_step.g_param_groups(og, 0.4), (0.8, 0.99), 1e-9, frozen=s2_step.FROZEN_G)
@@ -94,10 +104,14 @@ def test_resumable_checkpoints_round_trip_with_reference_optimizer(tmp_path):
     pg, pd = os.path.join(tmp_path, "G_latest.pth"), os.path.join(tmp_path, "D_latest.pth")
     ckpt.save_checkpoint(og, opt_g, 1e-4, 3, pg)
     ckpt.save_checkpoint(od, opt_d, 1e-4, 3, pd)
-    rg, rd = _ref_nets()
+    # the reference's networks index optimizer state by this parameter order: ours must have the same one
+    rg = models.SynthesizerTrn(1025, 32, n_speakers=300, **dict(s2_oracle.S2_MODEL))
+    rd = models.MultiPeriodDiscriminator(False)
+    _check_layout(rg.named_parameters(), "s2_g_params")
+    _check_layout(rd.named_parameters(), "s2_d_params")
     ropt_g, ropt_d = _ref_optim_g(rg), torch.optim.AdamW(rd.parameters(), 1e-4, betas=(0.8, 0.99), eps=1e-9)
-    _, _, lr, it = ref_ckpt.load_checkpoint(pd, rd, ropt_d)
-    _, _, lr, it = ref_ckpt.load_checkpoint(pg, rg, ropt_g)
+    lr, it = _ref_load_checkpoint(pd, rd, ropt_d)
+    lr, it = _ref_load_checkpoint(pg, rg, ropt_g)
     assert it == 3 and lr == 1e-4
     for (n, p), (n2, p2) in zip(rg.named_parameters(), og.named_parameters()):
         assert n == n2 and torch.equal(p.data, p2.data), n
@@ -106,12 +120,11 @@ def test_resumable_checkpoints_round_trip_with_reference_optimizer(tmp_path):
     assert abs(ropt_g.param_groups[0]["lr"] - 9.9e-5 * 0.999875) < 1e-12
     assert abs(ropt_g.param_groups[1]["lr"] - 0.4 * 9.9e-5 * 0.999875) < 1e-12
     # state tensors landed on the right parameters (index order == reference named_parameters order)
-    names = [n for n, _ in rg.named_parameters()]
     plist = [p for g in ropt_g.param_groups for p in g["params"]]
     idx = {id(p): i for i, p in enumerate(plist)}
     byname = dict(rg.named_parameters())
     for n in ("dec.conv_pre.weight", "enc_p.mrte.c_post.weight", "enc_q.enc.cond_layer.weight_v", "flow.flows.6.post.bias"):
-        i = idx[id(byname[n])]
+        assert id(byname[n]) in idx, n
         off, k = opt_g.slots[n]
         assert torch.equal(ropt_g.state[byname[n]]["exp_avg"].reshape(-1), opt_g.flat_m[off:off + k]), n
         assert float(ropt_g.state[byname[n]]["step"]) == 7.0
@@ -119,9 +132,9 @@ def test_resumable_checkpoints_round_trip_with_reference_optimizer(tmp_path):
     for p in rg.parameters():
         p.grad = torch.zeros_like(p)
     ropt_g.step()                                                 # a full torch AdamW step runs on the loaded state
-    # ---- and back: a reference-written checkpoint resumes in the flat optimizer
+    # ---- and back: a checkpoint in the reference's G_ format ({model, iteration, optimizer, learning_rate}) resumes in the flat optimizer
     rpath = os.path.join(tmp_path, "G_ref.pth")
-    ref_ckpt.save_checkpoint(rg, ropt_g, 1e-4, 4, rpath)
+    torch.save({"model": rg.state_dict(), "iteration": 4, "optimizer": ropt_g.state_dict(), "learning_rate": 1e-4}, rpath)
     og2 = models.SynthesizerTrn(1025, 32, n_speakers=300, **dict(s2_oracle.S2_MODEL))
     opt2 = s2_step.FlatAdamW(og2.named_parameters(), s2_step.g_param_groups(og2, 0.4), (0.8, 0.99), 1e-9, frozen=s2_step.FROZEN_G)
     _, _, _, it2 = ckpt.load_checkpoint(rpath, og2, opt2)

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the TMA-fed tcgen05 GEMM (csrc/gemm_tma.cu) on the stage-1 GPT shapes against the tap kernel and cuBLAS TF32."""
+"""Micro-benchmark of the TMA-fed wgmma GEMM (csrc/gemm_tma.cu) on the stage-1 GPT shapes against the tap kernel and cuBLAS TF32."""
 import os, sys, torch, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from easevoice_trainer_b200 import lib, ops
