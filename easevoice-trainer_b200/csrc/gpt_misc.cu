@@ -288,10 +288,14 @@ __global__ void sadam_update_kernel(float* __restrict__ p, float* __restrict__ g
 // ---- KV-cache attention of one new token (T2SBlock.decode_next_token, t2s_model.py:203-221) --------------------------------
 // Cache rows are the in_proj outputs [q | k | v] (3 * H * 32 floats, row pitch ld) of every position so far; the query is the
 // q block of the LAST row.  One CTA per (head, batch item), 128 threads, key-parallel (see the kernel).  Exact fp32 -- the sampled token must not depend on operand rounding.
+// skip (optional, [B][2]): item b never reads keys skip[b][0] .. skip[b][1] - 1 -- the right padding of its text in a batch whose
+// rows are padded to a common text length (infer_panel_batch_infer).  The remaining keys are walked as one list, so thread t owns
+// the same keys whatever the padding, and a padded key (possibly not finite) never enters a sum.
 __global__ void __launch_bounds__(128) attn_decode_kernel(const float* __restrict__ qkv, long long sb, int ld, int n, const int* __restrict__ n_dev,
-                                                           int H, float scale, float* __restrict__ out, int ldo) {
+                                                           const int* __restrict__ skip, int H, float scale, float* __restrict__ out, int ldo) {
   if (n_dev) n = *n_dev + 1;                                     // graph replay: keys 0 .. *n_dev (the row just appended)
   const int h = blockIdx.x, b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int s0 = skip ? skip[2 * b] : n, gap = skip ? skip[2 * b + 1] - s0 : 0;
   const float* base = qkv + (long long)b * sb;
   const int D = H * 32;
   // Key-parallel: thread t owns keys t, t + 128, ... (the whole 32-float q / k / v rows in registers: no per-key shuffle chain,
@@ -309,7 +313,8 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const float* __restric
   float m = -INFINITY, l = 0.f, acc[32];
 #pragma unroll
   for (int c = 0; c < 32; ++c) acc[c] = 0.f;
-  for (int j = threadIdx.x; j < n; j += 128) {
+  for (int t = threadIdx.x; t < n - gap; t += 128) {
+    const int j = t < s0 ? t : t + gap;
     const float4* kp = reinterpret_cast<const float4*>(base + (long long)j * ld + D + h * 32);
     const float4* vp = reinterpret_cast<const float4*>(base + (long long)j * ld + 2 * D + h * 32);
     float4 kv[8], vv[8];
@@ -355,50 +360,58 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const float* __restric
   }
 }
 
-// Skinny product of the AR token step:  y[r][n] = act(sum_c x[r][c] * W[n][c] + bias[n]),  R <= 4 rows.
+// Skinny product of the AR token step:  y[r][n] = act(sum_c x[r][c] * W[n][c] + bias[n]),  R <= 64 rows.
 // A one-row "GEMM" is a stream over the weight matrix (12.6 MB per GPT layer): through the 128-row tensor-core tiles it ran on
 // N/128 = 4..16 CTAs with one barrier round trip per 32 channels (25..100 us per Linear, 9.3 ms per token).  Here KS warps share
 // one output column (each takes every KS-th float4 group of the weight row: 512-byte coalesced warp loads, four in flight), the x
 // rows sit in shared memory, products are exact fp32 FMAs (the sampled token must not depend on operand rounding).
+// Rows that do not fit in shared memory at once (R * C floats > the staging budget) are staged CC channels at a time; the weight
+// is still read once, and every lane keeps walking its own float4 groups in increasing order across the chunks, so each output's
+// FMA chain, its warp sum and the sum over the KS warps are the same for every R: a row's result does not depend on the batch.
 template <int R>
 __global__ void __launch_bounds__(256) gemv_rows_kernel(const float* __restrict__ x, int ldx, int rows, const float* __restrict__ W, int ldw,
                                                         const float* __restrict__ bias, float* __restrict__ y, int ldy, int N, int C,
-                                                        int KS, int act, float slope) {
-  extern __shared__ __align__(16) float gv_x[];                   // [R][C] then [8][R] partial sums
-  float* part = gv_x + R * C;
-  for (int i = threadIdx.x; i < R * C; i += blockDim.x) {
-    const int r = i / C, c = i - r * C;
-    gv_x[i] = r < rows ? x[(size_t)r * ldx + c] : 0.f;
-  }
-  __syncthreads();
+                                                        int CC, int KS, int act, float slope) {
+  extern __shared__ __align__(16) float gv_x[];                   // [R][CC] staged channels, then [8][R] partial sums
+  float* part = gv_x + R * CC;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int per = 8 / KS;                                          // output columns per CTA
   const int n = blockIdx.x * per + warp / KS, ks = warp % KS;
+  const float4* wr = reinterpret_cast<const float4*>(W + (size_t)(n < N ? n : 0) * ldw);
+  const int step = 32 * KS;
+  int c4 = ks * 32 + lane;                                         // this lane's next float4 group of the weight row
   float acc[R];
 #pragma unroll
   for (int r = 0; r < R; ++r) acc[r] = 0.f;
-  if (n < N) {
-    const float4* wr = reinterpret_cast<const float4*>(W + (size_t)n * ldw);
-    const int C4 = C >> 2, step = 32 * KS;
-    int c4 = ks * 32 + lane;
-    for (; c4 + 3 * step < C4; c4 += 4 * step) {
-      float4 w[4];
+  for (int c0 = 0; c0 < C; c0 += CC) {
+    const int cc = min(CC, C - c0);
+    if (c0) __syncthreads();                                       // every warp is done with the previous chunk
+    for (int i = threadIdx.x; i < R * cc; i += blockDim.x) {
+      const int r = i / cc, c = i - r * cc;
+      gv_x[r * CC + c] = r < rows ? x[(size_t)r * ldx + c0 + c] : 0.f;
+    }
+    __syncthreads();
+    if (n < N) {
+      const int g0 = c0 >> 2, g1 = (c0 + cc) >> 2;
+      for (; c4 + 3 * step < g1; c4 += 4 * step) {
+        float4 w[4];
 #pragma unroll
-      for (int u = 0; u < 4; ++u) w[u] = __ldg(wr + c4 + u * step);
+        for (int u = 0; u < 4; ++u) w[u] = __ldg(wr + c4 + u * step);
 #pragma unroll
-      for (int u = 0; u < 4; ++u)
+        for (int u = 0; u < 4; ++u)
+#pragma unroll
+          for (int r = 0; r < R; ++r) {
+            const float4 xv = reinterpret_cast<const float4*>(gv_x + r * CC)[c4 - g0 + u * step];
+            acc[r] = fmaf(w[u].x, xv.x, fmaf(w[u].y, xv.y, fmaf(w[u].z, xv.z, fmaf(w[u].w, xv.w, acc[r]))));
+          }
+      }
+      for (; c4 < g1; c4 += step) {
+        const float4 w = __ldg(wr + c4);
 #pragma unroll
         for (int r = 0; r < R; ++r) {
-          const float4 xv = reinterpret_cast<const float4*>(gv_x + r * C)[c4 + u * step];
-          acc[r] = fmaf(w[u].x, xv.x, fmaf(w[u].y, xv.y, fmaf(w[u].z, xv.z, fmaf(w[u].w, xv.w, acc[r]))));
+          const float4 xv = reinterpret_cast<const float4*>(gv_x + r * CC)[c4 - g0];
+          acc[r] = fmaf(w.x, xv.x, fmaf(w.y, xv.y, fmaf(w.z, xv.z, fmaf(w.w, xv.w, acc[r]))));
         }
-    }
-    for (; c4 < C4; c4 += step) {
-      const float4 w = __ldg(wr + c4);
-#pragma unroll
-      for (int r = 0; r < R; ++r) {
-        const float4 xv = reinterpret_cast<const float4*>(gv_x + r * C)[c4];
-        acc[r] = fmaf(w.x, xv.x, fmaf(w.y, xv.y, fmaf(w.z, xv.z, fmaf(w.w, xv.w, acc[r]))));
       }
     }
   }
@@ -409,13 +422,15 @@ __global__ void __launch_bounds__(256) gemv_rows_kernel(const float* __restrict_
     for (int r = 0; r < R; ++r) part[warp * R + r] = acc[r];
   }
   __syncthreads();
-  if (ks == 0 && n < N && lane < rows && lane < R) {
-    float v = 0.f;
-    for (int k = 0; k < KS; ++k) v += part[(warp + k) * R + lane];
-    if (bias) v += bias[n];
-    if (act == EVK_ACT_RELU) v = fmaxf(v, 0.f);
-    else if (act == EVK_ACT_LRELU) v = v > 0.f ? v : v * slope;
-    y[(size_t)lane * ldy + n] = v;
+  if (ks == 0 && n < N) {
+    for (int r = lane; r < rows && r < R; r += 32) {
+      float v = 0.f;
+      for (int k = 0; k < KS; ++k) v += part[(warp + k) * R + r];
+      if (bias) v += bias[n];
+      if (act == EVK_ACT_RELU) v = fmaxf(v, 0.f);
+      else if (act == EVK_ACT_LRELU) v = v > 0.f ? v : v * slope;
+      y[(size_t)r * ldy + n] = v;
+    }
   }
 }
 
@@ -504,23 +519,49 @@ extern "C" int evk_scaled_adam(float* p, float* g, float* delta, float* v, const
   return check_launch("sadam_update");
 }
 
+template <int R>
+static int gemv_rows_launch(int grid, size_t smem, cudaStream_t st, const float* x, int ldx, int rows, const float* W, int ldw,
+                            const float* bias, float* y, int ldy, int N, int C, int CC, int KS, int act, float slope) {
+  if (smem > 48 * 1024) {                                          // opt in once per instance (before any graph capture uses it)
+    static unsigned opted = 0;                                     // one bit per device ordinal
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (!((opted >> (dev & 31)) & 1u)) {
+      EVK_REQUIRE(cudaFuncSetAttribute(gemv_rows_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024) == cudaSuccess,
+                  EVK_ERR_CUDA, "gemv_rows: shared-memory opt-in failed");
+      opted |= 1u << (dev & 31);
+    }
+  }
+  gemv_rows_kernel<R><<<grid, 256, smem, st>>>(x, ldx, rows, W, ldw, bias, y, ldy, N, C, CC, KS, act, slope);
+  return check_launch("gemv_rows");
+}
+
 extern "C" int evk_gemv_rows(const float* x, int32_t ldx, int32_t rows, const float* W, int32_t ldw, const float* bias, float* y,
                              int32_t ldy, int32_t N, int32_t C, int32_t act, float slope, cudaStream_t st) {
-  EVK_REQUIRE(x && W && y && rows >= 1 && rows <= 4 && N >= 1 && C >= 4, EVK_ERR_ARG, "gemv_rows: bad arguments (rows=%d N=%d C=%d)", rows, N, C);
+  EVK_REQUIRE(x && W && y && rows >= 1 && rows <= 64 && N >= 1 && C >= 4, EVK_ERR_ARG, "gemv_rows: bad arguments (rows=%d N=%d C=%d)", rows, N, C);
   EVK_REQUIRE(C % 4 == 0 && ldw % 4 == 0 && ldw >= C && ((uintptr_t)W % 16) == 0 && ldx >= C && ldy >= N, EVK_ERR_ARG,
               "gemv_rows: C and the weight pitch must be multiples of 4, W 16-byte aligned");
   EVK_REQUIRE(act == EVK_ACT_NONE || act == EVK_ACT_RELU || act == EVK_ACT_LRELU, EVK_ERR_UNSUPPORTED, "gemv_rows: activation %d", act);
-  const int R = rows == 1 ? 1 : (rows == 2 ? 2 : 4);
-  EVK_REQUIRE((size_t)R * C * 4 <= 40 * 1024, EVK_ERR_UNSUPPORTED, "gemv_rows: %d rows of %d channels exceed the staging buffer", R, C);
+  int R = 1;
+  while (R < rows) R *= 2;
+  // <= 4 rows: all C channels staged at once (40 KB at most); more rows: chunks of CC channels in a 64 KB staging buffer
+  int CC = C;
+  if (R <= 4) EVK_REQUIRE((size_t)R * C * 4 <= 40 * 1024, EVK_ERR_UNSUPPORTED, "gemv_rows: %d rows of %d channels exceed the staging buffer", R, C);
+  else CC = min(C, (64 * 1024 / 4 / R) & ~3);
   int KS = 1;
   while (KS < 8 && (long long)N * KS < kNumSMs * 8 && C / 4 >= 64 * KS) KS *= 2;      // enough warps to cover the chip, >= 2 float4 groups per lane
   const int per = 8 / KS;
-  const size_t smem = ((size_t)R * C + 8 * R) * sizeof(float);
+  const size_t smem = ((size_t)R * CC + 8 * R) * sizeof(float);
   const int grid = cdiv(N, per);
-  if (R == 1) gemv_rows_kernel<1><<<grid, 256, smem, st>>>(x, ldx, rows, W, ldw, bias, y, ldy, N, C, KS, act, slope);
-  else if (R == 2) gemv_rows_kernel<2><<<grid, 256, smem, st>>>(x, ldx, rows, W, ldw, bias, y, ldy, N, C, KS, act, slope);
-  else gemv_rows_kernel<4><<<grid, 256, smem, st>>>(x, ldx, rows, W, ldw, bias, y, ldy, N, C, KS, act, slope);
-  return check_launch("gemv_rows");
+  switch (R) {
+    case 1: return gemv_rows_launch<1>(grid, smem, st, x, ldx, rows, W, ldw, bias, y, ldy, N, C, CC, KS, act, slope);
+    case 2: return gemv_rows_launch<2>(grid, smem, st, x, ldx, rows, W, ldw, bias, y, ldy, N, C, CC, KS, act, slope);
+    case 4: return gemv_rows_launch<4>(grid, smem, st, x, ldx, rows, W, ldw, bias, y, ldy, N, C, CC, KS, act, slope);
+    case 8: return gemv_rows_launch<8>(grid, smem, st, x, ldx, rows, W, ldw, bias, y, ldy, N, C, CC, KS, act, slope);
+    case 16: return gemv_rows_launch<16>(grid, smem, st, x, ldx, rows, W, ldw, bias, y, ldy, N, C, CC, KS, act, slope);
+    case 32: return gemv_rows_launch<32>(grid, smem, st, x, ldx, rows, W, ldw, bias, y, ldy, N, C, CC, KS, act, slope);
+    default: return gemv_rows_launch<64>(grid, smem, st, x, ldx, rows, W, ldw, bias, y, ldy, N, C, CC, KS, act, slope);
+  }
 }
 
 extern "C" int evk_attn_decode(const float* qkv, int64_t batch_stride, int32_t ld, int32_t n_keys, int32_t B, int32_t H, float scale,
@@ -528,16 +569,16 @@ extern "C" int evk_attn_decode(const float* qkv, int64_t batch_stride, int32_t l
   EVK_REQUIRE(qkv && out && B >= 1 && H >= 1 && n_keys >= 1, EVK_ERR_ARG, "attn_decode: bad arguments");
   EVK_REQUIRE(ld >= 3 * H * 32 && ldo >= H * 32, EVK_ERR_ARG, "attn_decode: row pitch %d / %d too small for %d heads of 32", ld, ldo, H);
   EVK_REQUIRE(ld % 4 == 0 && batch_stride % 4 == 0 && ((uintptr_t)qkv % 16) == 0, EVK_ERR_ARG, "attn_decode: rows must be 16-byte aligned");
-  attn_decode_kernel<<<dim3(H, B), 128, 0, st>>>(qkv, batch_stride, ld, n_keys, nullptr, H, scale, out, ldo);
+  attn_decode_kernel<<<dim3(H, B), 128, 0, st>>>(qkv, batch_stride, ld, n_keys, nullptr, nullptr, H, scale, out, ldo);
   return check_launch("attn_decode");
 }
 
-extern "C" int evk_attn_decode_dev(const float* qkv, int64_t batch_stride, int32_t ld, const int32_t* n_prev_dev, int32_t B, int32_t H,
-                                   float scale, float* out, int32_t ldo, cudaStream_t st) {
+extern "C" int evk_attn_decode_dev(const float* qkv, int64_t batch_stride, int32_t ld, const int32_t* n_prev_dev, const int32_t* skip,
+                                   int32_t B, int32_t H, float scale, float* out, int32_t ldo, cudaStream_t st) {
   EVK_REQUIRE(qkv && out && n_prev_dev && B >= 1 && H >= 1, EVK_ERR_ARG, "attn_decode_dev: bad arguments");
   EVK_REQUIRE(ld >= 3 * H * 32 && ldo >= H * 32, EVK_ERR_ARG, "attn_decode_dev: row pitch %d / %d too small for %d heads of 32", ld, ldo, H);
   EVK_REQUIRE(ld % 4 == 0 && batch_stride % 4 == 0 && ((uintptr_t)qkv % 16) == 0, EVK_ERR_ARG, "attn_decode_dev: rows must be 16-byte aligned");
-  attn_decode_kernel<<<dim3(H, B), 128, 0, st>>>(qkv, batch_stride, ld, 0, n_prev_dev, H, scale, out, ldo);
+  attn_decode_kernel<<<dim3(H, B), 128, 0, st>>>(qkv, batch_stride, ld, 0, n_prev_dev, skip, H, scale, out, ldo);
   return check_launch("attn_decode_dev");
 }
 

@@ -24,6 +24,11 @@ from .models import ParamTree
 
 
 INFER_GRAPH = os.environ.get("EVK_INFER_GRAPH", "1") != "0"      # token step of infer_panel as one replayed CUDA graph
+# infer_panel_batch_infer replays its step graph this many times between two reads of the finished flags: a read costs a host
+# round trip (~tens of us), a step of 16 rows ~1 ms, so 8 replays keep the check under a few percent of the loop while a batch
+# runs at most 7 steps past its last row's finish.
+INFER_BATCH_K = 8
+MAX_DECODE_STEPS = 1500                                            # t2s_model.py:646 (`for idx in range(1500)`)
 
 
 def sine_table(length, dim):
@@ -194,26 +199,28 @@ class Text2SemanticDecoder(ParamTree):
             logits = torch.where(logits < v[:, -1].unsqueeze(-1), -float("inf"), logits)
         return torch.softmax(logits, dim=-1)
 
-    def _infer_layer(self, i, h, cache, n_prev, X=None, xl=None, yl=None):
-        """One post-LN block in inference.  Prompt pass (X given): h [1, L, D], prefix-LM attention, cache rows 0..L-1 filled
-        (T2SBlock.process_prompt, t2s_model.py:121-185).  Token pass: h [1, 1, D], its in_proj row is appended to the cache
-        and attends every cached position (decode_next_token, :187-221)."""
+    def _infer_layer(self, i, h, cache, n_prev, X=None, xl=None, yl=None, skip=None):
+        """One post-LN block in inference.  Prompt pass (X given): h [B, L, D], prefix-LM attention, cache rows 0..L-1 filled
+        (T2SBlock.process_prompt, t2s_model.py:121-185).  Token pass: h [B, 1, D], its in_proj row is appended to the cache
+        and attends every cached position (decode_next_token, :187-221).  skip ([B, 2] int32, batched token pass): row b leaves
+        out its text padding skip[b, 0] .. skip[b, 1] - 1, and the Linears run on ops.linear_rows (exact fp32 for up to 64 rows)."""
         p = f"h.layers.{i}."
         H = self.num_head
-        qkv = ops.linear(h, self.w(p + "self_attn.in_proj", suffix="_weight"), self.P(p + "self_attn.in_proj_bias"))
+        lin = ops.linear if skip is None else ops.linear_rows
+        qkv = lin(h, self.w(p + "self_attn.in_proj", suffix="_weight"), self.P(p + "self_attn.in_proj_bias"))
         L = qkv.shape[1]
         if torch.is_tensor(n_prev):                                # device-side position: the step is a replayed CUDA graph
-            a = ops.attn_decode_dev(cache, n_prev, H, qkv)
+            a = ops.attn_decode_dev(cache, n_prev, H, qkv, skip)
         elif X is not None:
             cache[:, n_prev:n_prev + L].copy_(qkv)
             a = ops.flash_attention(qkv, heads=H, prefix=X, xlen=xl, ylen=yl, p_drop=0.0, tag=f"gpt.infer{i}")
         else:
             cache[:, n_prev:n_prev + L].copy_(qkv)
             a = ops.attn_decode(cache, n_prev + 1, H)
-        a = ops.linear(a, self.w(p + "self_attn.out_proj"), self.b(p + "self_attn.out_proj"))
+        a = lin(a, self.w(p + "self_attn.out_proj"), self.b(p + "self_attn.out_proj"))
         h = ops.layernorm(h, self.P(p + "norm1.weight"), self.P(p + "norm1.bias"), res=a)
-        f = ops.linear(h, self.w(p + "linear1"), self.b(p + "linear1"), act=ops.ACT_RELU)
-        f = ops.linear(f, self.w(p + "linear2"), self.b(p + "linear2"))
+        f = lin(h, self.w(p + "linear1"), self.b(p + "linear1"), act=ops.ACT_RELU)
+        f = lin(f, self.w(p + "linear2"), self.b(p + "linear2"))
         return ops.layernorm(h, self.P(p + "norm2.weight"), self.P(p + "norm2.bias"), res=f)
 
     def _infer_state(self, dev, need_rows):
@@ -336,6 +343,183 @@ class Text2SemanticDecoder(ParamTree):
         """t2s_model.py:869-882."""
         return self.infer_panel_naive(x, x_lens, prompts, bert_feature, top_k, top_p, early_stop_num, temperature,
                                       repetition_penalty, **kwargs)
+
+
+    def infer_panel_naive_batched(self, x, x_lens, prompts, bert_feature, top_k=-100, top_p=100, early_stop_num=-1, temperature=1.0,
+                                  repetition_penalty=1.35, **kwargs):
+        """t2s_model.py:732-760: infer_panel_naive on each utterance in turn -> (list of 1-D y, list of idx)."""
+        y_list, idx_list = [], []
+        for i in range(len(x)):
+            y, idx = self.infer_panel_naive(x[i].unsqueeze(0), x_lens[i], prompts[i].unsqueeze(0) if prompts is not None else None,
+                                            bert_feature[i].unsqueeze(0), top_k, top_p, early_stop_num, temperature,
+                                            repetition_penalty, **kwargs)
+            y_list.append(y[0])
+            idx_list.append(idx)
+        return y_list, idx_list
+
+    def _batch_state(self, dev, B, need_rows):
+        """Per-layer caches [B, rows, 3 D] and the static buffers / graph of the batched token step, kept across calls while the
+        parameters, B and the capacity allow (one state at a time: a new shape frees the previous one first)."""
+        ver = sum(int(p._version) for p in self.parameters())
+        st = self.__dict__.get("_batch_st")
+        if st is not None and st["ver"] == ver and st["dev"] == dev and st["B"] == B and st["rows"] >= need_rows:
+            return st
+        self.__dict__.pop("_batch_st", None)
+        rows = (need_rows + 63) // 64 * 64
+        D, V, Vp = self.model_dim, self.vocab_size, (self.vocab_size + 3) // 4 * 4
+
+        def z(*shape, dtype=torch.float32):
+            return torch.zeros(shape, device=dev, dtype=dtype)
+        st = dict(ver=ver, dev=dev, B=B, rows=rows, graph=None,
+                  caches=[torch.empty((B, rows, 3 * D), device=dev, dtype=torch.float32) for _ in range(self.num_layers)],
+                  n=z(1, dtype=torch.int32), x=z(B, 1, D), logits=z(B, Vp), skip=z(B, 2, dtype=torch.int32),
+                  hist=z(B, rows, dtype=torch.int64), seen=z(B, (V + 31) // 32, dtype=torch.int32), fin=z(B, 2, dtype=torch.int32),
+                  icfg=z(6, dtype=torch.int64), fcfg=z(3), pe=self.pe(rows, dev))
+        self.__dict__["_batch_st"] = st
+        return st
+
+    def _capture_batch_step(self, st, head):
+        """One decoding step of every row as one CUDA graph: sample from st["logits"] (writes the token, the finished flags and
+        the next input row st["x"]), the 24 layers on st["x"], the vocabulary projection into st["logits"], position + 1."""
+        emb = self.P("ar_audio_embedding.word_embeddings.weight")
+        a_audio = self.P("ar_audio_position.alpha")
+
+        def step():
+            ops.sample_tokens(st["logits"], self.vocab_size, self.EOS, st["icfg"], st["fcfg"], st["n"], st["hist"], st["seen"],
+                              st["fin"], emb, st["pe"], a_audio, st["x"])
+            h = st["x"]
+            for i in range(self.num_layers):
+                h = self._infer_layer(i, h, st["caches"][i], st["n"], skip=st["skip"])
+            st["logits"].copy_(ops.linear_rows(h, head).view(st["logits"].shape))
+            st["n"].add_(1)
+        # warm-up and capture with every row marked finished (the sampler is then a no-op) at position 0 with nothing skipped;
+        # the caller overwrites all of it before the first replay
+        st["fin"].fill_(0)
+        st["n"].zero_()
+        st["skip"].zero_()
+        side = torch.cuda.Stream(device=st["dev"])
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):                              # outside capture: allocator, lazy inits, shared-memory opt-ins
+            step()
+        torch.cuda.current_stream().wait_stream(side)
+        st["n"].zero_()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            step()
+        st["graph"] = g
+
+    @torch.no_grad()
+    def infer_panel_batch_infer(self, x, x_lens, prompts, bert_feature, top_k=-100, top_p=100, early_stop_num=-1, temperature=1.0,
+                                repetition_penalty=1.35, **kwargs):
+        """t2s_model.py:563-730: every sentence of a batch decoded together on one KV cache -> (y_list, idx_list), y_list[b] a
+        1-D int64 device tensor (prompt + generated tokens), idx_list[b] an int.
+
+        x: list of 1-D phoneme-id tensors, or a padded [B, X] tensor (row b then has width X); bert_feature: list of [1024, X_b]
+        tensors of the same widths; x_lens [B]; prompts [B, Yp] (one prompt length for all rows, as TTS builds it with .expand);
+        kwargs["max_len"] (default x_lens.max()) is the common text length the rows are right-padded to.  top_k must lie in
+        [1, V].  With prompts None the call goes to infer_panel_naive_batched, as the reference does (:576-578; it does not
+        pass repetition_penalty on, so the default 1.35 applies), and that path does not implement prompt-free decoding.
+
+        Restated from the reference, quirks included:
+          - padded text positions (x_len_b <= t < max_len) are neither attended nor attending (:617-636); the position of row
+            b's next input is pe[Yp + idx] for every row (:705);
+          - EOS is excluded at step 0 only (`logits[:, :-1]` when idx == 0, :651-652; infer_panel_naive excludes it for the
+            first 11 steps);
+          - a row stops when its sampled token OR the argmax of its penalised logits is EOS (:662-672): the penalty is written
+            into the logits in place (utils.py:123), so the argmax sees it;
+          - a row finishing on EOS at step idx returns y[:-1] and idx - 1 (:673-677);
+          - when early_stop_num is reached (idx + 1 > early_stop_num, :688) or at idx == 1499, every remaining row stops at that
+            idx and returns y[:-1] and idx (:688-694);
+          - decoding is capped at 1500 steps (:646); rows that never set their index would get 1499 (:708-712), which the cap
+            already guarantees.
+        Device path: one prompt pass over [B, max_len + Yp] on the training kernels (ragged prefix-LM flash attention with
+        xlen = x_lens, ylen = Yp) fills per-layer caches of in_proj rows; then one CUDA graph per step (fused sampler + 24 layers
+        of exact-fp32 row Linears and per-row-key decode attention + vocabulary projection) is replayed INFER_BATCH_K times
+        between reads of the finished flags.  There is no per-token host sync.  Finished rows stay in the batch, frozen (the
+        reference compacts them away; rows are independent, so the results are the same).  The caches hold
+        max_len + Yp + min(1500, early_stop_num + 1) + INFER_BATCH_K rows (rounded up to 64) of 3 * 512 floats per layer and row:
+        24 layers x B x rows x 6 KiB, e.g. 1.4 GiB for B = 16, max_len 120, Yp 150, early_stop_num 300 (640 rows).
+        Random stream: the reference draws torch.exponential_ over a batch that shrinks as rows finish; here each Exp(1) draw is
+        a counter-based function of (seed, row, step, token id) with the seed drawn once per call from torch's CUDA default
+        generator, so torch.manual_seed still makes a run reproducible but sampled tokens differ from the reference's.
+        Greedy decoding (top_k = 1) does not depend on the stream.  kwargs["trace"] (a list, tests) receives the raw [B, V]
+        logits of every step and makes the host check the flags after every step."""
+        if prompts is None:
+            return self.infer_panel_naive_batched(x, x_lens, prompts, bert_feature, top_k=top_k, top_p=top_p,
+                                                  early_stop_num=early_stop_num, temperature=temperature, **kwargs)
+        B = len(x)
+        V, EOS, D = self.vocab_size, self.EOS, self.model_dim
+        if int(top_k) != top_k or not 1 <= top_k <= V:
+            raise ValueError(f"infer_panel_batch_infer: top_k must be an integer in [1, {V}], got {top_k!r}")
+        top_k = int(top_k)
+        if len(bert_feature) != B or prompts.dim() != 2 or prompts.shape[0] != B or len(x_lens) != B:
+            raise ValueError("infer_panel_batch_infer: x, x_lens, prompts and bert_feature must have one entry per row")
+        if B > 64:                                                 # the row Linears take 64 rows per launch
+            out = [self.infer_panel_batch_infer(x[i:i + 64], x_lens[i:i + 64], prompts[i:i + 64], bert_feature[i:i + 64], top_k,
+                                                top_p, early_stop_num, temperature, repetition_penalty,
+                                                **dict(kwargs, max_len=kwargs.get("max_len", max(int(v) for v in x_lens))))
+                   for i in range(0, B, 64)]
+            return [y for o in out for y in o[0]], [i for o in out for i in o[1]]
+        dev = prompts.device
+        xl_host = [int(v) for v in x_lens]
+        max_len = int(kwargs.get("max_len", max(xl_host)))
+        rows = [x[b] for b in range(B)]
+        for b in range(B):
+            if rows[b].dim() != 1 or bert_feature[b].shape != (1024, rows[b].shape[0]) or not 1 <= xl_host[b] <= rows[b].shape[0] <= max_len:
+                raise ValueError(f"infer_panel_batch_infer: row {b}: x {tuple(rows[b].shape)}, bert_feature {tuple(bert_feature[b].shape)}, "
+                                 f"x_len {xl_host[b]}, max_len {max_len}")
+        Yp = prompts.shape[1]
+        L0 = max_len + Yp
+        cap = MAX_DECODE_STEPS if early_stop_num == -1 else min(MAX_DECODE_STEPS, early_stop_num + 1)
+        K = INFER_BATCH_K
+        was_training = self.training
+        self.eval()
+        self._active, self._memo_pack = self.packed_for_inference(), True
+        try:
+            xp = torch.zeros((B, max_len), device=dev, dtype=torch.int64)
+            bp = torch.zeros((B, 1024, max_len), device=dev, dtype=torch.float32)
+            for b in range(B):
+                xp[b, :rows[b].shape[0]] = rows[b]
+                bp[b, :, :rows[b].shape[0]] = bert_feature[b]
+            st = self._batch_state(dev, B, L0 + cap + K)
+            Vp = st["logits"].shape[1]
+            head = self.w("ar_predict_layer", pad0=Vp)
+            if st["graph"] is None:
+                self._capture_batch_step(st, head)
+            # prompt pass (process_prompt with the padded mask, :596-646)
+            y = prompts.to(torch.int64)
+            xe = self._embed_text(xp, bp, False)
+            ye = ops.embedding(self.P("ar_audio_embedding.word_embeddings.weight"), y)
+            h = ops.gpt_embed(xe, ye, self.P("ar_text_position.alpha"), self.P("ar_audio_position.alpha"), st["pe"])
+            xl = torch.tensor(xl_host, device=dev, dtype=torch.int64)
+            yl = torch.full((B,), Yp, device=dev, dtype=torch.int64)
+            for i in range(self.num_layers):
+                h = self._infer_layer(i, h, st["caches"][i], 0, max_len, xl, yl)
+            st["logits"].copy_(ops.linear_rows(h[:, -1:].contiguous(), head).view(B, Vp))
+            # per-call state of the step graph
+            st["n"].fill_(L0)
+            st["skip"].copy_(torch.tensor([[v, max_len] for v in xl_host], dtype=torch.int32))
+            st["hist"][:, :Yp].copy_(y)
+            bits = torch.zeros((B, st["seen"].shape[1] * 32), device=dev, dtype=torch.int64).scatter_(1, y, 1)
+            words = (bits.view(B, -1, 32) << torch.arange(32, device=dev, dtype=torch.int64)).sum(-1)
+            st["seen"].copy_(torch.where(words >= 2 ** 31, words - 2 ** 32, words))      # uint32 bit patterns as int32
+            st["fin"].fill_(-1)
+            st["icfg"][0:1].copy_(torch.randint(0, 2 ** 62, (1,), device=dev, dtype=torch.int64))
+            st["icfg"][1:].copy_(torch.tensor([Yp, L0, top_k, early_stop_num, MAX_DECODE_STEPS], dtype=torch.int64))
+            st["fcfg"].copy_(torch.tensor([float(top_p), float(temperature), float(repetition_penalty)], dtype=torch.float32))
+            trace = kwargs.get("trace")
+            while True:
+                for _ in range(K if trace is None else 1):
+                    if trace is not None:
+                        trace.append(st["logits"][:, :V].clone())
+                    st["graph"].replay()
+                if not bool((st["fin"][:, 0] < 0).any()):
+                    break
+            fin = st["fin"].cpu().tolist()
+            return [st["hist"][b, :Yp + fin[b][0]].clone() for b in range(B)], [f[1] for f in fin]
+        finally:
+            self._active, self._memo_pack = None, False
+            self.train(was_training)
 
 
 def make_reject_y(y_o, y_lens, generator=None):

@@ -717,6 +717,14 @@ def _gemv_rows(x, w, bias, act, slope):
     return y
 
 
+def linear_rows(x, w: PackedW, bias=None, act=ACT_NONE, slope=0.0):
+    """Exact-fp32 Linear of the batched token step: [..., C] with 1..64 rows in total -> [..., N], one pass over the packed
+    weight (evk_gemv_rows).  A row's result does not depend on how many rows share the launch.  No gradient."""
+    rows = x.numel() // max(x.shape[-1], 1)
+    assert w.Q == 1 and 1 <= rows <= 64 and act in (ACT_NONE, ACT_RELU, ACT_LRELU), (rows, act)
+    return _gemv_rows(x, w, bias, act, slope)
+
+
 def linear(x, w: PackedW, bias=None, act=ACT_NONE, slope=0.0, out_len=None, in_len=None, res=None, drop=None):
     """nn.Linear / 1x1 conv on [B, T, C] or [rows, C].  drop = (p, tag): dropout_p(relu(x W^T + b)) with the dropout applied in
     the GEMM epilogue when fused_dropout_ok (else as a separate kernel)."""
@@ -1918,17 +1926,31 @@ def attn_decode(cache, n_keys, heads):
     return out
 
 
-def attn_decode_dev(cache, n_prev_dev, heads, row):
+def attn_decode_dev(cache, n_prev_dev, heads, row, skip=None):
     """Graph-replayable token step: append `row` [B, 1, 3 * heads * 32] at index *n_prev_dev (int32 device scalar) of the cache
-    and attend rows 0 .. *n_prev_dev.  -> [B, 1, heads * 32]."""
+    and attend rows 0 .. *n_prev_dev.  -> [B, 1, heads * 32].  skip: optional int32 device [B, 2]; item b then leaves out the
+    keys skip[b, 0] .. skip[b, 1] - 1 (its text padding in a batch padded to a common text length)."""
     assert cache.dim() == 3 and cache.stride(2) == 1 and cache.shape[2] == 3 * heads * 32 and n_prev_dev.dtype == torch.int32
+    assert skip is None or (skip.dtype == torch.int32 and skip.is_contiguous() and tuple(skip.shape) == (cache.shape[0], 2))
     B, W = cache.shape[0], cache.shape[2]
     row = row.contiguous()
     _call("evk_cache_append", _p(row), W, _p(cache), cache.stride(0), cache.stride(1), _p(n_prev_dev), B, W)
     out = torch.empty((B, 1, heads * 32), device=cache.device, dtype=torch.float32)
-    _call("evk_attn_decode_dev", _p(cache), cache.stride(0), cache.stride(1), _p(n_prev_dev), B, heads,
+    _call("evk_attn_decode_dev", _p(cache), cache.stride(0), cache.stride(1), _p(n_prev_dev), _p(skip), B, heads,
           ctypes.c_float(1.0 / math.sqrt(32.0)), _p(out), heads * 32)
     return out
+
+
+def sample_tokens(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, alpha, x_next, q=None):
+    """One fused sampling step over the rows of `logits` [B, >= V] (evk_sample_tokens; see include/evk.h for the buffers).
+    Everything it reads or writes stays in device memory, so it can be part of a captured CUDA graph."""
+    B, D = logits.shape[0], x_next.shape[-1]
+    assert logits.stride(-1) == 1 and hist.dtype == torch.int64 and seen.dtype == torch.int32 and fin.dtype == torch.int32
+    assert icfg.dtype == torch.int64 and fcfg.dtype == torch.float32 and x_next.is_contiguous() and pe.is_contiguous()
+    assert q is None or (q.shape[0] == B and q.stride(-1) == 1)
+    _call("evk_sample_tokens", _p(logits), logits.stride(0), B, V, eos, _p(icfg), _p(fcfg), _p(n_dev), _p(q),
+          q.stride(0) if q is not None else 0, _p(hist), hist.stride(0), _p(seen), _p(fin), _p(emb), _p(pe), _p(alpha),
+          _p(x_next), D)
 
 
 def ce_sum_topk(logits, targets, topk=3, ignore_index=1024, V=None):

@@ -389,16 +389,35 @@ int evk_sinepos_bwd(const float* dy, int32_t ldy, int64_t dy_sb, const float* pe
 int evk_attn_decode(const float* qkv, int64_t batch_stride, int32_t ld, int32_t n_keys, int32_t B, int32_t H, float scale,
                     float* out, int32_t ldo, evk_stream_t stream);
 /* Skinny Linear of the KV-cache token step (decode_next_token, t2s_model.py:187-221: one new row per utterance):
- * y[r][n] = act(sum_c x[r][c] * W[n][c] + bias[n]) for rows <= 4; W = the packed forward operand PA[0] ([N][ldw], row n = output
- * channel n).  Exact fp32 FMAs, one pass over W.  act: EVK_ACT_NONE / RELU / LRELU. */
+ * y[r][n] = act(sum_c x[r][c] * W[n][c] + bias[n]) for rows <= 64; W = the packed forward operand PA[0] ([N][ldw], row n = output
+ * channel n).  Exact fp32 FMAs, one pass over W.  A row's result does not depend on `rows` (same summation order for every
+ * batch size).  rows <= 4 requires rows_rounded_up_to_a_power_of_2 * C <= 10240.  act: EVK_ACT_NONE / RELU / LRELU. */
 int evk_gemv_rows(const float* x, int32_t ldx, int32_t rows, const float* W, int32_t ldw, const float* bias, float* y,
                   int32_t ldy, int32_t N, int32_t C, int32_t act, float slope, evk_stream_t stream);
 /* The same with the position in DEVICE memory (a decode step replayed as a CUDA graph): *n_prev_dev = rows already in the cache
- * before this token; evk_cache_append writes the token's row at that index, evk_attn_decode_dev attends rows 0 .. *n_prev_dev. */
-int evk_attn_decode_dev(const float* qkv, int64_t batch_stride, int32_t ld, const int32_t* n_prev_dev, int32_t B, int32_t H,
-                        float scale, float* out, int32_t ldo, evk_stream_t stream);
+ * before this token; evk_cache_append writes the token's row at that index, evk_attn_decode_dev attends rows 0 .. *n_prev_dev.
+ * skip: NULL, or device [B][2]: item b leaves out keys skip[b][0] .. skip[b][1] - 1 (the right padding of its text when a batch
+ * is padded to a common text length: skip[b] = (x_len_b, max_len)). */
+int evk_attn_decode_dev(const float* qkv, int64_t batch_stride, int32_t ld, const int32_t* n_prev_dev, const int32_t* skip,
+                        int32_t B, int32_t H, float scale, float* out, int32_t ldo, evk_stream_t stream);
 int evk_cache_append(const float* row, int32_t ldr, float* cache, int64_t batch_stride, int32_t ld, const int32_t* pos_dev,
                      int32_t B, int32_t W, evk_stream_t stream);
+/* Fused token sampler of batched KV-cache decoding (infer_panel_batch_infer, t2s_model.py:563-730; utils.py:109-157), one CTA
+ * per row b of logits [B][ldl] (V <= 2048 classes, eos = V - 1), in the reference's order: repetition penalty over the row's
+ * history (prompt included) -> top-p if top_p < 1 (descending order, cumulative softmax, `cum > top_p` removed, the first kept;
+ * on the penalised, un-tempered logits) -> / max(T, 1e-5) -> top-k (values >= the k-th largest kept) -> softmax ->
+ * argmax(p / q), q ~ Exp(1).  The step is idx = *n_dev - icfg[2]; at idx 0 EOS is excluded.  The row stops when the token or the
+ * argmax of the penalised logits is EOS (fin[b] = (idx, idx - 1)), else when idx + 1 > early_stop (!= -1) or idx == max_steps - 1
+ * (fin[b] = (idx, idx)); a row with fin[b][0] >= 0 is left untouched.  Otherwise hist[b][prefix + idx] = token, its bit is set
+ * in seen, and x_next[b] = emb[token] + alpha[0] * pe[prefix + idx].
+ *   icfg: device int64 [6] = (seed, prefix, n0, top_k >= 1, early_stop, max_steps);  fcfg: device float [3] = (top_p, T, penalty)
+ *   q: NULL (counter-based Exp(1) draws keyed by (seed, row, idx, class)) or supplied draws [B][ldq]
+ *   hist: int64 [B][ldh];  seen: uint32 [B][(V + 31) / 32] bitmap of the tokens in hist;  fin: int32 [B][2], -1 while running
+ *   emb: [V][D], pe: [*][D], x_next: [B][D]. */
+int evk_sample_tokens(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, const int64_t* icfg,
+                      const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist, int32_t ldh,
+                      uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha, float* x_next,
+                      int32_t D, evk_stream_t stream);
 int evk_ce_fwd(const float* logits, int32_t ld, const int64_t* targets, int32_t rows, int32_t V, int32_t topk,
                int64_t ignore_index, float* lse, float* nll, uint8_t* flags, float* out2, evk_stream_t stream);
 int evk_ce_bwd(const float* logits, int32_t ld, const int64_t* targets, const float* lse, const float* gscale,

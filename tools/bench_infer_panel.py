@@ -3,6 +3,9 @@
 (24 layers, d = 512), 120 phonemes + 150 prompt tokens, 300 generated tokens (early_stop_num), top_k 15 / top_p 1 / T 1 as TTS
 calls it.  CPU arm: the reference-equivalent KV-cache loop restated with torch ops on this box's cores (bounded: 40 tokens).
 One JSON line.   python tools/bench_infer_panel.py > gpurun_out/bench_infer_panel.json"""
+# --batch: instead, the same single-utterance number next to infer_panel_batch_infer for B in {1, 4, 16} sentences (each with the
+# same 120 phonemes / 150-token prompt / 300 tokens), as aggregate semantic tokens/s and ms per decoding step, with the card's
+# name and power limit read in the same run.  --profile DIR (with --batch): also a torch.profiler trace of one B = 16 call.
 import json
 import math
 import os
@@ -31,6 +34,41 @@ x = torch.randint(0, m["phoneme_vocab_size"], (1, X), generator=g)
 bert = torch.randn(1, 1024, X, generator=g)
 prompts = torch.randint(0, 1024, (1, Yp), generator=g)
 xd, bd, pd, xl = x.to(dev), bert.to(dev), prompts.to(dev), torch.tensor([X], device=dev)
+BATCH = "--batch" in sys.argv
+
+
+def bench_batch():
+    """infer_panel_batch_infer for B in {1, 4, 16}: aggregate generated tokens / wall time (prompt pass included)."""
+    import subprocess
+    out = {}
+    for B in (1, 4, 16):
+        xs, bs, ps = [xd[0]] * B, [bd[0]] * B, pd.expand(B, -1)
+        lens = torch.full((B,), X)
+        net.infer_panel_batch_infer(xs, lens, ps, bs, top_k=15, top_p=1, early_stop_num=8, temperature=1.0)        # warm-up, capture
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        ys, idx = net.infer_panel_batch_infer(xs, lens, ps, bs, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)
+        torch.cuda.synchronize()
+        s = time.perf_counter() - t0
+        gen = [int(y.shape[0]) - Yp for y in ys]
+        steps = max(gen) + 1
+        out[str(B)] = dict(tokens_per_s=sum(gen) / s, ms_per_step=s / steps * 1e3, generated=sum(gen), steps=steps, seconds=s)
+    if "--profile" in sys.argv:
+        d = sys.argv[sys.argv.index("--profile") + 1]
+        os.makedirs(d, exist_ok=True)
+        B = 16
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA]) as prof:
+            net.infer_panel_batch_infer([xd[0]] * B, torch.full((B,), X), pd.expand(B, -1), [bd[0]] * B, top_k=15, top_p=1,
+                                        early_stop_num=40, temperature=1.0)
+            torch.cuda.synchronize()
+        prof.export_chrome_trace(os.path.join(d, "infer_batch_b16.pt.trace.json"))
+        with open(os.path.join(d, "infer_batch_b16_kernels.txt"), "w") as f:
+            f.write(prof.key_averages().table(sort_by="cuda_time_total", row_limit=30))
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True).stdout.strip().splitlines()
+    return out, card[0] if card else "unknown"
+
+
 net.infer_panel(xd, xl, pd, bd, top_k=15, top_p=1, early_stop_num=8, temperature=1.0)     # warm-up (packs the weights once)
 torch.cuda.synchronize()
 t0 = time.perf_counter()
@@ -77,6 +115,13 @@ def cpu_cached_decode(n_new):
             last, kc[i], vc[i] = block(i, last, None, kc[i], vc[i])
 
 
+if BATCH:
+    batch, card = bench_batch()
+    print(json.dumps(dict(metric="Text2SemanticDecoder.infer_panel_batch_infer (batched KV-cache AR decoding)", unit="semantic-tokens/s",
+                          card=card, single_utterance=dict(tokens_per_s=new / gpu_s, ms_per_token=gpu_s / max(new, 1) * 1e3, generated=new),
+                          batch=batch, config=dict(layers=24, X=X, prompt=Yp, early_stop_num=NEW, top_k=15, top_p=1, temperature=1.0),
+                          note="aggregate generated tokens over wall time of one call, prompt pass included; 25 tokens = 1 s of audio")))
+    sys.exit(0)
 threads = min(16, os.cpu_count() or 1)
 torch.set_num_threads(threads)
 n_cpu = 40
