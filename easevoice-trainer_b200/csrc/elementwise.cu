@@ -637,8 +637,9 @@ extern "C" int evk_phase_split(const float* x, int32_t ldx, int64_t x_sb, float*
 }
 extern "C" int evk_embedding(const float* table, int32_t ldt, const int64_t* idx, int64_t rows, int32_t rep, float* y,
                              int32_t ldy, int32_t C, evk_stream_t stream) {
-  EVK_REQUIRE(table && idx && y && rep >= 1, EVK_ERR_ARG, "embedding: bad arguments");
-  if (rows * C == 0) return EVK_OK;
+  EVK_REQUIRE(rep >= 1, EVK_ERR_ARG, "embedding: bad arguments");
+  if (rows * C == 0) return EVK_OK;                          // nothing to read or write (an empty tensor may have a null pointer)
+  EVK_REQUIRE(table && idx && y, EVK_ERR_ARG, "embedding: bad arguments");
   embedding_kernel<<<grid1d(rows * C), 256, 0, ST>>>(table, ldt, (const long long*)idx, rows, rep, y, ldy, C);
   return check_launch("embedding");
 }

@@ -1,4 +1,5 @@
-// Fused token sampler of batched AR decoding (Text2SemanticDecoder.infer_panel_batch_infer, t2s_model.py:563-730):
+// Fused token sampler of batched AR decoding (Text2SemanticDecoder.infer_panel_batch_infer, t2s_model.py:563-730, and the
+// batched prompt-free path of infer_panel_naive_batched, :732-863):
 // one CTA per batch row does the whole of utils.py:109-157 on that row's logits, appends the token to the row's history and
 // writes the next input row, so a decode step needs no host round trip and replays as part of one CUDA graph.
 #include <float.h>
@@ -44,7 +45,7 @@ __device__ __forceinline__ void block_argmax(float& v, int& i, float* rv, int* r
 }
 
 __global__ void __launch_bounds__(kSampThreads) sample_tokens_kernel(
-    const float* __restrict__ logits, int ldl, int V, int eos, const long long* __restrict__ icfg, const float* __restrict__ fcfg,
+    const float* __restrict__ logits, int ldl, int V, int eos, int eos_steps, const long long* __restrict__ icfg, const float* __restrict__ fcfg,
     const int* __restrict__ n_dev, const float* __restrict__ q, int ldq, long long* __restrict__ hist, int ldh,
     unsigned* __restrict__ seen, int* __restrict__ fin, const float* __restrict__ emb, const float* __restrict__ pe,
     const float* __restrict__ alpha, float* __restrict__ x_next, int D) {
@@ -61,11 +62,12 @@ __global__ void __launch_bounds__(kSampThreads) sample_tokens_kernel(
   const int idx = *n_dev - n0;                                   // decoding step of this replay
   const int W = (V + 31) >> 5;
   const unsigned* sb = seen + (size_t)b * W;
-  // 1. repetition penalty over the row's history, prompt included (utils.py:117-123); step 0 leaves EOS out (:651-652)
+  // 1. repetition penalty over the row's history, prompt included (utils.py:117-123); steps idx < eos_steps leave EOS out
+  //    (batched decoding: step 0 only, :651-652; prompt-free decoding: the first 11 steps, :835-836)
   for (int i = tid; i < V; i += blockDim.x) {
     float l = logits[(size_t)b * ldl + i];
     if ((sb[i >> 5] >> (i & 31)) & 1u) l = l < 0.f ? l * pen : l / pen;
-    pl[i] = (idx == 0 && i == eos) ? -INFINITY : l;
+    pl[i] = (idx < eos_steps && i == eos) ? -INFINITY : l;
   }
   __syncthreads();
   float amv = -INFINITY;
@@ -151,15 +153,24 @@ __global__ void __launch_bounds__(kSampThreads) sample_tokens_kernel(
 
 using namespace evk;
 
-extern "C" int evk_sample_tokens(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, const int64_t* icfg,
-                                 const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist, int32_t ldh,
-                                 uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha, float* x_next,
-                                 int32_t D, cudaStream_t st) {
+extern "C" int evk_sample_tokens_ex(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, int32_t eos_steps,
+                                    const int64_t* icfg, const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq,
+                                    int64_t* hist, int32_t ldh, uint32_t* seen, int32_t* fin, const float* emb, const float* pe,
+                                    const float* alpha, float* x_next, int32_t D, cudaStream_t st) {
   EVK_REQUIRE(logits && icfg && fcfg && n_dev && hist && seen && fin && emb && pe && alpha && x_next, EVK_ERR_ARG,
               "sample_tokens: null argument");
   EVK_REQUIRE(B >= 1 && V >= 2 && V <= kSampMaxV && eos >= 0 && eos < V && ldl >= V && D >= 1 && (!q || ldq >= V), EVK_ERR_ARG,
               "sample_tokens: bad shape (B=%d V=%d eos=%d ldl=%d)", B, V, eos, ldl);
-  sample_tokens_kernel<<<B, kSampThreads, 0, st>>>(logits, ldl, V, eos, (const long long*)icfg, fcfg, n_dev, q, ldq, (long long*)hist,
-                                                   ldh, seen, fin, emb, pe, alpha, x_next, D);
+  EVK_REQUIRE(eos_steps >= 0, EVK_ERR_ARG, "sample_tokens: eos_steps must be >= 0, got %d", eos_steps);
+  sample_tokens_kernel<<<B, kSampThreads, 0, st>>>(logits, ldl, V, eos, eos_steps, (const long long*)icfg, fcfg, n_dev, q, ldq,
+                                                   (long long*)hist, ldh, seen, fin, emb, pe, alpha, x_next, D);
   return check_launch("sample_tokens");
+}
+
+extern "C" int evk_sample_tokens(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, const int64_t* icfg,
+                                 const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist, int32_t ldh,
+                                 uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha, float* x_next,
+                                 int32_t D, cudaStream_t st) {
+  return evk_sample_tokens_ex(logits, ldl, B, V, eos, 1, icfg, fcfg, n_dev, q, ldq, hist, ldh, seen, fin, emb, pe, alpha, x_next,
+                              D, st);
 }

@@ -266,18 +266,25 @@ class Text2SemanticDecoder(ParamTree):
         The prompt pass runs the training forward's kernels and fills a per-layer cache of in_proj rows; every further token is
         24 x (6 Linear launches on a one-row operand + one KV-cache attention + two LayerNorms).  Sampling follows utils.py:102-157
         (exponential-race multinomial on the device).  `trace` (list) receives the [1, V] logits of every step (tests).
-        Prompt-free decoding (prompts = None) is not implemented on this path."""
-        if prompts is None:
-            raise NotImplementedError("infer_panel: prompt-free decoding is not implemented on the sm_90a path")
-        assert x.shape[0] == 1 and prompts.shape[0] == 1, "one utterance at a time, like infer_panel_naive"
+        EOS is excluded for the first 11 steps (:835-836).
+        Prompt-free decoding (prompts = None, TTS's ref_text_free mode; :796-803, :858-862): the prompt pass covers the text
+        alone (full attention over it), the first logits come from the last text position, the token of step idx is embedded at
+        pe[idx], and the result is (generated tokens without the last sample [1, n], 0); early_stop_num = 0 gives [1, 0].
+        There is no CPU path: prompt-free inputs that are not CUDA tensors raise NotImplementedError."""
+        if prompts is None and not (x.is_cuda and bert_feature.is_cuda):
+            raise NotImplementedError("infer_panel: prompt-free decoding runs on CUDA tensors only (there is no CPU path)")
+        assert x.shape[0] == 1 and (prompts is None or prompts.shape[0] == 1), "one utterance at a time, like infer_panel_naive"
         was_training = self.training
         self.eval()
         self._active, self._memo_pack = self.packed_for_inference(), True
         try:
             dev = x.device
             D, V = self.model_dim, self.vocab_size
-            X, Yp = x.shape[1], prompts.shape[1]
-            y = prompts.to(torch.int64)
+            X = x.shape[1]
+            if prompts is None:                                          # :802: an empty token history
+                y, Yp = torch.zeros((1, 0), device=dev, dtype=torch.int64), 0
+            else:
+                y, Yp = prompts.to(torch.int64), prompts.shape[1]
             xe = self._embed_text(x, bert_feature, False)
             ye = ops.embedding(self.P("ar_audio_embedding.word_embeddings.weight"), y)
             pe = self.pe(max(X, Yp + max_steps + 2), dev)
@@ -320,7 +327,7 @@ class Text2SemanticDecoder(ParamTree):
                     stop = True
                 if stop:
                     break
-                # next input: embedding of the sampled token at position Yp + idx (t2s_model.py:861-862, x_scale = 1)
+                # next input: embedding of the sampled token at position Yp + idx (t2s_model.py:858-859, x_scale = 1)
                 last = (emb[y[:, -1:]] + a_audio * pe[Yp + idx]).contiguous()
                 if use_graph:
                     # the whole 24-layer token step (+ the vocabulary projection) is ONE graph replay; the position lives in
@@ -333,7 +340,7 @@ class Text2SemanticDecoder(ParamTree):
                     for i in range(self.num_layers):
                         last = self._infer_layer(i, last, caches[i], n)
                     n += 1
-            return y[:, :-1], idx - 1
+            return y[:, :-1], (0 if prompts is None else idx - 1)        # :861-863
         finally:
             self._active, self._memo_pack = None, False
             self.train(was_training)
@@ -347,7 +354,19 @@ class Text2SemanticDecoder(ParamTree):
 
     def infer_panel_naive_batched(self, x, x_lens, prompts, bert_feature, top_k=-100, top_p=100, early_stop_num=-1, temperature=1.0,
                                   repetition_penalty=1.35, **kwargs):
-        """t2s_model.py:732-760: infer_panel_naive on each utterance in turn -> (list of 1-D y, list of idx)."""
+        """t2s_model.py:732-760: infer_panel_naive on each utterance in turn -> (list of 1-D y, list of idx).
+
+        Prompt-free (prompts None, TTS's ref_text_free mode): x is a list of 1-D phoneme-id tensors or a padded [B, X] tensor,
+        bert_feature a list of [1024, width of x[b]].  As in the reference, row b's text is all of x[b] (x[b].shape[0] positions):
+        x_lens is not read, so the padding of a padded [B, X] tensor is decoded as text.  top_k must lie in [1, V].  On CUDA
+        inputs every row is decoded together (_infer_ref_free_batched); each row gives what infer_panel_naive(prompts=None)
+        gives on it alone, up to the sampling noise: (y_list, [0] * B), y_list[b] the generated tokens without the last sample.
+        Other inputs keep the per-row loop, which has no CPU path and raises NotImplementedError."""
+        if prompts is None:
+            self._check_ref_free(x, bert_feature, top_k)
+            if all(t.is_cuda for t in list(x) + list(bert_feature)):
+                return self._infer_ref_free_batched(x, bert_feature, top_k, top_p, early_stop_num, temperature, repetition_penalty,
+                                                    **kwargs)
         y_list, idx_list = [], []
         for i in range(len(x)):
             y, idx = self.infer_panel_naive(x[i].unsqueeze(0), x_lens[i], prompts[i].unsqueeze(0) if prompts is not None else None,
@@ -370,7 +389,7 @@ class Text2SemanticDecoder(ParamTree):
 
         def z(*shape, dtype=torch.float32):
             return torch.zeros(shape, device=dev, dtype=dtype)
-        st = dict(ver=ver, dev=dev, B=B, rows=rows, graph=None,
+        st = dict(ver=ver, dev=dev, B=B, rows=rows, graphs={},
                   caches=[torch.empty((B, rows, 3 * D), device=dev, dtype=torch.float32) for _ in range(self.num_layers)],
                   n=z(1, dtype=torch.int32), x=z(B, 1, D), logits=z(B, Vp), skip=z(B, 2, dtype=torch.int32),
                   hist=z(B, rows, dtype=torch.int64), seen=z(B, (V + 31) // 32, dtype=torch.int32), fin=z(B, 2, dtype=torch.int32),
@@ -378,7 +397,14 @@ class Text2SemanticDecoder(ParamTree):
         self.__dict__["_batch_st"] = st
         return st
 
-    def _capture_batch_step(self, st, head):
+    def _batch_step_graph(self, st, head, eos_steps):
+        """The step graph of `st` whose sampler excludes EOS at the steps idx < eos_steps (a kernel argument, fixed at capture:
+        1 for infer_panel_batch_infer, 11 for prompt-free decoding), captured on first use."""
+        if eos_steps not in st["graphs"]:
+            st["graphs"][eos_steps] = self._capture_batch_step(st, head, eos_steps)
+        return st["graphs"][eos_steps]
+
+    def _capture_batch_step(self, st, head, eos_steps):
         """One decoding step of every row as one CUDA graph: sample from st["logits"] (writes the token, the finished flags and
         the next input row st["x"]), the 24 layers on st["x"], the vocabulary projection into st["logits"], position + 1."""
         emb = self.P("ar_audio_embedding.word_embeddings.weight")
@@ -386,7 +412,7 @@ class Text2SemanticDecoder(ParamTree):
 
         def step():
             ops.sample_tokens(st["logits"], self.vocab_size, self.EOS, st["icfg"], st["fcfg"], st["n"], st["hist"], st["seen"],
-                              st["fin"], emb, st["pe"], a_audio, st["x"])
+                              st["fin"], emb, st["pe"], a_audio, st["x"], eos_steps=eos_steps)
             h = st["x"]
             for i in range(self.num_layers):
                 h = self._infer_layer(i, h, st["caches"][i], st["n"], skip=st["skip"])
@@ -406,7 +432,24 @@ class Text2SemanticDecoder(ParamTree):
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             step()
-        st["graph"] = g
+        return g
+
+    def _run_batch(self, st, graph, prefix, n0, top_k, early_stop_num, top_p, temperature, repetition_penalty, trace):
+        """Decode every row of `st` (prompt pass done: caches, logits, n, skip, hist and seen set) until all have finished ->
+        fin as a host list of [stop step, idx] per row.  The noise seed is drawn here, once per call, from torch's CUDA generator."""
+        dev, K = st["dev"], INFER_BATCH_K
+        st["fin"].fill_(-1)
+        st["icfg"][0:1].copy_(torch.randint(0, 2 ** 62, (1,), device=dev, dtype=torch.int64))
+        st["icfg"][1:].copy_(torch.tensor([prefix, n0, top_k, early_stop_num, MAX_DECODE_STEPS], dtype=torch.int64))
+        st["fcfg"].copy_(torch.tensor([float(top_p), float(temperature), float(repetition_penalty)], dtype=torch.float32))
+        while True:
+            for _ in range(K if trace is None else 1):
+                if trace is not None:
+                    trace.append(st["logits"][:, :self.vocab_size].clone())
+                graph.replay()
+            if not bool((st["fin"][:, 0] < 0).any()):
+                break
+        return st["fin"].cpu().tolist()
 
     @torch.no_grad()
     def infer_panel_batch_infer(self, x, x_lens, prompts, bert_feature, top_k=-100, top_p=100, early_stop_num=-1, temperature=1.0,
@@ -418,7 +461,7 @@ class Text2SemanticDecoder(ParamTree):
         tensors of the same widths; x_lens [B]; prompts [B, Yp] (one prompt length for all rows, as TTS builds it with .expand);
         kwargs["max_len"] (default x_lens.max()) is the common text length the rows are right-padded to.  top_k must lie in
         [1, V].  With prompts None the call goes to infer_panel_naive_batched, as the reference does (:576-578; it does not
-        pass repetition_penalty on, so the default 1.35 applies), and that path does not implement prompt-free decoding.
+        pass repetition_penalty on, so the default 1.35 applies), which decodes the rows prompt-free.
 
         Restated from the reference, quirks included:
           - padded text positions (x_len_b <= t < max_len) are neither attended nor attending (:617-636); the position of row
@@ -484,8 +527,7 @@ class Text2SemanticDecoder(ParamTree):
             st = self._batch_state(dev, B, L0 + cap + K)
             Vp = st["logits"].shape[1]
             head = self.w("ar_predict_layer", pad0=Vp)
-            if st["graph"] is None:
-                self._capture_batch_step(st, head)
+            graph = self._batch_step_graph(st, head, 1)
             # prompt pass (process_prompt with the padded mask, :596-646)
             y = prompts.to(torch.int64)
             xe = self._embed_text(xp, bp, False)
@@ -503,20 +545,77 @@ class Text2SemanticDecoder(ParamTree):
             bits = torch.zeros((B, st["seen"].shape[1] * 32), device=dev, dtype=torch.int64).scatter_(1, y, 1)
             words = (bits.view(B, -1, 32) << torch.arange(32, device=dev, dtype=torch.int64)).sum(-1)
             st["seen"].copy_(torch.where(words >= 2 ** 31, words - 2 ** 32, words))      # uint32 bit patterns as int32
-            st["fin"].fill_(-1)
-            st["icfg"][0:1].copy_(torch.randint(0, 2 ** 62, (1,), device=dev, dtype=torch.int64))
-            st["icfg"][1:].copy_(torch.tensor([Yp, L0, top_k, early_stop_num, MAX_DECODE_STEPS], dtype=torch.int64))
-            st["fcfg"].copy_(torch.tensor([float(top_p), float(temperature), float(repetition_penalty)], dtype=torch.float32))
-            trace = kwargs.get("trace")
-            while True:
-                for _ in range(K if trace is None else 1):
-                    if trace is not None:
-                        trace.append(st["logits"][:, :V].clone())
-                    st["graph"].replay()
-                if not bool((st["fin"][:, 0] < 0).any()):
-                    break
-            fin = st["fin"].cpu().tolist()
+            fin = self._run_batch(st, graph, Yp, L0, top_k, early_stop_num, top_p, temperature, repetition_penalty, kwargs.get("trace"))
             return [st["hist"][b, :Yp + fin[b][0]].clone() for b in range(B)], [f[1] for f in fin]
+        finally:
+            self._active, self._memo_pack = None, False
+            self.train(was_training)
+
+    def _check_ref_free(self, x, bert_feature, top_k):
+        """Argument checks of prompt-free batched decoding (ValueError, before anything runs)."""
+        V = self.vocab_size
+        if int(top_k) != top_k or not 1 <= top_k <= V:
+            raise ValueError(f"infer_panel_naive_batched: top_k must be an integer in [1, {V}], got {top_k!r}")
+        if len(bert_feature) != len(x):
+            raise ValueError("infer_panel_naive_batched: x and bert_feature must have one entry per row")
+        for b in range(len(x)):
+            if x[b].dim() != 1 or x[b].shape[0] < 1 or tuple(bert_feature[b].shape) != (1024, x[b].shape[0]):
+                raise ValueError(f"infer_panel_naive_batched: row {b}: x {tuple(x[b].shape)}, bert_feature {tuple(bert_feature[b].shape)}")
+
+    @torch.no_grad()
+    def _infer_ref_free_batched(self, x, bert_feature, top_k, top_p, early_stop_num, temperature, repetition_penalty, **kwargs):
+        """infer_panel_naive_batched with prompts None on CUDA inputs: infer_panel_naive(prompts=None) (t2s_model.py:762-863) for
+        every row at once, on the machinery of infer_panel_batch_infer.  Row b has len_b = x[b].shape[0] text positions.
+          - Prompt pass: one pass over the right-padded [B, max_len] text (prefix-LM flash attention with X = max_len,
+            xlen = len_b, ylen = 0: each row attends its own text, bidirectionally); row b's first logits come from its last
+            text position h[b, len_b - 1].  max_len = max(kwargs["max_len"], longest row); it does not change the results.
+          - Step idx: the token goes to cache row max_len + idx and is embedded at pe[idx] (y_len = 0, :858-859); each row leaves
+            out its text padding len_b .. max_len - 1; EOS is excluded for idx < 11 (:835-836); a row stops when its sample or
+            the argmax of its penalised logits is EOS, or at idx + 1 > early_stop_num, or at idx 1499.
+          - -> (y_list, [0] * B): y_list[b] the row's generated tokens without the last sample (:861-862).
+        Noise: counter-based Exp(1) draws as in infer_panel_batch_infer, seeded once per call from torch's CUDA generator, so
+        torch.manual_seed reproduces a run and greedy decoding does not depend on it.  kwargs["trace"] as there.  Batches of more
+        than 64 rows run in chunks of 64."""
+        B = len(x)
+        max_len = max([int(kwargs.get("max_len", 0))] + [int(x[b].shape[0]) for b in range(B)])
+        if B > 64:                                                 # the row Linears take 64 rows per launch
+            out = [self._infer_ref_free_batched(x[i:i + 64], bert_feature[i:i + 64], top_k, top_p, early_stop_num, temperature,
+                                                repetition_penalty, **dict(kwargs, max_len=max_len))
+                   for i in range(0, B, 64)]
+            return [y for o in out for y in o[0]], [i for o in out for i in o[1]]
+        dev = x[0].device
+        lens = [int(x[b].shape[0]) for b in range(B)]
+        cap = MAX_DECODE_STEPS if early_stop_num == -1 else min(MAX_DECODE_STEPS, early_stop_num + 1)
+        was_training = self.training
+        self.eval()
+        self._active, self._memo_pack = self.packed_for_inference(), True
+        try:
+            xp = torch.zeros((B, max_len), device=dev, dtype=torch.int64)
+            bp = torch.zeros((B, 1024, max_len), device=dev, dtype=torch.float32)
+            for b in range(B):
+                xp[b, :lens[b]] = x[b]
+                bp[b, :, :lens[b]] = bert_feature[b]
+            st = self._batch_state(dev, B, max_len + cap + INFER_BATCH_K)
+            Vp = st["logits"].shape[1]
+            head = self.w("ar_predict_layer", pad0=Vp)
+            graph = self._batch_step_graph(st, head, 11)
+            # prompt pass over the text alone (:796-803, :825)
+            xe = self._embed_text(xp, bp, False)
+            ye = ops.embedding(self.P("ar_audio_embedding.word_embeddings.weight"), torch.zeros((B, 0), device=dev, dtype=torch.int64))
+            h = ops.gpt_embed(xe, ye, self.P("ar_text_position.alpha"), self.P("ar_audio_position.alpha"), st["pe"])
+            xl = torch.tensor(lens, device=dev, dtype=torch.int64)
+            yl = torch.zeros((B,), device=dev, dtype=torch.int64)
+            for i in range(self.num_layers):
+                h = self._infer_layer(i, h, st["caches"][i], 0, max_len, xl, yl)
+            last = ops.slice_rows(h, xl - 1, 1)                    # [B, 1, D]: each row's last text position
+            st["logits"].copy_(ops.linear_rows(last, head).view(B, Vp))
+            # per-call state of the step graph: no history, position max_len, text padding skipped
+            st["n"].fill_(max_len)
+            st["skip"].copy_(torch.tensor([[v, max_len] for v in lens], dtype=torch.int32))
+            st["seen"].zero_()
+            fin = self._run_batch(st, graph, 0, max_len, int(top_k), early_stop_num, top_p, temperature, repetition_penalty,
+                                  kwargs.get("trace"))
+            return [st["hist"][b, :fin[b][0]].clone() for b in range(B)], [0] * B
         finally:
             self._active, self._memo_pack = None, False
             self.train(was_training)

@@ -1941,14 +1941,17 @@ def attn_decode_dev(cache, n_prev_dev, heads, row, skip=None):
     return out
 
 
-def sample_tokens(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, alpha, x_next, q=None):
-    """One fused sampling step over the rows of `logits` [B, >= V] (evk_sample_tokens; see include/evk.h for the buffers).
+def sample_tokens(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, alpha, x_next, q=None, eos_steps=1):
+    """One fused sampling step over the rows of `logits` [B, >= V] (evk_sample_tokens_ex; see include/evk.h for the buffers).
+    EOS is excluded at the steps idx < eos_steps (1: batched decoding with a prompt; 11: prompt-free decoding).
     Everything it reads or writes stays in device memory, so it can be part of a captured CUDA graph."""
     B, D = logits.shape[0], x_next.shape[-1]
+    if int(eos_steps) != eos_steps or eos_steps < 0:
+        raise ValueError(f"sample_tokens: eos_steps must be an integer >= 0, got {eos_steps!r}")
     assert logits.stride(-1) == 1 and hist.dtype == torch.int64 and seen.dtype == torch.int32 and fin.dtype == torch.int32
     assert icfg.dtype == torch.int64 and fcfg.dtype == torch.float32 and x_next.is_contiguous() and pe.is_contiguous()
     assert q is None or (q.shape[0] == B and q.stride(-1) == 1)
-    _call("evk_sample_tokens", _p(logits), logits.stride(0), B, V, eos, _p(icfg), _p(fcfg), _p(n_dev), _p(q),
+    _call("evk_sample_tokens_ex", _p(logits), logits.stride(0), B, V, eos, int(eos_steps), _p(icfg), _p(fcfg), _p(n_dev), _p(q),
           q.stride(0) if q is not None else 0, _p(hist), hist.stride(0), _p(seen), _p(fin), _p(emb), _p(pe), _p(alpha),
           _p(x_next), D)
 

@@ -216,7 +216,7 @@ int evk_reflect_pad_right(const float* x, int32_t T, float* y, int32_t Tp, int32
 int evk_transpose_bct_btc(const float* x, float* y, int32_t B, int32_t C, int32_t T, int32_t ld, int32_t to_btc,
                           evk_stream_t stream);
 /* embedding gather y[r][:] = table[idx[r / rep]][:]  (rep=2: models.py:924-927 nearest x2) and its
- * scatter-add gradient (rep must be 1) */
+ * scatter-add gradient (rep must be 1).  rows == 0 is a no-op (the pointers of an empty tensor may then be null). */
 int evk_embedding(const float* table, int32_t ldt, const int64_t* idx, int64_t rows, int32_t rep, float* y,
                   int32_t ldy, int32_t C, evk_stream_t stream);
 /* dtable[idx[r]][c] += dy[r][c] for the V-row table; every entry sums its rows in row order (reproducible). */
@@ -418,6 +418,12 @@ int evk_sample_tokens(const float* logits, int32_t ldl, int32_t B, int32_t V, in
                       const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist, int32_t ldh,
                       uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha, float* x_next,
                       int32_t D, evk_stream_t stream);
+/* The same with EOS excluded at every step idx < eos_steps (>= 0) instead of at step 0 only: evk_sample_tokens is this call with
+ * eos_steps = 1.  Prompt-free decoding (infer_panel_naive with prompts = None, t2s_model.py:835-836) passes 11 and prefix 0. */
+int evk_sample_tokens_ex(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, int32_t eos_steps,
+                         const int64_t* icfg, const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist,
+                         int32_t ldh, uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha,
+                         float* x_next, int32_t D, evk_stream_t stream);
 int evk_ce_fwd(const float* logits, int32_t ld, const int64_t* targets, int32_t rows, int32_t V, int32_t topk,
                int64_t ignore_index, float* lse, float* nll, uint8_t* flags, float* out2, evk_stream_t stream);
 int evk_ce_bwd(const float* logits, int32_t ld, const int64_t* targets, const float* lse, const float* gscale,

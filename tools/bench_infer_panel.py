@@ -6,6 +6,8 @@ One JSON line.   python tools/bench_infer_panel.py > gpurun_out/bench_infer_pane
 # --batch: instead, the same single-utterance number next to infer_panel_batch_infer for B in {1, 4, 16} sentences (each with the
 # same 120 phonemes / 150-token prompt / 300 tokens), as aggregate semantic tokens/s and ms per decoding step, with the card's
 # name and power limit read in the same run.  --profile DIR (with --batch): also a torch.profiler trace of one B = 16 call.
+# --ref-free: prompt-free decoding (TTS's ref_text_free mode), infer_panel_naive(prompts=None) on one utterance next to
+# infer_panel_naive_batched(prompts=None) for B in {1, 4, 16}, same 120 phonemes / 300 tokens / top_k 15, card name and power limit.
 import json
 import math
 import os
@@ -35,11 +37,52 @@ bert = torch.randn(1, 1024, X, generator=g)
 prompts = torch.randint(0, 1024, (1, Yp), generator=g)
 xd, bd, pd, xl = x.to(dev), bert.to(dev), prompts.to(dev), torch.tensor([X], device=dev)
 BATCH = "--batch" in sys.argv
+REF_FREE = "--ref-free" in sys.argv
+
+
+def card_name():
+    import subprocess
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True).stdout.strip().splitlines()
+    return card[0] if card else "unknown"
+
+
+def bench_ref_free():
+    """infer_panel_naive(prompts=None) on one utterance and infer_panel_naive_batched(prompts=None) for B in {1, 4, 16}: generated
+    tokens / wall time of one call (prompt pass included)."""
+    net.infer_panel_naive(xd, xl, None, bd, top_k=15, top_p=1, early_stop_num=8, temperature=1.0)              # warm-up
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    y, _ = net.infer_panel_naive(xd, xl, None, bd, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)
+    torch.cuda.synchronize()
+    s = time.perf_counter() - t0
+    single = dict(tokens_per_s=y.shape[1] / s, ms_per_token=s / max(y.shape[1], 1) * 1e3, generated=int(y.shape[1]))
+    out = {}
+    for B in (1, 4, 16):
+        xs, bs, lens = [xd[0]] * B, [bd[0]] * B, torch.full((B,), X)
+        net.infer_panel_naive_batched(xs, lens, None, bs, top_k=15, top_p=1, early_stop_num=8, temperature=1.0)   # warm-up, capture
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        ys, _ = net.infer_panel_naive_batched(xs, lens, None, bs, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)
+        torch.cuda.synchronize()
+        s = time.perf_counter() - t0
+        gen = [int(t.shape[0]) for t in ys]
+        steps = max(gen) + 1
+        out[str(B)] = dict(tokens_per_s=sum(gen) / s, ms_per_step=s / steps * 1e3, generated=sum(gen), steps=steps, seconds=s)
+    return single, out
+
+
+if REF_FREE:
+    single, batch = bench_ref_free()
+    print(json.dumps(dict(metric="Text2SemanticDecoder.infer_panel_naive_batched(prompts=None) (prompt-free batched KV-cache AR decoding)",
+                          unit="semantic-tokens/s", card=card_name(), single_utterance=single, batch=batch,
+                          config=dict(layers=24, X=X, prompt=0, early_stop_num=NEW, top_k=15, top_p=1, temperature=1.0),
+                          note="aggregate generated tokens over wall time of one call, prompt pass included; 25 tokens = 1 s of audio")))
+    sys.exit(0)
 
 
 def bench_batch():
     """infer_panel_batch_infer for B in {1, 4, 16}: aggregate generated tokens / wall time (prompt pass included)."""
-    import subprocess
     out = {}
     for B in (1, 4, 16):
         xs, bs, ps = [xd[0]] * B, [bd[0]] * B, pd.expand(B, -1)
@@ -64,9 +107,7 @@ def bench_batch():
         prof.export_chrome_trace(os.path.join(d, "infer_batch_b16.pt.trace.json"))
         with open(os.path.join(d, "infer_batch_b16_kernels.txt"), "w") as f:
             f.write(prof.key_averages().table(sort_by="cuda_time_total", row_limit=30))
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                          text=True).stdout.strip().splitlines()
-    return out, card[0] if card else "unknown"
+    return out, card_name()
 
 
 net.infer_panel(xd, xl, pd, bd, top_k=15, top_p=1, early_stop_num=8, temperature=1.0)     # warm-up (packs the weights once)
