@@ -1543,6 +1543,21 @@ def attention(q, k, v, *, heads, scale, Ek=None, Ev=None, window=None, fill=-1e4
     return _AttnFn.apply(q, k, v, Ek, Ev, cfg)
 
 
+def attention_pad(qkv, *, heads, lens, scale):
+    """Fused bidirectional attention, head dim 64, inference only (evk_attn_pad_fwd): qkv [B, L, >= 3*heads*64] holds q | k | v
+    column blocks (one packed QKV Linear output); lens int64 device [B] with 1 <= lens[b] <= L (key j is visible iff
+    j < lens[b]) -> [B, L, heads*64]."""
+    qkv = _c(qkv.detach())
+    B, T, ld = qkv.shape
+    D = heads * 64
+    assert ld >= 3 * D and lens.dtype == torch.int64 and lens.is_cuda and lens.numel() == B, (qkv.shape, heads, lens.dtype)
+    o = torch.empty((B, T, D), device=qkv.device, dtype=torch.float32)
+    base = qkv.data_ptr()
+    _call_f("evk_attn_pad_fwd", 4.0 * B * heads * T * T * 64, ctypes.c_void_p(base), ctypes.c_void_p(base + 4 * D),
+            ctypes.c_void_p(base + 8 * D), ld, _p(o), D, B, heads, T, _p(lens.contiguous()), ctypes.c_float(scale))
+    return o
+
+
 # ------------------------------------------------------------------------------------------------
 # VQ, losses, mel
 # ------------------------------------------------------------------------------------------------

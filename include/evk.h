@@ -447,6 +447,20 @@ int evk_scaled_adam(float* p, float* g, float* delta, float* v, const int64_t* c
                     float param_min_rms, float param_max_rms, float scalar_max, int32_t size_update_period,
                     int32_t zero_grad, evk_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * BERT text features (Normalize._get_bert_feature, normalize.py:88-106; TextPreprocessor.get_bert_feature,
+ * inference/preprocessor.py:180-193).  Linear layers / LayerNorm / GELU / embedding reuse the entry points above.
+ * ------------------------------------------------------------------------------------------ */
+/* Fused bidirectional attention with per-row key lengths, head dim 64, inference only:
+ *   O = softmax(Q K^T * scale + mask) V   per (batch b, head h),   mask: key j is visible to every query iff j < lens[b].
+ * q/k/v: [B, L, ld] with head h at columns h*64.. (usually the three column blocks of one packed QKV Linear output);
+ * o: [B, L, ldo].  Requires 1 <= lens[b] <= L <= 512 (lens: int64 device [B], values outside are clamped to [1, L]),
+ * ld % 4 == 0, ldo % 2 == 0, q/k/v 16-byte and o 8-byte aligned.  Query rows at or past lens[b] are computed like any
+ * other (finite).  Scores are never materialised (online softmax); TF32 mma.sync with fp32 accumulation (3xTF32 under
+ * evk_set_precise(1)); no atomics, bit-reproducible. */
+int evk_attn_pad_fwd(const float* q, const float* k, const float* v, int32_t ld, float* o, int32_t ldo, int32_t B,
+                     int32_t H, int32_t L, const int64_t* lens, float scale, evk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
