@@ -2052,3 +2052,81 @@ def gemm_tf32(a, b, out=None, bias=None, res=None, act=ACT_NONE, slope=0.0, spli
     _call_f("evk_gemm_tf32", 2.0 * M * N * K, _p(a), a.stride(0), _p(b), b.stride(0), _p(out), out.stride(0), M, N, K, _p(bias),
             _p(res), res.stride(0) if res is not None else 0, act, ctypes.c_float(slope), splits)
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# 2-D convolution family (UVR5 VR separator, uvr5.py): channels-last [B, H, W, pitch] operands
+# ------------------------------------------------------------------------------------------------
+C2_NONE, C2_RELU, C2_LRELU, C2_SIGMOID = 0, 1, 2, 3
+
+
+class CLView:
+    """Rows r0 .. r0+H and channels c0 .. c0+C of a contiguous channels-last fp32 CUDA buffer [B, Hs, W, pitch]: a layer
+    reads or writes a slice of a concat buffer in place."""
+    __slots__ = ("buf", "c0", "C", "r0", "H")
+
+    def __init__(self, buf, c0=0, C=None, r0=0, H=None):
+        assert buf.dim() == 4 and buf.is_contiguous() and buf.dtype == torch.float32 and buf.is_cuda, (buf.shape, buf.dtype)
+        self.buf, self.c0, self.r0 = buf, c0, r0
+        self.C = buf.shape[3] - c0 if C is None else C
+        self.H = buf.shape[1] - r0 if H is None else H
+        assert 0 <= c0 and c0 + self.C <= buf.shape[3] and 0 <= r0 and r0 + self.H <= buf.shape[1], (buf.shape, c0, C, r0, H)
+
+    @property
+    def B(self):
+        return self.buf.shape[0]
+
+    @property
+    def W(self):
+        return self.buf.shape[2]
+
+    def args(self):
+        """-> (pointer to channel c0 of pixel (0, r0, 0), pixel pitch, batch stride) in the library's argument order"""
+        pitch = self.buf.shape[3]
+        return (ctypes.c_void_p(self.buf.data_ptr() + 4 * (self.r0 * self.W * pitch + self.c0)), pitch,
+                self.buf.stride(0))
+
+
+def conv2d_out(n, k, stride, pad, dil):
+    return (n + 2 * pad - dil * (k - 1) - 1) // stride + 1
+
+
+def conv2d(x: CLView, w, y: CLView, *, k, stride=1, pad=0, dil=1, scale=None, bias=None, act=C2_NONE):
+    """y = act(conv2d(x) * scale + bias) (evk_conv2d_fwd): w [N, k, k, C] fp32 contiguous; y must be [B, Ho, Wo, N]."""
+    N = w.shape[0]
+    assert w.is_contiguous() and tuple(w.shape) == (N, k, k, x.C) and y.C == N and y.B == x.B, (w.shape, x.C, y.C)
+    Ho, Wo = conv2d_out(x.H, k, stride, pad, dil), conv2d_out(x.W, k, stride, pad, dil)
+    assert (y.H, y.W) == (Ho, Wo), ((y.H, y.W), (Ho, Wo))
+    _call_f("evk_conv2d_fwd", 2.0 * x.B * Ho * Wo * N * k * k * x.C, *x.args(), _p(w), _p(scale), _p(bias), *y.args(),
+            x.B, x.H, x.W, x.C, N, k, stride, pad, dil, act)
+
+
+def dwconv3x3(x: CLView, w, y: CLView, dil):
+    """depthwise 3x3, stride 1, padding = dil (evk_dwconv3x3_fwd): w [C, 9]"""
+    assert w.is_contiguous() and tuple(w.shape) == (x.C, 9) and (y.B, y.H, y.W, y.C) == (x.B, x.H, x.W, x.C)
+    _call("evk_dwconv3x3_fwd", *x.args(), _p(w), *y.args(), x.B, x.H, x.W, x.C, dil)
+
+
+def resize_bilinear_ac(x: CLView, y: CLView):
+    """F.interpolate(mode="bilinear", align_corners=True) from x's extent to y's (evk_resize_bilinear_ac)"""
+    assert y.B == x.B and y.C == x.C
+    _call("evk_resize_bilinear_ac", *x.args(), x.H, x.W, *y.args(), y.H, y.W, x.B, x.C)
+
+
+def mean_h(x: CLView):
+    """-> [B, 1, W, C] mean over rows (evk_mean_h)"""
+    y = torch.empty((x.B, 1, x.W, x.C), device=x.buf.device, dtype=torch.float32)
+    _call("evk_mean_h", *x.args(), _p(y), x.B, x.H, x.W, x.C)
+    return y
+
+
+def vr_mask_head(h: CLView, w, mix, offset, split_bin=0, e_lo=1.0, e_hi=1.0, use_agg=False):
+    """CascadedASPPNet's mask head (evk_vr_mask_head): h [B, max_bin, W, Ch], w [2, Ch], mix NCHW [B, 2, out_bin, W]
+    -> [B, 2, out_bin, W - 2 offset]"""
+    B, two, out_bin, W = mix.shape
+    assert two == 2 and mix.is_contiguous() and mix.dtype == torch.float32 and h.B == B and h.W == W, (mix.shape, h.B, h.W)
+    assert w.is_contiguous() and tuple(w.shape) == (2, h.C)
+    out = torch.empty((B, 2, out_bin, W - 2 * offset), device=mix.device, dtype=torch.float32)
+    _call("evk_vr_mask_head", *h.args(), _p(w), h.C, _p(mix), _p(out), B, h.H, out_bin, W, offset, split_bin,
+          ctypes.c_float(e_lo), ctypes.c_float(e_hi), 1 if use_agg else 0)
+    return out

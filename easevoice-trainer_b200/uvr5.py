@@ -1,0 +1,340 @@
+"""UVR5 VR vocal separation on the library's kernels: the CascadedASPPNet of the HP2 / HP3 / HP5 models
+(lib_v5/vr_network/nets.py, layers.py) and a batched drop-in for SeparateVR.inference (uvr5/separate.py:198-273).
+
+The reference runs the net on one 512-frame window per call, copying each result to the host before the next.  Here every
+window of a file, TTA windows included, goes through the net in batches of `max_windows`, and the result reaches the host
+once.  Activations are channels-last fp32; a layer writes straight into its slice of the next concat buffer:
+  * Encoder i's conv1 (the skip) writes channels [2 C_i, 3 C_i) of Decoder i's input, the x2 upsample of the layer below
+    writes channels [0, 2 C_i);
+  * the five (seven with `enlarge`) ASPP branches write slices of the bottleneck's input;
+  * the input x, aux1 (the two band nets, each on its half of the rows) and aux2 are slices of one [B, max_bin, W, 2 + ...]
+    buffer, so cat([x, aux1]) and cat([x, aux1, aux2]) are never built.
+Eval BatchNorm is folded into a per-channel scale and bias of the preceding convolution at load; Dropout is the identity.
+The librosa front and back ends (resampling, per-band STFT / iSTFT, combine_spectrograms, mirroring) stay with the caller.
+"""
+import numpy as np
+import torch
+
+from . import ops
+from .ops import CLView
+
+# get_nets_model(n_fft, size) parameter sets (nets.py:125-206): band-net width, bridge 2 (nin, nout), full-band net 2
+# width, bridge 3, full-band net 3 width, and whether the ASPP modules carry the two extra dilation-16 branches.
+SIZES = {
+    61968: dict(ch1=32, bridge2=(34, 16), ch2=32, bridge3=(66, 32), ch3=64, enlarge=False),
+    123812: dict(ch1=32, bridge2=(34, 16), ch2=32, bridge3=(66, 32), ch3=64, enlarge=False),
+    123821: dict(ch1=32, bridge2=(34, 16), ch2=32, bridge3=(66, 32), ch3=64, enlarge=False),
+    33966: dict(ch1=16, bridge2=(18, 8), ch2=16, bridge3=(34, 16), ch3=32, enlarge=True),
+    16983: dict(ch1=16, bridge2=(18, 8), ch2=16, bridge3=(34, 16), ch3=32, enlarge=False),
+    537227: dict(ch1=64, bridge2=(66, 32), ch2=64, bridge3=(130, 64), ch3=128, enlarge=True),
+    537238: dict(ch1=64, bridge2=(66, 32), ch2=64, bridge3=(130, 64), ch3=128, enlarge=True),
+}
+DILATIONS = (4, 8, 16)
+BN_EPS = 1e-5
+
+
+def _cbr_keys(spec, p, nin, nout, k):
+    spec[p] = ("cbr", (nout, nin, k, k))
+
+
+def _base_keys(spec, p, nin, ch, enlarge):
+    for i, (a, b) in enumerate([(nin, ch), (ch, 2 * ch), (2 * ch, 4 * ch), (4 * ch, 8 * ch)], 1):
+        _cbr_keys(spec, f"{p}.enc{i}.conv1", a, b, 3)
+        _cbr_keys(spec, f"{p}.enc{i}.conv2", b, b, 3)
+    c = 8 * ch
+    _cbr_keys(spec, f"{p}.aspp.conv1.1", c, c, 1)
+    _cbr_keys(spec, f"{p}.aspp.conv2", c, c, 1)
+    for i in range(3, 8 if enlarge else 6):
+        spec[f"{p}.aspp.conv{i}"] = ("sep", (c, c))
+    _cbr_keys(spec, f"{p}.aspp.bottleneck.0", c * (7 if enlarge else 5), 16 * ch, 1)
+    for i, (a, b) in zip((4, 3, 2, 1), [(24 * ch, 8 * ch), (12 * ch, 4 * ch), (6 * ch, 2 * ch), (3 * ch, ch)]):
+        _cbr_keys(spec, f"{p}.dec{i}.conv", a, b, 3)
+
+
+def layer_spec(size):
+    """-> {module prefix: (kind, shape)}: "cbr" = Conv2d (no bias) + BatchNorm2d, "sep" = depthwise 3x3 + 1x1 + BatchNorm2d
+    (shape (nin, nout)), "conv" = a bias-free 1x1 Conv2d"""
+    s = SIZES[size]
+    spec = {}
+    _base_keys(spec, "stg1_low_band_net", 2, s["ch1"], s["enlarge"])
+    _base_keys(spec, "stg1_high_band_net", 2, s["ch1"], s["enlarge"])
+    _cbr_keys(spec, "stg2_bridge", *s["bridge2"], 1)
+    _base_keys(spec, "stg2_full_band_net", s["bridge2"][1], s["ch2"], s["enlarge"])
+    _cbr_keys(spec, "stg3_bridge", *s["bridge3"], 1)
+    _base_keys(spec, "stg3_full_band_net", s["bridge3"][1], s["ch3"], s["enlarge"])
+    spec["out"] = ("conv", (2, s["ch3"], 1, 1))
+    spec["aux1_out"] = ("conv", (2, s["ch1"], 1, 1))
+    spec["aux2_out"] = ("conv", (2, s["ch2"], 1, 1))
+    return spec
+
+
+def state_dict_shapes(size):
+    """-> {state_dict key: shape} of the reference's get_nets_model(n_fft, size), num_batches_tracked left out"""
+    out = {}
+    for p, (kind, shape) in layer_spec(size).items():
+        if kind == "conv":
+            out[p + ".weight"] = shape
+            continue
+        if kind == "cbr":
+            out[p + ".conv.0.weight"] = shape
+            bn, n = p + ".conv.1", shape[0]
+        else:
+            nin, n = shape
+            out[p + ".conv.0.weight"] = (nin, 1, 3, 3)
+            out[p + ".conv.1.weight"] = (n, nin, 1, 1)
+            bn = p + ".conv.2"
+        for k in ("weight", "bias", "running_mean", "running_var"):
+            out[f"{bn}.{k}"] = (n,)
+    return out
+
+
+def _fold_bn(sd, bn):
+    """eval BatchNorm2d -> (scale, bias) with y = x * scale + bias, folded in float64"""
+    var, mean = sd[bn + ".running_var"].double(), sd[bn + ".running_mean"].double()
+    scale = sd[bn + ".weight"].double() / torch.sqrt(var + BN_EPS)
+    return scale.float(), (sd[bn + ".bias"].double() - mean * scale).float()
+
+
+def _cl_weight(w):
+    """[N, C, k, k] -> [N, k, k, C] fp32 (the implicit GEMM's tap-major, channel-minor K order)"""
+    return w.float().permute(0, 2, 3, 1).contiguous()
+
+
+class CascadedASPPNet:
+    """nets.CascadedASPPNet(n_fft, params) in eval mode on CUDA.  Input [B, 2, n_fft // 2 + 1, W] magnitudes (fp32)."""
+
+    def __init__(self, n_fft, size=61968):
+        if size not in SIZES:
+            raise ValueError(f"unknown VR net size {size}; known: {sorted(SIZES)}")
+        self.size, self.cfg = size, SIZES[size]
+        self.max_bin = n_fft // 2
+        self.output_bin = n_fft // 2 + 1
+        self.offset = 128
+        self.device = torch.device("cpu")
+        self.layers = None
+
+    # ---- weights -----------------------------------------------------------------------------------------
+    def load_state_dict(self, sd):
+        """Reference state_dict (fp16 or fp32 storage) -> folded, channels-last fp32 layers on self.device.  Keys ending in
+        num_batches_tracked are ignored; any other missing or unexpected key, or a wrong shape, raises ValueError."""
+        sd = {k: v for k, v in sd.items() if not k.endswith("num_batches_tracked")}
+        want = state_dict_shapes(self.size)
+        missing, unexpected = sorted(set(want) - set(sd)), sorted(set(sd) - set(want))
+        if missing or unexpected:
+            raise ValueError(f"state_dict does not match size {self.size}: missing {missing[:4]}, unexpected {unexpected[:4]}")
+        bad = [k for k, s in want.items() if tuple(sd[k].shape) != tuple(s)]
+        if bad:
+            raise ValueError(f"state_dict shapes do not match size {self.size}: {[(k, tuple(sd[k].shape)) for k in bad[:4]]}")
+        layers = {}
+        for p, (kind, shape) in layer_spec(self.size).items():
+            if kind == "conv":
+                layers[p] = dict(w=sd[p + ".weight"].float().reshape(shape[0], shape[1]).contiguous())
+            elif kind == "cbr":
+                scale, bias = _fold_bn(sd, p + ".conv.1")
+                layers[p] = dict(w=_cl_weight(sd[p + ".conv.0.weight"]), scale=scale, bias=bias, k=shape[-1])
+            else:
+                scale, bias = _fold_bn(sd, p + ".conv.2")
+                layers[p] = dict(dw=sd[p + ".conv.0.weight"].float().reshape(shape[0], 9).contiguous(),
+                                 w=_cl_weight(sd[p + ".conv.1.weight"]), scale=scale, bias=bias, k=1)
+        self.layers = {p: {k: (v.to(self.device) if torch.is_tensor(v) else v) for k, v in L.items()}
+                       for p, L in layers.items()}
+        return self
+
+    def to(self, device):
+        self.device = torch.device(device)
+        if self.layers is not None:
+            self.layers = {p: {k: (v.to(self.device) if torch.is_tensor(v) else v) for k, v in L.items()}
+                           for p, L in self.layers.items()}
+        return self
+
+    def eval(self):
+        return self
+
+    @classmethod
+    def from_pretrained(cls, path, n_fft=1344, device="cuda"):
+        """Load a VR-net .pth (HP2 / HP3 / HP5 ...): the parameter set is read from the weight shapes (band-net width from
+        enc1, `enlarge` from the presence of aspp.conv6 / conv7).  Weights that match no get_nets_model set raise
+        ValueError."""
+        sd = torch.load(path, map_location="cpu", weights_only=True)
+        return cls(n_fft, infer_size(sd)).to(device).load_state_dict(sd)
+
+    # ---- forward -----------------------------------------------------------------------------------------
+    def check_input(self, x, crop):
+        if not (torch.is_tensor(x) and x.dim() == 4 and x.shape[1] == 2 and x.shape[2] == self.output_bin):
+            raise ValueError(f"expected [B, 2, {self.output_bin}, W] magnitudes, got "
+                             f"{tuple(x.shape) if torch.is_tensor(x) else type(x)}")
+        self.check_shape(x.shape[3], crop)
+        if self.layers is None:
+            raise ValueError("no weights loaded")
+        if not x.is_cuda or self.device.type != "cuda":
+            raise ValueError("the VR net runs on CUDA tensors and weights only")
+
+    def check_shape(self, W, crop):
+        """The shapes the net takes: both band heights and W multiples of 16 (four stride-2 encoders, then x2 upsamples
+        that must meet their skips), and W > 2 * offset when cropped.  The reference fails inside torch.cat or asserts."""
+        if self.max_bin % 2 or (self.max_bin // 2) % 16:
+            raise ValueError(f"band height {self.max_bin // 2} (n_fft // 4) must be a multiple of 16 and n_fft // 2 even")
+        if W % 16:
+            raise ValueError(f"frame count {W} must be a multiple of 16")
+        if crop and W <= 2 * self.offset:
+            raise ValueError(f"frame count {W} must exceed 2 * offset = {2 * self.offset}")
+
+    def forward(self, x, aggressiveness=None):
+        """mask * x over all W frames: [B, 2, output_bin, W] (CascadedASPPNet.forward in eval mode)"""
+        self.check_input(x, crop=False)
+        return self._run(x, aggressiveness, 0)
+
+    __call__ = forward
+
+    def predict(self, x_mag, aggressiveness=None):
+        """forward cropped by `offset` frames on both time edges: [B, 2, output_bin, W - 256]"""
+        self.check_input(x_mag, crop=True)
+        return self._run(x_mag, aggressiveness, self.offset)
+
+    def _conv(self, p, x, y, stride=1, act=ops.C2_RELU, dil=1):
+        L = self.layers[p]
+        k = L["k"]
+        ops.conv2d(x, L["w"], y, k=k, stride=stride, pad=dil * (k // 2), dil=dil, scale=L["scale"], bias=L["bias"], act=act)
+
+    def _empty(self, B, H, W, C):
+        return torch.empty((B, H, W, C), device=self.device, dtype=torch.float32)
+
+    def _aspp(self, p, x, enlarge):
+        B, H, W, c = x.B, x.H, x.W, x.C
+        nb = 7 if enlarge else 5
+        A = self._empty(B, H, W, nb * c)
+        pooled = self._empty(B, 1, W, c)
+        self._conv(p + ".conv1.1", CLView(ops.mean_h(x)), CLView(pooled))
+        ops.resize_bilinear_ac(CLView(pooled), CLView(A, 0, c))
+        self._conv(p + ".conv2", x, CLView(A, c, c))
+        dw = self._empty(B, H, W, c)
+        dils = DILATIONS + ((DILATIONS[2],) * 2 if enlarge else ())
+        for j, d in enumerate(dils):
+            name = f"{p}.conv{3 + j}"
+            ops.dwconv3x3(x, self.layers[name]["dw"], CLView(dw), d)
+            self._conv(name, CLView(dw), CLView(A, (2 + j) * c, c))
+        out = self._empty(B, H, W, self.layers[p + ".bottleneck.0"]["w"].shape[0])
+        self._conv(p + ".bottleneck.0", CLView(A), CLView(out))
+        return out
+
+    def _base(self, p, x: CLView, out: CLView):
+        """BaseASPPNet: x [B, H, W, nin] -> out [B, H, W, ch] (H, W multiples of 16)"""
+        B, H, W = x.B, x.H, x.W
+        ch = self.layers[p + ".enc1.conv1"]["w"].shape[0]
+        dec_in, h = [], x
+        for i in range(4):
+            Ci, Hi, Wi = ch << i, H >> i, W >> i
+            D = self._empty(B, Hi, Wi, 3 * Ci)                    # [upsampled (2 Ci) | skip (Ci)]
+            skip = CLView(D, 2 * Ci, Ci)
+            self._conv(f"{p}.enc{i + 1}.conv1", h, skip, act=ops.C2_LRELU)
+            nxt = self._empty(B, Hi // 2, Wi // 2, Ci)
+            self._conv(f"{p}.enc{i + 1}.conv2", skip, CLView(nxt), stride=2, act=ops.C2_LRELU)
+            dec_in.append(D)
+            h = CLView(nxt)
+        h = CLView(self._aspp(p + ".aspp", h, self.cfg["enlarge"]))
+        for i in range(3, -1, -1):
+            D = dec_in[i]
+            ops.resize_bilinear_ac(h, CLView(D, 0, 2 * (ch << i)))
+            y = out if i == 0 else CLView(self._empty(B, H >> i, W >> i, ch << i))
+            self._conv(f"{p}.dec{i + 1}.conv", CLView(D), y)
+            h = y
+
+    def _run(self, x, aggressiveness, offset):
+        x = x.detach().float().contiguous()
+        B, _, _, W = x.shape
+        mb, bw = self.max_bin, self.max_bin // 2
+        c1, c2 = self.cfg["ch1"], self.cfg["ch2"]
+        # [x | aux1 | aux2] over all max_bin rows; the band nets read and write their own halves of the rows
+        cat3 = self._empty(B, mb, W, 2 + c1 + c2)
+        cat3[..., :2].copy_(x[:, :, :mb].permute(0, 2, 3, 1))
+        for name, r0 in (("stg1_low_band_net", 0), ("stg1_high_band_net", bw)):
+            self._base(name, CLView(cat3, 0, 2, r0, bw), CLView(cat3, 2, c1, r0, bw))
+        br2 = self._empty(B, mb, W, self.cfg["bridge2"][1])
+        self._conv("stg2_bridge", CLView(cat3, 0, 2 + c1), CLView(br2))
+        self._base("stg2_full_band_net", CLView(br2), CLView(cat3, 2 + c1, c2))
+        br3 = self._empty(B, mb, W, self.cfg["bridge3"][1])
+        self._conv("stg3_bridge", CLView(cat3), CLView(br3))
+        del cat3, br2
+        h = self._empty(B, mb, W, self.cfg["ch3"])
+        self._base("stg3_full_band_net", CLView(br3), CLView(h))
+        del br3
+        if aggressiveness:
+            v = aggressiveness["value"]
+            sb = int(aggressiveness["split_bin"])
+            sb = max(0, self.output_bin + sb) if sb < 0 else min(sb, self.output_bin)   # python slice bounds
+            return ops.vr_mask_head(CLView(h), self.layers["out"]["w"], x, offset, sb, 1 + v / 3, 1 + v, True)
+        return ops.vr_mask_head(CLView(h), self.layers["out"]["w"], x, offset)
+
+
+def infer_size(sd):
+    """-> the get_nets_model size whose layers match the shapes of state_dict sd; ValueError if none does"""
+    key = "stg1_low_band_net.enc1.conv1.conv.0.weight"
+    if key not in sd:
+        raise ValueError(f"not a VR CascadedASPPNet state_dict: no {key}")
+    ch = sd[key].shape[0]
+    enlarge = "stg1_low_band_net.aspp.conv6.conv.0.weight" in sd
+    for size, s in SIZES.items():
+        if s["ch1"] == ch and s["enlarge"] == enlarge:
+            want = state_dict_shapes(size)
+            have = {k: tuple(v.shape) for k, v in sd.items() if not k.endswith("num_batches_tracked")}
+            if have == {k: tuple(v) for k, v in want.items()}:
+                return size
+    raise ValueError(f"state_dict (band width {ch}, enlarge={enlarge}) matches no get_nets_model parameter set")
+
+
+def get_nets_model(n_fft, size=61968):
+    """nets.get_nets_model: an unloaded CascadedASPPNet (call load_state_dict, then .to("cuda"))"""
+    return CascadedASPPNet(n_fft, size)
+
+
+def make_padding(width, crop_size, offset):
+    """SeparateVR.make_padding -> (left, right, roi_size)"""
+    left = offset
+    roi_size = crop_size - left * 2
+    if roi_size == 0:
+        roi_size = crop_size
+    return left, roi_size - (width % roi_size) + left, roi_size
+
+
+def _windows(x_pre, pad_l, pad_r, roi, ws, n_window):
+    """[n_window, 2, bins, ws] windows of the zero-padded magnitudes, start i * roi (the reference's slices)"""
+    xp = torch.nn.functional.pad(x_pre, (pad_l, pad_r))
+    return xp.unfold(2, ws, roi)[:, :, :n_window].permute(2, 0, 1, 3)
+
+
+def inference(x_spec, device, model, aggressiveness, data, max_windows=16):
+    """SeparateVR.inference(x_spec, device, model, aggressiveness, data) with every window (and TTA window) of the file in
+    batches of max_windows: -> numpy (pred * coef, |x_spec|, exp(1j * angle(x_spec))).  |x|, the phase and coef are the
+    reference's numpy computations; an all-zero spectrum gives coef = 0 and, as in the reference, a NaN pred (0 / 0)."""
+    if max_windows < 1:
+        raise ValueError("max_windows must be >= 1")
+    ws = data["window_size"]
+    if x_spec.ndim != 3 or x_spec.shape[:2] != (2, model.output_bin):
+        raise ValueError(f"expected a [2, {model.output_bin}, n_frame] spectrogram, got {x_spec.shape}")
+    model.check_shape(ws, crop=True)
+    x_mag = np.abs(x_spec)
+    coef = x_mag.max()
+    x_mag_pre = x_mag / coef
+    n_frame = x_mag_pre.shape[2]
+    pad_l, pad_r, roi = make_padding(n_frame, ws, model.offset)
+    n_window = int(np.ceil(n_frame / roi))
+    dev = torch.device(device)
+    x_pre = torch.from_numpy(np.ascontiguousarray(x_mag_pre, dtype=np.float32)).to(dev)
+    wins = [_windows(x_pre, pad_l, pad_r, roi, ws, n_window)]
+    if data["tta"]:
+        wins.append(_windows(x_pre, pad_l + roi // 2, pad_r + roi // 2, roi, ws, n_window + 1))
+    wins = torch.cat(wins, 0)
+    outs = [model.predict(wins[i:i + max_windows].contiguous(), aggressiveness) for i in range(0, wins.shape[0], max_windows)]
+    out = torch.cat(outs, 0)                               # [n_windows (+ n_window + 1), 2, bins, roi], still running
+    phase = np.exp(1.0j * np.angle(x_spec))                # host work while the device runs the net
+    out = out.cpu().numpy()                                # the one copy to the host
+    bins = out.shape[2]
+
+    def join(o):
+        return o.transpose(1, 2, 0, 3).reshape(2, bins, -1)
+
+    pred = join(out[:n_window])[:, :, :n_frame]
+    if data["tta"]:
+        pred_tta = join(out[n_window:])[:, :, roi // 2:][:, :, :n_frame]
+        return (pred + pred_tta) * 0.5 * coef, x_mag, phase
+    return pred * coef, x_mag, phase

@@ -461,6 +461,41 @@ int evk_scaled_adam(float* p, float* g, float* delta, float* v, const int64_t* c
 int evk_attn_pad_fwd(const float* q, const float* k, const float* v, int32_t ld, float* o, int32_t ldo, int32_t B,
                      int32_t H, int32_t L, const int64_t* lens, float scale, evk_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * UVR5 VR vocal separation (CascadedASPPNet, uvr5.py), inference only.  Activations are channels-last fp32: pixel (b, y, x)
+ * of an operand starts at  p + b*bs + (y*W + x)*pitch  (floats), so a channel slice of a concat buffer is an operand.
+ * ------------------------------------------------------------------------------------------ */
+enum evk_conv2d_act { EVK_C2_NONE = 0, EVK_C2_RELU = 1, EVK_C2_LRELU = 2 /* slope 0.01 */, EVK_C2_SIGMOID = 3 };
+/* y = act(conv2d(x, w) * scale[n] + bias[n])  (scale / bias may be null: 1 / 0).  x: [B, H, W, C] (pitch x_pitch >= C,
+ * batch stride x_bs); w: [N][k][k][C] (k = 1 or 3); stride 1 or 2, zero padding pad, dilation dil >= 1; y: [B, Ho, Wo, N]
+ * (pitch y_pitch >= N, batch stride y_bs), Ho = (H + 2 pad - dil (k - 1) - 1) / stride + 1.  Implicit GEMM with TF32
+ * products and fp32 accumulation: wgmma when C, x_pitch and x_bs are multiples of 4 and x, w are 16-byte aligned,
+ * mma.sync otherwise and for 3xTF32 under evk_set_precise(1).  No atomics, and every output's sum has one order whatever
+ * B is, so results are bit-reproducible and independent of the batch. */
+int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale, const float* bias,
+                   float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W, int32_t C, int32_t N, int32_t k,
+                   int32_t stride, int32_t pad, int32_t dil, int32_t act, evk_stream_t stream);
+/* Depthwise 3x3, stride 1, zero padding = dil: y[b,y,x,c] = sum_{i,j} w[c][i][j] x[b, y + (i-1) dil, x + (j-1) dil, c]
+ * (fp32 FMA).  w: [C][3][3]. */
+int evk_dwconv3x3_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, float* y, int32_t y_pitch,
+                      int64_t y_bs, int32_t B, int32_t H, int32_t W, int32_t C, int32_t dil, evk_stream_t stream);
+/* Bilinear resize [B, Hi, Wi, C] -> [B, Ho, Wo, C] with align_corners=True (F.interpolate's index and weight rules; an
+ * input extent of 1 broadcasts). */
+int evk_resize_bilinear_ac(const float* x, int32_t x_pitch, int64_t x_bs, int32_t Hi, int32_t Wi, float* y,
+                           int32_t y_pitch, int64_t y_bs, int32_t Ho, int32_t Wo, int32_t B, int32_t C,
+                           evk_stream_t stream);
+/* y[b][x][c] = mean_y x[b, y, x, c]  (AdaptiveAvgPool2d((1, None))); y: contiguous [B, 1, W, C]. */
+int evk_mean_h(const float* x, int32_t x_pitch, int64_t x_bs, float* y, int32_t B, int32_t H, int32_t W, int32_t C,
+               evk_stream_t stream);
+/* Mask head of CascadedASPPNet.predict (nets.py:60-122): h [B, max_bin, W, Ch] (pitch / batch stride), w [2][Ch] (the
+ * bias-free 1x1 output conv), mix NCHW [B, 2, out_bin, W] ->
+ *   out[b, c, r, x - offset] = mask(c, min(r, max_bin - 1), x)^e(r) * mix[b, c, r, x]   for offset <= x < W - offset,
+ * mask = sigmoid(w[c] . h), e(r) = e_lo for r < split_bin, e_hi otherwise, and 1 when use_agg == 0.
+ * out: contiguous [B, 2, out_bin, W - 2 offset]. */
+int evk_vr_mask_head(const float* h, int32_t h_pitch, int64_t h_bs, const float* w, int32_t Ch, const float* mix,
+                     float* out, int32_t B, int32_t max_bin, int32_t out_bin, int32_t W, int32_t offset, int32_t split_bin,
+                     float e_lo, float e_hi, int32_t use_agg, evk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
