@@ -286,14 +286,16 @@ __global__ void sadam_update_kernel(float* __restrict__ p, float* __restrict__ g
 }
 
 // ---- KV-cache attention of one new token (T2SBlock.decode_next_token, t2s_model.py:203-221) --------------------------------
-// Cache rows are the in_proj outputs [q | k | v] (3 * H * 32 floats, row pitch ld) of every position so far; the query is the
-// q block of the LAST row.  One CTA per (head, batch item), 128 threads, key-parallel (see the kernel).  Exact fp32 -- the sampled token must not depend on operand rounding.
+// Cache rows are the in_proj outputs [q | k | v] (3 * H * 32 floats, row pitch ld) of every position so far: rows 0 .. *n_dev, the
+// last one just appended; the query is its q block.  The position lives in device memory so that the step can be a replayed CUDA
+// graph.  One CTA per (head, batch item), 128 threads, key-parallel (see the kernel).  Exact fp32 -- the sampled token must not
+// depend on operand rounding.
 // skip (optional, [B][2]): item b never reads keys skip[b][0] .. skip[b][1] - 1 -- the right padding of its text in a batch whose
 // rows are padded to a common text length (infer_panel_batch_infer).  The remaining keys are walked as one list, so thread t owns
 // the same keys whatever the padding, and a padded key (possibly not finite) never enters a sum.
-__global__ void __launch_bounds__(128) attn_decode_kernel(const float* __restrict__ qkv, long long sb, int ld, int n, const int* __restrict__ n_dev,
+__global__ void __launch_bounds__(128) attn_decode_kernel(const float* __restrict__ qkv, long long sb, int ld, const int* __restrict__ n_dev,
                                                            const int* __restrict__ skip, int H, float scale, float* __restrict__ out, int ldo) {
-  if (n_dev) n = *n_dev + 1;                                     // graph replay: keys 0 .. *n_dev (the row just appended)
+  const int n = *n_dev + 1;                                      // keys 0 .. *n_dev
   const int h = blockIdx.x, b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int s0 = skip ? skip[2 * b] : n, gap = skip ? skip[2 * b + 1] - s0 : 0;
   const float* base = qkv + (long long)b * sb;
@@ -564,21 +566,12 @@ extern "C" int evk_gemv_rows(const float* x, int32_t ldx, int32_t rows, const fl
   }
 }
 
-extern "C" int evk_attn_decode(const float* qkv, int64_t batch_stride, int32_t ld, int32_t n_keys, int32_t B, int32_t H, float scale,
-                               float* out, int32_t ldo, cudaStream_t st) {
-  EVK_REQUIRE(qkv && out && B >= 1 && H >= 1 && n_keys >= 1, EVK_ERR_ARG, "attn_decode: bad arguments");
-  EVK_REQUIRE(ld >= 3 * H * 32 && ldo >= H * 32, EVK_ERR_ARG, "attn_decode: row pitch %d / %d too small for %d heads of 32", ld, ldo, H);
-  EVK_REQUIRE(ld % 4 == 0 && batch_stride % 4 == 0 && ((uintptr_t)qkv % 16) == 0, EVK_ERR_ARG, "attn_decode: rows must be 16-byte aligned");
-  attn_decode_kernel<<<dim3(H, B), 128, 0, st>>>(qkv, batch_stride, ld, n_keys, nullptr, nullptr, H, scale, out, ldo);
-  return check_launch("attn_decode");
-}
-
 extern "C" int evk_attn_decode_dev(const float* qkv, int64_t batch_stride, int32_t ld, const int32_t* n_prev_dev, const int32_t* skip,
                                    int32_t B, int32_t H, float scale, float* out, int32_t ldo, cudaStream_t st) {
   EVK_REQUIRE(qkv && out && n_prev_dev && B >= 1 && H >= 1, EVK_ERR_ARG, "attn_decode_dev: bad arguments");
   EVK_REQUIRE(ld >= 3 * H * 32 && ldo >= H * 32, EVK_ERR_ARG, "attn_decode_dev: row pitch %d / %d too small for %d heads of 32", ld, ldo, H);
   EVK_REQUIRE(ld % 4 == 0 && batch_stride % 4 == 0 && ((uintptr_t)qkv % 16) == 0, EVK_ERR_ARG, "attn_decode_dev: rows must be 16-byte aligned");
-  attn_decode_kernel<<<dim3(H, B), 128, 0, st>>>(qkv, batch_stride, ld, 0, n_prev_dev, skip, H, scale, out, ldo);
+  attn_decode_kernel<<<dim3(H, B), 128, 0, st>>>(qkv, batch_stride, ld, n_prev_dev, skip, H, scale, out, ldo);
   return check_launch("attn_decode_dev");
 }
 

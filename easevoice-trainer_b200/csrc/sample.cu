@@ -1,5 +1,5 @@
-// Fused token sampler of batched AR decoding (Text2SemanticDecoder.infer_panel_batch_infer, t2s_model.py:563-730, and the
-// batched prompt-free path of infer_panel_naive_batched, :732-863):
+// Fused token sampler of the stage-1 GPT's KV-cache decoding (Text2SemanticDecoder.infer_panel_batch_infer, t2s_model.py:563-730,
+// and infer_panel_naive, :762-867, which also runs the prompt-free rows of infer_panel_naive_batched):
 // one CTA per batch row does the whole of utils.py:109-157 on that row's logits, appends the token to the row's history and
 // writes the next input row, so a decode step needs no host round trip and replays as part of one CUDA graph.
 #include <float.h>
@@ -63,7 +63,7 @@ __global__ void __launch_bounds__(kSampThreads) sample_tokens_kernel(
   const int W = (V + 31) >> 5;
   const unsigned* sb = seen + (size_t)b * W;
   // 1. repetition penalty over the row's history, prompt included (utils.py:117-123); steps idx < eos_steps leave EOS out
-  //    (batched decoding: step 0 only, :651-652; prompt-free decoding: the first 11 steps, :835-836)
+  //    (infer_panel_batch_infer: step 0 only, :651-652; infer_panel_naive: the first 11 steps, :835-836)
   for (int i = tid; i < V; i += blockDim.x) {
     float l = logits[(size_t)b * ldl + i];
     if ((sb[i >> 5] >> (i & 31)) & 1u) l = l < 0.f ? l * pen : l / pen;

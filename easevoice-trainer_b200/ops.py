@@ -1930,17 +1930,6 @@ class _CeFn(torch.autograd.Function):
         return dl, None, None, None, None
 
 
-def attn_decode(cache, n_keys, heads):
-    """cache [B, Lmax, 3 * heads * 32] = in_proj rows [q | k | v] of the positions so far -> attention output of the query in row
-    n_keys - 1 over keys 0 .. n_keys - 1: [B, 1, heads * 32].  No gradient (KV-cache decoding)."""
-    assert cache.dim() == 3 and cache.stride(2) == 1 and cache.shape[2] == 3 * heads * 32 and 1 <= n_keys <= cache.shape[1]
-    B = cache.shape[0]
-    out = torch.empty((B, 1, heads * 32), device=cache.device, dtype=torch.float32)
-    _call("evk_attn_decode", _p(cache), cache.stride(0), cache.stride(1), n_keys, B, heads, ctypes.c_float(1.0 / math.sqrt(32.0)),
-          _p(out), heads * 32)
-    return out
-
-
 def attn_decode_dev(cache, n_prev_dev, heads, row, skip=None):
     """Graph-replayable token step: append `row` [B, 1, 3 * heads * 32] at index *n_prev_dev (int32 device scalar) of the cache
     and attend rows 0 .. *n_prev_dev.  -> [B, 1, heads * 32].  skip: optional int32 device [B, 2]; item b then leaves out the
@@ -1958,7 +1947,7 @@ def attn_decode_dev(cache, n_prev_dev, heads, row, skip=None):
 
 def sample_tokens(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, alpha, x_next, q=None, eos_steps=1):
     """One fused sampling step over the rows of `logits` [B, >= V] (evk_sample_tokens_ex; see include/evk.h for the buffers).
-    EOS is excluded at the steps idx < eos_steps (1: batched decoding with a prompt; 11: prompt-free decoding).
+    EOS is excluded at the steps idx < eos_steps (1: infer_panel_batch_infer; 11: infer_panel_naive and prompt-free decoding).
     Everything it reads or writes stays in device memory, so it can be part of a captured CUDA graph."""
     B, D = logits.shape[0], x_next.shape[-1]
     if int(eos_steps) != eos_steps or eos_steps < 0:

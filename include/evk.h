@@ -383,19 +383,17 @@ int evk_sinepos_bwd(const float* dy, int32_t ldy, int64_t dy_sb, const float* pe
  * out2[0] = sum_r (lse_r - logit_r[target_r]); out2[1] = #hits / #valid, hit = fewer than top_k logits strictly above
  * the target's.  lse/nll: [rows] scratch kept for the backward; flags: [rows] bytes.
  * bwd: dl[r][c] = gscale[r / rows_per_g] * (softmax(logits_r)[c] - [c == target_r]). */
-/* KV-cache attention of one new token -- T2SBlock.decode_next_token (t2s_model.py:203-221), F.scaled_dot_product_attention
- * without mask.  qkv: the in_proj outputs [q | k | v] (3 * H * 32 floats per row, pitch ld, batch stride `batch_stride`) of
- * the n_keys positions so far; the query is the q block of row n_keys - 1.  out [B, H * 32] (pitch ldo).  Exact fp32. */
-int evk_attn_decode(const float* qkv, int64_t batch_stride, int32_t ld, int32_t n_keys, int32_t B, int32_t H, float scale,
-                    float* out, int32_t ldo, evk_stream_t stream);
 /* Skinny Linear of the KV-cache token step (decode_next_token, t2s_model.py:187-221: one new row per utterance):
  * y[r][n] = act(sum_c x[r][c] * W[n][c] + bias[n]) for rows <= 64; W = the packed forward operand PA[0] ([N][ldw], row n = output
  * channel n).  Exact fp32 FMAs, one pass over W.  A row's result does not depend on `rows` (same summation order for every
  * batch size).  rows <= 4 requires rows_rounded_up_to_a_power_of_2 * C <= 10240.  act: EVK_ACT_NONE / RELU / LRELU. */
 int evk_gemv_rows(const float* x, int32_t ldx, int32_t rows, const float* W, int32_t ldw, const float* bias, float* y,
                   int32_t ldy, int32_t N, int32_t C, int32_t act, float slope, evk_stream_t stream);
-/* The same with the position in DEVICE memory (a decode step replayed as a CUDA graph): *n_prev_dev = rows already in the cache
- * before this token; evk_cache_append writes the token's row at that index, evk_attn_decode_dev attends rows 0 .. *n_prev_dev.
+/* KV-cache attention of one new token -- T2SBlock.decode_next_token (t2s_model.py:203-221), F.scaled_dot_product_attention
+ * without mask -- with the position in DEVICE memory, so that a decode step replays as a CUDA graph.  qkv: the in_proj outputs
+ * [q | k | v] (3 * H * 32 floats per row, pitch ld, batch stride `batch_stride`) of the positions so far; *n_prev_dev = rows
+ * already in the cache before this token.  evk_cache_append writes the token's row at that index; evk_attn_decode_dev attends
+ * rows 0 .. *n_prev_dev with the q block of row *n_prev_dev as the query.  out [B, H * 32] (pitch ldo).  Exact fp32.
  * skip: NULL, or device [B][2]: item b leaves out keys skip[b][0] .. skip[b][1] - 1 (the right padding of its text when a batch
  * is padded to a common text length: skip[b] = (x_len_b, max_len)). */
 int evk_attn_decode_dev(const float* qkv, int64_t batch_stride, int32_t ld, const int32_t* n_prev_dev, const int32_t* skip,
@@ -419,7 +417,7 @@ int evk_sample_tokens(const float* logits, int32_t ldl, int32_t B, int32_t V, in
                       uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha, float* x_next,
                       int32_t D, evk_stream_t stream);
 /* The same with EOS excluded at every step idx < eos_steps (>= 0) instead of at step 0 only: evk_sample_tokens is this call with
- * eos_steps = 1.  Prompt-free decoding (infer_panel_naive with prompts = None, t2s_model.py:835-836) passes 11 and prefix 0. */
+ * eos_steps = 1.  infer_panel_naive (t2s_model.py:835-836) passes 11, with a prompt or without one (prefix 0). */
 int evk_sample_tokens_ex(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, int32_t eos_steps,
                          const int64_t* icfg, const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist,
                          int32_t ldh, uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha,

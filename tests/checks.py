@@ -1472,7 +1472,7 @@ def check_decode():
 
 def check_infer_panel():
     """SURVEY 8 row f4 (AR half): Text2SemanticDecoder.infer_panel -- prompt pass on the training kernels + KV-cache decoding
-    (evk_attn_decode) -- greedy, vs the token sequence and logits the REFERENCE decoded (tests/golden/infer_panel.json)."""
+    (evk_attn_decode_dev) -- greedy, vs the token sequence and logits the REFERENCE decoded (tests/golden/infer_panel.json)."""
     from easevoice_trainer_b200.models_gpt import Text2SemanticDecoder
     from oracle import gpt_oracle
     out = []
@@ -1491,13 +1491,14 @@ def check_infer_panel():
     # ---- the KV-cache attention kernel alone vs torch
     gg = _gen(5)
     cache = torch.randn(2, 700, 3 * 512, generator=gg).to(DEV)
-    for n in (1, 2, 37, 70, 128, 129, 700):
-        a = ops_mod().attn_decode(cache, n, 16)
+    for n in (1, 2, 37, 70, 128, 129, 700):                    # row n - 1 appended at n_prev = n - 1: keys 0 .. n - 1
+        a = ops_mod().attn_decode_dev(cache.clone(), torch.tensor([n - 1], dtype=torch.int32, device=DEV), 16,
+                                      cache[:, n - 1:n].clone())
         q = cache[:, n - 1, :512].view(2, 16, 1, 32).double().cpu()
         k = cache[:, :n, 512:1024].reshape(2, n, 16, 32).permute(0, 2, 1, 3).double().cpu()
         v = cache[:, :n, 1024:].reshape(2, n, 16, 32).permute(0, 2, 1, 3).double().cpu()
         ref = (torch.softmax(q @ k.transpose(-1, -2) / math.sqrt(32.0), -1) @ v).permute(0, 2, 1, 3).reshape(2, 1, 512)
-        out.append((f"attn_decode n_keys={n} vs float64 softmax(q k^T / sqrt(32)) v", rel(a, ref), 2e-6))
+        out.append((f"attn_decode_dev n_keys={n} vs float64 softmax(q k^T / sqrt(32)) v", rel(a, ref), 2e-6))
     # ---- the skinny Linear of the token step (evk_gemv_rows: exact fp32 over the packed, TF32-rounded weight) vs float64
     o = ops_mod()
     for rows, N, C, act in ((1, 1536, 512, o.ACT_NONE), (1, 512, 2048, o.ACT_NONE), (1, 2048, 512, o.ACT_RELU), (3, 1028, 512, o.ACT_NONE),

@@ -79,5 +79,8 @@ def test_cpu_inputs_have_no_prompt_free_path():
     x = [torch.zeros(5, dtype=torch.long)]
     with pytest.raises(NotImplementedError):
         _net().infer_panel_naive(x[0].unsqueeze(0), torch.tensor([5]), None, torch.zeros(1, 1024, 5), top_k=5)
+    with pytest.raises(NotImplementedError):                   # with a prompt there is no CPU path either
+        _net().infer_panel_naive(x[0].unsqueeze(0), torch.tensor([5]), torch.zeros(1, 3, dtype=torch.long), torch.zeros(1, 1024, 5),
+                                 top_k=5)
     with pytest.raises(NotImplementedError):
         _net().infer_panel_naive_batched(x, torch.tensor([5]), None, [torch.zeros(1024, 5)], top_k=5)

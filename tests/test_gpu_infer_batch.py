@@ -270,6 +270,54 @@ def test_batch_of_one_matches_infer_panel_naive(ops):
     assert torch.equal(y[0], yn[0]) and idx == [20] and idxn == 19    # at early stop the naive path returns idx - 1
 
 
+def test_eos_window_of_infer_panel_with_a_prompt(ops):
+    net = _net(1.0)
+    with torch.no_grad():
+        # the last LayerNorm's output then sums to D whatever its input, so EOS has the logit 0.1 * D = 51.2 at every step,
+        # far above every other class
+        net.P(f"h.layers.{net.num_layers - 1}.norm2.weight").fill_(1.0)
+        net.P(f"h.layers.{net.num_layers - 1}.norm2.bias").fill_(1.0)
+        net.P("ar_predict_layer.weight")[EOS].fill_(0.1)
+    x, bert, prompts = _inputs()
+    Yp = prompts.shape[1]
+    y, idx = net.infer_panel(x[0].unsqueeze(0), torch.tensor([x[0].shape[0]]), prompts[:1], bert[0].unsqueeze(0), top_k=1,
+                             early_stop_num=50)
+    assert tuple(y.shape) == (1, Yp + 11) and idx == 10                # EOS excluded for the first 11 steps, taken at step 11
+    yb, idxb = net.infer_panel_batch_infer(x[:1], torch.tensor([x[0].shape[0]]), prompts[:1], bert[:1], top_k=1, early_stop_num=50)
+    assert yb[0].shape[0] == Yp + 1 and idxb == [0]                    # excluded at step 0 only: stops at step 1
+    assert torch.equal(yb[0], y[0, :Yp + 1])
+
+
+def test_sampled_infer_panel_repeats_under_manual_seed(ops):
+    net = _net(1.0, n_layer=4)
+    x, bert, prompts = _inputs()
+    kw = dict(top_k=15, top_p=0.9, early_stop_num=40, temperature=1.0)
+    runs = []
+    for seed in (0, 0, 1):
+        torch.manual_seed(seed)
+        runs.append(net.infer_panel(x[0].unsqueeze(0), torch.tensor([x[0].shape[0]]), prompts[:1], bert[0].unsqueeze(0), **kw))
+    (y0, i0), (y1, i1), (y2, _) = runs
+    assert torch.equal(y0, y1) and i0 == i1
+    assert not torch.equal(y0, y2)                                      # the noise does come from the seeded generator
+    assert torch.equal(y0[0, :prompts.shape[1]], prompts[0]) and int(y0.max()) < EOS
+
+
+def test_infer_panel_reuses_its_step_graph(ops):
+    net = _net(1.0, n_layer=4)
+    x, bert, prompts = _inputs()
+
+    def one(n):                                                         # the first n phonemes of row 0
+        return net.infer_panel(x[0][None, :n], torch.tensor([n]), prompts[:1], bert[0][None, :, :n], top_k=1, early_stop_num=20)
+    n = x[0].shape[0]
+    one(n)
+    st = net.__dict__["_batch_st1"]
+    graph = st["graphs"][11]
+    one(n - 3)
+    net.infer_panel_batch_infer(x, torch.tensor(GOLD["cfg"]["x_lens"]), prompts, bert, top_k=1, early_stop_num=20)   # B > 1
+    one(n - 5)
+    assert net.__dict__["_batch_st1"] is st and st["graphs"][11] is graph
+
+
 def test_sampled_batch_of_16(ops):
     net = _net(1.0, n_layer=4)
     g = torch.Generator().manual_seed(4)

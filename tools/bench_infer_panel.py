@@ -8,6 +8,8 @@ One JSON line.   python tools/bench_infer_panel.py > gpurun_out/bench_infer_pane
 # name and power limit read in the same run.  --profile DIR (with --batch): also a torch.profiler trace of one B = 16 call.
 # --ref-free: prompt-free decoding (TTS's ref_text_free mode), infer_panel_naive(prompts=None) on one utterance next to
 # infer_panel_naive_batched(prompts=None) for B in {1, 4, 16}, same 120 phonemes / 300 tokens / top_k 15, card name and power limit.
+# --new N: N generated tokens (early_stop_num) instead of 300 in every mode, e.g. 40 for a short sentence, where the steps run
+# past a batch's last finish between two reads of the finished flags weigh the most.
 import json
 import math
 import os
@@ -30,7 +32,8 @@ P = gpt_oracle.init_params(gpt_oracle.gpt_param_spec(m), 35)
 net = Text2SemanticDecoder({"model": m})
 net.load_state_dict(P)
 net = net.to(dev).eval()
-X, Yp, NEW = 120, 150, 300
+X, Yp = 120, 150
+NEW = int(sys.argv[sys.argv.index("--new") + 1]) if "--new" in sys.argv else 300
 g = torch.Generator().manual_seed(2)
 x = torch.randint(0, m["phoneme_vocab_size"], (1, X), generator=g)
 bert = torch.randn(1, 1024, X, generator=g)
@@ -50,7 +53,7 @@ def card_name():
 def bench_ref_free():
     """infer_panel_naive(prompts=None) on one utterance and infer_panel_naive_batched(prompts=None) for B in {1, 4, 16}: generated
     tokens / wall time of one call (prompt pass included)."""
-    net.infer_panel_naive(xd, xl, None, bd, top_k=15, top_p=1, early_stop_num=8, temperature=1.0)              # warm-up
+    net.infer_panel_naive(xd, xl, None, bd, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)            # warm-up
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     y, _ = net.infer_panel_naive(xd, xl, None, bd, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)
@@ -60,7 +63,7 @@ def bench_ref_free():
     out = {}
     for B in (1, 4, 16):
         xs, bs, lens = [xd[0]] * B, [bd[0]] * B, torch.full((B,), X)
-        net.infer_panel_naive_batched(xs, lens, None, bs, top_k=15, top_p=1, early_stop_num=8, temperature=1.0)   # warm-up, capture
+        net.infer_panel_naive_batched(xs, lens, None, bs, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)  # warm-up, capture
         torch.cuda.synchronize()
         t0 = time.perf_counter()
         ys, _ = net.infer_panel_naive_batched(xs, lens, None, bs, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)
@@ -87,7 +90,7 @@ def bench_batch():
     for B in (1, 4, 16):
         xs, bs, ps = [xd[0]] * B, [bd[0]] * B, pd.expand(B, -1)
         lens = torch.full((B,), X)
-        net.infer_panel_batch_infer(xs, lens, ps, bs, top_k=15, top_p=1, early_stop_num=8, temperature=1.0)        # warm-up, capture
+        net.infer_panel_batch_infer(xs, lens, ps, bs, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)      # warm-up, capture
         torch.cuda.synchronize()
         t0 = time.perf_counter()
         ys, idx = net.infer_panel_batch_infer(xs, lens, ps, bs, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)
@@ -110,7 +113,9 @@ def bench_batch():
     return out, card_name()
 
 
-net.infer_panel(xd, xl, pd, bd, top_k=15, top_p=1, early_stop_num=8, temperature=1.0)     # warm-up (packs the weights once)
+# every warm-up runs at the timed size: it packs the weights, sizes the KV caches and captures the step graph, so that the timed
+# call measures decoding alone
+net.infer_panel(xd, xl, pd, bd, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)
 torch.cuda.synchronize()
 t0 = time.perf_counter()
 y, idx = net.infer_panel(xd, xl, pd, bd, top_k=15, top_p=1, early_stop_num=NEW, temperature=1.0)
@@ -172,7 +177,7 @@ with torch.no_grad():
     cpu_s = time.perf_counter() - t0
 print(json.dumps(dict(metric="Text2SemanticDecoder.infer_panel (KV-cache AR decoding), one utterance", unit="semantic-tokens/s",
                       value=new / gpu_s, generated=new, seconds=gpu_s, ms_per_token=gpu_s / max(new, 1) * 1e3,
-                      config=dict(layers=24, X=X, prompt=Yp, top_k=15, top_p=1, temperature=1.0, launch_mode="graph" if __import__("easevoice_trainer_b200.models_gpt", fromlist=["x"]).INFER_GRAPH else "eager"),
+                      config=dict(layers=24, X=X, prompt=Yp, early_stop_num=NEW, top_k=15, top_p=1, temperature=1.0),
                       note="prompt pass included in the time; 25 tokens = 1 s of audio",
                       cpu_baseline=dict(value=n_cpu / cpu_s, unit="semantic-tokens/s", cores=threads, kind="port",
                                         sample=f"prompt pass + {n_cpu} greedy tokens, torch CPU ops, KV cache as t2s_model.py:121-221"))))
