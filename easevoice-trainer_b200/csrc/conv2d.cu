@@ -1,10 +1,13 @@
-// 2-D convolution family of the UVR5 VR separator (CascadedASPPNet, uvr5.py), inference only, channels-last (NHWC) fp32.
+// 2-D convolution family of the UVR5 VR separators (CascadedASPPNet and the DeEcho / DeReverb CascadedNet, uvr5.py),
+// inference only, channels-last (NHWC) fp32.
 //
 // A pixel (b, y, x) of an activation lives at  base + b*bs + (y*W + x)*pitch  and holds C channels from there on, so a
 // layer can read or write a channel slice of a wider concat buffer (pointer advanced by the slice's channel offset).
 //
 //   conv2d_fwd   implicit GEMM: M = B*Ho*Wo output pixels, N = output channels, K = k*k*C (tap-major, channel-minor),
-//                CTA tile 128 rows x 32 K, fp32 accumulation.  Two kernels, chosen from the operands:
+//                CTA tile 128 rows x 32 K, fp32 accumulation.  Zero padding and dilation are per axis (conv2d_fwd_hw:
+//                the DeEcho net's ASPP dilates rows and columns differently; conv2d_fwd is the equal-axes call).
+//                Two kernels, chosen from the operands:
 //                * wgmma (TF32): C, pitches and pointers allow 16-byte copies and 3xTF32 is off.  Two consumer
 //                  warpgroups of 64 rows x 32 / 64 / 128 columns (the smallest that covers N), a 4-stage cp.async
 //                  ring in the 128-byte-swizzle layout, operands rounded to TF32 in shared memory.
@@ -30,7 +33,7 @@ struct ConvArgs {
   const float* x; const float* w; const float* scale; const float* bias; float* y;
   long long x_bs, y_bs;
   int x_pitch, y_pitch;
-  int B, H, W, C, N, k, stride, pad, dil, Ho, Wo, M, Kt, act;
+  int B, H, W, C, N, k, stride, pad_h, pad_w, dil_h, dil_w, Ho, Wo, M, Kt, act;
 };
 
 __device__ __forceinline__ float apply_act(float v, int act) {
@@ -61,8 +64,8 @@ __device__ __forceinline__ void load_slab(const ConvArgs& a, float* sA, float* s
       const int tap = k / a.C;
       c = k - tap * a.C;
       const int ky = tap / a.k;
-      dy = ky * a.dil;
-      dx = (tap - ky * a.k) * a.dil;
+      dy = ky * a.dil_h;
+      dx = (tap - ky * a.k) * a.dil_w;
     }
 #pragma unroll
     for (int i = 0; i < BM / 32; ++i) {
@@ -87,8 +90,8 @@ __device__ __forceinline__ void load_slab(const ConvArgs& a, float* sA, float* s
       const int tap = k / a.C;
       c = k - tap * a.C;
       const int ky = tap / a.k;
-      dy = ky * a.dil;
-      dx = (tap - ky * a.k) * a.dil;
+      dy = ky * a.dil_h;
+      dx = (tap - ky * a.k) * a.dil_w;
     }
 #pragma unroll 4
     for (int i = 0; i < BM / 8; ++i) {
@@ -120,8 +123,8 @@ __global__ void __launch_bounds__(NT, 2) conv2d_fwd_kernel(ConvArgs a) {
     if (m < a.M) {
       const int b = m / HWo, r = m - b * HWo, oy = r / a.Wo, ox = r - oy * a.Wo;
       rbase[tid] = (long long)b * a.x_bs;
-      riy[tid] = oy * a.stride - a.pad;
-      rix[tid] = ox * a.stride - a.pad;
+      riy[tid] = oy * a.stride - a.pad_h;
+      rix[tid] = ox * a.stride - a.pad_w;
     } else {
       rbase[tid] = 0; riy[tid] = -(1 << 29); rix[tid] = 0;      // never in bounds -> zero rows
     }
@@ -249,8 +252,8 @@ __device__ __forceinline__ void load_slab_sw(const ConvArgs& a, uint32_t sA, uin
     const int tap = k / a.C;
     c = k - tap * a.C;
     const int ky = tap / a.k;
-    dy = ky * a.dil;
-    dx = (tap - ky * a.k) * a.dil;
+    dy = ky * a.dil_h;
+    dx = (tap - ky * a.k) * a.dil_w;
   }
 #pragma unroll
   for (int i = 0; i < BM / 32; ++i) {
@@ -299,8 +302,8 @@ __global__ void __launch_bounds__(NT, 1) conv2d_fwd_wgmma_kernel(ConvArgs a) {
     if (m < a.M) {
       const int b = m / HWo, r = m - b * HWo, oy = r / a.Wo, ox = r - oy * a.Wo;
       rbase[tid] = (long long)b * a.x_bs;
-      riy[tid] = oy * a.stride - a.pad;
-      rix[tid] = ox * a.stride - a.pad;
+      riy[tid] = oy * a.stride - a.pad_h;
+      rix[tid] = ox * a.stride - a.pad_w;
     } else {
       rbase[tid] = 0; riy[tid] = -(1 << 29); rix[tid] = 0;
     }
@@ -503,24 +506,26 @@ extern int g_precise;
 
 using namespace evk;
 
-extern "C" int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale,
-                              const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W,
-                              int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad, int32_t dil, int32_t act,
-                              cudaStream_t st) {
+extern "C" int evk_conv2d_fwd_hw(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale,
+                                 const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W,
+                                 int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h,
+                                 int32_t dil_w, int32_t act, cudaStream_t st) {
   EVK_REQUIRE(x && w && y, EVK_ERR_ARG, "conv2d: null tensor");
   EVK_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && N > 0, EVK_ERR_ARG, "conv2d: bad sizes B=%d H=%d W=%d C=%d N=%d", B, H, W,
               C, N);
-  EVK_REQUIRE((k == 1 || k == 3) && (stride == 1 || stride == 2) && pad >= 0 && dil >= 1, EVK_ERR_ARG,
-              "conv2d: kernel %d stride %d pad %d dilation %d (kernel 1 or 3, stride 1 or 2)", k, stride, pad, dil);
+  EVK_REQUIRE((k == 1 || k == 3) && (stride == 1 || stride == 2) && pad_h >= 0 && pad_w >= 0 && dil_h >= 1 && dil_w >= 1,
+              EVK_ERR_ARG, "conv2d: kernel %d stride %d pad (%d, %d) dilation (%d, %d) (kernel 1 or 3, stride 1 or 2)", k,
+              stride, pad_h, pad_w, dil_h, dil_w);
   EVK_REQUIRE(act >= EVK_C2_NONE && act <= EVK_C2_SIGMOID, EVK_ERR_ARG, "conv2d: bad activation %d", act);
   EVK_REQUIRE(x_pitch >= C && y_pitch >= N, EVK_ERR_ARG, "conv2d: pitch smaller than the channel count");
-  const int span = dil * (k - 1) + 1;
-  EVK_REQUIRE(H + 2 * pad >= span && W + 2 * pad >= span, EVK_ERR_ARG, "conv2d: input smaller than the kernel");
-  const int Ho = (H + 2 * pad - span) / stride + 1, Wo = (W + 2 * pad - span) / stride + 1;
+  const int span_h = dil_h * (k - 1) + 1, span_w = dil_w * (k - 1) + 1;
+  EVK_REQUIRE(H + 2 * pad_h >= span_h && W + 2 * pad_w >= span_w, EVK_ERR_ARG, "conv2d: input smaller than the kernel");
+  const int Ho = (H + 2 * pad_h - span_h) / stride + 1, Wo = (W + 2 * pad_w - span_w) / stride + 1;
   const long long M = (long long)B * Ho * Wo, Kt = (long long)k * k * C;
   EVK_REQUIRE(M < (1ll << 31) && Kt < (1ll << 31) && (long long)N * Kt < (1ll << 31) && (long long)H * W < (1 << 30),
               EVK_ERR_ARG, "conv2d: problem too large");
-  ConvArgs a{x, w, scale, bias, y, x_bs, y_bs, x_pitch, y_pitch, B, H, W, C, N, k, stride, pad, dil, Ho, Wo, (int)M, (int)Kt, act};
+  ConvArgs a{x, w, scale, bias, y, x_bs, y_bs, x_pitch, y_pitch, B, H, W, C, N, k, stride,
+             pad_h, pad_w, dil_h, dil_w, Ho, Wo, (int)M, (int)Kt, act};
   dim3 grid(cdiv(M, BM), cdiv(N, BN));
   EVK_REQUIRE(grid.y <= 65535, EVK_ERR_ARG, "conv2d: too many output channels");
   const bool vec = C % 4 == 0 && x_pitch % 4 == 0 && x_bs % 4 == 0 && (uintptr_t)x % 16 == 0 && (uintptr_t)w % 16 == 0;
@@ -530,6 +535,14 @@ extern "C" int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, con
   if (N <= 32) return launch_conv_wgmma<32>(a, st);
   if (N <= 64) return launch_conv_wgmma<64>(a, st);
   return launch_conv_wgmma<128>(a, st);
+}
+
+extern "C" int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale,
+                              const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W,
+                              int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad, int32_t dil, int32_t act,
+                              cudaStream_t st) {
+  return evk_conv2d_fwd_hw(x, x_pitch, x_bs, w, scale, bias, y, y_pitch, y_bs, B, H, W, C, N, k, stride, pad, pad, dil, dil,
+                           act, st);
 }
 
 extern "C" int evk_dwconv3x3_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, float* y, int32_t y_pitch,

@@ -2081,13 +2081,17 @@ def conv2d_out(n, k, stride, pad, dil):
 
 
 def conv2d(x: CLView, w, y: CLView, *, k, stride=1, pad=0, dil=1, scale=None, bias=None, act=C2_NONE):
-    """y = act(conv2d(x) * scale + bias) (evk_conv2d_fwd): w [N, k, k, C] fp32 contiguous; y must be [B, Ho, Wo, N]."""
+    """y = act(conv2d(x) * scale + bias) (evk_conv2d_fwd): w [N, k, k, C] fp32 contiguous; y must be [B, Ho, Wo, N].
+    pad and dil are ints, or (rows, columns) pairs (evk_conv2d_fwd_hw)."""
     N = w.shape[0]
     assert w.is_contiguous() and tuple(w.shape) == (N, k, k, x.C) and y.C == N and y.B == x.B, (w.shape, x.C, y.C)
-    Ho, Wo = conv2d_out(x.H, k, stride, pad, dil), conv2d_out(x.W, k, stride, pad, dil)
+    hw = isinstance(pad, (tuple, list)) or isinstance(dil, (tuple, list))
+    (ph, pw), (dh, dw) = [v if isinstance(v, (tuple, list)) else (v, v) for v in (pad, dil)]
+    Ho, Wo = conv2d_out(x.H, k, stride, ph, dh), conv2d_out(x.W, k, stride, pw, dw)
     assert (y.H, y.W) == (Ho, Wo), ((y.H, y.W), (Ho, Wo))
-    _call_f("evk_conv2d_fwd", 2.0 * x.B * Ho * Wo * N * k * k * x.C, *x.args(), _p(w), _p(scale), _p(bias), *y.args(),
-            x.B, x.H, x.W, x.C, N, k, stride, pad, dil, act)
+    geo = ("evk_conv2d_fwd_hw", ph, pw, dh, dw) if hw else ("evk_conv2d_fwd", ph, dh)
+    _call_f(geo[0], 2.0 * x.B * Ho * Wo * N * k * k * x.C, *x.args(), _p(w), _p(scale), _p(bias), *y.args(),
+            x.B, x.H, x.W, x.C, N, k, stride, *geo[1:], act)
 
 
 def dwconv3x3(x: CLView, w, y: CLView, dil):
@@ -2119,3 +2123,30 @@ def vr_mask_head(h: CLView, w, mix, offset, split_bin=0, e_lo=1.0, e_hi=1.0, use
     _call("evk_vr_mask_head", *h.args(), _p(w), h.C, _p(mix), _p(out), B, h.H, out_bin, W, offset, split_bin,
           ctypes.c_float(e_lo), ctypes.c_float(e_hi), 1 if use_agg else 0)
     return out
+
+
+def transpose_rows(x, out=None):
+    """[B, T, C] -> [B, C, T] (evk_transpose_rows): x contiguous fp32; `out` may be given as a contiguous [B, C, T]"""
+    assert x.dim() == 3 and x.is_contiguous() and x.dtype == torch.float32 and x.is_cuda, (x.shape, x.dtype)
+    B, T, C = x.shape
+    if out is None:
+        out = torch.empty((B, C, T), device=x.device, dtype=torch.float32)
+    assert out.is_contiguous() and tuple(out.shape) == (B, C, T)
+    _call("evk_transpose_rows", _p(x), C, T * C, _p(out), T, C * T, B, T, C, 0)
+    return out
+
+
+def lstm_bidir(g, w_hh, order="tn"):
+    """Recurrence of a bidirectional one-layer nn.LSTM (evk_lstm_bidir_fwd).  g: the input projections with both biases
+    added, [T, N, 8H] (order "tn") or [N, T, 8H] (order "nt"), last axis [direction][gate i, f, g, o][H]; w_hh [2, 4H, H].
+    -> y with g's leading axes and 2H columns [h_forward | h_reverse], the nn.LSTM output layout."""
+    assert g.dim() == 3 and g.is_contiguous() and g.dtype == torch.float32 and g.is_cuda, (g.shape, g.dtype)
+    H = w_hh.shape[-1]
+    assert w_hh.is_contiguous() and tuple(w_hh.shape) == (2, 4 * H, H) and g.shape[2] == 8 * H, (g.shape, w_hh.shape)
+    T, N = g.shape[:2] if order == "tn" else g.shape[1::-1]
+    y = torch.empty(g.shape[:2] + (2 * H,), device=g.device, dtype=torch.float32)
+    gs, ys = (g.stride(0), g.stride(1)), (y.stride(0), y.stride(1))
+    if order != "tn":
+        gs, ys = gs[::-1], ys[::-1]
+    _call_f("evk_lstm_bidir_fwd", 2.0 * 2 * T * N * 4 * H * H, _p(g), *gs, _p(w_hh), _p(y), *ys, T, N, H)
+    return y

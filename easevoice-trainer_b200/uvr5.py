@@ -1,5 +1,7 @@
-"""UVR5 VR vocal separation on the library's kernels: the CascadedASPPNet of the HP2 / HP3 / HP5 models
-(lib_v5/vr_network/nets.py, layers.py) and a batched drop-in for SeparateVR.inference (uvr5/separate.py:198-273).
+"""UVR5 VR separation on the library's kernels: the CascadedASPPNet of the HP2 / HP3 / HP5 models
+(lib_v5/vr_network/nets.py, layers.py), the CascadedNet of the DeEcho / DeReverb models (nets_new.py, layers_new.py; see
+CascadedNet for its layout), and a batched drop-in for SeparateVR.inference (uvr5/separate.py:198-273), which
+SeparateVREcho inherits.
 
 The reference runs the net on one 512-frame window per call, copying each result to the host before the next.  Here every
 window of a file, TTA windows included, goes through the net in batches of `max_windows`, and the result reaches the host
@@ -100,18 +102,65 @@ def _cl_weight(w):
     return w.float().permute(0, 2, 3, 1).contiguous()
 
 
-class CascadedASPPNet:
+class _SpecNet:
+    """What the two VR nets share: bins, the device, the folded layers, and the shape rules of their inputs."""
+
+    def __init__(self, n_fft, offset):
+        self.max_bin = n_fft // 2
+        self.output_bin = n_fft // 2 + 1
+        self.offset = offset
+        self.device = torch.device("cpu")
+        self.layers = None
+
+    def to(self, device):
+        self.device = torch.device(device)
+        if self.layers is not None:
+            self.layers = {p: {k: (v.to(self.device) if torch.is_tensor(v) else v) for k, v in L.items()}
+                           for p, L in self.layers.items()}
+        return self
+
+    def eval(self):
+        return self
+
+    def check_input(self, x, crop):
+        if not (torch.is_tensor(x) and x.dim() == 4 and x.shape[1] == 2 and x.shape[2] == self.output_bin):
+            raise ValueError(f"expected [B, 2, {self.output_bin}, W] magnitudes, got "
+                             f"{tuple(x.shape) if torch.is_tensor(x) else type(x)}")
+        self.check_shape(x.shape[3], crop)
+        if self.layers is None:
+            raise ValueError("no weights loaded")
+        if not x.is_cuda or self.device.type != "cuda":
+            raise ValueError("the VR net runs on CUDA tensors and weights only")
+
+    def check_shape(self, W, crop):
+        """The shapes the net takes: both band heights and W multiples of 16 (four stride-2 encoders, then x2 upsamples
+        that must meet their skips), and W > 2 * offset when cropped.  The reference fails inside torch.cat or asserts."""
+        if self.max_bin % 2 or (self.max_bin // 2) % 16:
+            raise ValueError(f"band height {self.max_bin // 2} (n_fft // 4) must be a multiple of 16 and n_fft // 2 even")
+        if W % 16:
+            raise ValueError(f"frame count {W} must be a multiple of 16")
+        if crop and W <= 2 * self.offset:
+            raise ValueError(f"frame count {W} must exceed 2 * offset = {2 * self.offset}")
+
+    def _empty(self, B, H, W, C):
+        return torch.empty((B, H, W, C), device=self.device, dtype=torch.float32)
+
+    def _conv(self, p, x, y, stride=1, act=ops.C2_RELU, dil=1):
+        """folded Conv2d + BatchNorm + act of layer p; dil is an int or a (rows, columns) pair, padding = dil * (k // 2)"""
+        L = self.layers[p]
+        k = L["k"]
+        pad = tuple(d * (k // 2) for d in dil) if isinstance(dil, tuple) else dil * (k // 2)
+        ops.conv2d(x, L["w"], y, k=k, stride=stride, pad=pad, dil=dil, scale=L["scale"], bias=L["bias"], act=act)
+
+
+class CascadedASPPNet(_SpecNet):
     """nets.CascadedASPPNet(n_fft, params) in eval mode on CUDA.  Input [B, 2, n_fft // 2 + 1, W] magnitudes (fp32)."""
 
     def __init__(self, n_fft, size=61968):
         if size not in SIZES:
             raise ValueError(f"unknown VR net size {size}; known: {sorted(SIZES)}")
+        super().__init__(n_fft, 128)
         self.size, self.cfg = size, SIZES[size]
-        self.max_bin = n_fft // 2
-        self.output_bin = n_fft // 2 + 1
-        self.offset = 128
-        self.device = torch.device("cpu")
-        self.layers = None
 
     # ---- weights -----------------------------------------------------------------------------------------
     def load_state_dict(self, sd):
@@ -140,16 +189,6 @@ class CascadedASPPNet:
                        for p, L in layers.items()}
         return self
 
-    def to(self, device):
-        self.device = torch.device(device)
-        if self.layers is not None:
-            self.layers = {p: {k: (v.to(self.device) if torch.is_tensor(v) else v) for k, v in L.items()}
-                           for p, L in self.layers.items()}
-        return self
-
-    def eval(self):
-        return self
-
     @classmethod
     def from_pretrained(cls, path, n_fft=1344, device="cuda"):
         """Load a VR-net .pth (HP2 / HP3 / HP5 ...): the parameter set is read from the weight shapes (band-net width from
@@ -159,26 +198,6 @@ class CascadedASPPNet:
         return cls(n_fft, infer_size(sd)).to(device).load_state_dict(sd)
 
     # ---- forward -----------------------------------------------------------------------------------------
-    def check_input(self, x, crop):
-        if not (torch.is_tensor(x) and x.dim() == 4 and x.shape[1] == 2 and x.shape[2] == self.output_bin):
-            raise ValueError(f"expected [B, 2, {self.output_bin}, W] magnitudes, got "
-                             f"{tuple(x.shape) if torch.is_tensor(x) else type(x)}")
-        self.check_shape(x.shape[3], crop)
-        if self.layers is None:
-            raise ValueError("no weights loaded")
-        if not x.is_cuda or self.device.type != "cuda":
-            raise ValueError("the VR net runs on CUDA tensors and weights only")
-
-    def check_shape(self, W, crop):
-        """The shapes the net takes: both band heights and W multiples of 16 (four stride-2 encoders, then x2 upsamples
-        that must meet their skips), and W > 2 * offset when cropped.  The reference fails inside torch.cat or asserts."""
-        if self.max_bin % 2 or (self.max_bin // 2) % 16:
-            raise ValueError(f"band height {self.max_bin // 2} (n_fft // 4) must be a multiple of 16 and n_fft // 2 even")
-        if W % 16:
-            raise ValueError(f"frame count {W} must be a multiple of 16")
-        if crop and W <= 2 * self.offset:
-            raise ValueError(f"frame count {W} must exceed 2 * offset = {2 * self.offset}")
-
     def forward(self, x, aggressiveness=None):
         """mask * x over all W frames: [B, 2, output_bin, W] (CascadedASPPNet.forward in eval mode)"""
         self.check_input(x, crop=False)
@@ -190,14 +209,6 @@ class CascadedASPPNet:
         """forward cropped by `offset` frames on both time edges: [B, 2, output_bin, W - 256]"""
         self.check_input(x_mag, crop=True)
         return self._run(x_mag, aggressiveness, self.offset)
-
-    def _conv(self, p, x, y, stride=1, act=ops.C2_RELU, dil=1):
-        L = self.layers[p]
-        k = L["k"]
-        ops.conv2d(x, L["w"], y, k=k, stride=stride, pad=dil * (k // 2), dil=dil, scale=L["scale"], bias=L["bias"], act=act)
-
-    def _empty(self, B, H, W, C):
-        return torch.empty((B, H, W, C), device=self.device, dtype=torch.float32)
 
     def _aspp(self, p, x, enlarge):
         B, H, W, c = x.B, x.H, x.W, x.C
@@ -285,6 +296,289 @@ def infer_size(sd):
 def get_nets_model(n_fft, size=61968):
     """nets.get_nets_model: an unloaded CascadedASPPNet (call load_state_dict, then .to("cuda"))"""
     return CascadedASPPNet(n_fft, size)
+
+
+# ---- DeEcho / DeReverb: nets_new.CascadedNet (layers_new.py) ------------------------------------------------------
+ECHO_DILATIONS = ((4, 2), (8, 4), (12, 6))      # ASPP conv3..conv5, (rows, columns); padding = dilation
+
+
+def _round4(c):
+    return (c + 3) // 4 * 4
+
+
+def _skip_first(n_up, n_skip):
+    """Decoder input columns: the reference concatenates [upsampled (n_up) | skip (n_skip)]; the buffers here hold the skip
+    first, so every slice an encoder writes and reads starts 16-byte aligned -> where reference channel i goes"""
+    return [n_skip + i for i in range(n_up)] + list(range(n_skip))
+
+
+def _echo_base_keys(spec, p, nin, ch, nin_lstm, nout_lstm):
+    spec[p + ".enc1"] = ("cbr", (ch, nin, 3))
+    for i, (a, b) in zip(range(2, 6), [(ch, 2 * ch), (2 * ch, 4 * ch), (4 * ch, 6 * ch), (6 * ch, 8 * ch)]):
+        spec[f"{p}.enc{i}.conv1"] = ("cbr", (b, a, 3))
+        spec[f"{p}.enc{i}.conv2"] = ("cbr", (b, b, 3))
+    c = 8 * ch
+    spec[p + ".aspp.conv1.1"] = ("cbr", (c, c, 1))
+    spec[p + ".aspp.conv2"] = ("cbr", (c, c, 1))
+    for i in range(3, 6):
+        spec[f"{p}.aspp.conv{i}"] = ("cbr", (c, c, 3))
+    spec[p + ".aspp.bottleneck"] = ("cbr", (c, 5 * c, 1))
+    for i, (a, b) in zip((4, 3, 2), [(14 * ch, 6 * ch), (10 * ch, 4 * ch), (6 * ch, 2 * ch)]):
+        spec[f"{p}.dec{i}.conv1"] = ("cbr", (b, a, 3))
+    spec[p + ".lstm_dec2.conv"] = ("cbr", (1, 2 * ch, 1))
+    spec[p + ".lstm_dec2"] = ("lstm", (nin_lstm, nout_lstm // 2))
+    spec[p + ".dec1.conv1"] = ("cbr", (ch, 3 * ch + 1, 3))
+
+
+def echo_layer_spec(n_fft, nout, nout_lstm=128):
+    """-> {module prefix: (kind, shape)} of nets_new.CascadedNet(n_fft, nout, nout_lstm): "cbr" = Conv2d (no bias) +
+    BatchNorm2d + activation, shape (nout, nin, k); "lstm" = LSTMModule's bidirectional nn.LSTM + Linear + BatchNorm1d,
+    shape (bins, hidden per direction); "conv" = a bias-free 1x1 Conv2d."""
+    nin_lstm = n_fft // 2 // 2
+    spec = {}
+    _echo_base_keys(spec, "stg1_low_band_net.0", 2, nout // 2, nin_lstm // 2, nout_lstm)
+    spec["stg1_low_band_net.1"] = ("cbr", (nout // 4, nout // 2, 1))
+    _echo_base_keys(spec, "stg1_high_band_net", 2, nout // 4, nin_lstm // 2, nout_lstm // 2)
+    _echo_base_keys(spec, "stg2_low_band_net.0", nout // 4 + 2, nout, nin_lstm // 2, nout_lstm)
+    spec["stg2_low_band_net.1"] = ("cbr", (nout // 2, nout, 1))
+    _echo_base_keys(spec, "stg2_high_band_net", nout // 4 + 2, nout // 2, nin_lstm // 2, nout_lstm // 2)
+    _echo_base_keys(spec, "stg3_full_band_net", 3 * nout // 4 + 2, nout, nin_lstm, nout_lstm)
+    spec["out"] = ("conv", (2, nout))
+    spec["aux_out"] = ("conv", (2, 3 * nout // 4))
+    return spec
+
+
+def echo_state_dict_shapes(n_fft, nout, nout_lstm=128):
+    """-> {state_dict key: shape} of nets_new.CascadedNet(n_fft, nout, nout_lstm), num_batches_tracked left out"""
+    out = {}
+    for p, (kind, shape) in echo_layer_spec(n_fft, nout, nout_lstm).items():
+        if kind == "conv":
+            out[p + ".weight"] = shape + (1, 1)
+        elif kind == "cbr":
+            n, nin, k = shape
+            out[p + ".conv.0.weight"] = (n, nin, k, k)
+            for s in ("weight", "bias", "running_mean", "running_var"):
+                out[f"{p}.conv.1.{s}"] = (n,)
+        else:
+            nb, hid = shape
+            for d in ("", "_reverse"):
+                out[f"{p}.lstm.weight_ih_l0{d}"] = (4 * hid, nb)
+                out[f"{p}.lstm.weight_hh_l0{d}"] = (4 * hid, hid)
+                out[f"{p}.lstm.bias_ih_l0{d}"] = (4 * hid,)
+                out[f"{p}.lstm.bias_hh_l0{d}"] = (4 * hid,)
+            out[p + ".dense.0.weight"] = (nb, 2 * hid)
+            out[p + ".dense.0.bias"] = (nb,)
+            for s in ("weight", "bias", "running_mean", "running_var"):
+                out[f"{p}.dense.1.{s}"] = (nb,)
+    return out
+
+
+def infer_echo_config(sd):
+    """-> (nout, nout_lstm) of a nets_new.CascadedNet state_dict, read from stg1_low_band_net.0's enc1 (nout // 2 rows)
+    and LSTM (nout_lstm // 2 hidden units); ValueError if those keys are missing"""
+    k_enc = "stg1_low_band_net.0.enc1.conv.0.weight"
+    k_lstm = "stg1_low_band_net.0.lstm_dec2.lstm.weight_hh_l0"
+    if k_enc not in sd or k_lstm not in sd:
+        raise ValueError(f"not a DeEcho / DeReverb CascadedNet state_dict: no {k_enc if k_enc not in sd else k_lstm}")
+    return 2 * sd[k_enc].shape[0], 2 * sd[k_lstm].shape[1]
+
+
+class CascadedNet(_SpecNet):
+    """nets_new.CascadedNet(n_fft, nout, nout_lstm) of the DeEcho / DeReverb models in eval mode on CUDA.  Input
+    [B, 2, n_fft // 2 + 1, W] magnitudes (fp32).
+
+    Layout: the input x, aux1 and aux2 are slices of one [B, max_bin, W, Cx] buffer,
+    [x (2) | 0 0 | aux1 | 0.. | aux2 | 0..], so every stage input is a prefix of it whose width is a multiple of 4 (the
+    wgmma path); the weights get zero columns
+    for the pad channels, which are written as zeros.  A BaseNet's decoder inputs hold the encoder output (the skip) first
+    and the x2 upsample after it; dec1's input is [e1 | up(dec2) | up(lstm) | 0..].  LSTMModule: the 1x1 conv gives
+    [B, bins, frames] = [N][bins][T], evk_transpose_rows makes it [N][T][bins], one evk_gemm_tf32 the input projections of
+    both directions (biases summed at load), evk_lstm_bidir_fwd the recurrence, one evk_gemm_tf32 the dense layer with
+    BatchNorm1d folded in and ReLU, and evk_transpose_rows puts the result back as [N][bins][T], a one-channel image that
+    is upsampled into its dec1 channel.  Rows of the LSTM operands are in (n, t) order throughout."""
+
+    def __init__(self, n_fft, nout=32, nout_lstm=128):
+        if nout < 4:
+            raise ValueError(f"nout {nout} must be at least 4")
+        if nout_lstm != 128:
+            raise ValueError(f"nout_lstm {nout_lstm}: the recurrence kernel runs the hidden sizes of nout_lstm = 128 (64 and 32)")
+        super().__init__(n_fft, 64)
+        self.nout, self.nout_lstm = nout, nout_lstm
+        self.nin_lstm = self.max_bin // 2
+        q, h = nout // 4, nout // 2
+        # aux1 at [4, 4 + q), aux2 at [_a2, _a2 + h); stage 2 reads [0, _a2), stage 3 [0, _cx)
+        self._a2 = _round4(4 + q)
+        self._cx = _round4(self._a2 + h)
+        self._x_pads = [(2, 4), (4 + q, self._a2), (self._a2 + h, self._cx)]
+
+    # ---- weights -----------------------------------------------------------------------------------------
+    def _placements(self):
+        """-> {layer prefix: (input column of each reference input channel, input width)} for the layers whose input is
+        laid out differently from the reference's concatenation"""
+        q, h = self.nout // 4, self.nout // 2
+        x_cols = [0, 1]
+        stage_in = {"stg1_low_band_net.0": (x_cols, 4), "stg1_high_band_net": (x_cols, 4),
+                    "stg2_low_band_net.0": (x_cols + list(range(4, 4 + q)), self._a2),
+                    "stg2_high_band_net": (x_cols + list(range(4, 4 + q)), self._a2),
+                    "stg3_full_band_net": (x_cols + list(range(4, 4 + q)) + list(range(self._a2, self._a2 + h)), self._cx)}
+        out = {}
+        for p, cin in stage_in.items():
+            ch = {"stg1_low_band_net.0": h, "stg1_high_band_net": q, "stg2_low_band_net.0": self.nout,
+                  "stg2_high_band_net": h, "stg3_full_band_net": self.nout}[p]
+            out[p + ".enc1"] = cin
+            out[p + ".dec4.conv1"] = (_skip_first(8 * ch, 6 * ch), 14 * ch)
+            out[p + ".dec3.conv1"] = (_skip_first(6 * ch, 4 * ch), 10 * ch)
+            out[p + ".dec2.conv1"] = (_skip_first(4 * ch, 2 * ch), 6 * ch)
+            out[p + ".dec1.conv1"] = (_skip_first(2 * ch + 1, ch), _round4(3 * ch + 1))
+        return out
+
+    def load_state_dict(self, sd):
+        """Reference state_dict (fp16 or fp32 storage) -> folded, channels-last fp32 layers on self.device.  Keys ending in
+        num_batches_tracked are ignored; any other missing or unexpected key, or a wrong shape, raises ValueError."""
+        sd = {k: v for k, v in sd.items() if not k.endswith("num_batches_tracked")}
+        want = echo_state_dict_shapes(2 * self.max_bin, self.nout, self.nout_lstm)
+        tag = f"CascadedNet(n_fft={2 * self.max_bin}, nout={self.nout}, nout_lstm={self.nout_lstm})"
+        missing, unexpected = sorted(set(want) - set(sd)), sorted(set(sd) - set(want))
+        if missing or unexpected:
+            raise ValueError(f"state_dict does not match {tag}: missing {missing[:4]}, unexpected {unexpected[:4]}")
+        bad = [k for k, s in want.items() if tuple(sd[k].shape) != tuple(s)]
+        if bad:
+            raise ValueError(f"state_dict shapes do not match {tag}: {[(k, tuple(sd[k].shape)) for k in bad[:4]]}")
+        place = self._placements()
+        layers = {}
+        for p, (kind, shape) in echo_layer_spec(2 * self.max_bin, self.nout, self.nout_lstm).items():
+            if kind == "conv":
+                layers[p] = dict(w=sd[p + ".weight"].float().reshape(shape).contiguous())
+            elif kind == "cbr":
+                scale, bias = _fold_bn(sd, p + ".conv.1")
+                w = sd[p + ".conv.0.weight"]
+                if p in place:
+                    cols, C = place[p]
+                    wl = torch.zeros((w.shape[0], w.shape[2], w.shape[3], C), dtype=torch.float32)
+                    wl[..., cols] = w.float().permute(0, 2, 3, 1)
+                else:
+                    wl = _cl_weight(w)
+                layers[p] = dict(w=wl.contiguous(), scale=scale, bias=bias, k=shape[2])
+            else:
+                q = p + ".lstm."
+                d = ("", "_reverse")
+                w_ih = torch.cat([sd[q + "weight_ih_l0" + s].float() for s in d], 0)
+                b = torch.cat([(sd[q + "bias_ih_l0" + s].double() + sd[q + "bias_hh_l0" + s].double()).float() for s in d])
+                w_hh = torch.stack([sd[q + "weight_hh_l0" + s].float() for s in d])
+                bn = p + ".dense.1"
+                var, mean = sd[bn + ".running_var"].double(), sd[bn + ".running_mean"].double()
+                sc = sd[bn + ".weight"].double() / torch.sqrt(var + BN_EPS)
+                w_d = (sd[p + ".dense.0.weight"].double() * sc[:, None]).float()
+                b_d = ((sd[p + ".dense.0.bias"].double() - mean) * sc + sd[bn + ".bias"].double()).float()
+                layers[p] = dict(w_ih=w_ih.contiguous(), b=b, w_hh=w_hh.contiguous(), w_d=w_d.contiguous(), b_d=b_d)
+        self.layers = {p: {k: (v.to(self.device) if torch.is_tensor(v) else v) for k, v in L.items()}
+                       for p, L in layers.items()}
+        return self
+
+    @classmethod
+    def from_pretrained(cls, path, n_fft=1344, device="cuda"):
+        """Load a DeEcho / DeReverb .pth: nout and nout_lstm are read from the weight shapes (64 for DeReverb, 48 for the
+        DeEcho models).  Weights that do not form a CascadedNet at this n_fft raise ValueError."""
+        sd = torch.load(path, map_location="cpu", weights_only=True)
+        return cls(n_fft, *infer_echo_config(sd)).to(device).load_state_dict(sd)
+
+    # ---- forward -----------------------------------------------------------------------------------------
+    def forward(self, x):
+        """the mask [B, 2, output_bin, W] over all W frames (CascadedNet.forward in eval mode)"""
+        self.check_input(x, crop=False)
+        return self._run(x, torch.ones_like(x), 0)
+
+    __call__ = forward
+
+    def predict(self, x_mag, aggressiveness=None):
+        """x_mag * mask cropped by `offset` frames on both time edges: [B, 2, output_bin, W - 128].  `aggressiveness` is
+        accepted and ignored, as in the reference."""
+        self.check_input(x_mag, crop=True)
+        return self._run(x_mag, None, self.offset)
+
+    def _lstm(self, p, h: CLView):
+        """LSTMModule: dec2's output h [B, bins, T, 2 ch] -> [B, bins, T, 1]"""
+        L = self.layers[p]
+        B, nb, T = h.B, h.H, h.W
+        m = self._empty(B, nb, T, 1)
+        self._conv(p + ".conv", h, CLView(m))
+        g = ops.gemm_tf32(ops.transpose_rows(m.view(B, nb, T)).view(B * T, nb), L["w_ih"], bias=L["b"])
+        y = ops.lstm_bidir(g.view(B, T, -1), L["w_hh"], order="nt")
+        d = ops.gemm_tf32(y.view(B * T, -1), L["w_d"], bias=L["b_d"], act=ops.ACT_RELU)
+        out = self._empty(B, nb, T, 1)
+        ops.transpose_rows(d.view(B, T, nb), out=out.view(B, nb, T))
+        return out
+
+    def _aspp(self, p, x: CLView):
+        B, H, W, c = x.B, x.H, x.W, x.C
+        A = self._empty(B, H, W, 5 * c)
+        pooled = self._empty(B, 1, W, c)
+        self._conv(p + ".conv1.1", CLView(ops.mean_h(x)), CLView(pooled))
+        ops.resize_bilinear_ac(CLView(pooled), CLView(A, 0, c))
+        self._conv(p + ".conv2", x, CLView(A, c, c))
+        for j, d in enumerate(ECHO_DILATIONS):
+            self._conv(f"{p}.conv{3 + j}", x, CLView(A, (2 + j) * c, c), dil=d)
+        out = self._empty(B, H, W, c)
+        self._conv(p + ".bottleneck", CLView(A), CLView(out))
+        return out
+
+    def _base(self, p, x: CLView, out: CLView):
+        """BaseNet: x [B, H, W, nin] -> out [B, H, W, ch] (H, W multiples of 16)"""
+        B, H, W = x.B, x.H, x.W
+        ch = self.layers[p + ".enc1"]["w"].shape[0]
+        D1 = self._empty(B, H, W, _round4(3 * ch + 1))        # [e1 | up(dec2) | up(lstm) | 0..]
+        D1[..., 3 * ch + 1:].zero_()
+        self._conv(p + ".enc1", x, CLView(D1, 0, ch))
+        dec_in, h = [D1], CLView(D1, 0, ch)
+        for i, (cs, cu) in zip(range(2, 5), [(2 * ch, 4 * ch), (4 * ch, 6 * ch), (6 * ch, 8 * ch)]):
+            s = i - 1
+            t = self._empty(B, H >> s, W >> s, cs)
+            self._conv(f"{p}.enc{i}.conv1", h, CLView(t), stride=2, act=ops.C2_LRELU)
+            D = self._empty(B, H >> s, W >> s, cs + cu)          # [e_i | up(dec_{i+1})]
+            self._conv(f"{p}.enc{i}.conv2", CLView(t), CLView(D, 0, cs), act=ops.C2_LRELU)
+            dec_in.append(D)
+            h = CLView(D, 0, cs)
+        t = self._empty(B, H >> 4, W >> 4, 8 * ch)
+        self._conv(p + ".enc5.conv1", h, CLView(t), stride=2, act=ops.C2_LRELU)
+        e5 = self._empty(B, H >> 4, W >> 4, 8 * ch)
+        self._conv(p + ".enc5.conv2", CLView(t), CLView(e5), act=ops.C2_LRELU)
+        h = CLView(self._aspp(p + ".aspp", CLView(e5)))
+        for i in (4, 3, 2):
+            D = dec_in[i - 1]
+            cs = (2 * ch, 4 * ch, 6 * ch)[i - 2]
+            ops.resize_bilinear_ac(h, CLView(D, cs))
+            y = self._empty(B, H >> (i - 1), W >> (i - 1), self.layers[f"{p}.dec{i}.conv1"]["w"].shape[0])
+            self._conv(f"{p}.dec{i}.conv1", CLView(D), CLView(y))
+            h = CLView(y)
+        lstm = self._lstm(p + ".lstm_dec2", h)
+        ops.resize_bilinear_ac(h, CLView(D1, ch, 2 * ch))
+        ops.resize_bilinear_ac(CLView(lstm), CLView(D1, 3 * ch, 1))
+        self._conv(p + ".dec1.conv1", CLView(D1), out)
+
+    def _run(self, x, mix, offset):
+        """mask * mix (x when mix is None), cropped by offset frames"""
+        x = x.detach().float().contiguous()
+        B, _, _, W = x.shape
+        mb, bw = self.max_bin, self.max_bin // 2
+        q, h, a2 = self.nout // 4, self.nout // 2, self._a2
+        X = self._empty(B, mb, W, self._cx)                     # [x | 0 0 | aux1 | 0.. | aux2 | 0..]
+        X[..., :2].copy_(x[:, :, :mb].permute(0, 2, 3, 1))
+        for c0, c1 in self._x_pads:
+            X[..., c0:c1].zero_()
+        t = self._empty(B, bw, W, h)
+        self._base("stg1_low_band_net.0", CLView(X, 0, 4, 0, bw), CLView(t))
+        self._conv("stg1_low_band_net.1", CLView(t), CLView(X, 4, q, 0, bw))
+        self._base("stg1_high_band_net", CLView(X, 0, 4, bw, bw), CLView(X, 4, q, bw, bw))
+        t = self._empty(B, bw, W, self.nout)
+        self._base("stg2_low_band_net.0", CLView(X, 0, a2, 0, bw), CLView(t))
+        self._conv("stg2_low_band_net.1", CLView(t), CLView(X, a2, h, 0, bw))
+        self._base("stg2_high_band_net", CLView(X, 0, a2, bw, bw), CLView(X, a2, h, bw, bw))
+        del t
+        f3 = self._empty(B, mb, W, self.nout)
+        self._base("stg3_full_band_net", CLView(X), CLView(f3))
+        del X
+        return ops.vr_mask_head(CLView(f3), self.layers["out"]["w"], x if mix is None else mix.detach().float().contiguous(),
+                                offset)
 
 
 def make_padding(width, crop_size, offset):

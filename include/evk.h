@@ -460,8 +460,9 @@ int evk_attn_pad_fwd(const float* q, const float* k, const float* v, int32_t ld,
                      int32_t H, int32_t L, const int64_t* lens, float scale, evk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * UVR5 VR vocal separation (CascadedASPPNet, uvr5.py), inference only.  Activations are channels-last fp32: pixel (b, y, x)
- * of an operand starts at  p + b*bs + (y*W + x)*pitch  (floats), so a channel slice of a concat buffer is an operand.
+ * UVR5 VR separation (CascadedASPPNet and the DeEcho / DeReverb CascadedNet, uvr5.py), inference only.  Activations are
+ * channels-last fp32: pixel (b, y, x) of an operand starts at  p + b*bs + (y*W + x)*pitch  (floats), so a channel slice of
+ * a concat buffer is an operand.
  * ------------------------------------------------------------------------------------------ */
 enum evk_conv2d_act { EVK_C2_NONE = 0, EVK_C2_RELU = 1, EVK_C2_LRELU = 2 /* slope 0.01 */, EVK_C2_SIGMOID = 3 };
 /* y = act(conv2d(x, w) * scale[n] + bias[n])  (scale / bias may be null: 1 / 0).  x: [B, H, W, C] (pitch x_pitch >= C,
@@ -473,6 +474,13 @@ enum evk_conv2d_act { EVK_C2_NONE = 0, EVK_C2_RELU = 1, EVK_C2_LRELU = 2 /* slop
 int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale, const float* bias,
                    float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W, int32_t C, int32_t N, int32_t k,
                    int32_t stride, int32_t pad, int32_t dil, int32_t act, evk_stream_t stream);
+/* evk_conv2d_fwd with zero padding and dilation per axis (the DeEcho / DeReverb ASPP: dilation (4, 2), (8, 4), (12, 6)):
+ * Ho = (H + 2 pad_h - dil_h (k - 1) - 1) / stride + 1, Wo likewise with pad_w, dil_w.  Same kernels, dispatch and
+ * guarantees; evk_conv2d_fwd(..., pad, dil, ...) is this call with pad_h = pad_w = pad, dil_h = dil_w = dil. */
+int evk_conv2d_fwd_hw(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale, const float* bias,
+                      float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W, int32_t C, int32_t N,
+                      int32_t k, int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h, int32_t dil_w, int32_t act,
+                      evk_stream_t stream);
 /* Depthwise 3x3, stride 1, zero padding = dil: y[b,y,x,c] = sum_{i,j} w[c][i][j] x[b, y + (i-1) dil, x + (j-1) dil, c]
  * (fp32 FMA).  w: [C][3][3]. */
 int evk_dwconv3x3_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, float* y, int32_t y_pitch,
@@ -493,6 +501,15 @@ int evk_mean_h(const float* x, int32_t x_pitch, int64_t x_bs, float* y, int32_t 
 int evk_vr_mask_head(const float* h, int32_t h_pitch, int64_t h_bs, const float* w, int32_t Ch, const float* mix,
                      float* out, int32_t B, int32_t max_bin, int32_t out_bin, int32_t W, int32_t offset, int32_t split_bin,
                      float e_lo, float e_hi, int32_t use_agg, evk_stream_t stream);
+/* Recurrence of a bidirectional one-layer nn.LSTM (gate order i, f, g, o; zero initial h and c), inference only.
+ * g: the input projections with both biases added, row (t, n) at g + t*g_st + n*g_sn holding 8H floats
+ * [direction][gate][H] (direction 0 forward, 1 reverse); w_hh: [2][4H][H] (weight_hh_l0, weight_hh_l0_reverse);
+ * y: row (t, n) at y + t*y_st + n*y_sn receives [h_forward(t) | h_reverse(t)] (2H floats).  Strides are in floats, so
+ * (t, n) and (n, t) row orders both work.  H = 32 or 64 (EVK_ERR_ARG otherwise).  One persistent launch, W_hh held
+ * on chip; exact fp32 FMAs, accurate expf / tanhf, no atomics: bit-reproducible, and a row's result does not depend on
+ * the other rows of the batch. */
+int evk_lstm_bidir_fwd(const float* g, int64_t g_st, int64_t g_sn, const float* w_hh, float* y, int64_t y_st, int64_t y_sn,
+                       int32_t T, int32_t N, int32_t H, evk_stream_t stream);
 
 #ifdef __cplusplus
 }

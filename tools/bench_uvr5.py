@@ -6,7 +6,13 @@ frames, 673 bins, the default 61968 net with seeded weights), and on the same GP
   * fp32 with TF32 convolutions allowed.
 Also the rate of evk_conv2d_fwd on the decoder shapes of the 61968 net at 16 windows per launch.  Prints one JSON line.
 
-Usage:  python tools/bench_uvr5.py [--frames 16538] [--tta 0] [--max-windows 16] [--reps 3]
+--net deecho / dereverb measures the DeEcho (nout 48) / DeReverb (nout 64) CascadedNet on the same spectrogram instead
+(44 windows at roi 384): uvr5.inference with and without TTA, peak device memory, the time split of one predict between
+the convolutions and the LSTM, the stg3 LSTM recurrence alone, and the reference's algorithm on stock PyTorch
+(oracle/uvr5_echo_oracle.py's predict with cuDNN convolutions and LSTM, one window per call with a host copy, TTA off) in
+fp16 and in fp32 with TF32 allowed.
+
+Usage:  python tools/bench_uvr5.py [--net vr|deecho|dereverb] [--frames 16538] [--tta 0] [--max-windows 16] [--reps 3]
 """
 import argparse
 import json
@@ -21,6 +27,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from oracle import uvr5_echo_oracle as E  # noqa: E402
 from oracle import uvr5_oracle as O  # noqa: E402
 
 
@@ -92,14 +99,116 @@ def decoder_rates(ops, B, reps=20):
     return out
 
 
+def torch_echo_inference(P, lstms, spec, half):
+    """SeparateVREcho.inference's window loop on stock PyTorch (cuDNN convolutions and LSTM): one window per predict,
+    copied to the host after each, TTA off"""
+    dev = torch.device("cuda")
+    x_mag = np.abs(spec)
+    x_phase = np.angle(spec)
+    coef = x_mag.max()
+    x_pre = x_mag / coef
+    n = x_pre.shape[2]
+    l, r, roi = E.make_padding(n, 512, E.OFFSET)
+    xp = np.pad(x_pre, ((0, 0), (0, 0), (l, r)))
+    out = []
+    with torch.no_grad():
+        for i in range(int(np.ceil(n / roi))):
+            w = torch.from_numpy(xp[None, :, :, i * roi: i * roi + 512])
+            w = (w.half() if half else w).to(dev)
+            out.append(E.predict(P, w, None, 1344, lstms)[0].float().cpu().numpy())
+    return np.concatenate(out, 2)[:, :, :n] * coef, x_mag, np.exp(1.0j * x_phase)
+
+
+def lstm_alone(ops, reps=20):
+    """CUDA-event ms of the stg3 LSTMModule pieces at N = 16 windows, T = 256, I = 336, H = 64: the recurrence alone, and
+    the two projection GEMMs around it"""
+    N, T, I, H = 16, 256, 336, 64
+    x = torch.randn(N * T, I, device="cuda")
+    w_ih, b = torch.randn(8 * H, I, device="cuda") / I ** 0.5, torch.randn(8 * H, device="cuda") * 0.1
+    w_hh = (torch.rand(2, 4 * H, H, device="cuda") * 2 - 1) / H ** 0.5
+    w_d, b_d = torch.randn(I, 2 * H, device="cuda") / (2 * H) ** 0.5, torch.randn(I, device="cuda") * 0.1
+    g = ops.gemm_tf32(x, w_ih, bias=b).view(N, T, 8 * H)
+    y = ops.lstm_bidir(g, w_hh, order="nt")
+    out = {}
+    for name, fn in (("recurrence_ms", lambda: ops.lstm_bidir(g, w_hh, order="nt")),
+                     ("projections_ms", lambda: (ops.gemm_tf32(x, w_ih, bias=b),
+                                                 ops.gemm_tf32(y.view(N * T, 2 * H), w_d, bias=b_d, act=ops.ACT_RELU)))):
+        fn()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        out[name] = round(e0.elapsed_time(e1) / reps, 4)
+    return out
+
+
+def echo_main(a):
+    """--net deecho / dereverb: the DeEcho (nout 48) or DeReverb (nout 64) CascadedNet at n_fft 1344"""
+    assert torch.cuda.is_available(), "needs a GPU"
+    from easevoice_trainer_b200 import lib, ops, uvr5
+    lib.init().evk_set_precise(0)
+    nout = 48 if a.net == "deecho" else 64
+    P = E.init_params(E.param_spec(1344, nout), 51)
+    net = uvr5.CascadedNet(1344, nout).to("cuda").load_state_dict(P)
+    spec = E.make_spec(7, 673, a.frames)
+    roi = 512 - 2 * net.offset
+    n_win = int(np.ceil(a.frames / roi))
+    res = dict(gpu=gpu_info(), net=a.net, nout=nout, frames=a.frames, windows=n_win, windows_tta=2 * n_win + 1,
+               max_windows=a.max_windows)
+    t = time.perf_counter()
+    uvr5.inference(spec, "cuda", net, None, {"window_size": 512, "tta": False}, a.max_windows)   # allocator warm-up
+    res["evk_first_call_s"] = round(time.perf_counter() - t, 3)
+    for tta in (False, True):
+        data = {"window_size": 512, "tta": tta}
+        torch.cuda.reset_peak_memory_stats()
+        ts = timed(lambda: uvr5.inference(spec, "cuda", net, None, data, a.max_windows), a.reps)
+        res["evk_tta_s" if tta else "evk_s"] = [round(t, 3) for t in ts]
+        res["peak_mem_gib_tta" if tta else "peak_mem_gib"] = round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)
+    ops.profile_begin()
+    net.predict(torch.rand(a.max_windows, 2, 673, 512, device="cuda"))
+    prof = ops.profile_end()
+    tot = sum(v["ms"] for v in prof.values())
+    conv = [v for k, v in prof.items() if k.startswith("evk_conv2d_fwd")]
+    conv_ms, conv_fl = sum(v["ms"] for v in conv), sum(v["flops"] for v in conv)
+    lstm_ms = prof.get("evk_lstm_bidir_fwd", dict(ms=0.0))["ms"]
+    gemm_ms = sum(v["ms"] for k, v in prof.items() if k.startswith("evk_gemm_tf32"))
+    res["predict_ms_by_family"] = {k: round(v["ms"], 2) for k, v in sorted(prof.items(), key=lambda kv: -kv[1]["ms"])}
+    res["window_gflop_conv"] = round(conv_fl / a.max_windows / 1e9, 1)
+    res["predict_split"] = dict(conv2d=round(conv_ms / tot, 3), lstm_recurrence=round(lstm_ms / tot, 4),
+                                lstm_gemms=round(gemm_ms / tot, 4))
+    res["conv2d_tflops_in_predict"] = round(conv_fl / conv_ms / 1e9, 1)
+    res["lstm_stg3_alone"] = lstm_alone(ops)
+    pred = uvr5.inference(spec, "cuda", net, None, {"window_size": 512, "tta": False}, a.max_windows)[0]
+
+    if not a.skip_torch:
+        torch.backends.cudnn.benchmark = True
+        torch.backends.cudnn.allow_tf32 = True
+        torch.backends.cuda.matmul.allow_tf32 = True
+        for name, half in (("torch_fp16", True), ("torch_tf32", False)):
+            dt = torch.float16 if half else torch.float32
+            Pd = {k: (v.to(dt) if v.is_floating_point() else v).to("cuda") for k, v in P.items()}
+            lstms = E.lstm_modules(Pd, "cuda", dt)
+            torch_echo_inference(Pd, lstms, E.make_spec(1, 673, 600), half)             # warm-up (cuDNN algorithm choice)
+            ts = timed(lambda: torch_echo_inference(Pd, lstms, spec, half), a.reps)
+            res[name + "_s"] = [round(t, 3) for t in ts]
+            ref = torch_echo_inference(Pd, lstms, spec, half)[0]
+            res[name + "_rel_l2_vs_evk"] = float(np.linalg.norm(ref - pred) / np.linalg.norm(ref))
+    print(json.dumps(res))
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--net", choices=("vr", "deecho", "dereverb"), default="vr")
     ap.add_argument("--frames", type=int, default=16538)
     ap.add_argument("--tta", type=int, default=0)
     ap.add_argument("--max-windows", type=int, default=16)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--skip-torch", action="store_true")
     a = ap.parse_args()
+    if a.net != "vr":
+        return echo_main(a)
     assert torch.cuda.is_available(), "needs a GPU"
     from easevoice_trainer_b200 import lib, ops, uvr5
     lib.init().evk_set_precise(0)
