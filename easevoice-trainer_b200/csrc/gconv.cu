@@ -35,6 +35,7 @@ __device__ __forceinline__ float apply_act(float v, int act, float slope) {
   if (act == EVK_ACT_LRELU) return v > 0.f ? v : v * slope;
   if (act == EVK_ACT_RELU) return fmaxf(v, 0.f);
   if (act == EVK_ACT_TANH) return tanhf(v);
+  if (act == EVK_ACT_GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
   return v;
 }
 

@@ -151,6 +151,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gconv_tc_kernel(const __grid_co
             if (p.act == EVK_ACT_LRELU) t = t > 0.f ? t : t * p.slope;
             else if (p.act == EVK_ACT_RELU) t = fmaxf(t, 0.f);
             else if (p.act == EVK_ACT_TANH) t = tanhf(t);
+            else if (p.act == EVK_ACT_GELU) t = 0.5f * t * (1.f + erff(t * 0.70710678118654752f));
             v[e] = live ? t : 0.f;
           }
         }

@@ -178,6 +178,7 @@ __device__ __forceinline__ void epi_chunk(const GemmP& p, const float* __restric
       if (p.act == EVK_ACT_LRELU) t[e] = t[e] > 0.f ? t[e] : t[e] * p.slope;
       else if (p.act == EVK_ACT_RELU) t[e] = fmaxf(t[e], 0.f);
       else if (p.act == EVK_ACT_TANH) t[e] = tanhf(t[e]);
+      else if (p.act == EVK_ACT_GELU) t[e] = 0.5f * t[e] * (1.f + erff(t[e] * 0.70710678118654752f));
       if (!keep[i]) t[e] = 0.f;
     }
     if (dropk.thr) {                                     // group index = offset of the float4 in the output tensor / 4

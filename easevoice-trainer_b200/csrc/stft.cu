@@ -203,6 +203,67 @@ __global__ void __launch_bounds__(256) cplx_l1_kernel(const float2* __restrict__
   if (threadIdx.x == 0) loss[blockIdx.x] = tot * scale;      // per-block partial (ordered_sum adds them)
 }
 
+// Inverse STFT (torch.istft(center=True, normalized=False, onesided, length=None) with the Hann(n_fft) window), optionally of
+// stft * mask (bs_roformer.py:530-543): one block per frame (row r = b S + s, frame t) runs the C2R inverse DFT through the same
+// adjoint packing and forward FFT as stft_bwd_kernel (bins 0 and N/2 lose their imaginary parts), windows the frame and writes it
+// to work [(r T + t)][N]; istft_ola_kernel then overlap-adds the frames in frame order and divides by the sum of w^2.
+struct IstftP {
+  const float2* cplx; const float* mask; int ldm;
+  int S, T, N, hop;
+  float* work; float* out; int ldo; int Lout;
+};
+
+__global__ void __launch_bounds__(ST_THREADS) istft_frame_kernel(const IstftP p) {
+  extern __shared__ __align__(16) uint8_t ssm[];
+  const int NH = p.N >> 1, NB = NH + 1;
+  float2* d0 = reinterpret_cast<float2*>(ssm);
+  float2* d1 = d0 + NH;
+  float2* G = d1 + NH;
+  const long long frame = blockIdx.x;
+  const int r = (int)(frame / p.T), t = (int)(frame - (long long)r * p.T);
+  const int b = r / p.S, s = r - b * p.S;
+  const int tid = threadIdx.x;
+  const float inv = 1.f / (float)p.N;
+  for (int k = tid; k < NB; k += ST_THREADS) {
+    float2 x = p.cplx[frame * NB + k];
+    if (p.mask) {           // mask row (b, t), column ((k S + s), c): the mask estimator's 'b t (f s c)' layout
+      const float2 m = *reinterpret_cast<const float2*>(p.mask + ((long long)b * p.T + t) * p.ldm + 2 * (k * p.S + s));
+      x = stft_cmul(x, m);
+    }
+    const float sc = (k == 0 || k == NH) ? inv : 2.f * inv;  // irfft(X)[n] = sum_k Re(G[k] e^{2 pi i k n / N}) with these weights
+    G[k] = make_float2(x.x * sc, x.y * sc);
+  }
+  __syncthreads();
+  stft_adjoint_pack_phase(tid, ST_THREADS, p.N, G, g_stw, d0);
+  __syncthreads();
+  const float2* z = run_fft(NH, d0, d1);
+  float* fr = p.work + frame * p.N;
+  for (int m = tid; m < NH; m += ST_THREADS) {
+    const float2 v = z[m];
+    fr[2 * m] = v.x * stft_window(g_shann, 2 * m, p.N, p.N);
+    fr[2 * m + 1] = -v.y * stft_window(g_shann, 2 * m + 1, p.N, p.N);
+  }
+}
+
+// out[r][n] = sum_f frame_f[q - f hop] / sum_f w(q - f hop)^2 over the frames covering q = n + N/2 (ascending f)
+__global__ void istft_ola_kernel(const IstftP p) {
+  const int r = blockIdx.y;
+  for (long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x; n < p.Lout; n += (long long)gridDim.x * blockDim.x) {
+    const int q = (int)n + (p.N >> 1);
+    int lo = q - p.N + 1;
+    lo = lo <= 0 ? 0 : (lo + p.hop - 1) / p.hop;
+    const int hi = min(q / p.hop, p.T - 1);
+    float y = 0.f, env = 0.f;
+    for (int f = lo; f <= hi; ++f) {
+      const int j = q - f * p.hop;
+      const float w = stft_window(g_shann, j, p.N, p.N);
+      y += p.work[((long long)r * p.T + f) * p.N + j];
+      env += w * w;
+    }
+    p.out[(long long)r * p.ldo + n] = y / env;
+  }
+}
+
 int fill(StftP& p, const float* wav, const int32_t* lens, int B, int L, int ldw, int n_fft, int hop, int win, int pad, int T) {
   EVK_REQUIRE(B > 0 && L > 0 && T > 0 && hop > 0 && pad >= 0 && ldw >= L, EVK_ERR_ARG, "stft: bad sizes B=%d L=%d T=%d hop=%d pad=%d", B, L, T, hop, pad);
   EVK_REQUIRE(n_fft >= 256 && n_fft <= STFT_TAB && (n_fft & (n_fft - 1)) == 0, EVK_ERR_UNSUPPORTED, "stft: n_fft=%d must be a power of two in [256, 4096]", n_fft);
@@ -278,6 +339,33 @@ extern "C" int evk_stft_bwd(const float* gcplx, const float* dmel, int32_t ld_dm
   const long long blocks = (total + 255) / 256;
   stft_ola_kernel<<<(unsigned)(blocks < kNumSMs * 16 ? blocks : kNumSMs * 16), 256, 0, (cudaStream_t)stream>>>(p);
   return check_launch("stft_ola_kernel");
+}
+
+extern "C" int evk_istft(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft,
+                         int32_t hop, float* work, float* out, int32_t ld_out, evk_stream_t stream) {
+  EVK_REQUIRE(cplx && work && out, EVK_ERR_ARG, "istft: null tensor");
+  EVK_REQUIRE(n_fft >= 256 && n_fft <= STFT_TAB && (n_fft & (n_fft - 1)) == 0, EVK_ERR_UNSUPPORTED, "istft: n_fft=%d must be a power of two in [256, 4096]", n_fft);
+  EVK_REQUIRE(B > 0 && S > 0 && T >= 2 && hop > 0 && hop <= n_fft / 2 && (long long)B * S <= 65535, EVK_ERR_ARG,
+              "istft: bad sizes B=%d S=%d T=%d hop=%d", B, S, T, hop);
+  EVK_REQUIRE(!mask || (ld_mask >= 2 * S * (n_fft / 2 + 1) && (uintptr_t)mask % 8 == 0 && ld_mask % 2 == 0), EVK_ERR_ARG,
+              "istft: mask rows must hold 2 * S * (n_fft / 2 + 1) floats, 8-byte aligned");
+  const long long Lout = (long long)hop * (T - 1), frames = (long long)B * S * T;
+  EVK_REQUIRE(ld_out >= Lout && frames <= 0x7fffffff && Lout <= 0x7fffffff, EVK_ERR_ARG, "istft: output pitch %d < %lld", ld_out, Lout);
+  if (int rc = stft_init_tables()) return rc;
+  IstftP p{reinterpret_cast<const float2*>(cplx), mask, ld_mask, S, T, n_fft, hop, work, out, ld_out, (int)Lout};
+  const size_t smem = (size_t)(n_fft / 2) * 16 + (size_t)(n_fft / 2 + 1) * 8;
+  static size_t attr = 48 * 1024;
+  if (smem > attr) {
+    if (cudaFuncSetAttribute(istft_frame_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+      return check_launch("istft_frame_kernel");
+    attr = smem;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  istft_frame_kernel<<<(unsigned)frames, ST_THREADS, smem, st>>>(p);
+  if (int rc = check_launch("istft_frame_kernel")) return rc;
+  const long long bx = (Lout + 255) / 256;
+  istft_ola_kernel<<<dim3((unsigned)(bx < 1024 ? bx : 1024), (unsigned)(B * S)), 256, 0, st>>>(p);
+  return check_launch("istft_ola_kernel");
 }
 
 // loss[0] += scale * sum |a - b| over n complex elements; grad (nullable) = scale * (a - b) / |a - b|

@@ -15,6 +15,7 @@ import torch
 from . import lib as L
 
 ACT_NONE, ACT_LRELU, ACT_RELU, ACT_TANH = 0, 1, 2, 3
+ACT_GELU = 4             # exact erf GELU in the GEMM epilogue (forward only)
 USE_TMA_STRIDED = True   # strided conv forward: phase-split input + stride-1 multi-source tap sum on the TMA kernel
 USE_TMA_WGRAD = True     # weight gradients of tap-free layers: transposes + split-K TMA/wgmma GEMM
 UN_SCALE, UN_LRELU, UN_TANH, UN_MISH, UN_RELU, UN_TANH_FROM_OUT, UN_GELU = 0, 1, 2, 3, 4, 5, 6
@@ -2150,3 +2151,70 @@ def lstm_bidir(g, w_hh, order="tn"):
         gs, ys = gs[::-1], ys[::-1]
     _call_f("evk_lstm_bidir_fwd", 2.0 * 2 * T * N * 4 * H * H, _p(g), *gs, _p(w_hh), _p(y), *ys, T, N, H)
     return y
+
+
+# ------------------------------------------------------------------------------------------------
+# BS-Roformer (bs_roformer.py): rotary gated attention, band input, row L2 norm, inverse STFT
+# ------------------------------------------------------------------------------------------------
+def linear_into(x, w: PackedW, y, bias=None, act=ACT_NONE, res=None):
+    """y = act(x W^T + bias + res) written into y (no autograd): x [rows, C] and y [rows, N] are 2-D views with unit column
+    stride and any row pitch (column slices of wider buffers), res [rows, N] contiguous or None."""
+    rows, C = x.shape
+    N = w.D0
+    assert w.Q == 1 and y.shape == (rows, N) and C <= w.pa.shape[2], (x.shape, y.shape, w.pa.shape)
+    _fwd_like(x.unsqueeze(0), rows, w.pa, 0, 1, 1, w.pa.shape[2], N * w.pa.shape[2], C, N, y.unsqueeze(0), J=rows, P=1, is_=1,
+              os_=1, o0=0, Tout=rows, off=[0], bias=bias, res=res.unsqueeze(0) if res is not None else None, act=act)
+    return y
+
+
+def rope_attn(qkvg, cs, out, heads, L, n_outer, s_outer, n_inner, s_inner, s_tok):
+    """evk_rope_attn_fwd: qkvg [rows, ld] token rows [q | k | v | gate logits], cs [L, 32, 2] (cos, sin) -> out [rows, heads*64];
+    sequence (u, w) holds rows u*s_outer + w*s_inner + t*s_tok, t < L."""
+    assert qkvg.dim() == 2 and qkvg.stride(1) == 1 and out.dim() == 2 and out.stride(1) == 1 and cs.is_contiguous()
+    assert cs.shape[0] >= L
+    _call_f("evk_rope_attn_fwd", 4.0 * n_outer * n_inner * heads * L * L * 64, _p(qkvg), qkvg.stride(0), _p(cs), _p(out),
+            out.stride(0), heads, L, n_outer, s_outer, n_inner, s_inner, s_tok)
+    return out
+
+
+def row_l2norm(x, out=None):
+    """x / max(||x||_2, 1e-12) per row of a [rows, C] view (evk_row_l2norm)"""
+    rows, C = x.shape
+    assert x.stride(1) == 1
+    out = torch.empty((rows, C), device=x.device, dtype=torch.float32) if out is None else out
+    _call("evk_row_l2norm", _p(x), x.stride(0), _p(out), out.stride(0), rows, C)
+    return out
+
+
+def bs_band_input(cplx, B, S, band_off, out):
+    """evk_bs_band_input: cplx [B*S, T, n_bins, 2] (ops.stft) -> out [B*T, >= 2*S*n_bins] in 'b t (f s c)' order, each band's
+    segment L2-normalised; band_off int32 device [n_bands + 1] bin offsets."""
+    _, T, nb, _ = cplx.shape
+    assert cplx.is_contiguous() and out.stride(1) == 1 and band_off.dtype == torch.int32
+    _call("evk_bs_band_input", _p(cplx), B, S, T, nb, _p(band_off), band_off.numel() - 1, _p(out), out.stride(0))
+    return out
+
+
+def istft(cplx, B, S, n_fft, hop, mask=None, out=None, work=None):
+    """torch.istft(center=True, Hann(n_fft)) of cplx [B*S, T, n_fft/2+1, 2] (times the complex mask [B*T, (f s c)] when given)
+    -> [B*S, hop*(T-1)] (evk_istft).  work: scratch of B*S*T*n_fft floats (allocated when None)."""
+    T = cplx.shape[1]
+    assert cplx.is_contiguous() and cplx.shape[2] == n_fft // 2 + 1
+    if out is None:
+        out = torch.empty((B * S, hop * (T - 1)), device=cplx.device, dtype=torch.float32)
+    if work is None:
+        work = torch.empty(B * S * T * n_fft, device=cplx.device, dtype=torch.float32)
+    assert work.numel() >= B * S * T * n_fft and out.stride(1) == 1
+    if mask is not None:
+        assert mask.stride(1) == 1 and mask.shape[0] == B * T
+    _call("evk_istft", _p(cplx), _p(mask), mask.stride(0) if mask is not None else 0, B, S, T, n_fft, hop, _p(work), _p(out),
+          out.stride(0))
+    return out
+
+
+def glu_into(h, out):
+    """nn.GLU(dim=-1) of h [rows, 2C] written into out [rows, C] (a view with unit column stride; evk_glu_res with x = NULL)"""
+    rows, C2 = h.shape
+    assert h.stride(1) == 1 and out.stride(1) == 1 and out.shape == (rows, C2 // 2)
+    _call("evk_glu_res", None, 0, _p(h), h.stride(0), _p(out), out.stride(0), rows, C2 // 2)
+    return out

@@ -26,7 +26,8 @@ extern "C" {
 typedef struct CUstream_st* evk_stream_t;
 
 enum evk_status { EVK_OK = 0, EVK_ERR_ARG = -1, EVK_ERR_CUDA = -2, EVK_ERR_ARCH = -3, EVK_ERR_UNSUPPORTED = -4 };
-enum evk_act { EVK_ACT_NONE = 0, EVK_ACT_LRELU = 1, EVK_ACT_RELU = 2, EVK_ACT_TANH = 3 };
+/* EVK_ACT_GELU: exact erf form, x * 0.5 * (1 + erf(x / sqrt(2))) (nn.GELU()); forward epilogues only. */
+enum evk_act { EVK_ACT_NONE = 0, EVK_ACT_LRELU = 1, EVK_ACT_RELU = 2, EVK_ACT_TANH = 3, EVK_ACT_GELU = 4 };
 
 #define EVK_MAX_TAPS 48
 
@@ -510,6 +511,42 @@ int evk_vr_mask_head(const float* h, int32_t h_pitch, int64_t h_bs, const float*
  * the other rows of the batch. */
 int evk_lstm_bidir_fwd(const float* g, int64_t g_st, int64_t g_sn, const float* w_hh, float* y, int64_t y_st, int64_t y_sn,
                        int32_t T, int32_t N, int32_t H, evk_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * UVR5 BS-Roformer separation (BSRoformer, bs_roformer.py), inference only.  Linear layers run on evk_gconv_fwd, the mask
+ * estimator's GLU on evk_glu_res, the forward STFT on evk_stft_fwd.
+ * ------------------------------------------------------------------------------------------ */
+/* Fused axial self-attention with rotary embedding and per-head gates, head dim 64, no mask (Attention.forward of
+ * bs_roformer.py:106-121 from the QKV output to just before to_out).  A token row of qkvg (pitch ld floats) is
+ * [q (H*64) | k (H*64) | v (H*64) | gate logits (H)] (to_qkv and to_gates as one Linear).  q and k are rotated at their
+ * position p = 0 .. L-1 in the sequence with interleaved pairs, out[2i] = x[2i] cos - x[2i+1] sin and out[2i+1] =
+ * x[2i+1] cos + x[2i] sin, where cs [L][32][2] holds (cos, sin) of the angle p * theta_i; then
+ *   o = softmax(q k^T / 8) v * sigmoid(gate_h),  written as [h*64 + d] of the token's row of o (pitch ldo).
+ * Sequences: n = (u, w), u < n_outer, w < n_inner; token t of sequence n is row u*s_outer + w*s_inner + t*s_tok of both
+ * qkvg and o (strides in rows).  [B, T, F, C] activations: time axis n_outer = B, s_outer = T*F, n_inner = F, s_inner = 1,
+ * s_tok = F; frequency axis n_outer = B*T, s_outer = F, n_inner = 1, s_inner = 0, s_tok = 1.  Any L >= 1 (online softmax
+ * over 32-key tiles).  ld % 4 == 0, ldo % 2 == 0; qkvg 16-byte, o and cs 8-byte aligned.  TF32 mma.sync with fp32
+ * accumulation (3xTF32 under evk_set_precise(1)); no atomics, bit-reproducible. */
+int evk_rope_attn_fwd(const float* qkvg, int32_t ld, const float* cs, float* o, int32_t ldo, int32_t H, int32_t L,
+                      int32_t n_outer, int64_t s_outer, int32_t n_inner, int64_t s_inner, int64_t s_tok, evk_stream_t stream);
+/* Inverse of evk_stft_fwd's center=True transform with the periodic Hann(n_fft) window: torch.istft(n_fft, hop, n_fft, hann,
+ * center=True, normalized=False, onesided=True, length=None) of cplx [B*S*T][n_fft/2+1][2] (rows b*S + s), times mask when
+ * given (bs_roformer.py:530-543): bin k of row (b, s), frame t is multiplied by the complex mask at columns
+ * 2 (k S + s) .. +1 of mask row b*T + t (pitch ld_mask: the mask estimator's 'b t (f s c)' layout).  Per frame a C2R inverse
+ * DFT (imaginary parts of bins 0 and n_fft/2 ignored) and the window, written to work [B*S*T][n_fft]; then the overlap-add in
+ * frame order, divided by the sum of squared windows, trimmed by n_fft/2 at both ends: out [B*S][ld_out] gets hop*(T-1)
+ * samples per row.  n_fft a power of two in [256, 4096], T >= 2, hop <= n_fft / 2, B*S <= 65535. */
+int evk_istft(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft, int32_t hop,
+              float* work, float* out, int32_t ld_out, evk_stream_t stream);
+/* Band-split operand (bs_roformer.py:481-490 and each band's RMSNorm before its Linear): from evk_stft_fwd's cplx
+ * [B*S*T][n_bins][2] (rows b*S + s) to y [B*T][ld_y], row (b, t), column (f S + s) * 2 + c ('b t (f s c)'), with the columns
+ * [2 S band_off[i], 2 S band_off[i+1]) of band i divided by max(their L2 norm, 1e-12).  band_off: device int32
+ * [n_bands + 1] bin offsets (band_off[n_bands] = n_bins).  S = 1 or 2; 2 S n_bins floats must fit 48 KB. */
+int evk_bs_band_input(const float* cplx, int32_t B, int32_t S, int32_t T, int32_t n_bins, const int32_t* band_off,
+                      int32_t n_bands, float* y, int32_t ldy, evk_stream_t stream);
+/* y[r] = x[r] / max(||x[r]||_2, 1e-12) per row (F.normalize(dim=-1): the RMSNorms, whose gamma * sqrt(dim) the caller folds
+ * into the next Linear's weight columns). */
+int evk_row_l2norm(const float* x, int32_t ldx, float* y, int32_t ldy, int64_t rows, int32_t C, evk_stream_t stream);
 
 #ifdef __cplusplus
 }

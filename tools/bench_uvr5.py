@@ -12,7 +12,17 @@ the convolutions and the LSTM, the stg3 LSTM recurrence alone, and the reference
 (oracle/uvr5_echo_oracle.py's predict with cuDNN convolutions and LSTM, one window per call with a host copy, TTA off) in
 fp16 and in fp32 with TF32 allowed.
 
-Usage:  python tools/bench_uvr5.py [--net vr|deecho|dereverb] [--frames 16538] [--tta 0] [--max-windows 16] [--reps 3]
+--net roformer measures the BS-Roformer (bs_roformer.py, the shipped SeparateMDXC config with seeded weights) on a 3-minute
+stereo mix at 44.1 kHz (7 938 000 samples, 23 chunks): bs_roformer.demix_track (first call and `--reps` synchronised calls),
+peak device memory, device time by kernel family in a separate profiled forward of `--max-chunks` chunks, the rate of
+evk_rope_attn_fwd at the time and frequency shapes of 4 chunks, and the reference's algorithm on stock PyTorch
+(oracle/bs_roformer_oracle.py's forward driven by its demix_track: batches of 4, a host copy and accumulate after each, SDPA
+limited to the math and memory-efficient backends as Attend does off A100) with fp16 weights and chunks under autocast, as
+SeparateMDXC runs with cfg.is_half (when that does not run, the error is recorded and autocast with fp32 weights is timed
+instead), and in fp32 with TF32 allowed.  Every output is also compared with one run of the same algorithm in fp32 with TF32
+off.
+
+Usage:  python tools/bench_uvr5.py [--net vr|deecho|dereverb|roformer] [--frames 16538] [--tta 0] [--max-windows 16] [--reps 3]
 """
 import argparse
 import json
@@ -27,6 +37,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from oracle import bs_roformer_oracle as BR  # noqa: E402
 from oracle import uvr5_echo_oracle as E  # noqa: E402
 from oracle import uvr5_oracle as O  # noqa: E402
 
@@ -198,15 +209,124 @@ def echo_main(a):
     print(json.dumps(res))
 
 
+def rope_attn_rates(ops, reps=20):
+    """TFLOP/s of evk_rope_attn_fwd at the shapes of 4 chunks of the shipped config (801 frames x 62 bands, 8 heads):
+    time axis 248 sequences of 801 tokens, frequency axis 3 204 sequences of 62 tokens (CUDA events over `reps` launches)"""
+    B, T, F, H = 4, 801, 62, 8
+    ld = 3 * H * 64 + H
+    x = torch.randn(B * T * F, ld, device="cuda")
+    o = torch.empty(B * T * F, H * 64, device="cuda")
+    out = {}
+    for name, L, geo, nseq in (("time", T, (B, T * F, F, 1, F), B * F), ("freq", F, (B * T, F, 1, 0, 1), B * T)):
+        cs = torch.stack(BR.rotary_cos_sin(L), -1).contiguous().cuda()
+        fn = lambda: ops.rope_attn(x, cs, o, H, L, *geo)  # noqa: E731
+        fn()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / reps
+        out[name] = dict(sequences=nseq, L=L, ms=round(ms, 3), tflops=round(4.0 * nseq * H * L * L * 64 / ms / 1e9, 1))
+    return out
+
+
+FAMILIES = (("gemm", ("evk_gconv_fwd", "evk_conv_direct_fwd")), ("attention", ("evk_rope_attn_fwd",)),
+            ("norms", ("evk_row_l2norm", "evk_bs_band_input")), ("stft_istft", ("evk_stft_fwd", "evk_istft")))
+
+
+def torch_roformer_demix(P, cfg, mix, half, autocast):
+    """SeparateMDXC.demix_track on stock PyTorch: the oracle's forward on the GPU (half: chunks cast to fp16 as the
+    reference does under cfg.is_half; the weights are whatever P holds), batches of 4, each batch's output copied to the host
+    and accumulated there"""
+    from torch.nn.attention import SDPBackend, sdpa_kernel
+    dev = torch.device("cuda")
+
+    def net(a):
+        a = a.to(dev)
+        with torch.autocast("cuda", enabled=autocast), sdpa_kernel([SDPBackend.MATH, SDPBackend.EFFICIENT_ATTENTION]):
+            return BR.forward(P, cfg, a.half() if half else a).float().cpu()
+
+    return BR.demix_track(net, mix)["vocals"]
+
+
+def roformer_main(a):
+    assert torch.cuda.is_available(), "needs a GPU"
+    from easevoice_trainer_b200 import bs_roformer, lib, ops
+    lib.init().evk_set_precise(0)
+    cfg = dict(BR.SHIPPED)
+    P = BR.init_params(BR.param_spec(cfg), 81)
+    model = bs_roformer.BSRoformer(**cfg).to("cuda").load_state_dict(P)
+    mix = BR.make_audio(7, (2, 7938000))
+    res = dict(gpu=gpu_info(), net="roformer", samples=mix.shape[1], chunks=-(-mix.shape[1] // BR.CHUNK), max_chunks=a.max_chunks)
+    t = time.perf_counter()
+    out = bs_roformer.demix_track(model, mix, "cuda", a.max_chunks)["vocals"]
+    res["evk_first_call_s"] = round(time.perf_counter() - t, 3)
+    torch.cuda.reset_peak_memory_stats()
+    ts = timed(lambda: bs_roformer.demix_track(model, mix, "cuda", a.max_chunks), a.reps)
+    res["evk_s"] = [round(t, 3) for t in ts]
+    res["peak_mem_gib"] = round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)
+    batch = mix[:, :a.max_chunks * BR.CHUNK].reshape(2, a.max_chunks, BR.CHUNK).transpose(0, 1).contiguous().cuda()
+    model.forward(batch)
+    ops.profile_begin()
+    model.forward(batch)
+    prof = ops.profile_end()
+    tot = sum(v["ms"] for v in prof.values())
+    fam = {name: round(sum(v["ms"] for k, v in prof.items() if k.split(":")[0] in keys), 2) for name, keys in FAMILIES}
+    fam["other"] = round(tot - sum(fam.values()), 2)
+    res["forward_ms_by_family"] = fam
+    res["forward_device_ms"] = round(tot, 2)
+    gemm_fl = sum(v["flops"] for k, v in prof.items() if k.split(":")[0] in FAMILIES[0][1])
+    res["chunk_tflop_gemm"] = round(gemm_fl / a.max_chunks / 1e12, 2)
+    res["gemm_tflops_in_forward"] = round(gemm_fl / fam["gemm"] / 1e9, 1)
+    res["rope_attn"] = rope_attn_rates(ops)
+    if not a.skip_torch:
+        torch.backends.cudnn.allow_tf32 = True
+        small = BR.make_audio(8, (2, BR.CHUNK))
+        rel = lambda x, r: float(np.linalg.norm(x - r) / np.linalg.norm(r))  # noqa: E731
+        # accuracy yardstick: the same algorithm in fp32 with TF32 off (one run, not timed)
+        torch.backends.cuda.matmul.allow_tf32 = False
+        Pd = {k: v.cuda() for k, v in P.items()}
+        exact = torch_roformer_demix(Pd, cfg, mix, False, False)
+        res["evk_rel_l2_vs_torch_fp32"] = rel(out, exact)
+        torch.backends.cuda.matmul.allow_tf32 = True
+        # (name, weights in fp16, chunks in fp16, autocast): the shipped cfg.is_half path, then fp32 with TF32 allowed
+        arms = [("torch_fp16", True, True, True), ("torch_tf32", False, False, False)]
+        while arms:
+            name, wh, ch, ac = arms.pop(0)
+            Pd = {k: (v.half() if wh else v).cuda() for k, v in P.items()}
+            try:
+                torch_roformer_demix(Pd, cfg, small, ch, ac)                           # warm-up
+            except RuntimeError as e:
+                if name != "torch_fp16":
+                    raise
+                # the is_half configuration as written does not run: record why, then autocast with fp32 weights
+                res["torch_fp16_error"] = f"{type(e).__name__}: {str(e)[:300]}"
+                arms.insert(0, ("torch_autocast_fp32_weights", False, False, True))
+                continue
+            ts = timed(lambda: torch_roformer_demix(Pd, cfg, mix, ch, ac), a.reps)
+            res[name + "_s"] = [round(t, 3) for t in ts]
+            ref = torch_roformer_demix(Pd, cfg, mix, ch, ac)
+            res[name + "_rel_l2_vs_evk"] = rel(ref, out)
+            res[name + "_rel_l2_vs_torch_fp32"] = rel(ref, exact)
+            del Pd
+            torch.cuda.empty_cache()
+    print(json.dumps(res))
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--net", choices=("vr", "deecho", "dereverb"), default="vr")
+    ap.add_argument("--net", choices=("vr", "deecho", "dereverb", "roformer"), default="vr")
+    ap.add_argument("--max-chunks", type=int, default=4)
     ap.add_argument("--frames", type=int, default=16538)
     ap.add_argument("--tta", type=int, default=0)
     ap.add_argument("--max-windows", type=int, default=16)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--skip-torch", action="store_true")
     a = ap.parse_args()
+    if a.net == "roformer":
+        return roformer_main(a)
     if a.net != "vr":
         return echo_main(a)
     assert torch.cuda.is_available(), "needs a GPU"
