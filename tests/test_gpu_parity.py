@@ -27,7 +27,9 @@ def test_group(evk, idx):
 
 
 def test_precise_mode_tightens_conv(evk):
-    """3xTF32 mode must agree with the fp32 oracle ~100x tighter than plain TF32 (proves the error is rounding, not indexing)."""
+    """3xTF32 mode must agree with the fp32 oracle ~100x tighter than plain TF32 (proves the error is rounding, not indexing).
+    Precise mode runs every conv on the mma.sync kernels (gconv_f_kernel / gconv_w_kernel), so this pins their indexing; the
+    wgmma / TMA kernels that run outside it are pinned bit for bit by tests/test_gpu_exact_contractions.py."""
     from tests import checks
     evk.evk_set_precise(1)
     checks.PRECISE_MODE[0] = True
