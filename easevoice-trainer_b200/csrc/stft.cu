@@ -9,13 +9,38 @@
 #include "evk_common.cuh"
 #include <math.h>
 
+#include <vector>
+
 #include "stft_core.cuh"
 
 namespace evk {
 
 __device__ float2 g_stw[STFT_TAB];      // e^{-2 pi i k / 4096}
 __device__ float g_shann[STFT_TAB];     // periodic Hann(4096)
-static bool g_stft_ready = false;
+__device__ float2 g_mtw[STFT_TAB_MR];   // e^{-2 pi i k / 61440}: the mixed-radix sizes (stft_core.cuh)
+__device__ float g_mhann[STFT_TAB_MR];  // periodic Hann(61440)
+static bool g_stft_ready = false, g_stft_mr_ready = false;
+
+// device addresses of the mixed-radix tables (filled on first use); vr_wave.cu's kernels take them as arguments
+int stft_mr_tables(const float2** tw, const float** hann) {
+  if (!g_stft_mr_ready) {
+    std::vector<float2> t(STFT_TAB_MR);
+    std::vector<float> h(STFT_TAB_MR);
+    for (int i = 0; i < STFT_TAB_MR; ++i) {
+      const double a = 2.0 * M_PI * (double)i / (double)STFT_TAB_MR;
+      t[i] = make_float2((float)cos(a), (float)(-sin(a)));
+      h[i] = (float)(0.5 - 0.5 * cos(a));
+    }
+    if (cudaMemcpyToSymbol(g_mtw, t.data(), t.size() * sizeof(float2)) != cudaSuccess) return EVK_ERR_CUDA;
+    if (cudaMemcpyToSymbol(g_mhann, h.data(), h.size() * sizeof(float)) != cudaSuccess) return EVK_ERR_CUDA;
+    g_stft_mr_ready = true;
+  }
+  void *pt = nullptr, *ph = nullptr;
+  if (cudaGetSymbolAddress(&pt, g_mtw) != cudaSuccess || cudaGetSymbolAddress(&ph, g_mhann) != cudaSuccess) return EVK_ERR_CUDA;
+  *tw = static_cast<const float2*>(pt);
+  *hann = static_cast<const float*>(ph);
+  return EVK_OK;
+}
 
 int stft_init_tables() {
   if (g_stft_ready) return EVK_OK;
@@ -207,11 +232,23 @@ __global__ void __launch_bounds__(256) cplx_l1_kernel(const float2* __restrict__
 // stft * mask (bs_roformer.py:530-543): one block per frame (row r = b S + s, frame t) runs the C2R inverse DFT through the same
 // adjoint packing and forward FFT as stft_bwd_kernel (bins 0 and N/2 lose their imaginary parts), windows the frame and writes it
 // to work [(r T + t)][N]; istft_ola_kernel then overlap-adds the frames in frame order and divides by the sum of w^2.
+// Power-of-two sizes run on the 4096-entry tables, the mixed-radix sizes on the STFT_TAB_MR ones.
 struct IstftP {
   const float2* cplx; const float* mask; int ldm;
   int S, T, N, hop;
   float* work; float* out; int ldo; int Lout;
+  const float2* tw; const float* hann; int tab;
 };
+
+__device__ __forceinline__ const float2* run_fft_t(int NH, float2* d0, float2* d1, const float2* tw, int tab) {
+  float2 *src = d0, *dst = d1;
+  for (int Ns = 1; Ns < NH;) {
+    Ns = stft_pass_r(threadIdx.x, ST_THREADS, NH, Ns, stft_radix(NH, Ns), src, dst, tw, tab);
+    __syncthreads();
+    float2* t = src; src = dst; dst = t;
+  }
+  return src;
+}
 
 __global__ void __launch_bounds__(ST_THREADS) istft_frame_kernel(const IstftP p) {
   extern __shared__ __align__(16) uint8_t ssm[];
@@ -234,14 +271,14 @@ __global__ void __launch_bounds__(ST_THREADS) istft_frame_kernel(const IstftP p)
     G[k] = make_float2(x.x * sc, x.y * sc);
   }
   __syncthreads();
-  stft_adjoint_pack_phase(tid, ST_THREADS, p.N, G, g_stw, d0);
+  stft_adjoint_pack_phase_t(tid, ST_THREADS, p.N, G, p.tw, p.tab, d0);
   __syncthreads();
-  const float2* z = run_fft(NH, d0, d1);
+  const float2* z = run_fft_t(NH, d0, d1, p.tw, p.tab);
   float* fr = p.work + frame * p.N;
   for (int m = tid; m < NH; m += ST_THREADS) {
     const float2 v = z[m];
-    fr[2 * m] = v.x * stft_window(g_shann, 2 * m, p.N, p.N);
-    fr[2 * m + 1] = -v.y * stft_window(g_shann, 2 * m + 1, p.N, p.N);
+    fr[2 * m] = v.x * stft_window_t(p.hann, 2 * m, p.N, p.N, p.tab);
+    fr[2 * m + 1] = -v.y * stft_window_t(p.hann, 2 * m + 1, p.N, p.N, p.tab);
   }
 }
 
@@ -256,7 +293,7 @@ __global__ void istft_ola_kernel(const IstftP p) {
     float y = 0.f, env = 0.f;
     for (int f = lo; f <= hi; ++f) {
       const int j = q - f * p.hop;
-      const float w = stft_window(g_shann, j, p.N, p.N);
+      const float w = stft_window_t(p.hann, j, p.N, p.N, p.tab);
       y += p.work[((long long)r * p.T + f) * p.N + j];
       env += w * w;
     }
@@ -344,15 +381,26 @@ extern "C" int evk_stft_bwd(const float* gcplx, const float* dmel, int32_t ld_dm
 extern "C" int evk_istft(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft,
                          int32_t hop, float* work, float* out, int32_t ld_out, evk_stream_t stream) {
   EVK_REQUIRE(cplx && work && out, EVK_ERR_ARG, "istft: null tensor");
-  EVK_REQUIRE(n_fft >= 256 && n_fft <= STFT_TAB && (n_fft & (n_fft - 1)) == 0, EVK_ERR_UNSUPPORTED, "istft: n_fft=%d must be a power of two in [256, 4096]", n_fft);
+  const bool pow2 = n_fft >= 256 && n_fft <= STFT_TAB && (n_fft & (n_fft - 1)) == 0;
+  EVK_REQUIRE(pow2 || stft_mr_size_ok(n_fft), EVK_ERR_UNSUPPORTED,
+              "istft: n_fft=%d must be a power of two in [256, 4096] or an even divisor of %d in [16, 7680]", n_fft, STFT_TAB_MR);
   EVK_REQUIRE(B > 0 && S > 0 && T >= 2 && hop > 0 && hop <= n_fft / 2 && (long long)B * S <= 65535, EVK_ERR_ARG,
               "istft: bad sizes B=%d S=%d T=%d hop=%d", B, S, T, hop);
   EVK_REQUIRE(!mask || (ld_mask >= 2 * S * (n_fft / 2 + 1) && (uintptr_t)mask % 8 == 0 && ld_mask % 2 == 0), EVK_ERR_ARG,
               "istft: mask rows must hold 2 * S * (n_fft / 2 + 1) floats, 8-byte aligned");
   const long long Lout = (long long)hop * (T - 1), frames = (long long)B * S * T;
   EVK_REQUIRE(ld_out >= Lout && frames <= 0x7fffffff && Lout <= 0x7fffffff, EVK_ERR_ARG, "istft: output pitch %d < %lld", ld_out, Lout);
-  if (int rc = stft_init_tables()) return rc;
-  IstftP p{reinterpret_cast<const float2*>(cplx), mask, ld_mask, S, T, n_fft, hop, work, out, ld_out, (int)Lout};
+  IstftP p{reinterpret_cast<const float2*>(cplx), mask, ld_mask, S, T, n_fft, hop, work, out, ld_out, (int)Lout, nullptr, nullptr, 0};
+  if (pow2) {
+    if (int rc = stft_init_tables()) return rc;
+    void *pt = nullptr, *ph = nullptr;
+    EVK_REQUIRE(cudaGetSymbolAddress(&pt, g_stw) == cudaSuccess && cudaGetSymbolAddress(&ph, g_shann) == cudaSuccess, EVK_ERR_CUDA,
+                "istft: table address");
+    p.tw = static_cast<const float2*>(pt); p.hann = static_cast<const float*>(ph); p.tab = STFT_TAB;
+  } else {
+    if (int rc = stft_mr_tables(&p.tw, &p.hann)) return rc;
+    p.tab = STFT_TAB_MR;
+  }
   const size_t smem = (size_t)(n_fft / 2) * 16 + (size_t)(n_fft / 2 + 1) * 8;
   static size_t attr = 48 * 1024;
   if (smem > attr) {

@@ -2212,6 +2212,62 @@ def istft(cplx, B, S, n_fft, hop, mask=None, out=None, work=None):
     return out
 
 
+def vr_band_stft(wav, bands, l, row_gain, n_rows, high_band=-1, high_lo=0, high_h=0, zero_pad=True):
+    """evk_vr_band_stft: wav a flat fp32 device buffer holding every band's two rows; bands: one (offset, L, ldw, n_fft, hop,
+    crop_start, crop_stop, row0) tuple per band -> (combined spectrogram [2, n_rows, l, 2] (re, im; rows no band covers are
+    zero), the high-end slice [2, high_h, l, 2] of band high_band or None)"""
+    spec = torch.zeros((2, n_rows, l, 2), device=wav.device, dtype=torch.float32)
+    high = torch.empty((2, high_h, l, 2), device=wav.device, dtype=torch.float32) if high_band >= 0 else None
+    desc = (ctypes.c_int64 * (8 * len(bands)))(*[int(v) for b in bands for v in b])
+    assert wav.is_contiguous() and row_gain.numel() == n_rows
+    _call("evk_vr_band_stft", _p(wav), desc, len(bands), l, _p(row_gain), _p(spec), n_rows, high_band, high_lo, high_h, _p(high),
+          1 if zero_pad else 0)
+    return spec, high
+
+
+def vr_mag_norm(spec):
+    """evk_vr_mag_norm: complex spec [..., 2] -> (|spec| / max|spec| [...], max|spec| as a device tensor [1])"""
+    assert spec.is_contiguous() and spec.shape[-1] == 2
+    mag = torch.empty(spec.shape[:-1], device=spec.device, dtype=torch.float32)
+    coef = torch.empty(1, device=spec.device, dtype=torch.float32)
+    _call("evk_vr_mag_norm", _p(spec), mag.numel(), _p(mag), _p(coef))
+    return mag, coef
+
+
+def resample_poly(x, h, up, down, n_pre_remove, n_out, out=None):
+    """evk_resample_poly: scipy.signal.resample_poly of the rows of x [rows, L] with the zero-prefixed fp32 filter h (device)
+    -> [rows, n_out]"""
+    rows, L = x.shape
+    assert x.stride(1) == 1 and h.is_contiguous()
+    out = torch.empty((rows, n_out), device=x.device, dtype=torch.float32) if out is None else out
+    assert out.stride(1) == 1 and out.shape == (rows, n_out)
+    _call("evk_resample_poly", _p(x), rows, L, x.stride(0), _p(h), h.numel(), up, down, n_pre_remove, _p(out), n_out, out.stride(0))
+    return out
+
+
+def vr_assemble(x, pred, pred_tta, coef, bands, gains, high=None, mirror_lo=0, top=-1):
+    """evk_vr_assemble: combined spectrogram x [2, n_rows, l, 2], pred / pred_tta [2, n_rows, l] and coef [1] -> one
+    [4, l, n_fft/2+1, 2] frame tensor per band (rows y ch0, y ch1, v ch0, v ch1: evk_istft's input with B = 4, S = 1).
+    bands: (n_fft, crop_start, crop_stop, row0) per band; gains: one fp32 device vector of n_fft/2+1 per band."""
+    _, n_rows, l, _ = x.shape
+    assert x.is_contiguous() and pred.is_contiguous() and (pred_tta is None or pred_tta.is_contiguous())
+    nbs = [b[0] // 2 + 1 for b in bands]
+    out = torch.empty(sum(4 * l * nb * 2 for nb in nbs), device=x.device, dtype=torch.float32)
+    g = torch.cat(gains).contiguous()
+    desc, go, oo = [], 0, 0
+    for b, nb in zip(bands, nbs):
+        desc += [*b, go, oo]
+        go, oo = go + nb, oo + 4 * l * nb
+    high_h = high.shape[1] if high is not None else 0
+    _call("evk_vr_assemble", _p(x), _p(pred), _p(pred_tta), _p(coef), n_rows, l, _p(high), high_h, mirror_lo, top,
+          (ctypes.c_int64 * len(desc))(*desc), len(bands), _p(g), _p(out))
+    frames, o = [], 0
+    for nb in nbs:
+        frames.append(out[o:o + 8 * l * nb].view(4, l, nb, 2))
+        o += 8 * l * nb
+    return frames
+
+
 def glu_into(h, out):
     """nn.GLU(dim=-1) of h [rows, 2C] written into out [rows, C] (a view with unit column stride; evk_glu_res with x = NULL)"""
     rows, C2 = h.shape

@@ -12,8 +12,15 @@ once.  Activations are channels-last fp32; a layer writes straight into its slic
   * the input x, aux1 (the two band nets, each on its half of the rows) and aux2 are slices of one [B, max_bin, W, 2 + ...]
     buffer, so cat([x, aux1]) and cat([x, aux1, aux2]) are never built.
 Eval BatchNorm is folded into a per-channel scale and bias of the preceding convolution at load; Dropout is the identity.
-The librosa front and back ends (resampling, per-band STFT / iSTFT, combine_spectrograms, mirroring) stay with the caller.
+
+separate_wave runs the whole of SeparateVR.separate (uvr5/separate.py:103-196) from the decoded 44.1 kHz waveform to the two
+output waveforms on the device: the band loop's polyphase resampling, the per-band STFTs written into the combined
+spectrogram, the net, and per output the mask, mirroring, band filters, per-band iSTFTs and the FFT resampling that chains
+the bands.  One copy to the device and one back per file.  Decoding, and resampling inputs that are not at the top band's
+rate, stay with the caller.
 """
+import math
+
 import numpy as np
 import torch
 
@@ -596,6 +603,20 @@ def _windows(x_pre, pad_l, pad_r, roi, ws, n_window):
     return xp.unfold(2, ws, roi)[:, :, :n_window].permute(2, 0, 1, 3)
 
 
+def _predict_windows(x_pre, model, aggressiveness, ws, tta, max_windows):
+    """The net over every window (and TTA window) of the normalised magnitudes x_pre [2, bins, n_frame] (device), in batches
+    of max_windows -> (output [n_window (+ n_window + 1), 2, bins, roi] on the device, n_window, roi)"""
+    n_frame = x_pre.shape[2]
+    pad_l, pad_r, roi = make_padding(n_frame, ws, model.offset)
+    n_window = int(np.ceil(n_frame / roi))
+    wins = [_windows(x_pre, pad_l, pad_r, roi, ws, n_window)]
+    if tta:
+        wins.append(_windows(x_pre, pad_l + roi // 2, pad_r + roi // 2, roi, ws, n_window + 1))
+    wins = torch.cat(wins, 0)
+    outs = [model.predict(wins[i:i + max_windows].contiguous(), aggressiveness) for i in range(0, wins.shape[0], max_windows)]
+    return torch.cat(outs, 0), n_window, roi
+
+
 def inference(x_spec, device, model, aggressiveness, data, max_windows=16):
     """SeparateVR.inference(x_spec, device, model, aggressiveness, data) with every window (and TTA window) of the file in
     batches of max_windows: -> numpy (pred * coef, |x_spec|, exp(1j * angle(x_spec))).  |x|, the phase and coef are the
@@ -610,16 +631,8 @@ def inference(x_spec, device, model, aggressiveness, data, max_windows=16):
     coef = x_mag.max()
     x_mag_pre = x_mag / coef
     n_frame = x_mag_pre.shape[2]
-    pad_l, pad_r, roi = make_padding(n_frame, ws, model.offset)
-    n_window = int(np.ceil(n_frame / roi))
-    dev = torch.device(device)
-    x_pre = torch.from_numpy(np.ascontiguousarray(x_mag_pre, dtype=np.float32)).to(dev)
-    wins = [_windows(x_pre, pad_l, pad_r, roi, ws, n_window)]
-    if data["tta"]:
-        wins.append(_windows(x_pre, pad_l + roi // 2, pad_r + roi // 2, roi, ws, n_window + 1))
-    wins = torch.cat(wins, 0)
-    outs = [model.predict(wins[i:i + max_windows].contiguous(), aggressiveness) for i in range(0, wins.shape[0], max_windows)]
-    out = torch.cat(outs, 0)                               # [n_windows (+ n_window + 1), 2, bins, roi], still running
+    x_pre = torch.from_numpy(np.ascontiguousarray(x_mag_pre, dtype=np.float32)).to(torch.device(device))
+    out, n_window, roi = _predict_windows(x_pre, model, aggressiveness, ws, data["tta"], max_windows)
     phase = np.exp(1.0j * np.angle(x_spec))                # host work while the device runs the net
     out = out.cpu().numpy()                                # the one copy to the host
     bins = out.shape[2]
@@ -632,3 +645,252 @@ def inference(x_spec, device, model, aggressiveness, data, max_windows=16):
         pred_tta = join(out[n_window:])[:, :, roi // 2:][:, :, :n_frame]
         return (pred + pred_tta) * 0.5 * coef, x_mag, phase
     return pred * coef, x_mag, phase
+
+
+# ---- SeparateVR.separate from waveform to waveform -----------------------------------------------------------------
+WINDOW_SIZE = 512          # SeparateVR's data["window_size"]
+ZERO_PAD = True            # librosa 0.9's stft pad_mode default "constant" (unverified against a run of librosa 0.9.2)
+
+
+def stft_size_ok(n_fft):
+    """the frame sizes of the mixed-radix STFT core: even divisors of 61440 = 2^12 3 5 in [16, 7680]"""
+    return 16 <= n_fft <= 7680 and n_fft % 2 == 0 and 61440 % n_fft == 0
+
+
+def firwin_kaiser(numtaps, cutoff, beta=5.0):
+    """scipy.signal.firwin(numtaps, cutoff, window=("kaiser", beta)) (low-pass, scaled to unit gain at DC), float64"""
+    m = np.arange(numtaps) - (numtaps - 1) / 2.0
+    h = cutoff * np.sinc(cutoff * m)
+    alpha = (numtaps - 1) / 2.0
+    h = h * (np.i0(beta * np.sqrt(1.0 - ((np.arange(numtaps) - alpha) / alpha) ** 2)) / np.i0(beta))
+    return h / h.sum()
+
+
+def poly_filter(up, down):
+    """scipy.signal.resample_poly's default filter for (up, down) (already reduced): -> (the zero-prefixed fp32 taps times up,
+    half_len, n_pre_remove)"""
+    max_rate = max(up, down)
+    half_len = 10 * max_rate
+    h = firwin_kaiser(2 * half_len + 1, 1.0 / max_rate).astype(np.float32) * np.float32(up)
+    n_pre_pad = down - half_len % down
+    return np.concatenate([np.zeros(n_pre_pad, np.float32), h]), half_len, (half_len + n_pre_pad) // down
+
+
+def lp_gains(g, bin_start, bin_stop):
+    """spec_utils.fft_lp_filter applied to the per-bin gain vector g (float64)"""
+    v = 1.0
+    for b in range(bin_start, bin_stop):
+        v -= 1 / (bin_stop - bin_start)
+        g[b] = v * g[b]
+    g[bin_stop:] *= 0
+    return g
+
+
+def hp_gains(g, bin_start, bin_stop):
+    """spec_utils.fft_hp_filter applied to the per-bin gain vector g (float64)"""
+    v = 1.0
+    for b in range(bin_start, bin_stop, -1):
+        v -= 1 / (bin_start - bin_stop)
+        g[b] = v * g[b]
+    g[0:bin_stop + 1] *= 0
+    return g
+
+
+def band_gains(param):
+    """-> {band: float64 [n_fft/2 + 1]}: the filters cmb_spectrogram_to_wave applies to each band (spec_utils.py:356-431)"""
+    n = len(param["band"])
+    out = {}
+    for d in range(1, n + 1):
+        bp = param["band"][d]
+        g = np.ones(bp["n_fft"] // 2 + 1)
+        if d == n:
+            if bp["hpf_start"] > 0:
+                hp_gains(g, bp["hpf_start"], bp["hpf_stop"] - 1)
+        elif d == 1:
+            lp_gains(g, bp["lpf_start"], bp["lpf_stop"])
+        else:
+            hp_gains(g, bp["hpf_start"], bp["hpf_stop"] - 1)
+            lp_gains(g, bp["lpf_start"], bp["lpf_stop"])
+        out[d] = g
+    return out
+
+
+def pre_filter_gains(param):
+    """-> float32 [bins + 1]: the row gains of combine_spectrograms' pre-filter (1 elsewhere)"""
+    g = np.ones(param["bins"] + 1, np.float32)
+    if param["pre_filter_start"] > 0:
+        if len(param["band"]) == 1:
+            raise ValueError("single-band parameter sets (fft_lp_filter pre-filter) are not supported")
+        gp = 1
+        for b in range(param["pre_filter_start"] + 1, param["pre_filter_stop"]):
+            v = math.pow(10, -(b - param["pre_filter_start"]) * (3.5 - gp) / 20.0)
+            gp = v
+            g[b] = np.float32(v)
+    return g
+
+
+def high_end_head(param):
+    """SeparateVR.separate's input_high_end_h: the number of top-band bins `mirroring` replaces"""
+    bp = param["band"][len(param["band"])]
+    return (bp["n_fft"] // 2 - bp["crop_stop"]) + (param["pre_filter_stop"] - param["pre_filter_start"])
+
+
+def check_wave_param(param, high_end_process="mirroring"):
+    """ValueError unless separate_wave can run this ModelParameters.param (see separate_wave)"""
+    if high_end_process not in ("mirroring", "none"):
+        raise ValueError(f"high_end_process {high_end_process!r}: only 'mirroring' and 'none' are supported")
+    for k in ("mid_side", "mid_side_b2", "reverse"):
+        if param.get(k):
+            raise ValueError(f"parameter sets with {k} are not supported")
+    bands = param["band"]
+    n = len(bands)
+    if sorted(bands) != list(range(1, n + 1)):
+        raise ValueError("band keys must be the integers 1 .. n")
+    if n > 4:
+        raise ValueError(f"{n} bands: at most 4 are supported")
+    if n == 1:
+        raise ValueError("single-band parameter sets are not supported")
+    if bands[n]["sr"] != param["sr"]:
+        raise ValueError(f"top band rate {bands[n]['sr']} differs from the parameter set's sr {param['sr']}")
+    for d in range(1, n + 1):
+        bp = bands[d]
+        if not stft_size_ok(bp["n_fft"]):
+            raise ValueError(f"band {d}: n_fft {bp['n_fft']} is not an even divisor of 61440 (2^12 3 5) in [16, 7680]")
+        if not 0 < bp["hl"] <= bp["n_fft"] // 2:
+            raise ValueError(f"band {d}: hop {bp['hl']} must be in (0, n_fft / 2]")
+        if d < n:
+            up_sr = bands[d + 1]["sr"]
+            if bp["res_type"] != "polyphase" or up_sr % bp["sr"]:
+                raise ValueError(f"band {d}: only polyphase resampling by an integer factor is supported "
+                                 f"({bp['res_type']}, {up_sr} -> {bp['sr']})")
+            if bp["hl"] * up_sr != bands[d + 1]["hl"] * bp["sr"]:
+                raise ValueError(f"band {d}: hop {bp['hl']} at {bp['sr']} Hz does not cover the time of band {d + 1}'s hop")
+    if n > 1 and bands[1]["sr"] != bands[2]["sr"]:
+        raise ValueError("the back end's sinc_fastest step between bands 1 and 2 needs equal rates")
+    if sum(b["crop_stop"] - b["crop_start"] for b in bands.values()) > param["bins"]:
+        raise ValueError("Too much bins")
+    if high_end_process == "mirroring" and param["pre_filter_start"] - 10 - high_end_head(param) < 0:
+        raise ValueError("the mirrored rows start before row 0")
+
+
+def resampled_len(n, orig_sr, target_sr):
+    """librosa.resample's output length: n for equal rates, else int(ceil(n * (target_sr / orig_sr))) in float64 (fix_length
+    pads or trims scipy's output to it)"""
+    return n if orig_sr == target_sr else int(np.ceil(n * (float(target_sr) / orig_sr)))
+
+
+def band_lengths(L, param):
+    """-> {band: samples} down the band loop from L samples at the top band"""
+    bands = param["band"]
+    n = len(bands)
+    out = {n: L}
+    for d in range(n - 1, 0, -1):
+        out[d] = resampled_len(out[d + 1], bands[d + 1]["sr"], bands[d]["sr"])
+    return out
+
+
+def fft_resample(x, num):
+    """scipy.signal.resample(x, num, axis=-1) of float64 rows x [rows, Nx].  One transform of an arbitrary length (80 (l - 1)
+    samples at 7350 Hz, with factors such as 23 * 719) per band boundary: torch.fft's, a few milliseconds against the
+    net's hundreds."""
+    Nx = x.shape[-1]
+    X = torch.fft.rfft(x, dim=-1)
+    Y = torch.zeros(x.shape[:-1] + (num // 2 + 1,), dtype=X.dtype, device=x.device)
+    N = min(num, Nx)
+    nyq = N // 2 + 1
+    Y[..., :nyq] = X[..., :nyq]
+    if N % 2 == 0:
+        if num < Nx:
+            Y[..., N // 2] *= 2.0
+        elif Nx < num:
+            Y[..., N // 2] *= 0.5
+    return torch.fft.irfft(Y, n=num, dim=-1) * (float(num) / float(Nx))
+
+
+def separate_wave(wave, model, param, agg=10, tta=False, high_end_process="mirroring", max_windows=16):
+    """SeparateVR.separate (and SeparateVREcho's) from the decoded waveform to the two output waveforms, on the device:
+    -> (accompaniment, vocals), numpy float32 [hop_top * (l - 1), 2] each: the wav_accompaniment and wav_vocals of
+    separate.py:165-187 before `* 32768` and the int16 cast.
+
+    wave: float32 [2, L] or [L] (mono is duplicated) at the top band's rate, param["sr"].  param: ModelParameters.param (int
+    band keys), e.g. 4band_v2 (SeparateVR) or 4band_v3 (SeparateVREcho).  model: a CascadedASPPNet or CascadedNet on CUDA.
+    Parameter sets this path cannot take raise ValueError before any device work: mid_side / mid_side_b2 / reverse; a lower
+    band that is not a polyphase resampling by an integer factor; different rates at the back end's sinc_fastest step; an
+    n_fft that is not an even divisor of 61440 (2^12 3 5) in [16, 7680]; a top band rate other than param["sr"]; and
+    high_end_process other than "mirroring" / "none".  So do inputs too short for two frames of every band.  Where the
+    reference reads memory it never wrote (cmb_spectrogram_to_wave's np.ndarray: band 1's bins past crop_stop, the top
+    band's Nyquist bin), zeros are used.  An all-zero input gives NaN outputs, as the reference's 0 / 0."""
+    check_wave_param(param, high_end_process)
+    if max_windows < 1:
+        raise ValueError("max_windows must be >= 1")
+    if model.output_bin != param["bins"] + 1:
+        raise ValueError(f"the model has {model.output_bin} bins, the parameter set {param['bins'] + 1}")
+    wave = np.asarray(wave, dtype=np.float32)
+    if wave.ndim == 1:
+        wave = np.stack([wave, wave])
+    if wave.ndim != 2 or wave.shape[0] != 2:
+        raise ValueError(f"expected a [2, L] or [L] waveform, got {wave.shape}")
+    bands = param["band"]
+    n = len(bands)
+    lens = band_lengths(wave.shape[1], param)
+    l = min(1 + lens[d] // bands[d]["hl"] for d in bands)
+    if min(lens.values()) < 1 or l < 2:
+        raise ValueError(f"{wave.shape[1]} samples: too short for two frames of every band")
+    model.check_shape(WINDOW_SIZE, crop=True)
+    dev = model.device
+    # every band's two rows in one buffer; a band at the rate of the band above it is that band's rows
+    offs, total = {}, 0
+    for d in range(n, 0, -1):
+        if d < n and bands[d]["sr"] == bands[d + 1]["sr"]:
+            offs[d] = offs[d + 1]
+        else:
+            offs[d], total = total, total + 2 * lens[d]
+    buf = torch.empty(total, device=dev, dtype=torch.float32)
+    buf[offs[n]:offs[n] + 2 * lens[n]].copy_(torch.from_numpy(np.ascontiguousarray(wave)).view(-1))      # the one copy in
+    for d in range(n - 1, 0, -1):
+        if offs[d] != offs[d + 1]:
+            g = math.gcd(bands[d + 1]["sr"], bands[d]["sr"])
+            up, down = bands[d]["sr"] // g, bands[d + 1]["sr"] // g
+            h, _, n_pre_remove = poly_filter(up, down)
+            dst = buf[offs[d]:offs[d] + 2 * lens[d]].view(2, lens[d])
+            n_poly = min(-(-lens[d + 1] * up // down), lens[d])          # resample_poly's outputs, then fix_length's zeros
+            dst[:, n_poly:].zero_()
+            ops.resample_poly(buf[offs[d + 1]:offs[d + 1] + 2 * lens[d + 1]].view(2, lens[d + 1]), torch.from_numpy(h).to(dev), up,
+                              down, n_pre_remove, n_poly, out=dst[:, :n_poly])
+    rows, row0 = param["bins"] + 1, 0
+    stft_bands, asm_bands = [], []
+    for d in range(1, n + 1):
+        bp = bands[d]
+        stft_bands.append((offs[d], lens[d], lens[d], bp["n_fft"], bp["hl"], bp["crop_start"], bp["crop_stop"], row0))
+        asm_bands.append((bp["n_fft"], bp["crop_start"], bp["crop_stop"], row0))
+        row0 += bp["crop_stop"] - bp["crop_start"]
+    mirror = high_end_process == "mirroring"
+    hh = high_end_head(param) if mirror else 0
+    top = bands[n]
+    x, high = ops.vr_band_stft(buf, stft_bands, l, torch.from_numpy(pre_filter_gains(param)).to(dev), rows,
+                               high_band=n - 1 if mirror else -1, high_lo=top["n_fft"] // 2 - hh, high_h=hh, zero_pad=ZERO_PAD)
+    del buf
+    x_pre, coef = ops.vr_mag_norm(x)
+    aggressiveness = {"value": float(agg / 100), "split_bin": bands[1]["crop_stop"], "aggr_correction": param.get("aggr_correction")}
+    out, n_window, roi = _predict_windows(x_pre, model, aggressiveness, WINDOW_SIZE, tta, max_windows)
+    del x_pre
+
+    def join(o, skip):
+        return o.permute(1, 2, 0, 3).reshape(2, rows, -1)[:, :, skip:skip + l].contiguous()
+
+    pred = join(out[:n_window], 0)
+    pred_tta = join(out[n_window:], roi // 2) if tta else None
+    del out
+    gains = [torch.from_numpy(g.astype(np.float32)).to(dev) for g in band_gains(param).values()]
+    frames = ops.vr_assemble(x, pred, pred_tta, coef, asm_bands, gains, high=high,
+                             mirror_lo=param["pre_filter_start"] - 10 - hh, top=n - 1)
+    wav = None
+    for d in range(1, n + 1):
+        bp = bands[d]
+        w = ops.istft(frames[d - 1], 4, 1, bp["n_fft"], bp["hl"]).double()
+        frames[d - 1] = None
+        wav = w if wav is None else wav + w
+        if d < n and bands[d + 1]["sr"] != bp["sr"]:
+            wav = fft_resample(wav, resampled_len(wav.shape[1], bp["sr"], bands[d + 1]["sr"]))
+    res = wav.float().cpu().numpy()                                                           # the one copy out
+    return np.ascontiguousarray(res[0:2].T), np.ascontiguousarray(res[2:4].T)

@@ -535,7 +535,8 @@ int evk_rope_attn_fwd(const float* qkvg, int32_t ld, const float* cs, float* o, 
  * 2 (k S + s) .. +1 of mask row b*T + t (pitch ld_mask: the mask estimator's 'b t (f s c)' layout).  Per frame a C2R inverse
  * DFT (imaginary parts of bins 0 and n_fft/2 ignored) and the window, written to work [B*S*T][n_fft]; then the overlap-add in
  * frame order, divided by the sum of squared windows, trimmed by n_fft/2 at both ends: out [B*S][ld_out] gets hop*(T-1)
- * samples per row.  n_fft a power of two in [256, 4096], T >= 2, hop <= n_fft / 2, B*S <= 65535. */
+ * samples per row.  n_fft a power of two in [256, 4096], or an even divisor of 61440 (2^12 3 5) in [16, 7680] (the
+ * mixed-radix core: the UVR5 VR band sizes 320, 640, 960); T >= 2, hop <= n_fft / 2, B*S <= 65535. */
 int evk_istft(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft, int32_t hop,
               float* work, float* out, int32_t ld_out, evk_stream_t stream);
 /* Band-split operand (bs_roformer.py:481-490 and each band's RMSNorm before its Linear): from evk_stft_fwd's cplx
@@ -547,6 +548,40 @@ int evk_bs_band_input(const float* cplx, int32_t B, int32_t S, int32_t T, int32_
 /* y[r] = x[r] / max(||x[r]||_2, 1e-12) per row (F.normalize(dim=-1): the RMSNorms, whose gamma * sqrt(dim) the caller folds
  * into the next Linear's weight columns). */
 int evk_row_l2norm(const float* x, int32_t ldx, float* y, int32_t ldy, int64_t rows, int32_t C, evk_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * UVR5 VR front and back end (SeparateVR.separate, uvr5/separate.py:103-196; spec_utils.py), vr_wave.cu.  Frame sizes are
+ * those of the mixed-radix core: even divisors of 61440 in [16, 7680].
+ * ------------------------------------------------------------------------------------------ */
+/* librosa.stft(n_fft, hop, periodic Hann(n_fft), center=True) of frames 0 .. l-1 of every band and both channels, scattered
+ * into the combined spectrogram spec [2][n_rows][l] (complex, re/im interleaved): bins [crop_start, crop_stop) of a band go
+ * to rows row0 .. row0 + crop_stop - crop_start, times row_gain[row] (device [n_rows]).  Rows no band covers are left as
+ * they are.  bands: host int64 [n_bands][8] = (offset of the band's two rows in wav, L, row pitch ldw, n_fft, hop, crop_start,
+ * crop_stop, row0); n_bands <= 4; each band needs 1 + L / hop >= l frames.  zero_pad: edges padded with n_fft/2 zeros
+ * (librosa >= 0.9's pad_mode="constant"), else reflected.  high (nullable): bins [high_lo, high_lo + high_h) of band
+ * high_band, unscaled, to high [2][high_h][l] (the slice `mirroring` reads). */
+int evk_vr_band_stft(const float* wav, const int64_t* bands, int32_t n_bands, int32_t l, const float* row_gain, float* spec,
+                     int32_t n_rows, int32_t high_band, int32_t high_lo, int32_t high_h, float* high, int32_t zero_pad,
+                     evk_stream_t stream);
+/* mag[i] = |spec[i]| / coef over n complex elements, coef = max |spec| written to coef[0] (device).  An all-zero spectrum
+ * gives coef 0 and NaN magnitudes, as numpy's 0 / 0.  Max is exact, so the result does not depend on the reduction order. */
+int evk_vr_mag_norm(const float* spec, int64_t n, float* mag, float* coef, evk_stream_t stream);
+/* scipy.signal.resample_poly's output for a zero-prefixed filter h [nh] (device, the taps times up):
+ * y[r][n] = sum_i x[r][i] h[(n + n_pre_remove) down - i up] over the i with that index in [0, nh), ascending i, fp32;
+ * n = 0 .. n_out-1.  x [rows][ldx], y [rows][ldy]. */
+int evk_resample_poly(const float* x, int32_t rows, int32_t L, int32_t ldx, const float* h, int32_t nh, int32_t up, int32_t down,
+                      int32_t n_pre_remove, float* y, int32_t n_out, int32_t ldy, evk_stream_t stream);
+/* Half spectra of every band of both outputs, the input of evk_istft.  From the combined spectrogram x [2][n_rows][l]
+ * (complex) and the net's pred [2][n_rows][l] (pred_tta nullable: (pred + pred_tta) * 0.5 * coef, else pred * coef; coef a
+ * device scalar): y = pred exp(i angle(x)) (angle(0) = 0), v = x - y.  Band b (host int64 [n_bands][6] = (n_fft,
+ * crop_start, crop_stop, row0, offset of its gains in `gains`, offset of its frames in `out` in complex elements)) gets
+ * out [4][l][n_fft/2 + 1] complex, rows (y ch0, y ch1, v ch0, v ch1): bin k = gains[k] * (combined row row0 + k - crop_start
+ * for k in [crop_start, crop_stop), 0 elsewhere).  With high [2][high_h][l] (nullable), the top band's bins
+ * [n_fft/2 - high_h, n_fft/2) are spec_utils.mirroring of the output instead: the flipped magnitudes of its rows
+ * [mirror_lo, mirror_lo + high_h) with the phase of high, or high itself where |high| <= that. */
+int evk_vr_assemble(const float* x, const float* pred, const float* pred_tta, const float* coef, int32_t n_rows, int32_t l,
+                    const float* high, int32_t high_h, int32_t mirror_lo, int32_t top, const int64_t* bands, int32_t n_bands,
+                    const float* gains, float* out, evk_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -22,7 +22,15 @@ SeparateMDXC runs with cfg.is_half (when that does not run, the error is recorde
 instead), and in fp32 with TF32 allowed.  Every output is also compared with one run of the same algorithm in fp32 with TF32
 off.
 
-Usage:  python tools/bench_uvr5.py [--net vr|deecho|dereverb|roformer] [--frames 16538] [--tta 0] [--max-windows 16] [--reps 3]
+--wave measures SeparateVR.separate from waveform to waveform on a seeded 3-minute stereo mix (7 938 000 samples at 44.1
+kHz, l = 16 538 frames) with --net vr (61968, 4band_v2), deecho (nout 48) or dereverb (nout 64) (4band_v3) and --tta:
+uvr5.separate_wave with a host array in and host arrays out, synchronised; the reference's host path (the oracle's librosa
+restatement, which makes the numpy / scipy calls librosa makes, around uvr5.inference), split into host front end, net and
+host back end; and, in a separate profiled call, the device time of the new front / back-end kernels against the net.
+The parameter sets are read from tests/golden/uvr5_wave.pt.
+
+Usage:  python tools/bench_uvr5.py [--net vr|deecho|dereverb|roformer] [--wave] [--frames 16538] [--tta 0] [--max-windows 16]
+        [--reps 3]
 """
 import argparse
 import json
@@ -315,6 +323,60 @@ def roformer_main(a):
     print(json.dumps(res))
 
 
+WAVE_FAMILIES = ("evk_vr_band_stft", "evk_vr_mag_norm", "evk_resample_poly", "evk_vr_assemble", "evk_istft")
+
+
+def wave_main(a):
+    """--wave: uvr5.separate_wave against the reference's host front / back end around uvr5.inference"""
+    assert torch.cuda.is_available(), "needs a GPU"
+    from easevoice_trainer_b200 import lib, ops, uvr5
+    from oracle import uvr5_wave_oracle as W
+    lib.init().evk_set_precise(0)
+    gold = torch.load(os.path.join(ROOT, "tests", "golden", "uvr5_wave.pt"), weights_only=False)
+    if a.net == "vr":
+        param = gold["vr"]["param"]
+        net = uvr5.get_nets_model(1344).to("cuda").load_state_dict(O.init_params(O.param_spec(61968), 31))
+    else:
+        param = gold["echo"]["param"]
+        nout = 48 if a.net == "deecho" else 64
+        net = uvr5.CascadedNet(1344, nout).to("cuda").load_state_dict(E.init_params(E.param_spec(1344, nout), 51))
+    mix = W.make_clip(7, 180.0, extra=0)
+    assert mix.shape == (2, 7938000)
+    res = dict(gpu=gpu_info(), net=a.net, wave=True, samples=mix.shape[1], tta=bool(a.tta), max_windows=a.max_windows)
+    run = lambda: uvr5.separate_wave(mix, net, param, 10, bool(a.tta), max_windows=a.max_windows)  # noqa: E731
+    t = time.perf_counter()
+    acc, _ = run()
+    res["evk_first_call_s"] = round(time.perf_counter() - t, 3)
+    res["l"] = acc.shape[0] // 480 + 1
+    torch.cuda.reset_peak_memory_stats()
+    res["evk_separate_wave_s"] = [round(t, 3) for t in timed(run, a.reps)]
+    res["peak_mem_gib"] = round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)
+    ops.profile_begin()
+    run()
+    prof = ops.profile_end()
+    new = sum(v["ms"] for k, v in prof.items() if k.split(":")[0] in WAVE_FAMILIES)
+    tot = sum(v["ms"] for v in prof.values())
+    res["device_ms_front_back_kernels"] = round(new, 1)
+    res["device_ms_all_library_calls"] = round(tot, 1)
+    res["device_ms_by_new_kernel"] = {k: round(v["ms"], 2) for k, v in prof.items() if k.split(":")[0] in WAVE_FAMILIES}
+    if not a.skip_torch:
+        agg = {"value": 0.1, "split_bin": param["band"][1]["crop_stop"], "aggr_correction": None}
+        data = {"window_size": 512, "tta": bool(a.tta)}
+        split = dict(front=[], net=[], back=[])
+        for _ in range(a.reps):
+            t0 = time.perf_counter()
+            x_spec_m, ihe_h, ihe = W.front_end(mix, param)
+            t1 = time.perf_counter()
+            pred, _, phase = uvr5.inference(x_spec_m, "cuda", net, agg, data, a.max_windows)
+            t2 = time.perf_counter()
+            W.back_end(x_spec_m, pred, phase, param, ihe_h, ihe)
+            t3 = time.perf_counter()
+            for k, v in zip(split, (t1 - t0, t2 - t1, t3 - t2)):
+                split[k].append(round(v, 3))
+        res["host_path_s"] = split
+    print(json.dumps(res))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--net", choices=("vr", "deecho", "dereverb", "roformer"), default="vr")
@@ -324,7 +386,10 @@ def main():
     ap.add_argument("--max-windows", type=int, default=16)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--skip-torch", action="store_true")
+    ap.add_argument("--wave", action="store_true")
     a = ap.parse_args()
+    if a.wave:
+        return wave_main(a)
     if a.net == "roformer":
         return roformer_main(a)
     if a.net != "vr":
