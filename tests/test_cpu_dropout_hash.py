@@ -1,4 +1,4 @@
-"""Statistical quality of the attention probability-dropout draw (csrc/flash_common.cuh: drop_row / drop_pair / drop_one), restated
+"""Statistical quality of the attention probability-dropout draw (csrc/flash.cu: drop_row / drop_pair / drop_one), restated
 here in numpy uint32 arithmetic.  The draw was made as cheap as a counter-based generator can be (one multiply-compare per element:
 the attention kernels are bound by the integer pipe), so its statistics are checked explicitly: drop fraction, per-row / per-column
 fractions at the binomial spread, no correlation between neighbouring columns, the two draws of a column pair, rows, diagonals."""
