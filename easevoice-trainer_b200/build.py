@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libevk_sm90.so")
 SOURCES = ["api.cu", "gconv.cu", "gconv_tc.cu", "conv_direct.cu", "mel.cu", "elementwise.cu", "norm_weights.cu", "attention.cu",
            "vq_loss_optim.cu", "flash.cu", "gpt_misc.cu", "gemm_tma.cu", "stft.cu", "pack_batched.cu",
-           "sample.cu", "attn64.cu", "conv2d.cu", "lstm.cu", "bs_roformer.cu", "vr_wave.cu"]
+           "sample.cu", "attn64.cu", "conv2d.cu", "lstm.cu", "bs_roformer.cu", "vr_wave.cu", "vq_train.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]

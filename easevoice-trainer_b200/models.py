@@ -156,6 +156,7 @@ class SynthesizerTrn(ParamTree):
         self.upsample_rates, self.upsample_kernel_sizes = upsample_rates, upsample_kernel_sizes
         self.upsample_initial_channel, self.gin_channels = upsample_initial_channel, gin_channels
         self.freeze_quantizer = freeze_quantizer
+        self._cb_inited = None         # (version counter, value) of the codebook's `inited` flag (codebook_needs_init)
         self.window = 4
         self.style_dropout = 0.1
         self._build()
@@ -289,9 +290,14 @@ class SynthesizerTrn(ParamTree):
             for f in range(4):                                                  # modules.py:436-437
                 self.P(f"flow.flows.{2 * f}.post.weight").zero_()
                 self.P(f"flow.flows.{2 * f}.post.bias").zero_()
-            emb = self.P("quantizer.vq.layers.0._codebook.embed")
+            cb = "quantizer.vq.layers.0._codebook."
+            emb = self.P(cb + "embed")
             emb.copy_(torch.randn(emb.shape, generator=g))
-            self.P("quantizer.vq.layers.0._codebook.embed_avg").copy_(emb)
+            self.P(cb + "embed_avg").copy_(emb)
+            if self.freeze_quantizer is False:
+                # a fresh reference quantizer (kmeans_init=True, core_vq.py:124-138): zero codebook, k-means on the first batch
+                for n in ("embed", "embed_avg", "cluster_size", "inited"):
+                    self.P(cb + n).zero_()
 
     # ---------------------------------------------------------------------------------------------
     # blocks (channels-last)
@@ -460,28 +466,69 @@ class SynthesizerTrn(ParamTree):
             zf = ops.cat_flip(x0, x1)
         return zf
 
-    def forward_cl(self, ssl, spec, lengths, text, text_lengths, noise=None, ids_slice=None):
+    def forward_cl(self, ssl, spec, lengths, text, text_lengths, noise=None, ids_slice=None, vq_rows=None, kmeans_idx=None):
         """Channels-last forward.  ssl [B,T,768], spec [B,T,1025] (pitch may be padded), lengths/text_lengths int32 [B],
-        text int64 [B,X].  Returns a dict of channels-last tensors (same quantities as SynthesizerTrn.forward)."""
+        text int64 [B,X].  Returns a dict of channels-last tensors (same quantities as SynthesizerTrn.forward).
+        Trainable quantizer only: vq_rows (device int32 [1]) is the reference collate's frame count / 2, so that rows
+        past it (padding to a coarser grid) take no part in the codebook statistics or the commitment loss (default:
+        all T / 2 rows); kmeans_idx (int64 [1024]) replaces the random draw of the k-means initial means."""
         self.begin_pack()
         try:
-            return self._forward_cl(ssl, spec, lengths, text, text_lengths, noise, ids_slice)
+            return self._forward_cl(ssl, spec, lengths, text, text_lengths, noise, ids_slice, vq_rows, kmeans_idx)
         finally:
             self.end_pack()
 
-    def _forward_cl(self, ssl, spec, lengths, text, text_lengths, noise, ids_slice):
+    @property
+    def quantizer_trainable(self):
+        """freeze_quantizer: false (only an explicit False; None keeps the frozen path) and training mode."""
+        return self.freeze_quantizer is False and self.training
+
+    def codebook_needs_init(self):
+        """Host-side: does the next trainable-quantizer forward k-means-initialise the codebook (inited == 0)?  Reads the
+        device buffer (a synchronisation) only when it was written from PyTorch since the last read (checkpoint loads)."""
+        inited = self.P("quantizer.vq.layers.0._codebook.inited")
+        if self._cb_inited is None or self._cb_inited[0] != inited._version:
+            assert not (inited.is_cuda and torch.cuda.is_current_stream_capturing()), "codebook state must be known before capture"
+            self._cb_inited = (inited._version, bool(inited.item() != 0))
+        return not self._cb_inited[1]
+
+    def _quantize_train(self, ssl, vq_rows, kmeans_idx):
+        """VectorQuantization.forward in training mode (core_vq.py:203-228, 301-318): k-means init when inited == 0,
+        codes from the (new) codebook, EMA update of the buffers, straight-through value and commitment loss.
+        -> (quantized [B, T, 768], codes [B, T/2], commit loss)."""
+        cb = "quantizer.vq.layers.0._codebook."
+        embed, embed_avg = self.P(cb + "embed"), self.P(cb + "embed_avg")
+        cluster_size, inited = self.P(cb + "cluster_size"), self.P(cb + "inited")
+        x = ops.ssl_proj_fp32(ssl, self.P("ssl_proj.weight"), self.P("ssl_proj.bias"))      # [B, T/2, 768], exact fp32
+        if vq_rows is None:
+            vq_rows = torch.full((1,), x.shape[1], device=x.device, dtype=torch.int32)
+        with torch.no_grad():
+            if self.codebook_needs_init():
+                ops.vq_kmeans_init_(x, vq_rows, embed, embed_avg, cluster_size, inited, idx=kmeans_idx)
+                self._cb_inited = (inited._version, True)
+            codes = ops.vq_nearest(x, embed)
+            q = ops.embedding(embed, codes)                  # looked up before the EMA overwrites embed (core_vq.py:209-226)
+            ops.vq_ema_(x, codes, vq_rows, cluster_size, embed_avg, embed)
+        quantized, commit = ops.vq_straight_through(x, q, vq_rows)
+        return quantized, codes, commit
+
+    def _forward_cl(self, ssl, spec, lengths, text, text_lengths, noise, ids_slice, vq_rows=None, kmeans_idx=None):
         B, T, _ = spec.shape
         assert T % 2 == 0, "frame count must be even (TextAudioSpeakerCollate pads to 2*(Tmax//2+1))"
         I = self.inter_channels
         seg = self.segment_size
         ge = self._ref_enc(spec, lengths)                                        # [B, 1, 512]
-        with torch.no_grad():                                                    # frozen quantizer (models.py:911-921)
-            # exact fp32 products: a TF32-rounded (even a 3xTF32) projection flips the argmin of near-tie codewords
-            # (measured at the benchmarked shapes: 2, resp. 1, of 1 384 codes); the layer is 1 % of the forward flops
-            s = ops.conv_k2s2_fp32(ssl, self.P("ssl_proj.weight"), self.P("ssl_proj.bias"))
-            embed = self.P("quantizer.vq.layers.0._codebook.embed")
-            codes = ops.vq_nearest(s, embed)                                     # [B, T/2] int64
-            quantized = ops.embedding(embed, codes, rep=2)                       # nearest x2 (models.py:924-927)
+        commit = None
+        if self.quantizer_trainable:
+            quantized, codes, commit = self._quantize_train(ssl, vq_rows, kmeans_idx)
+        else:
+            with torch.no_grad():                                                # frozen quantizer (models.py:911-921)
+                # exact fp32 products: a TF32-rounded (even a 3xTF32) projection flips the argmin of near-tie codewords
+                # (measured at the benchmarked shapes: 2, resp. 1, of 1 384 codes); the layer is 1 % of the forward flops
+                s = ops.conv_k2s2_fp32(ssl, self.P("ssl_proj.weight"), self.P("ssl_proj.bias"))
+                embed = self.P("quantizer.vq.layers.0._codebook.embed")
+                codes = ops.vq_nearest(s, embed)                                 # [B, T/2] int64
+                quantized = ops.embedding(embed, codes, rep=2)                   # nearest x2 (models.py:924-927)
         # The prior encoder (12 attention layers of small kernels, none of which fills the GPU) only meets the rest of the
         # step again at the KL loss: run it on a side stream so that it overlaps the posterior encoder / flow / generator
         # (forward AND backward: autograd runs each node on its forward stream).  Inside a captured CUDA graph the fork/join
@@ -528,8 +575,11 @@ class SynthesizerTrn(ParamTree):
             torch.cuda.current_stream().wait_stream(side)
         if side2 is not None:
             torch.cuda.current_stream().wait_stream(side2)
-        return dict(y_hat=o, ids_slice=ids_slice, z=z, z_p=z_p, m_p=m_p, logs_p=logs_p, m_q=m_q, logs_q=logs_q,
-                    quantized=quantized, codes=codes, ge=ge, lengths=lengths)
+        r = dict(y_hat=o, ids_slice=ids_slice, z=z, z_p=z_p, m_p=m_p, logs_p=logs_p, m_q=m_q, logs_q=logs_q,
+                 quantized=quantized, codes=codes, ge=ge, lengths=lengths)
+        if commit is not None:
+            r["kl_ssl"] = commit
+        return r
 
     def forward(self, ssl, y, y_lengths, text, text_lengths, noise=None, ids_slice=None):
         """Reference contract (models.py:904-946): ssl [B,768,T], y = spec [B,1025,T], lengths int64.
@@ -544,7 +594,7 @@ class SynthesizerTrn(ParamTree):
         cf = ops.to_channels_first
         T = y.shape[2]
         y_mask = (torch.arange(T, device=y.device)[None, :] < y_lengths[:, None]).unsqueeze(1).to(y.dtype)
-        commit = torch.zeros((), device=y.device)          # frozen quantizer in eval: commit_loss == 0
+        commit = r.get("kl_ssl", torch.zeros((), device=y.device))     # frozen quantizer: commit_loss == 0
         lat = tuple(cf(r[k]) for k in ("z", "z_p", "m_p", "logs_p", "m_q", "logs_q"))
         return cf(r["y_hat"]), commit, r["ids_slice"], y_mask, y_mask, lat, cf(r["quantized"])
 

@@ -1596,6 +1596,109 @@ def vq_nearest(x, embed):
     return codes
 
 
+# ---- trainable quantizer (freeze_quantizer: false) ---------------------------------------------
+class _SslProjFn(torch.autograd.Function):
+    """ssl_proj (Conv1d kernel 2, stride 2) with the exact-fp32 forward of conv_k2s2_fp32 and a TF32 weight gradient:
+    dW2 [N, 2C] = dY^T X2 with X2 = the [rows, 2C] view of ssl (two frames per row), on the TMA-fed GEMM."""
+
+    @staticmethod
+    def forward(ctx, ssl, weight, bias):
+        ctx.save_for_backward(ssl)
+        ctx.wshape = weight.shape
+        return conv_k2s2_fp32(ssl, weight, bias)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (ssl,) = ctx.saved_tensors
+        N, C, _ = ctx.wshape
+        dy = dy.contiguous()
+        rows = dy.shape[0] * dy.shape[1]
+        x2 = ssl.contiguous().reshape(rows, 2 * C)
+        d2 = dy.reshape(rows, N)
+        rows4 = (rows + 3) // 4 * 4                                   # the GEMM's K (= rows) pitch must be 16-byte aligned
+        if rows4 != rows:
+            x2 = torch.nn.functional.pad(x2, (0, 0, 0, rows4 - rows))
+            d2 = torch.nn.functional.pad(d2, (0, 0, 0, rows4 - rows))
+        dyt = to_channels_first(d2.unsqueeze(0))[0]                  # [N, rows]
+        xt = to_channels_first(x2.unsqueeze(0))[0]                   # [2C, rows]
+        dw2 = gemm_tf32(dyt, xt)                                     # [N, 2C] = [n][tap][c]
+        dw = dw2.reshape(N, 2, C).permute(0, 2, 1).contiguous()      # weight layout [n][c][tap]
+        db = torch.empty(N, device=dy.device, dtype=torch.float32)
+        _call("evk_col_sum", _p(d2), rows4, N, _p(db))
+        return None, dw, db
+
+
+def ssl_proj_fp32(ssl, weight, bias):
+    """conv_k2s2_fp32 with gradients for weight / bias (the unfrozen quantizer's input projection)."""
+    return _SslProjFn.apply(ssl, weight, bias)
+
+
+def vq_kmeans_init_(x, rows_ref, embed, embed_avg, cluster_size, inited, iters=50, idx=None, tag="vq.kmeans"):
+    """init_embed_ (core_vq.py:141-149) on the device: k-means over the first min(500, rows) valid rows of x [B, T2, D]
+    (rows_ref: device int32 [1] = valid frames per batch row); sets embed = embed_avg = means, cluster_size = bins,
+    inited = 1.  idx (int64 [K], optional) replaces the Philox draw of the initial means.  -> the sample indices used."""
+    x = _c(x.detach())
+    B, T2, D = x.shape
+    K = embed.shape[0]
+    dev = x.device
+    samples = torch.empty((500, D), device=dev, dtype=torch.float32)
+    nsamp = torch.empty(1, device=dev, dtype=torch.int32)
+    means = torch.empty((K, D), device=dev, dtype=torch.float32)
+    idx_out = torch.empty(K, device=dev, dtype=torch.int64)
+    if idx is not None:
+        idx = idx.to(device=dev, dtype=torch.int64).contiguous()
+    _call("evk_vq_kmeans_draw", _p(x), D, B, T2, _p(rows_ref), K, D, _p(idx), _p(rng_state(dev)), ctypes.c_uint64(stream_id(tag)),
+          _p(samples), _p(nsamp), _p(means), _p(idx_out))
+    buckets = torch.empty(500, device=dev, dtype=torch.int32)
+    bins = torch.zeros(K, device=dev, dtype=torch.float32)
+    for _ in range(iters):
+        _call("evk_vq_kmeans_iter", _p(samples), _p(nsamp), _p(means), K, D, _p(buckets), _p(bins))
+    embed.copy_(means)
+    embed_avg.copy_(means)
+    cluster_size.copy_(bins)
+    inited.fill_(1.0)
+    return idx_out
+
+
+def vq_ema_(x, codes, rows_ref, cluster_size, embed_avg, embed, decay=0.99, eps=1e-5):
+    """EMA codebook update of EuclideanCodebook.forward in training mode (core_vq.py:218-226), in place."""
+    x = _c(x.detach())
+    B, T2, D = x.shape
+    _call("evk_vq_ema", _p(x), D, _p(codes.contiguous()), B, T2, _p(rows_ref), _p(cluster_size), _p(embed_avg), _p(embed),
+          embed.shape[0], D, ctypes.c_float(decay), ctypes.c_float(eps))
+
+
+class _VqStraightThroughFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, q, rows_ref):
+        x = _c(x)
+        q = _c(q.detach())
+        B, T2, D = x.shape
+        y = torch.empty((B, 2 * T2, D), device=x.device, dtype=torch.float32)
+        qst = torch.empty((B, T2, D), device=x.device, dtype=torch.float32)
+        loss = torch.empty(1, device=x.device, dtype=torch.float32)
+        _call("evk_vq_st_fwd", _p(x), D, _p(q), D, B, T2, D, _p(rows_ref), _p(y), _p(qst), _p(loss))
+        ctx.save_for_backward(x, qst, rows_ref)
+        return y, loss[0]
+
+    @staticmethod
+    def backward(ctx, dy, dloss):
+        x, qst, rows_ref = ctx.saved_tensors
+        B, T2, D = x.shape
+        dy = torch.zeros((B, 2 * T2, D), device=x.device, dtype=torch.float32) if dy is None else dy.contiguous()
+        g = torch.zeros(1, device=x.device, dtype=torch.float32) if dloss is None else dloss.reshape(1).contiguous()
+        dx = torch.empty_like(x)
+        _call("evk_vq_st_bwd", _p(dy), _p(x), D, _p(qst), B, T2, D, _p(rows_ref), _p(g), _p(dx))
+        return dx, None, None
+
+
+def vq_straight_through(x, q, rows_ref):
+    """VectorQuantization.forward in training mode (core_vq.py:308-316) + the nearest x2 upsample (models.py:924-927):
+    x [B, T2, D] (differentiable), q = its codewords -> (x + (q - x) upsampled to [B, 2*T2, D],
+    commit loss = mean((x + (q - x) - x)^2) over the rows t < rows_ref)."""
+    return _VqStraightThroughFn.apply(x, q, rows_ref)
+
+
 class _ReduceLossFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, a, b, kind, scale_):

@@ -154,7 +154,8 @@ class FlatAdamW:
                     mine["initial_lr"] = float(g["initial_lr"])
 
 
-FROZEN_G = ("ssl_proj.weight", "ssl_proj.bias")     # models.py:911-921: the quantizer front end runs under no_grad
+FROZEN_G = ("ssl_proj.weight", "ssl_proj.bias")     # models.py:911-921: the frozen quantizer's front end gets no gradient
+CODEBOOK = tuple("quantizer.vq.layers.0._codebook." + n for n in ("embed", "embed_avg", "cluster_size", "inited"))
 
 
 def g_param_groups(net_g, text_low_lr_rate):
@@ -204,8 +205,10 @@ class S2Step:
         self.world = world_size
         self.seg_frames = hps_train["segment_size"] // hps_data["hop_length"]
         betas = tuple(hps_train["betas"])
+        # freeze_quantizer: false trains ssl_proj and moves the codebook (an EMA of the batches' assignments)
+        self.vq_train = net_g.freeze_quantizer is False
         self.opt_g = FlatAdamW(net_g.named_parameters(), g_param_groups(net_g, hps_train["text_low_lr_rate"]), betas,
-                               hps_train["eps"], frozen=FROZEN_G)
+                               hps_train["eps"], frozen=() if self.vq_train else FROZEN_G)
         self.opt_d = FlatAdamW(net_d.named_parameters(), [(1.0, [n for n, _ in net_d.named_parameters()])], betas,
                                hps_train["eps"])
         self.lr = hps_train["learning_rate"]
@@ -219,12 +222,13 @@ class S2Step:
         self._pool = None            # one private memory pool shared by every captured graph
         self._shape_group = None     # gloo group for the host-side shape agreement (world > 1)
 
-    def losses(self, batch, noise=None, ids_slice=None):
+    def losses(self, batch, noise=None, ids_slice=None, kmeans_idx=None):
         """Forward + both losses (no optimiser).  batch: dict of channels-last device tensors:
-        ssl [B,T,768], spec [B,T,1025], lengths int32 [B], wav [B,L,1], text int64 [B,X], text_lengths int32 [B]."""
+        ssl [B,T,768], spec [B,T,1025], lengths int32 [B], wav [B,L,1], text int64 [B,X], text_lengths int32 [B],
+        optionally vq_rows int32 [1] (the trainable quantizer's reference row count, see SynthesizerTrn.forward_cl)."""
         hop, seg = self.d["hop_length"], self.t["segment_size"]
         r = self.net_g.forward_cl(batch["ssl"], batch["spec"], batch["lengths"], batch["text"], batch["text_lengths"],
-                                  noise, ids_slice)
+                                  noise, ids_slice, batch.get("vq_rows"), kmeans_idx)
         ids = r["ids_slice"]
         y_hat = r["y_hat"]                                                        # [B, seg, 1]
         B = y_hat.shape[0]
@@ -256,6 +260,9 @@ class S2Step:
         loss_fm = loss_fm * 2
         total = loss_gen + loss_fm + loss_mel + loss_kl                            # + kl_ssl == 0 (frozen quantizer)
         parts = dict(loss_gen=loss_gen, loss_fm=loss_fm, loss_mel=loss_mel, loss_kl=loss_kl)
+        if "kl_ssl" in r:                                                          # sovits.py:518: + kl_ssl * 1
+            total = total + r["kl_ssl"]
+            parts["kl_ssl"] = r["kl_ssl"]
         c_mr = float(self.t.get("c_mrstft", 0.0))
         if c_mr > 0.0:          # opt-in extension (BASELINE config 5): the MR-STFT term of bs_roformer.py:565-581 on the fused STFT kernel
             parts["loss_mrstft"] = ops.mrstft_loss(r["y_hat"].reshape(B, -1), r["y"].reshape(B, -1)) * c_mr
@@ -266,14 +273,21 @@ class S2Step:
         if self.world > 1:
             dist.all_reduce(opt.reduce_view)
 
+    def _broadcast_codebook(self):
+        """DDP(broadcast_buffers=True) semantics of the reference (sovits.py:321): before every G forward rank 0's codebook
+        buffers replace every other rank's, so codes come from rank 0's codebook and only rank 0's EMA survives."""
+        if self.vq_train and self.world > 1:
+            for n in CODEBOOK:
+                dist.broadcast(self.net_g.P(n), src=0)
+
     # The step in three segments, split where the data-parallel gradient exchanges happen:
     #   A: G forward, features, D forward, D backward -> flat D grads          | all-reduce(D grads)
     #   B: D AdamW, D forward (updated weights), G backward -> flat G grads    | all-reduce(G grads)
     #   C: G AdamW, RNG advance
     # EVK_NVTX=1 brackets the phases with NVTX ranges (ncu --nvtx --nvtx-include "s2/d_backward/" ... selects a phase's kernels).
-    def _seg_a(self, batch, noise=None, ids_slice=None):
+    def _seg_a(self, batch, noise=None, ids_slice=None, kmeans_idx=None):
         with ops.nvtx_range("s2/forward"):
-            r = self.losses(batch, noise, ids_slice)
+            r = self.losses(batch, noise, ids_slice, kmeans_idx)
             loss_d = self.d_loss(r)
         with ops.nvtx_range("s2/d_backward"), ops.grad_pool():
             self.opt_d.set_grads(torch.autograd.grad(loss_d, self.opt_d.params, allow_unused=True))
@@ -299,11 +313,13 @@ class S2Step:
         out.update({k: v.detach() for k, v in parts.items()})
         return out
 
-    def step(self, batch, noise=None, ids_slice=None, collectives=True):
-        """Eager step (every kernel launched from Python).  No host synchronisation anywhere.
-        collectives=False runs the rank-local math only (graph warm-up: a warm-up must never pair with another rank's
-        real gradient exchange)."""
-        r, loss_d = self._seg_a(batch, noise, ids_slice)
+    def step(self, batch, noise=None, ids_slice=None, collectives=True, kmeans_idx=None):
+        """Eager step (every kernel launched from Python).  No host synchronisation anywhere, except that a trainable
+        quantizer reads its `inited` flag once.  collectives=False runs the rank-local math only (graph warm-up: a warm-up
+        must never pair with another rank's real gradient exchange).  kmeans_idx: see SynthesizerTrn.forward_cl."""
+        if collectives:
+            self._broadcast_codebook()
+        r, loss_d = self._seg_a(batch, noise, ids_slice, kmeans_idx)
         if collectives:
             self._allreduce(self.opt_d)
         loss_g, parts = self._seg_b(r)
@@ -332,6 +348,8 @@ class S2Step:
         CAPTURE_AFTER-th time the shape shows up; before that the eager step runs."""
         key = (tuple(batch["ssl"].shape), tuple(batch["text"].shape))
         n = self._seen[key] = self._seen.get(key, 0) + 1
+        if self.vq_train and self.net_g.codebook_needs_init():
+            return self.step(batch)              # the k-means initialisation runs once, eagerly
         if key in self._graphs or n >= self.CAPTURE_AFTER:
             return self.graph_step(batch)
         return self.step(batch)
@@ -341,6 +359,8 @@ class S2Step:
         loss tensors.  noise / ids_slice (parity tests) become static inputs of a separately keyed graph; keep=True also
         returns the captured forward tensors (they stay valid until the next replay)."""
         key = (tuple(batch["ssl"].shape), tuple(batch["text"].shape), noise is not None, bool(keep))
+        if self.vq_train and self.net_g.codebook_needs_init():
+            raise RuntimeError("the codebook is not initialised yet (inited == 0): run one eager step() first")
         g = self._graphs.pop(key, None)
         if g is None:
             while len(self._graphs) >= self.MAX_GRAPHS:                  # evict the least recently used shape
@@ -355,6 +375,7 @@ class S2Step:
             src = noise if k == "noise" else ids_slice if k == "ids_slice" else batch[k]
             if static[k] is not src:
                 static[k].copy_(src, non_blocking=True)
+        self._broadcast_codebook()
         if len(graphs) == 1:
             graphs[0].replay()
         else:                               # data parallel: NCCL all-reduces run between the captured segments
@@ -378,6 +399,8 @@ class S2Step:
         # It runs WITHOUT collectives -- another rank may be replaying a real step right now.
         state = (self.opt_g.flat_p, self.opt_g.flat_m, self.opt_g.flat_v, self.opt_g.hyper, self.opt_d.flat_p, self.opt_d.flat_m,
                  self.opt_d.flat_v, self.opt_d.hyper, ops.rng_state(sp.device))
+        if self.vq_train:                        # the EMA moves the codebook buffers in every forward
+            state += tuple(self.net_g.P(n) for n in CODEBOOK)
         snap = [t.clone() for t in state]
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
@@ -388,6 +411,8 @@ class S2Step:
         for dst, src in zip(state, snap):
             dst.copy_(src)
         torch.cuda.synchronize()
+        if self.vq_train:
+            self.net_g.codebook_needs_init()     # the restore wrote `inited`: re-read it here, not during the capture
         if self._pool is None:
             self._pool = torch.cuda.graph_pool_handle()
         if self.world == 1:
@@ -441,9 +466,11 @@ def synthetic_batch(B, T, X, device, seed=1234, hop=640, bank=None, ragged=False
     return dict(ssl=ssl, wav=wav, text=text, lengths=lengths, text_lengths=text_lengths)
 
 
-def to_device_batch(host, device, bank, hop=640):
+def to_device_batch(host, device, bank, hop=640, vq_frames=None):
     """H2D + layout change + feature extraction that the reference does on CPU workers (data_utils.py:119-128):
-    wav -> |X| on the GPU with the fused mel kernel.  Returns the channels-last dict S2Step consumes."""
+    wav -> |X| on the GPU with the fused mel kernel.  Returns the channels-last dict S2Step consumes.
+    vq_frames (the trainable quantizer only): the frame count of the reference collate's batch before any further padding;
+    the batch then carries vq_rows = vq_frames // 2 as a device scalar."""
     wav = host["wav"].to(device, non_blocking=True)
     ssl = host["ssl"].to(device, non_blocking=True)
     text = host["text"].to(device, non_blocking=True)
@@ -453,5 +480,8 @@ def to_device_batch(host, device, bank, hop=640):
     # per-row sample counts (when the collate provides them): reflection at each utterance's own end (data_utils.py:119-128)
     lens = host["wav_lengths"].to(device, non_blocking=True).to(torch.int32) if "wav_lengths" in host else None
     spec, _ = ops.mel_frontend(wav.reshape(B, L), bank, hop, want_spec=True, want_mel=False, lens=lens)   # [B,T,1025], pitch 1028
-    return dict(ssl=ops.to_channels_last(ssl), spec=spec, lengths=lengths, wav=wav.reshape(B, L, 1), text=text,
-                text_lengths=text_lengths)
+    out = dict(ssl=ops.to_channels_last(ssl), spec=spec, lengths=lengths, wav=wav.reshape(B, L, 1), text=text,
+               text_lengths=text_lengths)
+    if vq_frames is not None:
+        out["vq_rows"] = torch.tensor([vq_frames // 2], dtype=torch.int32).to(device, non_blocking=True)
+    return out

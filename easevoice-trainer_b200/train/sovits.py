@@ -160,9 +160,10 @@ class SovitsTrain:
         for epoch in range(epoch_str, t["epochs"] + 1):
             sampler.set_epoch(epoch)
             for host in loader:
-                Tq, Xq = step.agree_shape(host["ssl"].shape[2], host["text"].shape[1])
+                T_ref = host["ssl"].shape[2]                          # the reference collate's padded frame count
+                Tq, Xq = step.agree_shape(T_ref, host["text"].shape[1])
                 host = s2data_pad(host, Tq, Xq, hop)
-                batch = s2_step.to_device_batch(host, device, step.bank, hop)
+                batch = s2_step.to_device_batch(host, device, step.bank, hop, vq_frames=T_ref if step.vq_train else None)
                 out = step.train_step(batch)
                 gs = self.global_step
                 if gs % 10 == 0:                                      # sovits.py:527-536
@@ -173,7 +174,7 @@ class SovitsTrain:
                     scalars = {"loss/g/total": float(out["loss_gen_all"]), "loss/d/total": float(out["loss_disc"]),
                                "learning_rate": step.lr, "grad_norm_d": float(out["grad_norm_d"]) ** 0.5,
                                "grad_norm_g": float(out["grad_norm_g"]) ** 0.5, "loss/g/fm": float(out["loss_fm"]),
-                               "loss/g/mel": float(out["loss_mel"]), "loss/g/kl_ssl": 0.0, "loss/g/kl": float(out["loss_kl"])}
+                               "loss/g/mel": float(out["loss_mel"]), "loss/g/kl_ssl": float(out["kl_ssl"]) if "kl_ssl" in out else 0.0, "loss/g/kl": float(out["loss_kl"])}
                     for k, v in scalars.items():
                         writer.add_scalar(k, v, gs)
                     writer.flush()

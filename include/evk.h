@@ -284,6 +284,33 @@ int evk_sgemm_nt_f32(const float* A, int32_t lda, const float* B, int32_t ldb, f
 int evk_vq_argmax(const float* dots, int32_t ldd, const float* x, int32_t ldx, const float* embed, int32_t lde,
                   int64_t rows, int32_t K, int32_t D, int64_t* codes, float* enorm_scratch, evk_stream_t stream);
 
+/* Trainable quantizer (freeze_quantizer: false; core_vq.py:71-93, 141-149, 203-228, 301-318).  x is [B, T2, D] with row
+ * pitch ldx; only rows (b, t < rows_ref[0]) take part (rows_ref: device int32, the reference collate's T / 2).  No float
+ * atomics: every sum runs in a fixed order.
+ * kmeans_draw: samples = the first n = min(500, B * rows_ref) valid rows in (b, t) order (nsamp[0] = n); means[k] =
+ *   samples[idx[k]], idx injected or drawn uniformly from [0, n) with the Philox stream (seed_offset, stream_id); idx_out
+ *   (optional) receives the indices.  samples: [500, D], means: [K, D].
+ * kmeans_iter: one Lloyd iteration: buckets[i] = argmax_k -sum_d (s_id - m_kd)^2 (direct differences, lowest index on
+ *   ties), bins[k] = its count, means[k] = ordered mean of its samples (kept when empty).  buckets: [500] int32.
+ * vq_ema: cluster_size <- decay cs + (1 - decay) counts, embed_avg <- decay ea + (1 - decay) (x^T onehot)^T, then
+ *   embed <- embed_avg / ((cs + eps) / (sum cs + K eps) * sum cs).  Per code, rows are summed in row order.
+ * vq_st_fwd: qst = x + (q - x) [B*T2, D], y = qst upsampled x2 in time [B, 2*T2, D], loss[0] = mean((qst - x)^2) over the
+ *   valid rows.  vq_st_bwd: dx = dy[2t] + dy[2t+1] + gloss * 2 (x - qst) / N on valid rows, 0 elsewhere ([B*T2, D]).
+ * col_sum: out[c] = sum_r x[r][c] (x dense [rows, C]), chunks of 64 rows added in order. */
+int evk_vq_kmeans_draw(const float* x, int32_t ldx, int32_t B, int32_t T2, const int32_t* rows_ref, int32_t K, int32_t D,
+                       const int64_t* idx, const uint64_t* seed_offset, uint64_t stream_id, float* samples, int32_t* nsamp,
+                       float* means, int64_t* idx_out, evk_stream_t stream);
+int evk_vq_kmeans_iter(const float* samples, const int32_t* nsamp, float* means, int32_t K, int32_t D, int32_t* buckets,
+                       float* bins, evk_stream_t stream);
+int evk_vq_ema(const float* x, int32_t ldx, const int64_t* codes, int32_t B, int32_t T2, const int32_t* rows_ref,
+               float* cluster_size, float* embed_avg, float* embed, int32_t K, int32_t D, float decay, float eps,
+               evk_stream_t stream);
+int evk_vq_st_fwd(const float* x, int32_t ldx, const float* q, int32_t ldq, int32_t B, int32_t T2, int32_t D,
+                  const int32_t* rows_ref, float* y, float* qst, float* loss, evk_stream_t stream);
+int evk_vq_st_bwd(const float* dy, const float* x, int32_t ldx, const float* qst, int32_t B, int32_t T2, int32_t D,
+                  const int32_t* rows_ref, const float* gloss, float* dx, evk_stream_t stream);
+int evk_col_sum(const float* x, int64_t rows, int32_t C, float* out, evk_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Loss reductions (losses.py:7-61, sovits.py:513): out[slot] += scale * sum(f(a,b))
  *   kind 0: (1-a)^2   1: a^2   2: |a-b|   ; bwd kinds write da (scaled by *gscale device scalar * scale)
