@@ -6,24 +6,9 @@
 
 namespace evk {
 
-struct DP {
-  const float* x; float* w; float* y; const float* res; const float* bias;
-  const int* in_len; const int* out_len;
-  long long x_sb, x_sh, w_sb, w_sh, w_sq, y_sb, y_sh, r_sb, r_sh;
-  int ldx, ldw, ldy, ldr;
-  int Z, H, C, N, Q, G, Tin, J, P, is, os, o0, Tout, act;
-  float slope;
-  int chunk;
-  int off[EVK_MAX_TAPS];
+struct DP : ConvP {
+  int chunk;                   // wgrad: positions per CTA
 };
-
-__device__ __forceinline__ float dact(float v, int act, float slope) {
-  if (act == EVK_ACT_LRELU) return v > 0.f ? v : v * slope;
-  if (act == EVK_ACT_RELU) return fmaxf(v, 0.f);
-  if (act == EVK_ACT_TANH) return tanhf(v);
-  if (act == EVK_ACT_GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
-  return v;
-}
 
 // one thread per output element (pos, n), n fastest
 __global__ void direct_fwd_thread(const __grid_constant__ DP p) {
@@ -51,7 +36,7 @@ __global__ void direct_fwd_thread(const __grid_constant__ DP p) {
   const long long orow = (long long)oj * p.P + w;
   if (p.bias) acc += p.bias[n];
   if (p.res) acc += (p.res + b * p.r_sb + h * p.r_sh)[orow * p.ldr + n];
-  acc = dact(acc, p.act, p.slope);
+  acc = conv_act(acc, p.act, p.slope);
   if (p.out_len && oj >= p.out_len[b]) acc = 0.f;
   (p.y + b * p.y_sb + h * p.y_sh)[orow * p.ldy + n] = acc;
 }
@@ -85,7 +70,7 @@ __global__ void direct_fwd_warp(const __grid_constant__ DP p) {
   const long long orow = (long long)oj * p.P + w;
   if (p.bias) acc += p.bias[n];
   if (p.res) acc += (p.res + b * p.r_sb + h * p.r_sh)[orow * p.ldr + n];
-  acc = dact(acc, p.act, p.slope);
+  acc = conv_act(acc, p.act, p.slope);
   if (p.out_len && oj >= p.out_len[b]) acc = 0.f;
   (p.y + b * p.y_sb + h * p.y_sh)[orow * p.ldy + n] = acc;
 }
@@ -148,32 +133,12 @@ __global__ void direct_wgrad(const __grid_constant__ DP p, float* __restrict__ p
   part[((long long)z * gridDim.x + blockIdx.x) * nw + widx] = acc;
 }
 
-static int fill_dp(const evk_gconv_desc* d, DP& p) {
-  EVK_REQUIRE(d != nullptr, EVK_ERR_ARG, "conv_direct: null descriptor");
-  EVK_REQUIRE(d->Q >= 1 && d->Q <= EVK_MAX_TAPS, EVK_ERR_ARG, "conv_direct: Q=%d out of range", d->Q);
-  const int G = d->G < 1 ? 1 : d->G;
-  EVK_REQUIRE(d->C % G == 0 && d->N % G == 0, EVK_ERR_ARG, "conv_direct: C=%d N=%d not divisible by G=%d", d->C, d->N, G);
-  EVK_REQUIRE(d->Z >= 1 && d->H >= 1 && d->P >= 1 && d->is >= 1 && d->os >= 1, EVK_ERR_ARG, "conv_direct: bad sizes");
-  p.x = d->x; p.w = d->w; p.y = d->y; p.res = d->res; p.bias = d->bias; p.in_len = d->in_len; p.out_len = d->out_len;
-  p.x_sb = d->x_sb; p.x_sh = d->x_sh; p.w_sb = d->w_sb; p.w_sh = d->w_sh; p.w_sq = d->w_sq;
-  p.y_sb = d->y_sb; p.y_sh = d->y_sh; p.r_sb = d->r_sb; p.r_sh = d->r_sh;
-  p.ldx = d->ldx; p.ldw = d->ldw; p.ldy = d->ldy; p.ldr = d->ldr;
-  p.Z = d->Z; p.H = d->H; p.C = d->C; p.N = d->N; p.Q = d->Q; p.G = G; p.Tin = d->Tin; p.J = d->J; p.P = d->P;
-  p.is = d->is; p.os = d->os; p.o0 = d->o0; p.Tout = d->Tout; p.act = d->act; p.slope = d->slope; p.chunk = 0;
-  for (int i = 0; i < EVK_MAX_TAPS; ++i) p.off[i] = i < d->Q ? d->off[i] : 0;
-  if (d->J > 0) {
-    long long last = (long long)d->o0 + (long long)(d->J - 1) * d->os;
-    EVK_REQUIRE(d->o0 >= 0 && last < d->Tout, EVK_ERR_ARG, "conv_direct: output positions exceed Tout");
-  }
-  return EVK_OK;
-}
-
 }  // namespace evk
 using namespace evk;
 
 extern "C" int evk_conv_direct_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
   DP p;
-  int rc = fill_dp(d, p);
+  int rc = conv_params(d, p, "conv_direct_fwd");
   if (rc) return rc;
   const long long total = (long long)p.J * p.P * p.N;
   if (total == 0) return EVK_OK;
@@ -191,7 +156,7 @@ extern "C" int evk_conv_direct_fwd(const evk_gconv_desc* d, evk_stream_t stream)
 
 extern "C" int evk_conv_direct_dgrad(const evk_gconv_desc* d, evk_stream_t stream) {
   DP p;
-  int rc = fill_dp(d, p);
+  int rc = conv_params(d, p, "conv_direct_dgrad");
   if (rc) return rc;
   const long long total = (long long)p.Tin * p.P * p.C;
   if (total == 0) return EVK_OK;
@@ -203,7 +168,7 @@ extern "C" int evk_conv_direct_dgrad(const evk_gconv_desc* d, evk_stream_t strea
 
 extern "C" int evk_conv_direct_wgrad(const evk_gconv_desc* d, evk_stream_t stream) {
   DP p;
-  int rc = fill_dp(d, p);
+  int rc = conv_params(d, p, "conv_direct_wgrad");
   if (rc) return rc;
   const long long nw = (long long)p.Q * p.N * (p.C / p.G);
   const long long npos = (long long)p.J * p.P;

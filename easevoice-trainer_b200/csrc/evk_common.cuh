@@ -27,6 +27,32 @@ static inline double desc_flops(const evk_gconv_desc* d) {
   return 2.0 * d->Z * (double)d->J * d->P * d->N * (d->C / (d->G > 0 ? d->G : 1)) * d->Q;
 }
 
+// ---- generalised 1-D convolution (evk_gconv_desc) -----------------------------------------------
+// The descriptor's operand fields as a kernel parameter block.  The mma.sync, wgmma and direct conv kernels each derive
+// their own parameters from it and add only their tuning fields.
+struct ConvP {
+  const float* x; float* w; float* y; const float* res; const float* bias;
+  const int* in_len; const int* out_len;
+  long long x_sb, x_sh, w_sb, w_sh, w_sq, y_sb, y_sh, r_sb, r_sh;
+  int ldx, ldw, ldy, ldr, b_sh;
+  int Z, H, C, N, Q, Tin, J, P, is, os, o0, Tout, act;
+  float slope;
+  int off_min, off_max;        // extremes of off[0, Q)
+  int off[EVK_MAX_TAPS];       // off[Q, EVK_MAX_TAPS) = 0
+  int G;                       // groups, >= 1 (the direct kernels; the tensor-core kernels take groups as H)
+};
+// Validates d and fills p; `who` names the entry point in the error message.  Returns EVK_OK or EVK_ERR_ARG.
+int conv_params(const evk_gconv_desc* d, ConvP& p, const char* who);
+
+// The evk_act epilogue.
+__device__ __forceinline__ float conv_act(float v, int act, float slope) {
+  if (act == EVK_ACT_LRELU) return v > 0.f ? v : v * slope;
+  if (act == EVK_ACT_RELU) return fmaxf(v, 0.f);
+  if (act == EVK_ACT_TANH) return tanhf(v);
+  if (act == EVK_ACT_GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
+  return v;
+}
+
 // SMs of an H100 SXM: sizes the grids of grid-stride and persistent launches (the TMA GEMM queries the device instead).
 constexpr int kNumSMs = 132;
 

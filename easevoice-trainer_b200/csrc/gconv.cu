@@ -16,28 +16,14 @@ namespace evk {
 constexpr int BM = 128;        // output positions per CTA (F kernel)
 constexpr int NT = 256;        // threads per CTA
 
-struct GP {
-  const float* x; float* w; float* y; const float* res; const float* bias;
-  const int* in_len; const int* out_len;
-  long long x_sb, x_sh, w_sb, w_sh, w_sq, y_sb, y_sh, r_sb, r_sh;
-  int ldx, ldw, ldy, ldr, b_sh;
-  int Z, H, C, N, Q, Tin, J, P, is, os, o0, Tout, act;
-  float slope;
-  int off_min, off_max;
+// Field order: (TG, NG) and (slab_rows, rch) each fill one 8-byte word, so a kernel can read a pair with one 64-bit
+// parameter load.
+struct GP : ConvP {
+  float* part;                // W: per-(z, position chunk, K warp) partials [z - zoff][S1][Q][N][C], summed by gconv_w_sum
+  int zoff;                    // W: first batch x group item of this launch (blockIdx.z counts from it)
   int KS, TG, NG, slab_rows;   // F: k-steps/tap/chunk, taps per group, groups, slab rows
   int rch;                     // W: positions per CTA
-  float* part;                 // W: per-(z, position chunk, K warp) partials [z - zoff][S1][Q][N][C], summed by gconv_w_sum
-  int zoff;                    // W: first batch x group item of this launch (blockIdx.z counts from it)
-  int off[EVK_MAX_TAPS];
 };
-
-__device__ __forceinline__ float apply_act(float v, int act, float slope) {
-  if (act == EVK_ACT_LRELU) return v > 0.f ? v : v * slope;
-  if (act == EVK_ACT_RELU) return fmaxf(v, 0.f);
-  if (act == EVK_ACT_TANH) return tanhf(v);
-  if (act == EVK_ACT_GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
-  return v;
-}
 
 // ============================================================================================
 // F kernel
@@ -204,7 +190,7 @@ __global__ void __launch_bounds__(NT) gconv_f_kernel(const __grid_constant__ GP 
             float v = acc[mf][nf][hf * 2 + e];
             if (p.bias) v += p.bias[h * p.b_sh + n + e];
             if (R) v += R[orow * p.ldr + n + e];
-            v = apply_act(v, p.act, p.slope);
+            v = conv_act(v, p.act, p.slope);
             Y[orow * p.ldy + n + e] = live ? v : 0.f;
           }
         }
@@ -358,15 +344,22 @@ __global__ void __launch_bounds__(NT) gconv_w_kernel(const __grid_constant__ GP 
 // ============================================================================================
 int g_precise = 0;          // 3xTF32 products on the mma.sync kernels (parity tests)
 int g_backend_tc = 1;       // use the TMA / wgmma kernels for eligible (stride-1) launches
-int gconv_tc_try(const evk_gconv_desc* d, cudaStream_t st);
+int gconv_tc_try(const ConvP& c, cudaStream_t st);
 int gemm_tma_try(const evk_gconv_desc* d, cudaStream_t st);
 
-static int fill_gp(const evk_gconv_desc* d, GP& p) {
-  EVK_REQUIRE(d != nullptr, EVK_ERR_ARG, "gconv: null descriptor");
-  EVK_REQUIRE(d->Q >= 1 && d->Q <= EVK_MAX_TAPS, EVK_ERR_ARG, "gconv: Q=%d out of range", d->Q);
+int conv_params(const evk_gconv_desc* d, ConvP& p, const char* who) {
+  EVK_REQUIRE(d != nullptr, EVK_ERR_ARG, "%s: null descriptor", who);
+  EVK_REQUIRE(d->Q >= 1 && d->Q <= EVK_MAX_TAPS, EVK_ERR_ARG, "%s: Q=%d out of range", who, d->Q);
   EVK_REQUIRE(d->Z >= 1 && d->H >= 1 && d->C >= 1 && d->N >= 1 && d->J >= 0 && d->P >= 1, EVK_ERR_ARG,
-              "gconv: bad sizes Z=%d H=%d C=%d N=%d J=%d P=%d", d->Z, d->H, d->C, d->N, d->J, d->P);
-  EVK_REQUIRE(d->is >= 1 && d->os >= 1, EVK_ERR_ARG, "gconv: strides must be >= 1");
+              "%s: bad sizes Z=%d H=%d C=%d N=%d J=%d P=%d", who, d->Z, d->H, d->C, d->N, d->J, d->P);
+  EVK_REQUIRE(d->is >= 1 && d->os >= 1, EVK_ERR_ARG, "%s: strides must be >= 1", who);
+  const int G = d->G < 1 ? 1 : d->G;
+  EVK_REQUIRE(d->C % G == 0 && d->N % G == 0, EVK_ERR_ARG, "%s: C=%d N=%d not divisible by G=%d", who, d->C, d->N, G);
+  if (d->J > 0) {
+    long long last = (long long)d->o0 + (long long)(d->J - 1) * d->os;
+    EVK_REQUIRE(d->o0 >= 0 && last < d->Tout, EVK_ERR_ARG, "%s: output positions exceed Tout (o0=%d J=%d os=%d Tout=%d)",
+                who, d->o0, d->J, d->os, d->Tout);
+  }
   p.x = d->x; p.w = d->w; p.y = d->y; p.res = d->res; p.bias = d->bias;
   p.in_len = d->in_len; p.out_len = d->out_len;
   p.x_sb = d->x_sb; p.x_sh = d->x_sh; p.w_sb = d->w_sb; p.w_sh = d->w_sh; p.w_sq = d->w_sq;
@@ -374,15 +367,11 @@ static int fill_gp(const evk_gconv_desc* d, GP& p) {
   p.ldx = d->ldx; p.ldw = d->ldw; p.ldy = d->ldy; p.ldr = d->ldr; p.b_sh = d->b_sh;
   p.Z = d->Z; p.H = d->H; p.C = d->C; p.N = d->N; p.Q = d->Q; p.Tin = d->Tin; p.J = d->J; p.P = d->P;
   p.is = d->is; p.os = d->os; p.o0 = d->o0; p.Tout = d->Tout; p.act = d->act; p.slope = d->slope;
+  p.G = G;
   int mn = d->off[0], mx = d->off[0];
   for (int i = 0; i < d->Q; ++i) { p.off[i] = d->off[i]; mn = min(mn, d->off[i]); mx = max(mx, d->off[i]); }
   for (int i = d->Q; i < EVK_MAX_TAPS; ++i) p.off[i] = 0;
   p.off_min = mn; p.off_max = mx;
-  if (d->J > 0) {
-    long long last = (long long)d->o0 + (long long)(d->J - 1) * d->os;
-    EVK_REQUIRE(d->o0 >= 0 && last < d->Tout, EVK_ERR_ARG, "gconv: output positions exceed Tout (o0=%d J=%d os=%d Tout=%d)",
-                d->o0, d->J, d->os, d->Tout);
-  }
   return EVK_OK;
 }
 
@@ -444,7 +433,7 @@ extern "C" int evk_set_backend(int32_t tensor_core) { g_backend_tc = tensor_core
 
 extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
   GP p;
-  int rc = fill_gp(d, p);
+  int rc = conv_params(d, p, "gconv_fwd");
   if (rc) return rc;
   rc = check_mma_alignment(d, "gconv_fwd");
   if (rc) return rc;
@@ -454,7 +443,7 @@ extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
     rc = gemm_tma_try(d, st);          // TMA-fed persistent wgmma GEMM / implicit-GEMM conv
     if (rc <= 0) { if (rc == 0) g_disp_flops[0] += desc_flops(d); return rc; }
     EVK_REQUIRE(!(d->drop_rng && d->drop_p > 0.f), EVK_ERR_UNSUPPORTED, "gconv_fwd: fused dropout needs a launch the TMA kernel takes");
-    rc = gconv_tc_try(d, st);
+    rc = gconv_tc_try(p, st);
     if (rc <= 0) { if (rc == 0) g_disp_flops[1] += desc_flops(d); return rc; }
   }
   EVK_REQUIRE(!(d->drop_rng && d->drop_p > 0.f), EVK_ERR_UNSUPPORTED, "gconv_fwd: fused dropout needs a launch the TMA kernel takes");
@@ -547,7 +536,7 @@ static int launch_w(GP& p, cudaStream_t st) {
 
 extern "C" int evk_gconv_wgrad(const evk_gconv_desc* d, evk_stream_t stream) {
   GP p;
-  int rc = fill_gp(d, p);
+  int rc = conv_params(d, p, "gconv_wgrad");
   if (rc) return rc;
   EVK_REQUIRE(d->G <= 1, EVK_ERR_UNSUPPORTED, "gconv_wgrad: pass groups as the inner batch (H = groups), not G");
   EVK_REQUIRE((d->ldx % 4) == 0 && (d->ldy % 4) == 0, EVK_ERR_ARG,

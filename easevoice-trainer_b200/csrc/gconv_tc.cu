@@ -13,17 +13,10 @@
 
 namespace evk {
 
-struct TP {
-  const float* x; const float* w; float* y; const float* res; const float* bias;
-  const int* in_len; const int* out_len;
-  long long x_sb, x_sh, w_sb, w_sh, w_sq, y_sb, y_sh, r_sb, r_sh;
-  int ldx, ldw, ldy, ldr, b_sh;
-  int Z, H, C, N, Q, Tin, J, P, os, o0, act;
-  float slope;
-  int off_min, off_max;
-  int KCH, TG, NG;          // 16-byte K-chunks per stage (2, 4 or 8), taps per group, groups
+struct TP : ConvP {
+  int TG, NG;               // taps per group, groups
   int slab_rows, a_pitch;   // rows staged per chunk, slab panel pitch (rows, == 4 mod 8)
-  int off[EVK_MAX_TAPS];
+  int KCH;                  // 16-byte K-chunks per stage (2, 4 or 8)
 };
 
 constexpr int TC_THREADS = 256;                       // two warpgroups
@@ -148,10 +141,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gconv_tc_kernel(const __grid_co
           if (n + e < p.N) {
             if (bias) t += bias[n + e];
             if (rr) t += rr[n + e];
-            if (p.act == EVK_ACT_LRELU) t = t > 0.f ? t : t * p.slope;
-            else if (p.act == EVK_ACT_RELU) t = fmaxf(t, 0.f);
-            else if (p.act == EVK_ACT_TANH) t = tanhf(t);
-            else if (p.act == EVK_ACT_GELU) t = 0.5f * t * (1.f + erff(t * 0.70710678118654752f));
+            t = conv_act(t, p.act, p.slope);
             v[e] = live ? t : 0.f;
           }
         }
@@ -202,25 +192,15 @@ static int launch_tc(TP& p, cudaStream_t st) {
   return check_launch("gconv_tc_kernel");
 }
 
-// returns 0 on success, < 0 on error, 1 if this launch is not eligible (caller uses the mma.sync kernel)
-int gconv_tc_try(const evk_gconv_desc* d, cudaStream_t st) {
-  if (d->is != 1 || (d->C % 4) != 0 || d->J <= 0) return 1;
+// c: the launch as evk_gconv_fwd validated it.  Returns 0 on success, < 0 on error, 1 if this launch is not eligible
+// (caller uses the mma.sync kernel).
+int gconv_tc_try(const ConvP& c, cudaStream_t st) {
+  if (c.is != 1 || (c.C % 4) != 0 || c.J <= 0) return 1;
   TP p;
-  p.x = d->x; p.w = d->w; p.y = d->y; p.res = d->res; p.bias = d->bias; p.in_len = d->in_len; p.out_len = d->out_len;
-  p.x_sb = d->x_sb; p.x_sh = d->x_sh; p.w_sb = d->w_sb; p.w_sh = d->w_sh; p.w_sq = d->w_sq;
-  p.y_sb = d->y_sb; p.y_sh = d->y_sh; p.r_sb = d->r_sb; p.r_sh = d->r_sh;
-  p.ldx = d->ldx; p.ldw = d->ldw; p.ldy = d->ldy; p.ldr = d->ldr; p.b_sh = d->b_sh;
-  p.Z = d->Z; p.H = d->H; p.C = d->C; p.N = d->N; p.Q = d->Q; p.Tin = d->Tin; p.J = d->J; p.P = d->P;
-  p.os = d->os; p.o0 = d->o0; p.act = d->act; p.slope = d->slope;
-  int mn = d->off[0], mx = d->off[0];
-  for (int i = 0; i < EVK_MAX_TAPS; ++i) {
-    p.off[i] = i < d->Q ? d->off[i] : 0;
-    if (i < d->Q) { mn = min(mn, d->off[i]); mx = max(mx, d->off[i]); }
-  }
-  p.off_min = mn; p.off_max = mx;
-  const long long npos = (long long)d->J * d->P;
+  static_cast<ConvP&>(p) = c;
+  const long long npos = (long long)c.J * c.P;
   const bool two = npos >= 4 * 128;                              // two M tiles per CTA: each weight tile is reused twice (flop/byte wins over CTA count)
-  const int N = d->N;
+  const int N = c.N;
   if (N > 64) return two ? launch_tc<128, 2>(p, st) : launch_tc<128, 1>(p, st);
   if (N > 32) return two ? launch_tc<64, 2>(p, st) : launch_tc<64, 1>(p, st);
   if (N > 16) return two ? launch_tc<32, 2>(p, st) : launch_tc<32, 1>(p, st);

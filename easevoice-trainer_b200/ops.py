@@ -16,8 +16,6 @@ from . import lib as L
 
 ACT_NONE, ACT_LRELU, ACT_RELU, ACT_TANH = 0, 1, 2, 3
 ACT_GELU = 4             # exact erf GELU in the GEMM epilogue (forward only)
-USE_TMA_STRIDED = True   # strided conv forward: phase-split input + stride-1 multi-source tap sum on the TMA kernel
-USE_TMA_WGRAD = True     # weight gradients of tap-free layers: transposes + split-K TMA/wgmma GEMM
 UN_SCALE, UN_LRELU, UN_TANH, UN_MISH, UN_RELU, UN_TANH_FROM_OUT, UN_GELU = 0, 1, 2, 3, 4, 5, 6
 
 _launches = 0          # number of libevk kernel-launching calls (bench.py reports it)
@@ -205,21 +203,15 @@ def stream_id(tag):
 # ------------------------------------------------------------------------------------------------
 # descriptor helpers
 # ------------------------------------------------------------------------------------------------
-def _desc(**kw):
-    d = L.GconvDesc()
-    off = kw.pop("off")
+def _desc(off=(), **kw):
+    """-> GconvDesc with the given fields; every other field is zero or null, except H and G, which default to 1.
+    Tensors are passed by data pointer, an int pointer field as the raw device address."""
+    d = L.GconvDesc(H=1, G=1)
     for k, v in kw.items():
-        if k in ("x", "w", "y", "res", "bias", "in_len", "out_len"):
-            setattr(d, k, v.data_ptr() if v is not None else None)
-        else:
-            setattr(d, k, v)
+        setattr(d, k, v.data_ptr() if isinstance(v, torch.Tensor) else v)
     assert len(off) <= L.MAX_TAPS
     for i, o in enumerate(off):
         d.off[i] = int(o)
-    if not d.H:
-        d.H = 1
-    if not d.G:
-        d.G = 1
     return d
 
 
@@ -478,11 +470,10 @@ def _fwd_like(x, Tin, w, wq0, wqstep, nq, ldw, w_sq, C, N, y, *, J, P, is_, os_,
     _, _, ldy = _rows(y)
     ldr = _rows(res)[2] if res is not None else 0
     wbase = w.data_ptr() + 4 * wq0 * w_sq
-    d = _desc(x=x, w=None, y=y, res=res, bias=bias, in_len=in_len, out_len=out_len,
-              x_sb=Tin * P * ldx, x_sh=x_sh, w_sb=0, w_sh=w_sh, w_sq=wqstep * w_sq, y_sb=Tout * P * ldy, y_sh=y_sh,
+    d = _desc(x=x, w=wbase, y=y, res=res, bias=bias, in_len=in_len, out_len=out_len,
+              x_sb=Tin * P * ldx, x_sh=x_sh, w_sh=w_sh, w_sq=wqstep * w_sq, y_sb=Tout * P * ldy, y_sh=y_sh,
               r_sb=Tout * P * ldr, r_sh=y_sh, ldx=ldx, ldw=ldw, ldy=ldy, ldr=ldr, b_sh=b_sh, Z=B * H, H=H, C=C, N=N, Q=nq,
-              G=1, Tin=Tin, J=J, P=P, is_=is_, os_=os_, o0=o0, Tout=Tout, act=act, slope=float(slope), off=off)
-    d.w = wbase
+              Tin=Tin, J=J, P=P, is_=is_, os_=os_, o0=o0, Tout=Tout, act=act, slope=float(slope), off=off)
     if drop is not None:                      # fused dropout after the activation (TMA kernel epilogue only; the library rejects other routes)
         d.drop_rng, d.drop_sid, d.drop_p = rng_state(x.device).data_ptr(), int(drop[1]), float(drop[0])
     mma = _aligned(x, ldx) and ldw % 4 == 0 and (wbase % 16 == 0) and (d.w_sq % 4 == 0) and x_sh % 4 == 0 and w_sh % 4 == 0
@@ -498,6 +489,15 @@ def _dgrad_phases(dy, Jy, pb, ldb, C, N, Q, dx, Tin, P, stride, pad, dil, H=1):
     for u0, Ju, q0, nq, off in dgrad_phase_plan(Q, stride, pad, dil, Tin):
         _fwd_like(dy, Jy, pb, q0, stride, nq, ldb, w_sq, N, C, dx, J=Ju, P=P, is_=1, os_=stride, o0=u0, Tout=Tin, off=off,
                   H=H, x_sh=N if H > 1 else 0, w_sh=N if H > 1 else 0, y_sh=C if H > 1 else 0)
+
+
+def _phase_split(x, ldx, B, Tin, P, C, stride):
+    """-> (xs, Jp): the stride phase copies of x [B, Tin*P, C], xs[r][b][j*P + w] = x[b][(j*stride + r)*P + w] (zero past
+    the end), j < Jp = ceil(Tin / stride).  A strided conv is a stride-1 tap sum over them."""
+    Jp = (Tin + stride - 1) // stride
+    xs = torch.empty((stride, B, Jp * P, C), device=x.device, dtype=torch.float32)
+    _call("evk_phase_split", _p(x), ldx, Tin * P * ldx, _p(xs), B * Jp * P * C, B, Tin, P, C, stride, Jp)
+    return xs, Jp
 
 
 def dgrad_phase_plan(Q, stride, pad, dil, Tin):
@@ -544,18 +544,15 @@ class _ConvFn(torch.autograd.Function):
         off = [q * dil - pad for q in range(Q)]
         gk = dict(H=G, x_sh=Cg, w_sh=Ng * lda, y_sh=Ng, b_sh=Ng) if G > 1 else {}
         _, _, ldx = _rows(x)
-        if (USE_TMA_STRIDED and 1 < stride <= 4 and G == 1 and in_len is None and C % 4 == 0 and C >= 32 and N >= 32 and lda % 4 == 0
+        if (1 < stride <= 4 and G == 1 and in_len is None and C % 4 == 0 and C >= 32 and N >= 32 and lda % 4 == 0
                 and B * J * P >= 2048 and J * P >= 64 and _aligned(x, ldx) and not _lib().evk_get_precise()):
             # strided conv = stride-1 tap sum over `stride` phase copies of the input (tap u = q*dil - pad reads phase u mod s
             # at shift floor(u / s)): runs on the TMA/wgmma kernel instead of the strided mma.sync one
-            Jp = (Tin + stride - 1) // stride
-            xs = torch.empty((stride, B, Jp * P, C), device=x.device, dtype=torch.float32)
-            _call("evk_phase_split", _p(x), ldx, Tin * P * ldx, _p(xs), B * Jp * P * C, B, Tin, P, C, stride, Jp)
+            xs, Jp = _phase_split(x, ldx, B, Tin, P, C, stride)
             ldr = _rows(res)[2] if res is not None else 0
-            d = _desc(x=xs, w=pa, y=y, res=res, bias=bias, in_len=None, out_len=out_len, x_sb=Jp * P * C, x_sh=0, w_sb=0, w_sh=0,
-                      w_sq=N * lda, y_sb=J * P * N, y_sh=0, r_sb=J * P * ldr, r_sh=0, ldx=C, ldw=lda, ldy=N, ldr=ldr, b_sh=0,
-                      Z=B, H=1, C=C, N=N, Q=Q, G=1, Tin=Jp, J=J, P=P, is_=1, os_=1, o0=0, Tout=J, act=act, slope=float(slope),
-                      off=[u // stride for u in off])
+            d = _desc(x=xs, w=pa, y=y, res=res, bias=bias, out_len=out_len, x_sb=Jp * P * C, w_sq=N * lda, y_sb=J * P * N,
+                      r_sb=J * P * ldr, ldx=C, ldw=lda, ldy=N, ldr=ldr, Z=B, C=C, N=N, Q=Q, Tin=Jp, J=J, P=P, is_=1, os_=1,
+                      Tout=J, act=act, slope=float(slope), off=[u // stride for u in off])
             srca = (ctypes.c_int32 * Q)(*[u % stride for u in off])
             global _launches
             _launches += 1
@@ -585,7 +582,7 @@ class _ConvFn(torch.autograd.Function):
         Ro = J * P
         _, _, ldx_ = _rows(x)
         mma_w = _aligned(x, ldx_) and _aligned(dy, N) and (G == 1 or (Cg % 4 == 0 and Ng % 4 == 0))
-        tma_w = bool(ctx.needs_input_grad[1] and mma_w and USE_TMA_WGRAD and 1 <= stride <= 4 and (stride == 1 or dil == 1) and G == 1
+        tma_w = bool(ctx.needs_input_grad[1] and mma_w and 1 <= stride <= 4 and (stride == 1 or dil == 1) and G == 1
                      and in_len is None and B * J * P >= 2048 and J * P >= 64 and C >= 32 and N >= 32 and C % 4 == 0
                      and not _lib().evk_get_precise())
         want_b = has_bias and ctx.needs_input_grad[3]
@@ -612,10 +609,8 @@ class _ConvFn(torch.autograd.Function):
                     dx.zero_()
                 _dgrad_phases(dy, J, pb, pb.shape[2], Cg, Ng, Q, dx, Tin, P, stride, pad, dil, H=G)
             else:
-                d = _desc(x=dx, w=pa, y=dy, res=None, bias=None, in_len=None, out_len=None,
-                          x_sb=Tin * P * C, x_sh=0, w_sb=0, w_sh=0, w_sq=N * lda, y_sb=J * P * N, y_sh=0, r_sb=0, r_sh=0,
-                          ldx=C, ldw=lda, ldy=N, ldr=0, b_sh=0, Z=B, H=1, C=C, N=N, Q=Q, G=G, Tin=Tin, J=J, P=P, is_=stride,
-                          os_=1, o0=0, Tout=J, act=0, slope=0.0, off=offs)
+                d = _desc(x=dx, w=pa, y=dy, x_sb=Tin * P * C, w_sq=N * lda, y_sb=J * P * N, ldx=C, ldw=lda, ldy=N, Z=B,
+                          C=C, N=N, Q=Q, G=G, Tin=Tin, J=J, P=P, is_=stride, os_=1, Tout=J, off=offs)
                 _run_desc("evk_conv_direct_dgrad", d)
             if in_len is not None:
                 dxm = torch.empty_like(dx)
@@ -633,9 +628,7 @@ class _ConvFn(torch.autograd.Function):
                 if stride == 1:
                     srcs = [(x, ldx, Tin, list(range(Q)), offs)]
                 else:
-                    Jp = (Tin + stride - 1) // stride
-                    xs = torch.empty((stride, B, Jp * P, C), device=dy.device, dtype=torch.float32)
-                    _call("evk_phase_split", _p(x), ldx, Tin * P * ldx, _p(xs), B * Jp * P * C, B, Tin, P, C, stride, Jp)
+                    xs, Jp = _phase_split(x, ldx, B, Tin, P, C, stride)
                     srcs = []
                     for rho in range(stride):
                         qs = [q for q in range(Q) if offs[q] % stride == rho]
@@ -659,19 +652,15 @@ class _ConvFn(torch.autograd.Function):
                     _call_f("evk_conv_wgrad_tma", 2.0 * B * Ro * N * C * nq, _p(dyt), ldo, N * ldo, _p(xt), ldi, C * ldi, B * C * ldi,
                             dpa.data_ptr() + 4 * qs[0] * N * lda, lda, qstep * N * lda, B, N, C, Ro, Ri, nq, P, offa, splits,
                             tag=f"B{B} Ro{Ro} P{P} C{C} N{N} nq{nq} splits{splits}")
-            elif mma:
-                d = _desc(x=x, w=dpa, y=dy, res=None, bias=None, in_len=in_len, out_len=None,
-                          x_sb=Tin * P * ldx, x_sh=Cg if G > 1 else 0, w_sb=0, w_sh=Ng * lda if G > 1 else 0, w_sq=N * lda,
-                          y_sb=J * P * N, y_sh=Ng if G > 1 else 0, r_sb=0, r_sh=0, ldx=ldx, ldw=lda, ldy=N, ldr=0, b_sh=0,
-                          Z=B * G, H=G, C=Cg, N=Ng, Q=Q, G=1, Tin=Tin, J=J, P=P, is_=stride, os_=1, o0=0, Tout=J, act=0,
-                          slope=0.0, off=offs)
-                _run_desc("evk_gconv_wgrad", d)
             else:
-                d = _desc(x=x, w=dpa, y=dy, res=None, bias=None, in_len=in_len, out_len=None,
-                          x_sb=Tin * P * ldx, x_sh=0, w_sb=0, w_sh=0, w_sq=N * lda, y_sb=J * P * N, y_sh=0, r_sb=0, r_sh=0,
-                          ldx=ldx, ldw=lda, ldy=N, ldr=0, b_sh=0, Z=B, H=1, C=C, N=N, Q=Q, G=G, Tin=Tin, J=J, P=P,
-                          is_=stride, os_=1, o0=0, Tout=J, act=0, slope=0.0, off=offs)
-                _run_desc("evk_conv_direct_wgrad", d)
+                # the mma.sync kernel runs the groups as the inner batch (H = groups), the direct kernel takes G
+                if mma and G > 1:
+                    grp = dict(Z=B * G, H=G, C=Cg, N=Ng, x_sh=Cg, w_sh=Ng * lda, y_sh=Ng)
+                else:
+                    grp = dict(Z=B, C=C, N=N, G=G)
+                d = _desc(x=x, w=dpa, y=dy, in_len=in_len, x_sb=Tin * P * ldx, w_sq=N * lda, y_sb=J * P * N, ldx=ldx, ldw=lda,
+                          ldy=N, Q=Q, Tin=Tin, J=J, P=P, is_=stride, os_=1, Tout=J, off=offs, **grp)
+                _run_desc("evk_gconv_wgrad" if mma else "evk_conv_direct_wgrad", d)
         if has_res and ctx.needs_input_grad[4]:
             dres = dy
         return dx, dpa, None, dbias, dres, None
@@ -702,9 +691,6 @@ def fused_dropout_ok(x, w, act):
     return w.Q == 1 and rows >= 512 and C >= 64 and C % 4 == 0 and N >= 64 and N % 4 == 0 and x.data_ptr() % 16 == 0
 
 
-USE_GEMV = os.environ.get("EVK_GEMV", "1") != "0"     # skinny (<= 4 rows, no-grad) Linear launches stream the weight once (evk_gemv_rows)
-
-
 def _gemv_rows(x, w, bias, act, slope):
     """The token step of the KV-cache decode: [..., C] with <= 4 rows in total -> [..., N], exact fp32, one pass over PA[0]."""
     C = x.shape[-1]
@@ -729,7 +715,8 @@ def linear_rows(x, w: PackedW, bias=None, act=ACT_NONE, slope=0.0):
 def linear(x, w: PackedW, bias=None, act=ACT_NONE, slope=0.0, out_len=None, in_len=None, res=None, drop=None):
     """nn.Linear / 1x1 conv on [B, T, C] or [rows, C].  drop = (p, tag): dropout_p(relu(x W^T + b)) with the dropout applied in
     the GEMM epilogue when fused_dropout_ok (else as a separate kernel)."""
-    if (USE_GEMV and not torch.is_grad_enabled() and w.Q == 1 and res is None and out_len is None and in_len is None
+    # skinny (<= 4 rows, no-grad) launches stream the weight once (evk_gemv_rows)
+    if (not torch.is_grad_enabled() and w.Q == 1 and res is None and out_len is None and in_len is None
             and (drop is None or drop[0] <= 0.0) and act in (ACT_NONE, ACT_RELU, ACT_LRELU)):
         C = x.shape[-1]
         rows = x.numel() // max(C, 1)
@@ -782,10 +769,8 @@ class _ConvTFn(torch.autograd.Function):
             dpa = dpa_buffer(pa)
             _, _, ldx = _rows(x)
             # dPA[q][ci][co] += sum_t X[t][ci] * dY[t*stride - pad + q][co]: "x" role = dY (shifted), "y" role = X
-            d = _desc(x=dy, w=dpa, y=x, res=None, bias=None, in_len=None, out_len=None,
-                      x_sb=Tout * Cout, x_sh=0, w_sb=0, w_sh=0, w_sq=Cin * lda, y_sb=Tin * ldx, y_sh=0, r_sb=0, r_sh=0,
-                      ldx=Cout, ldw=lda, ldy=ldx, ldr=0, b_sh=0, Z=B, H=1, C=Cout, N=Cin, Q=Q, G=1, Tin=Tout, J=Tin, P=1,
-                      is_=stride, os_=1, o0=0, Tout=Tin, act=0, slope=0.0, off=off)
+            d = _desc(x=dy, w=dpa, y=x, x_sb=Tout * Cout, w_sq=Cin * lda, y_sb=Tin * ldx, ldx=Cout, ldw=lda, ldy=ldx, Z=B,
+                      C=Cout, N=Cin, Q=Q, Tin=Tout, J=Tin, P=1, is_=stride, os_=1, Tout=Tin, off=off)
             mma = _aligned(dy, Cout) and _aligned(x, ldx)
             _run_desc("evk_gconv_wgrad" if mma else "evk_conv_direct_wgrad", d)
         if ctx.needs_input_grad[3]:
@@ -1437,9 +1422,8 @@ def _transpose_cl(x, ldT):
 
 
 def _bgemm(fn, x, x_sb, x_sh, ldx, w, w_sb, w_sh, ldw, y, y_sb, y_sh, ldy, Z, H, C, N, rows):
-    d = _desc(x=x, w=w, y=y, res=None, bias=None, in_len=None, out_len=None, x_sb=x_sb, x_sh=x_sh, w_sb=w_sb, w_sh=w_sh,
-              w_sq=0, y_sb=y_sb, y_sh=y_sh, r_sb=0, r_sh=0, ldx=ldx, ldw=ldw, ldy=ldy, ldr=0, b_sh=0, Z=Z, H=H, C=C, N=N, Q=1,
-              G=1, Tin=rows, J=rows, P=1, is_=1, os_=1, o0=0, Tout=rows, act=0, slope=0.0, off=[0])
+    d = _desc(x=x, w=w, y=y, x_sb=x_sb, x_sh=x_sh, w_sb=w_sb, w_sh=w_sh, y_sb=y_sb, y_sh=y_sh, ldx=ldx, ldw=ldw, ldy=ldy,
+              Z=Z, H=H, C=C, N=N, Q=1, Tin=rows, J=rows, P=1, is_=1, os_=1, Tout=rows)
     _run_desc(fn, d)
 
 
