@@ -176,8 +176,8 @@ using namespace evk;
 extern "C" int evk_attn_pad_fwd(const float* q, const float* k, const float* v, int32_t ld, float* o, int32_t ldo, int32_t B,
                                 int32_t H, int32_t L, const int64_t* lens, float scale, cudaStream_t st) {
   EVK_REQUIRE(q && k && v && o && lens, EVK_ERR_ARG, "attn_pad: null tensor");
-  EVK_REQUIRE(B > 0 && H > 0 && L > 0 && L <= 512 && B <= 65535 && H <= 65535, EVK_ERR_ARG,
-              "attn_pad: bad sizes B=%d H=%d L=%d (1 <= L <= 512)", B, H, L);
+  EVK_REQUIRE(B > 0 && H > 0 && L > 0 && H <= 65535 && (long long)B * cdiv(L, BQ) <= 0x7fffffff, EVK_ERR_ARG,
+              "attn_pad: bad sizes B=%d H=%d L=%d", B, H, L);
   EVK_REQUIRE(ld % 4 == 0 && ldo % 2 == 0 && ld >= HD && ldo >= HD, EVK_ERR_ARG,
               "attn_pad: row pitches must be multiples of 4 (ld) / 2 (ldo) floats");
   EVK_REQUIRE(((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) % 16 == 0 && (uintptr_t)o % 8 == 0, EVK_ERR_ARG,

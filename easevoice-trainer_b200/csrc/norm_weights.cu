@@ -343,17 +343,20 @@ __global__ void zero_kernel(float* p, int n) {
 // ---- per-channel normalisation over time (GroupNorm(C, C) of the HuBERT feature extractor), channels-last, forward only ------
 // One CTA per (32 channels, batch item): 8 time lanes x 32 channel lanes; pass 1 accumulates shifted sums (shift = the channel's
 // first sample, which keeps the one-pass variance stable on DC-heavy inputs), pass 2 normalises (+ optional exact GELU).
+// With lens, item b is normalised over its first n = lens[b] frames only and frames t >= n are written as 0: the sums visit
+// t = lane, lane + 8, ... < n in a fixed order, so the statistics of a row depend neither on T nor on what the padding holds.
 __global__ void __launch_bounds__(256) instnorm_cl_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ gamma,
                                                           const float* __restrict__ beta, float eps, int act_gelu, float* __restrict__ y,
-                                                          int ldy, int T, int C) {
+                                                          int ldy, int T, int C, const int* __restrict__ lens) {
   const int c = blockIdx.x * 32 + (threadIdx.x & 31), tl = threadIdx.x >> 5, b = blockIdx.y;
   const float* xb = x + (long long)b * T * ldx;
   float* yb = y + (long long)b * T * ldy;
+  const int n = lens ? min(max(lens[b], 0), T) : T;
   const bool ok = c < C;
   const float shift = ok ? xb[c] : 0.f;
   float s1 = 0.f, s2 = 0.f;
   if (ok)
-    for (int t = tl; t < T; t += 8) { const float v = xb[(long long)t * ldx + c] - shift; s1 += v; s2 += v * v; }
+    for (int t = tl; t < n; t += 8) { const float v = xb[(long long)t * ldx + c] - shift; s1 += v; s2 += v * v; }
   __shared__ float sh1[8][32], sh2[8][32];
   sh1[tl][threadIdx.x & 31] = s1; sh2[tl][threadIdx.x & 31] = s2;
   __syncthreads();
@@ -361,13 +364,14 @@ __global__ void __launch_bounds__(256) instnorm_cl_kernel(const float* __restric
 #pragma unroll
   for (int i = 0; i < 8; ++i) { a += sh1[i][threadIdx.x & 31]; q += sh2[i][threadIdx.x & 31]; }
   if (!ok) return;
-  const float md = a / (float)T, var = fmaxf(q / (float)T - md * md, 0.f);
+  const float md = a / (float)n, var = fmaxf(q / (float)n - md * md, 0.f);
   const float mean = md + shift, rstd = rsqrtf(var + eps), g = gamma[c] * rstd, bb = beta[c] - mean * g;
-  for (int t = tl; t < T; t += 8) {
+  for (int t = tl; t < n; t += 8) {
     float v = xb[(long long)t * ldx + c] * g + bb;
     if (act_gelu) v = 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
     yb[(long long)t * ldy + c] = v;
   }
+  for (int t = n + tl; t < T; t += 8) yb[(long long)t * ldy + c] = 0.f;
 }
 
 }  // namespace evk
@@ -493,8 +497,8 @@ extern "C" int evk_colsum(const float* x, int64_t rows, int32_t n, int32_t ld, f
 }
 
 extern "C" int evk_instnorm_cl(const float* x, int32_t ldx, const float* gamma, const float* beta, float eps, int32_t act_gelu, float* y,
-                               int32_t ldy, int32_t B, int32_t T, int32_t C, evk_stream_t stream) {
+                               int32_t ldy, int32_t B, int32_t T, int32_t C, const int32_t* lens, evk_stream_t stream) {
   EVK_REQUIRE(x && gamma && beta && y && B >= 1 && T >= 1 && C >= 1 && ldx >= C && ldy >= C, EVK_ERR_ARG, "instnorm_cl: bad arguments");
-  instnorm_cl_kernel<<<dim3(cdiv(C, 32), B), 256, 0, ST>>>(x, ldx, gamma, beta, eps, act_gelu, y, ldy, T, C);
+  instnorm_cl_kernel<<<dim3(cdiv(C, 32), B), 256, 0, ST>>>(x, ldx, gamma, beta, eps, act_gelu, y, ldy, T, C, lens);
   return check_launch("instnorm_cl");
 }

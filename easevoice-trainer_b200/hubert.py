@@ -8,8 +8,14 @@ model per file.  This module is that forward on the library's kernels, same stat
 
   feature extractor  strided Conv1d stack on the wgmma / mma.sync conv kernels, GroupNorm(512, 512) + GELU in one kernel
                      (`evk_instnorm_cl`), exact-erf GELU (`evk_unary` op 6)
-  encoder            grouped k = 128 positional conv (weight-norm folded on the host once), 12 post-LN blocks: three Linear
-                     launches for q / k / v, batched attention GEMMs + masked softmax (`ops.attention`), LayerNorm kernels
+  encoder            grouped k = 128 positional conv (weight-norm folded on the host once), 12 post-LN blocks: one packed QKV
+                     Linear, fused attention with per-row key lengths (`evk_attn_pad_fwd`, head dim 64), LayerNorm kernels
+
+Ragged batches: row b of `input_values` may hold only its first `lengths[b]` samples.  The strided convolutions need no mask (a
+valid output frame reads valid samples only); the GroupNorm of conv 0 takes its statistics over the row's own frames, the
+projected features are zeroed past the row's last frame before the positional conv (which then reads zeros there, as in a
+call on the row alone) and attention sees the row's own frames as keys.  Each valid frame is therefore what a call on that
+row alone computes, up to the rounding of GEMM tiles of another shape.
 
 Inference only (no gradients); fp32 storage, TF32 tensor-core products like the rest of the library.  No CPU fallback.
 """
@@ -101,6 +107,29 @@ class HubertModel(ParamTree):
         return net.to(device).eval()
 
     # ---- forward ------------------------------------------------------------------------------------------------------------
+    def conv_lengths(self, n_samples):
+        """Output frames of every feature-extractor conv for a row of n_samples samples (floor((n - k) / s) + 1 per layer)."""
+        out, n = [], int(n_samples)
+        for k, s in zip(self.cfg["conv_kernel"], self.cfg["conv_stride"]):
+            n = (n - k) // s + 1 if n >= k else 0
+            out.append(n)
+        return out
+
+    def num_frames(self, n_samples):
+        """Frames of last_hidden_state for a row of n_samples 16 kHz samples: floor((n - 400) / 320) + 1 for HuBERT-base,
+        0 below one receptive field."""
+        return self.conv_lengths(n_samples)[-1]
+
+    def _qkv(self, i):
+        """q_proj, k_proj and v_proj of layer i as one Linear: the weights concatenated and packed once per parameter version."""
+        key = ("qkv", i)
+        if key not in self._active:
+            p = f"encoder.layers.{i}.attention."
+            w = torch.cat([self.P(p + n + ".weight").detach() for n in ("q_proj", "k_proj", "v_proj")])
+            b = torch.cat([self.P(p + n + ".bias").detach() for n in ("q_proj", "k_proj", "v_proj")])
+            self._active[key] = (ops.pack_weight(w, None, need_pb=False), b)
+        return self._active[key]
+
     POS_PIECE = 48           # taps per launch of the positional conv (the descriptor holds EVK_MAX_TAPS = 48 tap offsets)
 
     def _pos_weight(self):
@@ -133,10 +162,25 @@ class HubertModel(ParamTree):
         return ops.gelu(pos)
 
     @torch.no_grad()
-    def forward(self, input_values):
-        """input_values [B, L] float (16 kHz samples, un-normalised as Normalize.ssl passes them) -> {"last_hidden_state": [B, T, H]}.
-        All rows are taken at full length (the reference runs one utterance per call)."""
+    def forward(self, input_values, lengths=None):
+        """input_values [B, L] float on the model's device (16 kHz samples, un-normalised as Normalize.ssl passes them), lengths
+        (optional, B ints): the valid samples of each row, None for every row at full length -> {"last_hidden_state": [B, T, H]}
+        with T = num_frames(L).  Frames t < num_frames(lengths[b]) of row b are that row's features; the frames after them
+        are finite and unspecified.  A row shorter than one receptive field (400 samples) raises ValueError."""
         c = self.cfg
+        B, L = input_values.shape
+        lens = [L] * B if lengths is None else [int(n) for n in lengths]
+        if len(lens) != B:
+            raise ValueError(f"{len(lens)} lengths for {B} rows")
+        for b, n in enumerate(lens):
+            if n > L or self.num_frames(n) < 1:
+                raise ValueError(f"row {b}: {n} samples; a row needs at least one receptive field of the feature extractor "
+                                 f"(400 samples for HuBERT-base) and at most the batch width {L}")
+        dev = input_values.device
+        fl = [self.conv_lengths(n) for n in lens]
+        idx = torch.tensor([f[0] for f in fl] + [f[-1] for f in fl], dtype=torch.int64).to(dev)      # one H2D copy
+        n0_d, nt_d = idx[:B].int(), idx[B:].int()
+        nt64_d = idx[B:]
         self._active, self._memo_pack = self.packed_for_inference(), True
         try:
             # channels-last [B, L, 1], widened to 4 zero-padded channels (16-byte rows) like the discriminators' waveform input
@@ -146,22 +190,22 @@ class HubertModel(ParamTree):
                 x = ops.conv(x, w, None, stride=s)
                 if i == 0:
                     x = ops.instnorm_cl(x, self.P("feature_extractor.conv_layers.0.layer_norm.weight"),
-                                        self.P("feature_extractor.conv_layers.0.layer_norm.bias"), c["layer_norm_eps"], gelu_after=True)
+                                        self.P("feature_extractor.conv_layers.0.layer_norm.bias"), c["layer_norm_eps"], gelu_after=True,
+                                        lens=n0_d)
                 else:
                     x = ops.gelu(x)
             eps = c["layer_norm_eps"]
             x = ops.layernorm(x, self.P("feature_projection.layer_norm.weight"), self.P("feature_projection.layer_norm.bias"), eps=eps)
             h = ops.linear(x, self.w("feature_projection.projection", need_pb=False), self.b("feature_projection.projection"))
+            h = ops.rowmask(h, nt_d)
             pos = self._pos_conv(h)
             h = ops.layernorm(h, self.P("encoder.layer_norm.weight"), self.P("encoder.layer_norm.bias"), res=pos, eps=eps)
             H = c["num_attention_heads"]
             scale = (c["hidden_size"] // H) ** -0.5
             for i in range(c["num_hidden_layers"]):
                 p = f"encoder.layers.{i}."
-                q = ops.linear(h, self.w(p + "attention.q_proj", need_pb=False), self.b(p + "attention.q_proj"))
-                k = ops.linear(h, self.w(p + "attention.k_proj", need_pb=False), self.b(p + "attention.k_proj"))
-                v = ops.linear(h, self.w(p + "attention.v_proj", need_pb=False), self.b(p + "attention.v_proj"))
-                a = ops.attention(q, k, v, heads=H, scale=scale, tag=f"hubert.attn{i}")
+                wqkv, bqkv = self._qkv(i)
+                a = ops.attention_pad(ops.linear(h, wqkv, bqkv), heads=H, lens=nt64_d, scale=scale)
                 a = ops.linear(a, self.w(p + "attention.out_proj", need_pb=False), self.b(p + "attention.out_proj"))
                 h = ops.layernorm(h, self.P(p + "layer_norm.weight"), self.P(p + "layer_norm.bias"), res=a, eps=eps)
                 f = ops.gelu(ops.linear(h, self.w(p + "feed_forward.intermediate_dense", need_pb=False),

@@ -832,14 +832,16 @@ def gelu(x):
     return y
 
 
-def instnorm_cl(x, gamma, beta, eps=1e-5, gelu_after=False):
-    """GroupNorm(C, C) over time of a channels-last [B, T, C] tensor (+ optional exact GELU); inference only."""
+def instnorm_cl(x, gamma, beta, eps=1e-5, gelu_after=False, lens=None):
+    """GroupNorm(C, C) over time of a channels-last [B, T, C] tensor (+ optional exact GELU); inference only.  lens (int32
+    device [B], optional): item b is normalised over its first lens[b] frames and the frames after them are 0."""
     x = _cl(x.detach())
     B, T, C = x.shape
     _, _, ld = _rows(x)
+    assert lens is None or (lens.dtype == torch.int32 and lens.is_cuda and lens.numel() == B)
     y = torch.empty((B, T, C), device=x.device, dtype=torch.float32)
     _call("evk_instnorm_cl", _p(x), ld, _p(gamma.detach().contiguous()), _p(beta.detach().contiguous()), ctypes.c_float(eps),
-          1 if gelu_after else 0, _p(y), C, B, T, C)
+          1 if gelu_after else 0, _p(y), C, B, T, C, _p(None if lens is None else lens.contiguous()))
     return y
 
 
@@ -2330,6 +2332,20 @@ def resample_poly(x, h, up, down, n_pre_remove, n_out, out=None):
     assert out.stride(1) == 1 and out.shape == (rows, n_out)
     _call("evk_resample_poly", _p(x), rows, L, x.stride(0), _p(h), h.numel(), up, down, n_pre_remove, _p(out), n_out, out.stride(0))
     return out
+
+
+def ssl_normalize(a, lens):
+    """evk_ssl_normalize: Normalize._name2go's loudness normalisation of the rows of a [B, L] (fp32 device, row b holding
+    lens[b] samples; lens int32 device [B]) -> (a32 int16 [B, L], a32b fp32 [B, L], status int32 [B]: EVK_SSL_OK = 0,
+    EVK_SSL_SKIP = 1, EVK_SSL_NONFINITE = 2); entries past a row's length are 0."""
+    assert a.dim() == 2 and a.dtype == torch.float32 and a.stride(1) == 1
+    assert lens.dtype == torch.int32 and lens.is_cuda and lens.numel() == a.shape[0]
+    B, L = a.shape
+    a32 = torch.empty((B, L), device=a.device, dtype=torch.int16)
+    a32b = torch.empty((B, L), device=a.device, dtype=torch.float32)
+    status = torch.empty(B, device=a.device, dtype=torch.int32)
+    _call("evk_ssl_normalize", _p(a), a.stride(0), _p(lens.contiguous()), B, L, _p(a32), L, _p(a32b), L, _p(status))
+    return a32, a32b, status
 
 
 def vr_assemble(x, pred, pred_tta, coef, bands, gains, high=None, mirror_lo=0, top=-1):

@@ -171,9 +171,11 @@ int evk_spec_to_mel(const float* spec, int64_t rows, int32_t ld_spec, int32_t n_
  * bwd: dx = dy*f'(x) (op 5 there: tanh with the derivative taken from the saved OUTPUT) */
 /* GroupNorm with one channel per group over the time axis of a channels-last tensor (torch.nn.GroupNorm(C, C) of the HuBERT
  * feature extractor, transformers modeling_hubert.py HubertGroupNormConvLayer): y[b][t][c] = (x - mean_t) * rsqrt(var_t + eps)
- * * gamma[c] + beta[c], biased variance; optional exact GELU applied to the result (act_gelu != 0).  Forward only. */
+ * * gamma[c] + beta[c], biased variance; optional exact GELU applied to the result (act_gelu != 0).  Forward only.
+ * lens (nullable, int32 device [B]): mean and variance of item b over t < lens[b] only, frames t >= lens[b] written as 0; a
+ * fixed summation order (no atomics), so an item's result does not depend on T or on the padding.  NULL: every frame. */
 int evk_instnorm_cl(const float* x, int32_t ldx, const float* gamma, const float* beta, float eps, int32_t act_gelu, float* y,
-                    int32_t ldy, int32_t B, int32_t T, int32_t C, evk_stream_t stream);
+                    int32_t ldy, int32_t B, int32_t T, int32_t C, const int32_t* lens, evk_stream_t stream);
 int evk_unary(int32_t op, float alpha, const float* x, int32_t ldx, float* y, int32_t ldy, int64_t rows, int32_t C,
               evk_stream_t stream);
 int evk_unary_bwd(int32_t op, float alpha, const float* x, int32_t ldx, const float* dy, int32_t lddy, float* dx,
@@ -480,9 +482,10 @@ int evk_scaled_adam(float* p, float* g, float* delta, float* v, const int64_t* c
 /* Fused bidirectional attention with per-row key lengths, head dim 64, inference only:
  *   O = softmax(Q K^T * scale + mask) V   per (batch b, head h),   mask: key j is visible to every query iff j < lens[b].
  * q/k/v: [B, L, ld] with head h at columns h*64.. (usually the three column blocks of one packed QKV Linear output);
- * o: [B, L, ldo].  Requires 1 <= lens[b] <= L <= 512 (lens: int64 device [B], values outside are clamped to [1, L]),
- * ld % 4 == 0, ldo % 2 == 0, q/k/v 16-byte and o 8-byte aligned.  Query rows at or past lens[b] are computed like any
- * other (finite).  Scores are never materialised (online softmax); TF32 mma.sync with fp32 accumulation (3xTF32 under
+ * o: [B, L, ldo].  Requires 1 <= lens[b] <= L (lens: int64 device [B], values outside are clamped to [1, L]),
+ * ld % 4 == 0, ldo % 2 == 0, q/k/v 16-byte and o 8-byte aligned.  L has no upper bound: keys stream through in tiles of 32
+ * and only the tiles that hold a visible key are read (BERT's 512-position limit is enforced by its caller).  Query rows at
+ * or past lens[b] are computed like any other (finite).  Scores are never materialised (online softmax); TF32 mma.sync with fp32 accumulation (3xTF32 under
  * evk_set_precise(1)); no atomics, bit-reproducible. */
 int evk_attn_pad_fwd(const float* q, const float* k, const float* v, int32_t ld, float* o, int32_t ldo, int32_t B,
                      int32_t H, int32_t L, const int64_t* lens, float scale, evk_stream_t stream);
@@ -598,6 +601,19 @@ int evk_vr_mag_norm(const float* spec, int64_t n, float* mag, float* coef, evk_s
  * n = 0 .. n_out-1.  x [rows][ldx], y [rows][ldy]. */
 int evk_resample_poly(const float* x, int32_t rows, int32_t L, int32_t ldx, const float* h, int32_t nh, int32_t up, int32_t down,
                       int32_t n_pre_remove, float* y, int32_t n_out, int32_t ldy, evk_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Normalize.ssl (normalize.py:151-179), the waveform half: loudness normalisation of B zero-padded rows of 32 kHz samples.
+ * ------------------------------------------------------------------------------------------ */
+enum evk_ssl_status { EVK_SSL_OK = 0, EVK_SSL_SKIP = 1, EVK_SSL_NONFINITE = 2 };
+/* Row b of a [B][lda] holds lens[b] (int32 device) samples.  m = max |a| (NaN if a sample is NaN);
+ * a32 [B][ld16] = int16((a / m * c1) + c2 * a) and a32b [B][ldb] = (a / m * c1b) + c2b * a with c1 = 0.95 * 0.5 * 32768,
+ * c2 = 0.5 * 32768, c1b = 0.95 * 0.5 * 1145.14, c2b = 0.5 * 1145.14 (float64 products rounded to float32), every operation a
+ * float32 operation in that order (bit-identical to numpy); the int16 conversion truncates to int32 and keeps the low 16 bits
+ * (x86 numpy's astype).  Entries at or past lens[b] are 0.  status[b] (int32 device): EVK_SSL_SKIP if (double)m > 2.2,
+ * else EVK_SSL_NONFINITE if m is 0 or NaN (the outputs are then NaN), else EVK_SSL_OK. */
+int evk_ssl_normalize(const float* a, int32_t lda, const int32_t* lens, int32_t B, int32_t L, int16_t* a32, int32_t ld16,
+                      float* a32b, int32_t ldb, int32_t* status, evk_stream_t stream);
 /* Half spectra of every band of both outputs, the input of evk_istft.  From the combined spectrogram x [2][n_rows][l]
  * (complex) and the net's pred [2][n_rows][l] (pred_tta nullable: (pred + pred_tta) * 0.5 * coef, else pred * coef; coef a
  * device scalar): y = pred exp(i angle(x)) (angle(0) = 0), v = x - y.  Band b (host int64 [n_bands][6] = (n_fft,
