@@ -1,31 +1,12 @@
 """Statistical quality of the attention probability-dropout draw (csrc/flash.cu: drop_row / drop_pair / drop_one), restated
-here in numpy uint32 arithmetic.  The draw was made as cheap as a counter-based generator can be (one multiply-compare per element:
-the attention kernels are bound by the integer pipe), so its statistics are checked explicitly: drop fraction, per-row / per-column
-fractions at the binomial spread, no correlation between neighbouring columns, the two draws of a column pair, rows, diagonals."""
+in numpy uint32 arithmetic by tests/attention_ref.py.  The draw was made as cheap as a counter-based generator can be (one
+multiply-compare per element: the attention kernels are bound by the integer pipe), so its statistics are checked explicitly:
+drop fraction, per-row / per-column fractions at the binomial spread, no correlation between neighbouring columns, the two draws
+of a column pair, rows, diagonals."""
 import numpy as np
 import pytest
 
-M32 = np.uint64(0xFFFFFFFF)
-C, M1, M2 = 0xC2B2AE3D, 0x7FEB352D, 0x846CA68B         # DROP_C, DROP_M1, DROP_M2
-
-
-def _u32(x):
-    return (x & M32).astype(np.uint64)
-
-
-def drop_row(row, s0):
-    x = _u32(row * np.uint64(0x9E3779B1) + np.uint64(s0))
-    x ^= x >> np.uint64(15); x = _u32(x * np.uint64(0x85EBCA77)); x ^= x >> np.uint64(13); x = _u32(x * np.uint64(0xC2B2AE35)); x ^= x >> np.uint64(16)
-    return x
-
-
-def keep_matrix(z, L, s0, s1, p):
-    thr = np.uint64(min(max(p * 4294967296.0, 1.0), 4294967295.0))
-    rh = drop_row(np.arange(L, dtype=np.uint64) + np.uint64(z * L), s0)[:, None]
-    cols = np.arange(L, dtype=np.uint64)
-    h = rh ^ _u32((cols >> np.uint64(1)) * np.uint64(C) + np.uint64(s1))[None, :]
-    x = np.where((cols & np.uint64(1)).astype(bool)[None, :], _u32(h * np.uint64(M2)), _u32(h * np.uint64(M1)))
-    return x >= thr
+from tests.attention_ref import keep_matrix, philox
 
 
 def _corr(a, b):
@@ -55,3 +36,10 @@ def test_dropout_draw_differs_between_heads_and_streams():
     assert (a != keep_matrix(1, 256, 123, 456, 0.1)).mean() > 0.1          # another (batch, head): rows hash differently
     assert (a != keep_matrix(0, 256, 124, 456, 0.1)).mean() > 0.1          # another seed word
     assert (a != keep_matrix(0, 256, 123, 457, 0.1)).mean() > 0.1
+
+
+def test_philox_known_answer():
+    """Philox-4x32-10 test vectors of Random123 (Salmon et al., SC'11): key (k0, k1), counter (c0, c1, c2, c3)"""
+    M = 0xFFFFFFFF
+    assert philox(0, 0, 0) == (0x6627E8D5, 0xE169C58D, 0xBC57AC4C, 0x9B00DBD8)
+    assert philox(M | M << 32, M | M << 32, M | M << 32) == (0x408F276D, 0x41C83B0E, 0xA20BC7C6, 0x6D5451FD)
