@@ -53,12 +53,15 @@ __global__ void attn_softmax_kernel(float* __restrict__ S, int lds, int H, int T
   for (int j = threadIdx.x; j < Tk; j += blockDim.x) s[j] *= inv;
 }
 
-// dS_raw = P * (dP - sum_j dP*P) * scale (in place on dP); drelk[row][r] = dS_raw[i][i + r - win]
-__global__ void attn_softmax_bwd_kernel(const float* __restrict__ P, float* __restrict__ dP, int lds, int Tq, int Tk, float scale,
-                                        float* __restrict__ drelk, int win) {
+// dS_raw = P * (dP - sum_j dP*P) * scale (in place on dP), 0 where the forward filled the logit (a filled logit passes no
+// gradient: with fill = -1e4 a dead query row holds 1/Tk, not 0); drelk[row][r] = dS_raw[i][i + r - win]
+__global__ void attn_softmax_bwd_kernel(const float* __restrict__ P, float* __restrict__ dP, int lds, int H, int Tq, int Tk,
+                                        float scale, float* __restrict__ drelk, int win, const int* __restrict__ qlen,
+                                        const int* __restrict__ klen) {
   __shared__ float red[33];
   const long long row = blockIdx.x;
-  const int i = (int)(row % Tq);
+  const int z = (int)(row / Tq), i = (int)(row - (long long)z * Tq), b = z / H;
+  const int kl = (qlen && i >= qlen[b]) ? 0 : (klen ? min(klen[b], Tk) : Tk);
   const float* p = P + row * lds;
   float* d = dP + row * lds;
   float dot = 0.f;
@@ -66,7 +69,7 @@ __global__ void attn_softmax_bwd_kernel(const float* __restrict__ P, float* __re
   dot = block_sum(dot, red);
   const int W = 2 * win + 1;
   for (int j = threadIdx.x; j < Tk; j += blockDim.x) {
-    const float v = p[j] * (d[j] - dot) * scale;
+    const float v = j < kl ? p[j] * (d[j] - dot) * scale : 0.f;
     d[j] = v;
     if (drelk) {
       const int r = j - i + win;
@@ -177,12 +180,12 @@ extern "C" int evk_attn_softmax(float* S, int32_t lds, int32_t Z, int32_t H, int
   attn_softmax_kernel<<<(unsigned)rows, bs, 0, ST>>>(S, lds, H, Tq, Tk, scale, relk, win, qlen, klen, fill);
   return check_launch("attn_softmax");
 }
-extern "C" int evk_attn_softmax_bwd(const float* P, float* dP, int32_t lds, int32_t Z, int32_t Tq, int32_t Tk, float scale,
-                                    float* drelk, int32_t win, evk_stream_t stream) {
-  EVK_REQUIRE(P && dP && Z >= 1, EVK_ERR_ARG, "attn_softmax_bwd: bad arguments");
+extern "C" int evk_attn_softmax_bwd(const float* P, float* dP, int32_t lds, int32_t Z, int32_t H, int32_t Tq, int32_t Tk, float scale,
+                                    float* drelk, int32_t win, const int32_t* qlen, const int32_t* klen, evk_stream_t stream) {
+  EVK_REQUIRE(P && dP && Z >= 1 && H >= 1, EVK_ERR_ARG, "attn_softmax_bwd: bad arguments");
   const long long rows = (long long)Z * Tq;
   const int bs = Tk >= 256 ? 256 : (Tk >= 128 ? 128 : 64);
-  attn_softmax_bwd_kernel<<<(unsigned)rows, bs, 0, ST>>>(P, dP, lds, Tq, Tk, scale, drelk, win);
+  attn_softmax_bwd_kernel<<<(unsigned)rows, bs, 0, ST>>>(P, dP, lds, H, Tq, Tk, scale, drelk, win, qlen, klen);
   return check_launch("attn_softmax_bwd");
 }
 extern "C" int evk_relk_logits(const float* q, int32_t ldq, const float* E, int32_t B, int32_t H, int32_t T, int32_t dk,

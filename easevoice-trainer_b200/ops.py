@@ -1506,7 +1506,8 @@ class _AttnFn(torch.autograd.Function):
             _call("evk_dropout", _p(dP), _p(dPn), dP.numel(), ctypes.c_float(p_drop), _p(rng_state(dev)), ctypes.c_uint64(sid))
             dP = dPn
         drel = torch.empty((Z, Tq, W), device=dev, dtype=torch.float32) if win is not None else None
-        _call("evk_attn_softmax_bwd", _p(P), _p(dP), ldS, Z, Tq, Tk, ctypes.c_float(scale_), _p(drel), win or 0)
+        _call("evk_attn_softmax_bwd", _p(P), _p(dP), ldS, Z, H, Tq, Tk, ctypes.c_float(scale_), _p(drel), win or 0, _p(qlen),
+              _p(klen))
         dS = dP
         # dQ = dS K  (K^T as the K-major operand)
         Kt = _transpose_cl(k, ldS)

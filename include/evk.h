@@ -257,9 +257,10 @@ int evk_layernorm_drop_bwd(const float* x, const float* res, const float* gamma,
  *   key j >= klen[b] or query i >= qlen[b] -> fill (finite -1e4 or -inf); softmax over j.  */
 int evk_attn_softmax(float* S, int32_t lds, int32_t Z, int32_t H, int32_t Tq, int32_t Tk, float scale, const float* relk,
                      int32_t win, const int32_t* qlen, const int32_t* klen, float fill, evk_stream_t stream);
-/* dS = P * (dP - sum_j dP*P) * scale, in place on dP; also emits drelk[z][i][r] = dS[i][i+r-win] (nullable) */
-int evk_attn_softmax_bwd(const float* P, float* dP, int32_t lds, int32_t Z, int32_t Tq, int32_t Tk, float scale, float* drelk,
-                         int32_t win, evk_stream_t stream);
+/* dS = P * (dP - sum_j dP*P) * scale, in place on dP, and 0 where the forward filled the logit (qlen, klen as given to
+ * evk_attn_softmax); also emits drelk[z][i][r] = dS[i][i+r-win] (nullable) */
+int evk_attn_softmax_bwd(const float* P, float* dP, int32_t lds, int32_t Z, int32_t H, int32_t Tq, int32_t Tk, float scale,
+                         float* drelk, int32_t win, const int32_t* qlen, const int32_t* klen, evk_stream_t stream);
 /* Windowed relative-position terms (attentions.py:254-288; skew helpers :312-365 replaced by band indexing).
  * E is [2*win+1][dk] (shared across heads); heads live in the channel dim: q[b][t][h*dk + d].
  *   relk_logits: rel[z][i][r] = q_i . E[r]                        (consumed by evk_attn_softmax)

@@ -267,6 +267,8 @@ def check_elementwise():
 
 
 def check_attention():
+    """Oracle-level relative-L2 row of the parity table; the element-wise gate of the same operator, with the kernel family
+    of each contraction asserted, lives in tests/test_gpu_s2_attention_elementwise.py."""
     from easevoice_trainer_b200 import ops
     out = []
     for name, B, Tq, Tk, C, H, win, fill in [("self relpos", 2, 45, 45, 192, 2, 4, -1e4), ("cross", 2, 45, 18, 512, 4, None, -1e4),
