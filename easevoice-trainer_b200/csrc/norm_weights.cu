@@ -1,10 +1,8 @@
-// Channel LayerNorm (modules.py:19-31) and weight-norm + operand packing (torch.nn.utils.weight_norm call
-// sites: modules.py:154-171,226-296; models.py:425-435,489-587).
+// Channel LayerNorm (modules.py:19-31), with and without a fused dropout on the residual, the column sums of bias gradients
+// and the per-channel instance norm of the HuBERT feature extractor.  Weight-norm + operand packing is in pack.cu.
 #include "evk_common.cuh"
 
 namespace evk {
-
-extern int g_precise;
 
 // one warp per row; C <= 32*MAXV
 constexpr int LN_MAXV = 32;   // up to 1024 channels
@@ -256,66 +254,6 @@ __global__ void __launch_bounds__(256) layernorm_drop_bwd_kernel(const float4* _
   }
 }
 
-// ---- weight-norm + pack ------------------------------------------------------------------
-// block per d0: w[d0][d1][q] = v * (g[d0] / ||v[d0]||);  PA[q][d0][d1], PB[q][d1][d0]
-// round_tf32: weights are rounded to TF32 (round-to-nearest) here, once, so the tensor-core kernels can stage them
-// with cp.async and still get rounded (not truncated) operands.
-__global__ void weight_pack_kernel(const float* __restrict__ v, const float* __restrict__ g, int D0, int D1, int Q,
-                                   float* __restrict__ pa, int lda, int D0p, float* __restrict__ pb, int ldb, int D1p,
-                                   int round_tf32) {
-  __shared__ float red[33];
-  const int d0 = blockIdx.x;
-  const long long n = (long long)D1 * Q;
-  const float* vr = v + (long long)d0 * n;
-  float scale = 1.f;
-  if (g) {
-    float s = 0.f;
-    for (long long i = threadIdx.x; i < n; i += blockDim.x) s += vr[i] * vr[i];
-    s = block_sum(s, red);
-    scale = g[d0] / sqrtf(s);
-  }
-  for (long long i = threadIdx.x; i < n; i += blockDim.x) {
-    const int d1 = (int)(i / Q), q = (int)(i - (long long)d1 * Q);
-    float w = vr[i] * scale;
-    if (round_tf32) w = __uint_as_float(f2tf32(w));
-    pa[((long long)q * D0p + d0) * lda + d1] = w;
-    if (pb) pb[((long long)q * D1p + d1) * ldb + d0] = w;
-  }
-}
-
-__global__ void weight_pack_bwd_kernel(const float* __restrict__ dpa, int lda, int D0p, const float* __restrict__ v,
-                                       const float* __restrict__ g, int D0, int D1, int Q, float* __restrict__ dv,
-                                       float* __restrict__ dg) {
-  __shared__ float red[33];
-  const int d0 = blockIdx.x;
-  const long long n = (long long)D1 * Q;
-  const float* vr = v + (long long)d0 * n;
-  float* dvr = dv + (long long)d0 * n;
-  if (!g) {
-    for (long long i = threadIdx.x; i < n; i += blockDim.x) {
-      const int d1 = (int)(i / Q), q = (int)(i - (long long)d1 * Q);
-      dvr[i] = dpa[((long long)q * D0p + d0) * lda + d1];
-    }
-    return;
-  }
-  float ss = 0.f, dot = 0.f;
-  for (long long i = threadIdx.x; i < n; i += blockDim.x) {
-    const int d1 = (int)(i / Q), q = (int)(i - (long long)d1 * Q);
-    const float vv = vr[i];
-    ss += vv * vv;
-    dot += dpa[((long long)q * D0p + d0) * lda + d1] * vv;
-  }
-  ss = block_sum(ss, red);
-  dot = block_sum(dot, red);
-  const float nrm = sqrtf(ss), gg = g[d0];
-  if (threadIdx.x == 0) dg[d0] = dot / nrm;
-  const float sc = gg / nrm, k = dot / ss;
-  for (long long i = threadIdx.x; i < n; i += blockDim.x) {
-    const int d1 = (int)(i / Q), q = (int)(i - (long long)d1 * Q);
-    dvr[i] = sc * (dpa[((long long)q * D0p + d0) * lda + d1] - vr[i] * k);
-  }
-}
-
 __global__ void colsum_kernel(const float* __restrict__ x, long long rows, int n, int ld, float* __restrict__ out,
                               int rows_per_block) {
   // blockDim = (32, 8): 32 columns x 8 row-lanes
@@ -441,36 +379,6 @@ extern "C" int evk_layernorm_drop_bwd(const float* x, const float* res, const fl
   if (int rc = check_launch("layernorm_drop_bwd")) return rc;
   if (int rc = ordered_sum(part, S, 2ll * C, 1, 1, C, dgamma, 0, 0, ST)) return rc;
   return ordered_sum(part + C, S, 2ll * C, 1, 1, C, dbeta, 0, 0, ST);
-}
-
-extern "C" int evk_weight_pack(const float* v, const float* g, int32_t D0, int32_t D1, int32_t Q, float* pa,
-                               int32_t lda, float* pb, int32_t ldb, evk_stream_t stream) {
-  EVK_REQUIRE(v && pa && D0 >= 1 && D1 >= 1 && Q >= 1 && lda >= D1 && (!pb || ldb >= D0), EVK_ERR_ARG,
-              "weight_pack: bad arguments");
-  weight_pack_kernel<<<D0, 256, 0, ST>>>(v, g, D0, D1, Q, pa, lda, D0, pb, ldb, D1, !g_precise);
-  return check_launch("weight_pack");
-}
-
-extern "C" int evk_weight_pack_p(const float* v, const float* g, int32_t D0, int32_t D1, int32_t Q, float* pa,
-                                 int32_t lda, int32_t D0p, float* pb, int32_t ldb, int32_t D1p, evk_stream_t stream) {
-  EVK_REQUIRE(v && pa && D0 >= 1 && D1 >= 1 && Q >= 1 && D0p >= D0 && D1p >= D1 && lda >= D1 && (!pb || ldb >= D0),
-              EVK_ERR_ARG, "weight_pack_p: bad arguments");
-  weight_pack_kernel<<<D0, 256, 0, ST>>>(v, g, D0, D1, Q, pa, lda, D0p, pb, ldb, D1p, !g_precise);
-  return check_launch("weight_pack_p");
-}
-
-extern "C" int evk_weight_pack_bwd(const float* dpa, int32_t lda, const float* v, const float* g, int32_t D0,
-                                   int32_t D1, int32_t Q, float* dv, float* dg, evk_stream_t stream) {
-  EVK_REQUIRE(dpa && v && dv && (!g || dg), EVK_ERR_ARG, "weight_pack_bwd: null tensor");
-  weight_pack_bwd_kernel<<<D0, 256, 0, ST>>>(dpa, lda, D0, v, g, D0, D1, Q, dv, dg);
-  return check_launch("weight_pack_bwd");
-}
-
-extern "C" int evk_weight_pack_bwd_p(const float* dpa, int32_t lda, int32_t D0p, const float* v, const float* g,
-                                     int32_t D0, int32_t D1, int32_t Q, float* dv, float* dg, evk_stream_t stream) {
-  EVK_REQUIRE(dpa && v && dv && (!g || dg) && D0p >= D0, EVK_ERR_ARG, "weight_pack_bwd_p: bad arguments");
-  weight_pack_bwd_kernel<<<D0, 256, 0, ST>>>(dpa, lda, D0p, v, g, D0, D1, Q, dv, dg);
-  return check_launch("weight_pack_bwd_p");
 }
 
 extern "C" int evk_colsum(const float* x, int64_t rows, int32_t n, int32_t ld, float* out, int32_t accumulate,

@@ -22,6 +22,11 @@ class GconvDesc(ctypes.Structure):
     )
 
 
+class PackJob(ctypes.Structure):
+    _fields_ = ([(n, ctypes.c_void_p) for n in ("v", "g", "pa", "pb", "dpa", "dv", "dg")]
+                + [(n, ctypes.c_int32) for n in ("D0", "D1", "Q", "lda", "D0p", "ldb", "D1p", "row0")])
+
+
 _CTYPE = {
     "int32_t": ctypes.c_int32, "int64_t": ctypes.c_int64, "uint64_t": ctypes.c_uint64, "float": ctypes.c_float,
     "int": ctypes.c_int, "evk_stream_t": ctypes.c_void_p,

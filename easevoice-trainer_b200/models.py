@@ -69,13 +69,13 @@ class ParamTree(nn.Module):
 
     # ---- packed-weight helpers (weight-norm folded into the packing pass) --------------------
     _frozen = False            # True: weights enter the graph as constants (no weight gradients are computed)
-    batch_packing = os.environ.get("EVK_BATCH_PACK", "1") != "0"     # one weight_pack launch per network and step (ops.PackPlan), not one per layer
 
     def begin_pack(self):
         """Call at the start of a forward pass.  The first pass of each kind (frozen or not) packs layer by layer and records
-        what it packs; later passes run the recorded plan in one launch and hand out views of its arenas."""
+        what it packs; later passes run the recorded plan in one launch and hand out views of its arenas.  Inference
+        without gradients on a network that is not frozen packs layer by layer on use."""
         self._active, self._recording = None, None
-        if not self.batch_packing or not torch.is_grad_enabled() and not self._frozen:
+        if not torch.is_grad_enabled() and not self._frozen:
             return
         plans = self.__dict__.setdefault("_plans", {})
         plan = plans.get(self._frozen)

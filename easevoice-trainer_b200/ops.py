@@ -239,14 +239,18 @@ def _pad4(n):
     return n if n < 4 else (n + 3) // 4 * 4
 
 
+def _pack_geometry(v, pad0, pad1):
+    """-> (D0, D1, Q, D0p, D1p, lda, ldb) of the packed operands PA [Q, D0p, lda] and PB [Q, D1p, ldb] of the torch-layout
+    weight v [D0, D1, Q(,1)].  Channel dims < 4 are zero-padded to pad0 / pad1 so every conv is 16-byte tileable."""
+    D0, D1 = v.shape[0], v.shape[1]
+    D0p, D1p = max(D0, pad0), max(D1, pad1)
+    return D0, D1, v.numel() // (D0 * D1), D0p, D1p, _pad4(D1p), _pad4(D0p)
+
+
 class _PackFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, v, g, need_pb, pad0, pad1):
-        D0 = v.shape[0]
-        D1 = v.shape[1]
-        Q = v.numel() // (D0 * D1)
-        D0p, D1p = max(D0, pad0), max(D1, pad1)          # channel dims < 4 are zero-padded so every conv is 16-byte tileable
-        lda, ldb = _pad4(D1p), _pad4(D0p)
+        D0, D1, Q, D0p, D1p, lda, ldb = _pack_geometry(v, pad0, pad1)
         exact = (D0p == D0 and D1p == D1)
         pa = (torch.zeros if (lda != D1 or not exact) else torch.empty)((Q, D0p, lda), device=v.device, dtype=torch.float32)
         pb = None
@@ -254,9 +258,10 @@ class _PackFn(torch.autograd.Function):
             pb = (torch.zeros if (ldb != D0 or not exact) else torch.empty)((Q, D1p, ldb), device=v.device, dtype=torch.float32)
         vc = v.contiguous()
         gc = g.contiguous() if g is not None else None
-        _call("evk_weight_pack_p", _p(vc), _p(gc), D0, D1, Q, _p(pa), lda, D0p, _p(pb), ldb, D1p)
+        job = L.PackJob(v=_p(vc), g=_p(gc), pa=_p(pa), pb=_p(pb), D0=D0, D1=D1, Q=Q, lda=lda, D0p=D0p, ldb=ldb, D1p=D1p)
+        _call("evk_weight_pack_one", ctypes.byref(job))
         ctx.save_for_backward(vc, gc)
-        ctx.dims = (D0, D1, Q, lda, D0p, tuple(v.shape), tuple(g.shape) if g is not None else None)
+        ctx.job = job
         if pb is None:
             pb = torch.empty(0, device=v.device)
         ctx.mark_non_differentiable(pb)
@@ -265,19 +270,20 @@ class _PackFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dpa, _dpb):
         v, g = ctx.saved_tensors
-        D0, D1, Q, lda, D0p, vshape, gshape = ctx.dims
         dpa = dpa.contiguous()
-        dv = torch.empty(vshape, device=v.device, dtype=torch.float32)
-        dg = torch.empty(gshape, device=v.device, dtype=torch.float32) if g is not None else None
-        _call("evk_weight_pack_bwd_p", _p(dpa), lda, D0p, _p(v), _p(g), D0, D1, Q, _p(dv), _p(dg))
+        dv = torch.empty_like(v)
+        dg = torch.empty_like(g) if g is not None else None
+        job = ctx.job
+        job.dpa, job.dv, job.dg = _p(dpa), _p(dv), _p(dg)
+        _call("evk_weight_pack_bwd_one", ctypes.byref(job))
         return dv, dg, None, None, None
 
 
 def pack_weight(v, g=None, need_pb=True, pad0=0, pad1=0):
     """weight-norm (if g) + pack.  v: torch-layout weight [D0, D1, Q(,1)]; pad0/pad1 zero-pad the channel dims."""
     pa, pb = _PackFn.apply(v, g, need_pb, pad0, pad1)
-    D0, D1 = max(v.shape[0], pad0), max(v.shape[1], pad1)
-    return PackedW(pa, pb if need_pb else None, D0, D1, v.numel() // (v.shape[0] * v.shape[1]))
+    _, _, Q, D0p, D1p, _, _ = _pack_geometry(v, pad0, pad1)
+    return PackedW(pa, pb if need_pb else None, D0p, D1p, Q)
 
 
 # ---- pooled zero-initialised scratch for small accumulators (bias gradients) -------------------------------------------
@@ -318,12 +324,7 @@ class grad_pool:
         return False
 
 
-# ---- whole-network packing: one launch per network per step (pack_batched.cu) ------------------------------------
-class PackJobC(ctypes.Structure):
-    _fields_ = ([(n, ctypes.c_void_p) for n in ("v", "g", "pa", "pb", "dpa", "dv", "dg")]
-                + [(n, ctypes.c_int32) for n in ("D0", "D1", "Q", "lda", "D0p", "ldb", "D1p", "row0")])
-
-
+# ---- whole-network packing: one launch per network per step (pack.cu) ---------------------------------------------
 _dpa_views = {}          # data_ptr of a packed weight -> its slice of the plan's (pre-zeroed) packed-gradient arena
 _dpa_taken = set()       # slices already handed to a backward since the plan was last zeroed
 
@@ -351,10 +352,7 @@ class PackPlan:
         al = lambda n: (n + 63) // 64 * 64                         # 256-byte aligned regions (TMA bases need 16)
         geo, off_pa, off_pb, off_g = [], 0, 0, 0
         for key, v, g, need_pb, pad0, pad1, wants in reqs:
-            D0, D1 = v.shape[0], v.shape[1]
-            Q = v.numel() // (D0 * D1)
-            D0p, D1p = max(D0, pad0), max(D1, pad1)
-            lda, ldb = _pad4(D1p), _pad4(D0p)
+            D0, D1, Q, D0p, D1p, lda, ldb = _pack_geometry(v, pad0, pad1)
             geo.append((D0, D1, Q, D0p, D1p, lda, ldb, off_pa, off_pb if need_pb else -1, off_g))
             off_pa += al(Q * D0p * lda)
             if need_pb:
@@ -364,7 +362,7 @@ class PackPlan:
         self.arena_pb = torch.zeros(max(off_pb, 1), device=dev, dtype=torch.float32)
         self.arena_dpa = torch.zeros(off_pa, device=dev, dtype=torch.float32) if with_grad else None
         self.arena_dvg = torch.zeros(off_g, device=dev, dtype=torch.float32) if with_grad else None
-        jobs = (PackJobC * len(reqs))()
+        jobs = (L.PackJob * len(reqs))()
         rows, rows_bwd, row0 = [], [], 0
         self.pa, self.pb, self.dpa, self.grads, self.params, self.sig = [], [], [], [], [], []
         for i, ((key, v, g, need_pb, pad0, pad1, wants), (D0, D1, Q, D0p, D1p, lda, ldb, opa, opb, og)) in enumerate(zip(reqs, geo)):
@@ -393,7 +391,7 @@ class PackPlan:
         self.rows = torch.tensor(rows, dtype=torch.int32, device=dev)
         # the backward table re-bases row0 per job: build a second job table whose row0 counts only the rows that run
         if with_grad:
-            jb = (PackJobC * len(reqs))()
+            jb = (L.PackJob * len(reqs))()
             ctypes.memmove(jb, jobs, ctypes.sizeof(jobs))
             r0 = 0
             for i, (req, ge) in enumerate(zip(reqs, geo)):
@@ -418,9 +416,8 @@ class PackPlan:
 
     def packed(self, i, pa=None):
         r = self.reqs[i]
-        v = r[1]
-        D0, D1 = max(v.shape[0], r[4]), max(v.shape[1], r[5])
-        return PackedW(self.pa[i] if pa is None else pa, self.pb[i], D0, D1, v.numel() // (v.shape[0] * v.shape[1]))
+        _, _, Q, D0p, D1p, _, _ = _pack_geometry(r[1], r[4], r[5])
+        return PackedW(self.pa[i] if pa is None else pa, self.pb[i], D0p, D1p, Q)
 
 
 class _PackAllFn(torch.autograd.Function):

@@ -31,7 +31,7 @@ enum evk_act { EVK_ACT_NONE = 0, EVK_ACT_LRELU = 1, EVK_ACT_RELU = 2, EVK_ACT_TA
 
 #define EVK_MAX_TAPS 48
 
-int evk_init(void);                    /* checks compute capability 10.x, raises smem limits */
+int evk_init(void);                    /* checks compute capability 9.0, raises smem limits */
 int evk_version(void);
 const char* evk_last_error(void);
 int evk_sync_check(evk_stream_t stream); /* cudaStreamSynchronize + error fetch (tests only) */
@@ -103,25 +103,22 @@ int evk_colsum(const float* x, int64_t rows, int32_t n, int32_t ld, float* out, 
 
 /* ------------------------------------------------------------------------------------------
  * Weight preparation: torch.nn.utils.weight_norm (modules.py:154-171, models.py:425-435,489-587)
- * folded into the operand-packing pass.  v is [D0][D1][Q] (torch layout), g is [D0] or NULL
- * (plain weight).  Produces PA[q][d0][d1] (pitch lda) and optionally PB[q][d1][d0] (pitch ldb).
+ * folded into the operand-packing pass (pack.cu).  One job: v is [D0][D1][Q] (torch layout), g is [D0] or NULL (plain
+ * weight).  Produces PA[q][d0][d1] ([Q][D0p][lda]) and, unless pb is NULL, PB[q][d1][d0] ([Q][D1p][ldb]); D0p x D1p
+ * zero-pad the channel dims (padding pre-zeroed by the caller) so 1-channel layers run on the tensor-core kernels.
+ * The backward takes dPA (gradient in PA layout) and writes dv [D0][D1][Q] and dg [D0] (when g is not NULL).
  * ------------------------------------------------------------------------------------------ */
-int evk_weight_pack(const float* v, const float* g, int32_t D0, int32_t D1, int32_t Q, float* pa, int32_t lda,
-                    float* pb, int32_t ldb, evk_stream_t stream);
-/* Same, with the channel dims zero-padded to D0p x D1p rows/cols (PA is [Q][D0p][lda], PB [Q][D1p][ldb], both
- * pre-zeroed by the caller): 1-channel layers are padded to 4 so they run on the tensor-core kernels. */
-int evk_weight_pack_p(const float* v, const float* g, int32_t D0, int32_t D1, int32_t Q, float* pa, int32_t lda,
-                      int32_t D0p, float* pb, int32_t ldb, int32_t D1p, evk_stream_t stream);
-int evk_weight_pack_bwd_p(const float* dpa, int32_t lda, int32_t D0p, const float* v, const float* g, int32_t D0,
-                          int32_t D1, int32_t Q, float* dv, float* dg, evk_stream_t stream);
-/* given dPA (gradient in PA layout) -> dv [D0][D1][Q] (written), dg [D0] (written) (g may be NULL) */
-/* Whole-network variants (pack_batched.cu): ONE launch packs / back-propagates every weight of a network.  `jobs` is a
- * device array of 88-byte records {v, g, pa, pb, dpa, dv, dg (pointers); D0, D1, Q, lda, D0p, ldb, D1p, row0 (int32)},
- * job_of_row [nrows] maps each (job, output-channel) row to its job.  All pointers are static arenas owned by the caller. */
-int evk_weight_pack_batched(const void* jobs, const int32_t* job_of_row, int32_t nrows, evk_stream_t stream);
-int evk_weight_pack_bwd_batched(const void* jobs, const int32_t* job_of_row, int32_t nrows, evk_stream_t stream);
-int evk_weight_pack_bwd(const float* dpa, int32_t lda, const float* v, const float* g, int32_t D0, int32_t D1,
-                        int32_t Q, float* dv, float* dg, evk_stream_t stream);
+typedef struct evk_pack_job {
+  const float* v; const float* g; float* pa; float* pb;
+  const float* dpa; float* dv; float* dg;             /* backward only */
+  int32_t D0, D1, Q, lda, D0p, ldb, D1p, row0;        /* row0: the job's first row (block) in a table; 0 for one job */
+} evk_pack_job;
+int evk_pack_job_size(void);           /* sizeof(evk_pack_job) as compiled: bindings check their mirror against it */
+int evk_weight_pack_one(const evk_pack_job* j, evk_stream_t stream);       /* one weight; *j is read on the host */
+int evk_weight_pack_bwd_one(const evk_pack_job* j, evk_stream_t stream);
+/* A whole network per launch: `jobs` is a DEVICE array, job_of_row [nrows] maps each (job, output-channel) row to its job. */
+int evk_weight_pack_batched(const evk_pack_job* jobs, const int32_t* job_of_row, int32_t nrows, evk_stream_t stream);
+int evk_weight_pack_bwd_batched(const evk_pack_job* jobs, const int32_t* job_of_row, int32_t nrows, evk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Fused mel front end (mel_processing.py:40-142): reflect-pad -> Hann -> rFFT(2048) ->

@@ -33,6 +33,14 @@ def test_descriptor_struct_layout():
     assert lib.load().evk_gconv_desc_size() == ctypes.sizeof(lib.GconvDesc)          # the compiled header agrees with the ctypes mirror
 
 
+def test_pack_job_struct_layout():
+    from easevoice_trainer_b200 import lib
+    # 7 pointers + 8 int32 (D0, D1, Q, lda, D0p, ldb, D1p, row0)
+    assert ctypes.sizeof(lib.PackJob) == 7 * 8 + 8 * 4
+    assert lib.PackJob.D0.offset == 56 and lib.PackJob.row0.offset == 84
+    assert lib.load().evk_pack_job_size() == ctypes.sizeof(lib.PackJob)
+
+
 def test_no_cpu_fallback():
     """Without an H100 the product path must fail loudly, never silently compute on the CPU."""
     if torch.cuda.is_available():
