@@ -2346,6 +2346,39 @@ def ssl_normalize(a, lens):
     return a32, a32b, status
 
 
+def frame_rms(x, lens, win, hop):
+    """evk_frame_rms: Slicer.get_rms of the rows of x [B, L] (fp32 device, row b holding lens[b] samples; lens int32 device
+    [B]) -> rms fp32 [B, 1 + (L + 2 (win // 2) - win) // hop]; frames past a row's own count are 0."""
+    assert x.dim() == 2 and x.dtype == torch.float32 and x.is_cuda and x.stride(1) == 1
+    assert lens.dtype == torch.int32 and lens.is_cuda and lens.numel() == x.shape[0]
+    B, Lm = x.shape
+    T = 1 + (Lm + 2 * (win // 2) - win) // hop
+    assert T >= 1, (Lm, win, hop)
+    rms = torch.empty((B, T), device=x.device, dtype=torch.float32)
+    _call("evk_frame_rms", _p(x), x.stride(0), _p(lens.contiguous()), B, win, hop, _p(rms), T, T)
+    return rms
+
+
+SLICE_MAX_CHUNKS = 65535        # chunks of one evk_slice_normalize call
+
+
+def slice_normalize(x, chunks, max_len, c1, c2, out=None):
+    """evk_slice_normalize: the chunk loop of AudioService.slicer over the flat fp32 device buffer x.  chunks: int64 device
+    [n, 2] = (offset, length), max_len >= every length -> (int16 buffer shaped like x, written at the chunks' offsets only,
+    m fp32 [n] = max |chunk|, status int32 [n]: EVK_SLICE_OK = 0, EVK_SLICE_SILENT = 1, EVK_SLICE_NONFINITE = 2)."""
+    assert x.dtype == torch.float32 and x.is_cuda and x.is_contiguous()
+    assert chunks.dtype == torch.int64 and chunks.is_cuda and chunks.is_contiguous() and chunks.dim() == 2 and chunks.shape[1] == 2
+    n = chunks.shape[0]
+    out = torch.empty(x.shape, device=x.device, dtype=torch.int16) if out is None else out
+    assert out.dtype == torch.int16 and out.is_contiguous() and out.shape == x.shape
+    m = torch.empty(n, device=x.device, dtype=torch.float32)
+    status = torch.empty(n, device=x.device, dtype=torch.int32)
+    for i in range(0, n, SLICE_MAX_CHUNKS):
+        k = min(SLICE_MAX_CHUNKS, n - i)
+        _call("evk_slice_normalize", _p(x), _p(chunks[i:]), k, int(max_len), float(c1), float(c2), _p(out), _p(m[i:]), _p(status[i:]))
+    return out, m, status
+
+
 def vr_assemble(x, pred, pred_tta, coef, bands, gains, high=None, mirror_lo=0, top=-1):
     """evk_vr_assemble: combined spectrogram x [2, n_rows, l, 2], pred / pred_tta [2, n_rows, l] and coef [1] -> one
     [4, l, n_fft/2+1, 2] frame tensor per band (rows y ch0, y ch1, v ch0, v ch1: evk_istft's input with B = 4, S = 1).

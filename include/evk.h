@@ -624,6 +624,27 @@ int evk_vr_assemble(const float* x, const float* pred, const float* pred_tta, co
                     const float* high, int32_t high_h, int32_t mirror_lo, int32_t top, const int64_t* bands, int32_t n_bands,
                     const float* gains, float* out, evk_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * AudioService.slicer (service/audio.py:142-183; audiokit/slicer/slicer.py), slicer.cu.
+ * ------------------------------------------------------------------------------------------ */
+/* Slicer.get_rms of B rows: row b of x [B][ldx] holds lens[b] (int32 device) samples.  rms [B][ldr], T <= ldr frames per row:
+ * frame t = sqrt(mean(x[t hop - win/2 .. t hop - win/2 + win)^2)) with zeros outside the row, for t < 1 + (lens[b] + 2 (win/2)
+ * - win) / hop (1 + lens[b] / hop for even win); later frames are 0.  Squares, sums, mean and root are float64 in a fixed
+ * order, rounded to float32 once: within 1 ulp of the exact value, and the same bits for a row alone or in any batch.
+ * win <= 64 hop; B <= 65535. */
+int evk_frame_rms(const float* x, int64_t ldx, const int32_t* lens, int32_t B, int32_t win, int32_t hop, float* rms, int32_t T,
+                  int32_t ldr, evk_stream_t stream);
+enum evk_slice_status { EVK_SLICE_OK = 0, EVK_SLICE_SILENT = 1, EVK_SLICE_NONFINITE = 2 };
+/* The chunk loop of audio.py:171-178.  chunks: int64 device [n_chunks][2] = (offset in x and y, length), max_len >= every
+ * length (host), n_chunks <= 65535.  Per chunk, m = max |x| (NaN if a sample is NaN) is written to m [n_chunks] (device) and
+ *   c = m > 1 ? x / m : x;   y = int16(((c / m * c1) + c2 * c) * 32767)
+ * to y at the chunk's offsets, every operation a float32 operation in that order (bit-identical to numpy); the int16
+ * conversion truncates to int32 and keeps the low 16 bits, NaN and values outside int32 giving 0 (x86 numpy's astype).
+ * status [n_chunks] (int32 device): EVK_SLICE_SILENT if m == 0 (every output is int16(NaN) = 0), EVK_SLICE_NONFINITE if m is
+ * NaN or Inf, else EVK_SLICE_OK.  Samples outside every chunk are not written. */
+int evk_slice_normalize(const float* x, const int64_t* chunks, int32_t n_chunks, int64_t max_len, float c1, float c2, int16_t* y,
+                        float* m, int32_t* status, evk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
