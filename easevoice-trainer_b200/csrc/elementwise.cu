@@ -258,29 +258,6 @@ __global__ void transpose_rows_kernel(const float* __restrict__ x, int ldx, long
   }
 }
 
-// all delayed copies of evk_transpose_rows in one pass over x: y[r][b][c][u] = x[b][u - r][c] for every r in `mask`
-// (bit r set, r = 0..3); the 32 x 32 tile is loaded once with a 3-row halo.
-__global__ void transpose_rows_multi_kernel(const float* __restrict__ x, int ldx, long long x_sb, float* __restrict__ y, int ldy,
-                                            long long y_sb, long long y_rs, int T, int C, int mask) {
-  __shared__ float tile[35][33];
-  const int b = blockIdx.z, c0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
-  const float* xb = x + b * x_sb;
-  for (int i = threadIdx.y; i < 35; i += blockDim.y) {
-    int t = t0 + i - 3, c = c0 + threadIdx.x;
-    tile[i][threadIdx.x] = (c < C && t >= 0 && t < T) ? xb[(long long)t * ldx + c] : 0.f;
-  }
-  __syncthreads();
-#pragma unroll
-  for (int r = 0; r < 4; ++r) {
-    if (!((mask >> r) & 1)) continue;
-    float* yb = y + r * y_rs + b * y_sb;
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-      int c = c0 + i, u = t0 + threadIdx.x;
-      if (u < T + r && c < C) yb[(long long)c * ldy + u] = tile[threadIdx.x + 3 - r][i];
-    }
-  }
-}
-
 // One pass over an output gradient for everything a conv's backward needs from it (round 1 ran three kernels -- activation
 // backward, transpose for the TMA weight gradient, column sums for the bias -- and four trips through memory):
 //   g[t][c]    = dy[t][c] * act'(y[t][c]) * (t < len*P)        -> dpre  (normal layout, only when it differs from dy)
@@ -597,15 +574,6 @@ extern "C" int evk_transpose_rows(const float* x, int32_t ldx, int64_t x_sb, flo
   EVK_REQUIRE(grid.y <= 65535 && grid.z <= 65535, EVK_ERR_ARG, "transpose_rows: grid too large");
   transpose_rows_kernel<<<grid, block, 0, ST>>>(x, ldx, x_sb, y, ldy, y_sb, T, C, shift);
   return check_launch("transpose_rows");
-}
-extern "C" int evk_transpose_rows_multi(const float* x, int32_t ldx, int64_t x_sb, float* y, int32_t ldy, int64_t y_sb, int64_t y_rs,
-                                        int32_t B, int32_t T, int32_t C, int32_t mask, evk_stream_t stream) {
-  EVK_REQUIRE(x && y && ldx >= C && ldy >= T + 3 && mask > 0 && mask < 16, EVK_ERR_ARG, "transpose_rows_multi: bad arguments");
-  if ((long long)B * C * T == 0) return EVK_OK;
-  dim3 grid(cdiv(T + 3, 32), cdiv(C, 32), B), block(32, 8);
-  EVK_REQUIRE(grid.y <= 65535 && grid.z <= 65535, EVK_ERR_ARG, "transpose_rows_multi: grid too large");
-  transpose_rows_multi_kernel<<<grid, block, 0, ST>>>(x, ldx, x_sb, y, ldy, y_sb, y_rs, T, C, mask);
-  return check_launch("transpose_rows_multi");
 }
 // dy [B][T][lddy] (T rows per batch item), yact = the conv's activated OUTPUT (nullable when act == 0), len (nullable int32 [B],
 // rows t >= len[b] * P are zeroed), outputs each nullable: dpre [B][T][ldp], dyt [B][C][ldt] (batch pitch t_sb), dbias [C]

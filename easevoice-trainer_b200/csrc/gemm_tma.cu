@@ -1,8 +1,8 @@
 // TMA-fed, warp-specialised, persistent wgmma GEMM (sm_90a):   D[M][N] (+)= epi( A[M][K] * B[N][K]^T )
 // fp32 storage, TF32 tensor-core math, fp32 accumulation in registers.  Serves every dense contraction without taps:
 // nn.Linear / 1x1 conv forward (A = activations rows, B = packed weight [N][C]), their data gradients
-// (A = dY rows, B = packed transposed weight [C][N]) and -- through evk_gemm_tf32 with split-K -- weight gradients
-// on pre-transposed operands.
+// (A = dY rows, B = packed transposed weight [C][N]) and, through evk_gemm_tf32 with split-K, weight gradients on
+// pre-transposed operands.  Conv weight gradients run on conv_wgrad_kernel (below), which shares the TMA / mbarrier plumbing.
 //
 //   warp 0 (one lane)  : TMA producer.  cp.async.bulk.tensor 2-D boxes [128 x 32 fl] (A) and [BN x 32 fl] (B), 128-byte
 //                        swizzle, into SA / SB-deep shared-memory rings; full[s] mbarrier with expect_tx.
@@ -37,10 +37,7 @@ struct GemmP {
   // implicit-GEMM convolution mode (stride 1): Z batch items, Q taps, period P; tap q reads input row pos + off[q]*P
   int Z, Q, P;
   int os, o0;                                        // output position of tile row pos: ((o0 + (pos / P) * os) * P + pos % P)
-  int src[EVK_MAX_TAPS];                             // mode 0: which of the (up to 4) A tensor maps tap q reads (stride phases)
-  int mode;                                          // 0: GEMM / conv forward-like;  1: conv weight gradient (see evk_conv_wgrad_tma)
-  int kbs;                                           // mode 1: K blocks per batch item
-  long long d_sq;                                    // mode 1: output pitch between taps
+  int src[EVK_MAX_TAPS];                             // which of the (up to 4) A tensor maps tap q reads (stride phases)
   long long y_sb, r_sb;
   const int* out_len;
   int off[EVK_MAX_TAPS];
@@ -193,8 +190,7 @@ __device__ __forceinline__ void epi_chunk(const GemmP& p, const float* __restric
   }
 }
 
-struct MapB4 { CUtensorMap m[4]; };                  // B: mode 1 uses one map per delayed copy of X^T, mode 0 only m[0]
-                                                     // A: mode 0 uses one map per stride phase of the input, mode 1 only m[0];
+struct MapB4 { CUtensorMap m[4]; };                  // B: only m[0];  A: one map per stride phase of the input;
                                                      //    slab mode: m[1] = the same tensor with a `span`-row box (the slab tail)
 constexpr int MAX_RING = 8;
 
@@ -228,13 +224,12 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gemm_tma_kernel(const __grid_co
   __syncthreads();
 
   const int tiles_mn = p.tiles_m * p.tiles_n;
-  // mode 0: tile -> (outer = batch item or K split, m tile, n tile); K iterations = taps x channel blocks (splits > 1 only
-  //         in plain GEMM mode, Z == Q == 1).   mode 1: outer = (tap, K split); K iterations = batch items x row blocks.
-  const int total = p.mode ? tiles_mn * p.splits * p.Q : tiles_mn * p.splits * p.Z;
-  const int kb_total = p.mode ? p.Z * p.kbs : (p.K + BK - 1) / BK;
+  // tile -> (outer = batch item or K split, m tile, n tile); K iterations = taps x channel blocks (splits > 1 only in plain
+  // GEMM mode, Z == Q == 1)
+  const int total = tiles_mn * p.splits * p.Z;
+  const int kb_total = (p.K + BK - 1) / BK;
   auto k_range = [&](int outer, int& k0, int& k1) {
-    if (p.mode) { const int sp = outer % p.splits; k0 = sp * p.kb_per_split; k1 = min(kb_total, k0 + p.kb_per_split); }
-    else if (p.splits > 1) { k0 = outer * p.kb_per_split; k1 = min(kb_total, k0 + p.kb_per_split); }
+    if (p.splits > 1) { k0 = outer * p.kb_per_split; k1 = min(kb_total, k0 + p.kb_per_split); }
     else { k0 = 0; k1 = p.Q * kb_total; }
   };
   const int slab = p.slab;
@@ -250,7 +245,7 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gemm_tma_kernel(const __grid_co
     for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
       const int outer = tile / tiles_mn, mn = tile - outer * tiles_mn;
       const int tm = mn / p.tiles_n, tn = mn - tm * p.tiles_n;
-      const int z = (p.splits > 1 || p.mode) ? 0 : outer;
+      const int z = p.splits > 1 ? 0 : outer;
       auto next_a = [&]() -> uint8_t* {
         mbar_wait(&emptyA[sA], phA);
         if (leader) mbar_expect_tx(&fullA[sA], (uint32_t)p.a_bytes);
@@ -276,7 +271,7 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gemm_tma_kernel(const __grid_co
             done_b();
           }
         }
-      } else if (!p.mode && p.splits == 1) {
+      } else if (p.splits == 1) {
         for (int q = 0; q < Q; ++q) {
           const CUtensorMap* am = &mapA4.m[p.src[q]];
           const int arow = tm * (MT * BM) + p.off[q] * p.P;
@@ -289,33 +284,16 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gemm_tma_kernel(const __grid_co
             done_b();
           }
         }
-      } else {
+      } else {                                                 // split-K plain GEMM (Z == Q == 1)
         int k0, k1;
         k_range(outer, k0, k1);
-        if (p.mode) {
-          const int q = outer / p.splits;
-          // TMA needs the inner coordinate 16-byte aligned: X[t + sh] is read from the copy delayed by r = (-sh) mod 4
-          // (xt_r[u] = X[u - r]) at the aligned coordinate t + sh + r
-          const int sh = p.off[q] * p.P, r = (((-sh) % 4) + 4) % 4;
-          int b = k0 / p.kbs, kk = k0 - b * p.kbs;
-          for (int ki = k0; ki < k1; ++ki) {
-            uint8_t* sa = next_a();
-            if (leader) tma_load_3d(sa, &mapA, kk * BK, tm * BM, b, &fullA[sA]);
-            done_a();
-            uint8_t* sb = next_b();
-            if (leader) tma_load_3d(sb, &mapB4.m[r], kk * BK + (sh + r), tn * BN, b, &fullB[sB]);
-            done_b();
-            if (++kk == p.kbs) { kk = 0; ++b; }
-          }
-        } else {                                               // split-K plain GEMM (Z == Q == 1)
-          for (int kb = k0; kb < k1; ++kb) {
-            uint8_t* sa = next_a();
-            if (leader) tma_load_3d(sa, &mapA, kb * BK, tm * (MT * BM), 0, &fullA[sA]);
-            done_a();
-            uint8_t* sb = next_b();
-            if (leader) tma_load_3d(sb, &mapB, kb * BK, tn * BN, 0, &fullB[sB]);
-            done_b();
-          }
+        for (int kb = k0; kb < k1; ++kb) {
+          uint8_t* sa = next_a();
+          if (leader) tma_load_3d(sa, &mapA, kb * BK, tm * (MT * BM), 0, &fullA[sA]);
+          done_a();
+          uint8_t* sb = next_b();
+          if (leader) tma_load_3d(sb, &mapB, kb * BK, tn * BN, 0, &fullB[sB]);
+          done_b();
         }
       }
     }
@@ -388,9 +366,9 @@ __global__ void __launch_bounds__(GT_THREADS, 1) gemm_tma_kernel(const __grid_co
       // ---- epilogue from registers
       const int outer = tile / tiles_mn, mn = tile - outer * tiles_mn;
       const int tm = mn / p.tiles_n, tn = mn - tm * p.tiles_n;
-      const int z = (p.splits > 1 || p.mode) ? 0 : outer;
-      float* dz = p.mode ? p.d + (size_t)(outer / p.splits) * p.d_sq : p.d + (size_t)z * p.y_sb;
-      if (p.atomic) dz += (size_t)(p.mode ? outer % p.splits : outer) * p.d_ssp;
+      const int z = p.splits > 1 ? 0 : outer;
+      float* dz = p.d + (size_t)z * p.y_sb;
+      if (p.atomic) dz += (size_t)outer * p.d_ssp;
       const float* rz = p.res ? p.res + (size_t)z * p.r_sb : nullptr;
       const int olen = p.out_len ? p.out_len[z] : 0x7fffffff;
       const int r_sub = lane >> 3;
@@ -475,8 +453,7 @@ float g_trunc_comp = 3.52e-4f;
 struct Operands {
   const float* A; int lda; long long a_sb, a_rows;     // activations: [Z][a_rows][K]
   const float* B; int ldb; long long b_sq;             // weights:     [Q][N][K]
-  long long b_rs;                                      // mode 1: pitch between the four residue copies of X^T
-  int a_phases; long long a_ps;                        // mode 0: stride phases of the input and their pitch
+  int a_phases; long long a_ps;                        // stride phases of the input and their pitch
   int raw_operands;                                    // how many of the two operands are un-rounded fp32 (truncated by the MMA)
 };
 
@@ -488,7 +465,7 @@ int launch_gemm(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
   MapB4 ma, mb;
   p.slab = 0;
   int span = 0;
-  if (!p.mode && g_opt_slab && o.a_phases == 1 && p.Q >= 2 && splits <= 1) {
+  if (g_opt_slab && o.a_phases == 1 && p.Q >= 2 && splits <= 1) {
     int mn = p.off[0], mx = p.off[0];
     for (int i = 1; i < p.Q; ++i) { mn = min(mn, p.off[i]); mx = max(mx, p.off[i]); }
     span = (mx - mn) * p.P;
@@ -502,20 +479,13 @@ int launch_gemm(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
     p.a_stage = p.a_bytes = MT * BM * BK * 4;
     p.SA = p.SB = min(MAX_RING, SMEM_BUDGET / (p.a_stage + B_BYTES));
   }
-  if (p.mode) {            // A = dY^T [Z][M = N_out][K = rows], B = residue copies of X^T [Z][N = C_in][in_rows - r]
-    if (!make_map(&ma.m[0], o.A, p.Z, o.a_sb, p.M, p.K, o.lda, BM)) return 1;
-    ma.m[1] = ma.m[2] = ma.m[3] = ma.m[0];
-    for (int r = 0; r < 4; ++r)
-      if (!make_map(&mb.m[r], o.B + r * o.b_rs, p.Z, o.b_sq, p.N, o.a_rows + r, o.ldb, BN)) return 1;
-  } else {
-    for (int ph = 0; ph < 4; ++ph) {
-      if (ph < o.a_phases) { if (!make_map(&ma.m[ph], o.A + ph * o.a_ps, p.Z, o.a_sb, o.a_rows, p.K, o.lda, MT * BM)) return 1; }
-      else ma.m[ph] = ma.m[0];
-    }
-    if (p.slab && !make_map(&ma.m[1], o.A, p.Z, o.a_sb, o.a_rows, p.K, o.lda, span)) return 1;
-    if (!make_map(&mb.m[0], o.B, p.Q, o.b_sq, p.N, p.K, o.ldb, BN)) return 1;
-    mb.m[1] = mb.m[2] = mb.m[3] = mb.m[0];
+  for (int ph = 0; ph < 4; ++ph) {
+    if (ph < o.a_phases) { if (!make_map(&ma.m[ph], o.A + ph * o.a_ps, p.Z, o.a_sb, o.a_rows, p.K, o.lda, MT * BM)) return 1; }
+    else ma.m[ph] = ma.m[0];
   }
+  if (p.slab && !make_map(&ma.m[1], o.A, p.Z, o.a_sb, o.a_rows, p.K, o.lda, span)) return 1;
+  if (!make_map(&mb.m[0], o.B, p.Q, o.b_sq, p.N, p.K, o.ldb, BN)) return 1;
+  mb.m[1] = mb.m[2] = mb.m[3] = mb.m[0];
   const size_t SMEM = (size_t)p.SA * p.a_stage + (size_t)p.SB * B_BYTES + 1024;
   auto kern = gemm_tma_kernel<BN, MT>;
   static bool attr_set = false;
@@ -528,19 +498,19 @@ int launch_gemm(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
   {
     auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
     const bool act_ok = p.act == EVK_ACT_NONE || p.act == EVK_ACT_LRELU || p.act == EVK_ACT_RELU;
-    p.fast = (act_ok && !p.atomic && !p.mode && (p.N % 4) == 0 && (p.ldd % 4) == 0 && (p.y_sb % 4) == 0 && al16(p.d) && (!p.bias || al16(p.bias)) &&
+    p.fast = (act_ok && !p.atomic && (p.N % 4) == 0 && (p.ldd % 4) == 0 && (p.y_sb % 4) == 0 && al16(p.d) && (!p.bias || al16(p.bias)) &&
               (!p.res || (al16(p.res) && (p.ldr % 4) == 0 && (p.r_sb % 4) == 0))) ? 1 : 0;
   }
   p.tiles_m = cdiv(p.M, MT * BM);
   p.tiles_n = cdiv(p.N, BN);
-  const int kb_total = p.mode ? p.Z * p.kbs : cdiv(p.K, BK);
+  const int kb_total = cdiv(p.K, BK);
   splits = max(1, min(splits, kb_total));
   p.kb_per_split = cdiv(kb_total, splits);
   p.splits = cdiv(kb_total, p.kb_per_split);
-  // split-K partials: [split][Q][M][N] in scratch (bounded: fewer splits when a large output would not fit)
-  const long long outq = (long long)(p.mode ? p.Q : 1) * p.M * p.N;
+  // split-K partials: [split][M][N] in scratch (bounded: fewer splits when a large output would not fit)
+  const long long outq = (long long)p.M * p.N;
   float* dst = p.d;
-  const long long dst_sq = p.d_sq, dst_ld = p.ldd;
+  const long long dst_ld = p.ldd;
   Scratch part_buf(0, st);
   if (p.atomic) {
     constexpr long long PART_CAP = 32ll << 20;
@@ -554,16 +524,16 @@ int launch_gemm(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
       part_buf.alloc((long long)p.splits * outq);
       p.d = part_buf.p;
       EVK_REQUIRE(p.d, EVK_ERR_CUDA, "gemm_tma: scratch allocation failed");
-      p.ldd = p.N; p.d_sq = (long long)p.M * p.N; p.d_ssp = outq;
+      p.ldd = p.N; p.d_ssp = outq;
     }
   }
-  const long long total = (long long)p.tiles_m * p.tiles_n * p.splits * (p.mode ? p.Q : p.Z);
+  const long long total = (long long)p.tiles_m * p.tiles_n * p.splits * p.Z;
   if (total > 0x7fffffff) return 1;
   if (total <= 0) return EVK_OK;
   const int grid = (int)(total < (long long)g_sm_count ? total : (long long)g_sm_count);
   kern<<<grid, GT_THREADS, SMEM, st>>>(ma, mb, p);
   if (int rc = check_launch("gemm_tma_kernel")) return rc;
-  return (p.atomic && p.d_ssp) ? ordered_sum(p.d, p.splits, outq, p.mode ? p.Q : 1, p.M, p.N, dst, dst_sq, dst_ld, st) : EVK_OK;
+  return (p.atomic && p.d_ssp) ? ordered_sum(p.d, p.splits, outq, 1, p.M, p.N, dst, 0, dst_ld, st) : EVK_OK;
 }
 
 // MT = 2 halves the weight-tile traffic per flop but doubles the tile: take it when the wave quantisation of the persistent
@@ -577,7 +547,7 @@ int launch_bn(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
     cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
   }
   if constexpr (BN == 32) {
-    if (g_opt_mt2 && !p.mode && splits <= 1 && p.M >= 2 * BM) {
+    if (g_opt_mt2 && splits <= 1 && p.M >= 2 * BM) {
       const long long per = (long long)cdiv(p.N, BN) * p.Z;
       const long long t1 = per * cdiv(p.M, BM), t2 = per * cdiv(p.M, 2 * BM);
       const double c1 = (double)cdiv(t1, g_sm_count), c2 = (double)cdiv(t2, g_sm_count) * 2.0 * 0.65;
@@ -593,6 +563,204 @@ int run_gemm(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
   if (p.N > 64) return launch_bn<128>(o, p, splits, st);
   if (p.N > 32) return launch_bn<64>(o, p, splits, st);
   return launch_bn<32>(o, p, splits, st);
+}
+
+
+// ---- conv weight gradient: dW[q][n][c] = sum_b sum_pos dY[b][pos][n] * X[b][pos + off[q] * P][c] -----------------------
+// The GEMM runs transposed, D[(q, c)][n]: the M rows are (tap, input channel) pairs, so one output tile holds 128 / C taps
+// of a narrow layer (4 at 32 channels, 2 at 64) and every tap of the tile shares the staged dY block.  K = positions.
+//   X side (A, from registers): per K block of 32 positions the producer stages, for each 32-row quarter of the tile,
+//     the channels-last box X[b][t0 + shift .. + 31][c0 .. c0 + 31] (128-byte swizzle).  The tap shift is the box's row
+//     coordinate (rows outside the input = the conv padding, zero-filled by the copy engine), so X is read in the layout
+//     the forward left it -- no transposed or delayed copies.  The consumer threads load their A fragments from that
+//     box with ordinary shared-memory loads (TF32 wgmma takes A from registers in any source layout).
+//   dY side (B, from shared memory): the K-major box dyt[b][n0 .. n0 + BN - 1][t0 .. t0 + 31] of the transposed output
+//     gradient that evk_dy_prep writes in its pass over dY (positions past the output are zero-filled).
+// Work item = (K split, m tile, n tile), n fastest; K iterations = batch items x 32-position blocks.  Splits store their
+// partials, which ordered_sum adds in split order, so the result does not depend on the schedule.
+struct WgradP {
+  float* d; int ldd; long long d_sq, d_ssp;           // output (pitch ldd, tap pitch d_sq); d_ssp > 0: split partials, else d += D
+  int N, C, Cp, nq, P;                                // Cp = C rounded up to 32: tile row r = q * Cp + c
+  int kbs, kb_total, tiles_m, tiles_n, splits, kb_per_split, ring;
+  int off[EVK_MAX_TAPS];
+  float comp;
+};
+
+constexpr int WG_A_BYTES = BM * BK * 4;               // four 32 x 32 X boxes
+
+template <int BN>
+__global__ void __launch_bounds__(GT_THREADS, 1) conv_wgrad_kernel(const __grid_constant__ CUtensorMap mapX,
+                                                                   const __grid_constant__ CUtensorMap mapD,
+                                                                   const __grid_constant__ WgradP p) {
+  constexpr int STAGE = WG_A_BYTES + BN * BK * 4;
+  extern __shared__ uint8_t gsm_raw[];
+  uint8_t* gsm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(gsm_raw) + 1023) & ~uintptr_t(1023));
+  __shared__ __align__(8) uint64_t full[MAX_RING], empty[MAX_RING];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < MAX_RING; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONSUMER_WARPS); }
+    asm volatile("fence.mbarrier_init.release.cluster;\n");
+    asm volatile("prefetch.tensormap [%0];\n" ::"l"(reinterpret_cast<uint64_t>(&mapX)));
+    asm volatile("prefetch.tensormap [%0];\n" ::"l"(reinterpret_cast<uint64_t>(&mapD)));
+  }
+  __syncthreads();
+  const int tiles_mn = p.tiles_m * p.tiles_n, total = tiles_mn * p.splits, ring = p.ring;
+
+  if (warp == 0) {
+    int s = 0, ph = 1;
+    const bool leader = elect_one();
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+      const int sp = tile / tiles_mn, mn = tile - sp * tiles_mn;
+      const int tm = mn / p.tiles_n, tn = mn - tm * p.tiles_n;
+      const int k0 = sp * p.kb_per_split, k1 = min(p.kb_total, k0 + p.kb_per_split);
+      int c0[4], sh[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {                            // quarter j of the tile = 32 channels of one tap
+        const int g = tm * 4 + j, per = p.Cp / 32;
+        const int q = min(g / per, p.nq - 1);                  // past the last tap: loaded, never written
+        c0[j] = (g - (g / per) * per) * 32;
+        sh[j] = p.off[q] * p.P;
+      }
+      int b = k0 / p.kbs, kk = k0 - b * p.kbs;
+      for (int ki = k0; ki < k1; ++ki) {
+        mbar_wait(&empty[s], ph);
+        if (leader) {
+          uint8_t* st = gsm + (size_t)s * STAGE;
+          mbar_expect_tx(&full[s], STAGE);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) tma_load_3d(st + j * (BK * BK * 4), &mapX, c0[j], kk * BK + sh[j], b, &full[s]);
+          tma_load_3d(st + WG_A_BYTES, &mapD, kk * BK, tn * BN, b, &full[s]);
+        }
+        if (++s == ring) { s = 0; ph ^= 1; }
+        if (++kk == p.kbs) { kk = 0; ++b; }
+      }
+    }
+  } else if (warp >= 4) {
+    const int cw = warp - 4, wg = cw >> 2, wq = cw & 3;
+    const int r0 = wg * 64 + wq * 16 + (lane >> 2);            // this thread's tile rows r0 and r0 + 8: quarter r0 / 32
+    // byte offsets of A(r0 + 8 e, k = lane % 4 + 4 h) in the swizzled box of quarter r0 / 32:
+    // position row k * 128, 16-byte chunk (channel / 4) ^ (k % 8); K step kstep adds 8 positions = 1024 bytes
+    uint32_t aoff[2][2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int cl = (r0 & 31) + 8 * e, k = (lane & 3) + 4 * h;
+        aoff[e][h] = (uint32_t)((r0 >> 5) * (BK * BK * 4) + k * 128 + ((((cl >> 2) ^ k) & 7) << 4) + (cl & 3) * 4);
+      }
+    const uint32_t ring_base = smem_u32(gsm);
+    int s = 0, ph = 0;
+    float acc[BN / 2];
+    float ra[BK / 8][4];
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+      const int sp = tile / tiles_mn, mn = tile - sp * tiles_mn;
+      const int tm = mn / p.tiles_n, tn = mn - tm * p.tiles_n;
+      const int k0 = sp * p.kb_per_split, k1 = min(p.kb_total, k0 + p.kb_per_split);
+      int rel = -1;
+      uint32_t accum = 0;
+      // One K block: retire the previous block's wgmma group (it read the A registers and the previous stage), load this
+      // block's A fragments, issue its four k8 steps.  The fragment loads overlap the TMA of the stages ahead.
+      for (int ki = k0; ki < k1; ++ki) {
+        mbar_wait(&full[s], ph);
+        wgmma_wait<0>();
+        if (lane == 0 && rel >= 0) mbar_arrive(&empty[rel]);
+        const uint32_t sa = ring_base + (uint32_t)s * STAGE;
+#pragma unroll
+        for (int k = 0; k < BK / 8; ++k)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              uint32_t v;
+              asm volatile("ld.shared.b32 %0, [%1];\n" : "=r"(v) : "r"(sa + aoff[e][h] + k * 1024));
+              ra[k][2 * h + e] = __uint_as_float(v & 0xffffe000u);    // TF32 by truncation, as the tensor core reads
+            }                                                         // a shared-memory operand
+        wgmma_fence();
+        const uint64_t db = wg_desc_sw128(sa + WG_A_BYTES);
+#pragma unroll
+        for (int k = 0; k < BK / 8; ++k) wgmma_tf32_rs<BN>(acc, ra[k], db + (uint64_t)(k * 2), accum | (uint32_t)k);
+        wgmma_commit();
+        rel = s;
+        accum = 1;
+        if (++s == ring) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (lane == 0 && rel >= 0) mbar_arrive(&empty[rel]);
+      if (!accum) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      }
+      // epilogue: D[(q, c)][n] -> dW[q][n][c]; acc[4 j + 2 h + x] = (row r0 + 8 h, column 8 j + 2 (lane % 4) + x)
+      float* dz = p.d + (size_t)sp * p.d_ssp;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = tm * BM + r0 + 8 * h, q = row / p.Cp, c = row - q * p.Cp;
+        if (q >= p.nq || c >= p.C) continue;
+        float* base = dz + (size_t)q * p.d_sq + c;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+          for (int x = 0; x < 2; ++x) {
+            const int n = tn * BN + 8 * j + 2 * (lane & 3) + x;
+            if (n >= p.N) continue;
+            float* dp = base + (size_t)n * p.ldd;
+            const float v = acc[4 * j + 2 * h + x] * p.comp;
+            *dp = p.d_ssp ? v : *dp + v;
+          }
+      }
+    }
+  }
+}
+
+template <int BN>
+int launch_wgrad(const CUtensorMap& mx, const float* dyt, int ld_dy, long long dy_sb, int B, int out_rows, WgradP& p, int splits,
+                 cudaStream_t st) {
+  constexpr int STAGE = WG_A_BYTES + BN * BK * 4;
+  CUtensorMap md;
+  if (!make_map(&md, dyt, B, dy_sb, p.N, out_rows, ld_dy, BN)) return 1;
+  if (!g_sm_count) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
+  }
+  p.ring = min(MAX_RING, SMEM_BUDGET / STAGE);
+  p.tiles_m = cdiv(p.nq * p.Cp, BM);
+  p.tiles_n = cdiv(p.N, BN);
+  p.kbs = cdiv(out_rows, BK);
+  p.kb_total = B * p.kbs;
+  p.comp = (1.f + g_trunc_comp) * (1.f + g_trunc_comp);     // both operands are raw activations / gradients
+  // split-K partials [split][nq][N][C] in scratch (bounded: fewer splits when a large output would not fit)
+  const long long outq = (long long)p.nq * p.N * p.C;
+  constexpr long long PART_CAP = 32ll << 20;
+  splits = max(1, min(splits, p.kb_total));
+  p.kb_per_split = cdiv(p.kb_total, splits);
+  p.splits = cdiv(p.kb_total, p.kb_per_split);
+  if ((long long)p.splits * outq > PART_CAP) {
+    splits = (int)max(1ll, PART_CAP / outq);
+    p.kb_per_split = cdiv(p.kb_total, splits);
+    p.splits = cdiv(p.kb_total, p.kb_per_split);
+  }
+  float* dst = p.d;
+  const long long dst_sq = p.d_sq, dst_ld = p.ldd;
+  Scratch part_buf(0, st);
+  p.d_ssp = 0;
+  if (p.splits > 1) {                                     // one split: every element has one writer, which adds in place
+    part_buf.alloc((long long)p.splits * outq);
+    EVK_REQUIRE(part_buf.p, EVK_ERR_CUDA, "conv_wgrad_tma: scratch allocation failed");
+    p.d = part_buf.p; p.ldd = p.C; p.d_sq = (long long)p.N * p.C; p.d_ssp = outq;
+  }
+  const long long total = (long long)p.tiles_m * p.tiles_n * p.splits;
+  if (total > 0x7fffffff) return 1;
+  const size_t SMEM = (size_t)p.ring * STAGE + 1024;
+  auto kern = conv_wgrad_kernel<BN>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET + 1024) != cudaSuccess) return 1;
+    attr_set = true;
+  }
+  kern<<<(int)min(total, (long long)g_sm_count), GT_THREADS, SMEM, st>>>(mx, md, p);
+  if (int rc = check_launch("conv_wgrad_kernel")) return rc;
+  return p.d_ssp ? ordered_sum(p.d, p.splits, outq, p.nq, p.N, p.C, dst, dst_sq, dst_ld, st) : EVK_OK;
 }
 
 }  // namespace
@@ -677,7 +845,7 @@ extern "C" int evk_gemm_tf32(const float* A, int32_t lda, const float* B, int32_
   p.d = D; p.ldd = ldd; p.bias = bias; p.res = res; p.ldr = ldr; p.M = M; p.N = N; p.K = K; p.act = act; p.slope = slope;
   p.atomic = splits > 1 ? 1 : 0;
   p.Z = 1; p.Q = 1; p.P = 1;
-  Operands o{A, lda, 0, M, B, ldb, 0, 0, 1, 0, 2};
+  Operands o{A, lda, 0, M, B, ldb, 0, 1, 0, 2};
   p.os = 1; p.o0 = 0;
   int rc = run_gemm(o, p, splits, st);
   EVK_REQUIRE(rc != 1, EVK_ERR_UNSUPPORTED, "gemm_tf32: cuTensorMapEncodeTiled unavailable or rejected the operand");
@@ -686,27 +854,30 @@ extern "C" int evk_gemm_tf32(const float* A, int32_t lda, const float* B, int32_
 }
 
 
-// Weight gradient of a stride-1 (dilated / period-folded) convolution on the TMA/wgmma GEMM:
+// Weight gradient of a stride-1 (dilated / period-folded) convolution on conv_wgrad_kernel:
 //   dW[q][n][c] += sum_b sum_pos dY[b][pos][n] * X[b][pos + off[q]*P][c]
-// with both operands pre-transposed so that the contraction index is contiguous: dyt [B][N][ld_dy] (rows = J*P valid),
-// xt [4][B][C][ld_x]: copy r is X^T delayed by r positions, xt_r[b][c][u] = X[b][u - r][c] (Tin*P + r valid; TMA box
-// coordinates along the contiguous dimension must be 16-byte aligned, so a tap shift s reads copy r = (-s) mod 4 at the
-// aligned offset s + r; only the copies that occur need to be filled).  One output tile per (tap, n tile, c tile, K split); out-of-range rows (the conv padding)
-// are zero-filled by the copy engine.  Accumulates into dW (pitch ldw, tap pitch w_sq): the K splits write partials that
-// are added in split order.
-extern "C" int evk_conv_wgrad_tma(const float* dyt, int32_t ld_dy, int64_t dy_sb, const float* xt, int32_t ld_x, int64_t x_sb, int64_t x_rs, float* dW,
+// x [B][in_rows][ldx] channels-last (batch pitch x_sb), read in place; dyt [B][N][ld_dy] = dY transposed (out_rows valid
+// positions per row, evk_dy_prep).  Out-of-range input rows (the conv padding) are zero-filled by the copy engine.
+// Accumulates into dW (pitch ldw, tap pitch w_sq): the K splits write partials that are added in split order.
+extern "C" int evk_conv_wgrad_tma(const float* x, int32_t ldx, int64_t x_sb, const float* dyt, int32_t ld_dy, int64_t dy_sb, float* dW,
                                   int32_t ldw, int64_t w_sq, int32_t B, int32_t N, int32_t C, int32_t out_rows, int32_t in_rows,
                                   int32_t Q, int32_t P, const int32_t* off, int32_t splits, cudaStream_t st) {
-  EVK_REQUIRE(B > 0 && N > 0 && C > 0 && out_rows > 0 && in_rows > 0 && Q > 0 && Q <= EVK_MAX_TAPS && off, EVK_ERR_ARG, "conv_wgrad_tma: bad sizes");
-  EVK_REQUIRE((ld_dy % 4) == 0 && (ld_x % 4) == 0 && (dy_sb % 4) == 0 && (x_sb % 4) == 0 && (x_rs % 4) == 0 && in_rows > 4 &&
-                  ((((uintptr_t)dyt) | ((uintptr_t)xt)) & 15) == 0,
+  EVK_REQUIRE(B > 0 && N > 0 && C > 0 && out_rows > 0 && in_rows > 0 && Q > 0 && Q <= EVK_MAX_TAPS && P > 0 && off, EVK_ERR_ARG,
+              "conv_wgrad_tma: bad sizes");
+  EVK_REQUIRE((C % 4) == 0 && (ldx % 4) == 0 && (ld_dy % 4) == 0 && (x_sb % 4) == 0 && (dy_sb % 4) == 0 &&
+                  ((((uintptr_t)x) | ((uintptr_t)dyt)) & 15) == 0,
               EVK_ERR_ARG, "conv_wgrad_tma: operands must be 16-byte aligned with pitches that are multiples of 4 floats");
-  GemmP p{};
-  p.d = dW; p.ldd = ldw; p.d_sq = w_sq; p.M = N; p.N = C; p.K = out_rows; p.atomic = 1; p.mode = 1;
-  p.Z = B; p.Q = Q; p.P = P; p.kbs = cdiv(out_rows, BK); p.os = 1; p.o0 = 0;
-  for (int i = 0; i < EVK_MAX_TAPS; ++i) p.off[i] = i < Q ? off[i] : 0;
-  Operands o{dyt, ld_dy, dy_sb, in_rows, xt, ld_x, x_sb, x_rs, 1, 0, 2};     // both operands are raw activations / gradients
-  int rc = run_gemm(o, p, splits < 1 ? 1 : splits, st);
+  CUtensorMap mx;
+  int rc = make_map(&mx, x, B, x_sb, in_rows, C, ldx, BK) ? 0 : 1;
+  if (rc == 0) {
+    WgradP p{};
+    p.d = dW; p.ldd = ldw; p.d_sq = w_sq; p.N = N; p.C = C; p.Cp = cdiv(C, 32) * 32; p.nq = Q; p.P = P;
+    for (int i = 0; i < EVK_MAX_TAPS; ++i) p.off[i] = i < Q ? off[i] : 0;
+    const int s = splits < 1 ? 1 : splits;
+    if (N > 64) rc = launch_wgrad<128>(mx, dyt, ld_dy, dy_sb, B, out_rows, p, s, st);
+    else if (N > 32) rc = launch_wgrad<64>(mx, dyt, ld_dy, dy_sb, B, out_rows, p, s, st);
+    else rc = launch_wgrad<32>(mx, dyt, ld_dy, dy_sb, B, out_rows, p, s, st);
+  }
   EVK_REQUIRE(rc != 1, EVK_ERR_UNSUPPORTED, "conv_wgrad_tma: cuTensorMapEncodeTiled unavailable or rejected the operand");
   if (rc == 0) g_disp_flops[4] += 2.0 * B * (double)out_rows * N * C * Q;
   return rc;

@@ -617,9 +617,10 @@ class _ConvFn(torch.autograd.Function):
             dpa = dpa_buffer(pa)
             ldx, mma = ldx_, mma_w
             if tma_w:
-                # dW[q][n][c] = sum_{b,pos} dY[b][pos][n] X[b][pos + shift_q][c]: both operands are transposed once (positions
-                # become the contiguous K dim), then the TMA-fed wgmma GEMM runs one output tile per (tap, n, c, K split)
-                # with the tap shift as a TMA coordinate (out-of-range rows = conv padding, zero-filled by the copy engine).
+                # dW[q][n][c] = sum_{b,pos} dY[b][pos][n] X[b][pos + shift_q][c] on conv_wgrad_kernel: X is read channels-last
+                # as the forward left it (the tap shift is a TMA row coordinate; out-of-range rows = conv padding,
+                # zero-filled by the copy engine), dY through the transposed copy dyt that evk_dy_prep wrote above.  The
+                # tile rows are (tap, input channel) pairs, so the taps of a narrow layer share each staged dY block.
                 # A strided conv is first split into `stride` phase copies of X (as in the forward): taps u = q - pad with
                 # u mod stride == rho form a stride-1 problem on copy rho with shifts floor(u / stride).
                 if stride == 1:
@@ -633,20 +634,17 @@ class _ConvFn(torch.autograd.Function):
                             srcs.append((xs[rho], C, Jp, qs, [offs[q] // stride for q in qs]))
                 for xsrc, ldsrc, Tsrc, qs, shifts in srcs:
                     Ri = Tsrc * P
-                    ldi = (Ri + 3 + 31) // 32 * 32
-                    xt = torch.empty((4, B, C, ldi), device=dy.device, dtype=torch.float32)
-                    mask = 0
-                    for sh in shifts:                                           # delayed copies: xt[r][b][c][u] = x[b][u - r][c]
-                        mask |= 1 << ((-sh * P) % 4)
-                    _call("evk_transpose_rows_multi", _p(xsrc), ldsrc, Ri * ldsrc, _p(xt), ldi, C * ldi, B * C * ldi, B, Ri, C, mask)
                     nq = len(qs)
                     qstep = (qs[1] - qs[0]) if nq > 1 else 1
-                    tiles = nq * ((N + 127) // 128) * ((C + 127) // 128)     # the TMA GEMM's tiles are at most 128 x 128
+                    # the split count fixes how the K sums are grouped, and so the bits of dW: it is a function of the layer
+                    # shape (taps x 128 x 128 channel blocks), not of the kernel's tiling, so a change of tiling leaves
+                    # the trained weights bit for bit where they were
+                    tiles = nq * ((N + 127) // 128) * ((C + 127) // 128)
                     kblocks = B * ((Ro + 31) // 32)
                     sms = torch.cuda.get_device_properties(dy.device).multi_processor_count
-                    splits = max(1, min(64, sms // tiles, kblocks // 8))        # one full wave of (tile, split) CTAs
+                    splits = max(1, min(64, sms // tiles, kblocks // 8))
                     offa = (ctypes.c_int32 * nq)(*shifts)
-                    _call_f("evk_conv_wgrad_tma", 2.0 * B * Ro * N * C * nq, _p(dyt), ldo, N * ldo, _p(xt), ldi, C * ldi, B * C * ldi,
+                    _call_f("evk_conv_wgrad_tma", 2.0 * B * Ro * N * C * nq, _p(xsrc), ldsrc, Ri * ldsrc, _p(dyt), ldo, N * ldo,
                             dpa.data_ptr() + 4 * qs[0] * N * lda, lda, qstep * N * lda, B, N, C, Ro, Ri, nq, P, offa, splits,
                             tag=f"B{B} Ro{Ro} P{P} C{C} N{N} nq{nq} splits{splits}")
             else:

@@ -349,14 +349,13 @@ int evk_gemm_tf32(const float* A, int32_t lda, const float* B, int32_t ldb, floa
                   int32_t K, const float* bias, const float* res, int32_t ldr, int32_t act, float slope, int32_t splits,
                   evk_stream_t stream);
 int evk_set_backend_tma(int32_t on);
-/* Weight gradient of a stride-1 (dilated, period-folded) conv on the same kernel:
+/* Weight gradient of a stride-1 (dilated, period-folded) conv on the TMA/wgmma path (conv_wgrad_kernel):
  *   dW[q][n][c] += sum_b sum_pos dY[b][pos][n] * X[b][pos + off[q]*P][c]
- * on operands transposed by evk_transpose_rows (contraction index contiguous): dyt [B][N][ld_dy] (out_rows = J*P valid),
- * xt [4][B][C][ld_x] with pitch x_rs between four copies delayed by r = 0..3 positions, xt_r[b][c][u] = X[b][u - r][c]
- * (in_rows + r valid, evk_transpose_rows with shift = r).  TMA coordinates along the contiguous dimension must be 16-byte
- * aligned: a tap shift s reads copy r = (-s) mod 4 at the aligned offset s + r; only the copies that occur need filling.  Rows outside the input (the conv padding) are zero-filled by the copy engine.
- * Accumulates the K splits' partials, added in split order, into dW (pitch ldw, tap pitch w_sq); off is a HOST array. */
-int evk_conv_wgrad_tma(const float* dyt, int32_t ld_dy, int64_t dy_sb, const float* xt, int32_t ld_x, int64_t x_sb, int64_t x_rs, float* dW,
+ * x [B][in_rows][ldx] channels-last (batch pitch x_sb, C % 4 == 0), read in place; dyt [B][N][ld_dy] = dY transposed
+ * (out_rows = J*P valid positions per row, evk_dy_prep).  Taps are stacked with the input channels in the tile rows, so the
+ * taps of a narrow layer share every staged dY block.  Rows outside the input (the conv padding) are zero-filled by the copy
+ * engine.  Accumulates the K splits' partials, added in split order, into dW (pitch ldw, tap pitch w_sq); off is a HOST array. */
+int evk_conv_wgrad_tma(const float* x, int32_t ldx, int64_t x_sb, const float* dyt, int32_t ld_dy, int64_t dy_sb, float* dW,
                        int32_t ldw, int64_t w_sq, int32_t B, int32_t N, int32_t C, int32_t out_rows, int32_t in_rows,
                        int32_t Q, int32_t P, const int32_t* off, int32_t splits, evk_stream_t stream);
 /* Everything a conv's backward needs from its output gradient in one pass (elementwise.cu): g = dy * act'(y) * (t < len*P);
@@ -380,9 +379,6 @@ int evk_gconv_fwd_phased(const evk_gconv_desc* d, int32_t phases, int64_t x_ps, 
  * y[b][c][u] = x[b][u - shift][c], zero for u < shift. */
 int evk_transpose_rows(const float* x, int32_t ldx, int64_t x_sb, float* y, int32_t ldy, int64_t y_sb, int32_t B, int32_t T,
                        int32_t C, int32_t shift, evk_stream_t stream);
-/* every delayed copy r (bit r of mask, r = 0..3) in one pass over x: y[r*y_rs + ...][b][c][u] = x[b][u - r][c]. */
-int evk_transpose_rows_multi(const float* x, int32_t ldx, int64_t x_sb, float* y, int32_t ldy, int64_t y_sb, int64_t y_rs,
-                             int32_t B, int32_t T, int32_t C, int32_t mask, evk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Stage-1 AR semantic-token GPT (t2s_model.py:431-490 forward_old, transformer.py:266-315, optim.py:123-622).
