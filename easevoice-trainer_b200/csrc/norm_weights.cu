@@ -35,13 +35,16 @@ __global__ void layernorm_fwd_kernel(const float* __restrict__ x, int ldx, const
 
 // A handful of rows (the token step of the KV-cache decode: ONE row of 512): the warp-per-row kernel above keeps 16 values per
 // lane in a run-time indexed array (local memory) and ran 11 us per launch; here a whole 256-thread block takes a row.
+// The block stages the row in shared memory and warp 0 takes both sums in the warp kernel's order (lane l adds channels l,
+// l + 32, ... in turn, then warp_sum), so a row's bits do not depend on whether 8 or 9 rows share the launch: a decode batch
+// of 9..64 rows gives each row what a batch of one gives it.
 __global__ void __launch_bounds__(256) layernorm_fwd_block_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ res, int ldr,
                                                                   const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
                                                                   float* __restrict__ y, int ldy, float* __restrict__ stats, int C) {
-  __shared__ float red[33];
+  __shared__ float sv[32 * LN_MAXV];
+  __shared__ float stat[2];
   const long long row = blockIdx.x;
   float v[4];
-  float s = 0.f;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int c = threadIdx.x + 256 * i;
@@ -49,18 +52,33 @@ __global__ void __launch_bounds__(256) layernorm_fwd_block_kernel(const float* _
     if (c < C) {
       t = x[row * ldx + c];
       if (res) t += res[row * ldr + c];
+      sv[c] = t;
     }
     v[i] = t;
-    s += t;
   }
-  const float mean = block_sum(s, red) / (float)C;
-  float q = 0.f;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float s = 0.f;
+    for (int c = threadIdx.x; c < C; c += 32) s += sv[c];
+    s = warp_sum(s);
+    if (threadIdx.x == 0) stat[0] = s / (float)C;
+  }
+  __syncthreads();
+  const float mean = stat[0];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const float d = (threadIdx.x + 256 * i < C) ? v[i] - mean : 0.f;
-    q += d * d;
+    const int c = threadIdx.x + 256 * i;
+    if (c < C) sv[c] = v[i] - mean;
   }
-  const float rstd = rsqrtf(block_sum(q, red) / (float)C + eps);
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float q = 0.f;
+    for (int c = threadIdx.x; c < C; c += 32) { const float d = sv[c]; q += d * d; }
+    q = warp_sum(q);
+    if (threadIdx.x == 0) stat[1] = rsqrtf(q / (float)C + eps);
+  }
+  __syncthreads();
+  const float rstd = stat[1];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int c = threadIdx.x + 256 * i;
