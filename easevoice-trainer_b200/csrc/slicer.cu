@@ -15,6 +15,10 @@
 // is above every number, as in np.abs(chunk).max().  Pass 2 applies the reference's float32 operations one by one, without
 // FMA contraction, and converts to int16 the way x86 numpy's astype does.  Both passes cut a chunk into tiles, so one long
 // chunk spreads over the whole device.
+//
+// evk_fragment_int16: TTS.audio_postprocess for every synthesised sentence at once.  The same max pass, then one apply pass that
+// divides by the max when it is above 1, scales by 32768, converts as above, writes each fragment at its place in the output
+// order and the silent interval after it.
 #include <limits.h>
 
 #include "evk_common.cuh"
@@ -83,6 +87,15 @@ __global__ void __launch_bounds__(RMS_THREADS) frame_rms_kernel(const float* __r
 
 constexpr int SL_THREADS = 256, SL_UNROLL = 8, SL_STEP = SL_THREADS * SL_UNROLL;
 
+// x86 numpy's float32 -> int16 astype: cvttss2si to int32 (NaN and everything outside int32 become INT_MIN, whose low 16 bits
+// are 0), then the low 16 bits
+__device__ __forceinline__ short to_int16_x86(float s) {
+  return (short)(fabsf(s) < 2147483648.f ? __float2int_rz(s) : INT_MIN);
+}
+
+// tile size for the longest of a set of ragged rows: at most 1024 tiles, of at least 8 * SL_STEP samples each
+inline long long slice_tile_size(long long max_len) { return max(8LL, (long long)cdiv(cdiv(max_len, 1024), SL_STEP)) * SL_STEP; }
+
 // tile blockIdx.x of chunk blockIdx.y -> the chunk's offset and [lo, hi) within the chunk
 __device__ __forceinline__ void slice_tile(const long long* __restrict__ chunks, long long tile, long long& off, long long& lo,
                                            long long& hi) {
@@ -138,10 +151,35 @@ __global__ void __launch_bounds__(SL_THREADS) slice_apply_kernel(const float* __
         const float v = x[i];
         const float c = loud ? __fdiv_rn(v, m) : v;                                   // audio.py:173-174, in place
         const float a = __fadd_rn(__fmul_rn(__fdiv_rn(c, m), c1), __fmul_rn(c2, c));  // audio.py:175: the old max again
-        const float s = __fmul_rn(a, 32767.f);
-        // cvttss2si: NaN and everything outside int32 become INT_MIN, whose low 16 bits are 0
-        const int k = fabsf(s) < 2147483648.f ? __float2int_rz(s) : INT_MIN;
-        y[i] = (short)k;
+        y[i] = to_int16_x86(__fmul_rn(a, 32767.f));
+      }
+    }
+  }
+}
+
+// TTS.audio_postprocess (inference/tts.py:878-907) for fragment blockIdx.y: y[dst, dst + len) = int16(c * 32768) with
+// c = m > 1 ? x / m : x, then y[dst + len, dst + len + gap) = 0.  Tiles of `tile` samples cover len + gap.
+__global__ void __launch_bounds__(SL_THREADS) fragment_apply_kernel(const float* __restrict__ x, const long long* __restrict__ frags,
+                                                                    const long long* __restrict__ dst, long long tile, long long gap,
+                                                                    const unsigned* __restrict__ mbits, short* __restrict__ y) {
+  const long long len = max(frags[2 * blockIdx.y + 1], 0LL), total = len + gap;
+  const long long lo = min(total, (long long)blockIdx.x * tile), hi = min(total, lo + tile);
+  if (lo >= hi) return;
+  x += frags[2 * blockIdx.y];
+  y += dst[blockIdx.y];
+  const float m = __uint_as_float(mbits[blockIdx.y]);
+  const bool loud = m > 1.f;
+  for (long long base = lo + threadIdx.x; base < hi; base += SL_STEP) {
+#pragma unroll
+    for (int u = 0; u < SL_UNROLL; ++u) {
+      const long long i = base + (long long)u * SL_THREADS;
+      if (i < hi) {
+        short k = 0;
+        if (i < len) {
+          const float v = x[i];
+          k = to_int16_x86(__fmul_rn(loud ? __fdiv_rn(v, m) : v, 32768.f));
+        }
+        y[i] = k;
       }
     }
   }
@@ -169,12 +207,24 @@ extern "C" int evk_slice_normalize(const float* x, const int64_t* chunks, int32_
                                    int16_t* y, float* m, int32_t* status, evk_stream_t stream) {
   EVK_REQUIRE(x && chunks && y && m && status && n_chunks >= 1 && n_chunks <= 65535 && max_len >= 1, EVK_ERR_ARG,
               "slice_normalize: bad arguments");
-  // at most 1024 tiles for the longest chunk, of at least 8 * SL_STEP samples each
-  const long long tile = max(8LL, (long long)cdiv(cdiv(max_len, 1024), SL_STEP)) * SL_STEP;
+  const long long tile = slice_tile_size(max_len);
   const dim3 grid(cdiv(max_len, tile), n_chunks);
   cudaStream_t st = (cudaStream_t)stream;
   if (cudaMemsetAsync(m, 0, sizeof(float) * n_chunks, st) != cudaSuccess) return check_launch("slice_normalize (memset)");
   slice_max_kernel<<<grid, SL_THREADS, 0, st>>>(x, (const long long*)chunks, tile, (unsigned*)m);
   slice_apply_kernel<<<grid, SL_THREADS, 0, st>>>(x, (const long long*)chunks, tile, (const unsigned*)m, c1, c2, y, status);
   return check_launch("slice_normalize");
+}
+
+extern "C" int evk_fragment_int16(const float* x, const int64_t* frags, const int64_t* dst, int32_t n_frags, int64_t max_len,
+                                  int64_t gap, int16_t* y, float* m, evk_stream_t stream) {
+  EVK_REQUIRE(x && frags && dst && y && m && n_frags >= 1 && n_frags <= 65535 && max_len >= 1 && gap >= 0, EVK_ERR_ARG,
+              "fragment_int16: bad arguments");
+  const long long tile = slice_tile_size(max_len);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (cudaMemsetAsync(m, 0, sizeof(float) * n_frags, st) != cudaSuccess) return check_launch("fragment_int16 (memset)");
+  slice_max_kernel<<<dim3(cdiv(max_len, tile), n_frags), SL_THREADS, 0, st>>>(x, (const long long*)frags, tile, (unsigned*)m);
+  fragment_apply_kernel<<<dim3(cdiv(max_len + gap, tile), n_frags), SL_THREADS, 0, st>>>(
+      x, (const long long*)frags, (const long long*)dst, tile, gap, (const unsigned*)m, y);
+  return check_launch("fragment_int16");
 }

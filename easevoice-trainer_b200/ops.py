@@ -2377,6 +2377,22 @@ def slice_normalize(x, chunks, max_len, c1, c2, out=None):
     return out, m, status
 
 
+def fragment_int16(x, frags, dst, max_len, gap, out):
+    """evk_fragment_int16: TTS.audio_postprocess over the flat fp32 device buffer x.  frags: int64 device [n, 2] = (offset in x,
+    length), dst: int64 device [n] = offset in out, max_len >= every length, gap the zero samples after every fragment; out:
+    int16 device buffer, written at [dst, dst + length + gap) of every fragment.  -> m fp32 [n] = max |fragment|."""
+    assert x.dtype == torch.float32 and x.is_cuda and x.is_contiguous()
+    assert frags.dtype == torch.int64 and frags.is_cuda and frags.is_contiguous() and frags.dim() == 2 and frags.shape[1] == 2
+    assert dst.dtype == torch.int64 and dst.is_contiguous() and dst.shape == (frags.shape[0],)
+    assert out.dtype == torch.int16 and out.is_cuda and out.is_contiguous()
+    n = frags.shape[0]
+    m = torch.empty(n, device=x.device, dtype=torch.float32)
+    for i in range(0, n, SLICE_MAX_CHUNKS):
+        k = min(SLICE_MAX_CHUNKS, n - i)
+        _call("evk_fragment_int16", _p(x), _p(frags[i:]), _p(dst[i:]), k, int(max_len), int(gap), _p(out), _p(m[i:]))
+    return m
+
+
 def vr_assemble(x, pred, pred_tta, coef, bands, gains, high=None, mirror_lo=0, top=-1):
     """evk_vr_assemble: combined spectrogram x [2, n_rows, l, 2], pred / pred_tta [2, n_rows, l] and coef [1] -> one
     [4, l, n_fft/2+1, 2] frame tensor per band (rows y ch0, y ch1, v ch0, v ch1: evk_istft's input with B = 4, S = 1).

@@ -640,6 +640,14 @@ enum evk_slice_status { EVK_SLICE_OK = 0, EVK_SLICE_SILENT = 1, EVK_SLICE_NONFIN
  * NaN or Inf, else EVK_SLICE_OK.  Samples outside every chunk are not written. */
 int evk_slice_normalize(const float* x, const int64_t* chunks, int32_t n_chunks, int64_t max_len, float c1, float c2, int16_t* y,
                         float* m, int32_t* status, evk_stream_t stream);
+/* TTS.audio_postprocess (inference/tts.py:878-907), tts.py.  frags: int64 device [n_frags][2] = (offset in x, length), dst:
+ * int64 device [n_frags] = offset in y, max_len >= every length (host), n_frags <= 65535, gap >= 0 (int(sr * interval)).
+ * Per fragment, m = max |x| (NaN if a sample is NaN) is written to m [n_frags] (device) and
+ *   y[dst + i] = int16((m > 1 ? x[i] / m : x[i]) * 32768)  for i < length,   y[dst + length + j] = 0  for j < gap,
+ * float32 operations without contraction, converted as evk_slice_normalize converts: 1.0 gives -32768, as the reference does.
+ * Samples of y outside every [dst, dst + length + gap) are not written. */
+int evk_fragment_int16(const float* x, const int64_t* frags, const int64_t* dst, int32_t n_frags, int64_t max_len, int64_t gap,
+                       int16_t* y, float* m, evk_stream_t stream);
 
 #ifdef __cplusplus
 }
