@@ -34,7 +34,7 @@ __global__ void direct_fwd_thread(const __grid_constant__ DP p) {
   }
   const int oj = p.o0 + j * p.os;
   const long long orow = (long long)oj * p.P + w;
-  if (p.bias) acc += p.bias[n];
+  if (p.bias) acc += p.bias[h * p.b_sh + n];
   if (p.res) acc += (p.res + b * p.r_sb + h * p.r_sh)[orow * p.ldr + n];
   acc = conv_act(acc, p.act, p.slope);
   if (p.out_len && oj >= p.out_len[b]) acc = 0.f;
@@ -68,7 +68,7 @@ __global__ void direct_fwd_warp(const __grid_constant__ DP p) {
   if (lane) return;
   const int oj = p.o0 + j * p.os;
   const long long orow = (long long)oj * p.P + w;
-  if (p.bias) acc += p.bias[n];
+  if (p.bias) acc += p.bias[h * p.b_sh + n];
   if (p.res) acc += (p.res + b * p.r_sb + h * p.r_sh)[orow * p.ldr + n];
   acc = conv_act(acc, p.act, p.slope);
   if (p.out_len && oj >= p.out_len[b]) acc = 0.f;
@@ -136,7 +136,7 @@ __global__ void direct_wgrad(const __grid_constant__ DP p, float* __restrict__ p
 }  // namespace evk
 using namespace evk;
 
-extern "C" int evk_conv_direct_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
+int evk::conv_direct_fwd(const evk_gconv_desc* d, cudaStream_t st) {
   DP p;
   int rc = conv_params(d, p, "conv_direct_fwd");
   if (rc) return rc;
@@ -145,10 +145,10 @@ extern "C" int evk_conv_direct_fwd(const evk_gconv_desc* d, evk_stream_t stream)
   const int K = p.Q * (p.C / p.G);
   if (K >= 512) {
     dim3 grid(cdiv(total * 32, 256), 1, p.Z);
-    direct_fwd_warp<<<grid, 256, 0, (cudaStream_t)stream>>>(p);
+    direct_fwd_warp<<<grid, 256, 0, st>>>(p);
   } else {
     dim3 grid(cdiv(total, 256), 1, p.Z);
-    direct_fwd_thread<<<grid, 256, 0, (cudaStream_t)stream>>>(p);
+    direct_fwd_thread<<<grid, 256, 0, st>>>(p);
   }
   g_disp_flops[3] += desc_flops(d);
   return check_launch("conv_direct_fwd");
@@ -166,7 +166,7 @@ extern "C" int evk_conv_direct_dgrad(const evk_gconv_desc* d, evk_stream_t strea
   return check_launch("conv_direct_dgrad");
 }
 
-extern "C" int evk_conv_direct_wgrad(const evk_gconv_desc* d, evk_stream_t stream) {
+int evk::conv_direct_wgrad(const evk_gconv_desc* d, cudaStream_t st) {
   DP p;
   int rc = conv_params(d, p, "conv_direct_wgrad");
   if (rc) return rc;
@@ -181,18 +181,18 @@ extern "C" int evk_conv_direct_wgrad(const evk_gconv_desc* d, evk_stream_t strea
   dim3 grid(cdiv(npos, chunk), wblocks, p.Z);
   EVK_REQUIRE(grid.y <= 65535, EVK_ERR_ARG, "conv_direct_wgrad: too many weights");
   const int chunks = (int)grid.x, Cg = p.C / p.G;
-  Scratch part_buf(nw * chunks * p.Z, (cudaStream_t)stream);
+  Scratch part_buf(nw * chunks * p.Z, st);
   float* part = part_buf.p;
   EVK_REQUIRE(part, EVK_ERR_CUDA, "conv_direct_wgrad: scratch allocation failed");
-  direct_wgrad<<<grid, 256, 0, (cudaStream_t)stream>>>(p, part);
+  direct_wgrad<<<grid, 256, 0, st>>>(p, part);
   g_disp_flops[6] += desc_flops(d);
   if (int rc2 = check_launch("conv_direct_wgrad")) return rc2;
   if (p.w_sb == 0 && p.w_sh == 0)                                  // one weight for every z: all partials in (z, chunk) order
-    return ordered_sum(part, p.Z * chunks, p.Q, p.N, Cg, p.w, p.w_sq, p.ldw, (cudaStream_t)stream);
+    return ordered_sum(part, p.Z * chunks, p.Q, p.N, Cg, p.w, p.w_sq, p.ldw, st);
   for (int z = 0; z < p.Z; ++z) {                                  // z in order, each adding its chunks
     const int b = z / p.H, h = z - b * p.H;
     if (int rc2 = ordered_sum(part + (long long)z * chunks * nw, chunks, p.Q, p.N, Cg, p.w + b * p.w_sb + h * p.w_sh, p.w_sq, p.ldw,
-                              (cudaStream_t)stream))
+                              st))
       return rc2;
   }
   return EVK_OK;

@@ -320,25 +320,6 @@ __global__ void __launch_bounds__(256) dy_prep_kernel(const float* __restrict__ 
   }
 }
 
-// stride-phase split: xs[rho][b][j*P + w][c] = x[b][(j*s + rho)*P + w][c] (zero when j*s + rho >= T), j < Jp
-__global__ void phase_split_kernel(const float* __restrict__ x, int ldx, long long x_sb, float* __restrict__ xs, long long xs_ps,
-                                   int B, int T, int P, int C, int s, int Jp) {
-  const int c4n = C / 4;
-  const long long n = (long long)s * B * Jp * P * c4n;
-  EW_LOOP(i, n) {
-    int c4 = (int)(i % c4n);
-    long long r = i / c4n;
-    int w = (int)(r % P); r /= P;
-    int j = (int)(r % Jp); r /= Jp;
-    int b = (int)(r % B);
-    int rho = (int)(r / B);
-    const int t = j * s + rho;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (t < T) v = *reinterpret_cast<const float4*>(x + b * x_sb + ((long long)t * P + w) * ldx + c4 * 4);
-    *reinterpret_cast<float4*>(xs + rho * xs_ps + (((long long)b * Jp + j) * P + w) * C + c4 * 4) = v;
-  }
-}
-
 __global__ void embedding_kernel(const float* __restrict__ tab, int ldt, const long long* __restrict__ idx, long long rows,
                                  int rep, float* __restrict__ y, int ldy, int C) {
   EW_LOOP(i, rows * C) {
@@ -593,15 +574,6 @@ extern "C" int evk_dy_prep(const float* dy, int32_t lddy, const float* yact, int
   dy_prep_kernel<<<grid, block, 0, ST>>>(dy, lddy, yact, ldy, act, slope, gscale, len, P, dpre, ldp, dyt, ldt, t_sb, part, T, C);
   if (int rc = check_launch("dy_prep")) return rc;
   return dbias ? ordered_sum(part, S, 1, 1, C, dbias, 0, 0, ST) : EVK_OK;
-}
-extern "C" int evk_phase_split(const float* x, int32_t ldx, int64_t x_sb, float* xs, int64_t xs_ps, int32_t B, int32_t T, int32_t P,
-                               int32_t C, int32_t stride, int32_t Jp, evk_stream_t stream) {
-  EVK_REQUIRE(x && xs && (C % 4) == 0 && (ldx % 4) == 0 && (x_sb % 4) == 0 && (xs_ps % 4) == 0 && stride >= 1 && Jp * stride >= T,
-              EVK_ERR_ARG, "phase_split: bad arguments");
-  long long n = (long long)stride * B * Jp * P * (C / 4);
-  if (n == 0) return EVK_OK;
-  phase_split_kernel<<<grid1d(n), 256, 0, ST>>>(x, ldx, x_sb, xs, xs_ps, B, T, P, C, stride, Jp);
-  return check_launch("phase_split");
 }
 extern "C" int evk_embedding(const float* table, int32_t ldt, const int64_t* idx, int64_t rows, int32_t rep, float* y,
                              int32_t ldy, int32_t C, evk_stream_t stream) {

@@ -346,6 +346,8 @@ int g_precise = 0;          // 3xTF32 products on the mma.sync kernels (parity t
 int g_backend_tc = 1;       // use the TMA / wgmma kernels for eligible (stride-1) launches
 int gconv_tc_try(const ConvP& c, cudaStream_t st);
 int gemm_tma_try(const evk_gconv_desc* d, cudaStream_t st);
+int gemm_tma_phased(const evk_gconv_desc* d, cudaStream_t st);
+int conv_wgrad_tma(const evk_gconv_desc* d, const float* dyt, int ld_dyt, cudaStream_t st);
 
 int conv_params(const evk_gconv_desc* d, ConvP& p, const char* who) {
   EVK_REQUIRE(d != nullptr, EVK_ERR_ARG, "%s: null descriptor", who);
@@ -375,14 +377,26 @@ int conv_params(const evk_gconv_desc* d, ConvP& p, const char* who) {
   return EVK_OK;
 }
 
-static int check_mma_alignment(const evk_gconv_desc* d, const char* who) {
-  EVK_REQUIRE(d->G <= 1, EVK_ERR_UNSUPPORTED, "%s: pass groups as the inner batch (H = groups), not G", who);
-  EVK_REQUIRE((d->ldx % 4) == 0 && (d->ldw % 4) == 0 && (d->w_sq % 4) == 0, EVK_ERR_ARG,
-              "%s: ldx, ldw, w_sq must be multiples of 4 (ldx=%d ldw=%d)", who, d->ldx, d->ldw);
-  EVK_REQUIRE((d->x_sb % 4) == 0 && (d->x_sh % 4) == 0 && (d->w_sb % 4) == 0 && (d->w_sh % 4) == 0, EVK_ERR_ARG,
-              "%s: batch strides must be multiples of 4", who);
-  EVK_REQUIRE(((uintptr_t)d->x % 16) == 0 && ((uintptr_t)d->w % 16) == 0, EVK_ERR_ARG, "%s: x/w must be 16-byte aligned", who);
-  return EVK_OK;
+// The launch with groups as the inner batch (z = b * G + g), the form the tensor-core kernels take.  False for a launch
+// that has both groups and an inner batch: only the direct kernels take that.
+static bool groups_as_batch(const evk_gconv_desc* d, evk_gconv_desc& h) {
+  h = *d;
+  if (d->G <= 1) return true;
+  if (d->H > 1) return false;
+  const int G = d->G, Cg = d->C / G, Ng = d->N / G;
+  h.Z = d->Z * G; h.H = G; h.G = 1; h.C = Cg; h.N = Ng;
+  h.x_sh = Cg; h.w_sh = (long long)Ng * d->ldw; h.y_sh = Ng; h.r_sh = Ng; h.b_sh = Ng;
+  return true;
+}
+
+// 16-byte tileable operands: what the tensor-core kernels stage with 16-byte copies (forward: X and W, weight gradient: X and dY)
+static bool fwd_tileable(const evk_gconv_desc* h) {
+  return (h->ldx % 4) == 0 && (h->ldw % 4) == 0 && (h->w_sq % 4) == 0 && (h->x_sb % 4) == 0 && (h->x_sh % 4) == 0 &&
+         (h->w_sb % 4) == 0 && (h->w_sh % 4) == 0 && ((uintptr_t)h->x % 16) == 0 && ((uintptr_t)h->w % 16) == 0;
+}
+static bool wgrad_tileable(const evk_gconv_desc* h) {
+  return (h->ldx % 4) == 0 && (h->ldy % 4) == 0 && (h->x_sb % 4) == 0 && (h->x_sh % 4) == 0 && (h->y_sb % 4) == 0 &&
+         (h->y_sh % 4) == 0 && ((uintptr_t)h->x % 16) == 0 && ((uintptr_t)h->y % 16) == 0;
 }
 
 template <int WARPS_M, int WARPS_N, int MF, int NF, bool PRECISE>
@@ -435,18 +449,21 @@ extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
   GP p;
   int rc = conv_params(d, p, "gconv_fwd");
   if (rc) return rc;
-  rc = check_mma_alignment(d, "gconv_fwd");
-  if (rc) return rc;
   EVK_REQUIRE(d->y != nullptr && d->x != nullptr && d->w != nullptr, EVK_ERR_ARG, "gconv_fwd: null tensor");
   cudaStream_t st = (cudaStream_t)stream;
-  if (g_backend_tc && !g_precise && (d->ldx % 4) == 0) {
-    rc = gemm_tma_try(d, st);          // TMA-fed persistent wgmma GEMM / implicit-GEMM conv
+  evk_gconv_desc h;
+  const bool tiled = groups_as_batch(d, h) && fwd_tileable(&h);
+  if (tiled && !g_precise) {
+    rc = h.is > 1 ? gemm_tma_phased(&h, st) : g_backend_tc ? gemm_tma_try(&h, st) : 1;
     if (rc <= 0) { if (rc == 0) g_disp_flops[0] += desc_flops(d); return rc; }
-    EVK_REQUIRE(!(d->drop_rng && d->drop_p > 0.f), EVK_ERR_UNSUPPORTED, "gconv_fwd: fused dropout needs a launch the TMA kernel takes");
+  }
+  EVK_REQUIRE(!(d->drop_rng && d->drop_p > 0.f), EVK_ERR_UNSUPPORTED, "gconv_fwd: fused dropout needs a launch the TMA kernel takes");
+  if (!tiled) return conv_direct_fwd(d, st);
+  conv_params(&h, p, "gconv_fwd");
+  if (g_backend_tc && !g_precise) {
     rc = gconv_tc_try(p, st);
     if (rc <= 0) { if (rc == 0) g_disp_flops[1] += desc_flops(d); return rc; }
   }
-  EVK_REQUIRE(!(d->drop_rng && d->drop_p > 0.f), EVK_ERR_UNSUPPORTED, "gconv_fwd: fused dropout needs a launch the TMA kernel takes");
   g_disp_flops[2] += desc_flops(d);
   // pick the N tile with the least padding (prefer wide)
   const int N = p.N;
@@ -534,18 +551,29 @@ static int launch_w(GP& p, cudaStream_t st) {
   return EVK_OK;
 }
 
-extern "C" int evk_gconv_wgrad(const evk_gconv_desc* d, evk_stream_t stream) {
+// conv_wgrad_kernel's launches (evk_gconv_wgrad_takes_dyt)
+static bool wgrad_tma_eligible(const evk_gconv_desc* d) {
+  const long long npos = (long long)d->J * d->P;
+  if (g_precise || d->is > 4 || d->os != 1 || d->o0 != 0 || d->H != 1 || d->G > 1 || d->w_sb || d->in_len || (d->C % 4) ||
+      d->C < 32 || d->N < 32 || npos < 64 || d->Z * npos < 2048 || !wgrad_tileable(d))
+    return false;
+  for (int q = 1; d->is > 1 && q < d->Q; ++q)
+    if (d->off[q] != d->off[0] + q) return false;
+  return true;
+}
+
+extern "C" int evk_gconv_wgrad_takes_dyt(const evk_gconv_desc* d) { return d && wgrad_tma_eligible(d) ? 1 : 0; }
+
+extern "C" int evk_gconv_wgrad(const evk_gconv_desc* d, const float* dyt, int32_t ld_dyt, evk_stream_t stream) {
   GP p;
   int rc = conv_params(d, p, "gconv_wgrad");
   if (rc) return rc;
-  EVK_REQUIRE(d->G <= 1, EVK_ERR_UNSUPPORTED, "gconv_wgrad: pass groups as the inner batch (H = groups), not G");
-  EVK_REQUIRE((d->ldx % 4) == 0 && (d->ldy % 4) == 0, EVK_ERR_ARG,
-              "gconv_wgrad: ldx, ldy must be multiples of 4 (ldx=%d ldy=%d)", d->ldx, d->ldy);
-  EVK_REQUIRE(((uintptr_t)d->x % 16) == 0 && ((uintptr_t)d->y % 16) == 0, EVK_ERR_ARG, "gconv_wgrad: x/y must be 16-byte aligned");
-  EVK_REQUIRE((d->x_sb % 4) == 0 && (d->x_sh % 4) == 0 && (d->y_sb % 4) == 0 && (d->y_sh % 4) == 0, EVK_ERR_ARG,
-              "gconv_wgrad: batch strides must be multiples of 4");
   EVK_REQUIRE(d->y != nullptr && d->x != nullptr && d->w != nullptr, EVK_ERR_ARG, "gconv_wgrad: null tensor");
   cudaStream_t st = (cudaStream_t)stream;
+  if (dyt && wgrad_tma_eligible(d)) return conv_wgrad_tma(d, dyt, ld_dyt, st);
+  evk_gconv_desc h;
+  if (!groups_as_batch(d, h) || !wgrad_tileable(&h)) return conv_direct_wgrad(d, st);
+  conv_params(&h, p, "gconv_wgrad");
   g_disp_flops[5] += desc_flops(d);
   const long long ncols = (long long)p.Q * ((p.C + 3) & ~3);
 #define EVK_W(...) (g_precise ? launch_w<__VA_ARGS__, true>(p, st) : launch_w<__VA_ARGS__, false>(p, st))

@@ -441,6 +441,14 @@ bool make_map(CUtensorMap* m, const float* base, long long outer, long long sb, 
 }
 
 int g_sm_count = 0;
+int sm_count() {
+  if (!g_sm_count) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
+  }
+  return g_sm_count;
+}
 int g_opt_slab = 1, g_opt_mt2 = 1;          // A/B switches (evk_set_tma_options)
 // The tensor core reads fp32 operands as TF32 by DROPPING the low 13 mantissa bits (truncation towards zero): every product
 // is biased by -2^-11 * E[1/m] = -3.5e-4 relative per truncated operand (m = mantissa in [1,2), log-uniform).  Weights are
@@ -541,11 +549,7 @@ int launch_gemm(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
 // the 32-channel layers use it: they are bound by operand traffic, the wider ones by the tensor core.
 template <int BN>
 int launch_bn(const Operands& o, GemmP& p, int splits, cudaStream_t st) {
-  if (!g_sm_count) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
-  }
+  sm_count();
   if constexpr (BN == 32) {
     if (g_opt_mt2 && splits <= 1 && p.M >= 2 * BM) {
       const long long per = (long long)cdiv(p.N, BN) * p.Z;
@@ -718,11 +722,7 @@ int launch_wgrad(const CUtensorMap& mx, const float* dyt, int ld_dy, long long d
   constexpr int STAGE = WG_A_BYTES + BN * BK * 4;
   CUtensorMap md;
   if (!make_map(&md, dyt, B, dy_sb, p.N, out_rows, ld_dy, BN)) return 1;
-  if (!g_sm_count) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
-  }
+  sm_count();
   p.ring = min(MAX_RING, SMEM_BUDGET / STAGE);
   p.tiles_m = cdiv(p.nq * p.Cp, BM);
   p.tiles_n = cdiv(p.N, BN);
@@ -767,10 +767,10 @@ int launch_wgrad(const CUtensorMap& mx, const float* dyt, int ld_dy, long long d
 
 int g_backend_tma = 1;
 
-// returns 0 on success, < 0 on error, 1 if this launch is not eligible (caller falls through to gconv_tc / mma.sync).
-// phases > 1: d->x points at `phases` stride-phase copies of the input (pitch x_ps floats, see evk_phase_split) and tap q
-// reads copy src[q] with row shift off[q] -- a strided conv expressed as a stride-1 multi-source tap sum.
-int gemm_tma_run(const evk_gconv_desc* d, int phases, long long x_ps, const int* src, cudaStream_t st) {
+// Fills o and p for the launch d: returns 0, or 1 if it is not eligible.  phases > 1: d->x points at `phases` stride-phase
+// copies of the input (pitch x_ps floats, see split_phases) and tap q reads copy src[q] with row shift off[q] -- a strided
+// conv expressed as a stride-1 multi-source tap sum.
+static int gemm_tma_plan(const evk_gconv_desc* d, int phases, long long x_ps, const int* src, Operands& o, GemmP& p) {
   if (!g_backend_tma) return 1;
   if (d->is != 1 || d->os < 1 || d->o0 < 0 || d->H != 1 || d->Q < 1 || d->Q > EVK_MAX_TAPS || phases < 1 || phases > 4) return 1;
   if (d->in_len) return 1;                                  // ragged inputs are masked at staging time by the tap kernel
@@ -778,7 +778,7 @@ int gemm_tma_run(const evk_gconv_desc* d, int phases, long long x_ps, const int*
   if (((uintptr_t)d->x | (uintptr_t)d->w | (uintptr_t)d->y) & 15) return 1;
   if ((d->x_sb % 4) || (d->w_sq % 4) || (x_ps % 4) || (d->Z > 1 && d->w_sb != 0) || d->w_sq < 0 || d->x_sb < 0) return 1;
   const long long npos = (long long)d->J * d->P, in_rows = (long long)d->Tin * d->P;
-  GemmP p{};
+  p = GemmP{};
   p.d = d->y; p.ldd = d->ldy; p.bias = d->bias; p.res = d->res; p.ldr = d->ldr;
   p.N = d->N; p.K = d->C; p.act = d->act; p.slope = d->slope; p.atomic = 0;
   p.Q = d->Q; p.P = d->P; p.out_len = d->out_len; p.os = d->os; p.o0 = d->o0;
@@ -789,7 +789,7 @@ int gemm_tma_run(const evk_gconv_desc* d, int phases, long long x_ps, const int*
     p.src[i] = (src && i < d->Q) ? src[i] : 0;
     if (p.src[i] < 0 || p.src[i] >= phases) return 1;
   }
-  Operands o{};
+  o = Operands{};
   o.B = d->w; o.ldb = d->ldw; o.b_sq = d->w_sq; o.a_phases = phases; o.a_ps = x_ps;
   o.raw_operands = 1;                                       // A = activations (raw fp32), B = packed weights (already TF32, rounded to nearest)
   const bool flat = phases == 1 && d->Q == 1 && d->off[0] == 0 && d->P == 1 && !d->out_len && d->J == d->Tin && d->os == 1 && d->o0 == 0 &&
@@ -805,10 +805,116 @@ int gemm_tma_run(const evk_gconv_desc* d, int phases, long long x_ps, const int*
     p.M = (int)npos; p.Z = d->Z; p.y_sb = d->y_sb; p.r_sb = d->r_sb;
     o.A = d->x; o.lda = d->ldx; o.a_sb = d->x_sb; o.a_rows = in_rows;
   }
+  return 0;
+}
+
+// returns 0 on success, < 0 on error, 1 if this launch is not eligible (caller falls through to gconv_tc / mma.sync)
+int gemm_tma_try(const evk_gconv_desc* d, cudaStream_t st) {
+  Operands o; GemmP p;
+  return gemm_tma_plan(d, 1, 0, nullptr, o, p) ? 1 : run_gemm(o, p, 1, st);
+}
+
+// The stride phases of a conv input: tap offset u reads phase copy u mod s at row shift floor(u / s).
+static void phase_of(int u, int s, int& copy, int& shift) {
+  copy = ((u % s) + s) % s;
+  shift = (u - copy) / s;
+}
+
+// stride-phase split: xs[rho][b][j*P + w][c] = x[b][(j*s + rho)*P + w][c] (zero when j*s + rho >= T), j < Jp
+__global__ void phase_split_kernel(const float* __restrict__ x, int ldx, long long x_sb, float* __restrict__ xs, long long xs_ps,
+                                   int B, int T, int P, int C, int s, int Jp) {
+  const int c4n = C / 4;
+  const long long n = (long long)s * B * Jp * P * c4n;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    int c4 = (int)(i % c4n);
+    long long r = i / c4n;
+    int w = (int)(r % P); r /= P;
+    int j = (int)(r % Jp); r /= Jp;
+    int b = (int)(r % B);
+    int rho = (int)(r / B);
+    const int t = j * s + rho;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (t < T) v = *reinterpret_cast<const float4*>(x + b * x_sb + ((long long)t * P + w) * ldx + c4 * 4);
+    *reinterpret_cast<float4*>(xs + rho * xs_ps + (((long long)b * Jp + j) * P + w) * C + c4 * 4) = v;
+  }
+}
+
+// d's input split into its `is` stride phases in scratch: copies x_ps floats apart, each [Z][ceil(Tin / is) * P][C]
+static int split_phases(const evk_gconv_desc* d, Scratch& xs, long long& x_ps, cudaStream_t st) {
+  const int Jp = cdiv(d->Tin, d->is);
+  x_ps = (long long)d->Z * Jp * d->P * d->C;
+  xs.alloc(d->is * x_ps);
+  EVK_REQUIRE(xs.p, EVK_ERR_CUDA, "gconv: scratch allocation for the stride phases failed");
+  const int blocks = min(cdiv(d->is * x_ps / 4, 256), kNumSMs * 32);          // grid-stride, a few waves of the SMs
+  phase_split_kernel<<<blocks, 256, 0, st>>>(d->x, d->ldx, d->x_sb, xs.p, x_ps, d->Z, d->Tin, d->P, d->C, d->is, Jp);
+  return check_launch("phase_split");
+}
+
+// evk_gconv_fwd's route 1 for a tileable launch; returns 1 when it does not apply.  All of its rule (here and in gemm_tma_plan:
+// H == 1, no in_len, C % 4 == 0, C, N >= 32, J*P >= 64) is checked before the input is split.
+int gemm_tma_phased(const evk_gconv_desc* d, cudaStream_t st) {
+  const int s = d->is, C = d->C;
+  if (s < 2 || s > 4 || d->no_phase_split || (long long)d->Z * d->J * d->P < 2048) return 1;
+  evk_gconv_desc e = *d;                                  // the stride-1 tap sum over the phase copies (x set after the split)
+  e.ldx = C; e.Tin = cdiv(d->Tin, s); e.x_sb = (long long)e.Tin * d->P * C; e.is = 1;
+  int src[EVK_MAX_TAPS];
+  for (int q = 0; q < d->Q; ++q) phase_of(d->off[q], s, src[q], e.off[q]);
+  Operands o; GemmP p;
+  if (gemm_tma_plan(&e, s, (long long)d->Z * e.x_sb, src, o, p)) return 1;
+  Scratch xs(0, st);
+  long long x_ps;
+  if (int rc = split_phases(d, xs, x_ps, st)) return rc;
+  o.A = xs.p;
   return run_gemm(o, p, 1, st);
 }
 
-int gemm_tma_try(const evk_gconv_desc* d, cudaStream_t st) { return gemm_tma_run(d, 1, 0, nullptr, st); }
+// Conv weight gradient on conv_wgrad_kernel (evk_gconv_wgrad's route 1):
+//   dW[q][n][c] += sum_b sum_pos dY[b][pos][n] * X[b][pos + off[q]*P][c]
+// X is read channels-last as the forward left it (the tap shift is a TMA row coordinate; out-of-range rows = the conv
+// padding, zero-filled by the copy engine), dY through dyt [B][N][ld_dyt], its transpose.  The tile rows are (tap, input
+// channel) pairs, so the taps of a narrow layer share each staged dY block.  A strided conv is first split into `stride`
+// phase copies of X (as in the forward): the taps of one phase form a stride-1 problem on that copy.
+int conv_wgrad_tma(const evk_gconv_desc* d, const float* dyt, int ld_dyt, cudaStream_t st) {
+  const int s = d->is, B = d->Z, P = d->P, C = d->C, N = d->N, out_rows = d->J * P;
+  const long long dy_sb = (long long)N * ld_dyt;
+  EVK_REQUIRE((ld_dyt % 4) == 0 && ld_dyt >= out_rows && ((uintptr_t)dyt & 15) == 0, EVK_ERR_ARG,
+              "gconv_wgrad: dyt must be 16-byte aligned with a pitch >= J*P that is a multiple of 4 floats");
+  const float* x = d->x;
+  int ldx = d->ldx, in_rows = d->Tin * P;
+  long long x_sb = d->x_sb, x_ps = 0;
+  Scratch xs(0, st);
+  if (s > 1) {
+    if (int rc = split_phases(d, xs, x_ps, st)) return rc;
+    x = xs.p; ldx = C; in_rows = cdiv(d->Tin, s) * P; x_sb = (long long)in_rows * C;
+  }
+  for (int rho = 0; rho < s; ++rho) {
+    WgradP p{};
+    int qs[EVK_MAX_TAPS], nq = 0;
+    for (int q = 0; q < d->Q; ++q) {
+      int copy, shift;
+      phase_of(d->off[q], s, copy, shift);
+      if (copy == rho) { qs[nq] = q; p.off[nq++] = shift; }
+    }
+    if (!nq) continue;
+    CUtensorMap mx;
+    EVK_REQUIRE(make_map(&mx, x + rho * x_ps, B, x_sb, in_rows, C, ldx, BK), EVK_ERR_UNSUPPORTED,
+                "gconv_wgrad: cuTensorMapEncodeTiled unavailable or rejected the operand");
+    p.d = d->w + qs[0] * d->w_sq; p.ldd = d->ldw; p.d_sq = (nq > 1 ? qs[1] - qs[0] : 1) * d->w_sq;
+    p.N = N; p.C = C; p.Cp = cdiv(C, 32) * 32; p.nq = nq; p.P = P;
+    // the split count fixes how the K sums are grouped, and so the bits of dW: it depends on the layer shape (taps x 128 x
+    // 128 channel blocks), not on the kernel's tiling, so a change of tiling leaves the trained weights bit for bit as they were
+    const int tiles = nq * cdiv(N, 128) * cdiv(C, 128), kblocks = B * cdiv(out_rows, 32);
+    const int splits = max(1, min(64, min(sm_count() / tiles, kblocks / 8)));
+    int rc;
+    if (N > 64) rc = launch_wgrad<128>(mx, dyt, ld_dyt, dy_sb, B, out_rows, p, splits, st);
+    else if (N > 32) rc = launch_wgrad<64>(mx, dyt, ld_dyt, dy_sb, B, out_rows, p, splits, st);
+    else rc = launch_wgrad<32>(mx, dyt, ld_dyt, dy_sb, B, out_rows, p, splits, st);
+    EVK_REQUIRE(rc != 1, EVK_ERR_UNSUPPORTED, "gconv_wgrad: cuTensorMapEncodeTiled unavailable or rejected the operand");
+    if (rc) return rc;
+    g_disp_flops[4] += 2.0 * B * (double)out_rows * N * C * nq;
+  }
+  return EVK_OK;
+}
 
 }  // namespace evk
 
@@ -820,18 +926,6 @@ extern "C" int evk_set_backend_tma(int32_t on) { g_backend_tma = on ? 1 : 0; ret
 extern "C" int evk_set_tma_options(int32_t slab, int32_t mt2, float trunc_comp) {
   g_opt_slab = slab ? 1 : 0; g_opt_mt2 = mt2 ? 1 : 0; g_trunc_comp = trunc_comp;
   return EVK_OK;
-}
-
-// Strided convolution forward on the TMA/wgmma kernel.  d describes the conv as a STRIDE-1 tap sum over `phases` (= the
-// conv stride, <= 4) phase copies of the input produced by evk_phase_split: d->x = copy 0, copies x_ps floats apart, each
-// [Z][Tin * P][ldx] with d->Tin = ceil(T / stride); tap q reads copy src[q] at row shift off[q] (src, d->off: host arrays).
-// Returns EVK_ERR_UNSUPPORTED when the launch is not eligible (caller keeps the strided mma.sync kernel).
-extern "C" int evk_gconv_fwd_phased(const evk_gconv_desc* d, int32_t phases, int64_t x_ps, const int32_t* src, cudaStream_t st) {
-  EVK_REQUIRE(d && src, EVK_ERR_ARG, "gconv_fwd_phased: null argument");
-  int rc = gemm_tma_run(d, phases, x_ps, src, st);
-  EVK_REQUIRE(rc != 1, EVK_ERR_UNSUPPORTED, "gconv_fwd_phased: launch not eligible for the TMA kernel");
-  if (rc == 0) g_disp_flops[0] += desc_flops(d);
-  return rc;
 }
 
 extern "C" int evk_gemm_tf32(const float* A, int32_t lda, const float* B, int32_t ldb, float* D, int32_t ldd, int32_t M, int32_t N,
@@ -853,32 +947,3 @@ extern "C" int evk_gemm_tf32(const float* A, int32_t lda, const float* B, int32_
   return rc;
 }
 
-
-// Weight gradient of a stride-1 (dilated / period-folded) convolution on conv_wgrad_kernel:
-//   dW[q][n][c] += sum_b sum_pos dY[b][pos][n] * X[b][pos + off[q]*P][c]
-// x [B][in_rows][ldx] channels-last (batch pitch x_sb), read in place; dyt [B][N][ld_dy] = dY transposed (out_rows valid
-// positions per row, evk_dy_prep).  Out-of-range input rows (the conv padding) are zero-filled by the copy engine.
-// Accumulates into dW (pitch ldw, tap pitch w_sq): the K splits write partials that are added in split order.
-extern "C" int evk_conv_wgrad_tma(const float* x, int32_t ldx, int64_t x_sb, const float* dyt, int32_t ld_dy, int64_t dy_sb, float* dW,
-                                  int32_t ldw, int64_t w_sq, int32_t B, int32_t N, int32_t C, int32_t out_rows, int32_t in_rows,
-                                  int32_t Q, int32_t P, const int32_t* off, int32_t splits, cudaStream_t st) {
-  EVK_REQUIRE(B > 0 && N > 0 && C > 0 && out_rows > 0 && in_rows > 0 && Q > 0 && Q <= EVK_MAX_TAPS && P > 0 && off, EVK_ERR_ARG,
-              "conv_wgrad_tma: bad sizes");
-  EVK_REQUIRE((C % 4) == 0 && (ldx % 4) == 0 && (ld_dy % 4) == 0 && (x_sb % 4) == 0 && (dy_sb % 4) == 0 &&
-                  ((((uintptr_t)x) | ((uintptr_t)dyt)) & 15) == 0,
-              EVK_ERR_ARG, "conv_wgrad_tma: operands must be 16-byte aligned with pitches that are multiples of 4 floats");
-  CUtensorMap mx;
-  int rc = make_map(&mx, x, B, x_sb, in_rows, C, ldx, BK) ? 0 : 1;
-  if (rc == 0) {
-    WgradP p{};
-    p.d = dW; p.ldd = ldw; p.d_sq = w_sq; p.N = N; p.C = C; p.Cp = cdiv(C, 32) * 32; p.nq = Q; p.P = P;
-    for (int i = 0; i < EVK_MAX_TAPS; ++i) p.off[i] = i < Q ? off[i] : 0;
-    const int s = splits < 1 ? 1 : splits;
-    if (N > 64) rc = launch_wgrad<128>(mx, dyt, ld_dy, dy_sb, B, out_rows, p, s, st);
-    else if (N > 32) rc = launch_wgrad<64>(mx, dyt, ld_dy, dy_sb, B, out_rows, p, s, st);
-    else rc = launch_wgrad<32>(mx, dyt, ld_dy, dy_sb, B, out_rows, p, s, st);
-  }
-  EVK_REQUIRE(rc != 1, EVK_ERR_UNSUPPORTED, "conv_wgrad_tma: cuTensorMapEncodeTiled unavailable or rejected the operand");
-  if (rc == 0) g_disp_flops[4] += 2.0 * B * (double)out_rows * N * C * Q;
-  return rc;
-}

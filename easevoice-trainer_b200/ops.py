@@ -216,10 +216,12 @@ def _desc(off=(), **kw):
 
 
 def _run_desc(fn, d):
+    """one descriptor launch; evk_gconv_wgrad also gets the transposed dY attached as d.dyt / d.ld_dyt (not C fields)"""
     global _launches
     _launches += 1
     flops = 2.0 * d.Z * d.J * d.P * d.N * (d.C // max(d.G, 1)) * d.Q
-    _timed(fn, lambda: L.check(getattr(_lib(), fn)(ctypes.byref(d), _st())), flops,
+    args = (getattr(d, "dyt", None), getattr(d, "ld_dyt", 0)) if fn == "evk_gconv_wgrad" else ()
+    _timed(fn, lambda: L.check(getattr(_lib(), fn)(ctypes.byref(d), *args, _st())), flops,
            tag=(f"Z{d.Z} J{d.J} P{d.P} C{d.C} N{d.N} Q{d.Q} s{d.is_}" if PROF_SHAPES else None))
 
 
@@ -459,24 +461,22 @@ def _conv_out_len(Tin, Q, stride, pad, dil):
 
 
 def _fwd_like(x, Tin, w, wq0, wqstep, nq, ldw, w_sq, C, N, y, *, J, P, is_, os_, o0, Tout, off, bias=None, res=None,
-              act=0, slope=0.0, in_len=None, out_len=None, H=1, x_sh=0, w_sh=0, y_sh=0, b_sh=0, drop=None):
-    """one launch of the generalised conv on the tensor-core kernel.  Grouped convs pass H = groups with the per-group
-    channel offsets x_sh / w_sh / y_sh / b_sh (C, N are then per-group sizes)."""
+              act=0, slope=0.0, in_len=None, out_len=None, G=1, H=1, x_sh=0, w_sh=0, y_sh=0, drop=None, no_phase_split=0):
+    """one forward-like launch of the generalised conv; evk_gconv_fwd picks the kernel.  Grouped convs pass G = groups
+    (C, N are then the total channel counts).  H > 1 runs an inner batch with the per-item offsets x_sh / w_sh / y_sh (the
+    grouped data gradient, whose PB operand is not in the [Q][N][C/G] layout that G describes)."""
     B = x.shape[0]
     _, _, ldx = _rows(x)
     _, _, ldy = _rows(y)
     ldr = _rows(res)[2] if res is not None else 0
-    wbase = w.data_ptr() + 4 * wq0 * w_sq
-    d = _desc(x=x, w=wbase, y=y, res=res, bias=bias, in_len=in_len, out_len=out_len,
+    d = _desc(x=x, w=w.data_ptr() + 4 * wq0 * w_sq, y=y, res=res, bias=bias, in_len=in_len, out_len=out_len,
               x_sb=Tin * P * ldx, x_sh=x_sh, w_sh=w_sh, w_sq=wqstep * w_sq, y_sb=Tout * P * ldy, y_sh=y_sh,
-              r_sb=Tout * P * ldr, r_sh=y_sh, ldx=ldx, ldw=ldw, ldy=ldy, ldr=ldr, b_sh=b_sh, Z=B * H, H=H, C=C, N=N, Q=nq,
-              Tin=Tin, J=J, P=P, is_=is_, os_=os_, o0=o0, Tout=Tout, act=act, slope=float(slope), off=off)
+              r_sb=Tout * P * ldr, r_sh=y_sh, ldx=ldx, ldw=ldw, ldy=ldy, ldr=ldr, Z=B * H, H=H, G=G, C=C, N=N, Q=nq,
+              Tin=Tin, J=J, P=P, is_=is_, os_=os_, o0=o0, Tout=Tout, act=act, slope=float(slope), off=off,
+              no_phase_split=no_phase_split)
     if drop is not None:                      # fused dropout after the activation (TMA kernel epilogue only; the library rejects other routes)
         d.drop_rng, d.drop_sid, d.drop_p = rng_state(x.device).data_ptr(), int(drop[1]), float(drop[0])
-    mma = _aligned(x, ldx) and ldw % 4 == 0 and (wbase % 16 == 0) and (d.w_sq % 4 == 0) and x_sh % 4 == 0 and w_sh % 4 == 0
-    if not mma:
-        assert H == 1, "grouped convs need 16-byte aligned group slices"
-    _run_desc("evk_gconv_fwd" if mma else "evk_conv_direct_fwd", d)
+    _run_desc("evk_gconv_fwd", d)
 
 
 def _dgrad_phases(dy, Jy, pb, ldb, C, N, Q, dx, Tin, P, stride, pad, dil, H=1):
@@ -486,15 +486,6 @@ def _dgrad_phases(dy, Jy, pb, ldb, C, N, Q, dx, Tin, P, stride, pad, dil, H=1):
     for u0, Ju, q0, nq, off in dgrad_phase_plan(Q, stride, pad, dil, Tin):
         _fwd_like(dy, Jy, pb, q0, stride, nq, ldb, w_sq, N, C, dx, J=Ju, P=P, is_=1, os_=stride, o0=u0, Tout=Tin, off=off,
                   H=H, x_sh=N if H > 1 else 0, w_sh=N if H > 1 else 0, y_sh=C if H > 1 else 0)
-
-
-def _phase_split(x, ldx, B, Tin, P, C, stride):
-    """-> (xs, Jp): the stride phase copies of x [B, Tin*P, C], xs[r][b][j*P + w] = x[b][(j*stride + r)*P + w] (zero past
-    the end), j < Jp = ceil(Tin / stride).  A strided conv is a stride-1 tap sum over them."""
-    Jp = (Tin + stride - 1) // stride
-    xs = torch.empty((stride, B, Jp * P, C), device=x.device, dtype=torch.float32)
-    _call("evk_phase_split", _p(x), ldx, Tin * P * ldx, _p(xs), B * Jp * P * C, B, Tin, P, C, stride, Jp)
-    return xs, Jp
 
 
 def dgrad_phase_plan(Q, stride, pad, dil, Tin):
@@ -533,31 +524,13 @@ class _ConvFn(torch.autograd.Function):
         assert R % P == 0
         Tin = R // P
         N, lda = pa.shape[1], pa.shape[2]
-        Cg, Ng = C // G, N // G
         J = _conv_out_len(Tin, Q, stride, pad, dil)
         y = torch.empty((B, J * P, N), device=x.device, dtype=torch.float32)
         if res is not None:
             res = _cl(res)
-        off = [q * dil - pad for q in range(Q)]
-        gk = dict(H=G, x_sh=Cg, w_sh=Ng * lda, y_sh=Ng, b_sh=Ng) if G > 1 else {}
-        _, _, ldx = _rows(x)
-        if (1 < stride <= 4 and G == 1 and in_len is None and C % 4 == 0 and C >= 32 and N >= 32 and lda % 4 == 0
-                and B * J * P >= 2048 and J * P >= 64 and _aligned(x, ldx) and not _lib().evk_get_precise()):
-            # strided conv = stride-1 tap sum over `stride` phase copies of the input (tap u = q*dil - pad reads phase u mod s
-            # at shift floor(u / s)): runs on the TMA/wgmma kernel instead of the strided mma.sync one
-            xs, Jp = _phase_split(x, ldx, B, Tin, P, C, stride)
-            ldr = _rows(res)[2] if res is not None else 0
-            d = _desc(x=xs, w=pa, y=y, res=res, bias=bias, out_len=out_len, x_sb=Jp * P * C, w_sq=N * lda, y_sb=J * P * N,
-                      r_sb=J * P * ldr, ldx=C, ldw=lda, ldy=N, ldr=ldr, Z=B, C=C, N=N, Q=Q, Tin=Jp, J=J, P=P, is_=1, os_=1,
-                      Tout=J, act=act, slope=float(slope), off=[u // stride for u in off])
-            srca = (ctypes.c_int32 * Q)(*[u % stride for u in off])
-            global _launches
-            _launches += 1
-            _timed("evk_gconv_fwd_phased", lambda: L.check(_lib().evk_gconv_fwd_phased(ctypes.byref(d), stride, B * Jp * P * C, srca, _st())),
-                   2.0 * B * J * P * N * C * Q)
-        else:
-            _fwd_like(x, Tin, pa, 0, 1, Q, lda, N * lda, Cg, Ng, y, J=J, P=P, is_=stride, os_=1, o0=0, Tout=J, off=off,
-                      bias=bias, res=res, act=act, slope=slope, in_len=in_len, out_len=out_len, drop=drop, **gk)
+        _fwd_like(x, Tin, pa, 0, 1, Q, lda, N * lda, C, N, y, J=J, P=P, is_=stride, os_=1, o0=0, Tout=J,
+                  off=[q * dil - pad for q in range(Q)], bias=bias, res=res, act=act, slope=slope, in_len=in_len, out_len=out_len,
+                  drop=drop, G=G)
         ctx.cfg = cfg
         ctx.dims = (B, Tin, C, N, J, lda)
         ctx.has = (bias is not None, res is not None)
@@ -577,11 +550,11 @@ class _ConvFn(torch.autograd.Function):
         Cg, Ng = C // G, N // G
         dy = dy.contiguous()
         Ro = J * P
-        _, _, ldx_ = _rows(x)
-        mma_w = _aligned(x, ldx_) and _aligned(dy, N) and (G == 1 or (Cg % 4 == 0 and Ng % 4 == 0))
-        tma_w = bool(ctx.needs_input_grad[1] and mma_w and 1 <= stride <= 4 and (stride == 1 or dil == 1) and G == 1
-                     and in_len is None and B * J * P >= 2048 and J * P >= 64 and C >= 32 and N >= 32 and C % 4 == 0
-                     and not _lib().evk_get_precise())
+        offs = [q * dil - pad for q in range(Q)]
+        _, _, ldx = _rows(x)
+        dw = _desc(x=x, y=dy, in_len=in_len, x_sb=Tin * P * ldx, w_sq=N * lda, y_sb=J * P * N, ldx=ldx, ldw=lda, ldy=N, Z=B, G=G,
+                   C=C, N=N, Q=Q, Tin=Tin, J=J, P=P, is_=stride, os_=1, Tout=J, off=offs)
+        tma_w = bool(ctx.needs_input_grad[1] and _lib().evk_gconv_wgrad_takes_dyt(ctypes.byref(dw)))
         want_b = has_bias and ctx.needs_input_grad[3]
         dyt = dbias = None
         if act or out_len is not None or tma_w or want_b:
@@ -590,13 +563,13 @@ class _ConvFn(torch.autograd.Function):
             dpre = torch.empty_like(dy) if need_pre else None
             ldo = (Ro + 31) // 32 * 32                                       # 128-byte aligned rows for the TMA boxes
             dyt = torch.empty((B, N, ldo), device=dy.device, dtype=torch.float32) if tma_w else None
+            dw.dyt, dw.ld_dyt = _p(dyt), ldo
             dbias = _zpool.take(N, dy.device) if want_b else None
             _call("evk_dy_prep", _p(dy), N, _p(y), N, act, ctypes.c_float(slope), ctypes.c_float(gscale), _p(out_len), P, _p(dpre), N, _p(dyt),
                   ldo, N * ldo, _p(dbias), B, Ro, N)
             if need_pre:
                 dy = dpre
         dx = dpa = dres = None
-        offs = [q * dil - pad for q in range(Q)]
         if ctx.needs_input_grad[0]:
             dx = torch.empty((B, Tin * P, C), device=dy.device, dtype=torch.float32)
             use_mma = (pb is not None and pb.numel() > 0 and _aligned(dy, N) and pb.shape[2] % 4 == 0
@@ -615,47 +588,8 @@ class _ConvFn(torch.autograd.Function):
                 dx = dxm
         if ctx.needs_input_grad[1]:
             dpa = dpa_buffer(pa)
-            ldx, mma = ldx_, mma_w
-            if tma_w:
-                # dW[q][n][c] = sum_{b,pos} dY[b][pos][n] X[b][pos + shift_q][c] on conv_wgrad_kernel: X is read channels-last
-                # as the forward left it (the tap shift is a TMA row coordinate; out-of-range rows = conv padding,
-                # zero-filled by the copy engine), dY through the transposed copy dyt that evk_dy_prep wrote above.  The
-                # tile rows are (tap, input channel) pairs, so the taps of a narrow layer share each staged dY block.
-                # A strided conv is first split into `stride` phase copies of X (as in the forward): taps u = q - pad with
-                # u mod stride == rho form a stride-1 problem on copy rho with shifts floor(u / stride).
-                if stride == 1:
-                    srcs = [(x, ldx, Tin, list(range(Q)), offs)]
-                else:
-                    xs, Jp = _phase_split(x, ldx, B, Tin, P, C, stride)
-                    srcs = []
-                    for rho in range(stride):
-                        qs = [q for q in range(Q) if offs[q] % stride == rho]
-                        if qs:
-                            srcs.append((xs[rho], C, Jp, qs, [offs[q] // stride for q in qs]))
-                for xsrc, ldsrc, Tsrc, qs, shifts in srcs:
-                    Ri = Tsrc * P
-                    nq = len(qs)
-                    qstep = (qs[1] - qs[0]) if nq > 1 else 1
-                    # the split count fixes how the K sums are grouped, and so the bits of dW: it is a function of the layer
-                    # shape (taps x 128 x 128 channel blocks), not of the kernel's tiling, so a change of tiling leaves
-                    # the trained weights bit for bit where they were
-                    tiles = nq * ((N + 127) // 128) * ((C + 127) // 128)
-                    kblocks = B * ((Ro + 31) // 32)
-                    sms = torch.cuda.get_device_properties(dy.device).multi_processor_count
-                    splits = max(1, min(64, sms // tiles, kblocks // 8))
-                    offa = (ctypes.c_int32 * nq)(*shifts)
-                    _call_f("evk_conv_wgrad_tma", 2.0 * B * Ro * N * C * nq, _p(xsrc), ldsrc, Ri * ldsrc, _p(dyt), ldo, N * ldo,
-                            dpa.data_ptr() + 4 * qs[0] * N * lda, lda, qstep * N * lda, B, N, C, Ro, Ri, nq, P, offa, splits,
-                            tag=f"B{B} Ro{Ro} P{P} C{C} N{N} nq{nq} splits{splits}")
-            else:
-                # the mma.sync kernel runs the groups as the inner batch (H = groups), the direct kernel takes G
-                if mma and G > 1:
-                    grp = dict(Z=B * G, H=G, C=Cg, N=Ng, x_sh=Cg, w_sh=Ng * lda, y_sh=Ng)
-                else:
-                    grp = dict(Z=B, C=C, N=N, G=G)
-                d = _desc(x=x, w=dpa, y=dy, in_len=in_len, x_sb=Tin * P * ldx, w_sq=N * lda, y_sb=J * P * N, ldx=ldx, ldw=lda,
-                          ldy=N, Q=Q, Tin=Tin, J=J, P=P, is_=stride, os_=1, Tout=J, off=offs, **grp)
-                _run_desc("evk_gconv_wgrad" if mma else "evk_conv_direct_wgrad", d)
+            dw.w, dw.y = dpa.data_ptr(), dy.data_ptr()
+            _run_desc("evk_gconv_wgrad", dw)
         if has_res and ctx.needs_input_grad[4]:
             dres = dy
         return dx, dpa, None, dbias, dres, None
@@ -759,15 +693,14 @@ class _ConvTFn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dx = torch.empty((B, Tin, Cin), device=dy.device, dtype=torch.float32)
             _fwd_like(dy, Tout, pa, 0, 1, Q, lda, Cin * lda, Cout, Cin, dx, J=Tin, P=1, is_=stride, os_=1, o0=0,
-                      Tout=Tin, off=off)
+                      Tout=Tin, off=off, no_phase_split=1)
         if ctx.needs_input_grad[1]:
             dpa = dpa_buffer(pa)
             _, _, ldx = _rows(x)
             # dPA[q][ci][co] += sum_t X[t][ci] * dY[t*stride - pad + q][co]: "x" role = dY (shifted), "y" role = X
             d = _desc(x=dy, w=dpa, y=x, x_sb=Tout * Cout, w_sq=Cin * lda, y_sb=Tin * ldx, ldx=Cout, ldw=lda, ldy=ldx, Z=B,
                       C=Cout, N=Cin, Q=Q, Tin=Tout, J=Tin, P=1, is_=stride, os_=1, Tout=Tin, off=off)
-            mma = _aligned(dy, Cout) and _aligned(x, ldx)
-            _run_desc("evk_gconv_wgrad" if mma else "evk_conv_direct_wgrad", d)
+            _run_desc("evk_gconv_wgrad", d)
         if ctx.needs_input_grad[3]:
             dbias = torch.empty(Cout, device=dy.device, dtype=torch.float32)
             _call("evk_colsum", _p(dy), B * Tout, Cout, Cout, _p(dbias), 0)

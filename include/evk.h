@@ -53,9 +53,9 @@ typedef struct evk_gconv_desc {
   const int32_t* in_len; const int32_t* out_len;
   int64_t x_sb, x_sh, w_sb, w_sh, w_sq, y_sb, y_sh, r_sb, r_sh;
   int32_t ldx, ldw, ldy, ldr;
-  int32_t b_sh;          /* bias offset per inner-batch index h (grouped convs run as H = groups) */
+  int32_t b_sh;          /* bias offset per inner-batch index h */
   int32_t Z, H;          /* batch count and inner (head) count: b = z / H, h = z % H */
-  int32_t C, N, Q, G;    /* in-channels, out-channels, taps, groups (G>1: direct kernels only) */
+  int32_t C, N, Q, G;    /* in-channels, out-channels, taps, groups (G > 1: W is [Q][N][C/G]) */
   int32_t Tin, J, P;     /* input positions per batch, output positions computed, inner width */
   int32_t is, os, o0;    /* input stride, output stride, output origin (in positions) */
   int32_t Tout;          /* output positions per batch (bounds for (o0 + j*os)) */
@@ -64,15 +64,25 @@ typedef struct evk_gconv_desc {
   /* optional fused dropout AFTER the activation (forward launches taken by gemm_tma_kernel only; any other route returns
    * EVK_ERR_UNSUPPORTED): y = dropout_p(act(...)); rng = device [seed, offset] (the library's RNG state), sid = stream id. */
   const uint64_t* drop_rng; uint64_t drop_sid; float drop_p;
+  /* 1: not route 1 of evk_gconv_fwd.  ConvTranspose1d's data gradient, which has always run on gconv_f_kernel: route 1
+   * would take it for the HiFi-GAN generator's stride-2 upsampling layers (128 -> 64, 64 -> 32) and change their bits. */
+  int32_t no_phase_split;
 } evk_gconv_desc;
 
+/* Any stride and alignment; groups as G.  Routes, the first that takes the launch runs it:
+ *   1. 1 < is <= 4, no_phase_split == 0, G <= 1, H == 1, no in_len, C % 4 == 0, C, N >= 32, Z*J*P >= 2048, J*P >= 64:
+ *      x split into `is` phase copies (library scratch), then a stride-1 tap sum over them on gemm_tma_kernel;
+ *   2. stride 1 on gemm_tma_kernel (shape rule in gemm_tma_plan);  3. stride 1 on gconv_tc_kernel;  4. gconv_f_kernel;
+ *   5. the direct kernel when X or W is not 16-byte tileable (x, w 16-byte aligned, ldx, ldw and strides multiples of 4).
+ * Routes 2-4 run groups as the inner batch.  Precise mode skips 1-3, evk_set_backend(0) 2-3, evk_set_backend_tma(0) 1-2.
+ * Fused dropout (drop_p > 0) needs route 1 or 2.  Route 1 checks all of gemm_tma_kernel's conditions before it splits x. */
 int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream);
 int evk_gconv_desc_size(void);         /* sizeof(evk_gconv_desc) as compiled: bindings check their mirror against it */
 /* 0 (default): one TF32 product per MAC.  1: 3xTF32 error-compensated products (~fp32 accuracy, 3x tensor work);
  * the parity tests use it to separate indexing errors from TF32 operand rounding. Process-wide. */
 int evk_set_precise(int32_t on);
 int evk_get_precise(void);
-/* 1 (default): eligible launches run on the wgmma kernels (gemm_tma.cu, gconv_tc.cu); 0: mma.sync kernels only. */
+/* 1 (default): eligible stride-1 launches run on the wgmma kernels (gemm_tma.cu, gconv_tc.cu); 0: on mma.sync. */
 int evk_set_backend(int32_t tensor_core);
 /* Dispatch accounting: algorithmic flops enqueued since the last reset, per kernel family (host-side counters; graph
  * replays add nothing).  out[i], i < EVK_DISPATCH_SLOTS:
@@ -89,14 +99,19 @@ int evk_dispatch_stats(double* out, int32_t n);
 int evk_dispatch_stats_reset(void);
 /* Weight gradient of the same operator:  W[z][q][n][c] += sum_{j,w} Yg[z][orow][n] * X[z][irow][c]
  * (d->y is read as the output gradient, d->w is accumulated -- partial sums added in a fixed order, so the result is
- * reproducible; when w_sb == w_sh == 0 the
- * sum also runs over z).  Replaces autograd's conv weight-gradient kernels for the call sites above. */
-int evk_gconv_wgrad(const evk_gconv_desc* d, evk_stream_t stream);
-/* Direct (CUDA-core) variants for skinny layers: C/G < 8 (1-channel inputs, grouped k=41 convs of
+ * reproducible; when w_sb == w_sh == 0 the sum also runs over z).  Replaces autograd's conv weight-gradient kernels for the
+ * call sites above.  dyt (nullable) [Z][N][ld_dyt] = Yg transposed (evk_dy_prep).  Routes:
+ *   1. dyt given and evk_gconv_wgrad_takes_dyt: conv_wgrad_kernel, per stride phase's taps on phase copies of X (scratch),
+ *      K split in max(1, min(64, SMs / tiles, Z * ceil(J*P / 32) / 8)), tiles = taps * ceil(N / 128) * ceil(C / 128);
+ *   2. gconv_w_kernel, groups as the inner batch;  3. the direct kernel when X or Yg is not 16-byte tileable. */
+int evk_gconv_wgrad(const evk_gconv_desc* d, const float* dyt, int32_t ld_dyt, evk_stream_t stream);
+/* 1 when evk_gconv_wgrad takes route 1 given dyt (callers ask evk_dy_prep for dyt only then): is <= 4 (taps at consecutive
+ * offsets when strided: any dilation when Q == 1), G <= 1, H == 1, os == 1, o0 == 0, w_sb == 0, no in_len, C % 4 == 0,
+ * C, N >= 32, Z*J*P >= 2048, J*P >= 64, X and Yg 16-byte tileable, not precise. */
+int evk_gconv_wgrad_takes_dyt(const evk_gconv_desc* d);
+/* Direct (CUDA-core) data gradient for skinny layers: C/G < 8 (1-channel inputs, grouped k=41 convs of
  * DiscriminatorS, models.py:563-575).  Same descriptor; W is [Q][N][C/G]. */
-int evk_conv_direct_fwd(const evk_gconv_desc* d, evk_stream_t stream);
 int evk_conv_direct_dgrad(const evk_gconv_desc* d, evk_stream_t stream);  /* d->x is WRITTEN (dX), d->y read */
-int evk_conv_direct_wgrad(const evk_gconv_desc* d, evk_stream_t stream);
 
 /* out[n] (+)= sum_rows x[row][n]  -- bias gradients */
 int evk_colsum(const float* x, int64_t rows, int32_t n, int32_t ld, float* out, int32_t accumulate, evk_stream_t stream);
@@ -349,17 +364,8 @@ int evk_gemm_tf32(const float* A, int32_t lda, const float* B, int32_t ldb, floa
                   int32_t K, const float* bias, const float* res, int32_t ldr, int32_t act, float slope, int32_t splits,
                   evk_stream_t stream);
 int evk_set_backend_tma(int32_t on);
-/* Weight gradient of a stride-1 (dilated, period-folded) conv on the TMA/wgmma path (conv_wgrad_kernel):
- *   dW[q][n][c] += sum_b sum_pos dY[b][pos][n] * X[b][pos + off[q]*P][c]
- * x [B][in_rows][ldx] channels-last (batch pitch x_sb, C % 4 == 0), read in place; dyt [B][N][ld_dy] = dY transposed
- * (out_rows = J*P valid positions per row, evk_dy_prep).  Taps are stacked with the input channels in the tile rows, so the
- * taps of a narrow layer share every staged dY block.  Rows outside the input (the conv padding) are zero-filled by the copy
- * engine.  Accumulates the K splits' partials, added in split order, into dW (pitch ldw, tap pitch w_sq); off is a HOST array. */
-int evk_conv_wgrad_tma(const float* x, int32_t ldx, int64_t x_sb, const float* dyt, int32_t ld_dy, int64_t dy_sb, float* dW,
-                       int32_t ldw, int64_t w_sq, int32_t B, int32_t N, int32_t C, int32_t out_rows, int32_t in_rows,
-                       int32_t Q, int32_t P, const int32_t* off, int32_t splits, evk_stream_t stream);
 /* Everything a conv's backward needs from its output gradient in one pass (elementwise.cu): g = dy * act'(y) * (t < len*P);
- * dpre (nullable) = g in the layout of dy; dyt (nullable) [B][C][ldt] = g transposed (the K-major operand of evk_conv_wgrad_tma);
+ * dpre (nullable) = g in the layout of dy; dyt (nullable) [B][C][ldt] = g transposed (the K-major operand of evk_gconv_wgrad);
  * dbias (nullable, [C], zero-initialised by the caller) += column sums of g.  act: evk_act of the forward epilogue, yact = its
  * OUTPUT (derivatives are taken from the output: leaky-ReLU / ReLU by sign, tanh by 1 - y^2). */
 int evk_dy_prep(const float* dy, int32_t lddy, const float* yact, int32_t ldy, int32_t act, float slope, float gscale, const int32_t* len,
@@ -367,14 +373,6 @@ int evk_dy_prep(const float* dy, int32_t lddy, const float* yact, int32_t ldy, i
                 evk_stream_t stream);
 /* gscale multiplies g: 1/(1-p) when the forward epilogue applied dropout after a ReLU -- the saved OUTPUT is then zero exactly
  * where the element was dropped or the ReLU was off, so no mask needs to be regenerated. */
-/* Strided conv forward on the same kernel: the input is first split into `stride` phase copies
- *   xs[rho][b][j*P + w][c] = x[b][(j*stride + rho)*P + w][c]   (zero for j*stride + rho >= T; j < Jp = ceil(T / stride))
- * and the conv becomes a stride-1 tap sum in which tap q (u = q*dil - pad) reads copy src[q] = u mod stride at row shift
- * off[q] = floor(u / stride).  d describes that stride-1 form (d->x = copy 0, d->Tin = Jp, d->is = 1, d->off = shifts);
- * copies are x_ps floats apart; src is a HOST array.  Returns EVK_ERR_UNSUPPORTED if the launch is not eligible. */
-int evk_phase_split(const float* x, int32_t ldx, int64_t x_sb, float* xs, int64_t xs_ps, int32_t B, int32_t T, int32_t P,
-                    int32_t C, int32_t stride, int32_t Jp, evk_stream_t stream);
-int evk_gconv_fwd_phased(const evk_gconv_desc* d, int32_t phases, int64_t x_ps, const int32_t* src, evk_stream_t stream);
 /* [B][T][ldx] (C valid, batch pitch x_sb) -> [B][C][ldy] (T + shift valid, batch pitch y_sb):
  * y[b][c][u] = x[b][u - shift][c], zero for u < shift. */
 int evk_transpose_rows(const float* x, int32_t ldx, int64_t x_sb, float* y, int32_t ldy, int64_t y_sb, int32_t B, int32_t T,

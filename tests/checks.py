@@ -88,7 +88,7 @@ def check_conv():
         ("TMA conv_pre k7 192->512", 5, 500, 192, 512, 7, 1, 3, 1, 1, 1, 0, False, False),
         ("TMA discP 512->1024 k5 s1 p=3", 3, 310, 512, 1024, 5, 1, 2, 1, 3, 1, 1, False, False),
         ("TMA k3 32->96 (C tail zero-fill)", 2, 1100, 36, 96, 3, 1, 1, 1, 1, 1, 0, False, False),
-        # strided forwards through evk_phase_split + the multi-source tap sum; dgrad phases use the os/o0 output mapping
+        # strided forwards through the phase split + the multi-source tap sum; dgrad phases use the os/o0 output mapping
         ("TMA discP 128->512 k5 s3 p=2 (phased)", 4, 1000, 128, 512, 5, 3, 2, 1, 2, 1, 1, False, False),
         ("TMA discP 32->128 k5 s3 p=5 (phased)", 3, 410, 32, 128, 5, 3, 2, 1, 5, 1, 0, False, False),
         ("TMA ssl_proj k2 s2 768->768 (phased)", 6, 700, 768, 768, 2, 2, 0, 1, 1, 1, 0, False, False),

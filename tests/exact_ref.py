@@ -83,7 +83,8 @@ LINEAR_CASES = [(1, 512, 64, 64, "brr"), (3, 171, 68, 96, "lrelu"), (1, 4097, 51
 
 # Conv cases through ops.conv: name, B, Tin, C, N, Q, stride, pad, dil, P, groups, act, res, masks ("" / "out" / "inout"),
 # forward family, data-gradient family (None: not asserted; "-": no backward, e.g. tanh), weight-gradient family,
-# TMA options (slab, mt2).
+# TMA options (slab, mt2) and optionally a mode: "x+1" (x starts one float into its rows: not 16-byte aligned) or
+# "precise" (3xTF32 products, evk_set_precise).
 CONV_CASES = [
     # the "TMA ..." shapes of tests/checks.py check_conv (the s3 p=2 one at Tin = 1000: at 341 it is below the phased
     # path's 2048-row threshold and runs on mma.sync)
@@ -127,6 +128,21 @@ CONV_CASES = [
     # direct fp32 kernels: channel counts that are not multiples of 4
     ("direct C=6 k5", 2, 300, 6, 32, 5, 1, 2, 1, 1, 1, ACT_LRELU, False, "", "fwd_direct", None, "wgrad_direct", (1, 1)),
     ("direct C=2 k5 s3 P=5", 2, 200, 2, 32, 5, 3, 2, 1, 5, 1, ACT_LRELU, False, "", "fwd_direct", None, "wgrad_direct", (1, 1)),
+    # the routing rules on both sides of each threshold: phase-split TMA forward and TMA weight gradient for strided convs
+    # (B*J*P >= 2048, J*P >= 64, C >= 32, N >= 32, stride <= 4, 16-byte x, no in_len, not precise), grouped convs
+    ("route B*J*P 2047 s2", 1, 4093, 32, 32, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "", "fwd_mma_sync", None, "wgrad_mma_sync", (1, 1)),
+    ("route B*J*P 2048 s2", 1, 4095, 32, 32, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "", "fwd_gemm_tma", None, "wgrad_gemm_tma", (1, 1)),
+    ("route J*P 63 s2", 33, 125, 32, 32, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "", "fwd_mma_sync", None, "wgrad_mma_sync", (1, 1)),
+    ("route J*P 64 s2", 32, 127, 32, 32, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "", "fwd_gemm_tma", None, "wgrad_gemm_tma", (1, 1)),
+    ("route C 28 s2", 1, 4095, 28, 32, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "", "fwd_mma_sync", None, "wgrad_mma_sync", (1, 1)),
+    ("route N 28 s2", 1, 4095, 32, 28, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "", "fwd_mma_sync", None, "wgrad_mma_sync", (1, 1)),
+    ("route stride 5", 3, 4000, 32, 32, 5, 5, 2, 1, 1, 1, ACT_NONE, False, "", "fwd_mma_sync", None, "wgrad_mma_sync", (1, 1)),
+    ("route x+1 s2", 1, 4095, 32, 32, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "", "fwd_direct", None, "wgrad_direct", (1, 1, "x+1")),
+    ("route in_len s2", 1, 4095, 32, 32, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "inout", "fwd_mma_sync", None, "wgrad_mma_sync", (1, 1)),
+    ("route precise s2", 1, 4095, 32, 32, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "", "fwd_mma_sync", None, "wgrad_mma_sync", (1, 1, "precise")),
+    ("route grouped g2 8->6 Ng 3", 2, 300, 8, 6, 5, 1, 2, 1, 1, 2, ACT_NONE, False, "", "fwd_gconv_tc", None, "wgrad_direct", (1, 1)),
+    # group slices that are not 16-byte tileable (C / G = 3): the direct kernels take the grouped conv as G
+    ("route grouped g2 6->8 Cg 3", 2, 300, 6, 8, 5, 1, 2, 1, 1, 2, ACT_LRELU, False, "", "fwd_direct", "fwd_direct", "wgrad_direct", (1, 1)),
 ]
 # conv_post: 16 -> 1 channel carried as 4 (zero weight rows), tanh: B, Tin, C, Q, pad
 CONV_POST = (2, 700, 16, 7, 3)

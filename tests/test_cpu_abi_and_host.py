@@ -25,12 +25,45 @@ def test_library_exports_every_symbol_declared_in_header():
 
 def test_descriptor_struct_layout():
     from easevoice_trainer_b200 import lib
-    # 7 pointers + 9 int64 + 19 int32 + float + int32[48] + (pointer, uint64, float) of the fused-dropout request, padded to 8 bytes
-    expect = 7 * 8 + 9 * 8 + 19 * 4 + 4 + 48 * 4 + 8 + 8 + 4
+    # 7 pointers + 9 int64 + 19 int32 + float + int32[48] + (pointer, uint64, float) of the fused-dropout request + int32
+    # no_phase_split, padded to 8 bytes
+    expect = 7 * 8 + 9 * 8 + 19 * 4 + 4 + 48 * 4 + 8 + 8 + 4 + 4
     assert ctypes.sizeof(lib.GconvDesc) == (expect + 7) // 8 * 8
     assert lib.GconvDesc.off.offset == 7 * 8 + 9 * 8 + 19 * 4 + 4
     assert lib.GconvDesc.drop_rng.offset == 400 and lib.GconvDesc.drop_sid.offset == 408 and lib.GconvDesc.drop_p.offset == 416
+    assert lib.GconvDesc.no_phase_split.offset == 420                                 # fills the tail padding: the size is unchanged
     assert lib.load().evk_gconv_desc_size() == ctypes.sizeof(lib.GconvDesc)          # the compiled header agrees with the ctypes mirror
+
+
+def test_run_desc_hook_keeps_the_transposed_dy(monkeypatch):
+    """Timing hooks (bench.py --config 5) wrap ops._run_desc(fn, d) with two arguments: the weight gradient's transposed dY
+    travels on the descriptor, so a wrapped launch still reaches evk_gconv_wgrad with it."""
+    from easevoice_trainer_b200 import ops
+    seen = []
+
+    class FakeLib:
+        def evk_gconv_wgrad(self, d, dyt, ld_dyt, stream):
+            seen.append((dyt, ld_dyt))
+            return 0
+
+        def evk_gconv_fwd(self, d, stream):
+            seen.append(())
+            return 0
+
+    monkeypatch.setattr(ops, "_lib", FakeLib)
+    monkeypatch.setattr(ops, "_st", lambda: None)
+    orig = ops._run_desc
+
+    def hook(fn, d):
+        orig(fn, d)
+
+    d = ops._desc(Z=1, C=4, N=4, Q=1, J=1, P=1)
+    d.dyt, d.ld_dyt = ctypes.c_void_p(4096), 32
+    hook("evk_gconv_wgrad", d)
+    hook("evk_gconv_wgrad", ops._desc(Z=1, C=4, N=4, Q=1, J=1, P=1))
+    hook("evk_gconv_fwd", d)
+    assert seen[0][0].value == 4096 and seen[0][1] == 32
+    assert seen[1] == (None, 0) and seen[2] == ()
 
 
 def test_pack_job_struct_layout():

@@ -67,7 +67,7 @@ def test_case_tables_reach_their_paths():
     for name, B, Tin, C, N, Q, stride, pad, dil, P, G, act, res, masks, ffam, dfam, wfam, opts in R.CONV_CASES:
         J = R.conv_out_len(Tin, Q, stride, pad, dil)
         assert J > 0, name
-        if wfam == "wgrad_gemm_tma":                 # ops.conv's TMA weight-gradient eligibility
+        if wfam == "wgrad_gemm_tma":                 # the library's TMA weight-gradient eligibility
             assert B * J * P >= 2048 and J * P >= 64 and C >= 32 and N >= 32 and C % 4 == 0 and G == 1 and not masks.startswith("in"), name
         if ffam == "fwd_gemm_tma" and stride > 1:    # the phased strided forward
             assert B * J * P >= 2048 and J * P >= 64 and C % 4 == 0 and C >= 32 and N >= 32, name

@@ -1,4 +1,4 @@
-"""Conv weight gradients on conv_wgrad_kernel (evk_conv_wgrad_tma), element for element against float64.
+"""Conv weight gradients on conv_wgrad_kernel (evk_gconv_wgrad given dY transposed), element for element against float64.
 
 The kernel stacks (tap, input channel) pairs in its tile rows and reads X channels-last with the tap shift as a copy-engine
 row coordinate.  With small-integer operands every product and partial sum is exact in fp32 (tests/exact_ref.py), so with
@@ -49,7 +49,7 @@ def _to_cl(t):
 
 
 def _splits(B, J, P, C, N, stride, Q):
-    """the split count ops.conv picks for the largest stride phase (mirrors _ConvFn.backward)"""
+    """the split count evk_gconv_wgrad picks for the largest stride phase"""
     nq = (Q + stride - 1) // stride
     tiles = nq * ((N + 127) // 128) * ((C + 127) // 128)
     sms = torch.cuda.get_device_properties(DEV).multi_processor_count

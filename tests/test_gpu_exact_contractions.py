@@ -5,7 +5,7 @@ truncation compensation off each kernel must reproduce the float64 result exactl
 predicate, a dropped K block or split, a tap shift into the wrong residue copy or a misplaced float4 of the epilogue
 changes an output by a whole unit.  A whole-tensor relative-L2 gate cannot see one such output among millions.
 
-Kernels: gemm_tma_kernel (evk_gemm_tf32, the flat Linear path, tap-sum and phased strided convs, evk_conv_wgrad_tma),
+Kernels: gemm_tma_kernel (evk_gemm_tf32, the flat Linear path, tap-sum and phased strided convs), conv_wgrad_kernel,
 gconv_tc_kernel, the mma.sync and direct fallbacks, and both kernels of evk_conv2d_fwd[_hw].  Every case asserts from
 the library's dispatch accounting that its flops went to the kernel family it is about.
 """
@@ -211,9 +211,12 @@ def _to_cl(t):
 
 def _run_conv(ops, case, seed, backward=True, comp=0.0):
     """-> list of (what, got, ref, axes, tiles) after running the case and its float64 reference"""
-    name, B, Tin, C, N, Q, stride, pad, dil, P, G, act, use_res, masks, ffam, dfam, wfam, (slab, mt2) = case
+    name, B, Tin, C, N, Q, stride, pad, dil, P, G, act, use_res, masks, ffam, dfam, wfam, (slab, mt2, *mode) = case
     from easevoice_trainer_b200 import lib
     lib.init().evk_set_tma_options(slab, mt2, comp)
+    if "precise" in mode:
+        lib.init().evk_set_precise(1)
+    x0 = 1 if "x+1" in mode else 0
     for what, bnd in zip(("forward", "data gradient", "weight gradient"), R.conv_case_bounds(case)):
         assert_bound(bnd, f"{name} {what}")
     g = torch.Generator().manual_seed(seed)
@@ -239,14 +242,14 @@ def _run_conv(ops, case, seed, backward=True, comp=0.0):
 
     # ours: input as a channel slice whose pitch padding is NaN
     xbuf = torch.full((B, Tin * P, C + 4), NAN, device=DEV)
-    xbuf[..., :C] = _to_cl(x).to(DEV)
+    xbuf[..., x0:x0 + C] = _to_cl(x).to(DEV)
     xbuf.requires_grad_(backward)
     vd, bd = v.float().to(DEV).requires_grad_(backward), bias.float().to(DEV).requires_grad_(backward)
     resd = _to_cl(res).float().to(DEV).requires_grad_(backward) if use_res else None
     ln = lens.to(DEV, torch.int32) if masks else None
     pw = ops.pack_weight(vd)
     ops.dispatch_reset()
-    yo = ops.conv(xbuf[..., :C], pw, bd, stride=stride, pad=pad, dil=dil, P=P, groups=G, act=act, slope=R.LRELU_SLOPE, res=resd,
+    yo = ops.conv(xbuf[..., x0:x0 + C], pw, bd, stride=stride, pad=pad, dil=dil, P=P, groups=G, act=act, slope=R.LRELU_SLOPE, res=resd,
                   in_len=ln if masks == "inout" else None, out_len=ln)
     torch.cuda.synchronize()
     assert_family(ops, ffam, FWD + WGRAD, f"{name} forward")
@@ -260,8 +263,8 @@ def _run_conv(ops, case, seed, backward=True, comp=0.0):
     assert_family(ops, wfam, WGRAD, f"{name} weight gradient")
     if dfam:
         assert_family(ops, dfam, FWD, f"{name} data gradient")
-    assert (xbuf.grad[..., C:] == 0).all()
-    out += [("dx", xbuf.grad[..., :C], _to_cl(xr.grad), ("b", "row", "c"), {"row": 128, "c": _bn(C)}),
+    assert (xbuf.grad[..., :x0] == 0).all() and (xbuf.grad[..., x0 + C:] == 0).all()
+    out += [("dx", xbuf.grad[..., x0:x0 + C], _to_cl(xr.grad), ("b", "row", "c"), {"row": 128, "c": _bn(C)}),
             ("dW", vd.grad, vr.grad, ("n", "c", "tap"), {"n": 128, "c": 128}),
             ("dbias", bd.grad, br.grad, ("n",), None)]
     if use_res:
@@ -454,7 +457,7 @@ def test_compensation_applied_once(ops, exact_mode):
         torch.cuda.synchronize()
         assert_family(ops, "gemm_tf32", FWD + WGRAD + ("gemm_tf32",), "gemm_tf32")
         _assert_compensated(out, a.to(DEV) @ b.to(DEV).t(), 2, 4 + splits, f"gemm_tf32 splits {splits}")
-    # raw operands = 2: evk_conv_wgrad_tma, at a shape that runs one K split and at one that runs several
+    # raw operands = 2: conv_wgrad_kernel, at a shape that runs one K split and at one that runs several
     for B, T, C, N, Q in ((1, 2048, 512, 512, 5), (2, 2048, 64, 64, 3)):
         x, v, gy = R.ints((B, C, T, 1), 3, g, lo=1), R.ints((N, C, Q), 1, g, lo=1), R.ints((B, N, T, 1), 3, g, lo=1)
         vd = v.float().to(DEV).requires_grad_(True)
@@ -463,7 +466,7 @@ def test_compensation_applied_once(ops, exact_mode):
         y.backward(_to_cl(gy).float().to(DEV))
         torch.cuda.synchronize()
         assert_family(ops, "wgrad_gemm_tma", WGRAD, "conv wgrad")
-        tiles = Q * ((N + 127) // 128) * ((C + 127) // 128)                  # the split count ops.conv picks
+        tiles = Q * ((N + 127) // 128) * ((C + 127) // 128)                  # the split count evk_gconv_wgrad picks
         splits = max(1, min(64, torch.cuda.get_device_properties(DEV).multi_processor_count // tiles, B * ((T + 31) // 32) // 8))
         vr = v.to(DEV).requires_grad_(True)
         R.conv1d_ref(x.to(DEV), vr, None, 1, Q // 2, 1).backward(gy.to(DEV))

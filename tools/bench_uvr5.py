@@ -240,7 +240,7 @@ def rope_attn_rates(ops, reps=20):
     return out
 
 
-FAMILIES = (("gemm", ("evk_gconv_fwd", "evk_conv_direct_fwd")), ("attention", ("evk_rope_attn_fwd",)),
+FAMILIES = (("gemm", ("evk_gconv_fwd",)), ("attention", ("evk_rope_attn_fwd",)),
             ("norms", ("evk_row_l2norm", "evk_bs_band_input")), ("stft_istft", ("evk_stft_fwd", "evk_istft")))
 
 
