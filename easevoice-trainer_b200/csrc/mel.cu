@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(MEL_WPB * 32, 2) mel_fwd_warp_kernel(
     const int bb = (int)(fr / T), ff = (int)(fr - (long long)bb * T);
     const int ss = ff * hop - padc;
     const int LL = lens ? min(lens[bb], Lmax) : Lmax;
-    if (LL + 2 * padc < NFFT || ff >= (LL + 2 * padc - NFFT) / hop + 1) return false;
+    if (LL <= padc || LL + 2 * padc < NFFT || ff >= (LL + 2 * padc - NFFT) / hop + 1) return false;
     src = wav + (long long)bb * ldw + ss;
     return ss >= 0 && ss + NFFT <= LL && ((reinterpret_cast<uintptr_t>(src) & 15) == 0);
   };
@@ -150,9 +150,10 @@ __global__ void __launch_bounds__(MEL_WPB * 32, 2) mel_fwd_warp_kernel(
   const int pad = (NFFT - hop) / 2, s0 = f * hop - pad;
   const float* wv = wav + (long long)b * ldw;
   // per-row length: the reflection sits at the row's OWN end (the reference runs spectrogram_torch per utterance,
-  // data_utils.py:119-128) and frames past the row's own count hold what the zero-padded collate holds
+  // data_utils.py:119-128) and frames past the row's own count hold what the zero-padded collate holds.  A row too short to
+  // reflect once (L <= pad: its reflected tail would index before the row) has no frames at all, as in stft.cu.
   const int L = lens ? min(lens[b], Lmax) : Lmax;
-  if (f >= (L + 2 * pad - NFFT) / hop + 1 || L + 2 * pad < NFFT) {
+  if (L <= pad || L + 2 * pad < NFFT || f >= (L + 2 * pad - NFFT) / hop + 1) {
     for (int k = t; k < NBIN; k += 32) {
       if (spec) spec[frame * ld_spec + k] = 0.f;
       if (cplx) reinterpret_cast<float2*>(cplx)[frame * NBIN + k] = make_float2(0.f, 0.f);

@@ -72,9 +72,12 @@ struct StftP {
   float* frbuf;              // backward: windowed adjoint of every frame [B*T][N], overlap-added by stft_ola_kernel
 };
 
+// frames of a row of Lrow valid samples.  A row too short to reflect once (Lrow <= pad) has none: its frames would read
+// reflected positions outside [0, Lrow); it holds what the zero-padded collate holds, and the adjoint follows.  With
+// Lrow > pad every position a frame reads, -pad .. Lrow + pad - 1, reflects into [0, Lrow).
 __device__ __forceinline__ int frames_of_row(int Lrow, int pad, int N, int hop) {
   const int span = Lrow + 2 * pad - N;
-  return span < 0 ? 0 : span / hop + 1;
+  return (span < 0 || Lrow <= pad) ? 0 : span / hop + 1;
 }
 
 // shared memory: d0[NH] d1[NH] float2 | sx[NH + 1] float2 | mag[NH + 1 (+3)] float

@@ -29,7 +29,9 @@ EVK_HD float2 stft_cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y
 EVK_HD int stft_reflect(int i, int L) {
   if (i < 0) i = -i;
   if (i >= L) i = 2 * (L - 1) - i;
-  if (i < 0) i = 0;                       // only for rows shorter than the padding (never the case for real inputs)
+  if (i < 0) i = 0;                       // only for rows no longer than the padding: stft.cu gives those no frames, so
+                                          // there it is unreachable; vr_wave.cu's reflect mode reaches it for bands of
+                                          // <= n_fft / 2 samples
   return i;
 }
 
