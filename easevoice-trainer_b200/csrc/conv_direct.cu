@@ -75,7 +75,7 @@ __global__ void direct_fwd_warp(const __grid_constant__ DP p) {
   (p.y + b * p.y_sb + h * p.y_sh)[orow * p.ldy + n] = acc;
 }
 
-// dX[ipos][c] = sum_q sum_{n in group} dY[orow(j)][n] * W[q][n][c_local],  j*is + off[q] == ij
+// dX[ipos][c] = sum_q sum_{n in group} dY[orow(j)][n] * W[q][n][c_local] (+ bias[c]),  j*is + off[q] == ij
 __global__ void direct_dgrad(const __grid_constant__ DP p) {
   const int z = blockIdx.z, b = z / p.H, h = z - b * p.H;
   const long long nin = (long long)p.Tin * p.P;
@@ -101,6 +101,7 @@ __global__ void direct_dgrad(const __grid_constant__ DP p) {
       for (int n = 0; n < Ng; ++n) acc = fmaf(yr[n], wr[(long long)n * p.ldw], acc);
     }
   }
+  if (p.bias) acc += p.bias[h * p.b_sh + c];
   (const_cast<float*>(p.x) + b * p.x_sb + h * p.x_sh)[ipos * p.ldx + c] = acc;
 }
 
@@ -154,14 +155,14 @@ int evk::conv_direct_fwd(const evk_gconv_desc* d, cudaStream_t st) {
   return check_launch("conv_direct_fwd");
 }
 
-extern "C" int evk_conv_direct_dgrad(const evk_gconv_desc* d, evk_stream_t stream) {
+int evk::conv_direct_dgrad(const evk_gconv_desc* d, cudaStream_t st) {
   DP p;
   int rc = conv_params(d, p, "conv_direct_dgrad");
   if (rc) return rc;
   const long long total = (long long)p.Tin * p.P * p.C;
   if (total == 0) return EVK_OK;
   dim3 grid(cdiv(total, 256), 1, p.Z);
-  direct_dgrad<<<grid, 256, 0, (cudaStream_t)stream>>>(p);
+  direct_dgrad<<<grid, 256, 0, st>>>(p);
   g_disp_flops[3] += desc_flops(d);
   return check_launch("conv_direct_dgrad");
 }

@@ -43,8 +43,9 @@ struct ConvP {
 };
 // Validates d and fills p; `who` names the entry point in the error message.  Returns EVK_OK or EVK_ERR_ARG.
 int conv_params(const evk_gconv_desc* d, ConvP& p, const char* who);
-// The direct CUDA-core kernels (conv_direct.cu): evk_gconv_fwd / evk_gconv_wgrad run the launches they cannot tile on them.
+// The direct CUDA-core kernels (conv_direct.cu): the conv entry points run the launches they cannot tile on them.
 int conv_direct_fwd(const evk_gconv_desc* d, cudaStream_t st);
+int conv_direct_dgrad(const evk_gconv_desc* d, cudaStream_t st);   // d->x is written (dX), d->y read (dY)
 int conv_direct_wgrad(const evk_gconv_desc* d, cudaStream_t st);
 
 // The evk_act epilogue.

@@ -9,6 +9,7 @@
 //
 // Replaces the cuDNN / cuBLAS kernels behind the reference's Conv1d / Conv2d(k,1) / ConvTranspose1d /
 // Linear / matmul call sites (see include/evk.h for file:line).
+#include "dgrad_plan.h"
 #include "evk_common.cuh"
 
 namespace evk {
@@ -445,21 +446,17 @@ extern "C" int evk_set_precise(int32_t on) { g_precise = on ? 1 : 0; return EVK_
 extern "C" int evk_get_precise(void) { return g_precise; }
 extern "C" int evk_set_backend(int32_t tensor_core) { g_backend_tc = tensor_core ? 1 : 0; return EVK_OK; }
 
-extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
+// Routes 2-4 of evk_gconv_fwd for a launch h in the groups-as-batch form with 16-byte tileable operands (route 2 takes
+// stride 1 only).  d is the launch as its caller described it: its flops go to the slot of the kernel that runs it.
+static int fwd_tiled(const evk_gconv_desc* d, const evk_gconv_desc* h, cudaStream_t st) {
   GP p;
-  int rc = conv_params(d, p, "gconv_fwd");
+  int rc = conv_params(h, p, "gconv_fwd");
   if (rc) return rc;
-  EVK_REQUIRE(d->y != nullptr && d->x != nullptr && d->w != nullptr, EVK_ERR_ARG, "gconv_fwd: null tensor");
-  cudaStream_t st = (cudaStream_t)stream;
-  evk_gconv_desc h;
-  const bool tiled = groups_as_batch(d, h) && fwd_tileable(&h);
-  if (tiled && !g_precise) {
-    rc = h.is > 1 ? gemm_tma_phased(&h, st) : g_backend_tc ? gemm_tma_try(&h, st) : 1;
+  if (h->is == 1 && g_backend_tc && !g_precise) {
+    rc = gemm_tma_try(h, st);
     if (rc <= 0) { if (rc == 0) g_disp_flops[0] += desc_flops(d); return rc; }
   }
   EVK_REQUIRE(!(d->drop_rng && d->drop_p > 0.f), EVK_ERR_UNSUPPORTED, "gconv_fwd: fused dropout needs a launch the TMA kernel takes");
-  if (!tiled) return conv_direct_fwd(d, st);
-  conv_params(&h, p, "gconv_fwd");
   if (g_backend_tc && !g_precise) {
     rc = gconv_tc_try(p, st);
     if (rc <= 0) { if (rc == 0) g_disp_flops[1] += desc_flops(d); return rc; }
@@ -484,6 +481,75 @@ extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
     default: return EVK_F(8, 1, 1, 1);
   }
 #undef EVK_F
+}
+
+extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
+  GP p;
+  int rc = conv_params(d, p, "gconv_fwd");
+  if (rc) return rc;
+  EVK_REQUIRE(d->y != nullptr && d->x != nullptr && d->w != nullptr, EVK_ERR_ARG, "gconv_fwd: null tensor");
+  cudaStream_t st = (cudaStream_t)stream;
+  evk_gconv_desc h;
+  if (!groups_as_batch(d, h) || !fwd_tileable(&h)) {
+    EVK_REQUIRE(!(d->drop_rng && d->drop_p > 0.f), EVK_ERR_UNSUPPORTED, "gconv_fwd: fused dropout needs a launch the TMA kernel takes");
+    return conv_direct_fwd(d, st);
+  }
+  if (h.is > 1 && !g_precise) {
+    rc = gemm_tma_phased(&h, st);
+    if (rc <= 0) { if (rc == 0) g_disp_flops[0] += desc_flops(d); return rc; }
+  }
+  return fwd_tiled(d, &h, st);
+}
+
+// Route 1 of evk_gconv_dgrad: dY and PB tileable, and group slices of whole 16-byte pieces
+static bool dgrad_polyphase_ok(const evk_gconv_desc* d, const float* wt, int ld_wt) {
+  const int G = d->G < 1 ? 1 : d->G;
+  return wt && (ld_wt % 4) == 0 && ((uintptr_t)wt % 16) == 0 && (d->ldy % 4) == 0 && (d->y_sb % 4) == 0 &&
+         ((uintptr_t)d->y % 16) == 0 && (G == 1 || ((d->C / G) % 4 == 0 && (d->N / G) % 4 == 0));
+}
+
+// One stride-1 forward launch per phase of dgrad_plan.h: dY is the input, PB the weight, dX the output at rows u0 + is*jj,
+// grouped convs as the inner batch.
+static int dgrad_polyphase(const evk_gconv_desc* d, const float* wt, int ld_wt, cudaStream_t st) {
+  const int s = d->is, G = d->G < 1 ? 1 : d->G, Cg = d->C / G, Ng = d->N / G;
+  for (int q = 1; s > 1 && q < d->Q; ++q)
+    EVK_REQUIRE(d->off[q] == d->off[0] + q, EVK_ERR_UNSUPPORTED, "gconv_dgrad: a strided conv needs taps at consecutive offsets");
+  if (d->Q < s) {                                            // rows of the residues without a tap are not written below
+    EVK_REQUIRE(cudaMemsetAsync(const_cast<float*>(d->x), 0, (size_t)d->Z * d->x_sb * sizeof(float), st) == cudaSuccess, EVK_ERR_CUDA,
+                "gconv_dgrad: memset failed");
+  }
+  evk_gconv_desc h = {};
+  h.x = d->y; h.y = const_cast<float*>(d->x); h.bias = d->bias;
+  h.x_sb = d->y_sb; h.w_sq = (long long)s * Cg * ld_wt; h.y_sb = d->x_sb;
+  h.ldx = d->ldy; h.ldw = ld_wt; h.ldy = d->ldx;
+  h.Z = d->Z * G; h.H = G; h.G = 1; h.C = Ng; h.N = Cg;
+  h.Tin = d->J; h.P = d->P; h.is = 1; h.os = s; h.Tout = d->Tin;
+  if (G > 1) { h.x_sh = Ng; h.w_sh = Ng; h.y_sh = Cg; h.r_sh = Cg; h.b_sh = Cg; }
+  for (int rho = 0; rho < s; ++rho) {
+    DgradPhase ph;
+    if (!dgrad_phase(d->off, d->Q, s, d->Tin, rho, ph)) continue;
+    h.w = const_cast<float*>(wt) + (long long)ph.q0 * Cg * ld_wt;
+    h.Q = ph.nq; h.J = ph.J; h.o0 = ph.u0;
+    for (int k = 0; k < EVK_MAX_TAPS; ++k) h.off[k] = k < ph.nq ? ph.off[k] : 0;
+    if (int rc = fwd_tiled(&h, &h, st)) return rc;
+  }
+  return EVK_OK;
+}
+
+extern "C" int evk_gconv_dgrad(const evk_gconv_desc* d, const float* wt, int32_t ld_wt, evk_stream_t stream) {
+  GP p;
+  int rc = conv_params(d, p, "gconv_dgrad");
+  if (rc) return rc;
+  EVK_REQUIRE(d->y != nullptr && d->x != nullptr && d->w != nullptr, EVK_ERR_ARG, "gconv_dgrad: null tensor");
+  EVK_REQUIRE(d->H == 1 && d->ldx == d->C && d->x_sb == (long long)d->Tin * d->P * d->C, EVK_ERR_ARG,
+              "gconv_dgrad: dX must be a dense [Z][Tin*P][C] tensor, H = 1");
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = dgrad_polyphase_ok(d, wt, ld_wt) ? dgrad_polyphase(d, wt, ld_wt, st) : conv_direct_dgrad(d, st);
+  if (rc || !d->in_len) return rc;
+  // the forward reads row t*P + w as zero when t >= in_len[b]: with P*C floats per t, that is a row mask over t
+  float* dx = const_cast<float*>(d->x);
+  const int ld = d->P * d->C;
+  return evk_rowmask(dx, ld, dx, ld, d->Z, d->Tin, ld, d->in_len, stream);
 }
 
 // W[b'][h'][q][n][c] += sum over the batch items b of [b0, b0 + nb) (all of them when w_sb == 0, else b = b') and the groups h

@@ -215,18 +215,19 @@ def _desc(off=(), **kw):
     return d
 
 
+# the extra operand of an entry point, attached to the descriptor object (not C fields): wgrad's transposed dY, dgrad's PB
+_DESC_EXTRA = {"evk_gconv_wgrad": ("dyt", "ld_dyt"), "evk_gconv_dgrad": ("wt", "ld_wt")}
+
+
 def _run_desc(fn, d):
-    """one descriptor launch; evk_gconv_wgrad also gets the transposed dY attached as d.dyt / d.ld_dyt (not C fields)"""
+    """one descriptor launch; evk_gconv_wgrad / evk_gconv_dgrad also get the operand attached as d.dyt / d.wt (_DESC_EXTRA)"""
     global _launches
     _launches += 1
     flops = 2.0 * d.Z * d.J * d.P * d.N * (d.C // max(d.G, 1)) * d.Q
-    args = (getattr(d, "dyt", None), getattr(d, "ld_dyt", 0)) if fn == "evk_gconv_wgrad" else ()
+    extra = _DESC_EXTRA.get(fn)
+    args = (getattr(d, extra[0], None), getattr(d, extra[1], 0)) if extra else ()
     _timed(fn, lambda: L.check(getattr(_lib(), fn)(ctypes.byref(d), *args, _st())), flops,
            tag=(f"Z{d.Z} J{d.J} P{d.P} C{d.C} N{d.N} Q{d.Q} s{d.is_}" if PROF_SHAPES else None))
-
-
-def _aligned(t, ld):
-    return (ld % 4 == 0) and (t.data_ptr() % 16 == 0)
 
 
 class PackedW:
@@ -460,56 +461,20 @@ def _conv_out_len(Tin, Q, stride, pad, dil):
     return (Tin + 2 * pad - dil * (Q - 1) - 1) // stride + 1
 
 
-def _fwd_like(x, Tin, w, wq0, wqstep, nq, ldw, w_sq, C, N, y, *, J, P, is_, os_, o0, Tout, off, bias=None, res=None,
-              act=0, slope=0.0, in_len=None, out_len=None, G=1, H=1, x_sh=0, w_sh=0, y_sh=0, drop=None, no_phase_split=0):
-    """one forward-like launch of the generalised conv; evk_gconv_fwd picks the kernel.  Grouped convs pass G = groups
-    (C, N are then the total channel counts).  H > 1 runs an inner batch with the per-item offsets x_sh / w_sh / y_sh (the
-    grouped data gradient, whose PB operand is not in the [Q][N][C/G] layout that G describes)."""
+def _fwd_like(x, Tin, w, ldw, w_sq, C, N, y, *, J, P, is_, off, bias=None, res=None, act=0, slope=0.0, in_len=None,
+              out_len=None, G=1, drop=None, no_phase_split=0):
+    """one forward-like launch of the generalised conv, len(off) taps, output rows j < J; evk_gconv_fwd picks the kernel.
+    Grouped convs pass G = groups (C, N are then the total channel counts)."""
     B = x.shape[0]
     _, _, ldx = _rows(x)
     _, _, ldy = _rows(y)
     ldr = _rows(res)[2] if res is not None else 0
-    d = _desc(x=x, w=w.data_ptr() + 4 * wq0 * w_sq, y=y, res=res, bias=bias, in_len=in_len, out_len=out_len,
-              x_sb=Tin * P * ldx, x_sh=x_sh, w_sh=w_sh, w_sq=wqstep * w_sq, y_sb=Tout * P * ldy, y_sh=y_sh,
-              r_sb=Tout * P * ldr, r_sh=y_sh, ldx=ldx, ldw=ldw, ldy=ldy, ldr=ldr, Z=B * H, H=H, G=G, C=C, N=N, Q=nq,
-              Tin=Tin, J=J, P=P, is_=is_, os_=os_, o0=o0, Tout=Tout, act=act, slope=float(slope), off=off,
-              no_phase_split=no_phase_split)
+    d = _desc(x=x, w=w, y=y, res=res, bias=bias, in_len=in_len, out_len=out_len, x_sb=Tin * P * ldx, w_sq=w_sq, y_sb=J * P * ldy,
+              r_sb=J * P * ldr, ldx=ldx, ldw=ldw, ldy=ldy, ldr=ldr, Z=B, G=G, C=C, N=N, Q=len(off), Tin=Tin, J=J, P=P, is_=is_,
+              os_=1, Tout=J, act=act, slope=float(slope), off=off, no_phase_split=no_phase_split)
     if drop is not None:                      # fused dropout after the activation (TMA kernel epilogue only; the library rejects other routes)
         d.drop_rng, d.drop_sid, d.drop_p = rng_state(x.device).data_ptr(), int(drop[1]), float(drop[0])
     _run_desc("evk_gconv_fwd", d)
-
-
-def _dgrad_phases(dy, Jy, pb, ldb, C, N, Q, dx, Tin, P, stride, pad, dil, H=1):
-    """dX[u] = sum_q sum_n dY[(u+pad-q*dil)/stride][n] * PB[q][c][n] as one F launch per stride phase.
-    C, N are per-group sizes when H (= groups) > 1; PB is [Q][C][ldb] with the group's n-columns at offset h*N."""
-    w_sq = pb.shape[1] * ldb
-    for u0, Ju, q0, nq, off in dgrad_phase_plan(Q, stride, pad, dil, Tin):
-        _fwd_like(dy, Jy, pb, q0, stride, nq, ldb, w_sq, N, C, dx, J=Ju, P=P, is_=1, os_=stride, o0=u0, Tout=Tin, off=off,
-                  H=H, x_sh=N if H > 1 else 0, w_sh=N if H > 1 else 0, y_sh=C if H > 1 else 0)
-
-
-def dgrad_phase_plan(Q, stride, pad, dil, Tin):
-    """Polyphase decomposition of a conv's data gradient (also of ConvTranspose1d's forward).
-
-    dX[u] = sum_q dY[(u + pad - q*dil)/stride] W[q] over the taps for which the division is exact.  For every residue
-    rho of (u + pad) mod stride this yields a stride-1 tap-sum over dY writing every stride-th u:
-        -> list of (u0, Ju, q0, nq, off):  u = u0 + stride*jj (jj < Ju) uses taps q0, q0+stride, ... (nq of them) and
-           reads dY[jj + off[k]].
-    """
-    assert stride == 1 or dil == 1, "strided convs must have dilation 1"
-    plan = []
-    for rho in range(stride):
-        taps = list(range(rho, Q, stride))
-        u0 = (rho - pad) % stride
-        if u0 >= Tin or not taps:
-            continue
-        Ju = (Tin - u0 + stride - 1) // stride
-        if stride == 1:
-            off = [pad - q * dil for q in taps]
-        else:
-            off = [(u0 + pad - q) // stride for q in taps]
-        plan.append((u0, Ju, taps[0], len(taps), off))
-    return plan
 
 
 class _ConvFn(torch.autograd.Function):
@@ -528,9 +493,8 @@ class _ConvFn(torch.autograd.Function):
         y = torch.empty((B, J * P, N), device=x.device, dtype=torch.float32)
         if res is not None:
             res = _cl(res)
-        _fwd_like(x, Tin, pa, 0, 1, Q, lda, N * lda, C, N, y, J=J, P=P, is_=stride, os_=1, o0=0, Tout=J,
-                  off=[q * dil - pad for q in range(Q)], bias=bias, res=res, act=act, slope=slope, in_len=in_len, out_len=out_len,
-                  drop=drop, G=G)
+        _fwd_like(x, Tin, pa, lda, N * lda, C, N, y, J=J, P=P, is_=stride, off=[q * dil - pad for q in range(Q)], bias=bias,
+                  res=res, act=act, slope=slope, in_len=in_len, out_len=out_len, drop=drop, G=G)
         ctx.cfg = cfg
         ctx.dims = (B, Tin, C, N, J, lda)
         ctx.has = (bias is not None, res is not None)
@@ -547,7 +511,6 @@ class _ConvFn(torch.autograd.Function):
         B, Tin, C, N, J, lda = ctx.dims
         x, pa, pb, y = ctx.saved_tensors
         has_bias, has_res = ctx.has
-        Cg, Ng = C // G, N // G
         dy = dy.contiguous()
         Ro = J * P
         offs = [q * dil - pad for q in range(Q)]
@@ -572,20 +535,12 @@ class _ConvFn(torch.autograd.Function):
         dx = dpa = dres = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty((B, Tin * P, C), device=dy.device, dtype=torch.float32)
-            use_mma = (pb is not None and pb.numel() > 0 and _aligned(dy, N) and pb.shape[2] % 4 == 0
-                       and (G == 1 or (Ng % 4 == 0 and Cg % 4 == 0)))
-            if use_mma:
-                if Q < stride:
-                    dx.zero_()
-                _dgrad_phases(dy, J, pb, pb.shape[2], Cg, Ng, Q, dx, Tin, P, stride, pad, dil, H=G)
-            else:
-                d = _desc(x=dx, w=pa, y=dy, x_sb=Tin * P * C, w_sq=N * lda, y_sb=J * P * N, ldx=C, ldw=lda, ldy=N, Z=B,
-                          C=C, N=N, Q=Q, G=G, Tin=Tin, J=J, P=P, is_=stride, os_=1, Tout=J, off=offs)
-                _run_desc("evk_conv_direct_dgrad", d)
-            if in_len is not None:
-                dxm = torch.empty_like(dx)
-                _call("evk_rowmask", _p(dx), C, _p(dxm), C, B, Tin * P, C, _p(in_len))
-                dx = dxm
+            d = _desc(x=dx, w=pa, y=dy, in_len=in_len, x_sb=Tin * P * C, w_sq=N * lda, y_sb=J * P * N, ldx=C, ldw=lda, ldy=N, Z=B,
+                      C=C, N=N, Q=Q, G=G, Tin=Tin, J=J, P=P, is_=stride, os_=1, Tout=J, off=offs)
+            if pb is not None and pb.numel():
+                assert pb.shape[1] == C // G, "PB must be [Q][C/G][ldb]"
+                d.wt, d.ld_wt = _p(pb), pb.shape[2]
+            _run_desc("evk_gconv_dgrad", d)
         if ctx.needs_input_grad[1]:
             dpa = dpa_buffer(pa)
             dw.w, dw.y = dpa.data_ptr(), dy.data_ptr()
@@ -662,20 +617,23 @@ def linear(x, w: PackedW, bias=None, act=ACT_NONE, slope=0.0, out_len=None, in_l
 
 
 class _ConvTFn(torch.autograd.Function):
-    """ConvTranspose1d: v [Cin][Cout][Q] packed as pa = [Q][Cin][Cout], pb = [Q][Cout][Cin]."""
+    """ConvTranspose1d: v [Cin][Cout][Q] packed as pa = [Q][Cin][Cout], pb = [Q][Cout][Cin].  It is the conv with Cout
+    input and Cin output channels, weight PA, run backwards: the forward is that conv's data gradient, the data gradient
+    its forward."""
 
     @staticmethod
     def forward(ctx, x, pa, pb, bias, cfg):
         Q, stride, pad = cfg
         x = _cl(x)
         B, Tin, Cin = x.shape
-        Cout, ldb = pb.shape[1], pb.shape[2]
+        Cout, lda = pb.shape[1], pa.shape[2]
         Tout = (Tin - 1) * stride - 2 * pad + Q
-        y = (torch.zeros if Q < stride else torch.empty)((B, Tout, Cout), device=x.device, dtype=torch.float32)
-        w_sq = Cout * ldb
-        for u0, Ju, q0, nq, off in dgrad_phase_plan(Q, stride, pad, 1, Tout):
-            _fwd_like(x, Tin, pb, q0, stride, nq, ldb, w_sq, Cin, Cout, y, J=Ju, P=1, is_=1, os_=stride, o0=u0, Tout=Tout,
-                      off=off, bias=bias)
+        y = torch.empty((B, Tout, Cout), device=x.device, dtype=torch.float32)
+        _, _, ldx = _rows(x)
+        d = _desc(x=y, w=pa, y=x, bias=bias, x_sb=Tout * Cout, w_sq=Cin * lda, y_sb=Tin * ldx, ldx=Cout, ldw=lda, ldy=ldx, Z=B,
+                  C=Cout, N=Cin, Q=Q, Tin=Tout, J=Tin, P=1, is_=stride, os_=1, Tout=Tin, off=[q - pad for q in range(Q)])
+        d.wt, d.ld_wt = _p(pb), pb.shape[2]
+        _run_desc("evk_gconv_dgrad", d)
         ctx.cfg = cfg
         ctx.dims = (B, Tin, Cin, Cout, Tout)
         ctx.save_for_backward(x, pa)
@@ -692,8 +650,7 @@ class _ConvTFn(torch.autograd.Function):
         dx = dpa = dbias = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty((B, Tin, Cin), device=dy.device, dtype=torch.float32)
-            _fwd_like(dy, Tout, pa, 0, 1, Q, lda, Cin * lda, Cout, Cin, dx, J=Tin, P=1, is_=stride, os_=1, o0=0,
-                      Tout=Tin, off=off, no_phase_split=1)
+            _fwd_like(dy, Tout, pa, lda, Cin * lda, Cout, Cin, dx, J=Tin, P=1, is_=stride, off=off, no_phase_split=1)
         if ctx.needs_input_grad[1]:
             dpa = dpa_buffer(pa)
             _, _, ldx = _rows(x)
@@ -2180,8 +2137,8 @@ def linear_into(x, w: PackedW, y, bias=None, act=ACT_NONE, res=None):
     rows, C = x.shape
     N = w.D0
     assert w.Q == 1 and y.shape == (rows, N) and C <= w.pa.shape[2], (x.shape, y.shape, w.pa.shape)
-    _fwd_like(x.unsqueeze(0), rows, w.pa, 0, 1, 1, w.pa.shape[2], N * w.pa.shape[2], C, N, y.unsqueeze(0), J=rows, P=1, is_=1,
-              os_=1, o0=0, Tout=rows, off=[0], bias=bias, res=res.unsqueeze(0) if res is not None else None, act=act)
+    _fwd_like(x.unsqueeze(0), rows, w.pa, w.pa.shape[2], N * w.pa.shape[2], C, N, y.unsqueeze(0), J=rows, P=1, is_=1, off=[0],
+              bias=bias, res=res.unsqueeze(0) if res is not None else None, act=act)
     return y
 
 

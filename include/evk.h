@@ -45,8 +45,8 @@ int evk_sync_check(evk_stream_t stream); /* cudaStreamSynchronize + error fetch 
  * z = b*H + h addresses a two-level batch (X + b*x_sb + h*x_sh, same for W/Y/R; w_sb = w_sh = 0
  * shares one weight).  epi(v) = mask(act(v + bias[n] + R[...][n])) with mask = (row/P < out_len[b]).
  * Covers: Conv1d / Conv2d(k,1) forward (models.py:452-471,538-587; modules.py:187-212,298-311;
- * attentions.py:408-416), their data gradients (one call per stride phase), ConvTranspose1d
- * (models.py:460), nn.Linear / 1x1 convs, and the attention GEMMs (attentions.py:243-292).
+ * attentions.py:408-416), their data gradients (evk_gconv_dgrad), ConvTranspose1d (models.py:460; the data gradient of
+ * a conv), nn.Linear / 1x1 convs, and the attention GEMMs (attentions.py:243-292).
  * ------------------------------------------------------------------------------------------ */
 typedef struct evk_gconv_desc {
   const float* x; float* w; float* y; const float* res; const float* bias;
@@ -109,9 +109,19 @@ int evk_gconv_wgrad(const evk_gconv_desc* d, const float* dyt, int32_t ld_dyt, e
  * offsets when strided: any dilation when Q == 1), G <= 1, H == 1, os == 1, o0 == 0, w_sb == 0, no in_len, C % 4 == 0,
  * C, N >= 32, Z*J*P >= 2048, J*P >= 64, X and Yg 16-byte tileable, not precise. */
 int evk_gconv_wgrad_takes_dyt(const evk_gconv_desc* d);
-/* Direct (CUDA-core) data gradient for skinny layers: C/G < 8 (1-channel inputs, grouped k=41 convs of
- * DiscriminatorS, models.py:563-575).  Same descriptor; W is [Q][N][C/G]. */
-int evk_conv_direct_dgrad(const evk_gconv_desc* d, evk_stream_t stream);  /* d->x is WRITTEN (dX), d->y read */
+/* Data gradient of the conv that d describes as evk_gconv_fwd takes it (is = stride, off[q] = q*dil - pad, W = PA
+ * [Q][N][C/G]), with the roles of x and y swapped: d->y is dY [Z][J*P][N] and is read, d->x is dX and is written, a dense
+ * [Z][Tin*P][C] tensor (ldx == C; H == 1).  wt (nullable) is the transposed weight PB [Q][C/G][ld_wt].  d->bias
+ * (nullable) is added to every row of dX: ConvTranspose1d's forward is this call.  Routes:
+ *   1. wt 16-byte tileable (ld_wt % 4 == 0, 16-byte aligned), dY too (ldy, y_sb multiples of 4, 16-byte aligned) and,
+ *      when G > 1, C/G and N/G multiples of 4: the polyphase plan (csrc/dgrad_plan.h), one stride-1 launch of routes
+ *      2-4 of evk_gconv_fwd per residue of the taps mod is, each writing every is-th row of dX: dY as the input, PB
+ *      offset by q0 taps with an is-fold tap pitch as the weight, os = is, o0 = the phase's first row, groups as the
+ *      inner batch.  A strided conv needs taps at consecutive offsets (dilation 1).  When Q < is, dX is zeroed first
+ *      (rows of a residue with no tap stay zero, without the bias);
+ *   2. otherwise the direct kernel.
+ * With d->in_len, rows t*P + w of dX with t >= in_len[b] are zeroed afterwards: the forward read them as zero. */
+int evk_gconv_dgrad(const evk_gconv_desc* d, const float* wt, int32_t ld_wt, evk_stream_t stream);
 
 /* out[n] (+)= sum_rows x[row][n]  -- bias gradients */
 int evk_colsum(const float* x, int64_t rows, int32_t n, int32_t ld, float* out, int32_t accumulate, evk_stream_t stream);

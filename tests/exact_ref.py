@@ -110,6 +110,8 @@ CONV_CASES = [
     ("P=3 k3 +res", 2, 400, 64, 32, 3, 1, 1, 1, 3, 1, ACT_LRELU, True, "", "fwd_gemm_tma", "fwd_gemm_tma", "wgrad_gemm_tma", (1, 1)),
     ("P=5 k5 +out_len", 3, 140, 36, 64, 5, 1, 2, 1, 5, 1, ACT_NONE, False, "out", "fwd_gemm_tma", "fwd_gemm_tma", "wgrad_gemm_tma", (1, 1)),
     ("P=11 k5", 2, 100, 64, 128, 5, 1, 2, 1, 11, 1, ACT_LRELU, False, "", "fwd_gemm_tma", "fwd_gemm_tma", "wgrad_gemm_tma", (1, 1)),
+    # in_len with a period fold: the forward reads rows t*P + w with t >= in_len as zero, so those rows of dx are zero
+    ("P=2 k5 +in_len", 3, 40, 32, 32, 5, 1, 2, 1, 2, 1, ACT_NONE, False, "inout", "fwd_gconv_tc", None, "wgrad_mma_sync", (1, 1)),
     ("phased s2 P=2 k4", 2, 1100, 64, 64, 4, 2, 1, 1, 2, 1, ACT_RELU, False, "", "fwd_gemm_tma", "fwd_gemm_tma", "wgrad_gemm_tma", (1, 1)),
     ("phased s4 P=5 k8 +out_len", 2, 1000, 32, 64, 8, 4, 2, 1, 5, 1, ACT_NONE, False, "out", "fwd_gemm_tma", "fwd_gemm_tma", "wgrad_gemm_tma", (1, 1)),
     # gconv_tc_kernel: in_len-masked input (WN in_layer), 16-channel resblock, grouped (DiscriminatorS groups at stride 1),
@@ -141,13 +143,16 @@ CONV_CASES = [
     ("route in_len s2", 1, 4095, 32, 32, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "inout", "fwd_mma_sync", None, "wgrad_mma_sync", (1, 1)),
     ("route precise s2", 1, 4095, 32, 32, 3, 2, 1, 1, 1, 1, ACT_NONE, False, "", "fwd_mma_sync", None, "wgrad_mma_sync", (1, 1, "precise")),
     ("route grouped g2 8->6 Ng 3", 2, 300, 8, 6, 5, 1, 2, 1, 1, 2, ACT_NONE, False, "", "fwd_gconv_tc", None, "wgrad_direct", (1, 1)),
+    # N / G = 3: the strided grouped data gradient takes the direct kernel, the forward mma.sync
+    ("route grouped g2 8->6 Ng 3 s2", 2, 300, 8, 6, 5, 2, 2, 1, 1, 2, ACT_LRELU, False, "", "fwd_mma_sync", "fwd_direct", "wgrad_direct", (1, 1)),
     # group slices that are not 16-byte tileable (C / G = 3): the direct kernels take the grouped conv as G
     ("route grouped g2 6->8 Cg 3", 2, 300, 6, 8, 5, 1, 2, 1, 1, 2, ACT_LRELU, False, "", "fwd_direct", "fwd_direct", "wgrad_direct", (1, 1)),
 ]
 # conv_post: 16 -> 1 channel carried as 4 (zero weight rows), tanh: B, Tin, C, Q, pad
 CONV_POST = (2, 700, 16, 7, 3)
-# ConvTranspose1d, the shapes of check_conv_transpose that run on the TMA kernel: Cin, Cout, Q, stride, T
-CONVT_CASES = [(256, 128, 16, 8, 1100), (64, 32, 4, 2, 1500), (128, 64, 8, 2, 130)]
+# ConvTranspose1d, the shapes of check_conv_transpose that run on the TMA kernel: Cin, Cout, Q, stride, T, and optionally
+# "x+1" (x starts one float into its rows: not 16-byte aligned, so the forward and the weight gradient run on the direct kernels)
+CONVT_CASES = [(256, 128, 16, 8, 1100), (64, 32, 4, 2, 1500), (128, 64, 8, 2, 130), (64, 32, 4, 2, 300, "x+1")]
 
 
 def conv_case_bounds(case):

@@ -3,6 +3,7 @@ import ctypes
 import io
 import json
 import os
+import subprocess
 from contextlib import redirect_stdout
 
 import pytest
@@ -37,13 +38,18 @@ def test_descriptor_struct_layout():
 
 def test_run_desc_hook_keeps_the_transposed_dy(monkeypatch):
     """Timing hooks (bench.py --config 5) wrap ops._run_desc(fn, d) with two arguments: the weight gradient's transposed dY
-    travels on the descriptor, so a wrapped launch still reaches evk_gconv_wgrad with it."""
+    and the data gradient's transposed weight travel on the descriptor, so a wrapped launch still reaches evk_gconv_wgrad /
+    evk_gconv_dgrad with them."""
     from easevoice_trainer_b200 import ops
     seen = []
 
     class FakeLib:
         def evk_gconv_wgrad(self, d, dyt, ld_dyt, stream):
             seen.append((dyt, ld_dyt))
+            return 0
+
+        def evk_gconv_dgrad(self, d, wt, ld_wt, stream):
+            seen.append(("dgrad", wt, ld_wt))
             return 0
 
         def evk_gconv_fwd(self, d, stream):
@@ -62,8 +68,14 @@ def test_run_desc_hook_keeps_the_transposed_dy(monkeypatch):
     hook("evk_gconv_wgrad", d)
     hook("evk_gconv_wgrad", ops._desc(Z=1, C=4, N=4, Q=1, J=1, P=1))
     hook("evk_gconv_fwd", d)
+    dd = ops._desc(Z=1, C=4, N=4, Q=1, J=1, P=1)
+    dd.wt, dd.ld_wt = ctypes.c_void_p(8192), 12
+    hook("evk_gconv_dgrad", dd)
+    hook("evk_gconv_dgrad", ops._desc(Z=1, C=4, N=4, Q=1, J=1, P=1))
     assert seen[0][0].value == 4096 and seen[0][1] == 32
     assert seen[1] == (None, 0) and seen[2] == ()
+    assert seen[3][0] == "dgrad" and seen[3][1].value == 8192 and seen[3][2] == 12
+    assert seen[4] == ("dgrad", None, 0)
 
 
 def test_pack_job_struct_layout():
@@ -122,8 +134,43 @@ def test_generator_lr_groups():
     assert all(n.startswith("enc_p.encoder_text.") for n in groups[2][1]) and len(groups[1][1]) == 1
 
 
-def test_dgrad_phase_plan_covers_every_tap_exactly_once():
-    from easevoice_trainer_b200.ops import dgrad_phase_plan
+_PLAN_SHIM = r"""
+#include "dgrad_plan.h"
+// the conv's taps at off[q] = q*dil - pad; out = {u0, J, q0, nq, off[0..nq)}
+extern "C" int dgrad_phase_c(int Q, int s, int pad, int dil, int Tin, int rho, int* out) {
+  int off[EVK_MAX_TAPS];
+  for (int q = 0; q < Q; ++q) off[q] = q * dil - pad;
+  evk::DgradPhase ph;
+  if (!evk::dgrad_phase(off, Q, s, Tin, rho, ph)) return 0;
+  out[0] = ph.u0; out[1] = ph.J; out[2] = ph.q0; out[3] = ph.nq;
+  for (int k = 0; k < ph.nq; ++k) out[4 + k] = ph.off[k];
+  return 1;
+}
+"""
+
+
+@pytest.fixture(scope="module")
+def dgrad_plan(tmp_path_factory):
+    """the library's polyphase plan of a conv data gradient (csrc/dgrad_plan.h) compiled for the host"""
+    d = tmp_path_factory.mktemp("dgrad_plan")
+    (d / "shim.cpp").write_text(_PLAN_SHIM)
+    so = str(d / "libdgrad_plan.so")
+    subprocess.run(["g++", "-O2", "-shared", "-fPIC", "-I", os.path.join(ROOT, "easevoice-trainer_b200", "csrc"), "-o", so,
+                    str(d / "shim.cpp")], check=True)
+    fn = ctypes.CDLL(so).dgrad_phase_c
+    fn.argtypes = [ctypes.c_int] * 6 + [ctypes.POINTER(ctypes.c_int)]
+
+    def plan(Q, s, pad, dil, Tin):
+        """-> [(u0, Ju, q0, nq, off)] over the tap residues, as evk_gconv_dgrad launches them"""
+        out, phases = (ctypes.c_int * 64)(), []
+        for rho in range(s):
+            if fn(Q, s, pad, dil, Tin, rho, out):
+                phases.append((out[0], out[1], out[2], out[3], list(out[4:4 + out[3]])))
+        return phases
+    return plan
+
+
+def test_library_dgrad_plan_covers_every_tap_exactly_once(dgrad_plan):
     for Q, s, pad, dil, Tin in [(5, 3, 2, 1, 37), (41, 4, 20, 1, 100), (16, 10, 3, 1, 64), (11, 1, 25, 5, 50), (2, 2, 0, 1, 9),
                                 (15, 1, 7, 1, 33), (8, 2, 3, 1, 21)]:
         J = (Tin + 2 * pad - dil * (Q - 1) - 1) // s + 1 if s > 1 or True else 0
@@ -134,7 +181,7 @@ def test_dgrad_phase_plan_covers_every_tap_exactly_once():
                 if 0 <= u < Tin:
                     want.setdefault(u, set()).add((q, j))
         got = {}
-        for u0, Ju, q0, nq, off in dgrad_phase_plan(Q, s, pad, dil, Tin):
+        for u0, Ju, q0, nq, off in dgrad_plan(Q, s, pad, dil, Tin):
             for jj in range(Ju):
                 u = u0 + s * jj
                 assert 0 <= u < Tin

@@ -297,10 +297,11 @@ def test_conv_post_tanh(ops):
     assert (y[..., 1:] == 0).all()
 
 
-@pytest.mark.parametrize("case", R.CONVT_CASES, ids=[f"{a}-{b}-k{k}-s{s}-T{t}" for a, b, k, s, t in R.CONVT_CASES])
+@pytest.mark.parametrize("case", R.CONVT_CASES, ids=["-".join([f"{a}-{b}-k{k}-s{s}-T{t}"] + m) for a, b, k, s, t, *m in R.CONVT_CASES])
 def test_conv_transpose(ops, case):
     """ConvTranspose1d forward: the os / o0 output mapping of the TMA kernel's epilogue; backward on mma.sync"""
-    Cin, Cout, Q, s, T = case
+    (Cin, Cout, Q, s, T), mode = case[:5], case[5:]
+    x0 = 1 if "x+1" in mode else 0
     pad = (Q - s) // 2
     g = torch.Generator().manual_seed(Cin + Q + T)
     x, v, bias = R.ints((2, Cin, T), R.RX, g), R.ints((Cin, Cout, Q), R.RW, g), R.ints((Cout,), R.RB, g)
@@ -311,19 +312,21 @@ def test_conv_transpose(ops, case):
     xr, vr, br = [t.to(DEV).requires_grad_(True) for t in (x, v, bias)]
     yr = R.conv_transpose1d_ref(xr, vr, br, s, pad)
     yr.backward(gy.to(DEV))
-    xd = x.transpose(1, 2).float().to(DEV).requires_grad_(True)
+    xbuf = torch.zeros((2, T, x0 + Cin), device=DEV)
+    xbuf[..., x0:] = x.transpose(1, 2).to(DEV)
+    xbuf.requires_grad_(True)
     vd, bd = v.float().to(DEV).requires_grad_(True), bias.float().to(DEV).requires_grad_(True)
     ops.dispatch_reset()
-    yo = ops.conv_transpose(xd, ops.pack_weight(vd), bd, stride=s, pad=pad)
+    yo = ops.conv_transpose(xbuf[..., x0:], ops.pack_weight(vd), bd, stride=s, pad=pad)
     torch.cuda.synchronize()
-    assert_family(ops, "fwd_gemm_tma" if T >= 1000 else "fwd_gconv_tc", FWD, "convT forward")
+    assert_family(ops, "fwd_direct" if x0 else "fwd_gemm_tma" if T >= 1000 else "fwd_gconv_tc", FWD, "convT forward")
     ops.dispatch_reset()
     yo.backward(gy.transpose(1, 2).float().to(DEV))
     torch.cuda.synchronize()
-    assert_family(ops, "wgrad_mma_sync", WGRAD, "convT weight gradient")
-    n = f"convT[{Cin}->{Cout} k{Q} s{s} T{T}]"
+    assert_family(ops, "wgrad_direct" if x0 else "wgrad_mma_sync", WGRAD, "convT weight gradient")
+    n = f"convT[{Cin}->{Cout} k{Q} s{s} T{T}{' x+1' if x0 else ''}]"
     assert_exact(yo, yr.detach().transpose(1, 2), n + " y", ("b", "t", "n"), {"t": 128, "n": _bn(Cout)})
-    assert_exact(xd.grad, xr.grad.transpose(1, 2), n + " dx", ("b", "t", "c"), {"t": 128})
+    assert_exact(xbuf.grad[..., x0:], xr.grad.transpose(1, 2), n + " dx", ("b", "t", "c"), {"t": 128})
     assert_exact(vd.grad, vr.grad, n + " dW", ("ci", "co", "tap"), None)
     assert_exact(bd.grad, br.grad, n + " dbias", ("n",), None)
 
