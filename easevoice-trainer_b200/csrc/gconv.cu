@@ -11,6 +11,7 @@
 // Linear / matmul call sites (see include/evk.h for file:line).
 #include "dgrad_plan.h"
 #include "evk_common.cuh"
+#include "gemv_route.h"
 
 namespace evk {
 
@@ -438,6 +439,37 @@ static int launch_f(GP& p, cudaStream_t st) {
   return check_launch("gconv_f_kernel");
 }
 
+// The dropout of a launch whose epilogue had none, in place over its outputs: the keep function of gemm_tma_kernel's
+// epilogue, keyed by the output's element offset from y, so the pattern does not depend on the route.
+__global__ void gconv_drop_kernel(const __grid_constant__ GP p, const unsigned long long* rng, unsigned long long sid, float drop_p) {
+  const DropK dk = dropk_make(rng, sid, drop_p);
+  const long long npos = (long long)p.J * p.P, total = (long long)p.Z * npos * p.N;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int n = (int)(i % p.N);
+    const long long r = i / p.N;
+    const int z = (int)(r / npos), pos = (int)(r - z * npos);
+    const int b = z / p.H, h = z - b * p.H, j = pos / p.P, w = pos - j * p.P;
+    const long long e = b * p.y_sb + h * p.y_sh + ((long long)(p.o0 + j * p.os) * p.P + w) * p.ldy + n;
+    float m[4];
+    dropk_scale4(dk, (unsigned long long)e >> 2, m);
+    p.y[e] *= m[e & 3];
+  }
+}
+
+static bool drops(const evk_gconv_desc* d) { return d->drop_rng && d->drop_p > 0.f; }
+
+// rc of the route that served d, then d's dropout when that route's epilogue has none
+static int unfused_drop(int rc, const evk_gconv_desc* d, cudaStream_t st) {
+  if (rc || !drops(d)) return rc;
+  GP p;
+  conv_params(d, p, "gconv_fwd");
+  const long long total = (long long)d->Z * d->J * d->P * d->N;
+  if (total == 0) return EVK_OK;
+  gconv_drop_kernel<<<(unsigned)min((long long)kNumSMs * 16, (total + 255) / 256), 256, 0, st>>>(
+      p, reinterpret_cast<const unsigned long long*>(d->drop_rng), d->drop_sid, d->drop_p);
+  return check_launch("gconv_drop");
+}
+
 }  // namespace evk
 
 using namespace evk;
@@ -453,13 +485,12 @@ static int fwd_tiled(const evk_gconv_desc* d, const evk_gconv_desc* h, cudaStrea
   int rc = conv_params(h, p, "gconv_fwd");
   if (rc) return rc;
   if (h->is == 1 && g_backend_tc && !g_precise) {
-    rc = gemm_tma_try(h, st);
+    rc = gemm_tma_try(h, st);                  // dropout in the epilogue
     if (rc <= 0) { if (rc == 0) g_disp_flops[0] += desc_flops(d); return rc; }
   }
-  EVK_REQUIRE(!(d->drop_rng && d->drop_p > 0.f), EVK_ERR_UNSUPPORTED, "gconv_fwd: fused dropout needs a launch the TMA kernel takes");
   if (g_backend_tc && !g_precise) {
     rc = gconv_tc_try(p, st);
-    if (rc <= 0) { if (rc == 0) g_disp_flops[1] += desc_flops(d); return rc; }
+    if (rc <= 0) { if (rc == 0) g_disp_flops[1] += desc_flops(d); return unfused_drop(rc, d, st); }
   }
   g_disp_flops[2] += desc_flops(d);
   // pick the N tile with the least padding (prefer wide)
@@ -474,13 +505,14 @@ static int fwd_tiled(const evk_gconv_desc* d, const evk_gconv_desc* h, cudaStrea
   }
 #define EVK_F(WM, WN, MF_, NF_) (g_precise ? launch_f<WM, WN, MF_, NF_, true>(p, st) : launch_f<WM, WN, MF_, NF_, false>(p, st))
   switch (best) {
-    case 128: return EVK_F(4, 2, 2, 8);
-    case 64: return EVK_F(4, 2, 2, 4);
-    case 32: return EVK_F(8, 1, 1, 4);
-    case 16: return EVK_F(8, 1, 1, 2);
-    default: return EVK_F(8, 1, 1, 1);
+    case 128: rc = EVK_F(4, 2, 2, 8); break;
+    case 64: rc = EVK_F(4, 2, 2, 4); break;
+    case 32: rc = EVK_F(8, 1, 1, 4); break;
+    case 16: rc = EVK_F(8, 1, 1, 2); break;
+    default: rc = EVK_F(8, 1, 1, 1);
   }
 #undef EVK_F
+  return unfused_drop(rc, d, st);
 }
 
 extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
@@ -488,14 +520,17 @@ extern "C" int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream) {
   int rc = conv_params(d, p, "gconv_fwd");
   if (rc) return rc;
   EVK_REQUIRE(d->y != nullptr && d->x != nullptr && d->w != nullptr, EVK_ERR_ARG, "gconv_fwd: null tensor");
+  EVK_REQUIRE(!drops(d) || d->act == EVK_ACT_RELU, EVK_ERR_ARG, "gconv_fwd: dropout needs act = EVK_ACT_RELU, got %d", d->act);
   cudaStream_t st = (cudaStream_t)stream;
-  evk_gconv_desc h;
-  if (!groups_as_batch(d, h) || !fwd_tileable(&h)) {
-    EVK_REQUIRE(!(d->drop_rng && d->drop_p > 0.f), EVK_ERR_UNSUPPORTED, "gconv_fwd: fused dropout needs a launch the TMA kernel takes");
-    return conv_direct_fwd(d, st);
+  if (gconv_fwd_gemv(d)) {
+    rc = evk_gemv_rows(d->x, d->ldx, d->Z * d->J * d->P, d->w, d->ldw, d->bias, d->y, d->ldy, d->N, d->C, d->act, d->slope, stream);
+    if (rc == 0) g_disp_flops[8] += desc_flops(d);
+    return rc;
   }
+  evk_gconv_desc h;
+  if (!groups_as_batch(d, h) || !fwd_tileable(&h)) return unfused_drop(conv_direct_fwd(d, st), d, st);
   if (h.is > 1 && !g_precise) {
-    rc = gemm_tma_phased(&h, st);
+    rc = gemm_tma_phased(&h, st);                // dropout in the epilogue
     if (rc <= 0) { if (rc == 0) g_disp_flops[0] += desc_flops(d); return rc; }
   }
   return fwd_tiled(d, &h, st);

@@ -1,6 +1,7 @@
 // Stage-1 AR GPT odds and ends: sinusoidal position add (embedding.py:36-81), summed cross-entropy + top-k accuracy
 // (t2s_model.py:486-489), and ScaledAdam (optim.py:123-622) over one flat fp32 arena.
 #include "evk_common.cuh"
+#include "gemv_route.h"
 
 namespace evk {
 namespace {
@@ -546,10 +547,9 @@ extern "C" int evk_gemv_rows(const float* x, int32_t ldx, int32_t rows, const fl
   EVK_REQUIRE(act == EVK_ACT_NONE || act == EVK_ACT_RELU || act == EVK_ACT_LRELU, EVK_ERR_UNSUPPORTED, "gemv_rows: activation %d", act);
   int R = 1;
   while (R < rows) R *= 2;
-  // <= 4 rows: all C channels staged at once (40 KB at most); more rows: chunks of CC channels in a 64 KB staging buffer
-  int CC = C;
-  if (R <= 4) EVK_REQUIRE((size_t)R * C * 4 <= 40 * 1024, EVK_ERR_UNSUPPORTED, "gemv_rows: %d rows of %d channels exceed the staging buffer", R, C);
-  else CC = min(C, (64 * 1024 / 4 / R) & ~3);
+  // <= 4 rows: all C channels staged at once (gemv_rows_fit); more rows: chunks of CC channels in a 64 KB staging buffer
+  EVK_REQUIRE(gemv_rows_fit(rows, C), EVK_ERR_UNSUPPORTED, "gemv_rows: %d rows of %d channels exceed the staging buffer", R, C);
+  const int CC = R <= 4 ? C : min(C, (64 * 1024 / 4 / R) & ~3);
   int KS = 1;
   while (KS < 8 && (long long)N * KS < kNumSMs * 8 && C / 4 >= 64 * KS) KS *= 2;      // enough warps to cover the chip, >= 2 float4 groups per lane
   const int per = 8 / KS;

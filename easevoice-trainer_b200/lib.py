@@ -18,7 +18,8 @@ class GconvDesc(ctypes.Structure):
         + [(n, ctypes.c_int32) for n in ("ldx", "ldw", "ldy", "ldr", "b_sh", "Z", "H", "C", "N", "Q", "G", "Tin", "J", "P",
                                          "is_", "os_", "o0", "Tout", "act")]
         + [("slope", ctypes.c_float), ("off", ctypes.c_int32 * MAX_TAPS)]
-        + [("drop_rng", ctypes.c_void_p), ("drop_sid", ctypes.c_uint64), ("drop_p", ctypes.c_float), ("no_phase_split", ctypes.c_int32)]
+        + [("drop_rng", ctypes.c_void_p), ("drop_sid", ctypes.c_uint64), ("drop_p", ctypes.c_float), ("no_phase_split", ctypes.c_int32),
+           ("no_grad", ctypes.c_int32)]
     )
 
 

@@ -82,7 +82,7 @@ def profile_end():
 
 
 DISPATCH_SLOTS = ("fwd_gemm_tma", "fwd_gconv_tc", "fwd_mma_sync", "fwd_direct", "wgrad_gemm_tma", "wgrad_mma_sync", "wgrad_direct",
-                  "gemm_tf32")
+                  "gemm_tf32", "fwd_gemv")
 
 
 def dispatch_reset():
@@ -206,9 +206,7 @@ def stream_id(tag):
 def _desc(off=(), **kw):
     """-> GconvDesc with the given fields; every other field is zero or null, except H and G, which default to 1.
     Tensors are passed by data pointer, an int pointer field as the raw device address."""
-    d = L.GconvDesc(H=1, G=1)
-    for k, v in kw.items():
-        setattr(d, k, v.data_ptr() if isinstance(v, torch.Tensor) else v)
+    d = L.GconvDesc(**{"H": 1, "G": 1, **{k: v.data_ptr() if isinstance(v, torch.Tensor) else v for k, v in kw.items()}})
     assert len(off) <= L.MAX_TAPS
     for i, o in enumerate(off):
         d.off[i] = int(o)
@@ -462,19 +460,36 @@ def _conv_out_len(Tin, Q, stride, pad, dil):
 
 
 def _fwd_like(x, Tin, w, ldw, w_sq, C, N, y, *, J, P, is_, off, bias=None, res=None, act=0, slope=0.0, in_len=None,
-              out_len=None, G=1, drop=None, no_phase_split=0):
+              out_len=None, G=1, drop=None, no_phase_split=0, no_grad=0):
     """one forward-like launch of the generalised conv, len(off) taps, output rows j < J; evk_gconv_fwd picks the kernel.
-    Grouped convs pass G = groups (C, N are then the total channel counts)."""
+    Grouped convs pass G = groups (C, N are then the total channel counts).  drop = (p, stream id): dropout after the
+    activation (ReLU only).  no_grad: no gradient is taken through the launch, so the library may serve it exactly."""
     B = x.shape[0]
     _, _, ldx = _rows(x)
     _, _, ldy = _rows(y)
     ldr = _rows(res)[2] if res is not None else 0
     d = _desc(x=x, w=w, y=y, res=res, bias=bias, in_len=in_len, out_len=out_len, x_sb=Tin * P * ldx, w_sq=w_sq, y_sb=J * P * ldy,
               r_sb=J * P * ldr, ldx=ldx, ldw=ldw, ldy=ldy, ldr=ldr, Z=B, G=G, C=C, N=N, Q=len(off), Tin=Tin, J=J, P=P, is_=is_,
-              os_=1, Tout=J, act=act, slope=float(slope), off=off, no_phase_split=no_phase_split)
-    if drop is not None:                      # fused dropout after the activation (TMA kernel epilogue only; the library rejects other routes)
+              os_=1, Tout=J, act=act, slope=float(slope), off=off, no_phase_split=no_phase_split, no_grad=no_grad)
+    if drop is not None:
         d.drop_rng, d.drop_sid, d.drop_p = rng_state(x.device).data_ptr(), int(drop[1]), float(drop[0])
     _run_desc("evk_gconv_fwd", d)
+
+
+def _conv_forward(x, pa, bias, res, cfg):
+    """the launch of _ConvFn's forward for a channels-last x: -> y"""
+    Q, stride, pad, dil, P, G, act, slope, in_len, out_len, drop, no_grad = cfg
+    B, R, C = x.shape
+    assert R % P == 0
+    Tin = R // P
+    N, lda = pa.shape[1], pa.shape[2]
+    J = _conv_out_len(Tin, Q, stride, pad, dil)
+    y = torch.empty((B, J * P, N), device=x.device, dtype=torch.float32)
+    if res is not None:
+        res = _cl(res)
+    _fwd_like(x, Tin, pa, lda, N * lda, C, N, y, J=J, P=P, is_=stride, off=[q * dil - pad for q in range(Q)], bias=bias,
+              res=res, act=act, slope=slope, in_len=in_len, out_len=out_len, drop=drop, G=G, no_grad=no_grad)
+    return y
 
 
 class _ConvFn(torch.autograd.Function):
@@ -482,30 +497,19 @@ class _ConvFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, pa, pb, bias, res, cfg):
-        Q, stride, pad, dil, P, G, act, slope, in_len, out_len = cfg[:10]
-        drop = cfg[10] if len(cfg) > 10 else None
         x = _cl(x)
-        B, R, C = x.shape
-        assert R % P == 0
-        Tin = R // P
-        N, lda = pa.shape[1], pa.shape[2]
-        J = _conv_out_len(Tin, Q, stride, pad, dil)
-        y = torch.empty((B, J * P, N), device=x.device, dtype=torch.float32)
-        if res is not None:
-            res = _cl(res)
-        _fwd_like(x, Tin, pa, lda, N * lda, C, N, y, J=J, P=P, is_=stride, off=[q * dil - pad for q in range(Q)], bias=bias,
-                  res=res, act=act, slope=slope, in_len=in_len, out_len=out_len, drop=drop, G=G)
+        y = _conv_forward(x, pa, bias, res, cfg)
+        P, act = cfg[4], cfg[6]
         ctx.cfg = cfg
-        ctx.dims = (B, Tin, C, N, J, lda)
+        ctx.dims = (x.shape[0], x.shape[1] // P, x.shape[2], pa.shape[1], y.shape[1] // P, pa.shape[2])
         ctx.has = (bias is not None, res is not None)
         ctx.save_for_backward(x, pa, pb, y if act else None)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        Q, stride, pad, dil, P, G, act, slope, in_len, out_len = ctx.cfg[:10]
-        drop = ctx.cfg[10] if len(ctx.cfg) > 10 else None
-        # dropout fused after a ReLU: the saved output is zero exactly where the element was dropped or the ReLU was off, so
+        Q, stride, pad, dil, P, G, act, slope, in_len, out_len, drop, _ = ctx.cfg
+        # dropout after a ReLU: the saved output is zero exactly where the element was dropped or the ReLU was off, so
         # the activation backward only needs the extra 1/(1-p) factor -- no mask is regenerated
         gscale = 1.0 / (1.0 - drop[0]) if drop is not None else 1.0
         B, Tin, C, N, J, lda = ctx.dims
@@ -551,69 +555,43 @@ class _ConvFn(torch.autograd.Function):
 
 
 def conv(x, w: PackedW, bias=None, *, stride=1, pad=0, dil=1, P=1, groups=1, act=ACT_NONE, slope=0.0, res=None,
-         in_len=None, out_len=None, precise=False):
-    """Conv1d (P == 1) / Conv2d with (k,1) kernels over a period-folded view (P == period).
-    precise=True: this launch uses 3xTF32 error-compensated products (fp32-class accuracy; forward-only call sites)."""
-    cfg = (w.Q, stride, pad, dil, P, groups, act, slope, in_len, out_len)
-    if precise:
-        lib = _lib()
-        was = lib.evk_get_precise()
-        lib.evk_set_precise(1)           # read when the launch is enqueued (also at graph capture): a per-call switch
-        try:
-            return _ConvFn.apply(x, w.pa, w.pb, bias, res, cfg)
-        finally:
-            lib.evk_set_precise(was)
+         in_len=None, out_len=None):
+    """Conv1d (P == 1) / Conv2d with (k,1) kernels over a period-folded view (P == period)."""
+    cfg = (w.Q, stride, pad, dil, P, groups, act, slope, in_len, out_len, None, 0)
     return _ConvFn.apply(x, w.pa, w.pb, bias, res, cfg)
 
 
-def fused_dropout_ok(x, w, act):
-    """can `linear(..., act=ReLU, drop=...)` fuse the dropout into the GEMM epilogue?  Mirrors the flat-GEMM eligibility of
-    gemm_tma_run (csrc/gemm_tma.cu); the library raises if a launch with dropout requested is not taken by that kernel."""
-    if act != ACT_RELU or x.dim() != 3 or not x.is_contiguous() or _lib().evk_get_precise():
-        return False
-    rows, C, N = x.shape[0] * x.shape[1], x.shape[2], w.D0
-    return w.Q == 1 and rows >= 512 and C >= 64 and C % 4 == 0 and N >= 64 and N % 4 == 0 and x.data_ptr() % 16 == 0
-
-
-def _gemv_rows(x, w, bias, act, slope):
-    """The token step of the KV-cache decode: [..., C] with <= 4 rows in total -> [..., N], exact fp32, one pass over PA[0]."""
+def linear_rows(x, w: PackedW, bias=None, act=ACT_NONE, slope=0.0):
+    """Exact-fp32 Linear of the batched token step: [..., C] with 1..64 rows in total -> [..., N], one pass over the packed
+    weight (evk_gemv_rows).  A row's result does not depend on how many rows share the launch.  No gradient."""
     C = x.shape[-1]
     x2 = x.reshape(-1, C)
     if x2.stride(1) != 1:
         x2 = x2.contiguous()
     rows, N = x2.shape[0], w.pa.shape[1]
+    assert w.Q == 1 and 1 <= rows <= 64 and act in (ACT_NONE, ACT_RELU, ACT_LRELU), (rows, act)
     y = torch.empty(x.shape[:-1] + (N,), device=x.device, dtype=torch.float32)
     _call_f("evk_gemv_rows", 2.0 * rows * N * C, _p(x2), x2.stride(0), rows, _p(w.pa), w.pa.shape[2], _p(bias), _p(y), N, N, C,
             int(act), ctypes.c_float(float(slope)))
     return y
 
 
-def linear_rows(x, w: PackedW, bias=None, act=ACT_NONE, slope=0.0):
-    """Exact-fp32 Linear of the batched token step: [..., C] with 1..64 rows in total -> [..., N], one pass over the packed
-    weight (evk_gemv_rows).  A row's result does not depend on how many rows share the launch.  No gradient."""
-    rows = x.numel() // max(x.shape[-1], 1)
-    assert w.Q == 1 and 1 <= rows <= 64 and act in (ACT_NONE, ACT_RELU, ACT_LRELU), (rows, act)
-    return _gemv_rows(x, w, bias, act, slope)
-
-
 def linear(x, w: PackedW, bias=None, act=ACT_NONE, slope=0.0, out_len=None, in_len=None, res=None, drop=None):
-    """nn.Linear / 1x1 conv on [B, T, C] or [rows, C].  drop = (p, tag): dropout_p(relu(x W^T + b)) with the dropout applied in
-    the GEMM epilogue when fused_dropout_ok (else as a separate kernel)."""
-    # skinny (<= 4 rows, no-grad) launches stream the weight once (evk_gemv_rows)
-    if (not torch.is_grad_enabled() and w.Q == 1 and res is None and out_len is None and in_len is None
-            and (drop is None or drop[0] <= 0.0) and act in (ACT_NONE, ACT_RELU, ACT_LRELU)):
-        C = x.shape[-1]
-        rows = x.numel() // max(C, 1)
-        if 1 <= rows <= 4 and C >= 4 and C % 4 == 0 and C <= w.pa.shape[2] and (1 if rows == 1 else 2 if rows == 2 else 4) * C <= 10240:
-            return _gemv_rows(x, w, bias, act, slope)
+    """nn.Linear / 1x1 conv on [B, T, C] or [rows, C].  drop = (p, tag): dropout_p(relu(x W^T + b)), act must be ReLU.
+    Without autograd recording, the library may serve a launch of a few rows exactly in fp32 (evk_gconv_fwd's route 0)."""
     if drop is not None and drop[0] > 0.0:
-        if fused_dropout_ok(x, w, act) and out_len is None and in_len is None and res is None:
-            cfg = (w.Q, 1, 0, 1, 1, 1, act, slope, None, None, (float(drop[0]), stream_id(drop[1])))
-            return _ConvFn.apply(x, w.pa, w.pb, bias, None, cfg)
-        return dropout(linear(x, w, bias, act, slope, out_len, in_len, res), drop[0], drop[1])
-    if x.dim() == 2:
-        return conv(x.unsqueeze(0), w, bias, act=act, slope=slope, res=res.unsqueeze(0) if res is not None else None).squeeze(0)
-    return conv(x, w, bias, act=act, slope=slope, out_len=out_len, in_len=in_len, res=res)
+        assert act == ACT_RELU, "linear(drop=...) needs act=ACT_RELU: the backward recovers the mask from the saved output"
+        drop = (float(drop[0]), stream_id(drop[1]))
+    else:
+        drop = None
+    no_grad = int(not torch.is_grad_enabled())
+    flat = x.dim() == 2
+    if flat:
+        x, res, in_len, out_len = x.unsqueeze(0), res.unsqueeze(0) if res is not None else None, None, None
+    cfg = (w.Q, 1, 0, 1, 1, 1, act, slope, in_len, out_len, drop, no_grad)
+    # no autograd recording: the launch alone, without the Function's bookkeeping (host time of the skinny decode Linears)
+    y = _conv_forward(_cl(x), w.pa, bias, res, cfg) if no_grad else _ConvFn.apply(x, w.pa, w.pb, bias, res, cfg)
+    return y.squeeze(0) if flat else y
 
 
 class _ConvTFn(torch.autograd.Function):

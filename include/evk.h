@@ -61,21 +61,30 @@ typedef struct evk_gconv_desc {
   int32_t Tout;          /* output positions per batch (bounds for (o0 + j*os)) */
   int32_t act; float slope;
   int32_t off[EVK_MAX_TAPS];
-  /* optional fused dropout AFTER the activation (forward launches taken by gemm_tma_kernel only; any other route returns
-   * EVK_ERR_UNSUPPORTED): y = dropout_p(act(...)); rng = device [seed, offset] (the library's RNG state), sid = stream id. */
+  /* optional dropout AFTER the activation, forward only: y = mask(dropout_p(act(...))); rng = device [seed, offset] (the
+   * library's RNG state), sid = stream id; active when drop_rng && drop_p > 0, and then act must be EVK_ACT_RELU (EVK_ERR_ARG
+   * otherwise: a backward recovers the mask from the saved output).  The output at element offset e from y is kept (scaled
+   * by 1/(1-p)) or dropped by dropk_scale4(e / 4)[e % 4] (csrc/evk_common.cuh), whatever route serves the launch: routes 1
+   * and 2 apply it in gemm_tma_kernel's epilogue, every other route in one in-place pass over y after the launch. */
   const uint64_t* drop_rng; uint64_t drop_sid; float drop_p;
   /* 1: not route 1 of evk_gconv_fwd.  ConvTranspose1d's data gradient, which has always run on gconv_f_kernel: route 1
    * would take it for the HiFi-GAN generator's stride-2 upsampling layers (128 -> 64, 64 -> 32) and change their bits. */
   int32_t no_phase_split;
+  /* 1: the caller takes no gradient through this launch, so route 0 of evk_gconv_fwd may serve it exactly in fp32. */
+  int32_t no_grad;
 } evk_gconv_desc;
 
 /* Any stride and alignment; groups as G.  Routes, the first that takes the launch runs it:
+ *   0. no_grad, a Linear of 1 <= Z*J*P <= 4 dense rows (Q == 1, off[0] == 0, is == os == 1, o0 == 0, J <= Tin, G <= 1,
+ *      H == 1, x_sb == J*P*ldx and y_sb == J*P*ldy unless Z == 1), no res, in_len, out_len or dropout, act NONE / RELU /
+ *      LRELU, 4 <= C <= ldw, C % 4 == 0, ldw % 4 == 0, w 16-byte aligned, ldx >= C, ldy >= N, within evk_gemv_rows'
+ *      staging limit: evk_gemv_rows, exact fp32 (the rule is gconv_fwd_gemv in csrc/gemv_route.h);
  *   1. 1 < is <= 4, no_phase_split == 0, G <= 1, H == 1, no in_len, C % 4 == 0, C, N >= 32, Z*J*P >= 2048, J*P >= 64:
  *      x split into `is` phase copies (library scratch), then a stride-1 tap sum over them on gemm_tma_kernel;
  *   2. stride 1 on gemm_tma_kernel (shape rule in gemm_tma_plan);  3. stride 1 on gconv_tc_kernel;  4. gconv_f_kernel;
  *   5. the direct kernel when X or W is not 16-byte tileable (x, w 16-byte aligned, ldx, ldw and strides multiples of 4).
  * Routes 2-4 run groups as the inner batch.  Precise mode skips 1-3, evk_set_backend(0) 2-3, evk_set_backend_tma(0) 1-2.
- * Fused dropout (drop_p > 0) needs route 1 or 2.  Route 1 checks all of gemm_tma_kernel's conditions before it splits x. */
+ * Route 1 checks all of gemm_tma_kernel's conditions before it splits x. */
 int evk_gconv_fwd(const evk_gconv_desc* d, evk_stream_t stream);
 int evk_gconv_desc_size(void);         /* sizeof(evk_gconv_desc) as compiled: bindings check their mirror against it */
 /* 0 (default): one TF32 product per MAC.  1: 3xTF32 error-compensated products (~fp32 accuracy, 3x tensor work);
@@ -89,12 +98,13 @@ int evk_set_backend(int32_t tensor_core);
  *   0 conv/linear fwd-like on gemm_tma_kernel (TMA + wgmma)   1 ... on gconv_tc_kernel (wgmma, staged slab)
  *   2 ... on gconv_f_kernel (mma.sync)                          3 ... on the direct CUDA-core kernels
  *   4 weight gradients on gemm_tma_kernel                        5 ... on gconv_w_kernel (mma.sync)
- *   6 ... on the direct kernels                                  7 plain evk_gemm_tf32 calls */
+ *   6 ... on the direct kernels                                  7 plain evk_gemm_tf32 calls
+ *   8 conv/linear fwd-like on evk_gemv_rows (route 0 of evk_gconv_fwd) */
 /* A/B switches of gemm_tma_kernel: slab (default 1) = stride-1 tap sums stage one input slab per channel block and run every
  * tap from it; mt2 (default 1) = 256-row tiles where the persistent grid's wave quantisation allows; trunc_comp (default
  * 3.52e-4) = accumulator compensation per raw fp32 operand for the tensor core's TF32 operand truncation (0 disables). */
 int evk_set_tma_options(int32_t slab, int32_t mt2, float trunc_comp);
-#define EVK_DISPATCH_SLOTS 8
+#define EVK_DISPATCH_SLOTS 9
 int evk_dispatch_stats(double* out, int32_t n);
 int evk_dispatch_stats_reset(void);
 /* Weight gradient of the same operator:  W[z][q][n][c] += sum_{j,w} Yg[z][orow][n] * X[z][irow][c]
@@ -418,7 +428,8 @@ int evk_sinepos_bwd(const float* dy, int32_t ldy, int64_t dy_sb, const float* pe
 /* Skinny Linear of the KV-cache token step (decode_next_token, t2s_model.py:187-221: one new row per utterance):
  * y[r][n] = act(sum_c x[r][c] * W[n][c] + bias[n]) for rows <= 64; W = the packed forward operand PA[0] ([N][ldw], row n = output
  * channel n).  Exact fp32 FMAs, one pass over W.  A row's result does not depend on `rows` (same summation order for every
- * batch size).  rows <= 4 requires rows_rounded_up_to_a_power_of_2 * C <= 10240.  act: EVK_ACT_NONE / RELU / LRELU. */
+ * batch size).  rows <= 4 requires rows_rounded_up_to_a_power_of_2 * C * 4 bytes <= 40 KB (gemv_rows_fit in csrc/gemv_route.h).
+ * act: EVK_ACT_NONE / RELU / LRELU. */
 int evk_gemv_rows(const float* x, int32_t ldx, int32_t rows, const float* W, int32_t ldw, const float* bias, float* y,
                   int32_t ldy, int32_t N, int32_t C, int32_t act, float slope, evk_stream_t stream);
 /* KV-cache attention of one new token -- T2SBlock.decode_next_token (t2s_model.py:203-221), F.scaled_dot_product_attention

@@ -496,8 +496,14 @@ def check_fused_dropout():
     b = (torch.randn(256, generator=g) * 0.1).to(DEV)
     gy = torch.randn(4, 256, 256, generator=g).to(DEV)
     xa, va, ba = [t.clone().requires_grad_(True) for t in (x, v, b)]
-    yf = ops.linear(xa, ops.pack_weight(va, None), ba, act=ops.ACT_RELU, drop=(p, "chk.drop.lin"))
-    out.append(("fused dropout taken by the GEMM epilogue", 0.0 if ops.fused_dropout_ok(x, ops.pack_weight(v, None), ops.ACT_RELU) else 1.0, 0.5))
+    pw = ops.pack_weight(va, None)
+    ops.dispatch_reset()
+    yf = ops.linear(xa, pw, ba, act=ops.ACT_RELU, drop=(p, "chk.drop.lin"))
+    # TF32 mode: the dropout is fused into gemm_tma_kernel's epilogue; 3xTF32 mode runs mma.sync and then the dropout pass
+    want = "fwd_mma_sync" if PRECISE_MODE[0] else "fwd_gemm_tma"
+    disp = ops.dispatch_stats()
+    served = disp[want] > 0 and not any(disp[k] for k in ops.DISPATCH_SLOTS if k.startswith("fwd_") and k != want)
+    out.append((f"linear + ReLU + dropout served by {want}", 0.0 if served else 1.0, 0.5))
     yf.backward(gy)
     xb, vb, bb = [t.clone().requires_grad_(True) for t in (x, v, b)]
     yp = ops.linear(xb, ops.pack_weight(vb, None), bb, act=ops.ACT_RELU)

@@ -16,7 +16,7 @@ EXACT_BOUND = 2 ** 20
 # value ranges (inclusive, symmetric): activations, weights, upstream gradients, bias / residual
 RX, RW, RDY, RB = 3, 2, 2, 4
 LRELU_SLOPE = 0.25            # exact in binary: the leaky-ReLU derivative keeps gradients on a grid of 1/4
-ACT_NONE, ACT_LRELU, ACT_RELU, ACT_TANH = 0, 1, 2, 3
+ACT_NONE, ACT_LRELU, ACT_RELU, ACT_TANH, ACT_GELU = 0, 1, 2, 3, 4
 
 
 def ints(shape, r, gen, lo=None):
@@ -80,6 +80,22 @@ SPLITK_CASES = [(512, 384, 8192, 8), (200, 130, 1000, 5), (129, 64, 4096, 2), (3
 # Linear (1x1 conv) through evk_gconv_fwd on the flat GEMM path: B, T, C, N, epilogue (B > 1 folds into rows)
 LINEAR_CASES = [(1, 512, 64, 64, "brr"), (3, 171, 68, 96, "lrelu"), (1, 4097, 512, 1536, "none"), (4, 1024, 512, 96, "brr"),
                 (2, 2049, 68, 1536, "lrelu")]
+# Linear launches of a few rows on both sides of each rule of evk_gconv_fwd's route 0 (evk_gemv_rows, exact fp32): name, B, T,
+# C, N, act, residual, no_grad, dispatch slot.  The staging limit is pow2(rows) * C <= 10240 (rows 3 count as 4).
+GEMV_CASES = [
+    ("rows 4", 1, 4, 512, 96, ACT_RELU, False, True, "fwd_gemv"),
+    ("rows 5", 1, 5, 512, 96, ACT_RELU, False, True, "fwd_gconv_tc"),
+    ("rows 4 as batch", 4, 1, 512, 96, ACT_LRELU, False, True, "fwd_gemv"),
+    ("rows 3 C 2560", 1, 3, 2560, 96, ACT_NONE, False, True, "fwd_gemv"),
+    ("rows 3 C 2564", 1, 3, 2564, 96, ACT_NONE, False, True, "fwd_gconv_tc"),
+    ("rows 1 C 10240", 1, 1, 10240, 64, ACT_NONE, False, True, "fwd_gemv"),
+    ("rows 1 C 10244", 1, 1, 10244, 64, ACT_NONE, False, True, "fwd_gconv_tc"),
+    ("C 64", 1, 2, 64, 96, ACT_NONE, False, True, "fwd_gemv"),
+    ("C 66", 1, 2, 66, 96, ACT_NONE, False, True, "fwd_direct"),
+    ("grad enabled", 1, 2, 512, 96, ACT_RELU, False, False, "fwd_gconv_tc"),
+    ("res", 1, 2, 512, 96, ACT_RELU, True, True, "fwd_gconv_tc"),
+    ("gelu", 1, 2, 512, 96, ACT_GELU, False, True, "fwd_gconv_tc"),
+]
 
 # Conv cases through ops.conv: name, B, Tin, C, N, Q, stride, pad, dil, P, groups, act, res, masks ("" / "out" / "inout"),
 # forward family, data-gradient family (None: not asserted; "-": no backward, e.g. tanh), weight-gradient family,

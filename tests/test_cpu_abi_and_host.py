@@ -26,13 +26,14 @@ def test_library_exports_every_symbol_declared_in_header():
 
 def test_descriptor_struct_layout():
     from easevoice_trainer_b200 import lib
-    # 7 pointers + 9 int64 + 19 int32 + float + int32[48] + (pointer, uint64, float) of the fused-dropout request + int32
-    # no_phase_split, padded to 8 bytes
-    expect = 7 * 8 + 9 * 8 + 19 * 4 + 4 + 48 * 4 + 8 + 8 + 4 + 4
-    assert ctypes.sizeof(lib.GconvDesc) == (expect + 7) // 8 * 8
+    # 7 pointers + 9 int64 + 19 int32 + float + int32[48] + (pointer, uint64, float) of the dropout request + int32
+    # no_phase_split + int32 no_grad, padded to 8 bytes
+    expect = 7 * 8 + 9 * 8 + 19 * 4 + 4 + 48 * 4 + 8 + 8 + 4 + 4 + 4
+    assert ctypes.sizeof(lib.GconvDesc) == (expect + 7) // 8 * 8 == 432
     assert lib.GconvDesc.off.offset == 7 * 8 + 9 * 8 + 19 * 4 + 4
     assert lib.GconvDesc.drop_rng.offset == 400 and lib.GconvDesc.drop_sid.offset == 408 and lib.GconvDesc.drop_p.offset == 416
-    assert lib.GconvDesc.no_phase_split.offset == 420                                 # fills the tail padding: the size is unchanged
+    assert lib.GconvDesc.no_phase_split.offset == 420
+    assert lib.GconvDesc.no_grad.offset == 424
     assert lib.load().evk_gconv_desc_size() == ctypes.sizeof(lib.GconvDesc)          # the compiled header agrees with the ctypes mirror
 
 
@@ -327,3 +328,61 @@ def test_bench_reference_arm_prints_one_json_line():
     assert d["impl"] == "reference" and d["higher_is_better"] is True and d["n_gpus"] == 1
     assert d["metric"].startswith("s2 SoVITS+HiFiGAN") and d["unit"] == "audio-s/s" and d["value"] > 0
     assert d["cpu_baseline"]["kind"] == "port" and d["cpu_baseline"]["cores"] >= 1 and d["e2e"]["h2d_bytes_per_step"] == 0
+
+
+_GEMV_SHIM = r"""
+#include "gemv_route.h"
+extern "C" int gemv_route_c(const evk_gconv_desc* d) { return evk::gconv_fwd_gemv(d) ? 1 : 0; }
+"""
+
+
+def test_library_gemv_route_keeps_the_python_rule(tmp_path):
+    """Route 0 of evk_gconv_fwd (csrc/gemv_route.h, compiled for the host) takes exactly the Linear launches that ops.linear
+    sent to evk_gemv_rows before the rule moved into the library, for descriptors as ops.linear builds them."""
+    from easevoice_trainer_b200 import lib, ops
+    (tmp_path / "shim.cpp").write_text(_GEMV_SHIM)
+    so = str(tmp_path / "libgemv_route.so")
+    subprocess.run(["g++", "-O2", "-shared", "-fPIC", "-I", os.path.join(ROOT, "easevoice-trainer_b200", "csrc"), "-o", so,
+                    str(tmp_path / "shim.cpp")], check=True)
+    route = ctypes.CDLL(so).gemv_route_c
+    route.argtypes = [ctypes.POINTER(lib.GconvDesc)]
+
+    def python_rule(rows, C, ldw, act, no_grad, res, out_len, in_len, drop):
+        """ops.linear's skinny-row condition as it stood before the move (packed weights: Q == 1, ldw % 4 == 0, aligned)"""
+        pow2 = 1 if rows == 1 else 2 if rows == 2 else 4
+        return (no_grad and not res and not out_len and not in_len and not drop and act in (ops.ACT_NONE, ops.ACT_RELU, ops.ACT_LRELU)
+                and 1 <= rows <= 4 and C >= 4 and C % 4 == 0 and C <= ldw and pow2 * C <= 10240)
+
+    n = taken = 0
+    for B, T in ((1, 1), (1, 2), (2, 1), (1, 3), (3, 1), (2, 2), (1, 4), (4, 1), (1, 5), (5, 1), (2, 3), (1, 64)):
+        rows = B * T
+        for C in (1, 2, 3, 4, 6, 8, 510, 512, 2048, 2556, 2560, 2564, 3412, 3416, 5120, 5124, 10240, 10244):
+            for ldw in sorted({C, C + 2, C + 4, (C + 3) // 4 * 4, C - 4 if C > 4 else C}):
+                if ldw % 4:
+                    continue                                   # packed weights: lda is a multiple of 4 (or < 4 with C < 4)
+                for act in (ops.ACT_NONE, ops.ACT_RELU, ops.ACT_LRELU, ops.ACT_TANH, ops.ACT_GELU):
+                    for flags in range(32):
+                        no_grad, res, out_len, in_len, drop = [(flags >> k) & 1 for k in range(5)]
+                        if drop and act != ops.ACT_RELU:
+                            continue                           # the library rejects these launches before routing
+                        N = 96
+                        # as _fwd_like builds it: x [B, T, C] dense with pitch C, y [B, T, N], res [B, T, N]
+                        d = ops._desc(x=0x10000, w=0x20000, y=0x30000, res=0x40000 if res else 0, out_len=0x50000 if out_len else 0,
+                                      in_len=0x60000 if in_len else 0, x_sb=T * C, w_sq=N * ldw, y_sb=T * N, r_sb=T * N if res else 0,
+                                      ldx=C, ldw=ldw, ldy=N, ldr=N if res else 0, Z=B, C=C, N=N, Q=1, Tin=T, J=T, P=1, is_=1,
+                                      os_=1, Tout=T, act=act, off=[0], no_grad=no_grad)
+                        if drop:
+                            d.drop_rng, d.drop_sid, d.drop_p = 0x70000, 1, 0.1
+                        want = python_rule(rows, C, ldw, act, no_grad, res, out_len, in_len, drop)
+                        assert bool(route(ctypes.byref(d))) == want, (B, T, C, ldw, act, flags)
+                        n += 1
+                        taken += want
+    assert n > 10000 and taken > 100, (n, taken)
+    # what the Python rule never saw: a misaligned or unevenly pitched weight, and rows that are not evenly spaced
+    d = ops._desc(x=0x10000, w=0x20004, y=0x30000, x_sb=2 * 64, w_sq=96 * 64, y_sb=2 * 96, ldx=64, ldw=64, ldy=96, Z=2, C=64, N=96, Q=1,
+                  Tin=2, J=2, P=1, is_=1, os_=1, Tout=2, off=[0], no_grad=1)
+    assert not route(ctypes.byref(d))
+    d.w = 0x20000
+    assert route(ctypes.byref(d))
+    d.x_sb = 3 * 64
+    assert not route(ctypes.byref(d))

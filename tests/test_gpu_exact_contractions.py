@@ -22,7 +22,7 @@ pytestmark = pytest.mark.gpu
 
 DEV = torch.device("cuda", 0)
 TRUNC_COMP = 3.52e-4                   # the library's default compensation per truncated operand
-FWD = ("fwd_gemm_tma", "fwd_gconv_tc", "fwd_mma_sync", "fwd_direct")
+FWD = ("fwd_gemm_tma", "fwd_gconv_tc", "fwd_mma_sync", "fwd_direct", "fwd_gemv")
 WGRAD = ("wgrad_gemm_tma", "wgrad_mma_sync", "wgrad_direct")
 NAN = float("nan")
 
@@ -177,6 +177,38 @@ def test_linear_flat(ops, case):
     assert_exact(y, ref, f"linear B{B} T{T} C{C} N{N} {epi}", ("b", "t", "n"), {"n": _bn(N)})
 
 
+# the dropout of a Linear on every route of evk_gconv_fwd: route name -> dispatch slot
+DROP_ROUTES = {"tma": "fwd_gemm_tma", "gconv_tc": "fwd_gconv_tc", "mma_sync": "fwd_mma_sync", "precise": "fwd_mma_sync",
+               "direct": "fwd_direct"}
+
+
+def _dropout_linear(ops, L, route):
+    """-> (y, 2 relu(pre)) of linear + ReLU + dropout(0.5) with the same seed and tag, on the given route"""
+    B, T, C, N = 2, 1000, 64, 96
+    g = torch.Generator().manual_seed(5)
+    x, w, bias = R.ints((B, T, C), R.RX, g), R.ints((N, C), R.RW, g), R.ints((N,), R.RB, g)
+    xd = x.float().to(DEV)
+    if route == "direct":                                # x one float into its buffer: not 16-byte aligned
+        buf = torch.empty(xd.numel() + 1, device=DEV)
+        buf[1:] = xd.flatten()
+        xd = buf[1:].view(B, T, C)
+    {"gconv_tc": lambda: L.evk_set_backend_tma(0), "mma_sync": lambda: L.evk_set_backend(0),
+     "precise": lambda: L.evk_set_precise(1)}.get(route, lambda: None)()
+    try:
+        with torch.no_grad():
+            pw = ops.pack_weight(w.float().to(DEV).unsqueeze(-1))
+            ops.manual_seed(11)
+            ops.dispatch_reset()
+            y = ops.linear(xd, pw, bias.float().to(DEV), act=ops.ACT_RELU, drop=(0.5, "exact-dropout"))
+            torch.cuda.synchronize()
+    finally:
+        L.evk_set_precise(0)
+        L.evk_set_backend(1)
+        L.evk_set_backend_tma(1)
+    keep = 2.0 * torch.relu(x.reshape(-1, C).to(DEV) @ w.to(DEV).t() + bias.to(DEV)).reshape(B, T, N)
+    return y.double(), keep
+
+
 def test_linear_fused_dropout(ops):
     """the DROP instantiation of the fast epilogue: every output is 0 or exactly 2 relu(pre) at p = 0.5"""
     B, T, C, N = 2, 1000, 64, 96
@@ -196,6 +228,65 @@ def test_linear_fused_dropout(ops):
     live = keep > 0
     frac = float((y[live] != 0).double().mean())
     assert 0.45 < frac < 0.55, frac
+
+
+@pytest.mark.parametrize("route", [r for r in DROP_ROUTES if r != "tma"])
+def test_linear_dropout_pass(ops, exact_mode, route):
+    """the routes whose epilogue has no dropout: the pass after the launch leaves every output 0 or exactly 2 relu(pre)"""
+    y, keep = _dropout_linear(ops, exact_mode, route)
+    assert_family(ops, DROP_ROUTES[route], FWD, f"dropout linear on {route}")
+    ok = (y == 0) | (y == keep)
+    assert ok.all(), f"{int((~ok).sum())} outputs are neither dropped nor 2 relu(pre); first at {(~ok).nonzero()[0].tolist()}"
+    live = keep > 0
+    frac = float((y[live] != 0).double().mean())
+    assert 0.45 < frac < 0.55, frac
+
+
+def test_linear_dropout_mask_is_the_same_on_every_route(ops, exact_mode):
+    """the keep pattern depends on (seed, offset, stream id, output index) only, not on the kernel that computed y"""
+    dropped = {}
+    for route in DROP_ROUTES:
+        y, keep = _dropout_linear(ops, exact_mode, route)
+        dropped[route] = (y == 0) & (keep > 0)
+    first = dropped["tma"]
+    assert first.any()
+    for route, d in dropped.items():
+        assert torch.equal(d, first), f"{route}: {int((d != first).sum())} positions dropped differently from the TMA epilogue"
+
+
+def test_dropout_needs_relu(ops):
+    """the library rejects dropout after any activation but ReLU (a backward recovers the mask from the saved output)"""
+    x = torch.ones(1, 600, 64, device=DEV)
+    pw = ops.pack_weight(torch.ones(64, 64, 1, device=DEV))
+    y = torch.empty(1, 600, 64, device=DEV)
+    with pytest.raises(RuntimeError, match="error -1.*EVK_ACT_RELU"):
+        ops._fwd_like(x, 600, pw.pa, pw.pa.shape[2], 64 * pw.pa.shape[2], 64, 64, y, J=600, P=1, is_=1, off=[0],
+                      act=ops.ACT_GELU, drop=(0.5, ops.stream_id("exact-dropout")))
+
+
+# ---- Linear of a few rows: route 0 (evk_gemv_rows) or a TF32 route ---------------------------------------------------------
+@pytest.mark.parametrize("case", R.GEMV_CASES, ids=[c[0].replace(" ", "_") for c in R.GEMV_CASES])
+def test_linear_skinny_route(ops, case):
+    name, B, T, C, N, act, use_res, no_grad, fam = case
+    g = torch.Generator().manual_seed(B * 100 + T + C)
+    x, w, bias, res = R.ints((B, T, C), R.RX, g), R.ints((N, C), R.RW, g), R.ints((N,), R.RB, g), R.ints((B, T, N), R.RB, g)
+    assert_bound(R.gemm_case_bound(C), name)
+    with torch.no_grad():
+        pw = ops.pack_weight(w.float().to(DEV).unsqueeze(-1))
+    with torch.set_grad_enabled(not no_grad):
+        ops.dispatch_reset()
+        y = ops.linear(x.float().to(DEV), pw, bias.float().to(DEV), act=act, slope=R.LRELU_SLOPE,
+                       res=res.float().to(DEV) if use_res else None)
+        torch.cuda.synchronize()
+    assert_family(ops, fam, FWD, name)
+    wr = pw.pa[0, :N, :C].double()                      # the operand the kernels read
+    pre = (x.reshape(-1, C).to(DEV) @ wr.t() + bias.to(DEV)).reshape(B, T, N) + (res.to(DEV) if use_res else 0)
+    if act == R.ACT_GELU:
+        ref = torch.nn.functional.gelu(pre)
+        err = float(((y.double() - ref).abs() / (ref.abs() + 1)).max())
+        assert err < 1e-6, f"{name}: GELU epilogue off by {err}"
+    else:
+        assert_exact(y, R.act_ref(pre, act), name, ("b", "t", "n"))
 
 
 # ---- convolutions through ops.conv --------------------------------------------------------------------------------------
