@@ -42,13 +42,20 @@ __global__ void sinepos_bwd_kernel(const float* __restrict__ dy, int ldy, long l
 }
 
 // ------------------------------------------------------------------------------------------------
+// position r % T of row r counts unless count is given and r % T >= *count (see evk_ce_fwd_ex)
+__device__ __forceinline__ bool counted(int row, const int* count, int T) { return count == nullptr || row % T < *count; }
+
 // one warp per row: lse, nll, top-k hit (count of logits strictly above the target logit < k), valid = target != ignore
 __global__ void ce_fwd_kernel(const float* __restrict__ logits, int ld, const long long* __restrict__ tgt, int rows, int V,
-                              int topk, long long ignore, float* __restrict__ lse, float* __restrict__ nll,
-                              unsigned char* __restrict__ flags) {
+                              int topk, long long ignore, const int* __restrict__ count, int T, float* __restrict__ lse,
+                              float* __restrict__ nll, unsigned char* __restrict__ flags) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
+  if (!counted(row, count, T)) {                               // past the counted length: no loss, not valid, not a hit
+    if (lane == 0) { lse[row] = 0.f; nll[row] = 0.f; flags[row] = 0; }
+    return;
+  }
   const float* l = logits + (size_t)row * ld;
   const long long tg = tgt[row];
   float mx = -INFINITY;
@@ -96,27 +103,31 @@ __global__ void ce_finalize_kernel(const float* __restrict__ nll, const unsigned
 // dlogits[row][c] = gscale * (exp(l - lse) - [c == tgt])
 __global__ void ce_bwd_kernel(const float* __restrict__ logits, int ld, const long long* __restrict__ tgt,
                               const float* __restrict__ lse, const float* __restrict__ gscale, int rows_per_g,
-                              float* __restrict__ dl, int lddl, int rows, int V) {
+                              const int* __restrict__ count, int T, float* __restrict__ dl, int lddl, int rows, int V) {
   const long long n = (long long)rows * V;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     int c = (int)(i % V);
     int r = (int)(i / V);
+    if (!counted(r, count, T)) { dl[(size_t)r * lddl + c] = 0.f; continue; }
     float p = expf(logits[(size_t)r * ld + c] - lse[r]);
     dl[(size_t)r * lddl + c] = gscale[r / rows_per_g] * (p - ((long long)c == tgt[r] ? 1.f : 0.f));
   }
 }
 
 // DPO head (t2s_model.py:421-427, utils.py:160-192, reference_free, beta): A_b = -sum_t nll_c[b][t], R_b = -sum_t nll_r[b][t]
+//   (t < min(Yc, *count_c) / t < min(Yr, *count_r) when the counts are given)
 //   loss_2 = mean_b softplus(-beta (A_b - R_b));   out3 = (loss_1 = sum nll_c, loss_2, loss_1 + loss_2)
 //   coef_c[b] = d total / d nll_c[b][t] = 1 + beta * sigmoid(-beta (A_b - R_b)) / B ;  coef_r[b] = -(coef_c[b] - 1)
-__global__ void dpo_head_kernel(const float* __restrict__ nll_c, int Yc, const float* __restrict__ nll_r, int Yr, int B, float beta,
-                                float* __restrict__ out3, float* __restrict__ coef_c, float* __restrict__ coef_r) {
+__global__ void dpo_head_kernel(const float* __restrict__ nll_c, int Yc, const int* __restrict__ count_c, const float* __restrict__ nll_r,
+                                int Yr, const int* __restrict__ count_r, int B, float beta, float* __restrict__ out3,
+                                float* __restrict__ coef_c, float* __restrict__ coef_r) {
   __shared__ float red[33];
+  const int nc = count_c ? min(Yc, *count_c) : Yc, nr = count_r ? min(Yr, *count_r) : Yr;
   float l1 = 0.f, l2 = 0.f;
   for (int b = 0; b < B; ++b) {
     float sc = 0.f, sr = 0.f;
-    for (int t = threadIdx.x; t < Yc; t += blockDim.x) sc += nll_c[(size_t)b * Yc + t];
-    for (int t = threadIdx.x; t < Yr; t += blockDim.x) sr += nll_r[(size_t)b * Yr + t];
+    for (int t = threadIdx.x; t < nc; t += blockDim.x) sc += nll_c[(size_t)b * Yc + t];
+    for (int t = threadIdx.x; t < nr; t += blockDim.x) sr += nll_r[(size_t)b * Yr + t];
     sc = block_sum(sc, red);
     sr = block_sum(sr, red);
     const float z = -beta * ((-sc) - (-sr));                 // -beta (A - R)
@@ -437,6 +448,19 @@ __global__ void __launch_bounds__(256) gemv_rows_kernel(const float* __restrict_
   }
 }
 
+// DPO rejected rows (evk_dpo_reject_rows): one CTA per row b, out[b][t] = y[b][t] for t < i1, y[b][t - (i1 - i0)] for
+// i1 <= t < Yc + i1 - i0, 0 after; spans are clamped into [0, Yc] so a bad span never reads outside the row
+__global__ void dpo_reject_rows_kernel(const long long* __restrict__ y, int ldy, const int* __restrict__ spans,
+                                       const int* __restrict__ yc, long long* __restrict__ out, int Yr, long long* __restrict__ lens) {
+  const int b = blockIdx.x;
+  const int Yc = min(max(*yc, 0), ldy);
+  const int i0 = min(max(spans[2 * b], 0), Yc), i1 = min(max(spans[2 * b + 1], i0), Yc);
+  const int d = i1 - i0, L = Yc + d;
+  const long long* src = y + (size_t)b * ldy;
+  for (int t = threadIdx.x; t < Yr; t += blockDim.x) out[(size_t)b * Yr + t] = t < i1 ? src[t] : (t < L ? src[t - d] : 0ll);
+  if (threadIdx.x == 0) lens[b] = L;
+}
+
 // cache[b][*pos][0 .. W) = row[b][0 .. W): the position comes from device memory so that the step can be a replayed CUDA graph
 __global__ void cache_append_kernel(const float* __restrict__ row, int ldr, float* __restrict__ cache, long long sb, int ld,
                                     const int* __restrict__ pos, int W) {
@@ -472,28 +496,54 @@ extern "C" int evk_sinepos_bwd(const float* dy, int ldy, int64_t dy_sb, const fl
   return ordered_sum(part, blocks, 1, 1, 1, dalpha, 0, 0, st);
 }
 
-extern "C" int evk_ce_fwd(const float* logits, int ld, const int64_t* targets, int rows, int V, int topk, int64_t ignore_index,
-                          float* lse, float* nll, uint8_t* flags, float* out2, cudaStream_t st) {
+extern "C" int evk_ce_fwd_ex(const float* logits, int ld, const int64_t* targets, int rows, int V, int topk, int64_t ignore_index,
+                             const int32_t* count, int T, float* lse, float* nll, uint8_t* flags, float* out2, cudaStream_t st) {
   EVK_REQUIRE(rows > 0 && V > 0, EVK_ERR_ARG, "ce_fwd: empty");
-  ce_fwd_kernel<<<cdiv(rows, 8), 256, 0, st>>>(logits, ld, (const long long*)targets, rows, V, topk, ignore_index, lse, nll, flags);
+  EVK_REQUIRE(!count || (T > 0 && rows % T == 0), EVK_ERR_ARG, "ce_fwd: %d rows are not whole rows of T = %d positions", rows, T);
+  ce_fwd_kernel<<<cdiv(rows, 8), 256, 0, st>>>(logits, ld, (const long long*)targets, rows, V, topk, ignore_index, count, T, lse,
+                                               nll, flags);
   if (int rc = check_launch("ce_fwd")) return rc;
   ce_finalize_kernel<<<1, 1024, 0, st>>>(nll, flags, rows, out2);
   return check_launch("ce_finalize");
 }
 
+extern "C" int evk_ce_fwd(const float* logits, int ld, const int64_t* targets, int rows, int V, int topk, int64_t ignore_index,
+                          float* lse, float* nll, uint8_t* flags, float* out2, cudaStream_t st) {
+  return evk_ce_fwd_ex(logits, ld, targets, rows, V, topk, ignore_index, nullptr, 1, lse, nll, flags, out2, st);
+}
+
+extern "C" int evk_dpo_head_ex(const float* nll_c, int Yc, const int32_t* count_c, const float* nll_r, int Yr, const int32_t* count_r,
+                               int B, float beta, float* out3, float* coef_c, float* coef_r, cudaStream_t st) {
+  EVK_REQUIRE(B > 0 && Yc > 0 && Yr > 0, EVK_ERR_ARG, "dpo_head: empty");
+  dpo_head_kernel<<<1, 256, 0, st>>>(nll_c, Yc, count_c, nll_r, Yr, count_r, B, beta, out3, coef_c, coef_r);
+  return check_launch("dpo_head");
+}
+
 extern "C" int evk_dpo_head(const float* nll_c, int Yc, const float* nll_r, int Yr, int B, float beta, float* out3, float* coef_c,
                             float* coef_r, cudaStream_t st) {
-  EVK_REQUIRE(B > 0 && Yc > 0 && Yr > 0, EVK_ERR_ARG, "dpo_head: empty");
-  dpo_head_kernel<<<1, 256, 0, st>>>(nll_c, Yc, nll_r, Yr, B, beta, out3, coef_c, coef_r);
-  return check_launch("dpo_head");
+  return evk_dpo_head_ex(nll_c, Yc, nullptr, nll_r, Yr, nullptr, B, beta, out3, coef_c, coef_r, st);
+}
+
+extern "C" int evk_ce_bwd_ex(const float* logits, int ld, const int64_t* targets, const float* lse, const float* gscale,
+                             int rows_per_g, const int32_t* count, int T, float* dl, int lddl, int rows, int V, cudaStream_t st) {
+  EVK_REQUIRE(rows_per_g > 0, EVK_ERR_ARG, "ce_bwd: rows_per_g");
+  EVK_REQUIRE(!count || (T > 0 && rows % T == 0), EVK_ERR_ARG, "ce_bwd: %d rows are not whole rows of T = %d positions", rows, T);
+  long long n = (long long)rows * V;
+  ce_bwd_kernel<<<(int)min((long long)kNumSMs * 16, (n + 255) / 256), 256, 0, st>>>(logits, ld, (const long long*)targets, lse, gscale,
+                                                                                    rows_per_g, count, T, dl, lddl, rows, V);
+  return check_launch("ce_bwd");
 }
 
 extern "C" int evk_ce_bwd(const float* logits, int ld, const int64_t* targets, const float* lse, const float* gscale,
                           int rows_per_g, float* dl, int lddl, int rows, int V, cudaStream_t st) {
-  EVK_REQUIRE(rows_per_g > 0, EVK_ERR_ARG, "ce_bwd: rows_per_g");
-  long long n = (long long)rows * V;
-  ce_bwd_kernel<<<(int)min((long long)kNumSMs * 16, (n + 255) / 256), 256, 0, st>>>(logits, ld, (const long long*)targets, lse, gscale, rows_per_g, dl, lddl, rows, V);
-  return check_launch("ce_bwd");
+  return evk_ce_bwd_ex(logits, ld, targets, lse, gscale, rows_per_g, nullptr, 1, dl, lddl, rows, V, st);
+}
+
+extern "C" int evk_dpo_reject_rows(const int64_t* y, int ldy, int B, const int32_t* spans, const int32_t* yc, int64_t* out, int Yr,
+                                   int64_t* lens, cudaStream_t st) {
+  EVK_REQUIRE(y && spans && yc && out && lens && B > 0 && Yr > 0 && ldy > 0, EVK_ERR_ARG, "dpo_reject_rows: bad arguments");
+  dpo_reject_rows_kernel<<<B, 256, 0, st>>>((const long long*)y, ldy, spans, yc, (long long*)out, Yr, (long long*)lens);
+  return check_launch("dpo_reject_rows");
 }
 
 extern "C" int evk_scaled_adam(float* p, float* g, float* delta, float* v, const int64_t* chunks, int nchunks,

@@ -87,6 +87,8 @@ class Text2SemanticDecoder(ParamTree):
 
     def pe(self, length, device):
         if self._pe is None or self._pe.shape[0] < length or self._pe.device != device:
+            if self._pe is not None:                   # captured training graphs keep reading the table they were captured with
+                self.__dict__.setdefault("_pe_old", []).append(self._pe)
             self._pe = sine_table(max(length, 2048), self.model_dim).to(device)
         return self._pe
 
@@ -120,10 +122,12 @@ class Text2SemanticDecoder(ParamTree):
             f = ops.linear(h, self.w(p + "linear1"), self.b(p + "linear1"), act=ops.ACT_RELU, drop=(pd, f"{tagp}gpt.df.{i}"))
             f = ops.linear(f, self.w(p + "linear2"), self.b(p + "linear2"))
             h = ops.layernorm(h, self.P(p + "norm2.weight"), self.P(p + "norm2.bias"), res=f, res_drop=(pd, f"{tagp}gpt.d2.{i}"))
+        # one offset vector per (B, X), kept for good: the training graphs of several padded shapes each read their own
+        xoffs = self.__dict__.setdefault("_xoffs", {})
         key = (B, X, str(dev))
-        if getattr(self, "_xoff_key", None) != key:
-            self._xoff, self._xoff_key = torch.full((B,), X, device=dev, dtype=torch.int64), key
-        hy = ops.slice_rows(h, self._xoff, Y)
+        if key not in xoffs:
+            xoffs[key] = torch.full((B,), X, device=dev, dtype=torch.int64)
+        hy = ops.slice_rows(h, xoffs[key], Y)
         Vp = (self.vocab_size + 3) // 4 * 4
         return ops.linear(hy, self.w("ar_predict_layer", pad0=Vp))
 
@@ -132,9 +136,11 @@ class Text2SemanticDecoder(ParamTree):
         xe = ops.embedding(self.P("ar_text_embedding.word_embeddings.weight"), x.to(torch.int64))
         return ops.linear(bert_cl, self.w("bert_proj", need_pb=False), self.b("bert_proj"), res=xe)
 
-    def forward(self, x, x_lens, y, y_lens, bert_feature, reject=None, bert_channels_last=False):
+    def forward(self, x, x_lens, y, y_lens, bert_feature, reject=None, bert_channels_last=False, count=None):
         """DPO variant (t2s_model.py:393-429): CE(sum) on the given y plus a reference-free DPO term (beta 0.2) against
         a synthetically corrupted `reject` = (reject_y, reject_y_lens); built by `make_reject_y` when not given.
+        count: None, or int32 device [2] = (the collate's Y, max(reject_y_lens)) for a batch padded further: positions at or
+        past them add nothing to either branch (ops.dpo_ce), so the loss is the one at the collate's shape.
         -> (loss, acc)."""
         if reject is None:
             reject = make_reject_y(y, y_lens)
@@ -145,22 +151,24 @@ class Text2SemanticDecoder(ParamTree):
         ry_in, rtg = self.make_targets(ry, ryl)
         self.begin_pack()
         try:
-            return self._forward_dpo(x, bert_feature, bert_channels_last, y_in, tg, ry_in, rtg, x_lens, y_lens, ryl, X)
+            return self._forward_dpo(x, bert_feature, bert_channels_last, y_in, tg, ry_in, rtg, x_lens, y_lens, ryl, X, count)
         finally:
             self.end_pack()
 
-    def _forward_dpo(self, x, bert_feature, bert_channels_last, y_in, tg, ry_in, rtg, x_lens, y_lens, ryl, X):
+    def _forward_dpo(self, x, bert_feature, bert_channels_last, y_in, tg, ry_in, rtg, x_lens, y_lens, ryl, X, count=None):
         # the text prefix is embedded once per branch in the reference (two make_input_data calls); the branches only share
         # weights, so the second pass re-runs it to keep the dropout streams independent as well
         lc = self._decode(self._embed_text(x, bert_feature, bert_channels_last), y_in, x_lens, y_lens, X)
         lr_ = self._decode(self._embed_text(x, bert_feature, bert_channels_last), ry_in, x_lens, ryl, X, tagp="rej.")
-        loss, metrics = ops.dpo_ce(lc, tg, lr_, rtg, self.top_k, self.EOS, V=self.vocab_size, beta=0.2)
+        loss, metrics = ops.dpo_ce(lc, tg, lr_, rtg, self.top_k, self.EOS, V=self.vocab_size, beta=0.2, count=count)
         self.last_logits, self.last_dpo = lc.detach(), metrics
         return loss, metrics[2]
 
-    def forward_old(self, x, x_lens, y, y_lens, bert_feature, targets=None, bert_channels_last=False):
+    def forward_old(self, x, x_lens, y, y_lens, bert_feature, targets=None, bert_channels_last=False, count=None):
         """-> (loss, acc) like t2s_model.py:431-490; `loss` is differentiable, `acc` a device scalar.
-        bert_feature: [B, 1024, X] (reference layout), or [B, X, 1024] with bert_channels_last=True."""
+        bert_feature: [B, 1024, X] (reference layout), or [B, X, 1024] with bert_channels_last=True.
+        count: None, or an int32 device scalar, the collate's Y of a batch padded further: positions at or past it add no
+        loss, accuracy or gradient (ops.ce_sum_topk), so the loss is the one at the collate's shape."""
         B, X = x.shape
         x_lens, y_lens = x_lens.to(torch.int64).contiguous(), y_lens.to(torch.int64).contiguous()
         y_in, tg = self.make_targets(y, y_lens) if targets is None else targets
@@ -169,7 +177,7 @@ class Text2SemanticDecoder(ParamTree):
             logits = self._decode(self._embed_text(x, bert_feature, bert_channels_last), y_in, x_lens, y_lens, X)
         finally:
             self.end_pack()
-        loss, out2 = ops.ce_sum_topk(logits, tg.reshape(-1), self.top_k, self.EOS, V=self.vocab_size)
+        loss, out2 = ops.ce_sum_topk(logits, tg.reshape(-1), self.top_k, self.EOS, V=self.vocab_size, count=count)
         self.last_logits = logits.detach()        # detached: a retained graph would pin AccumulateGrad nodes to this stream
         return loss, out2[1]
 
@@ -474,17 +482,34 @@ class Text2SemanticDecoder(ParamTree):
             self._active, self._memo_pack = None, False
             self.train(was_training)
 
+def reject_spans(y_lens, Yc, generator=None):
+    """The host draw of make_reject_y: per item, sorted(randint(0, Yc, (2,))) -> int32 [B, 2] of spans (i0, i1).  The same
+    torch.randint calls in the same order as the reference (utils.py:195-232 draws over the PADDED row of width Yc)."""
+    return torch.tensor([sorted(torch.randint(0, Yc, size=(2,), generator=generator).tolist()) for _ in range(len(y_lens))],
+                        dtype=torch.int32).reshape(len(y_lens), 2)
+
+
+def reject_width(spans, Yc):
+    """max(reject_y_lens) of make_reject_y for these spans: Yc + the longest span."""
+    return int(Yc) + int((spans[:, 1] - spans[:, 0]).max())
+
+
 def make_reject_y(y_o, y_lens, generator=None):
     """utils.py:195-232: per item, duplicate a random span of the PADDED row (the reference's `randint(0, 1)` always picks
-    the repeat branch); rows are re-padded with 0 to the longest result.  Host-side integer work, as in the reference."""
-    rows, lens = [], []
-    for b in range(len(y_lens)):
+    the repeat branch); rows are re-padded with 0 to the longest result.  The spans are drawn on the host (reject_spans);
+    CUDA rows are then built by ops.dpo_reject_rows, host rows on the host."""
+    Yc = y_o.shape[1]
+    spans = reject_spans(y_lens, Yc, generator)
+    Ym = reject_width(spans, Yc)
+    if y_o.is_cuda:
+        yc = torch.tensor([Yc], dtype=torch.int32).to(y_o.device, non_blocking=True)
+        out, lens = ops.dpo_reject_rows(y_o.to(torch.int64).contiguous(), spans.to(y_o.device, non_blocking=True), yc, Ym)
+        return out.to(y_o.dtype), lens.to(y_lens.device)
+    out = torch.zeros((len(spans), Ym), dtype=y_o.dtype)
+    lens = []
+    for b, (i0, i1) in enumerate(spans.tolist()):
         y = y_o[b]
-        i0, i1 = sorted(torch.randint(0, len(y), size=(2,), generator=generator).tolist())
-        rows.append(torch.cat([y[:i0], y[i0:i1], y[i0:i1], y[i1:]]))
-        lens.append(len(rows[-1]))
-    Ym = max(lens)
-    out = torch.zeros((len(rows), Ym), dtype=y_o.dtype, device=y_o.device)
-    for b, r in enumerate(rows):
+        r = torch.cat([y[:i0], y[i0:i1], y[i0:i1], y[i1:]])
         out[b, :len(r)] = r
+        lens.append(len(r))
     return out, torch.tensor(lens, device=y_lens.device)

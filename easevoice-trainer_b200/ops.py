@@ -1858,30 +1858,40 @@ def gpt_embed(xe, ye, alpha_x, alpha_y, pe):
 
 class _CeFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, logits, targets, topk, ignore, V):
+    def forward(ctx, logits, targets, topk, ignore, V, count):
         logits = _cl(logits)
         rows, Vp, ld = _rows(logits)
         targets = targets.contiguous()
         dev = logits.device
+        T = _count_period(logits, count)
         lse = torch.empty(rows, device=dev, dtype=torch.float32)
         nll = torch.empty(rows, device=dev, dtype=torch.float32)
         flags = torch.empty(rows, device=dev, dtype=torch.uint8)
         out2 = torch.empty(2, device=dev, dtype=torch.float32)
-        _call("evk_ce_fwd", _p(logits), ld, _p(targets), rows, V, topk, ignore, _p(lse), _p(nll), _p(flags), _p(out2))
-        ctx.save_for_backward(logits, targets, lse)
-        ctx.V = V
+        _call("evk_ce_fwd_ex", _p(logits), ld, _p(targets), rows, V, topk, ignore, _p(count), T, _p(lse), _p(nll), _p(flags), _p(out2))
+        ctx.save_for_backward(logits, targets, lse, count)
+        ctx.V, ctx.T = V, T
         ctx.mark_non_differentiable(out2)
         return out2[0].clone(), out2
 
     @staticmethod
     def backward(ctx, gloss, _g2):
-        logits, targets, lse = ctx.saved_tensors
+        logits, targets, lse, count = ctx.saved_tensors
         rows, Vp, ld = _rows(logits)
         V = ctx.V
         gl = gloss.reshape(1).contiguous().float()
         dl = (torch.empty if Vp == V else torch.zeros)(logits.shape, device=logits.device, dtype=torch.float32)
-        _call("evk_ce_bwd", _p(logits), ld, _p(targets), _p(lse), _p(gl), rows, _p(dl), Vp, rows, V)
-        return dl, None, None, None, None
+        _call("evk_ce_bwd_ex", _p(logits), ld, _p(targets), _p(lse), _p(gl), rows, _p(count), ctx.T, _p(dl), Vp, rows, V)
+        return dl, None, None, None, None, None
+
+
+def _count_period(logits, count):
+    """-> T, the positions per batch row of [B, T, Vp] logits that a counted-length bound `count` refers to (1 without one)."""
+    if count is None:
+        return 1
+    assert logits.dim() == 3, "a counted length needs [B, T, V] logits"
+    assert count.dtype == torch.int32 and count.is_cuda and count.numel() == 1, "count: one int32 device value"
+    return logits.shape[1]
 
 
 def attn_decode_dev(cache, n_prev_dev, heads, row, skip=None):
@@ -1914,10 +1924,11 @@ def sample_tokens(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, a
           _p(x_next), D)
 
 
-def ce_sum_topk(logits, targets, topk=3, ignore_index=1024, V=None):
+def ce_sum_topk(logits, targets, topk=3, ignore_index=1024, V=None, count=None):
     """-> (sum cross-entropy (differentiable), device float32 [2] = (loss, top-k accuracy ignoring ignore_index)).
-    V: number of real classes when the last dim of `logits` is zero-padded."""
-    loss, out2 = _CeFn.apply(logits, targets, int(topk), int(ignore_index), int(V or logits.shape[-1]))
+    V: number of real classes when the last dim of `logits` is zero-padded.  count: None, or an int32 device scalar n for
+    [B, T, Vp] logits: positions t >= n of every row add no loss, no accuracy count and no gradient (evk_ce_fwd_ex)."""
+    loss, out2 = _CeFn.apply(logits, targets, int(topk), int(ignore_index), int(V or logits.shape[-1]), count)
     return loss, out2
 
 
@@ -1925,24 +1936,28 @@ class _DpoCeFn(torch.autograd.Function):
     """loss_1 + loss_2 of Text2SemanticDecoder.forward (t2s_model.py:417-427) from chosen / rejected logits."""
 
     @staticmethod
-    def forward(ctx, lc, tc, lr_, tr, topk, ignore, V, beta):
+    def forward(ctx, lc, tc, lr_, tr, topk, ignore, V, beta, count):
         lc, lr_ = _cl(lc), _cl(lr_)
         B, Yc = tc.shape
         Yr = tr.shape[1]
         dev = lc.device
         tc, tr = tc.reshape(-1).contiguous(), tr.reshape(-1).contiguous()
+        if count is not None:
+            assert count.dtype == torch.int32 and count.is_cuda and count.numel() == 2, "count: int32 device (chosen, rejected)"
+        cnt = (None, None) if count is None else (count[0:1], count[1:2])
         bufs = []
-        for lg, tg, rows in ((lc, tc, B * Yc), (lr_, tr, B * Yr)):
+        for lg, tg, rows, T, cn in ((lc, tc, B * Yc, Yc, cnt[0]), (lr_, tr, B * Yr, Yr, cnt[1])):
             lse = torch.empty(rows, device=dev, dtype=torch.float32)
             nll = torch.empty(rows, device=dev, dtype=torch.float32)
             flags = torch.empty(rows, device=dev, dtype=torch.uint8)
             o2 = torch.empty(2, device=dev, dtype=torch.float32)
-            _call("evk_ce_fwd", _p(lg), _rows(lg)[2], _p(tg), rows, V, topk, ignore, _p(lse), _p(nll), _p(flags), _p(o2))
+            _call("evk_ce_fwd_ex", _p(lg), _rows(lg)[2], _p(tg), rows, V, topk, ignore, _p(cn), T, _p(lse), _p(nll), _p(flags), _p(o2))
             bufs.append((lse, nll, o2))
         out3 = torch.empty(3, device=dev, dtype=torch.float32)
         coef = torch.empty((2, B), device=dev, dtype=torch.float32)
-        _call("evk_dpo_head", _p(bufs[0][1]), Yc, _p(bufs[1][1]), Yr, B, ctypes.c_float(beta), _p(out3), _p(coef[0]), _p(coef[1]))
-        ctx.save_for_backward(lc, tc, bufs[0][0], lr_, tr, bufs[1][0], coef)
+        _call("evk_dpo_head_ex", _p(bufs[0][1]), Yc, _p(cnt[0]), _p(bufs[1][1]), Yr, _p(cnt[1]), B, ctypes.c_float(beta), _p(out3),
+              _p(coef[0]), _p(coef[1]))
+        ctx.save_for_backward(lc, tc, bufs[0][0], lr_, tr, bufs[1][0], coef, count)
         ctx.k = (B, Yc, Yr, V)
         metrics = torch.stack([out3[0], out3[1], bufs[0][2][1]])        # (loss_1, loss_2, top-k acc of the chosen branch)
         ctx.mark_non_differentiable(metrics)
@@ -1950,16 +1965,17 @@ class _DpoCeFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g, _gm):
-        lc, tc, lsec, lr_, tr, lser, coef = ctx.saved_tensors
+        lc, tc, lsec, lr_, tr, lser, coef, count = ctx.saved_tensors
         B, Yc, Yr, V = ctx.k
         gc = _AxpbyFn_scale(coef, g)
+        cnt = (None, None) if count is None else (count[0:1], count[1:2])
         outs = []
-        for lg, tg, lse, Yn, cf in ((lc, tc, lsec, Yc, gc[0]), (lr_, tr, lser, Yr, gc[1])):
+        for lg, tg, lse, Yn, cf, cn in ((lc, tc, lsec, Yc, gc[0], cnt[0]), (lr_, tr, lser, Yr, gc[1], cnt[1])):
             rows, Vp, ld = _rows(lg)
             dl = (torch.empty if Vp == V else torch.zeros)(lg.shape, device=lg.device, dtype=torch.float32)
-            _call("evk_ce_bwd", _p(lg), ld, _p(tg), _p(lse), _p(cf), Yn, _p(dl), Vp, rows, V)
+            _call("evk_ce_bwd_ex", _p(lg), ld, _p(tg), _p(lse), _p(cf), Yn, _p(cn), Yn, _p(dl), Vp, rows, V)
             outs.append(dl)
-        return outs[0], None, outs[1], None, None, None, None, None
+        return outs[0], None, outs[1], None, None, None, None, None, None
 
 
 def _AxpbyFn_scale(coef, g):
@@ -1967,10 +1983,26 @@ def _AxpbyFn_scale(coef, g):
     return (coef * g.reshape(1, 1)).contiguous()
 
 
-def dpo_ce(logits_c, targets_c, logits_r, targets_r, topk=3, ignore_index=1024, V=None, beta=0.2):
-    """-> (loss_1 + loss_2 (differentiable), device [3] = (loss_1, loss_2, top-k acc))."""
+def dpo_ce(logits_c, targets_c, logits_r, targets_r, topk=3, ignore_index=1024, V=None, beta=0.2, count=None):
+    """-> (loss_1 + loss_2 (differentiable), device [3] = (loss_1, loss_2, top-k acc)).  count: None, or int32 device [2] =
+    (chosen, rejected) counted lengths: positions at or past a branch's count add no loss, accuracy or gradient, and do not
+    enter that branch's log-prob sums (evk_ce_fwd_ex / evk_dpo_head_ex)."""
     return _DpoCeFn.apply(logits_c, targets_c, logits_r, targets_r, int(topk), int(ignore_index),
-                          int(V or logits_c.shape[-1]), float(beta))
+                          int(V or logits_c.shape[-1]), float(beta), count)
+
+
+def dpo_reject_rows(y, spans, yc, width):
+    """Rejected rows of the DPO variant on the device (evk_dpo_reject_rows) -> (rows int64 [B, width], lens int64 [B]):
+    row b = y[b, :i0] ++ y[b, i0:i1] ++ y[b, i0:i1] ++ y[b, i1:Yc], zero after, with (i0, i1) = spans[b] (int32 device
+    [B, 2]) and Yc = yc (int32 device scalar).  width must hold the longest row (Yc + max(i1 - i0)).  No host sync."""
+    assert y.dtype == torch.int64 and y.dim() == 2 and y.stride(1) == 1 and y.is_cuda
+    assert spans.dtype == torch.int32 and spans.is_contiguous() and tuple(spans.shape) == (y.shape[0], 2)
+    assert yc.dtype == torch.int32 and yc.numel() == 1
+    B = y.shape[0]
+    out = torch.empty((B, int(width)), device=y.device, dtype=torch.int64)
+    lens = torch.empty(B, device=y.device, dtype=torch.int64)
+    _call("evk_dpo_reject_rows", _p(y), y.stride(0), B, _p(spans), _p(yc), _p(out), int(width), _p(lens))
+    return out, lens
 
 
 def scaled_adam(st, gscale=1.0, zero_grad=True):

@@ -93,6 +93,26 @@ class Text2SemanticDataset(torch.utils.data.Dataset):
                     bert_feature=bert)
 
 
+def pad_host_batch(host, Xq, Yq, pad_val=1024):
+    """Pad a collated batch (Text2SemanticDataset.collate layout) to Xq phonemes / Yq semantic tokens: phonemes and BERT
+    features with 0, semantic ids with pad_val, as the collate pads.  The lengths are unchanged, so the padding is inert
+    apart from the loss terms the counted length removes (GptStep.prepare).  Pinned inputs give pinned outputs, so the
+    copies to the device stay asynchronous."""
+    B, X = host["phoneme_ids"].shape
+    Y = host["semantic_ids"].shape[1]
+    if X == Xq and Y == Yq:
+        return host
+    assert Xq >= X and Yq >= Y
+    pin = host["semantic_ids"].is_pinned()
+    out = dict(host)
+    for k, shape, fill in (("phoneme_ids", (B, Xq), 0), ("semantic_ids", (B, Yq), pad_val), ("bert_feature", (B, 1024, Xq), 0)):
+        src = host[k]
+        dst = torch.full(shape, fill, dtype=src.dtype, pin_memory=pin)
+        dst[..., :src.shape[-1]] = src
+        out[k] = dst
+    return out
+
+
 class DistributedBucketSampler(torch.utils.data.Sampler):
     """bucket_sampler.py:30-167: 2-second duration buckets, shuffle inside buckets, chunk into world*batch groups, shuffle
     the groups, pad to a multiple of world, stride by rank.  Yields sample indices (the DataLoader batches them)."""

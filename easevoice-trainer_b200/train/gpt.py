@@ -100,14 +100,16 @@ class GPTTrain:
         if world > 1 and not dist.is_initialized():
             dist.init_process_group("nccl", rank=rank, world_size=world, device_id=device)
         net = self._build(device)
-        step = gpt_step.GptStep(net, world_size=world, dpo=bool(t["if_dpo"]))
+        step = self.gpt_step = gpt_step.GptStep(net, world_size=world, dpo=bool(t["if_dpo"]))
         ops.manual_seed(t["seed"] + rank)
         ds = self.dataset or data_gpt.Text2SemanticDataset(c["train_phoneme_path"], c["train_semantic_path"],
                                                             max_sec=c["data"]["max_sec"], pad_val=c["data"]["pad_val"])
         bs = t["batch_size"] // 2 if t["if_dpo"] else t["batch_size"]           # data_module.py:39-41
         bs = max(min(bs, len(ds) // 4), 1)
         sampler = data_gpt.DistributedBucketSampler(ds, world, rank, batch_size=bs)
-        loader = torch.utils.data.DataLoader(ds, batch_size=bs, sampler=sampler, collate_fn=ds.collate, num_workers=0, pin_memory=True)
+        # two worker processes: in the main process, loading and collating (~20 ms per batch of 12) stalled the GPU step
+        # (tools/bench_gpt_train.py); the sampler order and the main process's RNG draws are the same
+        loader = torch.utils.data.DataLoader(ds, batch_size=bs, sampler=sampler, collate_fn=ds.collate, num_workers=2, pin_memory=True)
         start_epoch = 0
         newest = self._get_newest_ckpt(os.listdir(self.train_ckpts_output))
         if newest:                                    # resume (gpt.py:171-172)
@@ -121,9 +123,10 @@ class GPTTrain:
             sampler.set_epoch(epoch)
             step.batch_idx = 0                        # Lightning's batch_idx restarts every epoch; grads carry over
             for host in loader:
-                batch = {k: (v.to(device, non_blocking=True) if torch.is_tensor(v) else v) for k, v in host.items() if k != "ids"}
+                # padded to the agreed 32-token grid; the loss still counts the collate's shape only (GptStep.prepare)
+                batch = step.prepare(host, device)
                 did = step.wants_step()
-                loss, acc = step.step(batch)
+                loss, acc = step.train_step(batch)
                 self.global_step += int(did)
                 if rank == 0:                         # the only host reads of the loop (t2s_lightning_module.py:83-89)
                     connector.write_loss(cstep, loss=float(loss), other={"acc": float(acc), "lr": step.lr, "epoch": epoch})

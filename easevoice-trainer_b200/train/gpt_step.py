@@ -15,10 +15,16 @@ import torch
 import torch.distributed as dist
 
 from .. import ops
+from ..models_gpt import reject_spans, reject_width
 
 SCALED_ADAM_DEFAULTS = dict(lr=0.01, betas=(0.9, 0.95), clipping_scale=2.0, clipping_update_period=1000, scalar_lr_scale=0.1,
                             eps=1e-8, param_min_rms=1e-5, param_max_rms=3.0, scalar_max=10.0, size_update_period=4)
 CHUNK = 8192
+GRID = 32                # padded lengths (phonemes, semantic tokens, rejected rows) are rounded up to this many tokens
+
+
+def quantize_len(n, q=GRID):
+    return (int(n) + q - 1) // q * q
 
 
 class FlatScaledAdam:
@@ -112,6 +118,8 @@ class GptStep:
 
     ACCUM = 4
     LR_FIRST, LR_LOCKED = 0.01, 0.002          # lr_schedulers.py:36-65 (see module docstring)
+    MAX_GRAPHS = 12          # LRU bound on the shapes train_step keeps captured (all graphs share one memory pool)
+    CAPTURE_AFTER = 2        # train_step captures a shape the 2nd time it is seen; before that the eager step runs
 
     def __init__(self, model, world_size=1, dpo=False, **optim_kw):
         self.model, self.world, self.dpo = model, world_size, dpo
@@ -121,22 +129,35 @@ class GptStep:
         self._graph = None
         self._static = None
         self.last = None
+        self._graphs = {}            # train_step: shape key -> (graph, static inputs, outputs); insertion order = LRU order
+        self._seen = {}              # shape key -> sightings
+        self._pool = None            # one private memory pool shared by every train_step graph
+        self._opt_graph = None       # the ScaledAdam update, captured once in that pool (it does not depend on the shape)
+        self._shape_group = None     # gloo group of the host-side shape agreement (world > 1)
+        self.stats = dict(captures=0, replays=0, eager=0)
 
     # ---- eager pieces --------------------------------------------------------------------------
     def forward_backward(self, batch):
-        """loss/acc + gradient accumulation for one micro-batch (no optimizer step)."""
+        """loss/acc + gradient accumulation for one micro-batch (no optimizer step).  A batch padded past the collate's
+        shape (train_step) carries count = int32 device [2] (the collate's Y, the rejected rows' max length) and, for DPO,
+        spans (int32 device [B, 2], reject_spans) and reject_width (the padded width of the rejected rows)."""
         m = self.model
+        count = batch.get("count")
         if self.dpo:                                   # t2s_lightning_module.py:44 (if_dpo): CE + reference-free DPO term
+            reject = batch.get("reject")
+            if "spans" in batch:
+                reject = ops.dpo_reject_rows(batch["semantic_ids"], batch["spans"], count[0:1], batch["reject_width"])
             loss, acc = m.forward(batch["phoneme_ids"], batch["phoneme_ids_len"], batch["semantic_ids"], batch["semantic_ids_len"],
-                                  batch["bert_feature"], reject=batch.get("reject"),
-                                  bert_channels_last=batch.get("bert_channels_last", False))
+                                  batch["bert_feature"], reject=reject,
+                                  bert_channels_last=batch.get("bert_channels_last", False), count=count)
             with ops.grad_pool():
                 grads = torch.autograd.grad(loss, self.opt.params, allow_unused=True)
                 self.opt.accumulate(grads)
             return loss.detach(), acc
         loss, acc = m.forward_old(batch["phoneme_ids"], batch["phoneme_ids_len"], batch["semantic_ids"],
                                   batch["semantic_ids_len"], batch["bert_feature"], targets=batch.get("targets"),
-                                  bert_channels_last=batch.get("bert_channels_last", False))
+                                  bert_channels_last=batch.get("bert_channels_last", False),
+                                  count=None if count is None else count[0:1])
         with ops.grad_pool():
             grads = torch.autograd.grad(loss, self.opt.params, allow_unused=True)
             self.opt.accumulate(grads)
@@ -209,6 +230,101 @@ class GptStep:
         self.batch_idx += 1
         self.last = self._gout
         return self._gout
+
+    # ---- padded shapes: grid, rank agreement and one graph per shape ------------------------------------------
+    def agree_shape(self, X, Y, Yr=0):
+        """-> (Xq, Yq, Yrq): the padded shape EVERY rank uses for this micro-batch.  Each rank's collate pads to its own
+        batch maximum, so the local lengths (phonemes, semantic tokens, rejected rows; Yr = 0 without DPO) are rounded up
+        to the GRID and MAX-reduced over a gloo (host-side) group: no GPU synchronisation, and all ranks capture, replay
+        or fall back to the eager step at the same micro-batches, so their gradient all-reduces pair up."""
+        q = [quantize_len(X), quantize_len(Y), quantize_len(Yr)]
+        if self.world > 1:
+            if self._shape_group is None:
+                self._shape_group = dist.new_group(backend="gloo")
+            t = torch.tensor(q, dtype=torch.int64)
+            dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self._shape_group)
+            q = [int(v) for v in t]
+        return tuple(q)
+
+    def prepare(self, host, device):
+        """A collated host batch (data_gpt layout, pinned) -> the device batch train_step takes.  DPO spans are drawn
+        here (reject_spans: the same torch.randint calls, in the same order, as make_reject_y in the eager forward); the
+        batch is padded to the agreed shape and the counts + spans cross to the device in one pinned int32 buffer."""
+        from .data_gpt import pad_host_batch
+        Yc = host["semantic_ids"].shape[1]
+        spans = reject_spans(host["semantic_ids_len"], Yc) if self.dpo else None
+        Yr = reject_width(spans, Yc) if self.dpo else 0
+        Xq, Yq, Yrq = self.agree_shape(host["phoneme_ids"].shape[1], Yc, Yr)
+        host = pad_host_batch(host, Xq, Yq)
+        meta = torch.tensor([Yc, Yr], dtype=torch.int32)
+        if spans is not None:
+            meta = torch.cat([meta, spans.reshape(-1)])
+        meta = meta.pin_memory().to(device, non_blocking=True)
+        batch = {k: host[k].to(device, non_blocking=True)
+                 for k in ("phoneme_ids", "phoneme_ids_len", "semantic_ids", "semantic_ids_len", "bert_feature")}
+        batch["count"] = meta[:2]
+        if spans is not None:
+            batch["spans"], batch["reject_width"] = meta[2:].view(-1, 2), Yrq
+        return batch
+
+    def train_step(self, batch):
+        """What the trainer calls, on a batch from prepare(): replay the CUDA graph of this padded shape, capturing it
+        the CAPTURE_AFTER-th time the shape shows up (at most MAX_GRAPHS kept, least recently used evicted); before that
+        the eager step runs.  Same schedule, RNG stream and results as step() on the same batch."""
+        key = (tuple(batch["phoneme_ids"].shape), tuple(batch["semantic_ids"].shape), batch.get("reject_width", 0))
+        n = self._seen[key] = self._seen.get(key, 0) + 1
+        if key not in self._graphs and n < self.CAPTURE_AFTER:
+            self.stats["eager"] += 1
+            return self.step(batch)
+        g = self._graphs.pop(key, None)
+        if g is None:
+            while len(self._graphs) >= self.MAX_GRAPHS:
+                self._graphs.pop(next(iter(self._graphs)))
+            g = self._capture_shape(batch)
+            self.stats["captures"] += 1
+        else:
+            self.stats["replays"] += 1
+        self._graphs[key] = g                                            # (re)insert as most recently used
+        graph, static, out = g
+        for k, v in static.items():
+            v.copy_(batch[k], non_blocking=True)
+        graph.replay()
+        if self.wants_step():
+            if self.world > 1:
+                dist.all_reduce(self.opt.flat_g)
+            self._opt_graph.replay()
+            self.opt.set_lr(self.LR_LOCKED)
+            self.lr = self.LR_LOCKED
+        self.batch_idx += 1
+        self.last = out
+        return out
+
+    def _capture_shape(self, batch):
+        static = {k: v.clone() for k, v in batch.items() if torch.is_tensor(v)}
+        feed = dict(batch, **static)
+        # warm-up (allocator, lazy initialisation) on a side stream; it must not count as training
+        snap = (self.opt.flat_g.clone(), ops.rng_state().clone())
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                self.forward_backward(feed)
+        torch.cuda.current_stream().wait_stream(side)
+        self.opt.flat_g.copy_(snap[0])
+        ops.rng_state().copy_(snap[1])
+        torch.cuda.synchronize()
+        if self._pool is None:
+            self._pool = torch.cuda.graph_pool_handle()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, pool=self._pool):
+            if self.model.training:
+                ops.advance_rng()
+            out = self.forward_backward(feed)
+        if self._opt_graph is None:                  # captured, not run: the optimizer state is untouched
+            self._opt_graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self._opt_graph, pool=self._pool):
+                self.opt.step(gscale=1.0 / self.world, zero_grad=True)
+        return graph, static, out
 
 
 def synthetic_batch(B=16, X=256, Y=1024, seed=0, device="cpu", ragged=False):

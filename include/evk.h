@@ -475,6 +475,30 @@ int evk_ce_bwd(const float* logits, int32_t ld, const int64_t* targets, const fl
  * (logp_chosen_b - logp_rejected_b)), their sum); coef_c/coef_r [B] = d out3[2] / d nll_{c,r}[b][t] (feeds evk_ce_bwd). */
 int evk_dpo_head(const float* nll_c, int32_t Yc, const float* nll_r, int32_t Yr, int32_t B, float beta, float* out3,
                  float* coef_c, float* coef_r, evk_stream_t stream);
+/* Counted-length bound on the three calls above, for batches padded past the collate's length (the stage-1 trainer pads to
+ * a 32-token grid so that a CUDA graph can serve many batches).  The rows are [B][T] positions (row r is position r % T).
+ * count: NULL, or a device int32 scalar n: positions t >= n add no loss, no accuracy count (neither valid nor hit) and no
+ * gradient (evk_ce_bwd_ex writes 0 to their logit gradients).  count == NULL is exactly evk_ce_fwd / evk_ce_bwd.
+ * The bound reproduces the loss at the collate's shape: the reference sums CE over every position of its padded batch (EOS
+ * targets included), so positions added by further padding must not count. */
+int evk_ce_fwd_ex(const float* logits, int32_t ld, const int64_t* targets, int32_t rows, int32_t V, int32_t topk,
+                  int64_t ignore_index, const int32_t* count, int32_t T, float* lse, float* nll, uint8_t* flags, float* out2,
+                  evk_stream_t stream);
+int evk_ce_bwd_ex(const float* logits, int32_t ld, const int64_t* targets, const float* lse, const float* gscale,
+                  int32_t rows_per_g, const int32_t* count, int32_t T, float* dl, int32_t lddl, int32_t rows, int32_t V,
+                  evk_stream_t stream);
+/* evk_dpo_head with counted lengths: count_c / count_r NULL, or device int32 scalars; the per-row log-prob sums (and so
+ * loss_1) then run over t < min(Yc, *count_c) resp. t < min(Yr, *count_r).  NULL for both is exactly evk_dpo_head.  The
+ * stage-1 trainer passes the collate's Y for the chosen branch and max(reject_lens) for the rejected one. */
+int evk_dpo_head_ex(const float* nll_c, int32_t Yc, const int32_t* count_c, const float* nll_r, int32_t Yr,
+                    const int32_t* count_r, int32_t B, float beta, float* out3, float* coef_c, float* coef_r, evk_stream_t stream);
+/* Rejected rows of the DPO variant (utils.py:195-232, the repeat branch) from host-drawn spans, capturable in a CUDA graph:
+ * row b of y [B][ldy] (int64, padded chosen rows) with span (i0, i1) = spans[b] (int32 [B][2], 0 <= i0 <= i1 <= Yc) becomes
+ *   out[b] = y[b][:i0] ++ y[b][i0:i1] ++ y[b][i0:i1] ++ y[b][i1:Yc]  followed by 0 up to Yr   (out: int64 [B][Yr])
+ * and lens[b] = Yc + i1 - i0 (int64).  yc: device int32 scalar Yc (<= ldy), the collate's width of y.  Every row must fit:
+ * Yc + i1 - i0 <= Yr (positions past Yr are not written). */
+int evk_dpo_reject_rows(const int64_t* y, int32_t ldy, int32_t B, const int32_t* spans, const int32_t* yc, int64_t* out,
+                        int32_t Yr, int64_t* lens, evk_stream_t stream);
 /* ScaledAdam (optim.py:123-622) over flat arenas p/g/delta/v.  chunks: [nchunks][3] = (tensor id, begin, count), numel: [nt].
  * Per-tensor state: rms, sv (scale_exp_avg_sq) [nt]; sg (scale_grads) [size_update_period][nt]; stats [nt][3] and
  * coef [nt][2] are scratch (stats must be zero on first use; the call leaves it zero).  hyper: device [lr];
