@@ -30,74 +30,67 @@ BATCH = 4               # the reference's chunks per model call (its fade-window
 ROPE_THETA = 10000.0
 
 
-class BSRoformer:
-    """BSRoformer(**config) for inference on CUDA.  Takes the reference's keyword arguments; the training-only ones
-    (`*_dropout`, `multi_stft_*`, `flash_attn`) are accepted and ignored.  Raises ValueError for what the kernels do not
-    take: dim_head != 64, linear_transformer_depth != 0, num_stems != 1, stft_n_fft not a power of two in [256, 4096],
-    stft_win_length != stft_n_fft, stft_normalized, a custom stft_window_fn, a hop above n_fft / 2, and bands that do not
-    sum to n_fft // 2 + 1."""
+def check_stft(stft_n_fft, stft_win_length, stft_hop_length, stft_normalized, stft_window_fn):
+    """-> n_fft; ValueError for an STFT the kernels do not take (shared by BSRoformer and MelBandRoformer)"""
+    n_fft = int(stft_n_fft)
+    if n_fft < 256 or n_fft > 4096 or n_fft & (n_fft - 1):
+        raise ValueError(f"stft_n_fft must be a power of two in [256, 4096], got {n_fft}")
+    if stft_win_length != n_fft:
+        raise ValueError(f"stft_win_length ({stft_win_length}) must equal stft_n_fft ({n_fft})")
+    if stft_normalized or stft_window_fn is not None:
+        raise ValueError("only the default un-normalised Hann STFT is supported")
+    if not 0 < stft_hop_length <= n_fft // 2:
+        raise ValueError(f"stft_hop_length must be in [1, n_fft // 2], got {stft_hop_length}")
+    return n_fft
 
-    def __init__(self, dim, *, depth, stereo=False, num_stems=1, time_transformer_depth=2, freq_transformer_depth=2,
-                 linear_transformer_depth=0, freqs_per_bands=SHIPPED_CONFIG["freqs_per_bands"], dim_head=64, heads=8,
-                 dim_freqs_in=1025, stft_n_fft=2048, stft_hop_length=512, stft_win_length=2048, stft_normalized=False,
-                 stft_window_fn=None, mask_estimator_depth=2, attn_dropout=0.0, ff_dropout=0.0, flash_attn=True,
-                 multi_stft_resolution_loss_weight=1.0, multi_stft_resolutions_window_sizes=(4096, 2048, 1024, 512, 256),
-                 multi_stft_hop_size=147, multi_stft_normalized=False, multi_stft_window_fn=None):
-        n_fft = int(stft_n_fft)
-        bands = tuple(int(f) for f in freqs_per_bands)
-        if dim_head != 64:
-            raise ValueError(f"dim_head must be 64, got {dim_head}")
-        if linear_transformer_depth != 0:
-            raise ValueError("linear_transformer_depth > 0 (LinearAttention) is not supported")
-        if num_stems != 1:
-            raise ValueError(f"num_stems must be 1, got {num_stems}")
-        if n_fft < 256 or n_fft > 4096 or n_fft & (n_fft - 1):
-            raise ValueError(f"stft_n_fft must be a power of two in [256, 4096], got {n_fft}")
-        if stft_win_length != n_fft:
-            raise ValueError(f"stft_win_length ({stft_win_length}) must equal stft_n_fft ({n_fft})")
-        if stft_normalized or stft_window_fn is not None:
-            raise ValueError("only the default un-normalised Hann STFT is supported")
-        if not 0 < stft_hop_length <= n_fft // 2:
-            raise ValueError(f"stft_hop_length must be in [1, n_fft // 2], got {stft_hop_length}")
-        if len(bands) < 2 or min(bands) < 1 or sum(bands) != n_fft // 2 + 1:
-            raise ValueError(f"freqs_per_bands must sum to n_fft // 2 + 1 = {n_fft // 2 + 1}, got {sum(bands)}")
-        if dim < 4 or dim % 4 or heads < 1 or depth < 1 or mask_estimator_depth < 1:
-            raise ValueError(f"bad sizes: dim {dim} (a multiple of 4), heads {heads}, depth {depth}, "
-                             f"mask_estimator_depth {mask_estimator_depth}")
+
+def check_sizes(dim, heads, depth, mask_estimator_depth):
+    if dim < 4 or dim % 4 or heads < 1 or depth < 1 or mask_estimator_depth < 1:
+        raise ValueError(f"bad sizes: dim {dim} (a multiple of 4), heads {heads}, depth {depth}, "
+                         f"mask_estimator_depth {mask_estimator_depth}")
+
+
+class AxialRoformer:
+    """What BSRoformer and MelBandRoformer share: depth x (time, frequency) Transformers of rotary gated attention and GELU
+    feed-forward layers over [B, T, bands, dim] activations, one Linear per band from the band-split operand, one MLP + GLU
+    per band to the complex masks, the weight folding and packing, and the input checks.  Subclasses define the bands."""
+
+    def __init__(self, dim, depth, heads, stereo, time_transformer_depth, freq_transformer_depth, n_fft, hop,
+                 mask_estimator_depth, mask_linears):
         self.dim, self.depth, self.heads = int(dim), int(depth), int(heads)
         self.stereo, self.S = bool(stereo), 2 if stereo else 1
         self.t_depth, self.f_depth = int(time_transformer_depth), int(freq_transformer_depth)
-        self.bands, self.n_fft, self.hop = bands, n_fft, int(stft_hop_length)
+        self.n_fft, self.hop = n_fft, int(hop)
         self.mask_depth = int(mask_estimator_depth)
+        self.mask_linears = int(mask_linears)           # Linears per mask MLP (tanh between them)
         self.device = torch.device("cpu")
         self.host_w, self.bias = None, None
         self._packed = {}
         self._rope = {}
 
     # ---- weights -------------------------------------------------------------------------------------------------------
-    def _dims_in(self):
-        return [2 * f * self.S for f in self.bands]
-
-    def state_dict_shapes(self):
-        """-> {key: shape} of the reference's BSRoformer(**config).state_dict() (rotary modules hold no state there)"""
+    def _layer_shapes(self, p, n):
+        """{key: shape} of the n Attention + FeedForward layers of the Transformer at prefix p"""
         dim, inner = self.dim, self.heads * 64
         spec = {}
-        for i in range(self.depth):
-            for a, n in ((0, self.t_depth), (1, self.f_depth)):
-                for j in range(n):
-                    p = f"layers.{i}.{a}.layers.{j}"
-                    spec.update({p + ".0.norm.gamma": (dim,), p + ".0.to_qkv.weight": (3 * inner, dim),
-                                 p + ".0.to_gates.weight": (self.heads, dim), p + ".0.to_gates.bias": (self.heads,),
-                                 p + ".0.to_out.0.weight": (dim, inner), p + ".1.net.0.gamma": (dim,),
-                                 p + ".1.net.1.weight": (4 * dim, dim), p + ".1.net.1.bias": (4 * dim,),
-                                 p + ".1.net.4.weight": (dim, 4 * dim), p + ".1.net.4.bias": (dim,)})
-        spec["final_norm.gamma"] = (dim,)
-        for i, d in enumerate(self._dims_in()):
+        for j in range(n):
+            q = f"{p}.layers.{j}"
+            spec.update({q + ".0.norm.gamma": (dim,), q + ".0.to_qkv.weight": (3 * inner, dim),
+                         q + ".0.to_gates.weight": (self.heads, dim), q + ".0.to_gates.bias": (self.heads,),
+                         q + ".0.to_out.0.weight": (dim, inner), q + ".1.net.0.gamma": (dim,),
+                         q + ".1.net.1.weight": (4 * dim, dim), q + ".1.net.1.bias": (4 * dim,),
+                         q + ".1.net.4.weight": (dim, 4 * dim), q + ".1.net.4.bias": (dim,)})
+        return spec
+
+    def _band_shapes(self, dims_in):
+        """{key: shape} of band_split and the mask estimator for band-split widths dims_in"""
+        dim, spec = self.dim, {}
+        for i, d in enumerate(dims_in):
             p = f"band_split.to_features.{i}"
             spec.update({p + ".0.gamma": (d,), p + ".1.weight": (dim, d), p + ".1.bias": (dim,)})
-        for i, d in enumerate(self._dims_in()):
-            io = [dim] + [4 * dim] * (self.mask_depth - 1) + [2 * d]
-            for k in range(self.mask_depth):
+        for i, d in enumerate(dims_in):
+            io = [dim] + [4 * dim] * (self.mask_linears - 1) + [2 * d]
+            for k in range(self.mask_linears):
                 p = f"mask_estimators.0.to_freqs.{i}.0.{2 * k}"
                 spec.update({p + ".weight": (io[k + 1], io[k]), p + ".bias": (io[k + 1],)})
         return spec
@@ -119,53 +112,57 @@ class BSRoformer:
         missing = [k for k in spec if k not in sd]
         unexpected = [k for k in sd if k not in spec]
         if missing or unexpected:
-            raise ValueError(f"state_dict does not match BSRoformer: missing {missing[:5]}{'...' if len(missing) > 5 else ''}, "
-                             f"unexpected {unexpected[:5]}{'...' if len(unexpected) > 5 else ''}")
+            raise ValueError(f"state_dict does not match {type(self).__name__}: missing {missing[:5]}"
+                             f"{'...' if len(missing) > 5 else ''}, unexpected {unexpected[:5]}{'...' if len(unexpected) > 5 else ''}")
         for k, shape in spec.items():
             v = sd[k]
             if not torch.is_tensor(v) or not v.is_floating_point() or tuple(v.shape) != tuple(shape):
                 raise ValueError(f"{k}: expected a float tensor of shape {tuple(shape)}, got "
                                  f"{tuple(v.shape) if torch.is_tensor(v) else type(v).__name__}")
         folded = self._fold({k: sd[k].detach().cpu().to(torch.float32) for k in spec})
-        # unpacked weights stay on the host (each precision mode packs its own device copy from them); biases go to the device
+        # unpacked weights stay on the host (each precision mode packs its own device copy from them); biases (and any
+        # other vectors the forward reads) go to the device
         self.host_w = {k[:-2]: v for k, v in folded.items() if k.endswith(".w")}
-        self.bias = {k: v.to(self.device) for k, v in folded.items() if k.endswith(".b")}
+        self.bias = {k: v.to(self.device) for k, v in folded.items() if not k.endswith(".w")}
         self._packed = {}
         return self
 
-    def _fold(self, sd):
-        """RMSNorm gamma * sqrt(dim) into the next Linear's columns (in float64), to_gates appended to to_qkv"""
-        def fold(w, gamma):
-            return (w.double() * (gamma.double() * math.sqrt(gamma.numel()))[None, :]).float()
+    @staticmethod
+    def _fold_gamma(w, gamma):
+        """RMSNorm gamma * sqrt(dim) into the next Linear's columns (in float64)"""
+        return (w.double() * (gamma.double() * math.sqrt(gamma.numel()))[None, :]).float()
 
+    def _fold_layers(self, sd, p, n, out):
+        """the n layers of the Transformer at prefix p: norm gammas folded, to_gates appended to to_qkv"""
+        fold = self._fold_gamma
         D, H = self.heads * 64, self.heads
         ldq = (3 * D + H + 3) // 4 * 4
-        out = {}
-        for i in range(self.depth):
-            for a, n in ((0, self.t_depth), (1, self.f_depth)):
-                for j in range(n):
-                    p = f"layers.{i}.{a}.layers.{j}"
-                    g = sd[p + ".0.norm.gamma"]
-                    w = torch.zeros(ldq, self.dim)
-                    w[:3 * D] = sd[p + ".0.to_qkv.weight"]
-                    w[3 * D:3 * D + H] = sd[p + ".0.to_gates.weight"]
-                    b = torch.zeros(ldq)
-                    b[3 * D:3 * D + H] = sd[p + ".0.to_gates.bias"]
-                    out[p + ".qkvg.w"], out[p + ".qkvg.b"] = fold(w, g), b
-                    out[p + ".out.w"] = sd[p + ".0.to_out.0.weight"]
-                    out[p + ".ff1.w"] = fold(sd[p + ".1.net.1.weight"], sd[p + ".1.net.0.gamma"])
-                    out[p + ".ff1.b"] = sd[p + ".1.net.1.bias"]
-                    out[p + ".ff2.w"], out[p + ".ff2.b"] = sd[p + ".1.net.4.weight"], sd[p + ".1.net.4.bias"]
-        for i in range(len(self.bands)):
+        for j in range(n):
+            q = f"{p}.layers.{j}"
+            g = sd[q + ".0.norm.gamma"]
+            w = torch.zeros(ldq, self.dim)
+            w[:3 * D] = sd[q + ".0.to_qkv.weight"]
+            w[3 * D:3 * D + H] = sd[q + ".0.to_gates.weight"]
+            b = torch.zeros(ldq)
+            b[3 * D:3 * D + H] = sd[q + ".0.to_gates.bias"]
+            out[q + ".qkvg.w"], out[q + ".qkvg.b"] = fold(w, g), b
+            out[q + ".out.w"] = sd[q + ".0.to_out.0.weight"]
+            out[q + ".ff1.w"] = fold(sd[q + ".1.net.1.weight"], sd[q + ".1.net.0.gamma"])
+            out[q + ".ff1.b"] = sd[q + ".1.net.1.bias"]
+            out[q + ".ff2.w"], out[q + ".ff2.b"] = sd[q + ".1.net.4.weight"], sd[q + ".1.net.4.bias"]
+
+    def _fold_bands(self, sd, nb, mask_gamma, out):
+        """band_split (its RMSNorm gammas folded) and the mask MLPs (mask_gamma, the norm before them, folded into layer 0)"""
+        fold = self._fold_gamma
+        for i in range(nb):
             p = f"band_split.to_features.{i}"
             out[f"band.{i}.w"] = fold(sd[p + ".1.weight"], sd[p + ".0.gamma"])
             out[f"band.{i}.b"] = sd[p + ".1.bias"]
-            for k in range(self.mask_depth):
+            for k in range(self.mask_linears):
                 q = f"mask_estimators.0.to_freqs.{i}.0.{2 * k}"
                 w = sd[q + ".weight"]
-                out[f"mask.{i}.{k}.w"] = fold(w, sd["final_norm.gamma"]) if k == 0 else w
+                out[f"mask.{i}.{k}.w"] = fold(w, mask_gamma) if k == 0 else w
                 out[f"mask.{i}.{k}.b"] = sd[q + ".bias"]
-        return out
 
     def to(self, device):
         self.device = torch.device(device)
@@ -192,12 +189,6 @@ class BSRoformer:
             ang = torch.arange(L, dtype=torch.float32)[:, None] * inv[None, :]
             self._rope[L] = torch.stack([ang.cos(), ang.sin()], -1).contiguous().to(self.device)
         return self._rope[L]
-
-    @classmethod
-    def from_pretrained(cls, path, device="cuda"):
-        """The SeparateMDXC model (SHIPPED_CONFIG) with the weights of a reference checkpoint file, on `device`."""
-        sd = torch.load(path, map_location="cpu", weights_only=True)
-        return cls(**SHIPPED_CONFIG).to(device).load_state_dict(sd)
 
     # ---- forward -------------------------------------------------------------------------------------------------------
     def check_input(self, raw_audio):
@@ -237,39 +228,107 @@ class BSRoformer:
             del f
         return x
 
+    def _band_split(self, feat, off, rows):
+        """band i's Linear on the columns [2 S off[i], 2 S off[i+1]) of the band-split operand -> [rows * bands, dim]"""
+        W, sd, S, dim, nb = self._weights(), self.bias, self.S, self.dim, len(off) - 1
+        h = torch.empty((rows, nb * dim), device=feat.device)
+        for i in range(nb):
+            ops.linear_into(feat[:, 2 * S * off[i]:2 * S * off[i + 1]], W[f"band.{i}"], h[:, i * dim:(i + 1) * dim],
+                            bias=sd[f"band.{i}.b"])
+        return h.view(rows * nb, dim)
+
+    def _mask_estimator(self, xn, off, out):
+        """band i's MLP and GLU on its dim columns of xn [rows, bands * dim] -> the columns [2 S off[i], 2 S off[i+1]) of out"""
+        W, sd, S, dim, rows = self._weights(), self.bias, self.S, self.dim, xn.shape[0]
+        for i in range(len(off) - 1):
+            hc = xn[:, i * dim:(i + 1) * dim]
+            for k in range(self.mask_linears):
+                w = W[f"mask.{i}.{k}"]
+                last = k == self.mask_linears - 1
+                hc = ops.linear_into(hc, w, torch.empty((rows, w.D0), device=xn.device), bias=sd[f"mask.{i}.{k}.b"],
+                                     act=ops.ACT_NONE if last else ops.ACT_TANH)
+            ops.glu_into(hc, out[:, 2 * S * off[i]:2 * S * off[i + 1]])
+        return out
+
+
+class BSRoformer(AxialRoformer):
+    """BSRoformer(**config) for inference on CUDA.  Takes the reference's keyword arguments; the training-only ones
+    (`*_dropout`, `multi_stft_*`, `flash_attn`) are accepted and ignored.  Raises ValueError for what the kernels do not
+    take: dim_head != 64, linear_transformer_depth != 0, num_stems != 1, stft_n_fft not a power of two in [256, 4096],
+    stft_win_length != stft_n_fft, stft_normalized, a custom stft_window_fn, a hop above n_fft / 2, and bands that do not
+    sum to n_fft // 2 + 1."""
+
+    def __init__(self, dim, *, depth, stereo=False, num_stems=1, time_transformer_depth=2, freq_transformer_depth=2,
+                 linear_transformer_depth=0, freqs_per_bands=SHIPPED_CONFIG["freqs_per_bands"], dim_head=64, heads=8,
+                 dim_freqs_in=1025, stft_n_fft=2048, stft_hop_length=512, stft_win_length=2048, stft_normalized=False,
+                 stft_window_fn=None, mask_estimator_depth=2, attn_dropout=0.0, ff_dropout=0.0, flash_attn=True,
+                 multi_stft_resolution_loss_weight=1.0, multi_stft_resolutions_window_sizes=(4096, 2048, 1024, 512, 256),
+                 multi_stft_hop_size=147, multi_stft_normalized=False, multi_stft_window_fn=None):
+        bands = tuple(int(f) for f in freqs_per_bands)
+        if dim_head != 64:
+            raise ValueError(f"dim_head must be 64, got {dim_head}")
+        if linear_transformer_depth != 0:
+            raise ValueError("linear_transformer_depth > 0 (LinearAttention) is not supported")
+        if num_stems != 1:
+            raise ValueError(f"num_stems must be 1, got {num_stems}")
+        n_fft = check_stft(stft_n_fft, stft_win_length, stft_hop_length, stft_normalized, stft_window_fn)
+        if len(bands) < 2 or min(bands) < 1 or sum(bands) != n_fft // 2 + 1:
+            raise ValueError(f"freqs_per_bands must sum to n_fft // 2 + 1 = {n_fft // 2 + 1}, got {sum(bands)}")
+        check_sizes(dim, heads, depth, mask_estimator_depth)
+        super().__init__(dim, depth, heads, stereo, time_transformer_depth, freq_transformer_depth, n_fft, stft_hop_length,
+                         mask_estimator_depth, mask_estimator_depth)
+        self.bands = bands
+
+    # ---- weights -------------------------------------------------------------------------------------------------------
+    def _dims_in(self):
+        return [2 * f * self.S for f in self.bands]
+
+    def state_dict_shapes(self):
+        """-> {key: shape} of the reference's BSRoformer(**config).state_dict() (rotary modules hold no state there)"""
+        spec = {}
+        for i in range(self.depth):
+            for a, n in ((0, self.t_depth), (1, self.f_depth)):
+                spec.update(self._layer_shapes(f"layers.{i}.{a}", n))
+        spec["final_norm.gamma"] = (self.dim,)
+        spec.update(self._band_shapes(self._dims_in()))
+        return spec
+
+    def _fold(self, sd):
+        """RMSNorm gamma * sqrt(dim) into the next Linear's columns (in float64), to_gates appended to to_qkv"""
+        out = {}
+        for i in range(self.depth):
+            for a, n in ((0, self.t_depth), (1, self.f_depth)):
+                self._fold_layers(sd, f"layers.{i}.{a}", n, out)
+        self._fold_bands(sd, len(self.bands), sd["final_norm.gamma"], out)
+        return out
+
+    @classmethod
+    def from_pretrained(cls, path, device="cuda"):
+        """The SeparateMDXC model (SHIPPED_CONFIG) with the weights of a reference checkpoint file, on `device`."""
+        sd = torch.load(path, map_location="cpu", weights_only=True)
+        return cls(**SHIPPED_CONFIG).to(device).load_state_dict(sd)
+
+    # ---- forward -------------------------------------------------------------------------------------------------------
     @torch.no_grad()
     def forward(self, raw_audio):
         """raw_audio CUDA [B, S, L] (or [B, L] when mono) -> [B, S, hop * (L // hop)], as the reference's forward"""
         x = self.check_input(raw_audio)
         B, S, L = x.shape
         dev, dim, nb, NB = x.device, self.dim, len(self.bands), self.n_fft // 2 + 1
-        W, sd = self._weights(), self.bias
         cplx = ops.stft(x.view(B * S, L), self.n_fft, self.hop)                     # [B*S, T, NB, 2]
         T = cplx.shape[1]
         off = np.concatenate([[0], np.cumsum(self.bands)])
         feat = ops.bs_band_input(cplx, B, S, torch.tensor(off, dtype=torch.int32).to(dev),
                                  torch.empty((B * T, 2 * S * NB), device=dev))
-        h = torch.empty((B * T, nb * dim), device=dev)
-        for i in range(nb):
-            ops.linear_into(feat[:, 2 * S * off[i]:2 * S * off[i + 1]], W[f"band.{i}"], h[:, i * dim:(i + 1) * dim],
-                            bias=sd[f"band.{i}.b"])
+        x = self._band_split(feat, off, B * T)
         del feat
-        x = h.view(B * T * nb, dim)
         cs_t, cs_f = self._rope_table(T), self._rope_table(nb)
         for i in range(self.depth):
             x = self._transformer(x, f"layers.{i}.0", self.t_depth, cs_t, T, (B, T * nb, nb, 1, nb))
             x = self._transformer(x, f"layers.{i}.1", self.f_depth, cs_f, nb, (B * T, nb, 1, 0, 1))
         xn = ops.row_l2norm(x).view(B * T, nb * dim)
         del x
-        mask = torch.empty((B * T, 2 * S * NB), device=dev)
-        for i in range(nb):
-            hc = xn[:, i * dim:(i + 1) * dim]
-            for k in range(self.mask_depth):
-                w = W[f"mask.{i}.{k}"]
-                last = k == self.mask_depth - 1
-                hc = ops.linear_into(hc, w, torch.empty((B * T, w.D0), device=dev), bias=sd[f"mask.{i}.{k}.b"],
-                                     act=ops.ACT_NONE if last else ops.ACT_TANH)
-            ops.glu_into(hc, mask[:, 2 * S * off[i]:2 * S * off[i + 1]])
+        mask = self._mask_estimator(xn, off, torch.empty((B * T, 2 * S * NB), device=dev))
         del xn
         out = ops.istft(cplx, B, S, self.n_fft, self.hop, mask=mask)
         return out.view(B, S, -1)

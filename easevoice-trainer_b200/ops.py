@@ -2180,20 +2180,58 @@ def bs_band_input(cplx, B, S, band_off, out):
     return out
 
 
-def istft(cplx, B, S, n_fft, hop, mask=None, out=None, work=None):
+def istft(cplx, B, S, n_fft, hop, mask=None, out=None, work=None, length=None):
     """torch.istft(center=True, Hann(n_fft)) of cplx [B*S, T, n_fft/2+1, 2] (times the complex mask [B*T, (f s c)] when given)
-    -> [B*S, hop*(T-1)] (evk_istft).  work: scratch of B*S*T*n_fft floats (allocated when None)."""
+    -> [B*S, hop*(T-1)] (evk_istft), or [B*S, length] as torch.istft(length=length) (evk_istft_length).  work: scratch of
+    B*S*T*n_fft floats (allocated when None)."""
     T = cplx.shape[1]
     assert cplx.is_contiguous() and cplx.shape[2] == n_fft // 2 + 1
     if out is None:
-        out = torch.empty((B * S, hop * (T - 1)), device=cplx.device, dtype=torch.float32)
+        out = torch.empty((B * S, hop * (T - 1) if length is None else length), device=cplx.device, dtype=torch.float32)
     if work is None:
         work = torch.empty(B * S * T * n_fft, device=cplx.device, dtype=torch.float32)
     assert work.numel() >= B * S * T * n_fft and out.stride(1) == 1
     if mask is not None:
         assert mask.stride(1) == 1 and mask.shape[0] == B * T
-    _call("evk_istft", _p(cplx), _p(mask), mask.stride(0) if mask is not None else 0, B, S, T, n_fft, hop, _p(work), _p(out),
-          out.stride(0))
+    ldm = mask.stride(0) if mask is not None else 0
+    if length is None:
+        _call("evk_istft", _p(cplx), _p(mask), ldm, B, S, T, n_fft, hop, _p(work), _p(out), out.stride(0))
+    else:
+        _call("evk_istft_length", _p(cplx), _p(mask), ldm, B, S, T, n_fft, hop, int(length), _p(work), _p(out), out.stride(0))
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
+# Mel-Band Roformer (mel_band_roformer.py): overlapping band input, averaged band masks, RMSNorm with gamma
+# ------------------------------------------------------------------------------------------------
+def melband_input(cplx, B, S, band_off, bins, out):
+    """evk_melband_input: cplx [B*S, T, n_bins, 2] (ops.stft) -> out [B*T, >= 2*S*len(bins)]: band i's bins
+    bins[band_off[i]:band_off[i+1]] in 'b t (f s c)' order, each band's segment L2-normalised; band_off, bins int32 device."""
+    _, T, nb, _ = cplx.shape
+    assert cplx.is_contiguous() and out.stride(1) == 1 and band_off.dtype == torch.int32 and bins.dtype == torch.int32
+    assert out.shape[0] == B * T and out.shape[1] >= 2 * S * bins.numel()
+    _call("evk_melband_input", _p(cplx), B, S, T, nb, _p(band_off), _p(bins), band_off.numel() - 1, _p(out), out.stride(0))
+    return out
+
+
+def melband_mask_avg(g, S, cover_off, cover, out):
+    """evk_melband_mask_avg: band-major complex masks g [rows, 2*S*n_slots] -> out [rows, 2*S*n_bins] (evk_istft's mask
+    layout), each (bin, channel) the mean over the bands covering the bin; cover_off int32 device [n_bins + 1], cover int32
+    device: the slots of each bin in ascending band order."""
+    rows = g.shape[0]
+    n_bins = cover_off.numel() - 1
+    assert g.stride(1) == 1 and out.stride(1) == 1 and out.shape == (rows, 2 * S * n_bins)
+    assert cover_off.dtype == torch.int32 and cover.dtype == torch.int32
+    _call("evk_melband_mask_avg", _p(g), g.stride(0), _p(cover_off), _p(cover), S, n_bins, rows, _p(out), out.stride(0))
+    return out
+
+
+def row_rmsnorm(x, gamma, out=None):
+    """x / max(||x||_2, 1e-12) * sqrt(C) * gamma per row of a [rows, C] view (evk_row_rmsnorm); out may be x"""
+    rows, C = x.shape
+    assert x.stride(1) == 1 and gamma.is_contiguous() and gamma.numel() == C and gamma.dtype == torch.float32
+    out = torch.empty((rows, C), device=x.device, dtype=torch.float32) if out is None else out
+    _call("evk_row_rmsnorm", _p(x), x.stride(0), _p(gamma), _p(out), out.stride(0), rows, C)
     return out
 
 

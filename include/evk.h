@@ -615,6 +615,32 @@ int evk_bs_band_input(const float* cplx, int32_t B, int32_t S, int32_t T, int32_
 /* y[r] = x[r] / max(||x[r]||_2, 1e-12) per row (F.normalize(dim=-1): the RMSNorms, whose gamma * sqrt(dim) the caller folds
  * into the next Linear's weight columns). */
 int evk_row_l2norm(const float* x, int32_t ldx, float* y, int32_t ldy, int64_t rows, int32_t C, evk_stream_t stream);
+/* evk_istft with torch.istft's length=length: out gets `length` samples per row, computed by the same overlap-add (past
+ * hop*(T-1) from the frames' tails); 0 < length < hop*(T-1) + n_fft/2. */
+int evk_istft_length(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft,
+                     int32_t hop, int32_t length, float* work, float* out, int32_t ld_out, evk_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Mel-Band Roformer (mel_band_roformer.py; lib_v5/vr_network/mel_band_roformer.py:244-478), mel_roformer.cu.  The bands
+ * overlap: band i holds the bins bins[band_off[i] .. band_off[i+1]) (ascending), and a bin may belong to two bands.
+ * ------------------------------------------------------------------------------------------ */
+/* Band-split operand (mel_band_roformer.py:419-425 and each band's RMSNorm before its Linear): from evk_stft_fwd's cplx
+ * [B*S*T][n_bins][2] (rows b*S + s) to y [B*T][ld_y], row (b, t), column (j S + s) * 2 + c for slot j of the bin table
+ * (bin bins[j]), with the columns [2 S band_off[i], 2 S band_off[i+1]) of band i divided by max(their L2 norm, 1e-12).
+ * band_off: device int32 [n_bands + 1]; bins: device int32 [band_off[n_bands]], each < n_bins.  S = 1 or 2; 2 S n_bins
+ * floats must fit 48 KB; ld_y >= 2 S band_off[n_bands]. */
+int evk_melband_input(const float* cplx, int32_t B, int32_t S, int32_t T, int32_t n_bins, const int32_t* band_off,
+                      const int32_t* bins, int32_t n_bands, float* y, int32_t ldy, evk_stream_t stream);
+/* Averaged mask (mel_band_roformer.py:455-466): g [rows][ldg] holds the mask estimators' complex outputs in the band-split
+ * column order of evk_melband_input.  mask [rows][ld_mask] at columns 2 (f S + s) .. +1 (evk_istft's mask layout) gets the
+ * sum over k in [cover_off[f], cover_off[f+1]) of g's complex pair (cover[k] S + s), summed in that order, divided by the
+ * count cover_off[f+1] - cover_off[f] (>= 1).  cover lists the slots of bin f in ascending band order.  No atomics. */
+int evk_melband_mask_avg(const float* g, int32_t ldg, const int32_t* cover_off, const int32_t* cover, int32_t S, int32_t n_bins,
+                         int64_t rows, float* mask, int32_t ld_mask, evk_stream_t stream);
+/* y[r] = x[r] / max(||x[r]||_2, 1e-12) * sqrt(C) * gamma per row (RMSNorm with its gamma, the output norm of each
+ * Transformer; in fp32 in that order).  gamma: device [C].  y may be x (in place, ldy == ldx). */
+int evk_row_rmsnorm(const float* x, int32_t ldx, const float* gamma, float* y, int32_t ldy, int64_t rows, int32_t C,
+                    evk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * UVR5 VR front and back end (SeparateVR.separate, uvr5/separate.py:103-196; spec_utils.py), vr_wave.cu.  Frame sizes are

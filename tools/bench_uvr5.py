@@ -29,7 +29,12 @@ restatement, which makes the numpy / scipy calls librosa makes, around uvr5.infe
 host back end; and, in a separate profiled call, the device time of the new front / back-end kernels against the net.
 The parameter sets are read from tests/golden/uvr5_wave.pt.
 
-Usage:  python tools/bench_uvr5.py [--net vr|deecho|dereverb|roformer] [--wave] [--frames 16538] [--tta 0] [--max-windows 16]
+--net melroformer measures the Mel-Band Roformer (mel_band_roformer.py, the widely distributed vocal model's configuration
+with seeded weights) the same way on the same mix, with the two new kernel families (evk_melband_input,
+evk_melband_mask_avg) split out of the device time, and oracle/mel_roformer_oracle.py's forward as the stock PyTorch arms.
+It skips the rope_attn rates, whose shapes are the BS-Roformer's.
+
+Usage:  python tools/bench_uvr5.py [--net vr|deecho|dereverb|roformer|melroformer] [--wave] [--frames 16538] [--tta 0] [--max-windows 16]
         [--reps 3]
 """
 import argparse
@@ -46,6 +51,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from oracle import bs_roformer_oracle as BR  # noqa: E402
+from oracle import mel_roformer_oracle as MR  # noqa: E402
 from oracle import uvr5_echo_oracle as E  # noqa: E402
 from oracle import uvr5_oracle as O  # noqa: E402
 
@@ -244,30 +250,40 @@ FAMILIES = (("gemm", ("evk_gconv_fwd",)), ("attention", ("evk_rope_attn_fwd",)),
             ("norms", ("evk_row_l2norm", "evk_bs_band_input")), ("stft_istft", ("evk_stft_fwd", "evk_istft")))
 
 
-def torch_roformer_demix(P, cfg, mix, half, autocast):
+def torch_roformer_demix(P, cfg, mix, half, autocast, forward=BR.forward):
     """SeparateMDXC.demix_track on stock PyTorch: the oracle's forward on the GPU (half: chunks cast to fp16 as the
     reference does under cfg.is_half; the weights are whatever P holds), batches of 4, each batch's output copied to the host
-    and accumulated there"""
+    and accumulated there.  forward: the BS-Roformer oracle's, or the Mel-Band Roformer oracle's"""
     from torch.nn.attention import SDPBackend, sdpa_kernel
     dev = torch.device("cuda")
 
     def net(a):
         a = a.to(dev)
         with torch.autocast("cuda", enabled=autocast), sdpa_kernel([SDPBackend.MATH, SDPBackend.EFFICIENT_ATTENTION]):
-            return BR.forward(P, cfg, a.half() if half else a).float().cpu()
+            return forward(P, cfg, a.half() if half else a).float().cpu()
 
     return BR.demix_track(net, mix)["vocals"]
 
 
+MEL_FAMILIES = (("gemm", ("evk_gconv_fwd",)), ("attention", ("evk_rope_attn_fwd",)), ("norms", ("evk_row_l2norm", "evk_row_rmsnorm")),
+                ("melband_input", ("evk_melband_input",)), ("melband_mask_avg", ("evk_melband_mask_avg",)),
+                ("stft_istft", ("evk_stft_fwd", "evk_istft", "evk_istft_length")))
+
+
 def roformer_main(a):
     assert torch.cuda.is_available(), "needs a GPU"
-    from easevoice_trainer_b200 import bs_roformer, lib, ops
+    from easevoice_trainer_b200 import bs_roformer, lib, mel_band_roformer, ops
     lib.init().evk_set_precise(0)
-    cfg = dict(BR.SHIPPED)
-    P = BR.init_params(BR.param_spec(cfg), 81)
-    model = bs_roformer.BSRoformer(**cfg).to("cuda").load_state_dict(P)
+    if a.net == "melroformer":
+        cfg, families, forward = dict(MR.DEFAULT), MEL_FAMILIES, MR.forward
+        P = MR.init_params(MR.param_spec(cfg), 181)
+        model = mel_band_roformer.MelBandRoformer(**cfg).to("cuda").load_state_dict(P)
+    else:
+        cfg, families, forward = dict(BR.SHIPPED), FAMILIES, BR.forward
+        P = BR.init_params(BR.param_spec(cfg), 81)
+        model = bs_roformer.BSRoformer(**cfg).to("cuda").load_state_dict(P)
     mix = BR.make_audio(7, (2, 7938000))
-    res = dict(gpu=gpu_info(), net="roformer", samples=mix.shape[1], chunks=-(-mix.shape[1] // BR.CHUNK), max_chunks=a.max_chunks)
+    res = dict(gpu=gpu_info(), net=a.net, samples=mix.shape[1], chunks=-(-mix.shape[1] // BR.CHUNK), max_chunks=a.max_chunks)
     t = time.perf_counter()
     out = bs_roformer.demix_track(model, mix, "cuda", a.max_chunks)["vocals"]
     res["evk_first_call_s"] = round(time.perf_counter() - t, 3)
@@ -281,14 +297,15 @@ def roformer_main(a):
     model.forward(batch)
     prof = ops.profile_end()
     tot = sum(v["ms"] for v in prof.values())
-    fam = {name: round(sum(v["ms"] for k, v in prof.items() if k.split(":")[0] in keys), 2) for name, keys in FAMILIES}
+    fam = {name: round(sum(v["ms"] for k, v in prof.items() if k.split(":")[0] in keys), 2) for name, keys in families}
     fam["other"] = round(tot - sum(fam.values()), 2)
     res["forward_ms_by_family"] = fam
     res["forward_device_ms"] = round(tot, 2)
-    gemm_fl = sum(v["flops"] for k, v in prof.items() if k.split(":")[0] in FAMILIES[0][1])
+    gemm_fl = sum(v["flops"] for k, v in prof.items() if k.split(":")[0] in families[0][1])
     res["chunk_tflop_gemm"] = round(gemm_fl / a.max_chunks / 1e12, 2)
     res["gemm_tflops_in_forward"] = round(gemm_fl / fam["gemm"] / 1e9, 1)
-    res["rope_attn"] = rope_attn_rates(ops)
+    if a.net == "roformer":
+        res["rope_attn"] = rope_attn_rates(ops)
     if not a.skip_torch:
         torch.backends.cudnn.allow_tf32 = True
         small = BR.make_audio(8, (2, BR.CHUNK))
@@ -296,7 +313,7 @@ def roformer_main(a):
         # accuracy yardstick: the same algorithm in fp32 with TF32 off (one run, not timed)
         torch.backends.cuda.matmul.allow_tf32 = False
         Pd = {k: v.cuda() for k, v in P.items()}
-        exact = torch_roformer_demix(Pd, cfg, mix, False, False)
+        exact = torch_roformer_demix(Pd, cfg, mix, False, False, forward)
         res["evk_rel_l2_vs_torch_fp32"] = rel(out, exact)
         torch.backends.cuda.matmul.allow_tf32 = True
         # (name, weights in fp16, chunks in fp16, autocast): the shipped cfg.is_half path, then fp32 with TF32 allowed
@@ -305,7 +322,7 @@ def roformer_main(a):
             name, wh, ch, ac = arms.pop(0)
             Pd = {k: (v.half() if wh else v).cuda() for k, v in P.items()}
             try:
-                torch_roformer_demix(Pd, cfg, small, ch, ac)                           # warm-up
+                torch_roformer_demix(Pd, cfg, small, ch, ac, forward)                  # warm-up
             except RuntimeError as e:
                 if name != "torch_fp16":
                     raise
@@ -313,9 +330,9 @@ def roformer_main(a):
                 res["torch_fp16_error"] = f"{type(e).__name__}: {str(e)[:300]}"
                 arms.insert(0, ("torch_autocast_fp32_weights", False, False, True))
                 continue
-            ts = timed(lambda: torch_roformer_demix(Pd, cfg, mix, ch, ac), a.reps)
+            ts = timed(lambda: torch_roformer_demix(Pd, cfg, mix, ch, ac, forward), a.reps)
             res[name + "_s"] = [round(t, 3) for t in ts]
-            ref = torch_roformer_demix(Pd, cfg, mix, ch, ac)
+            ref = torch_roformer_demix(Pd, cfg, mix, ch, ac, forward)
             res[name + "_rel_l2_vs_evk"] = rel(ref, out)
             res[name + "_rel_l2_vs_torch_fp32"] = rel(ref, exact)
             del Pd
@@ -379,7 +396,7 @@ def wave_main(a):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--net", choices=("vr", "deecho", "dereverb", "roformer"), default="vr")
+    ap.add_argument("--net", choices=("vr", "deecho", "dereverb", "roformer", "melroformer"), default="vr")
     ap.add_argument("--max-chunks", type=int, default=4)
     ap.add_argument("--frames", type=int, default=16538)
     ap.add_argument("--tta", type=int, default=0)
@@ -390,7 +407,7 @@ def main():
     a = ap.parse_args()
     if a.wave:
         return wave_main(a)
-    if a.net == "roformer":
+    if a.net in ("roformer", "melroformer"):
         return roformer_main(a)
     if a.net != "vr":
         return echo_main(a)
