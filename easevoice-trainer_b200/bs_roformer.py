@@ -63,6 +63,7 @@ class AxialRoformer:
         self.n_fft, self.hop = n_fft, int(hop)
         self.mask_depth = int(mask_estimator_depth)
         self.mask_linears = int(mask_linears)           # Linears per mask MLP (tanh between them)
+        self.chunk_size = CHUNK                         # demix_track's chunk length
         self.device = torch.device("cpu")
         self.host_w, self.bias = None, None
         self._packed = {}
@@ -362,19 +363,20 @@ def zeroed_samples(n, c=CHUNK, batch=BATCH):
 @torch.no_grad()
 def demix_track(model, mix, device="cuda", max_chunks=4):
     """SeparateMDXC.demix_track(model, mix, device) on the device: mix [S, n] (torch or numpy, fp32) -> {"vocals": np.ndarray
-    [S, n]}.  Chunks of CHUNK samples with no overlap; the last is reflect-padded when longer than CHUNK // 2 + 1, else
-    zero-padded.  `max_chunks` chunks go through the model per call and the result reaches the host once.  Each chunk's
-    output is the model's output, except the samples whose fade weight is 0 under the reference's batches of four, which are
-    0 (the reference divides 0 by 0 there and replaces the NaN)."""
+    [S, n]}, or for a model with several targets {"vocals": target 0, "other": target 1} (the reference's zip over the
+    target axis of its estimate).  Chunks of model.chunk_size samples (CHUNK for the roformers) with no overlap; the last is
+    reflect-padded when longer than half a chunk + 1, else zero-padded.  `max_chunks` chunks go through the model per call
+    and the result reaches the host once.  Each chunk's output is the model's output, except the samples whose fade weight
+    is 0 under the reference's batches of four, which are 0 (the reference divides 0 by 0 there and replaces the NaN)."""
     mix = np.asarray(mix.cpu().numpy() if torch.is_tensor(mix) else mix, dtype=np.float32)
     if mix.ndim != 2 or mix.shape[1] < 1:
         raise ValueError(f"mix must be [channels, samples], got {mix.shape}")
     if max_chunks < 1:
         raise ValueError("max_chunks must be >= 1")
-    if CHUNK % model.hop:
-        raise ValueError(f"the model's hop {model.hop} must divide the chunk length {CHUNK}")
+    c = int(model.chunk_size)
+    if c % model.hop:
+        raise ValueError(f"the model's hop {model.hop} must divide the chunk length {c}")
     S, n = mix.shape
-    c = CHUNK
     starts, lengths, _ = chunk_plan(n, c)
     tail = mix[:, starts[-1]:]
     if lengths[-1] < c:
@@ -382,12 +384,17 @@ def demix_track(model, mix, device="cuda", max_chunks=4):
         tail = np.pad(tail, pad, mode="reflect") if lengths[-1] > c // 2 + 1 else np.pad(tail, pad)
     padded = torch.from_numpy(np.ascontiguousarray(np.concatenate([mix[:, :starts[-1]], tail], 1))).to(device)
     nch = len(starts)
-    out = torch.empty((S, nch * c), device=device, dtype=torch.float32)
+    out = None
     for j0 in range(0, nch, max_chunks):
         k = min(max_chunks, nch - j0)
         batch = padded[:, j0 * c:(j0 + k) * c].reshape(S, k, c).transpose(0, 1).contiguous()
-        out.view(S, nch, c)[:, j0:j0 + k] = model.forward(batch).transpose(0, 1)
+        y = model.forward(batch)
+        y = y.view(k, -1, S, c)                                     # [chunks, targets, S, c]
+        if out is None:
+            out = torch.empty((y.shape[1], S, nch * c), device=device, dtype=torch.float32)
+        out.view(-1, S, nch, c)[:, :, j0:j0 + k] = y.permute(1, 2, 0, 3)
     z = zeroed_samples(n, c)
     if len(z):
-        out[:, torch.from_numpy(z).to(device)] = 0.0
-    return {"vocals": out[:, :n].cpu().numpy()}
+        out[..., torch.from_numpy(z).to(device)] = 0.0
+    est = out[..., :n].cpu().numpy()
+    return {k: v for k, v in zip(["vocals", "other"], est)}

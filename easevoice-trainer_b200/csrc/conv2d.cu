@@ -13,6 +13,7 @@
 //                  ring in the 128-byte-swizzle layout, operands rounded to TF32 in shared memory.
 //                * mma.sync m16n8k8: everything else (the 2-channel first layer, the bridges) and 3xTF32 under
 //                  evk_set_precise(1).  Eight warps of 32 x 32 over 64 columns, a 3-stage cp.async ring.
+//                Kernel 1, 2 (the MDX23C 2x2 stride-2 downscale) or 3.
 //                Fused epilogue: y = act(acc * scale[n] + bias[n]).  Every output is summed over K in one fixed order
 //                that does not depend on the pixel's place in the launch, and there are no atomics, so a window gives
 //                the same bits alone or in a batch.
@@ -40,6 +41,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   if (act == EVK_C2_RELU) return fmaxf(v, 0.f);
   if (act == EVK_C2_LRELU) return v >= 0.f ? v : 0.01f * v;
   if (act == EVK_C2_SIGMOID) return 1.f / (1.f + __expf(-v));
+  if (act == EVK_C2_GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
   return v;
 }
 
@@ -513,10 +515,10 @@ extern "C" int evk_conv2d_fwd_hw(const float* x, int32_t x_pitch, int64_t x_bs, 
   EVK_REQUIRE(x && w && y, EVK_ERR_ARG, "conv2d: null tensor");
   EVK_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && N > 0, EVK_ERR_ARG, "conv2d: bad sizes B=%d H=%d W=%d C=%d N=%d", B, H, W,
               C, N);
-  EVK_REQUIRE((k == 1 || k == 3) && (stride == 1 || stride == 2) && pad_h >= 0 && pad_w >= 0 && dil_h >= 1 && dil_w >= 1,
-              EVK_ERR_ARG, "conv2d: kernel %d stride %d pad (%d, %d) dilation (%d, %d) (kernel 1 or 3, stride 1 or 2)", k,
+  EVK_REQUIRE((k >= 1 && k <= 3) && (stride == 1 || stride == 2) && pad_h >= 0 && pad_w >= 0 && dil_h >= 1 && dil_w >= 1,
+              EVK_ERR_ARG, "conv2d: kernel %d stride %d pad (%d, %d) dilation (%d, %d) (kernel 1, 2 or 3, stride 1 or 2)", k,
               stride, pad_h, pad_w, dil_h, dil_w);
-  EVK_REQUIRE(act >= EVK_C2_NONE && act <= EVK_C2_SIGMOID, EVK_ERR_ARG, "conv2d: bad activation %d", act);
+  EVK_REQUIRE(act >= EVK_C2_NONE && act <= EVK_C2_GELU, EVK_ERR_ARG, "conv2d: bad activation %d", act);
   EVK_REQUIRE(x_pitch >= C && y_pitch >= N, EVK_ERR_ARG, "conv2d: pitch smaller than the channel count");
   const int span_h = dil_h * (k - 1) + 1, span_w = dil_w * (k - 1) + 1;
   EVK_REQUIRE(H + 2 * pad_h >= span_h && W + 2 * pad_w >= span_w, EVK_ERR_ARG, "conv2d: input smaller than the kernel");

@@ -301,6 +301,25 @@ __global__ void zero_kernel(float* p, int n) {
 // first sample, which keeps the one-pass variance stable on DC-heavy inputs), pass 2 normalises (+ optional exact GELU).
 // With lens, item b is normalised over its first n = lens[b] frames only and frames t >= n are written as 0: the sums visit
 // t = lane, lane + 8, ... < n in a fixed order, so the statistics of a row depend neither on T nor on what the padding holds.
+// The split form (instnorm_part_kernel, instnorm_apply_kernel) shares the sums and the normalisation below.
+
+// shifted sums of channel c over frames t0 + tl, t0 + tl + 8, ... < t1
+__device__ __forceinline__ void instnorm_sums(const float* xb, int ldx, int c, float shift, long long t0, long long t1, int tl,
+                                              float& s1, float& s2) {
+  for (long long t = t0 + tl; t < t1; t += 8) { const float v = xb[t * ldx + c] - shift; s1 += v; s2 += v * v; }
+}
+// (scale, offset) of y = x * scale + offset from the shifted sums a, q over n frames
+__device__ __forceinline__ float2 instnorm_coef(float a, float q, float n, float shift, float gamma, float beta, float eps) {
+  const float md = a / n, var = fmaxf(q / n - md * md, 0.f);
+  const float mean = md + shift, rstd = rsqrtf(var + eps), g = gamma * rstd, bb = beta - mean * g;
+  return make_float2(g, bb);
+}
+__device__ __forceinline__ float instnorm_apply(float x, float2 gb, int act_gelu) {
+  float v = x * gb.x + gb.y;
+  if (act_gelu) v = 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
+  return v;
+}
+
 __global__ void __launch_bounds__(256) instnorm_cl_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ gamma,
                                                           const float* __restrict__ beta, float eps, int act_gelu, float* __restrict__ y,
                                                           int ldy, int T, int C, const int* __restrict__ lens) {
@@ -311,8 +330,7 @@ __global__ void __launch_bounds__(256) instnorm_cl_kernel(const float* __restric
   const bool ok = c < C;
   const float shift = ok ? xb[c] : 0.f;
   float s1 = 0.f, s2 = 0.f;
-  if (ok)
-    for (int t = tl; t < n; t += 8) { const float v = xb[(long long)t * ldx + c] - shift; s1 += v; s2 += v * v; }
+  if (ok) instnorm_sums(xb, ldx, c, shift, 0, n, tl, s1, s2);
   __shared__ float sh1[8][32], sh2[8][32];
   sh1[tl][threadIdx.x & 31] = s1; sh2[tl][threadIdx.x & 31] = s2;
   __syncthreads();
@@ -320,14 +338,50 @@ __global__ void __launch_bounds__(256) instnorm_cl_kernel(const float* __restric
 #pragma unroll
   for (int i = 0; i < 8; ++i) { a += sh1[i][threadIdx.x & 31]; q += sh2[i][threadIdx.x & 31]; }
   if (!ok) return;
-  const float md = a / (float)n, var = fmaxf(q / (float)n - md * md, 0.f);
-  const float mean = md + shift, rstd = rsqrtf(var + eps), g = gamma[c] * rstd, bb = beta[c] - mean * g;
-  for (int t = tl; t < n; t += 8) {
-    float v = xb[(long long)t * ldx + c] * g + bb;
-    if (act_gelu) v = 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
-    yb[(long long)t * ldy + c] = v;
-  }
+  const float2 gb = instnorm_coef(a, q, (float)n, shift, gamma[c], beta[c], eps);
+  for (int t = tl; t < n; t += 8) yb[(long long)t * ldy + c] = instnorm_apply(xb[(long long)t * ldx + c], gb, act_gelu);
   for (int t = n + tl; t < T; t += 8) yb[(long long)t * ldy + c] = 0.f;
+}
+
+// Split statistics over a plane of T pixels: CTA (32 channels, chunk, item) sums pixels [chunk * per, min(T, (chunk + 1) * per))
+// as instnorm_cl_kernel does (same shift: the item's first pixel) and writes part[chunk][b][{s1, s2}][c]; ordered_sum adds the
+// chunks in chunk order.  `per` depends on T only, so an item's statistics do not depend on B.
+constexpr long long INORM_PER = 2048;
+__global__ void __launch_bounds__(256) instnorm_part_kernel(const float* __restrict__ x, int ldx, long long T, int C,
+                                                            float* __restrict__ part) {
+  const int c = blockIdx.x * 32 + (threadIdx.x & 31), tl = threadIdx.x >> 5, b = blockIdx.z, B = gridDim.z;
+  const float* xb = x + (long long)b * T * ldx;
+  const bool ok = c < C;
+  const float shift = ok ? xb[c] : 0.f;
+  const long long t0 = blockIdx.y * INORM_PER, t1 = min(T, t0 + INORM_PER);
+  float s1 = 0.f, s2 = 0.f;
+  if (ok) instnorm_sums(xb, ldx, c, shift, t0, t1, tl, s1, s2);
+  __shared__ float sh1[8][32], sh2[8][32];
+  sh1[tl][threadIdx.x & 31] = s1; sh2[tl][threadIdx.x & 31] = s2;
+  __syncthreads();
+  if (tl != 0 || !ok) return;
+  float a = 0.f, q = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { a += sh1[i][threadIdx.x & 31]; q += sh2[i][threadIdx.x & 31]; }
+  float* pp = part + ((long long)blockIdx.y * B + b) * 2 * C;
+  pp[c] = a;
+  pp[C + c] = q;
+}
+
+// y = norm(x) (+ GELU) element-wise from the summed statistics stats[b][{s1, s2}][c]
+__global__ void instnorm_apply_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ stats,
+                                      const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int act_gelu,
+                                      float* __restrict__ y, int ldy, int B, long long T, int C) {
+  const long long total = (long long)B * T * C;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const long long p = i / C;
+    const int b = (int)(p / T);
+    const float* st = stats + (long long)b * 2 * C;
+    const float shift = x[b * T * ldx + c];
+    const float2 gb = instnorm_coef(st[c], st[C + c], (float)T, shift, gamma[c], beta[c], eps);
+    y[p * ldy + c] = instnorm_apply(x[p * ldx + c], gb, act_gelu);
+  }
 }
 
 }  // namespace evk
@@ -427,4 +481,25 @@ extern "C" int evk_instnorm_cl(const float* x, int32_t ldx, const float* gamma, 
   EVK_REQUIRE(x && gamma && beta && y && B >= 1 && T >= 1 && C >= 1 && ldx >= C && ldy >= C, EVK_ERR_ARG, "instnorm_cl: bad arguments");
   instnorm_cl_kernel<<<dim3(cdiv(C, 32), B), 256, 0, ST>>>(x, ldx, gamma, beta, eps, act_gelu, y, ldy, T, C, lens);
   return check_launch("instnorm_cl");
+}
+
+extern "C" int evk_instnorm_plane(const float* x, int32_t ldx, const float* gamma, const float* beta, float eps, int32_t act_gelu,
+                                  float* y, int32_t ldy, int32_t B, int64_t T, int32_t C, evk_stream_t stream) {
+  EVK_REQUIRE(x && gamma && beta && y && B >= 1 && T >= 1 && C >= 1 && ldx >= C && ldy >= C, EVK_ERR_ARG,
+              "instnorm_plane: bad arguments");
+  const long long chunks = (T + INORM_PER - 1) / INORM_PER;
+  EVK_REQUIRE(chunks <= 65535 && B <= 65535, EVK_ERR_ARG, "instnorm_plane: plane of %lld pixels too large", (long long)T);
+  Scratch part_buf(chunks * B * 2 * C + (long long)B * 2 * C, ST);
+  float* part = part_buf.p;
+  EVK_REQUIRE(part, EVK_ERR_CUDA, "instnorm_plane: scratch allocation failed");
+  float* stats = part + chunks * B * 2 * C;
+  instnorm_part_kernel<<<dim3(cdiv(C, 32), (unsigned)chunks, B), 256, 0, ST>>>(x, ldx, T, C, part);
+  if (int rc = check_launch("instnorm_part")) return rc;
+  zero_kernel<<<cdiv(2ll * B * C, 256), 256, 0, ST>>>(stats, 2 * B * C);
+  if (int rc = check_launch("instnorm_zero")) return rc;
+  if (int rc = ordered_sum(part, (int)chunks, (long long)B * 2 * C, 1, 1, B * 2 * C, stats, 0, 0, ST)) return rc;
+  const long long total = (long long)B * T * C, blocks = (total + 255) / 256;
+  instnorm_apply_kernel<<<(unsigned)(blocks < kNumSMs * 32 ? blocks : kNumSMs * 32), 256, 0, ST>>>(x, ldx, stats, gamma, beta, eps,
+                                                                                                    act_gelu, y, ldy, B, T, C);
+  return check_launch("instnorm_apply");
 }

@@ -1,4 +1,4 @@
-// General STFT front end and its adjoint (runtime n_fft = 256 .. 4096, hop, win <= n_fft, any reflect padding, per-row
+// General STFT front end and its adjoint (runtime n_fft = 256 .. 8192, hop, win <= n_fft, any reflect padding, per-row
 // lengths): complex spectrum, |X| and log-mel of every frame, one thread block per frame, fp32 Stockham FFT in shared memory
 // (index arithmetic in stft_core.cuh, validated on the host against numpy by tests/test_cpu_stft_core.py).
 //   forward : spectrogram_torch / spec_to_mel_torch / mel_spectrogram_torch of mel_processing.py:40-142 for any
@@ -15,8 +15,8 @@
 
 namespace evk {
 
-__device__ float2 g_stw[STFT_TAB];      // e^{-2 pi i k / 4096}
-__device__ float g_shann[STFT_TAB];     // periodic Hann(4096)
+__device__ float2 g_stw[STFT_TAB];      // e^{-2 pi i k / 8192}
+__device__ float g_shann[STFT_TAB];     // periodic Hann(8192)
 __device__ float2 g_mtw[STFT_TAB_MR];   // e^{-2 pi i k / 61440}: the mixed-radix sizes (stft_core.cuh)
 __device__ float g_mhann[STFT_TAB_MR];  // periodic Hann(61440)
 static bool g_stft_ready = false, g_stft_mr_ready = false;
@@ -235,7 +235,7 @@ __global__ void __launch_bounds__(256) cplx_l1_kernel(const float2* __restrict__
 // stft * mask (bs_roformer.py:530-543): one block per frame (row r = b S + s, frame t) runs the C2R inverse DFT through the same
 // adjoint packing and forward FFT as stft_bwd_kernel (bins 0 and N/2 lose their imaginary parts), windows the frame and writes it
 // to work [(r T + t)][N]; istft_ola_kernel then overlap-adds the frames in frame order and divides by the sum of w^2.
-// Power-of-two sizes run on the 4096-entry tables, the mixed-radix sizes on the STFT_TAB_MR ones.
+// Power-of-two sizes run on the 8192-entry tables, the mixed-radix sizes on the STFT_TAB_MR ones.
 struct IstftP {
   const float2* cplx; const float* mask; int ldm;
   int S, T, N, hop;
@@ -306,7 +306,7 @@ __global__ void istft_ola_kernel(const IstftP p) {
 
 int fill(StftP& p, const float* wav, const int32_t* lens, int B, int L, int ldw, int n_fft, int hop, int win, int pad, int T) {
   EVK_REQUIRE(B > 0 && L > 0 && T > 0 && hop > 0 && pad >= 0 && ldw >= L, EVK_ERR_ARG, "stft: bad sizes B=%d L=%d T=%d hop=%d pad=%d", B, L, T, hop, pad);
-  EVK_REQUIRE(n_fft >= 256 && n_fft <= STFT_TAB && (n_fft & (n_fft - 1)) == 0, EVK_ERR_UNSUPPORTED, "stft: n_fft=%d must be a power of two in [256, 4096]", n_fft);
+  EVK_REQUIRE(n_fft >= 256 && n_fft <= STFT_TAB && (n_fft & (n_fft - 1)) == 0, EVK_ERR_UNSUPPORTED, "stft: n_fft=%d must be a power of two in [256, 8192]", n_fft);
   EVK_REQUIRE(win >= 2 && win <= n_fft && (win & (win - 1)) == 0, EVK_ERR_UNSUPPORTED, "stft: win=%d must be a power of two <= n_fft", win);
   EVK_REQUIRE(pad < L, EVK_ERR_ARG, "stft: reflect padding %d must be smaller than the signal length %d", pad, L);
   EVK_REQUIRE((long long)(T - 1) * hop - pad + n_fft <= (long long)L + pad, EVK_ERR_ARG, "stft: T=%d frames do not fit L=%d with padding %d", T, L, pad);
@@ -388,7 +388,7 @@ int istft_run(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, 
   EVK_REQUIRE(cplx && work && out, EVK_ERR_ARG, "istft: null tensor");
   const bool pow2 = n_fft >= 256 && n_fft <= STFT_TAB && (n_fft & (n_fft - 1)) == 0;
   EVK_REQUIRE(pow2 || stft_mr_size_ok(n_fft), EVK_ERR_UNSUPPORTED,
-              "istft: n_fft=%d must be a power of two in [256, 4096] or an even divisor of %d in [16, 7680]", n_fft, STFT_TAB_MR);
+              "istft: n_fft=%d must be a power of two in [256, 8192] or an even divisor of %d in [16, 7680]", n_fft, STFT_TAB_MR);
   EVK_REQUIRE(B > 0 && S > 0 && T >= 2 && hop > 0 && hop <= n_fft / 2 && (long long)B * S <= 65535, EVK_ERR_ARG,
               "istft: bad sizes B=%d S=%d T=%d hop=%d", B, S, T, hop);
   EVK_REQUIRE(!mask || (ld_mask >= 2 * S * (n_fft / 2 + 1) && (uintptr_t)mask % 8 == 0 && ld_mask % 2 == 0), EVK_ERR_ARG,

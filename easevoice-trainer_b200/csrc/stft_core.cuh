@@ -6,9 +6,11 @@
 //   tw[i]   = (cos(2 pi i / tab), -sin(2 pi i / tab)),  i < tab         (forward twiddles)
 //   hann[i] = 0.5 - 0.5 cos(2 pi i / tab),              i < tab         (periodic Hann of length tab; a window of length `win`
 //             dividing tab is hann[j * (tab / win)], exactly torch.hann_window(win)[j] up to fp32 rounding)
-// Two tables exist: STFT_TAB = 4096 serves the power-of-two sizes (n_fft 256 .. 4096, radix 4 plus one radix-2 pass), and
+// Two tables exist: STFT_TAB = 8192 serves the power-of-two sizes (n_fft 256 .. 8192, radix 4 plus one radix-2 pass), and
 // STFT_TAB_MR = 4096 * 15 every even N dividing it, i.e. N = 2^a 3^b 5^c with a <= 12, b, c <= 1 (the UVR5 band sizes
-// 320, 640, 960 among them).  The functions without a `tab` argument are the power-of-two ones on STFT_TAB.
+// 320, 640, 960 among them).  The functions without a `tab` argument are the power-of-two ones on STFT_TAB.  Entry j * 2 of the
+// 8192-entry tables is bit for bit entry j of a 4096-entry one (2 pi (2j) / 8192 and 2 pi j / 4096 are the same double), and
+// every index scales with tab, so the sizes up to 4096 compute exactly what they did on 4096-entry tables.
 #pragma once
 
 #ifndef EVK_HD
@@ -21,7 +23,7 @@
 
 namespace evk {
 
-constexpr int STFT_TAB = 4096;
+constexpr int STFT_TAB = 8192;
 constexpr int STFT_TAB_MR = 4096 * 15;
 
 EVK_HD float2 stft_cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }

@@ -2077,7 +2077,7 @@ def conv2d(x: CLView, w, y: CLView, *, k, stride=1, pad=0, dil=1, scale=None, bi
     assert (y.H, y.W) == (Ho, Wo), ((y.H, y.W), (Ho, Wo))
     geo = ("evk_conv2d_fwd_hw", ph, pw, dh, dw) if hw else ("evk_conv2d_fwd", ph, dh)
     _call_f(geo[0], 2.0 * x.B * Ho * Wo * N * k * k * x.C, *x.args(), _p(w), _p(scale), _p(bias), *y.args(),
-            x.B, x.H, x.W, x.C, N, k, stride, *geo[1:], act)
+            x.B, x.H, x.W, x.C, N, k, stride, *geo[1:], act, tag=f"k{k}")
 
 
 def dwconv3x3(x: CLView, w, y: CLView, dil):
@@ -2360,3 +2360,69 @@ def glu_into(h, out):
     assert h.stride(1) == 1 and out.stride(1) == 1 and out.shape == (rows, C2 // 2)
     _call("evk_glu_res", None, 0, _p(h), h.stride(0), _p(out), out.stride(0), rows, C2 // 2)
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# MDX23C (mdx23c.py): plane instance norm, TDF Linear, transposed 2x2 conv, spectral layouts, residual adds
+# ------------------------------------------------------------------------------------------------
+C2_GELU = 4
+
+
+def instnorm_plane(x: CLView, gamma, beta, y: CLView, eps=1e-5, gelu_after=True):
+    """nn.InstanceNorm2d(affine=True) over the H*W pixels of each (item, channel) of x (+ exact GELU) into y
+    (evk_instnorm_plane); x and y cover whole [B, H, W] planes, each a channel slice of its buffer."""
+    assert x.r0 == 0 and x.H == x.buf.shape[1] and (y.B, y.H, y.W, y.C) == (x.B, x.H, x.W, x.C)
+    assert gamma.is_contiguous() and beta.is_contiguous() and gamma.numel() == x.C and beta.numel() == x.C
+    _call("evk_instnorm_plane", x.args()[0], x.args()[1], _p(gamma), _p(beta), ctypes.c_float(eps), 1 if gelu_after else 0,
+          y.args()[0], y.args()[1], x.B, x.H * x.W, x.C)
+    return y
+
+
+def mdx_tdf(x: CLView, w, y: CLView, res: CLView = None):
+    """y[b, h, m, :] = sum_k w[m, k] x[b, h, k, :] (+ res) along the frequency (W) axis (evk_mdx_tdf): w [W_out, W_in]"""
+    M, K = w.shape
+    assert w.is_contiguous() and x.W == K and (y.B, y.H, y.W, y.C) == (x.B, x.H, M, x.C), (w.shape, x.W, y.W)
+    (xp, xl, _), (yp, yl, _) = x.args(), y.args()
+    r = res.args() if res is not None else (None, 0, 0)
+    if res is not None:
+        assert (res.B, res.H, res.W, res.C) == (y.B, y.H, y.W, y.C)
+    _call_f("evk_mdx_tdf", 2.0 * x.B * x.H * M * K * x.C, _p(w), xp, xl, K * xl, r[0], r[1],
+            M * r[1], yp, yl, M * yl, x.B * x.H, M, x.C, K)
+    return y
+
+
+def convt2x2(x: CLView, w, y: CLView):
+    """ConvTranspose2d(kernel 2, stride 2, no bias) (evk_convt2x2_fwd): w [2, 2, N, C]; y [B, 2H, 2W, N]"""
+    N = w.shape[2]
+    assert w.is_contiguous() and tuple(w.shape) == (2, 2, N, x.C) and (y.B, y.H, y.W, y.C) == (x.B, 2 * x.H, 2 * x.W, N)
+    assert x.r0 == 0 and y.r0 == 0 and x.H == x.buf.shape[1] and y.H == y.buf.shape[1]
+    _call_f("evk_convt2x2_fwd", 2.0 * x.B * x.H * x.W * 4 * N * x.C, *x.args(), _p(w), *y.args(), x.B, x.H, x.W, x.C, N)
+    return y
+
+
+def mdx_front(cplx, B, S, k, F, y: CLView):
+    """evk_mdx_front: cplx [B*S, T, n_bins, 2] (ops.stft) -> y [B, T, F, 2*S*k] (cac2cws of the first k*F bins)"""
+    _, T, nb, _ = cplx.shape
+    assert cplx.is_contiguous() and y.r0 == 0 and (y.B, y.H, y.W, y.C) == (B, T, F, 2 * S * k)
+    _call("evk_mdx_front", _p(cplx), B, S, T, nb, k, F, y.args()[0], y.args()[1])
+    return y
+
+
+def mdx_back(x: CLView, nt, S, k, n_bins, out=None):
+    """evk_mdx_back: x [B, T, F, nt*2*S*k] -> cplx [B*nt*S, T, n_bins, 2] (cws2cac, zero bins from k*F on)"""
+    B, T, F = x.B, x.H, x.W
+    assert x.r0 == 0 and x.C == nt * 2 * S * k
+    out = torch.empty((B * nt * S, T, n_bins, 2), device=x.buf.device, dtype=torch.float32) if out is None else out
+    assert out.is_contiguous() and tuple(out.shape) == (B * nt * S, T, n_bins, 2)
+    _call("evk_mdx_back", x.args()[0], x.args()[1], B, nt, S, T, n_bins, k, F, _p(out))
+    return out
+
+
+def mdx_add(a: CLView, b: CLView, y: CLView, m: CLView = None):
+    """y = (a + b) * m (evk_mdx_add; m optional) over whole planes of equal shape"""
+    for v in (a, b, y) + ((m,) if m is not None else ()):
+        assert v.r0 == 0 and v.H == v.buf.shape[1] and (v.B, v.H, v.W, v.C) == (a.B, a.H, a.W, a.C)
+    ma = m.args() if m is not None else (None, 0, 0)
+    _call("evk_mdx_add", a.args()[0], a.args()[1], b.args()[0], b.args()[1], ma[0], ma[1], y.args()[0], y.args()[1],
+          a.B * a.H * a.W, a.C)
+    return y

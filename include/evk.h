@@ -173,7 +173,7 @@ int evk_set_mel_variant(int32_t v);
 int evk_mel_bwd(const float* dmel, int32_t ld_dmel, const float* cplx, const float* mel, int32_t ld_mel, const int32_t* lens,
                 int32_t B, int32_t L, int32_t ldw, int32_t hop, int32_t n_mels, const int32_t* fb_ptr, const int32_t* fb_idx,
                 const float* fb_val, float* dwav, evk_stream_t stream);
-/* General STFT (stft.cu): n_fft in {256..4096} (power of two), any hop, power-of-two win <= n_fft (periodic Hann, centred in
+/* General STFT (stft.cu): n_fft in {256..8192} (power of two), any hop, power-of-two win <= n_fft (periodic Hann, centred in
  * the frame as torch.stft does), reflect padding `pad` on both sides, T frames per row starting at f*hop - pad:
  *   mel_processing.py:40-74  -> pad = (n_fft - hop) / 2, T = (L + 2 pad - n_fft) / hop + 1
  *   torch.stft(center=True)  -> pad = n_fft / 2,         T = 1 + L / hop        (bs_roformer.py:565-581, the MR-STFT loss)
@@ -208,6 +208,12 @@ int evk_spec_to_mel(const float* spec, int64_t rows, int32_t ld_spec, int32_t n_
  * fixed summation order (no atomics), so an item's result does not depend on T or on the padding.  NULL: every frame. */
 int evk_instnorm_cl(const float* x, int32_t ldx, const float* gamma, const float* beta, float eps, int32_t act_gelu, float* y,
                     int32_t ldy, int32_t B, int32_t T, int32_t C, const int32_t* lens, evk_stream_t stream);
+/* evk_instnorm_cl without lens for large planes (nn.InstanceNorm2d(affine=True) over the T = H * W pixels of a channels-last
+ * [B, H, W, C] operand, the MDX23C U-Net's norm before every conv and Linear): the same shifted sums, split over chunks of
+ * 2048 pixels whose partials are added in chunk order (no atomics; an item's result does not depend on B), then one
+ * element-wise pass that normalises (+ exact GELU).  Item b's pixels start at x + b T ldx. */
+int evk_instnorm_plane(const float* x, int32_t ldx, const float* gamma, const float* beta, float eps, int32_t act_gelu,
+                       float* y, int32_t ldy, int32_t B, int64_t T, int32_t C, evk_stream_t stream);
 int evk_unary(int32_t op, float alpha, const float* x, int32_t ldx, float* y, int32_t ldy, int64_t rows, int32_t C,
               evk_stream_t stream);
 int evk_unary_bwd(int32_t op, float alpha, const float* x, int32_t ldx, const float* dy, int32_t lddy, float* dx,
@@ -532,9 +538,10 @@ int evk_attn_pad_fwd(const float* q, const float* k, const float* v, int32_t ld,
  * channels-last fp32: pixel (b, y, x) of an operand starts at  p + b*bs + (y*W + x)*pitch  (floats), so a channel slice of
  * a concat buffer is an operand.
  * ------------------------------------------------------------------------------------------ */
-enum evk_conv2d_act { EVK_C2_NONE = 0, EVK_C2_RELU = 1, EVK_C2_LRELU = 2 /* slope 0.01 */, EVK_C2_SIGMOID = 3 };
+enum evk_conv2d_act { EVK_C2_NONE = 0, EVK_C2_RELU = 1, EVK_C2_LRELU = 2 /* slope 0.01 */, EVK_C2_SIGMOID = 3,
+                      EVK_C2_GELU = 4 /* exact erf */ };
 /* y = act(conv2d(x, w) * scale[n] + bias[n])  (scale / bias may be null: 1 / 0).  x: [B, H, W, C] (pitch x_pitch >= C,
- * batch stride x_bs); w: [N][k][k][C] (k = 1 or 3); stride 1 or 2, zero padding pad, dilation dil >= 1; y: [B, Ho, Wo, N]
+ * batch stride x_bs); w: [N][k][k][C] (k = 1, 2 or 3); stride 1 or 2, zero padding pad, dilation dil >= 1; y: [B, Ho, Wo, N]
  * (pitch y_pitch >= N, batch stride y_bs), Ho = (H + 2 pad - dil (k - 1) - 1) / stride + 1.  Implicit GEMM with TF32
  * products and fp32 accumulation: wgmma when C, x_pitch and x_bs are multiples of 4 and x, w are 16-byte aligned,
  * mma.sync otherwise and for 3xTF32 under evk_set_precise(1).  No atomics, and every output's sum has one order whatever
@@ -602,7 +609,7 @@ int evk_rope_attn_fwd(const float* qkvg, int32_t ld, const float* cs, float* o, 
  * 2 (k S + s) .. +1 of mask row b*T + t (pitch ld_mask: the mask estimator's 'b t (f s c)' layout).  Per frame a C2R inverse
  * DFT (imaginary parts of bins 0 and n_fft/2 ignored) and the window, written to work [B*S*T][n_fft]; then the overlap-add in
  * frame order, divided by the sum of squared windows, trimmed by n_fft/2 at both ends: out [B*S][ld_out] gets hop*(T-1)
- * samples per row.  n_fft a power of two in [256, 4096], or an even divisor of 61440 (2^12 3 5) in [16, 7680] (the
+ * samples per row.  n_fft a power of two in [256, 8192], or an even divisor of 61440 (2^12 3 5) in [16, 7680] (the
  * mixed-radix core: the UVR5 VR band sizes 320, 640, 960); T >= 2, hop <= n_fft / 2, B*S <= 65535. */
 int evk_istft(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft, int32_t hop,
               float* work, float* out, int32_t ld_out, evk_stream_t stream);
@@ -619,6 +626,39 @@ int evk_row_l2norm(const float* x, int32_t ldx, float* y, int32_t ldy, int64_t r
  * hop*(T-1) from the frames' tails); 0 < length < hop*(T-1) + n_fft/2. */
 int evk_istft_length(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft,
                      int32_t hop, int32_t length, float* work, float* out, int32_t ld_out, evk_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * UVR5 MDX23C (the TFC-TDF v3 U-Net, mdx23c.py; lib_v5/vr_network/tfc_tdf_v3.py), mdx23c.cu, inference only.  Activations are
+ * channels-last fp32 [B, H, W, C] with the spatial axes (time frames, frequency bins), as the VR nets' operands above.  The
+ * 3x3, 1x1 and 2x2 stride-2 convolutions run on evk_conv2d_fwd, the instance norms on evk_instnorm_plane.
+ * ------------------------------------------------------------------------------------------ */
+/* TDF Linear along the frequency axis: for every slab z < Z (one (item, frame) row of W = K pixels),
+ *   y[z][m][n] = sum_k a[m][k] x[z][k][n] (+ r[z][m][n])
+ * a: the Linear's weight [M][K] contiguous; x row k of slab z at x + z x_zs + k ldx (ldx = the pixel pitch), likewise r, y.
+ * r may be y (in place).  TF32 mma.sync with fp32 accumulation in one K order (3xTF32 under evk_set_precise(1)); no atomics,
+ * bit-reproducible and independent of Z. */
+int evk_mdx_tdf(const float* a, const float* x, int32_t ldx, int64_t x_zs, const float* r, int32_t ldr, int64_t r_zs,
+                float* y, int32_t ldy, int64_t y_zs, int32_t Z, int32_t M, int32_t N, int32_t K, evk_stream_t stream);
+/* ConvTranspose2d(C, N, kernel 2, stride 2, no bias): y[b, 2i + dy, 2j + dx, n] = sum_c x[b, i, j, c] w[dy][dx][n][c]
+ * (w: the reference's [C][N][2][2] weight as [2][2][N][C]).  x [B, H, W, C] (pitch x_pitch, x_bs = H W x_pitch), y [B, 2H,
+ * 2W, N] (pitch y_pitch, y_bs = 4 H W y_pitch): a channel slice of a concat buffer.  Four evk_conv2d_fwd 1x1 launches, one
+ * per output phase, with its precision, determinism and batch independence. */
+int evk_convt2x2_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, float* y, int32_t y_pitch, int64_t y_bs,
+                     int32_t B, int32_t H, int32_t W, int32_t C, int32_t N, evk_stream_t stream);
+/* STFT -> U-Net input (STFT.__call__ and cac2cws): from evk_stft_fwd's cplx [B*S*T][n_bins][2] (rows b*S + s) to
+ * y[b, t, j, (2 s + c) k + u] = cplx[b S + s][t][u F + j][c], j < F, u < k: the first k F bins, channels (s, re/im, subband),
+ * pixel (t, j) at y + ((b T + t) F + j) ldy. */
+int evk_mdx_front(const float* cplx, int32_t B, int32_t S, int32_t T, int32_t n_bins, int32_t k, int32_t F, float* y,
+                  int32_t ldy, evk_stream_t stream);
+/* final_conv output -> evk_istft's input (cws2cac, the target split and STFT.inverse's zero bins): x [B, T, F, ldx] holding
+ * nt * 2 S k channels to cplx [(b nt + g) S + s][t][f][c] = x[b, t, f % F, g 2 S k + (2 s + c) k + f / F] for f < k F, 0 up
+ * to n_bins. */
+int evk_mdx_back(const float* x, int32_t ldx, int32_t B, int32_t nt, int32_t S, int32_t T, int32_t n_bins, int32_t k, int32_t F,
+                 float* cplx, evk_stream_t stream);
+/* y[p][c] = (a[p][c] + b[p][c]) * m[p][c] for P pixels of C channels (row pitches lda, ldb, ldm, ldy; m nullable: no product):
+ * the TFC-TDF residual adds, and the last one's `x * first_conv_out`. */
+int evk_mdx_add(const float* a, int32_t lda, const float* b, int32_t ldb, const float* m, int32_t ldm, float* y, int32_t ldy,
+                int64_t P, int32_t C, evk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Mel-Band Roformer (mel_band_roformer.py; lib_v5/vr_network/mel_band_roformer.py:244-478), mel_roformer.cu.  The bands

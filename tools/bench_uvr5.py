@@ -34,7 +34,13 @@ with seeded weights) the same way on the same mix, with the two new kernel famil
 evk_melband_mask_avg) split out of the device time, and oracle/mel_roformer_oracle.py's forward as the stock PyTorch arms.
 It skips the rope_attn rates, whose shapes are the BS-Roformer's.
 
-Usage:  python tools/bench_uvr5.py [--net vr|deecho|dereverb|roformer|melroformer] [--wave] [--frames 16538] [--tta 0] [--max-windows 16]
+--net mdx23c measures MDX23C (mdx23c.py, the 8K-FFT InstVoc configuration with seeded weights) the same way on the same mix
+(31 chunks of 261 120 samples): demix_track wall time and peak memory, the device time of one profiled forward of
+`--max-chunks` chunks split into 3x3 convs, 2x2 down / up convs, TDF Linears, instance norms, STFT / iSTFT and the rest, the
+conv FLOP rate with FLOPs computed from the layer shapes here, and oracle/mdx23c_oracle.py's forward (the reference module
+restated) as the stock PyTorch arms.
+
+Usage:  python tools/bench_uvr5.py [--net vr|deecho|dereverb|roformer|melroformer|mdx23c] [--wave] [--frames 16538] [--tta 0] [--max-windows 16]
         [--reps 3]
 """
 import argparse
@@ -51,6 +57,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from oracle import bs_roformer_oracle as BR  # noqa: E402
+from oracle import mdx23c_oracle as MX  # noqa: E402
 from oracle import mel_roformer_oracle as MR  # noqa: E402
 from oracle import uvr5_echo_oracle as E  # noqa: E402
 from oracle import uvr5_oracle as O  # noqa: E402
@@ -343,6 +350,117 @@ def roformer_main(a):
 WAVE_FAMILIES = ("evk_vr_band_stft", "evk_vr_mag_norm", "evk_resample_poly", "evk_vr_assemble", "evk_istft")
 
 
+def mdx_conv_flops(cfg, B):
+    """-> {family: FLOPs} of one forward of B chunks, computed from the layer shapes (2 per multiply-add)"""
+    a, m = cfg["audio"], cfg["model"]
+    T, F_ = a["chunk_size"] // a["hop_length"] + 1, a["dim_f"] // m["num_subbands"]
+    k, S, n, l, c, g, bn = (m["num_subbands"], a["num_channels"], m["num_scales"], m["num_blocks_per_scale"],
+                            m["num_channels"], m["growth"], m["bottleneck_factor"])
+    nt = 1 if cfg["training"]["target_instrument"] else len(cfg["training"]["instruments"])
+    D = 2 * S * k
+    fl = dict(conv3x3=0.0, conv2x2=0.0, conv1x1=0.0, tdf=0.0)
+
+    def block(in_c, c, h, w):
+        for _ in range(l):
+            fl["conv3x3"] += 2 * B * h * w * 9 * (in_c * c + c * c)
+            fl["conv1x1"] += 2 * B * h * w * in_c * c
+            fl["tdf"] += 2 * 2 * B * h * c * w * (w // bn)
+            in_c = c
+
+    h, w = T, F_
+    fl["conv1x1"] += 2 * B * h * w * D * c + 2 * B * h * w * ((c + D) * c + c * nt * D)
+    for _ in range(n):
+        block(c, c, h, w)
+        fl["conv2x2"] += 2 * B * (h // 2) * (w // 2) * 4 * c * (c + g)
+        h, w, c = h // 2, w // 2, c + g
+    block(c, c, h, w)
+    for _ in range(n):
+        fl["conv2x2"] += 2 * B * h * w * 4 * c * (c - g)
+        h, w, c = h * 2, w * 2, c - g
+        block(2 * c, c, h, w)
+    return fl
+
+
+MDX_FAMILIES = (("conv3x3_1x1", ("evk_conv2d_fwd",)), ("conv2x2_down", ("evk_conv2d_fwd_k2",)),
+                ("conv2x2_up", ("evk_convt2x2_fwd",)), ("tdf", ("evk_mdx_tdf",)), ("instnorm", ("evk_instnorm_plane",)),
+                ("stft_istft", ("evk_stft_fwd", "evk_istft")))
+
+
+def mdx_main(a):
+    """--net mdx23c: MDX23C at the 8K-FFT InstVoc configuration"""
+    assert torch.cuda.is_available(), "needs a GPU"
+    from easevoice_trainer_b200 import bs_roformer, lib, mdx23c, ops
+    lib.init().evk_set_precise(0)
+    cfg = MX.config({})
+    P = MX.init_params(MX.param_spec(cfg), 321)
+    model = mdx23c.MDX23C(cfg).to("cuda").load_state_dict(P)
+    c = cfg["audio"]["chunk_size"]
+    mix = BR.make_audio(7, (2, 7938000))
+    res = dict(gpu=gpu_info(), net=a.net, samples=mix.shape[1], chunks=-(-mix.shape[1] // c), max_chunks=a.max_chunks)
+    t = time.perf_counter()
+    out = bs_roformer.demix_track(model, mix, "cuda", a.max_chunks)
+    res["evk_first_call_s"] = round(time.perf_counter() - t, 3)
+    torch.cuda.reset_peak_memory_stats()
+    ts = timed(lambda: bs_roformer.demix_track(model, mix, "cuda", a.max_chunks), a.reps)
+    res["evk_s"] = [round(t, 3) for t in ts]
+    res["peak_mem_gib"] = round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)
+    batch = mix[:, :a.max_chunks * c].reshape(2, a.max_chunks, c).transpose(0, 1).contiguous().cuda()
+    model.forward(batch)
+    ops.PROF_SHAPES = True                 # conv2d's profile keys then carry the kernel size, which splits 2x2 from 3x3 / 1x1
+    ops.profile_begin()
+    model.forward(batch)
+    prof = ops.profile_end()
+    ops.PROF_SHAPES = False
+    agg = {}
+    for key, v in prof.items():
+        name = key.split("|")[0].split(":")[0]
+        if name == "evk_conv2d_fwd" and key.endswith("|k2"):
+            name = "evk_conv2d_fwd_k2"
+        e = agg.setdefault(name, dict(ms=0.0, flops=0.0))
+        e["ms"] += v["ms"]
+        e["flops"] += v["flops"]
+    tot = sum(v["ms"] for v in agg.values())
+    fam = {name: round(sum(v["ms"] for k, v in agg.items() if k in keys), 2) for name, keys in MDX_FAMILIES}
+    fam["other"] = round(tot - sum(fam.values()), 2)
+    res["forward_ms_by_family"] = fam
+    res["forward_device_ms"] = round(tot, 2)
+    fl = mdx_conv_flops(cfg, a.max_chunks)
+    res["chunk_tflop_by_family"] = {k: round(v / a.max_chunks / 1e12, 3) for k, v in fl.items()}
+    conv_ms = fam["conv3x3_1x1"] + fam["conv2x2_down"] + fam["conv2x2_up"]
+    res["conv_tflops_in_forward"] = round((fl["conv3x3"] + fl["conv1x1"] + fl["conv2x2"]) / conv_ms / 1e9, 1)
+    res["tdf_tflops_in_forward"] = round(fl["tdf"] / fam["tdf"] / 1e9, 1)
+    if not a.skip_torch:
+        rel = lambda x, r: float(np.linalg.norm(x - r) / np.linalg.norm(r))  # noqa: E731
+        small = BR.make_audio(8, (2, c))
+        ev = np.stack([out["vocals"], out["other"]])
+        torch.backends.cudnn.allow_tf32 = True
+        torch.backends.cuda.matmul.allow_tf32 = True
+        arms = [("torch_fp16", True, True, True), ("torch_tf32", False, False, False)]
+        while arms:
+            name, wh, ch, ac = arms.pop(0)
+            Pd = {k: (v.half() if wh else v).cuda() for k, v in P.items()}
+
+            def net(x):
+                x = x.cuda()
+                with torch.no_grad(), torch.autocast("cuda", enabled=ac):
+                    return MX.forward(Pd, cfg, x.half() if ch else x).float().cpu()
+            try:
+                MX.demix_track(net, small, c)                                      # warm-up
+            except RuntimeError as e:
+                if name != "torch_fp16":
+                    raise
+                res["torch_fp16_error"] = f"{type(e).__name__}: {str(e)[:300]}"
+                arms.insert(0, ("torch_autocast_fp32_weights", False, False, True))
+                continue
+            ts = timed(lambda: MX.demix_track(net, mix, c), a.reps)
+            res[name + "_s"] = [round(t, 3) for t in ts]
+            ref = MX.demix_track(net, mix, c)
+            res[name + "_rel_l2_vs_evk"] = rel(np.stack([ref["vocals"], ref["other"]]), ev)
+            del Pd
+            torch.cuda.empty_cache()
+    print(json.dumps(res))
+
+
 def wave_main(a):
     """--wave: uvr5.separate_wave against the reference's host front / back end around uvr5.inference"""
     assert torch.cuda.is_available(), "needs a GPU"
@@ -396,7 +514,7 @@ def wave_main(a):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--net", choices=("vr", "deecho", "dereverb", "roformer", "melroformer"), default="vr")
+    ap.add_argument("--net", choices=("vr", "deecho", "dereverb", "roformer", "melroformer", "mdx23c"), default="vr")
     ap.add_argument("--max-chunks", type=int, default=4)
     ap.add_argument("--frames", type=int, default=16538)
     ap.add_argument("--tta", type=int, default=0)
@@ -409,6 +527,8 @@ def main():
         return wave_main(a)
     if a.net in ("roformer", "melroformer"):
         return roformer_main(a)
+    if a.net == "mdx23c":
+        return mdx_main(a)
     if a.net != "vr":
         return echo_main(a)
     assert torch.cuda.is_available(), "needs a GPU"
