@@ -2426,3 +2426,77 @@ def mdx_add(a: CLView, b: CLView, y: CLView, m: CLView = None):
     _call("evk_mdx_add", a.args()[0], a.args()[1], b.args()[0], b.args()[1], ma[0], ma[1], y.args()[0], y.args()[1],
           a.B * a.H * a.W, a.C)
     return y
+
+
+# ------------------------------------------------------------------------------------------------
+# Whisper transcription (whisper.py): log-mel front end, decode attention with slot tables, beam step
+# ------------------------------------------------------------------------------------------------
+def whisper_logmel(wav, lens, basis, fb, out=None):
+    """evk_whisper_logmel: wav [B, L] fp32 (row b holds lens[b] 16 kHz samples; lens int32 device [B]), basis [2, 400, 201],
+    fb [201, n_mels] -> [B, 3000, n_mels] normalised log-mel, zero after each clip's lens[b] // 160 frames."""
+    assert wav.dim() == 2 and wav.stride(1) == 1 and lens.dtype == torch.int32 and basis.is_contiguous() and fb.is_contiguous()
+    B, M = wav.shape[0], fb.shape[1]
+    out = torch.empty((B, 3000, M), device=wav.device, dtype=torch.float32) if out is None else out
+    assert out.is_contiguous() and out.shape == (B, 3000, M)
+    _call("evk_whisper_logmel", _p(wav), wav.stride(0), _p(lens), B, _p(basis), _p(fb), M, _p(out))
+    return out
+
+
+def whisper_embed(tok, emb, pe, pos, out):
+    """out[r] = emb[tok[r]] + pe[*pos] (evk_whisper_embed)."""
+    _call("evk_whisper_embed", _p(tok), _p(emb), _p(pe), _p(pos), tok.numel(), emb.shape[1], _p(out))
+    return out
+
+
+def whisper_add_pos(x, pe):
+    """x [B, T, d] (contiguous) += pe[:T] in place (evk_whisper_add_pos)."""
+    assert x.is_contiguous() and pe.is_contiguous()
+    B, T, d = x.shape
+    _call("evk_whisper_add_pos", _p(x), B * T, T, d, _p(pe))
+    return x
+
+
+def whisper_self_kv(qkv, pool, tab, pos, S):
+    """Write every row's K | V (columns d..3d of qkv [R, 3d]) into its slot r * S + *pos of pool [R * S, >= 2d] and list the
+    slot in tab [R, >= S] (evk_whisper_self_kv)."""
+    R, d = qkv.shape[0], qkv.shape[1] // 3
+    assert qkv.stride(1) == 1 and pool.stride(1) == 1 and tab.dtype == torch.int32 and tab.stride(1) == 1
+    _call("evk_whisper_self_kv", _p(qkv), qkv.stride(0), d, _p(pool), pool.stride(0), _p(tab), tab.stride(0), _p(pos), R, S)
+
+
+def whisper_attn(q, kv, v_off, heads, out, *, tab=None, pos=None, n_keys, nq=1):
+    """evk_whisper_attn, head dim 64, exact fp32.  tab given: row r attends the pool rows tab[r, :*pos + 1] (n_keys = table
+    width); otherwise rows g * nq + a attend kv rows g * n_keys .. g * n_keys + n_keys - 1 (cross-attention of a clip's beams)."""
+    assert q.stride(1) == 1 and kv.stride(1) == 1 and out.stride(1) == 1
+    groups = q.shape[0] // nq
+    _call_f("evk_whisper_attn", 4.0 * q.shape[0] * heads * n_keys * 64, _p(q), q.stride(0), _p(kv), kv.stride(0), v_off, _p(tab),
+            tab.stride(0) if tab is not None else 0, _p(pos), n_keys, groups, nq, heads, ctypes.c_float(0.125), _p(out), out.stride(0))
+    return out
+
+
+def whisper_layernorm(x, gamma, beta, eps=1e-5):
+    """evk_whisper_layernorm over the last dim of x (any width) -> a new tensor of x's shape."""
+    x = _cl(x.detach())
+    rows, C, ld = _rows(x)
+    y = torch.empty(x.shape, device=x.device, dtype=torch.float32)
+    _call("evk_whisper_layernorm", _p(x), ld, _p(gamma.detach()), _p(beta.detach()), ctypes.c_float(eps), _p(y), C, rows, C)
+    return y
+
+
+def whisper_first_pass(logits, nospeech, lang_ids, nsp, lang_tok):
+    """evk_whisper_first_pass: nsp[r] = softmax(logits[r])[nospeech], lang_tok[r] = argmax of logits[r] over lang_ids."""
+    assert logits.stride(1) == 1 and lang_ids.dtype == torch.int32
+    _call("evk_whisper_first_pass", _p(logits), logits.stride(0), logits.shape[0], logits.shape[1], int(nospeech), _p(lang_ids),
+          lang_ids.numel(), _p(nsp), _p(lang_tok))
+
+
+def whisper_beam_step(logits, st, beam, lay, length_penalty=1.0):
+    """evk_whisper_beam_step on the decode state `st` (whisper.WhisperModel._state) with token layout `lay` =
+    (eot, notimestamps, ts_begin, max_init_ts, prompt_len, max_length)."""
+    clips = logits.shape[0] // beam
+    assert st["fin_seq"].stride(1) == st["hist"].stride(0) and st["tab"].stride(0) <= 448
+    _call("evk_whisper_beam_step", _p(logits), logits.stride(0), clips, beam, logits.shape[1], *[int(v) for v in lay],
+          _p(st["sup"]), st["sup"].numel(), _p(st["bsup"]), st["bsup"].numel(), _p(st["g"]), ctypes.c_float(length_penalty),
+          _p(st["cv"]), _p(st["ci"]), _p(st["score"]), _p(st["hist"]), st["hist"].stride(0), _p(st["tab"]), st["tab"].stride(0),
+          _p(st["tok"]), _p(st["parent"]), _p(st["fin_score"]), _p(st["fin_seq"]), _p(st["fin_len"]),
+          _p(st["fin_flag"]), _p(st["unsat"]))

@@ -758,6 +758,65 @@ int evk_slice_normalize(const float* x, const int64_t* chunks, int32_t n_chunks,
 int evk_fragment_int16(const float* x, const int64_t* frags, const int64_t* dst, int32_t n_frags, int64_t max_len, int64_t gap,
                        int16_t* y, float* m, evk_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Whisper transcription (whisper.py, asr.py), inference only: csrc/whisper.cu.  Token, position and counter arguments
+ * named *_dev / pos / gstep are int32 device scalars, so the decode step replays as a CUDA graph.
+ * ------------------------------------------------------------------------------------------ */
+/* Whisper's log-mel features of B clips of 16 kHz samples: row b of wav [B][ld_wav] holds lens[b] (int32 device, 201 <= lens[b]
+ * <= 480000) samples.  out [B][3000][n_mels]: frame t < lens[b] / 160 of row b is the 400-point periodic-Hann STFT (hop 160,
+ * centre reflect padding) as a direct DFT against basis = [400][201] window * cos | [400][201] -window * sin, |X|^2 @ fb
+ * ([201][n_mels]), log10(max(., 1e-10)), then max(x, clip max - 8) and (x + 4) / 4 with the max over the clip's own frames;
+ * frames from lens[b] / 160 on are 0 (padding in the feature domain).  fp32 FMAs in a fixed order: the same bits alone or in
+ * any batch.  n_mels <= 256, B <= 65535. */
+int evk_whisper_logmel(const float* wav, int64_t ld_wav, const int32_t* lens, int32_t B, const float* basis, const float* fb,
+                       int32_t n_mels, float* out, evk_stream_t stream);
+/* x[r] = emb[tok[r]] + pe[*pos] for r < R (rows of d floats, contiguous). */
+int evk_whisper_embed(const int32_t* tok, const float* emb, const float* pe, const int32_t* pos, int32_t R, int32_t d, float* x,
+                      evk_stream_t stream);
+/* x[r] += pe[r % T] for the rows < rows of x [rows][d] (contiguous): the encoder's fixed positions. */
+int evk_whisper_add_pos(float* x, int64_t rows, int32_t T, int32_t d, const float* pe, evk_stream_t stream);
+/* Self-attention cache without per-step copies: row r < R writes its K | V (columns [d, 3d) of qkv [R][ldq]) once, into slot
+ * s = r * S + *pos of pool (rows of ld_pool floats, K at 0, V at d), and sets tab[r][*pos] = s (tab [R][ld_tab], S <= ld_tab).
+ * A slot is written at most once per decode, so a beam reordering gathers only the tables. */
+int evk_whisper_self_kv(const float* qkv, int32_t ldq, int32_t d, float* pool, int64_t ld_pool, int32_t* tab, int32_t ld_tab,
+                        const int32_t* pos, int32_t R, int32_t S, evk_stream_t stream);
+/* Decode attention, head dim 64, exact fp32 (no tensor cores), softmax(scale q k^T) v per head h < H.  Query row g * nq + a
+ * (a < nq) of q [.][ldq]; output o [.][ldo] at the same row.  K of key row k is kv + k * ld_kv + h * 64, V is v_off further.
+ *   tab != null (self-attention): nq == 1, the keys of group g are rows tab[g][j], j <= *pos, and *pos < n_keys <= ld_tab;
+ *   tab == null (cross-attention): the keys of group g are rows g * n_keys + j, j < n_keys, read once for the group's nq
+ *   (<= 8) queries: the beams of a clip share its cross K / V.
+ * Each row's result depends only on its own query and keys: the same bits in any batch.  kv 16-byte aligned, ld_kv and v_off
+ * multiples of 4; nq * (64 + n_keys) floats of shared memory (<= 200 KB). */
+int evk_whisper_attn(const float* q, int32_t ldq, const float* kv, int64_t ld_kv, int32_t v_off, const int32_t* tab,
+                     int32_t ld_tab, const int32_t* pos, int32_t n_keys, int32_t groups, int32_t nq, int32_t H, float scale,
+                     float* o, int32_t ldo, evk_stream_t stream);
+/* y = LayerNorm(x) * gamma + beta over the C floats of each row < rows of x [rows][ldx] (y [rows][ldy], not in place), any C:
+ * one row per block, mean and centred variance summed in a fixed order, so a row's bits do not depend on the batch. */
+int evk_whisper_layernorm(const float* x, int32_t ldx, const float* gamma, const float* beta, float eps, float* y, int32_t ldy,
+                          int64_t rows, int32_t C, evk_stream_t stream);
+/* The pass at <|startoftranscript|>: per row r < R of logits [R][ld] (V classes), nsp[r] = softmax(row)[nospeech] and
+ * lang_tok[r] = the id in lang_ids [n_lang] (device) with the largest logit (the lowest id on a tie). */
+int evk_whisper_first_pass(const float* logits, int64_t ld, int32_t R, int32_t V, int32_t nospeech, const int32_t* lang_ids,
+                           int32_t n_lang, float* nsp, int32_t* lang_tok, evk_stream_t stream);
+/* One beam-search step of transformers' Whisper generate (num_beams = beam <= 8, early_stopping False) for `clips` clips of
+ * `beam` rows each (row = clip * beam + b).  *gstep = g, the tokens generated so far; the logits [clips * beam][ld] are those
+ * of position plen - 1 + g.  Per row (cand_val / cand_tok [rows][2 beam] scratch): log_softmax; suppress `sup` [n_sup], and
+ * `bsup` [n_bsup] when g == 0 (device lists); WhisperTimeStampLogitsProcessor with eot, nots = <|notimestamps|>, tsb = first
+ * timestamp, mit = max_initial_timestamp_index (< 0: none); plus run_score[row]; the top 2 beam.  Per clip, as
+ * GenerationMixin._beam_search: the top 2 beam of the clip's candidates, the best `beam` non-eot ones become the next rows
+ * (tok, parent = source row, run_score), eot hypotheses among the first `beam` (and all at plen + g + 1 == maxlen) enter the
+ * finished set (fin_score [clips][beam], score / (g + 1)^length_penalty; fin_seq [clips][beam][ld_hist], fin_len, fin_flag),
+ * and unsat[clip] becomes 0 when the running beams can no longer beat it; a clip with unsat == 0 is not touched.  hist
+ * [rows][ld_hist] (generated tokens) and tab [rows][ld_tab] (slot tables, entries <= plen - 1 + g) of the new rows are
+ * gathered from their parents.  The caller advances *gstep.  Everything stays in device memory.  ld_hist, ld_tab <= 448,
+ * maxlen - plen <= ld_hist, maxlen <= ld_tab, V <= 262144. */
+int evk_whisper_beam_step(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot, int32_t nots,
+                          int32_t tsb, int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup, int32_t n_sup,
+                          const int32_t* bsup, int32_t n_bsup, const int32_t* gstep, float length_penalty, float* cand_val,
+                          int32_t* cand_tok, float* run_score, int32_t* hist, int32_t ld_hist, int32_t* tab, int32_t ld_tab,
+                          int32_t* tok, int32_t* parent, float* fin_score, int32_t* fin_seq, int32_t* fin_len, int32_t* fin_flag,
+                          int32_t* unsat, evk_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
