@@ -3,8 +3,10 @@
 
 Differences from the reference, which runs faster-whisper: the model is a local Hugging Face Whisper directory (config.json,
 model.safetensors or pytorch_model.bin, generation_config.json, tokenizer.json), decoding follows transformers' `generate`
-(5 beams, timestamps, at most 224 new tokens) without the temperature-fallback ladder or the VAD filter, and clips are decoded
-in batches.  See INTEGRATION.md.
+(5 beams, timestamps, at most 224 new tokens per 30 s window) without the temperature-fallback ladder, conditioning on the
+previous window or the VAD filter, and clips are decoded in batches.  Clips of at most 30 s are decoded whole; longer ones
+follow transformers' long-form generate (30 s windows moved by the predicted timestamps, `WhisperModel.transcribe_long`),
+with the windows of several clips decoded together.  See INTEGRATION.md.
 """
 import os
 import zlib
@@ -30,11 +32,15 @@ NO_SPEECH_THRESHOLD, LOGPROB_THRESHOLD = 0.6, -1.0
 # device memory for one batch's per-clip buffers: cross K/V (1500 x layers x 2 d fp32) and the self-attention slots of its
 # 5 beams (448 x layers x 2 d fp32 each).  large-v3: 0.49 GB + 0.73 GB per clip, so 16 GiB holds 14 clips
 DEFAULT_MEMORY_BUDGET = 16 << 30
+# share of the budget for a pool of long clips' whole-clip log-mels (fp32 [frames, n_mels]; large-v3: 512 bytes per 10 ms, so
+# 2 GiB of a 16 GiB budget holds about 11.6 hours of audio); the decode batch of long clips takes the rest
+LONG_POOL_SHARE = 1 / 8
 
 
-def read_clip(path):
+def read_clip(path, max_seconds=30):
     """-> float32 16 kHz samples of a 16 or 32 kHz wav (32 kHz through resample_poly(x, 1, 2) with the SSL taps), or raises
-    ValueError.  int16 is scaled by 1 / 32768, float is taken as it is; other sample formats are rejected."""
+    ValueError.  int16 is scaled by 1 / 32768, float is taken as it is; other sample formats are rejected.  max_seconds: the
+    longest clip accepted (None: any length)."""
     from scipy.io import wavfile
     sr, x = wavfile.read(path)
     if sr not in (16000, 32000):
@@ -48,8 +54,8 @@ def read_clip(path):
     else:
         raise ValueError(f"{path}: {x.dtype} samples (int16 or float)")
     n16 = x.size if sr == 16000 else (x.size + 1) // 2
-    if n16 > 30 * 16000:
-        raise ValueError(f"{path}: {n16 / 16000:.2f} s (clips of at most 30 s)")
+    if max_seconds is not None and n16 > max_seconds * 16000:
+        raise ValueError(f"{path}: {n16 / 16000:.2f} s (clips of at most {max_seconds} s)")
     if n16 < 201:
         raise ValueError(f"{path}: {n16} samples at 16 kHz (at least 201)")
     return x, sr
@@ -72,6 +78,26 @@ def is_no_speech(no_speech_prob, avg_logprob):
 def clips_per_batch(cfg, budget=DEFAULT_MEMORY_BUDGET, beams=5):
     per = 4 * cfg["decoder_layers"] * 2 * cfg["d_model"] * (1500 + beams * cfg["max_target_positions"])
     return max(1, int(budget // per))
+
+
+def samples_16k(x, sr):
+    return x.size if sr == 16000 else (x.size + 1) // 2
+
+
+def long_pools(n16, n_mels, budget=DEFAULT_MEMORY_BUDGET):
+    """Consecutive groups of the long clips (16 kHz sample counts n16, in list order) whose whole-clip log-mel buffer
+    [clips, longest // 160, n_mels] fp32 fits LONG_POOL_SHARE of the budget; a clip too long for it alone is a pool of one.
+    -> list of lists of indices into n16."""
+    cap, pools = budget * LONG_POOL_SHARE, []
+    for i, n in enumerate(n16):
+        if pools:
+            p = pools[-1]
+            T = max(n, max(n16[j] for j in p)) // 160
+            if (len(p) + 1) * T * n_mels * 4 <= cap:
+                p.append(i)
+                continue
+        pools.append([i])
+    return pools
 
 
 class WhisperAsr:
@@ -113,7 +139,7 @@ class WhisperAsr:
         trace_data, clips = {}, []
         for f in file_list:                                  # validate every file first, in list order
             try:
-                clips.append(read_clip(f))
+                clips.append(read_clip(f, max_seconds=None))
             except Exception as e:   # noqa: BLE001
                 print(f"{f}: {e!r}")
                 trace_data[f] = ResponseStatus.FAILED
@@ -121,27 +147,54 @@ class WhisperAsr:
             trace_data[f] = ResponseStatus.SUCCESS
         dev = torch.device("cuda", torch.cuda.current_device())
         h = torch.from_numpy(resample_taps()[1]).to(dev)
-        nb, sp, output, info = clips_per_batch(model.cfg, self.memory_budget), model.sp, [], {}
-        for s in range(0, len(clips), nb):
-            part = clips[s:s + nb]
+        nb, sp, lines, info = clips_per_batch(model.cfg, self.memory_budget), model.sp, {}, {}
+
+        def wav_rows(idx):
             rows = []
-            for x, sr in part:
+            for i in idx:
+                x, sr = clips[i]
                 xd = torch.from_numpy(x).to(dev)[None]
                 if sr == 32000:
                     xd = ops.resample_poly(xd, h, 1, 2, 64, (x.size + 1) // 2)
                 rows.append(xd[0])
-            L = max(r.numel() for r in rows)
-            wav = torch.zeros(len(rows), L, device=dev)
+            wav = torch.zeros(len(rows), max(r.numel() for r in rows), device=dev)
             for i, r in enumerate(rows):
                 wav[i, :r.numel()] = r
-            feats = model.features(wav, [r.numel() for r in rows])
-            for f, o in zip(file_list[s:s + nb], model.transcribe_features(feats, language=self.language)):
+            return wav, [r.numel() for r in rows]
+
+        n16 = [samples_16k(x, sr) for x, sr in clips]
+        short = [i for i, n in enumerate(n16) if n <= 30 * 16000]
+        long = [i for i, n in enumerate(n16) if n > 30 * 16000]
+        for s in range(0, len(short), nb):                  # clips of at most 30 s: whole, in batches of nb
+            idx = short[s:s + nb]
+            feats = model.features(*wav_rows(idx))
+            for i, o in zip(idx, model.transcribe_features(feats, language=self.language)):
+                f = file_list[i]
                 text = decode_text(tokenizer, o["tokens"], sp["eot"])
                 if is_no_speech(o["no_speech_prob"], o["score"]):
                     text = ""
-                output.append(f"{f}|{o['language'].lower()}|{text}")
+                lines[i] = f"{f}|{o['language'].lower()}|{text}"
                 info[f] = dict(status=ResponseStatus.SUCCESS, avg_logprob=o["score"], compression_ratio=compression_ratio(text),
                                no_speech_prob=o["no_speech_prob"])
+        nb_long = clips_per_batch(model.cfg, self.memory_budget * (1 - LONG_POOL_SHARE))
+        for pool in long_pools([n16[i] for i in long], model.cfg["num_mel_bins"], self.memory_budget):
+            idx = [long[j] for j in pool]                    # longer clips: 30 s windows, pool by pool
+            wav, lens = wav_rows(idx)
+            lm = model.features_long(wav, lens)
+            del wav
+            res = model.transcribe_long(lm, [n // 160 for n in lens], language=self.language, clips_per_batch=nb_long)
+            del lm
+            for i, o in zip(idx, res):
+                f, ws = file_list[i], o["windows"]
+                text = decode_text(tokenizer, o["tokens"], sp["eot"])
+                lines[i] = f"{f}|{o['language'].lower()}|{text}"
+                spoken = [w["avg_logprob"] for w in ws if not w["skipped"]] or [ws[0]["avg_logprob"]]
+                info[f] = dict(status=ResponseStatus.SUCCESS, avg_logprob=sum(spoken) / len(spoken),
+                               compression_ratio=compression_ratio(text), no_speech_prob=ws[0]["no_speech_prob"],
+                               windows=[dict(start_s=w["seek"] / 100, end_s=(w["seek"] + w["n_frames"]) / 100,
+                                             avg_logprob=w["avg_logprob"], no_speech_prob=w["no_speech_prob"],
+                                             skipped=w["skipped"]) for w in ws])
+        output, info = [lines[i] for i in range(len(file_list))], {f: info[f] for f in file_list}
         with open(output_file, "w", encoding="utf-8") as fo:
             fo.write("\n".join(output))
         with open(dump_file, "w", encoding="utf-8") as fo:

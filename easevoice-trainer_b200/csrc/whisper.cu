@@ -10,7 +10,13 @@
 //   row_layernorm_kernel                LayerNorm of any width, one row per block (large-v3 has 1280 channels)
 //   first_pass_kernel                   no-speech probability and the language argmax at <|startoftranscript|>
 //   cand_kernel / merge_kernel          the beam step: transformers' logits processors on the log-softmax, per-row top
-//                                       candidates, then the per-clip merge of GenerationMixin._beam_search
+//                                       candidates, then the per-clip merge of GenerationMixin._beam_search; optionally the
+//                                       log-sum-exp of each processed row summed along every hypothesis (long-form
+//                                       avg_logprob)
+//   logmel_long_kernel / logmel_max_kernel / logmel_norm_long_kernel
+//                                       the same log-mel over whole clips of any length: partial maxima per 256 frames,
+//                                       combined in a fixed order per clip, then the clamp and scale
+//   window_kernel                       30 s windows [seek, seek + n) of whole-clip log-mels, zero after n
 #include <math.h>
 
 #include "evk_common.cuh"
@@ -22,21 +28,47 @@ constexpr int kNfft = 400, kHop = 160, kBins = 201, kFrames = 3000;
 constexpr int kFpb = 16;                       // frames per logmel block
 constexpr int kMaxBeam = 8, kMaxLd = 448, kMaxK = 16;
 
-// One block per (16 frames, clip).  Thread k < 201 owns DFT bin k for all 16 frames; the basis is [400][201] (cos | sin,
-// window folded in), so a warp reads consecutive bins.  Frames past the clip's num_frames are not written.
-__global__ void __launch_bounds__(256) logmel_kernel(const float* __restrict__ wav, long long ldw, const int* __restrict__ lens,
-                                                     const float* __restrict__ cosb, const float* __restrict__ sinb,
-                                                     const float* __restrict__ fb, int M, float* __restrict__ out) {
+__device__ __forceinline__ float block_max(float v, float* red) {
+  v = warp_max(v);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : -INFINITY;
+    t = warp_max(t);
+    if (threadIdx.x == 0) red[32] = t;
+  }
+  __syncthreads();
+  return red[32];
+}
+
+__device__ __forceinline__ float block_add(float v, float* red) {
+  v = warp_sum(v);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
+    t = warp_sum(t);
+    if (threadIdx.x == 0) red[32] = t;
+  }
+  __syncthreads();
+  return red[32];
+}
+
+// Frames t0 .. t0 + 15 of one clip (n samples at x, nf frames): thread k < 201 owns DFT bin k for all 16 frames; the basis
+// is [400][201] (cos | sin, window folded in), so a warp reads consecutive bins.  Frame t goes to out + t * M; frames past
+// nf are not written.  Shared by the 30 s front end and the whole-clip one, so both compute the same bits per frame.
+__device__ __forceinline__ void logmel_block(const float* __restrict__ x, int n, int nf, int t0, const float* __restrict__ cosb,
+                                             const float* __restrict__ sinb, const float* __restrict__ fb, int M,
+                                             float* __restrict__ out) {
   __shared__ float fr[kFpb][kNfft];
   __shared__ float pw[kFpb][kBins + 1];
-  const int b = blockIdx.y, t0 = blockIdx.x * kFpb, n = lens[b], nf = n / kHop;
-  if (t0 >= nf) return;
-  const float* x = wav + (long long)b * ldw;
   for (int e = threadIdx.x; e < kFpb * kNfft; e += blockDim.x) {
     const int f = e / kNfft, i = e - f * kNfft;
-    int s = (t0 + f) * kHop + i - kNfft / 2;                 // reflect about the first and last sample
+    long long s = (long long)(t0 + f) * kHop + i - kNfft / 2;   // reflect about the first and last sample
     if (s < 0) s = -s;
-    if (s >= n) s = 2 * (n - 1) - s;
+    if (s >= n) s = 2 * (long long)(n - 1) - s;
     s = s < 0 ? 0 : (s >= n ? n - 1 : s);                   // clips shorter than 201 samples are rejected by the caller
     fr[f][i] = (t0 + f < nf) ? x[s] : 0.f;
   }
@@ -63,8 +95,17 @@ __global__ void __launch_bounds__(256) logmel_kernel(const float* __restrict__ w
     if (t0 + f >= nf) continue;
     float acc = 0.f;
     for (int q = 0; q < kBins; ++q) acc = fmaf(pw[f][q], fb[q * M + m], acc);
-    out[((long long)b * kFrames + t0 + f) * M + m] = log10f(fmaxf(acc, 1e-10f));
+    out[(long long)(t0 + f) * M + m] = log10f(fmaxf(acc, 1e-10f));
   }
+}
+
+// One block per (16 frames, clip) of a [B][3000][M] buffer.
+__global__ void __launch_bounds__(256) logmel_kernel(const float* __restrict__ wav, long long ldw, const int* __restrict__ lens,
+                                                     const float* __restrict__ cosb, const float* __restrict__ sinb,
+                                                     const float* __restrict__ fb, int M, float* __restrict__ out) {
+  const int b = blockIdx.y, t0 = blockIdx.x * kFpb, n = lens[b], nf = n / kHop;
+  if (t0 >= nf) return;
+  logmel_block(wav + (long long)b * ldw, n, nf, t0, cosb, sinb, fb, M, out + (long long)b * kFrames * M);
 }
 
 // One block per clip: the max over its frames, then the clamp and scale in place; frames from num_frames on are zeroed.
@@ -86,6 +127,57 @@ __global__ void __launch_bounds__(1024) logmel_norm_kernel(const int* __restrict
   __syncthreads();
   const float lo = red[32] - 8.f;
   for (long long e = threadIdx.x; e < nall; e += blockDim.x) o[e] = e < nv ? (fmaxf(o[e], lo) + 4.f) * 0.25f : 0.f;
+}
+
+constexpr int kMaxChunk = 256;                 // frames per partial maximum of the whole-clip front end
+
+// One block per (16 frames, clip) of a [B][T][M] buffer: the whole clip, any length.
+__global__ void __launch_bounds__(256) logmel_long_kernel(const float* __restrict__ wav, long long ldw, const int* __restrict__ lens,
+                                                          const float* __restrict__ cosb, const float* __restrict__ sinb,
+                                                          const float* __restrict__ fb, int M, int T, float* __restrict__ out) {
+  const int b = blockIdx.y, t0 = blockIdx.x * kFpb, n = lens[b], nf = n / kHop;
+  if (t0 >= nf) return;
+  logmel_block(wav + (long long)b * ldw, n, nf, t0, cosb, sinb, fb, M, out + (long long)b * T * M);
+}
+
+// One block per (256 frames, clip): part[b][c] = the max over the clip's frames [256 c, 256 c + 256) (-inf past its end).
+__global__ void __launch_bounds__(256) logmel_max_kernel(const int* __restrict__ lens, int M, int T, const float* __restrict__ lm,
+                                                         float* __restrict__ part) {
+  __shared__ float red[33];
+  const int b = blockIdx.y, c = blockIdx.x, nf = lens[b] / kHop;
+  const int f0 = c * kMaxChunk, f1 = min(nf, f0 + kMaxChunk);
+  const float* o = lm + (long long)b * T * M;
+  float mx = -INFINITY;
+  for (long long e = (long long)f0 * M + threadIdx.x; e < (long long)f1 * M; e += blockDim.x) mx = fmaxf(mx, o[e]);
+  mx = block_max(mx, red);
+  if (threadIdx.x == 0) part[(long long)b * gridDim.x + c] = mx;
+}
+
+// Blocks (slice, clip): every block folds its clip's partial maxima in chunk order, then clamps and scales its slice of
+// frames; frames from the clip's num_frames to T are zeroed.  The same formula as logmel_norm_kernel: a clip of at most
+// 3000 frames gets the bits of evk_whisper_logmel.
+__global__ void __launch_bounds__(256) logmel_norm_long_kernel(const int* __restrict__ lens, int M, int T, int n_part,
+                                                               const float* __restrict__ part, float* __restrict__ lm) {
+  const int b = blockIdx.y, nf = lens[b] / kHop;
+  float mx = -INFINITY;
+  for (int c = 0; c < n_part; ++c) mx = fmaxf(mx, part[(long long)b * n_part + c]);
+  const float lo = mx - 8.f;
+  float* o = lm + (long long)b * T * M;
+  const long long nv = (long long)nf * M, nall = (long long)T * M;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < nall; e += (long long)gridDim.x * blockDim.x)
+    o[e] = e < nv ? (fmaxf(o[e], lo) + 4.f) * 0.25f : 0.f;
+}
+
+// Blocks (frame group, output row): row r is frames [seek, seek + n) of clip row tab[r] = (clip, seek, n), zero after n
+// (and past the source's T frames).
+__global__ void __launch_bounds__(256) window_kernel(const float* __restrict__ lm, int T, int M, const int* __restrict__ tab,
+                                                     float* __restrict__ out) {
+  const int r = blockIdx.y, clip = tab[3 * r], seek = tab[3 * r + 1], n = tab[3 * r + 2];
+  const float* src = lm + ((long long)clip * T + seek) * M;
+  float* dst = out + (long long)r * kFrames * M;
+  const long long e1 = (long long)min(kFrames, (blockIdx.x + 1) * kFpb) * M;
+  const long long nv = (long long)min(n, T - seek) * M;
+  for (long long e = (long long)blockIdx.x * kFpb * M + threadIdx.x; e < e1; e += blockDim.x) dst[e] = e < nv ? src[e] : 0.f;
 }
 
 __global__ void embed_kernel(const int* __restrict__ tok, const float* __restrict__ emb, const float* __restrict__ pe,
@@ -178,34 +270,6 @@ __global__ void __launch_bounds__(128) attn_kernel(const float* __restrict__ q, 
     for (int a = 0; a < nq; ++a) o[(long long)(q0 + a) * ldo + h * 64 + c] = (red[0][a * 64 + c] + red[1][a * 64 + c]) / stat[a][0];
 }
 
-__device__ __forceinline__ float block_max(float v, float* red) {
-  v = warp_max(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : -INFINITY;
-    t = warp_max(t);
-    if (threadIdx.x == 0) red[32] = t;
-  }
-  __syncthreads();
-  return red[32];
-}
-
-__device__ __forceinline__ float block_add(float v, float* red) {
-  v = warp_sum(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
-    t = warp_sum(t);
-    if (threadIdx.x == 0) red[32] = t;
-  }
-  __syncthreads();
-  return red[32];
-}
-
 // LayerNorm of one row per block, any width (large-v3's 1280 channels exceed evk_layernorm_fwd's 1024): mean, then the
 // centred variance, each summed thread-strided and reduced in a fixed order, so a row's bits do not depend on the batch.
 __global__ void __launch_bounds__(256) row_layernorm_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ gamma,
@@ -278,7 +342,7 @@ __device__ __forceinline__ float masked_lp(float lp, int v, const RowRules& R, c
 __global__ void __launch_bounds__(512) cand_kernel(const float* __restrict__ lg, long long ld, StepCfg c,
                                                    const int* __restrict__ hist, int ld_hist, const int* __restrict__ gstep,
                                                    const float* __restrict__ run_score, int K, float* __restrict__ cv,
-                                                   int* __restrict__ ci) {
+                                                   int* __restrict__ ci, float* __restrict__ row_lse) {
   extern __shared__ unsigned bits[];             // [ceil(V / 32)]
   __shared__ float red[33];
   __shared__ RowRules R;
@@ -337,6 +401,18 @@ __global__ void __launch_bounds__(512) cand_kernel(const float* __restrict__ lg,
   st = block_add(st, red);
   const float ts_lse = mt == -INFINITY ? -INFINITY : mt + logf(st);
   Rl.force_ts = ts_lse > mx;
+  if (row_lse) {                                 // log-sum-exp of the processed row: its log_softmax is lp - this
+    float m3 = -INFINITY;
+    for (int v = tid; v < c.V; v += blockDim.x) m3 = fmaxf(m3, masked_lp((x[v] - m) - ls, v, Rl, c, bits));
+    m3 = block_max(m3, red);
+    float s3 = 0.f;
+    for (int v = tid; v < c.V; v += blockDim.x) {
+      const float a = masked_lp((x[v] - m) - ls, v, Rl, c, bits);
+      s3 += a == -INFINITY ? 0.f : expf(a - m3);
+    }
+    s3 = block_add(s3, red);
+    if (tid == 0) row_lse[r] = m3 + logf(s3);
+  }
   // candidates: per-thread sorted top K, then K rounds of a block argmax over the threads' heads
   const float base = run_score[r];
   Cand top[kMaxK];
@@ -366,13 +442,15 @@ __global__ void __launch_bounds__(512) cand_kernel(const float* __restrict__ lg,
 struct MergeBufs {
   float* run_score; int* hist; int ld_hist; int* tab; int ld_tab; int* tok; int* parent;
   float* fin_score; int* fin_seq; int* fin_len; int* fin_flag; int* unsat;
+  const float* row_lse; float* run_lse; float* fin_lse;      // null: no log-sum-exp tracking
 };
 
 // One block per clip.  Thread 0 runs the bookkeeping of _beam_search on the clip's beam * K candidates: the top 2 * beam by
 // accumulated log-prob, the running beams (hits pushed down by 1e9), the finished set (length-normalised, merged with the
 // earlier finished hypotheses, best beam kept) and the early-stop heuristic.  The block then gathers the new rows' token
 // histories and slot tables from their parents, and copies finished sequences.  A clip whose heuristic has stopped it is
-// left as it is: transformers keeps running its beams but can no longer change its finished set.
+// left as it is: transformers keeps running its beams but can no longer change its finished set.  With row_lse, run_lse /
+// fin_lse follow the hypotheses as their scores do: the sum over a hypothesis' steps of its processed rows' log-sum-exp.
 __global__ void __launch_bounds__(128) merge_kernel(const float* __restrict__ cv, const int* __restrict__ ci, int beam, int K,
                                                     int V, int eot, int plen, int max_length, const int* __restrict__ gstep,
                                                     float length_penalty, MergeBufs B) {
@@ -445,6 +523,14 @@ __global__ void __launch_bounds__(128) merge_kernel(const float* __restrict__ cv
       B.run_score[r0 + b] = nsc[b];
       B.tok[r0 + b] = sel_tok[b];
       B.parent[r0 + b] = r0 + sel_par[b];
+    }
+    if (B.row_lse) {
+      float nrl[kMaxBeam], nfl[kMaxBeam];
+      for (int b = 0; b < beam; ++b) nrl[b] = B.run_lse[r0 + sel_par[b]] + B.row_lse[r0 + sel_par[b]];
+      for (int j = 0; j < beam; ++j)
+        nfl[j] = fin_src[j] >= 0 ? B.fin_lse[(long long)clip * beam + fin_src[j]] : B.run_lse[-fin_src[j] - 1] + B.row_lse[-fin_src[j] - 1];
+      for (int b = 0; b < beam; ++b) B.run_lse[r0 + b] = nrl[b];
+      for (int j = 0; j < beam; ++j) B.fin_lse[(long long)clip * beam + j] = nfl[j];
     }
     B.unsat[clip] = any ? 1 : 0;
   }
@@ -550,12 +636,12 @@ extern "C" int evk_whisper_first_pass(const float* logits, int64_t ld, int32_t R
   return check_launch("whisper_first_pass");
 }
 
-extern "C" int evk_whisper_beam_step(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot,
-                                     int32_t nots, int32_t tsb, int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup, int32_t n_sup, const int32_t* bsup, int32_t n_bsup, const int32_t* gstep,
-                                     float length_penalty, float* cand_val, int32_t* cand_tok, float* run_score, int32_t* hist,
-                                     int32_t ld_hist, int32_t* tab, int32_t ld_tab, int32_t* tok, int32_t* parent,
-                                     float* fin_score, int32_t* fin_seq, int32_t* fin_len, int32_t* fin_flag, int32_t* unsat,
-                                     evk_stream_t stream) {
+static int beam_step(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot, int32_t nots, int32_t tsb,
+                     int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup, int32_t n_sup, const int32_t* bsup, int32_t n_bsup,
+                     const int32_t* gstep, float length_penalty, float* cand_val, int32_t* cand_tok, float* run_score, int32_t* hist,
+                     int32_t ld_hist, int32_t* tab, int32_t ld_tab, int32_t* tok, int32_t* parent, float* fin_score, int32_t* fin_seq,
+                     int32_t* fin_len, int32_t* fin_flag, int32_t* unsat, float* row_lse, float* run_lse, float* fin_lse,
+                     evk_stream_t stream) {
   EVK_REQUIRE(logits && gstep && cand_val && cand_tok && run_score && hist && tab && tok && parent && fin_score && fin_seq &&
               fin_len && fin_flag && unsat, EVK_ERR_ARG, "whisper_beam_step: null tensor");
   EVK_REQUIRE(clips > 0 && beam >= 1 && beam <= kMaxBeam && V > 0 && ld >= V && ld_hist <= kMaxLd && ld_tab <= kMaxLd &&
@@ -567,10 +653,60 @@ extern "C" int evk_whisper_beam_step(const float* logits, int64_t ld, int32_t cl
   cudaStream_t st = (cudaStream_t)stream;
   const size_t smem = (size_t)((V + 31) / 32) * sizeof(unsigned);
   EVK_REQUIRE(smem <= 32 * 1024, EVK_ERR_UNSUPPORTED, "whisper_beam_step: vocabulary of %d too large", V);
-  cand_kernel<<<clips * beam, 512, smem, st>>>(logits, ld, c, hist, ld_hist, gstep, run_score, K, cand_val, cand_tok);
+  cand_kernel<<<clips * beam, 512, smem, st>>>(logits, ld, c, hist, ld_hist, gstep, run_score, K, cand_val, cand_tok, row_lse);
   int rc = check_launch("whisper_beam_cand");
   if (rc) return rc;
-  MergeBufs B{run_score, hist, ld_hist, tab, ld_tab, tok, parent, fin_score, fin_seq, fin_len, fin_flag, unsat};
+  MergeBufs B{run_score, hist, ld_hist, tab, ld_tab, tok, parent, fin_score, fin_seq, fin_len, fin_flag, unsat, row_lse, run_lse, fin_lse};
   merge_kernel<<<clips, 128, 0, st>>>(cand_val, cand_tok, beam, K, V, eot, plen, maxlen, gstep, length_penalty, B);
   return check_launch("whisper_beam_merge");
+}
+
+extern "C" int evk_whisper_beam_step(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot,
+                                     int32_t nots, int32_t tsb, int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup, int32_t n_sup, const int32_t* bsup, int32_t n_bsup, const int32_t* gstep,
+                                     float length_penalty, float* cand_val, int32_t* cand_tok, float* run_score, int32_t* hist,
+                                     int32_t ld_hist, int32_t* tab, int32_t ld_tab, int32_t* tok, int32_t* parent,
+                                     float* fin_score, int32_t* fin_seq, int32_t* fin_len, int32_t* fin_flag, int32_t* unsat,
+                                     evk_stream_t stream) {
+  return beam_step(logits, ld, clips, beam, V, eot, nots, tsb, mit, plen, maxlen, sup, n_sup, bsup, n_bsup, gstep, length_penalty,
+                   cand_val, cand_tok, run_score, hist, ld_hist, tab, ld_tab, tok, parent, fin_score, fin_seq, fin_len, fin_flag, unsat,
+                   nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" int evk_whisper_beam_step_lse(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot,
+                                         int32_t nots, int32_t tsb, int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup,
+                                         int32_t n_sup, const int32_t* bsup, int32_t n_bsup, const int32_t* gstep, float length_penalty,
+                                         float* cand_val, int32_t* cand_tok, float* run_score, int32_t* hist, int32_t ld_hist,
+                                         int32_t* tab, int32_t ld_tab, int32_t* tok, int32_t* parent, float* fin_score,
+                                         int32_t* fin_seq, int32_t* fin_len, int32_t* fin_flag, int32_t* unsat, float* row_lse,
+                                         float* run_lse, float* fin_lse, evk_stream_t stream) {
+  EVK_REQUIRE(row_lse && run_lse && fin_lse, EVK_ERR_ARG, "whisper_beam_step_lse: null log-sum-exp buffer");
+  return beam_step(logits, ld, clips, beam, V, eot, nots, tsb, mit, plen, maxlen, sup, n_sup, bsup, n_bsup, gstep, length_penalty,
+                   cand_val, cand_tok, run_score, hist, ld_hist, tab, ld_tab, tok, parent, fin_score, fin_seq, fin_len, fin_flag, unsat,
+                   row_lse, run_lse, fin_lse, stream);
+}
+
+extern "C" int evk_whisper_logmel_long(const float* wav, int64_t ld_wav, const int32_t* lens, int32_t B, int32_t T,
+                                       const float* basis, const float* fb, int32_t n_mels, float* part, float* out,
+                                       evk_stream_t stream) {
+  EVK_REQUIRE(wav && lens && basis && fb && part && out, EVK_ERR_ARG, "whisper_logmel_long: null tensor");
+  EVK_REQUIRE(B > 0 && B <= 65535 && T > 0 && n_mels > 0 && n_mels <= 256 && ld_wav >= kNfft / 2 + 1, EVK_ERR_ARG,
+              "whisper_logmel_long: bad sizes B=%d T=%d n_mels=%d ld_wav=%lld", B, T, n_mels, (long long)ld_wav);
+  cudaStream_t st = (cudaStream_t)stream;
+  logmel_long_kernel<<<dim3((T + kFpb - 1) / kFpb, B), 256, 0, st>>>(wav, ld_wav, lens, basis, basis + kNfft * kBins, fb, n_mels, T, out);
+  int rc = check_launch("whisper_logmel_long");
+  if (rc) return rc;
+  const int n_part = (T + kMaxChunk - 1) / kMaxChunk;
+  logmel_max_kernel<<<dim3(n_part, B), 256, 0, st>>>(lens, n_mels, T, out, part);
+  rc = check_launch("whisper_logmel_max");
+  if (rc) return rc;
+  const long long blocks = ((long long)T * n_mels + 256 * 16 - 1) / (256 * 16);
+  logmel_norm_long_kernel<<<dim3((unsigned)blocks, B), 256, 0, st>>>(lens, n_mels, T, n_part, part, out);
+  return check_launch("whisper_logmel_norm_long");
+}
+
+extern "C" int evk_whisper_window(const float* lm, int32_t B, int32_t T, int32_t n_mels, const int32_t* tab, int32_t R, float* out,
+                                  evk_stream_t stream) {
+  EVK_REQUIRE(lm && tab && out && B > 0 && T > 0 && n_mels > 0 && R > 0 && R <= 65535, EVK_ERR_ARG, "whisper_window: bad arguments");
+  window_kernel<<<dim3((kFrames + kFpb - 1) / kFpb, R), 256, 0, (cudaStream_t)stream>>>(lm, T, n_mels, tab, out);
+  return check_launch("whisper_window");
 }

@@ -2500,3 +2500,38 @@ def whisper_beam_step(logits, st, beam, lay, length_penalty=1.0):
           _p(st["cv"]), _p(st["ci"]), _p(st["score"]), _p(st["hist"]), st["hist"].stride(0), _p(st["tab"]), st["tab"].stride(0),
           _p(st["tok"]), _p(st["parent"]), _p(st["fin_score"]), _p(st["fin_seq"]), _p(st["fin_len"]),
           _p(st["fin_flag"]), _p(st["unsat"]))
+
+
+def whisper_beam_step_lse(logits, st, beam, lay, length_penalty=1.0):
+    """evk_whisper_beam_step_lse: whisper_beam_step that also carries st["run_lse"] / st["fin_lse"], each hypothesis' sum of
+    its processed rows' log-sum-exp (st["row_lse"] is scratch)."""
+    clips = logits.shape[0] // beam
+    assert st["fin_seq"].stride(1) == st["hist"].stride(0) and st["tab"].stride(0) <= 448
+    _call("evk_whisper_beam_step_lse", _p(logits), logits.stride(0), clips, beam, logits.shape[1], *[int(v) for v in lay],
+          _p(st["sup"]), st["sup"].numel(), _p(st["bsup"]), st["bsup"].numel(), _p(st["g"]), ctypes.c_float(length_penalty),
+          _p(st["cv"]), _p(st["ci"]), _p(st["score"]), _p(st["hist"]), st["hist"].stride(0), _p(st["tab"]), st["tab"].stride(0),
+          _p(st["tok"]), _p(st["parent"]), _p(st["fin_score"]), _p(st["fin_seq"]), _p(st["fin_len"]),
+          _p(st["fin_flag"]), _p(st["unsat"]), _p(st["row_lse"]), _p(st["run_lse"]), _p(st["fin_lse"]))
+
+
+def whisper_logmel_long(wav, lens, T, basis, fb):
+    """evk_whisper_logmel_long: wav [B, L] fp32 (row b holds lens[b] 16 kHz samples; lens int32 device [B]) -> [B, T, n_mels]
+    normalised log-mel of each whole clip (max over all its frames), zero after its lens[b] // 160 frames."""
+    assert wav.dim() == 2 and wav.stride(1) == 1 and lens.dtype == torch.int32 and basis.is_contiguous() and fb.is_contiguous()
+    B, M = wav.shape[0], fb.shape[1]
+    out = torch.empty((B, T, M), device=wav.device, dtype=torch.float32)
+    part = torch.empty((B, (T + 255) // 256), device=wav.device, dtype=torch.float32)
+    _call("evk_whisper_logmel_long", _p(wav), wav.stride(0), _p(lens), B, T, _p(basis), _p(fb), M, _p(part), _p(out))
+    return out
+
+
+def whisper_window(lm, tab, out=None):
+    """evk_whisper_window: lm [B, T, n_mels], tab int32 device [R, 3] of (clip, seek, n) -> [R, 3000, n_mels], row r the frames
+    [seek, seek + n) of clip, zero after n."""
+    assert lm.is_contiguous() and tab.dtype == torch.int32 and tab.is_contiguous() and tab.shape[1] == 3
+    B, T, M = lm.shape
+    R = tab.shape[0]
+    out = torch.empty((R, 3000, M), device=lm.device, dtype=torch.float32) if out is None else out
+    assert out.is_contiguous() and out.shape == (R, 3000, M)
+    _call("evk_whisper_window", _p(lm), B, T, M, _p(tab), R, _p(out))
+    return out

@@ -1,5 +1,6 @@
 """Whisper transcription on the library's kernels: transformers' `WhisperForConditionalGeneration` (inference only) and the beam
-search of its `generate(num_beams=5, return_timestamps=True, task="transcribe", max_new_tokens=224)` for clips of at most 30 s.
+search of its `generate(num_beams=5, return_timestamps=True, task="transcribe", max_new_tokens=224)`: short-form for clips of
+at most 30 s, long-form (`transcribe_long`: 30 s windows moved by the predicted timestamps) for longer ones.
 
   front end   evk_whisper_logmel: 400-point periodic-Hann STFT (hop 160, centre reflect padding) as a direct DFT, |X|^2, the
               Slaney mel bank (fmax 8 kHz), log10, max(x, clip max - 8), (x + 4) / 4 over the clip's own frames; the
@@ -10,6 +11,10 @@ search of its `generate(num_beams=5, return_timestamps=True, task="transcribe", 
   decoder     one step of all rows: token + learned position, per layer causal self-attention on slot tables
               (evk_whisper_self_kv / evk_whisper_attn), cross-attention, MLP; final LayerNorm; logits from the tied token
               embedding; evk_whisper_beam_step.  The step is captured as a CUDA graph per batch shape and replayed.
+  long-form   evk_whisper_logmel_long: the same log-mel over the whole clip, clamped at the whole clip's max - 8;
+              evk_whisper_window cuts the 3000-frame window at each clip's seek; the windows of several clips are encoded and
+              decoded together as above (evk_whisper_beam_step_lse, which also yields transformers' avg_logprob), and each
+              clip's seek moves on the host by transformers' _retrieve_segment rules.
 
 Compute is fp32 storage with TF32 tensor-core products in the Linears and the encoder's attention (3xTF32 under
 `evk_set_precise(1)`); the decode attention and the beam step are exact fp32.  Special-token ids come from the generation
@@ -27,6 +32,9 @@ from .models import ParamTree
 N_FFT, HOP, N_FRAMES, N_CTX = 400, 160, 3000, 1500
 MAX_SAMPLES = 30 * 16000
 NUM_BEAMS, MAX_NEW_TOKENS = 5, 224
+# transformers' long-form skip rule (generate(no_speech_threshold=0.6, logprob_threshold=-1.0)): a window whose first pass
+# puts more than 0.6 on <|nospeech|> and whose best hypothesis averages below -1.0 log-prob per token adds no text
+NO_SPEECH_THRESHOLD, LOGPROB_THRESHOLD = 0.6, -1.0
 CONFIG_KEYS = ("num_mel_bins", "d_model", "encoder_layers", "decoder_layers", "encoder_attention_heads",
                "decoder_attention_heads", "encoder_ffn_dim", "decoder_ffn_dim", "vocab_size", "max_source_positions",
                "max_target_positions")
@@ -69,6 +77,20 @@ def special_tokens(gen):
                 suppress=[int(t) for t in gen.get("suppress_tokens") or []],
                 begin_suppress=[int(t) for t in gen.get("begin_suppress_tokens") or []],
                 max_initial_ts=gen.get("max_initial_timestamp_index"))
+
+
+def retrieve_segment(seq, ts_begin, n_frames):
+    """transformers' WhisperGenerationMixin._retrieve_segment for one window's best hypothesis seq (generated ids without the
+    eot it ended on) -> (the tokens kept: those of its segments, how many frames seek moves).  A hypothesis with a pair of
+    consecutive timestamps that does not end in a single timestamp keeps the tokens up to its last pair and moves seek to the
+    pair's first timestamp (2 frames per 20 ms step); otherwise it keeps every token and seek moves by the whole window."""
+    ts = [t >= ts_begin for t in seq]
+    single_ending = ts[-2:] == [False, True]
+    pairs = [i + 1 for i in range(len(seq) - 1) if ts[i] and ts[i + 1]]
+    if not pairs or single_ending:
+        return list(seq), n_frames
+    last = pairs[-1] + 1
+    return list(seq[:last]), (seq[last - 2] - ts_begin) * 2
 
 
 class WhisperModel(ParamTree):
@@ -220,6 +242,18 @@ class WhisperModel(ParamTree):
         return ops.whisper_logmel(wav.float().contiguous(), ln, pk["basis"], pk["fb"])
 
     @torch.no_grad()
+    def features_long(self, wav, lens):
+        """wav [B, L] fp32 device 16 kHz (row b holds lens[b] >= 201 samples, any length) -> [B, max lens // 160, n_mels]: the
+        log-mel of each whole clip normalised with its own max over all its frames, zero after its lens[b] // 160 frames."""
+        lens = [int(n) for n in lens]
+        for b, n in enumerate(lens):
+            if not (N_FFT // 2 + 1 <= n <= wav.shape[1]):
+                raise ValueError(f"row {b}: {n} samples (a clip takes at least 201 samples of 16 kHz audio)")
+        pk = self._packed()
+        ln = torch.tensor(lens, dtype=torch.int32).to(wav.device)
+        return ops.whisper_logmel_long(wav.float().contiguous(), ln, max(lens) // HOP, pk["basis"], pk["fb"])
+
+    @torch.no_grad()
     def encode(self, feats):
         """feats [B, 3000, n_mels] -> encoder last_hidden_state [B, 1500, d_model]."""
         c, pk = self.cfg, self._packed()
@@ -261,7 +295,8 @@ class WhisperModel(ParamTree):
                     ckv=torch.zeros(clips * N_CTX, Ld * 2 * d, device=dev), score=torch.zeros(R, device=dev),
                     cv=torch.zeros(R, 2 * beam, device=dev), ci=it(R, 2 * beam), fin_score=torch.zeros(clips, beam, device=dev),
                     fin_seq=it(clips, beam, S), fin_len=it(clips, beam), fin_flag=it(clips, beam), unsat=it(clips),
-                    nsp=torch.zeros(R, device=dev), lang_tok=it(R),
+                    nsp=torch.zeros(R, device=dev), lang_tok=it(R), row_lse=torch.zeros(R, device=dev),
+                    run_lse=torch.zeros(R, device=dev), fin_lse=torch.zeros(clips, beam, device=dev),
                     sup=torch.tensor(sp["suppress"], dtype=torch.int32, device=dev),
                     bsup=torch.tensor(sp["begin_suppress"], dtype=torch.int32, device=dev),
                     lang_ids=torch.tensor(sorted(sp["langs"].values()), dtype=torch.int32, device=dev))
@@ -297,24 +332,27 @@ class WhisperModel(ParamTree):
         mit = sp["max_initial_ts"]
         return (sp["eot"], sp["notimestamps"], sp["ts_begin"], -1 if mit is None else int(mit), plen, plen + max_new_tokens)
 
-    def _graph(self, clips, beam, dev, max_new_tokens):
-        """The decode step (forward of every row, beam step, position + 1) captured once per (clips, beam, max_new_tokens).
-        Graphs of one (clips, beam) share one decode state; a batch of another shape replaces that state and its graphs
-        rather than adding to the device memory a batch is sized for (cross K/V and slots for every clip)."""
+    def _graph(self, clips, beam, dev, max_new_tokens, track_lse=False):
+        """The decode step (forward of every row, beam step, position + 1) captured once per (clips, beam, max_new_tokens,
+        track_lse).  Graphs of one (clips, beam) share one decode state; a batch of another shape replaces that state and its
+        graphs rather than adding to the device memory a batch is sized for (cross K/V and slots for every clip).  track_lse:
+        the step is evk_whisper_beam_step_lse, which also carries what transformers' long-form avg_logprob needs."""
         skey = (clips, beam, str(dev))
         if self.__dict__.get("_gstate") is None or self._gstate[0] != skey:
             self._graphs.clear()
             self._gstate = None
             torch.cuda.empty_cache()
             self._gstate = (skey, self._state(clips, beam, dev))
-        if max_new_tokens in self._graphs:
-            return self._graphs[max_new_tokens]
+        gkey = (max_new_tokens, track_lse)
+        if gkey in self._graphs:
+            return self._graphs[gkey]
         st = self._gstate[1]
         lay = self._layout(3, max_new_tokens)
+        beam_step = ops.whisper_beam_step_lse if track_lse else ops.whisper_beam_step
 
         def step():
             lg = self._forward_rows(st)
-            ops.whisper_beam_step(lg, st, beam, lay)
+            beam_step(lg, st, beam, lay)
             st["pos"].add_(1)
             st["g"].add_(1)
             return lg
@@ -327,8 +365,8 @@ class WhisperModel(ParamTree):
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             step()
-        self._graphs[max_new_tokens] = (g, st)
-        return self._graphs[max_new_tokens]
+        self._graphs[gkey] = (g, st)
+        return self._graphs[gkey]
 
     @torch.no_grad()
     def transcribe_features(self, feats, language=None, num_beams=NUM_BEAMS, max_new_tokens=MAX_NEW_TOKENS, check_every=8,
@@ -346,12 +384,25 @@ class WhisperModel(ParamTree):
             if lg is not None and lg not in sp["langs"]:
                 raise ValueError(f"language {lg!r} is not in the generation config")
         enc = self.encode(feats) if enc is None else enc
-        g, st = self._graph(B, num_beams, dev, max_new_tokens)
-        R = st["R"]
+        return self._decode(enc, langs, num_beams, max_new_tokens, check_every)[0]
+
+    def _decode(self, enc, langs, num_beams, max_new_tokens, check_every, active=None, track_lse=False):
+        """Beam search of the clips of enc [B, 1500, d] (langs: a code or None per clip).  active: 0 / 1 per clip; a clip with
+        0 is finished before the first step, so it adds no steps and its result is empty.  track_lse: each result also has
+        avg_logprob, transformers' long-form mean of log_softmax(processed row)[token] over the hypothesis' tokens.
+        -> (results, number of decode steps)."""
+        sp = self.sp
+        B, dev = enc.shape[0], enc.device
+        g, st = self._graph(B, num_beams, dev, max_new_tokens, track_lse)
         self.cross_kv(enc, st["ckv"])
         for k in ("hist", "tab", "fin_seq", "fin_len", "fin_flag", "pos", "g"):
             st[k].zero_()
         st["unsat"].fill_(1)
+        if active is not None:
+            st["unsat"].copy_(torch.tensor(active, dtype=torch.int32))
+        if track_lse:
+            st["run_lse"].zero_()
+            st["fin_lse"].zero_()
         st["fin_score"].fill_(-1.0e9)
         st["score"].fill_(-1.0e9)
         st["score"].view(B, num_beams)[:, 0] = 0.0
@@ -366,15 +417,69 @@ class WhisperModel(ParamTree):
         self._forward_rows(st)
         st["pos"].fill_(2)
         st["tok"].fill_(sp["transcribe"])
+        steps = 0
         for n in range(max_new_tokens):
             g.replay()
+            steps += 1
             if (n + 1) % check_every == 0 and not bool(st["unsat"].any()):
                 break
         inv = {v: k for k, v in sp["langs"].items()}
         fin_len, fin_seq = st["fin_len"][:, 0].tolist(), st["fin_seq"][:, 0].tolist()
         sc, nsp = st["fin_score"][:, 0].tolist(), st["nsp"].view(B, num_beams)[:, 0].tolist()
-        return [dict(language=inv[lang_rows[b]], tokens=fin_seq[b][:fin_len[b]], score=sc[b], no_speech_prob=nsp[b])
-                for b in range(B)]
+        out = [dict(language=inv[lang_rows[b]], tokens=fin_seq[b][:fin_len[b]], score=sc[b], no_speech_prob=nsp[b])
+               for b in range(B)]
+        if track_lse:
+            for o, lse in zip(out, st["fin_lse"][:, 0].tolist()):
+                o["avg_logprob"] = o["score"] - lse / max(1, len(o["tokens"]))
+        return out, steps
+
+    @torch.no_grad()
+    def transcribe_long(self, lm, frames, language=None, clips_per_batch=8, num_beams=NUM_BEAMS, max_new_tokens=MAX_NEW_TOKENS,
+                        check_every=8):
+        """Long-form transcription of a pool of clips: transformers' long-form `generate` (temperature 0 only, no conditioning
+        on the previous window, no_speech_threshold 0.6, logprob_threshold -1.0) for each clip on its own.
+
+        lm [P, T, n_mels]: features_long of the pool; frames[i]: clip i's frame count.  language: a code, a list of them or
+        None (detected per clip on its first window, then forced on its later windows).  Each round takes the next window of
+        up to clips_per_batch unfinished clips, round-robin over the pool, and decodes them as one batch of
+        min(clips_per_batch, P) rows (one captured graph per pool); rows without a window are finished before the first step.
+        -> per clip dict(language, tokens: the kept tokens of its windows in order, windows: per window dict(seek, n_frames,
+        tokens (the best hypothesis), kept, score, avg_logprob, no_speech_prob, skipped, steps (decode steps of its round)))."""
+        sp = self.sp
+        P = len(frames)
+        langs = [language] * P if language is None or isinstance(language, str) else list(language)
+        for lg in langs:
+            if lg is not None and lg not in sp["langs"]:
+                raise ValueError(f"language {lg!r} is not in the generation config")
+        if max_new_tokens + 3 > self.cfg["max_target_positions"]:
+            raise ValueError(f"max_new_tokens {max_new_tokens} + 3 prompt tokens exceed {self.cfg['max_target_positions']} positions")
+        frames = [int(f) for f in frames]
+        nb, dev = max(1, min(int(clips_per_batch), P)), lm.device
+        seek, windows, cursor = [0] * P, [[] for _ in range(P)], 0
+        while True:
+            pick = [i for i in ((cursor + k) % P for k in range(P)) if seek[i] < frames[i]][:nb]
+            if not pick:
+                break
+            cursor = (pick[-1] + 1) % P
+            n = [min(N_FRAMES, frames[i] - seek[i]) for i in pick]
+            idle = nb - len(pick)
+            tab = torch.tensor([[i, seek[i], k] for i, k in zip(pick, n)] + [[0, 0, 0]] * idle, dtype=torch.int32).to(dev)
+            enc = self.encode(ops.whisper_window(lm, tab)[:len(pick)])
+            if idle:
+                enc = torch.cat([enc, enc.new_zeros((idle,) + tuple(enc.shape[1:]))])
+            res, steps = self._decode(enc, [langs[i] for i in pick] + [None] * idle, num_beams, max_new_tokens, check_every,
+                                      active=[1] * len(pick) + [0] * idle, track_lse=True)
+            for i, k, o in zip(pick, n, res):
+                if langs[i] is None:
+                    langs[i] = o["language"]
+                seq = o["tokens"][:-1] if o["tokens"] and o["tokens"][-1] == sp["eot"] else o["tokens"]
+                skipped = o["no_speech_prob"] > NO_SPEECH_THRESHOLD and o["avg_logprob"] < LOGPROB_THRESHOLD
+                kept, off = ([], k) if skipped else retrieve_segment(seq, sp["ts_begin"], k)
+                windows[i].append(dict(seek=seek[i], n_frames=k, tokens=o["tokens"], kept=kept, score=o["score"],
+                                       avg_logprob=o["avg_logprob"], no_speech_prob=o["no_speech_prob"], skipped=skipped,
+                                       steps=steps))
+                seek[i] += off
+        return [dict(language=langs[i], tokens=[t for w in windows[i] for t in w["kept"]], windows=windows[i]) for i in range(P)]
 
     @torch.no_grad()
     def teacher_forced_logits(self, enc, tokens):

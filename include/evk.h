@@ -816,6 +816,31 @@ int evk_whisper_beam_step(const float* logits, int64_t ld, int32_t clips, int32_
                           int32_t* cand_tok, float* run_score, int32_t* hist, int32_t ld_hist, int32_t* tab, int32_t ld_tab,
                           int32_t* tok, int32_t* parent, float* fin_score, int32_t* fin_seq, int32_t* fin_len, int32_t* fin_flag,
                           int32_t* unsat, evk_stream_t stream);
+/* evk_whisper_beam_step that also follows each hypothesis' log-sum-exp of its processed rows: row_lse [rows] (scratch) gets
+ * the log-sum-exp of each row's processed log-probs, run_lse [rows] of the new rows is their parent's run_lse + row_lse,
+ * and fin_lse [clips][beam] moves with the finished set as fin_score does.  For a finished hypothesis of L tokens,
+ * fin_score - fin_lse / L (length_penalty 1) is transformers' long-form avg_logprob: the mean of log_softmax(processed
+ * row)[token].  The caller zeroes run_lse and fin_lse before the first step.  Tokens and scores are those of
+ * evk_whisper_beam_step. */
+int evk_whisper_beam_step_lse(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot, int32_t nots,
+                              int32_t tsb, int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup, int32_t n_sup,
+                              const int32_t* bsup, int32_t n_bsup, const int32_t* gstep, float length_penalty, float* cand_val,
+                              int32_t* cand_tok, float* run_score, int32_t* hist, int32_t ld_hist, int32_t* tab, int32_t ld_tab,
+                              int32_t* tok, int32_t* parent, float* fin_score, int32_t* fin_seq, int32_t* fin_len,
+                              int32_t* fin_flag, int32_t* unsat, float* row_lse, float* run_lse, float* fin_lse,
+                              evk_stream_t stream);
+/* evk_whisper_logmel over whole clips of any length: out [B][T][n_mels], frame t < lens[b] / 160 of row b as
+ * evk_whisper_logmel computes it (the same code), clamped at the max over all of the clip's frames - 8 and scaled; frames
+ * from lens[b] / 160 to T are 0.  The max is taken per 256 frames into part [B][ceil(T / 256)] and folded in chunk order, so
+ * a clip's bits do not depend on the batch, and a clip of at most 3000 frames gets the bits of evk_whisper_logmel.
+ * lens[b] / 160 <= T, B <= 65535. */
+int evk_whisper_logmel_long(const float* wav, int64_t ld_wav, const int32_t* lens, int32_t B, int32_t T, const float* basis,
+                            const float* fb, int32_t n_mels, float* part, float* out, evk_stream_t stream);
+/* 30 s windows of whole-clip log-mels lm [B][T][n_mels]: output row r < R of out [R][3000][n_mels] is frames
+ * [seek, seek + n) of clip row `clip`, zero from n on, with (clip, seek, n) = tab[r][0..2] (int32 device, clip < B,
+ * 0 <= seek, n <= 3000).  Frames at or past T read as 0.  n = 0 gives a zero row. */
+int evk_whisper_window(const float* lm, int32_t B, int32_t T, int32_t n_mels, const int32_t* tab, int32_t R, float* out,
+                       evk_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,14 @@ device memory, the device-time split (front end, encoder, cross K/V, decode step
 profiled eager step), the encoder's TFLOP/s from shapes, and the comparator arms (fp32 with TF32 allowed and fp16, one clip per
 call and batched) on the first `--compare-clips` clips.  The card's name and power limit are read in the same run.
 
+--long: long-form transcription (`WhisperModel.transcribe_long`) of `--clips` (default 8) seeded 16 kHz clips of 40-300 s in
+one pool, every 30 s window decoding `--tokens-per-window` tokens (eot suppressed, as above); reports audio-seconds/s end
+to end, the device-time split (whole-clip front end, encoder, decode), peak memory and the comparator: transformers'
+long-form `generate` (attention_mask, temperature 0, logprob / no-speech thresholds) on the same features, fp32 with TF32 and
+fp16, batched.
+
 Usage:  python tools/bench_asr.py [--clips 256] [--compare-clips 16] [--no-compare]
+        python tools/bench_asr.py --long [--clips 8] [--tokens-per-window 120] [--no-compare]
 """
 import argparse
 import json
@@ -84,9 +91,13 @@ def main():
     ap.add_argument("--no-compare", action="store_true")
     ap.add_argument("--tokens-per-second", type=float, default=4.0)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--long", action="store_true")
+    ap.add_argument("--tokens-per-window", type=int, default=120)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_asr needs a GPU")
+    if a.long:
+        return main_long(a)
     from easevoice_trainer_b200 import asr, lib, normalize_ssl, ops, whisper
     lib.init().evk_set_precise(0)
     dev = torch.device("cuda", 0)
@@ -169,6 +180,108 @@ def main():
     if not a.no_compare:
         res["transformers"] = compare(net, cfg, gen, xs[:a.compare_clips], budget[:a.compare_clips], nb, feats_of, dev)
     print(json.dumps(res))
+
+
+def main_long(a):
+    from easevoice_trainer_b200 import asr, lib, whisper
+    lib.init().evk_set_precise(0)
+    dev = torch.device("cuda", 0)
+    cfg, gen = dict(whisper.LARGE_V3), generation_config()
+    with torch.device(dev):
+        net = whisper.WhisperModel(cfg, gen)
+    net = net.to(dev).eval()
+    seed_weights(net, a.seed)
+    n = a.clips if a.clips != 256 else 8
+    rng = np.random.default_rng(a.seed + 1)
+    xs = []
+    for _ in range(n):
+        t = np.arange(int(rng.uniform(40.0, 300.0) * 16000)) / 16000
+        xs.append((0.2 * np.sin(2 * np.pi * rng.uniform(100, 400) * t) + 0.05 * rng.standard_normal(t.size)).astype(np.float32))
+    lens = [x.size for x in xs]
+    frames = [m // 160 for m in lens]
+    nb = asr.clips_per_batch(cfg, asr.DEFAULT_MEMORY_BUDGET * (1 - asr.LONG_POOL_SHARE))
+    tpw = a.tokens_per_window
+    timing = dict(encoder=0.0, decode=0.0)
+    encode, decode = net.encode, net._decode
+
+    def timed(key, fn):
+        def run(*args, **kw):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            out = fn(*args, **kw)
+            e1.record()
+            torch.cuda.synchronize()
+            timing[key] += e0.elapsed_time(e1)
+            return out
+        return run
+
+    def wav():
+        w = torch.zeros(n, max(lens), device=dev)
+        for i, x in enumerate(xs):
+            w[i, :x.size] = torch.from_numpy(x).to(dev)
+        return w
+
+    with torch.no_grad():
+        w = wav()
+        lm = net.features_long(w[:2], lens[:2])                      # warm up: front end, encoder, the pool's graph
+        net._graph(min(nb, n), 5, dev, tpw, True)
+        net.encode(torch.zeros(1, 3000, cfg["num_mel_bins"], device=dev))
+        del lm
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        net.encode, net._decode = timed("encoder", encode), timed("decode", decode)
+        t0 = time.perf_counter()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        lm = net.features_long(wav(), lens)
+        e1.record()
+        res = net.transcribe_long(lm, frames, language="en", clips_per_batch=nb, max_new_tokens=tpw, check_every=1 << 30)
+        torch.cuda.synchronize()
+        wall = time.perf_counter() - t0
+        net.encode, net._decode = encode, decode
+        peak = torch.cuda.max_memory_allocated() / 2 ** 30
+    audio = sum(lens) / 16000
+    out = dict(metric="whisper large-v3-shaped long-form transcription audio-seconds/s", card=card(), clips=n, audio_s=audio,
+               clip_s=[round(m / 16000, 1) for m in lens], windows=sum(len(o["windows"]) for o in res), clips_per_batch=min(nb, n),
+               tokens_per_window=tpw, value=audio / wall, wall_s=wall, peak_mem_gib=peak,
+               device_ms=dict(front_end=e0.elapsed_time(e1), encoder=timing["encoder"], decode_incl_cross_kv=timing["decode"]))
+    if not a.no_compare:
+        out["transformers"] = compare_long(net, cfg, gen, lm, frames, audio, min(nb, n), tpw, dev)
+    print(json.dumps(out))
+
+
+def compare_long(net, cfg, gen, lm, frames, audio, nb, tpw, dev):
+    """transformers' long-form generate on the same whole-clip features, batches of nb clips with an attention_mask."""
+    from transformers import GenerationConfig, WhisperConfig, WhisperForConditionalGeneration
+    torch.backends.cuda.matmul.allow_tf32 = True
+    torch.backends.cudnn.allow_tf32 = True
+    hc = WhisperConfig(**cfg, decoder_start_token_id=50258, eos_token_id=50257, pad_token_id=50257, bos_token_id=50257,
+                       activation_function="gelu", scale_embedding=False, tie_word_embeddings=True)
+    with torch.device(dev):
+        ref = WhisperForConditionalGeneration(hc)
+    missing, unexpected = ref.load_state_dict({k: v.detach() for k, v in net.state_dict().items()}, strict=False)
+    assert not unexpected and set(missing) <= {"proj_out.weight"}, (missing, unexpected)
+    ref.tie_weights()
+    ref.eval().to(dev)
+    feats = lm.transpose(1, 2).contiguous()
+    mask = (torch.arange(feats.shape[2], device=dev)[None] < torch.tensor(frames, device=dev)[:, None]).long()
+    kw = dict(num_beams=5, return_timestamps=True, task="transcribe", language="en", temperature=0.0, logprob_threshold=-1.0,
+              no_speech_threshold=0.6, condition_on_prev_tokens=False)
+    out = {}
+    for dt in (torch.float32, torch.float16):
+        m = ref.to(dt)
+        m.generation_config = GenerationConfig(**gen)
+        with torch.no_grad():
+            m.generate(feats[:1, :, :3000].to(dt), num_beams=5, return_timestamps=True, task="transcribe", language="en",
+                       max_new_tokens=4)
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            for i in range(0, feats.shape[0], nb):
+                T = max(frames[i:i + nb])
+                m.generate(feats[i:i + nb, :, :T].to(dt), attention_mask=mask[i:i + nb, :T], max_new_tokens=tpw, **kw)
+            torch.cuda.synchronize()
+        out[f"{str(dt).split('.')[-1]}_batched"] = dict(audio_s_per_s=audio / (time.perf_counter() - t0), clips=feats.shape[0])
+    return out
 
 
 def compare(net, cfg, gen, xs, budget, nb, feats_of, dev):
