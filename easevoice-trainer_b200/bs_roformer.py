@@ -4,8 +4,8 @@
 Activations stay in one [B, T, bands, dim] layout, B*T*bands rows of `dim` floats.  The time transformer attends over the
 T rows of each (b, band) at a stride of `bands` rows, the frequency transformer over the `bands` consecutive rows of each
 (b, t); evk_rope_attn_fwd takes both as stride descriptions, so the reference's per-layer 'b t f d -> b f t d' permutes
-are never made.  Every RMSNorm is an L2 normalisation (evk_row_l2norm, evk_bs_band_input) whose gamma * sqrt(dim) is folded
-into the next Linear's weight columns at load; to_gates is appended to to_qkv as extra output rows.  Linears run on the
+are never made.  Every RMSNorm is an L2 normalisation (evk_row_norm without gamma, evk_band_input) whose gamma * sqrt(dim) is
+folded into the next Linear's weight columns at load; to_gates is appended to to_qkv as extra output rows.  Linears run on the
 TF32 tensor-core GEMM (3xTF32 under evk_set_precise(1)) with GELU, tanh and residual adds in its epilogue.  The complex mask
 multiply is fused into the inverse STFT.  Dropout is the identity.
 """
@@ -53,10 +53,14 @@ def check_sizes(dim, heads, depth, mask_estimator_depth):
 class AxialRoformer:
     """What BSRoformer and MelBandRoformer share: depth x (time, frequency) Transformers of rotary gated attention and GELU
     feed-forward layers over [B, T, bands, dim] activations, one Linear per band from the band-split operand, one MLP + GLU
-    per band to the complex masks, the weight folding and packing, and the input checks.  Subclasses define the bands."""
+    per band to the complex masks, the weight folding and packing, the input checks and the forward pass.  Subclasses
+    define the bands: band i holds the bins bins[band_off[i]:band_off[i+1]]; when bands overlap, bin f is held by the slots
+    cover[cover_off[f]:cover_off[f+1]] of `bins` and its mask is their average (cover and cover_off None: no overlap).
+    match_input_audio_length trims the output to the input's length instead of hop * (L // hop)."""
 
     def __init__(self, dim, depth, heads, stereo, time_transformer_depth, freq_transformer_depth, n_fft, hop,
-                 mask_estimator_depth, mask_linears):
+                 mask_estimator_depth, mask_linears, bins, band_off, cover=None, cover_off=None,
+                 match_input_audio_length=False):
         self.dim, self.depth, self.heads = int(dim), int(depth), int(heads)
         self.stereo, self.S = bool(stereo), 2 if stereo else 1
         self.t_depth, self.f_depth = int(time_transformer_depth), int(freq_transformer_depth)
@@ -64,10 +68,13 @@ class AxialRoformer:
         self.mask_depth = int(mask_estimator_depth)
         self.mask_linears = int(mask_linears)           # Linears per mask MLP (tanh between them)
         self.chunk_size = CHUNK                         # demix_track's chunk length
+        self.bins, self.band_off, self.cover, self.cover_off = bins, band_off, cover, cover_off
+        self.match_input_audio_length = bool(match_input_audio_length)
         self.device = torch.device("cpu")
         self.host_w, self.bias = None, None
         self._packed = {}
         self._rope = {}
+        self._tab = None
 
     # ---- weights -------------------------------------------------------------------------------------------------------
     def _layer_shapes(self, p, n):
@@ -169,7 +176,7 @@ class AxialRoformer:
         self.device = torch.device(device)
         if self.bias is not None:
             self.bias = {k: v.to(self.device) for k, v in self.bias.items()}
-        self._packed, self._rope = {}, {}
+        self._packed, self._rope, self._tab = {}, {}, None
         return self
 
     def eval(self):
@@ -190,6 +197,13 @@ class AxialRoformer:
             ang = torch.arange(L, dtype=torch.float32)[:, None] * inv[None, :]
             self._rope[L] = torch.stack([ang.cos(), ang.sin()], -1).contiguous().to(self.device)
         return self._rope[L]
+
+    def _tables(self):
+        """the band tables as device int32 tensors (bins, band_off, cover, cover_off), None where a table is None"""
+        if self._tab is None:
+            self._tab = [None if t is None else torch.from_numpy(t).to(self.device)
+                         for t in (self.bins, self.band_off, self.cover, self.cover_off)]
+        return self._tab
 
     # ---- forward -------------------------------------------------------------------------------------------------------
     def check_input(self, raw_audio):
@@ -215,14 +229,14 @@ class AxialRoformer:
         h = torch.empty_like(x)
         for j in range(depth):
             q = f"{p}.layers.{j}"
-            ops.row_l2norm(x, out=h)
+            ops.row_norm(x, out=h)
             wq = W[q + ".qkvg"]
             qkvg = ops.linear_into(h, wq, torch.empty((R, wq.D0), device=x.device), bias=sd[q + ".qkvg.b"])
             a = ops.rope_attn(qkvg, cs, torch.empty((R, D), device=x.device), self.heads, L, *geo)
             del qkvg
             x = ops.linear_into(a, W[q + ".out"], torch.empty_like(x), res=x)
             del a
-            ops.row_l2norm(x, out=h)
+            ops.row_norm(x, out=h)
             f = ops.linear_into(h, W[q + ".ff1"], torch.empty((R, 4 * self.dim), device=x.device), bias=sd[q + ".ff1.b"],
                                 act=ops.ACT_GELU)
             x = ops.linear_into(f, W[q + ".ff2"], torch.empty_like(x), bias=sd[q + ".ff2.b"], res=x)
@@ -251,6 +265,39 @@ class AxialRoformer:
             ops.glu_into(hc, out[:, 2 * S * off[i]:2 * S * off[i + 1]])
         return out
 
+    @torch.no_grad()
+    def forward(self, raw_audio):
+        """raw_audio CUDA [B, S, L] (or [B, L] when mono) -> [B, S, hop * (L // hop)], or [B, S, L] with
+        match_input_audio_length, as the reference's forward"""
+        x = self.check_input(raw_audio)
+        B, S, L = x.shape
+        dev, dim, nb, NB, n_slots = x.device, self.dim, len(self.band_off) - 1, self.n_fft // 2 + 1, len(self.bins)
+        bins, band_off, cover, cover_off = self._tables()
+        cplx = ops.stft(x.view(B * S, L), self.n_fft, self.hop)                     # [B*S, T, NB, 2]
+        T = cplx.shape[1]
+        feat = ops.band_input(cplx, B, S, band_off, bins, torch.empty((B * T, 2 * S * n_slots), device=dev))
+        x = self._band_split(feat, self.band_off, B * T)
+        del feat
+        cs_t, cs_f = self._rope_table(T), self._rope_table(nb)
+        for i in range(self.depth):
+            for a, n, cs, Lq, geo in ((0, self.t_depth, cs_t, T, (B, T * nb, nb, 1, nb)),
+                                      (1, self.f_depth, cs_f, nb, (B * T, nb, 1, 0, 1))):
+                p = f"layers.{i}.{a}"
+                x = self._transformer(x, p, n, cs, Lq, geo)
+                if p + ".norm.g" in self.bias:                               # a Transformer's own output RMSNorm
+                    ops.row_norm(x, self.bias[p + ".norm.g"], out=x)
+        xn = ops.row_norm(x).view(B * T, nb * dim)                   # the last norm; its gamma is folded into the mask MLPs
+        del x
+        # without overlapping bands the GLU writes straight into the mask layout the inverse STFT reads
+        mask = self._mask_estimator(xn, self.band_off, torch.empty((B * T, 2 * S * n_slots), device=dev))
+        del xn
+        if cover is not None:
+            mask = ops.melband_mask_avg(mask, S, cover_off, cover, torch.empty((B * T, 2 * S * NB), device=dev))
+        out = ops.istft(cplx, B, S, self.n_fft, self.hop, mask=mask, length=L if self.match_input_audio_length else None)
+        return out.view(B, S, -1)
+
+    __call__ = forward
+
 
 class BSRoformer(AxialRoformer):
     """BSRoformer(**config) for inference on CUDA.  Takes the reference's keyword arguments; the training-only ones
@@ -277,7 +324,8 @@ class BSRoformer(AxialRoformer):
             raise ValueError(f"freqs_per_bands must sum to n_fft // 2 + 1 = {n_fft // 2 + 1}, got {sum(bands)}")
         check_sizes(dim, heads, depth, mask_estimator_depth)
         super().__init__(dim, depth, heads, stereo, time_transformer_depth, freq_transformer_depth, n_fft, stft_hop_length,
-                         mask_estimator_depth, mask_estimator_depth)
+                         mask_estimator_depth, mask_estimator_depth, np.arange(n_fft // 2 + 1, dtype=np.int32),
+                         np.concatenate([[0], np.cumsum(bands)]).astype(np.int32))
         self.bands = bands
 
     # ---- weights -------------------------------------------------------------------------------------------------------
@@ -308,33 +356,6 @@ class BSRoformer(AxialRoformer):
         """The SeparateMDXC model (SHIPPED_CONFIG) with the weights of a reference checkpoint file, on `device`."""
         sd = torch.load(path, map_location="cpu", weights_only=True)
         return cls(**SHIPPED_CONFIG).to(device).load_state_dict(sd)
-
-    # ---- forward -------------------------------------------------------------------------------------------------------
-    @torch.no_grad()
-    def forward(self, raw_audio):
-        """raw_audio CUDA [B, S, L] (or [B, L] when mono) -> [B, S, hop * (L // hop)], as the reference's forward"""
-        x = self.check_input(raw_audio)
-        B, S, L = x.shape
-        dev, dim, nb, NB = x.device, self.dim, len(self.bands), self.n_fft // 2 + 1
-        cplx = ops.stft(x.view(B * S, L), self.n_fft, self.hop)                     # [B*S, T, NB, 2]
-        T = cplx.shape[1]
-        off = np.concatenate([[0], np.cumsum(self.bands)])
-        feat = ops.bs_band_input(cplx, B, S, torch.tensor(off, dtype=torch.int32).to(dev),
-                                 torch.empty((B * T, 2 * S * NB), device=dev))
-        x = self._band_split(feat, off, B * T)
-        del feat
-        cs_t, cs_f = self._rope_table(T), self._rope_table(nb)
-        for i in range(self.depth):
-            x = self._transformer(x, f"layers.{i}.0", self.t_depth, cs_t, T, (B, T * nb, nb, 1, nb))
-            x = self._transformer(x, f"layers.{i}.1", self.f_depth, cs_f, nb, (B * T, nb, 1, 0, 1))
-        xn = ops.row_l2norm(x).view(B * T, nb * dim)
-        del x
-        mask = self._mask_estimator(xn, off, torch.empty((B * T, 2 * S * NB), device=dev))
-        del xn
-        out = ops.istft(cplx, B, S, self.n_fft, self.hop, mask=mask)
-        return out.view(B, S, -1)
-
-    __call__ = forward
 
 
 def chunk_plan(n, c=CHUNK, batch=BATCH):

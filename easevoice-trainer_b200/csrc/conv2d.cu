@@ -5,8 +5,8 @@
 // layer can read or write a channel slice of a wider concat buffer (pointer advanced by the slice's channel offset).
 //
 //   conv2d_fwd   implicit GEMM: M = B*Ho*Wo output pixels, N = output channels, K = k*k*C (tap-major, channel-minor),
-//                CTA tile 128 rows x 32 K, fp32 accumulation.  Zero padding and dilation are per axis (conv2d_fwd_hw:
-//                the DeEcho net's ASPP dilates rows and columns differently; conv2d_fwd is the equal-axes call).
+//                CTA tile 128 rows x 32 K, fp32 accumulation.  Zero padding and dilation are per axis (the DeEcho
+//                net's ASPP dilates rows and columns differently).
 //                Two kernels, chosen from the operands:
 //                * wgmma (TF32): C, pitches and pointers allow 16-byte copies and 3xTF32 is off.  Two consumer
 //                  warpgroups of 64 rows x 32 / 64 / 128 columns (the smallest that covers N), a 4-stage cp.async
@@ -508,10 +508,10 @@ extern int g_precise;
 
 using namespace evk;
 
-extern "C" int evk_conv2d_fwd_hw(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale,
-                                 const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W,
-                                 int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h,
-                                 int32_t dil_w, int32_t act, cudaStream_t st) {
+extern "C" int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale,
+                              const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W,
+                              int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h,
+                              int32_t dil_w, int32_t act, cudaStream_t st) {
   EVK_REQUIRE(x && w && y, EVK_ERR_ARG, "conv2d: null tensor");
   EVK_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && N > 0, EVK_ERR_ARG, "conv2d: bad sizes B=%d H=%d W=%d C=%d N=%d", B, H, W,
               C, N);
@@ -537,14 +537,6 @@ extern "C" int evk_conv2d_fwd_hw(const float* x, int32_t x_pitch, int64_t x_bs, 
   if (N <= 32) return launch_conv_wgmma<32>(a, st);
   if (N <= 64) return launch_conv_wgmma<64>(a, st);
   return launch_conv_wgmma<128>(a, st);
-}
-
-extern "C" int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale,
-                              const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W,
-                              int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad, int32_t dil, int32_t act,
-                              cudaStream_t st) {
-  return evk_conv2d_fwd_hw(x, x_pitch, x_bs, w, scale, bias, y, y_pitch, y_bs, B, H, W, C, N, k, stride, pad, pad, dil, dil,
-                           act, st);
 }
 
 extern "C" int evk_dwconv3x3_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, float* y, int32_t y_pitch,

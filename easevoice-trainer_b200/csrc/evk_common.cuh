@@ -147,6 +147,23 @@ __device__ __forceinline__ float block_sum(float v, float* red /* >= 33 floats *
   return red[32];
 }
 
+// block-wide max in the order of block_sum (result valid in all threads)
+__device__ __forceinline__ float block_max(float v, float* red /* >= 33 floats */) {
+  int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  v = warp_max(v);
+  __syncthreads();
+  if (lane == 0) red[w] = v;
+  __syncthreads();
+  int nw = (blockDim.x + 31) >> 5;
+  float t = (threadIdx.x < nw) ? red[threadIdx.x] : -INFINITY;
+  if (w == 0) {
+    t = warp_max(t);
+    if (lane == 0) red[32] = t;
+  }
+  __syncthreads();
+  return red[32];
+}
+
 // Philox-4x32-10 counter RNG (graph-safe: state = (seed, offset) read from device memory)
 struct Philox {
   uint32_t k0, k1;

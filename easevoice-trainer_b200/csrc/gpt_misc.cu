@@ -42,7 +42,7 @@ __global__ void sinepos_bwd_kernel(const float* __restrict__ dy, int ldy, long l
 }
 
 // ------------------------------------------------------------------------------------------------
-// position r % T of row r counts unless count is given and r % T >= *count (see evk_ce_fwd_ex)
+// position r % T of row r counts unless count is given and r % T >= *count (see evk_ce_fwd)
 __device__ __forceinline__ bool counted(int row, const int* count, int T) { return count == nullptr || row % T < *count; }
 
 // one warp per row: lse, nll, top-k hit (count of logits strictly above the target logit < k), valid = target != ignore
@@ -496,8 +496,8 @@ extern "C" int evk_sinepos_bwd(const float* dy, int ldy, int64_t dy_sb, const fl
   return ordered_sum(part, blocks, 1, 1, 1, dalpha, 0, 0, st);
 }
 
-extern "C" int evk_ce_fwd_ex(const float* logits, int ld, const int64_t* targets, int rows, int V, int topk, int64_t ignore_index,
-                             const int32_t* count, int T, float* lse, float* nll, uint8_t* flags, float* out2, cudaStream_t st) {
+extern "C" int evk_ce_fwd(const float* logits, int ld, const int64_t* targets, int rows, int V, int topk, int64_t ignore_index,
+                          const int32_t* count, int T, float* lse, float* nll, uint8_t* flags, float* out2, cudaStream_t st) {
   EVK_REQUIRE(rows > 0 && V > 0, EVK_ERR_ARG, "ce_fwd: empty");
   EVK_REQUIRE(!count || (T > 0 && rows % T == 0), EVK_ERR_ARG, "ce_fwd: %d rows are not whole rows of T = %d positions", rows, T);
   ce_fwd_kernel<<<cdiv(rows, 8), 256, 0, st>>>(logits, ld, (const long long*)targets, rows, V, topk, ignore_index, count, T, lse,
@@ -507,36 +507,21 @@ extern "C" int evk_ce_fwd_ex(const float* logits, int ld, const int64_t* targets
   return check_launch("ce_finalize");
 }
 
-extern "C" int evk_ce_fwd(const float* logits, int ld, const int64_t* targets, int rows, int V, int topk, int64_t ignore_index,
-                          float* lse, float* nll, uint8_t* flags, float* out2, cudaStream_t st) {
-  return evk_ce_fwd_ex(logits, ld, targets, rows, V, topk, ignore_index, nullptr, 1, lse, nll, flags, out2, st);
-}
-
-extern "C" int evk_dpo_head_ex(const float* nll_c, int Yc, const int32_t* count_c, const float* nll_r, int Yr, const int32_t* count_r,
-                               int B, float beta, float* out3, float* coef_c, float* coef_r, cudaStream_t st) {
+extern "C" int evk_dpo_head(const float* nll_c, int Yc, const int32_t* count_c, const float* nll_r, int Yr, const int32_t* count_r,
+                            int B, float beta, float* out3, float* coef_c, float* coef_r, cudaStream_t st) {
   EVK_REQUIRE(B > 0 && Yc > 0 && Yr > 0, EVK_ERR_ARG, "dpo_head: empty");
   dpo_head_kernel<<<1, 256, 0, st>>>(nll_c, Yc, count_c, nll_r, Yr, count_r, B, beta, out3, coef_c, coef_r);
   return check_launch("dpo_head");
 }
 
-extern "C" int evk_dpo_head(const float* nll_c, int Yc, const float* nll_r, int Yr, int B, float beta, float* out3, float* coef_c,
-                            float* coef_r, cudaStream_t st) {
-  return evk_dpo_head_ex(nll_c, Yc, nullptr, nll_r, Yr, nullptr, B, beta, out3, coef_c, coef_r, st);
-}
-
-extern "C" int evk_ce_bwd_ex(const float* logits, int ld, const int64_t* targets, const float* lse, const float* gscale,
-                             int rows_per_g, const int32_t* count, int T, float* dl, int lddl, int rows, int V, cudaStream_t st) {
+extern "C" int evk_ce_bwd(const float* logits, int ld, const int64_t* targets, const float* lse, const float* gscale,
+                          int rows_per_g, const int32_t* count, int T, float* dl, int lddl, int rows, int V, cudaStream_t st) {
   EVK_REQUIRE(rows_per_g > 0, EVK_ERR_ARG, "ce_bwd: rows_per_g");
   EVK_REQUIRE(!count || (T > 0 && rows % T == 0), EVK_ERR_ARG, "ce_bwd: %d rows are not whole rows of T = %d positions", rows, T);
   long long n = (long long)rows * V;
   ce_bwd_kernel<<<(int)min((long long)kNumSMs * 16, (n + 255) / 256), 256, 0, st>>>(logits, ld, (const long long*)targets, lse, gscale,
                                                                                     rows_per_g, count, T, dl, lddl, rows, V);
   return check_launch("ce_bwd");
-}
-
-extern "C" int evk_ce_bwd(const float* logits, int ld, const int64_t* targets, const float* lse, const float* gscale,
-                          int rows_per_g, float* dl, int lddl, int rows, int V, cudaStream_t st) {
-  return evk_ce_bwd_ex(logits, ld, targets, lse, gscale, rows_per_g, nullptr, 1, dl, lddl, rows, V, st);
 }
 
 extern "C" int evk_dpo_reject_rows(const int64_t* y, int ldy, int B, const int32_t* spans, const int32_t* yc, int64_t* out, int Yr,

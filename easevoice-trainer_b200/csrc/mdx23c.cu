@@ -226,11 +226,6 @@ inline unsigned grid_of(long long total) {
 
 using namespace evk;
 
-extern "C" int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale,
-                              const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W,
-                              int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad, int32_t dil, int32_t act,
-                              cudaStream_t st);
-
 extern "C" int evk_mdx_tdf(const float* a, const float* x, int32_t ldx, int64_t x_zs, const float* r, int32_t ldr, int64_t r_zs,
                            float* y, int32_t ldy, int64_t y_zs, int32_t Z, int32_t M, int32_t N, int32_t K, evk_stream_t stream) {
   EVK_REQUIRE(a && x && y, EVK_ERR_ARG, "mdx_tdf: null tensor");
@@ -252,7 +247,7 @@ extern "C" int evk_convt2x2_fwd(const float* x, int32_t x_pitch, int64_t x_bs, c
     for (int dx = 0; dx < 2; ++dx)
       if (int rc = evk_conv2d_fwd(x, x_pitch, (int64_t)W * x_pitch, w + (long long)(dy * 2 + dx) * N * C, nullptr, nullptr,
                                   y + ((long long)dy * 2 * W + dx) * y_pitch, 2 * y_pitch, 4ll * W * y_pitch, B * H, 1, W, C, N, 1,
-                                  1, 0, 1, EVK_C2_NONE, (cudaStream_t)stream))
+                                  1, 0, 0, 1, 1, EVK_C2_NONE, stream))
         return rc;
   return EVK_OK;
 }

@@ -153,10 +153,10 @@ __global__ void __launch_bounds__(kSampThreads) sample_tokens_kernel(
 
 using namespace evk;
 
-extern "C" int evk_sample_tokens_ex(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, int32_t eos_steps,
-                                    const int64_t* icfg, const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq,
-                                    int64_t* hist, int32_t ldh, uint32_t* seen, int32_t* fin, const float* emb, const float* pe,
-                                    const float* alpha, float* x_next, int32_t D, cudaStream_t st) {
+extern "C" int evk_sample_tokens(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, int32_t eos_steps,
+                                 const int64_t* icfg, const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq,
+                                 int64_t* hist, int32_t ldh, uint32_t* seen, int32_t* fin, const float* emb, const float* pe,
+                                 const float* alpha, float* x_next, int32_t D, cudaStream_t st) {
   EVK_REQUIRE(logits && icfg && fcfg && n_dev && hist && seen && fin && emb && pe && alpha && x_next, EVK_ERR_ARG,
               "sample_tokens: null argument");
   EVK_REQUIRE(B >= 1 && V >= 2 && V <= kSampMaxV && eos >= 0 && eos < V && ldl >= V && D >= 1 && (!q || ldq >= V), EVK_ERR_ARG,
@@ -165,12 +165,4 @@ extern "C" int evk_sample_tokens_ex(const float* logits, int32_t ldl, int32_t B,
   sample_tokens_kernel<<<B, kSampThreads, 0, st>>>(logits, ldl, V, eos, eos_steps, (const long long*)icfg, fcfg, n_dev, q, ldq,
                                                    (long long*)hist, ldh, seen, fin, emb, pe, alpha, x_next, D);
   return check_launch("sample_tokens");
-}
-
-extern "C" int evk_sample_tokens(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, const int64_t* icfg,
-                                 const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist, int32_t ldh,
-                                 uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha, float* x_next,
-                                 int32_t D, cudaStream_t st) {
-  return evk_sample_tokens_ex(logits, ldl, B, V, eos, 1, icfg, fcfg, n_dev, q, ldq, hist, ldh, seen, fin, emb, pe, alpha, x_next,
-                              D, st);
 }

@@ -381,11 +381,12 @@ extern "C" int evk_stft_bwd(const float* gcplx, const float* dmel, int32_t ld_dm
   return check_launch("stft_ola_kernel");
 }
 
-namespace {
-// Lout < 0: hop * (T - 1) samples per row (torch.istft's length=None); else Lout samples (length=Lout)
-int istft_run(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft, int32_t hop,
-              float* work, float* out, int32_t ld_out, long long Lout, cudaStream_t st) {
+// length 0: hop * (T - 1) samples per row (torch.istft's length=None); else length samples (length=length)
+extern "C" int evk_istft(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft,
+                         int32_t hop, int32_t length, float* work, float* out, int32_t ld_out, evk_stream_t stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
   EVK_REQUIRE(cplx && work && out, EVK_ERR_ARG, "istft: null tensor");
+  EVK_REQUIRE(length >= 0, EVK_ERR_ARG, "istft: length %d must not be negative", length);
   const bool pow2 = n_fft >= 256 && n_fft <= STFT_TAB && (n_fft & (n_fft - 1)) == 0;
   EVK_REQUIRE(pow2 || stft_mr_size_ok(n_fft), EVK_ERR_UNSUPPORTED,
               "istft: n_fft=%d must be a power of two in [256, 8192] or an even divisor of %d in [16, 7680]", n_fft, STFT_TAB_MR);
@@ -393,7 +394,7 @@ int istft_run(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, 
               "istft: bad sizes B=%d S=%d T=%d hop=%d", B, S, T, hop);
   EVK_REQUIRE(!mask || (ld_mask >= 2 * S * (n_fft / 2 + 1) && (uintptr_t)mask % 8 == 0 && ld_mask % 2 == 0), EVK_ERR_ARG,
               "istft: mask rows must hold 2 * S * (n_fft / 2 + 1) floats, 8-byte aligned");
-  if (Lout < 0) Lout = (long long)hop * (T - 1);
+  const long long Lout = length ? length : (long long)hop * (T - 1);
   EVK_REQUIRE(Lout > 0 && Lout < (long long)hop * (T - 1) + n_fft / 2, EVK_ERR_ARG,
               "istft: %lld output samples; the frames cover fewer than %lld", Lout, (long long)hop * (T - 1) + n_fft / 2);
   const long long frames = (long long)B * S * T;
@@ -421,19 +422,6 @@ int istft_run(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, 
   const long long bx = (Lout + 255) / 256;
   istft_ola_kernel<<<dim3((unsigned)(bx < 1024 ? bx : 1024), (unsigned)(B * S)), 256, 0, st>>>(p);
   return check_launch("istft_ola_kernel");
-}
-}  // namespace
-
-extern "C" int evk_istft(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft,
-                         int32_t hop, float* work, float* out, int32_t ld_out, evk_stream_t stream) {
-  return istft_run(cplx, mask, ld_mask, B, S, T, n_fft, hop, work, out, ld_out, -1, (cudaStream_t)stream);
-}
-
-extern "C" int evk_istft_length(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T,
-                                int32_t n_fft, int32_t hop, int32_t length, float* work, float* out, int32_t ld_out,
-                                evk_stream_t stream) {
-  EVK_REQUIRE(length > 0, EVK_ERR_ARG, "istft_length: length %d must be positive", length);
-  return istft_run(cplx, mask, ld_mask, B, S, T, n_fft, hop, work, out, ld_out, length, (cudaStream_t)stream);
 }
 
 // loss[0] += scale * sum |a - b| over n complex elements; grad (nullable) = scale * (a - b) / |a - b|

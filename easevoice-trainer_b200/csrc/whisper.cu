@@ -1,8 +1,11 @@
 // Whisper transcription (whisper.py, asr.py), inference only.  The encoder and the decoder's Linears, LayerNorms and the
 // encoder's attention run on the library's existing kernels; this file holds what they lack:
-//   logmel_kernel / logmel_norm_kernel  the 400-point periodic-Hann STFT (hop 160, centre reflect padding) as a direct DFT
-//                                       against a precomputed basis, |X|^2, the Slaney mel bank, log10(max(., 1e-10)); then
-//                                       max(x, clip max - 8), (x + 4) / 4 over each clip's own frames, zero after them
+//   logmel_kernel / logmel_max_kernel / logmel_norm_kernel
+//                                       the 400-point periodic-Hann STFT (hop 160, centre reflect padding) as a direct DFT
+//                                       against a precomputed basis, |X|^2, the Slaney mel bank, log10(max(., 1e-10)) over
+//                                       whole clips of any length; partial maxima per 256 frames, combined in a fixed order
+//                                       per clip; then max(x, clip max - 8), (x + 4) / 4 over each clip's own frames, zero
+//                                       after them
 //   embed_kernel / add_pos_kernel       token + learned position rows; the encoder's sinusoidal positions
 //   self_kv_kernel                      a row's new self-attention K / V written once into its slot, listed in its slot table
 //   attn_kernel                         head-dim-64 decode attention in exact fp32: one query row against its slot table, or
@@ -13,9 +16,6 @@
 //                                       candidates, then the per-clip merge of GenerationMixin._beam_search; optionally the
 //                                       log-sum-exp of each processed row summed along every hypothesis (long-form
 //                                       avg_logprob)
-//   logmel_long_kernel / logmel_max_kernel / logmel_norm_long_kernel
-//                                       the same log-mel over whole clips of any length: partial maxima per 256 frames,
-//                                       combined in a fixed order per clip, then the clamp and scale
 //   window_kernel                       30 s windows [seek, seek + n) of whole-clip log-mels, zero after n
 #include <math.h>
 
@@ -28,40 +28,16 @@ constexpr int kNfft = 400, kHop = 160, kBins = 201, kFrames = 3000;
 constexpr int kFpb = 16;                       // frames per logmel block
 constexpr int kMaxBeam = 8, kMaxLd = 448, kMaxK = 16;
 
-__device__ __forceinline__ float block_max(float v, float* red) {
-  v = warp_max(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : -INFINITY;
-    t = warp_max(t);
-    if (threadIdx.x == 0) red[32] = t;
-  }
-  __syncthreads();
-  return red[32];
-}
-
-__device__ __forceinline__ float block_add(float v, float* red) {
-  v = warp_sum(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
-    t = warp_sum(t);
-    if (threadIdx.x == 0) red[32] = t;
-  }
-  __syncthreads();
-  return red[32];
-}
-
-// Frames t0 .. t0 + 15 of one clip (n samples at x, nf frames): thread k < 201 owns DFT bin k for all 16 frames; the basis
-// is [400][201] (cos | sin, window folded in), so a warp reads consecutive bins.  Frame t goes to out + t * M; frames past
-// nf are not written.  Shared by the 30 s front end and the whole-clip one, so both compute the same bits per frame.
-__device__ __forceinline__ void logmel_block(const float* __restrict__ x, int n, int nf, int t0, const float* __restrict__ cosb,
-                                             const float* __restrict__ sinb, const float* __restrict__ fb, int M,
-                                             float* __restrict__ out) {
+// One block per (16 frames t0 .. t0 + 15, clip) of a [B][T][M] buffer, the whole clip, any length: thread k < 201 owns DFT bin
+// k for all 16 frames; the basis is [400][201] (cos | sin, window folded in), so a warp reads consecutive bins.  Frame t of
+// clip b (n samples, nf frames) goes to out + (b T + t) M; frames past nf are not written.
+__global__ void __launch_bounds__(256) logmel_kernel(const float* __restrict__ wav, long long ldw, const int* __restrict__ lens,
+                                                     const float* __restrict__ cosb, const float* __restrict__ sinb,
+                                                     const float* __restrict__ fb, int M, int T, float* __restrict__ out) {
+  const int b = blockIdx.y, t0 = blockIdx.x * kFpb, n = lens[b], nf = n / kHop;
+  if (t0 >= nf) return;
+  const float* x = wav + (long long)b * ldw;
+  out += (long long)b * T * M;
   __shared__ float fr[kFpb][kNfft];
   __shared__ float pw[kFpb][kBins + 1];
   for (int e = threadIdx.x; e < kFpb * kNfft; e += blockDim.x) {
@@ -99,46 +75,7 @@ __device__ __forceinline__ void logmel_block(const float* __restrict__ x, int n,
   }
 }
 
-// One block per (16 frames, clip) of a [B][3000][M] buffer.
-__global__ void __launch_bounds__(256) logmel_kernel(const float* __restrict__ wav, long long ldw, const int* __restrict__ lens,
-                                                     const float* __restrict__ cosb, const float* __restrict__ sinb,
-                                                     const float* __restrict__ fb, int M, float* __restrict__ out) {
-  const int b = blockIdx.y, t0 = blockIdx.x * kFpb, n = lens[b], nf = n / kHop;
-  if (t0 >= nf) return;
-  logmel_block(wav + (long long)b * ldw, n, nf, t0, cosb, sinb, fb, M, out + (long long)b * kFrames * M);
-}
-
-// One block per clip: the max over its frames, then the clamp and scale in place; frames from num_frames on are zeroed.
-__global__ void __launch_bounds__(1024) logmel_norm_kernel(const int* __restrict__ lens, int M, float* __restrict__ out) {
-  __shared__ float red[33];
-  const int b = blockIdx.x, nf = lens[b] / kHop;
-  float* o = out + (long long)b * kFrames * M;
-  const long long nv = (long long)nf * M, nall = (long long)kFrames * M;
-  float mx = -INFINITY;
-  for (long long e = threadIdx.x; e < nv; e += blockDim.x) mx = fmaxf(mx, o[e]);
-  mx = warp_max(mx);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : -INFINITY;
-    v = warp_max(v);
-    if (threadIdx.x == 0) red[32] = v;
-  }
-  __syncthreads();
-  const float lo = red[32] - 8.f;
-  for (long long e = threadIdx.x; e < nall; e += blockDim.x) o[e] = e < nv ? (fmaxf(o[e], lo) + 4.f) * 0.25f : 0.f;
-}
-
-constexpr int kMaxChunk = 256;                 // frames per partial maximum of the whole-clip front end
-
-// One block per (16 frames, clip) of a [B][T][M] buffer: the whole clip, any length.
-__global__ void __launch_bounds__(256) logmel_long_kernel(const float* __restrict__ wav, long long ldw, const int* __restrict__ lens,
-                                                          const float* __restrict__ cosb, const float* __restrict__ sinb,
-                                                          const float* __restrict__ fb, int M, int T, float* __restrict__ out) {
-  const int b = blockIdx.y, t0 = blockIdx.x * kFpb, n = lens[b], nf = n / kHop;
-  if (t0 >= nf) return;
-  logmel_block(wav + (long long)b * ldw, n, nf, t0, cosb, sinb, fb, M, out + (long long)b * T * M);
-}
+constexpr int kMaxChunk = 256;                 // frames per partial maximum
 
 // One block per (256 frames, clip): part[b][c] = the max over the clip's frames [256 c, 256 c + 256) (-inf past its end).
 __global__ void __launch_bounds__(256) logmel_max_kernel(const int* __restrict__ lens, int M, int T, const float* __restrict__ lm,
@@ -154,10 +91,9 @@ __global__ void __launch_bounds__(256) logmel_max_kernel(const int* __restrict__
 }
 
 // Blocks (slice, clip): every block folds its clip's partial maxima in chunk order, then clamps and scales its slice of
-// frames; frames from the clip's num_frames to T are zeroed.  The same formula as logmel_norm_kernel: a clip of at most
-// 3000 frames gets the bits of evk_whisper_logmel.
-__global__ void __launch_bounds__(256) logmel_norm_long_kernel(const int* __restrict__ lens, int M, int T, int n_part,
-                                                               const float* __restrict__ part, float* __restrict__ lm) {
+// frames; frames from the clip's num_frames to T are zeroed.
+__global__ void __launch_bounds__(256) logmel_norm_kernel(const int* __restrict__ lens, int M, int T, int n_part,
+                                                          const float* __restrict__ part, float* __restrict__ lm) {
   const int b = blockIdx.y, nf = lens[b] / kHop;
   float mx = -INFINITY;
   for (int c = 0; c < n_part; ++c) mx = fmaxf(mx, part[(long long)b * n_part + c]);
@@ -279,10 +215,10 @@ __global__ void __launch_bounds__(256) row_layernorm_kernel(const float* __restr
   const float* xr = x + (long long)blockIdx.x * ldx;
   float s = 0.f;
   for (int c = threadIdx.x; c < C; c += blockDim.x) s += xr[c];
-  const float mean = block_add(s, red) / (float)C;
+  const float mean = block_sum(s, red) / (float)C;
   float q = 0.f;
   for (int c = threadIdx.x; c < C; c += blockDim.x) { const float d = xr[c] - mean; q += d * d; }
-  const float rstd = rsqrtf(block_add(q, red) / (float)C + eps);
+  const float rstd = rsqrtf(block_sum(q, red) / (float)C + eps);
   float* yr = y + (long long)blockIdx.x * ldy;
   for (int c = threadIdx.x; c < C; c += blockDim.x) yr[c] = (xr[c] - mean) * rstd * gamma[c] + beta[c];
 }
@@ -298,7 +234,7 @@ __global__ void __launch_bounds__(512) first_pass_kernel(const float* __restrict
   m = block_max(m, red);
   float s = 0.f;
   for (int v = threadIdx.x; v < V; v += blockDim.x) s += expf(x[v] - m);
-  s = block_add(s, red);
+  s = block_sum(s, red);
   if (threadIdx.x == 0) {
     nsp[blockIdx.x] = expf(x[nospeech] - m) / s;
     int best = lang_ids[0];
@@ -373,7 +309,7 @@ __global__ void __launch_bounds__(512) cand_kernel(const float* __restrict__ lg,
   m = block_max(m, red);
   float s = 0.f;
   for (int v = tid; v < c.V; v += blockDim.x) s += expf(x[v] - m);
-  const float ls = logf(block_add(s, red));
+  const float ls = logf(block_sum(s, red));
   RowRules Rl = R;
   // the timestamp processor's own log_softmax of the masked scores, then logsumexp over timestamps vs the best text token
   float m2 = -INFINITY;
@@ -384,7 +320,7 @@ __global__ void __launch_bounds__(512) cand_kernel(const float* __restrict__ lg,
     const float a = masked_lp((x[v] - m) - ls, v, Rl, c, bits);
     s2 += a == -INFINITY ? 0.f : expf(a - m2);
   }
-  const float ls2 = logf(block_add(s2, red));
+  const float ls2 = logf(block_sum(s2, red));
   float mt = -INFINITY, mx = -INFINITY;
   for (int v = tid; v < c.V; v += blockDim.x) {
     const float l2 = (masked_lp((x[v] - m) - ls, v, Rl, c, bits) - m2) - ls2;
@@ -398,7 +334,7 @@ __global__ void __launch_bounds__(512) cand_kernel(const float* __restrict__ lg,
       const float l2 = (masked_lp((x[v] - m) - ls, v, Rl, c, bits) - m2) - ls2;
       st += l2 == -INFINITY ? 0.f : expf(l2 - mt);
     }
-  st = block_add(st, red);
+  st = block_sum(st, red);
   const float ts_lse = mt == -INFINITY ? -INFINITY : mt + logf(st);
   Rl.force_ts = ts_lse > mx;
   if (row_lse) {                                 // log-sum-exp of the processed row: its log_softmax is lp - this
@@ -410,7 +346,7 @@ __global__ void __launch_bounds__(512) cand_kernel(const float* __restrict__ lg,
       const float a = masked_lp((x[v] - m) - ls, v, Rl, c, bits);
       s3 += a == -INFINITY ? 0.f : expf(a - m3);
     }
-    s3 = block_add(s3, red);
+    s3 = block_sum(s3, red);
     if (tid == 0) row_lse[r] = m3 + logf(s3);
   }
   // candidates: per-thread sorted top K, then K rounds of a block argmax over the threads' heads
@@ -563,19 +499,6 @@ __global__ void __launch_bounds__(128) merge_kernel(const float* __restrict__ cv
 
 using namespace evk;
 
-extern "C" int evk_whisper_logmel(const float* wav, int64_t ld_wav, const int32_t* lens, int32_t B, const float* basis,
-                                  const float* fb, int32_t n_mels, float* out, evk_stream_t stream) {
-  EVK_REQUIRE(wav && lens && basis && fb && out, EVK_ERR_ARG, "whisper_logmel: null tensor");
-  EVK_REQUIRE(B > 0 && B <= 65535 && n_mels > 0 && n_mels <= 256 && ld_wav >= kNfft / 2 + 1, EVK_ERR_ARG,
-              "whisper_logmel: bad sizes B=%d n_mels=%d ld_wav=%lld", B, n_mels, (long long)ld_wav);
-  cudaStream_t st = (cudaStream_t)stream;
-  logmel_kernel<<<dim3((kFrames + kFpb - 1) / kFpb, B), 256, 0, st>>>(wav, ld_wav, lens, basis, basis + kNfft * kBins, fb, n_mels, out);
-  int rc = check_launch("whisper_logmel");
-  if (rc) return rc;
-  logmel_norm_kernel<<<B, 1024, 0, st>>>(lens, n_mels, out);
-  return check_launch("whisper_logmel_norm");
-}
-
 extern "C" int evk_whisper_embed(const int32_t* tok, const float* emb, const float* pe, const int32_t* pos, int32_t R, int32_t d,
                                  float* x, evk_stream_t stream) {
   EVK_REQUIRE(tok && emb && pe && pos && x && R > 0 && d > 0, EVK_ERR_ARG, "whisper_embed: bad arguments");
@@ -636,14 +559,17 @@ extern "C" int evk_whisper_first_pass(const float* logits, int64_t ld, int32_t R
   return check_launch("whisper_first_pass");
 }
 
-static int beam_step(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot, int32_t nots, int32_t tsb,
-                     int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup, int32_t n_sup, const int32_t* bsup, int32_t n_bsup,
-                     const int32_t* gstep, float length_penalty, float* cand_val, int32_t* cand_tok, float* run_score, int32_t* hist,
-                     int32_t ld_hist, int32_t* tab, int32_t ld_tab, int32_t* tok, int32_t* parent, float* fin_score, int32_t* fin_seq,
-                     int32_t* fin_len, int32_t* fin_flag, int32_t* unsat, float* row_lse, float* run_lse, float* fin_lse,
-                     evk_stream_t stream) {
+extern "C" int evk_whisper_beam_step(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot,
+                                     int32_t nots, int32_t tsb, int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup,
+                                     int32_t n_sup, const int32_t* bsup, int32_t n_bsup, const int32_t* gstep, float length_penalty,
+                                     float* cand_val, int32_t* cand_tok, float* run_score, int32_t* hist, int32_t ld_hist,
+                                     int32_t* tab, int32_t ld_tab, int32_t* tok, int32_t* parent, float* fin_score,
+                                     int32_t* fin_seq, int32_t* fin_len, int32_t* fin_flag, int32_t* unsat, float* row_lse,
+                                     float* run_lse, float* fin_lse, evk_stream_t stream) {
   EVK_REQUIRE(logits && gstep && cand_val && cand_tok && run_score && hist && tab && tok && parent && fin_score && fin_seq &&
               fin_len && fin_flag && unsat, EVK_ERR_ARG, "whisper_beam_step: null tensor");
+  EVK_REQUIRE(!row_lse == !run_lse && !row_lse == !fin_lse, EVK_ERR_ARG,
+              "whisper_beam_step: row_lse, run_lse and fin_lse are all given or all null");
   EVK_REQUIRE(clips > 0 && beam >= 1 && beam <= kMaxBeam && V > 0 && ld >= V && ld_hist <= kMaxLd && ld_tab <= kMaxLd &&
               (n_sup == 0 || sup) && (n_bsup == 0 || bsup), EVK_ERR_ARG, "whisper_beam_step: bad sizes clips=%d beam=%d V=%d", clips, beam, V);
   EVK_REQUIRE(eot >= 0 && eot < V && tsb > eot && tsb <= V && plen >= 1 && maxlen > plen && maxlen - plen <= ld_hist &&
@@ -661,47 +587,23 @@ static int beam_step(const float* logits, int64_t ld, int32_t clips, int32_t bea
   return check_launch("whisper_beam_merge");
 }
 
-extern "C" int evk_whisper_beam_step(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot,
-                                     int32_t nots, int32_t tsb, int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup, int32_t n_sup, const int32_t* bsup, int32_t n_bsup, const int32_t* gstep,
-                                     float length_penalty, float* cand_val, int32_t* cand_tok, float* run_score, int32_t* hist,
-                                     int32_t ld_hist, int32_t* tab, int32_t ld_tab, int32_t* tok, int32_t* parent,
-                                     float* fin_score, int32_t* fin_seq, int32_t* fin_len, int32_t* fin_flag, int32_t* unsat,
-                                     evk_stream_t stream) {
-  return beam_step(logits, ld, clips, beam, V, eot, nots, tsb, mit, plen, maxlen, sup, n_sup, bsup, n_bsup, gstep, length_penalty,
-                   cand_val, cand_tok, run_score, hist, ld_hist, tab, ld_tab, tok, parent, fin_score, fin_seq, fin_len, fin_flag, unsat,
-                   nullptr, nullptr, nullptr, stream);
-}
-
-extern "C" int evk_whisper_beam_step_lse(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot,
-                                         int32_t nots, int32_t tsb, int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup,
-                                         int32_t n_sup, const int32_t* bsup, int32_t n_bsup, const int32_t* gstep, float length_penalty,
-                                         float* cand_val, int32_t* cand_tok, float* run_score, int32_t* hist, int32_t ld_hist,
-                                         int32_t* tab, int32_t ld_tab, int32_t* tok, int32_t* parent, float* fin_score,
-                                         int32_t* fin_seq, int32_t* fin_len, int32_t* fin_flag, int32_t* unsat, float* row_lse,
-                                         float* run_lse, float* fin_lse, evk_stream_t stream) {
-  EVK_REQUIRE(row_lse && run_lse && fin_lse, EVK_ERR_ARG, "whisper_beam_step_lse: null log-sum-exp buffer");
-  return beam_step(logits, ld, clips, beam, V, eot, nots, tsb, mit, plen, maxlen, sup, n_sup, bsup, n_bsup, gstep, length_penalty,
-                   cand_val, cand_tok, run_score, hist, ld_hist, tab, ld_tab, tok, parent, fin_score, fin_seq, fin_len, fin_flag, unsat,
-                   row_lse, run_lse, fin_lse, stream);
-}
-
-extern "C" int evk_whisper_logmel_long(const float* wav, int64_t ld_wav, const int32_t* lens, int32_t B, int32_t T,
-                                       const float* basis, const float* fb, int32_t n_mels, float* part, float* out,
-                                       evk_stream_t stream) {
-  EVK_REQUIRE(wav && lens && basis && fb && part && out, EVK_ERR_ARG, "whisper_logmel_long: null tensor");
+extern "C" int evk_whisper_logmel(const float* wav, int64_t ld_wav, const int32_t* lens, int32_t B, int32_t T,
+                                  const float* basis, const float* fb, int32_t n_mels, float* part, float* out,
+                                  evk_stream_t stream) {
+  EVK_REQUIRE(wav && lens && basis && fb && part && out, EVK_ERR_ARG, "whisper_logmel: null tensor");
   EVK_REQUIRE(B > 0 && B <= 65535 && T > 0 && n_mels > 0 && n_mels <= 256 && ld_wav >= kNfft / 2 + 1, EVK_ERR_ARG,
-              "whisper_logmel_long: bad sizes B=%d T=%d n_mels=%d ld_wav=%lld", B, T, n_mels, (long long)ld_wav);
+              "whisper_logmel: bad sizes B=%d T=%d n_mels=%d ld_wav=%lld", B, T, n_mels, (long long)ld_wav);
   cudaStream_t st = (cudaStream_t)stream;
-  logmel_long_kernel<<<dim3((T + kFpb - 1) / kFpb, B), 256, 0, st>>>(wav, ld_wav, lens, basis, basis + kNfft * kBins, fb, n_mels, T, out);
-  int rc = check_launch("whisper_logmel_long");
+  logmel_kernel<<<dim3((T + kFpb - 1) / kFpb, B), 256, 0, st>>>(wav, ld_wav, lens, basis, basis + kNfft * kBins, fb, n_mels, T, out);
+  int rc = check_launch("whisper_logmel");
   if (rc) return rc;
   const int n_part = (T + kMaxChunk - 1) / kMaxChunk;
   logmel_max_kernel<<<dim3(n_part, B), 256, 0, st>>>(lens, n_mels, T, out, part);
   rc = check_launch("whisper_logmel_max");
   if (rc) return rc;
   const long long blocks = ((long long)T * n_mels + 256 * 16 - 1) / (256 * 16);
-  logmel_norm_long_kernel<<<dim3((unsigned)blocks, B), 256, 0, st>>>(lens, n_mels, T, n_part, part, out);
-  return check_launch("whisper_logmel_norm_long");
+  logmel_norm_kernel<<<dim3((unsigned)blocks, B), 256, 0, st>>>(lens, n_mels, T, n_part, part, out);
+  return check_launch("whisper_logmel_norm");
 }
 
 extern "C" int evk_whisper_window(const float* lm, int32_t B, int32_t T, int32_t n_mels, const int32_t* tab, int32_t R, float* out,

@@ -5,11 +5,11 @@ It is the BS-Roformer (bs_roformer.AxialRoformer: the same rotary gated axial at
 Linears and folded weights) with three differences:
   * the bands are the non-zero bins of the rows of a Slaney mel filterbank (mel_processing.slaney_filterbank, the
     restatement of librosa.filters.mel, with its first and last weight forced to 1), so adjacent bands share bins.
-    evk_melband_input gathers each band's bins through a device bin table and L2-normalises its segment;
+    evk_band_input gathers each band's bins through a device bin table and L2-normalises its segment;
   * each band's mask covers its own bins.  evk_melband_mask_avg sums the bands covering a bin in ascending band order and
     divides by their count (the reference's scatter_add_ / num_bands_per_freq), into the mask layout the inverse STFT takes;
   * every Transformer ends in its own RMSNorm and there is no final norm.  Those norms sit on the residual stream between
-    transformers, so they run as evk_row_rmsnorm with their gamma, except the last, which feeds only the mask estimators and
+    transformers, so they run as evk_row_norm with their gamma, except the last, which feeds only the mask estimators and
     is folded into their first Linear like every other RMSNorm.
 """
 import re
@@ -17,7 +17,6 @@ import re
 import numpy as np
 import torch
 
-from . import ops
 from .bs_roformer import AxialRoformer, check_sizes, check_stft
 from .mel_processing import slaney_filterbank
 
@@ -73,16 +72,15 @@ class MelBandRoformer(AxialRoformer):
         n_fft = check_stft(stft_n_fft, stft_win_length, stft_hop_length, stft_normalized, stft_window_fn)
         if num_bands < 1:
             raise ValueError(f"num_bands must be >= 1, got {num_bands}")
-        self.bins, self.band_off, self.cover, self.cover_off = band_tables(sample_rate, n_fft, int(num_bands))
+        tables = band_tables(sample_rate, n_fft, int(num_bands))
         if mask_estimator_depth < 0:
             raise ValueError(f"mask_estimator_depth must be >= 0, got {mask_estimator_depth}")
         check_sizes(dim, heads, depth, mask_estimator_depth + 1)
         # the reference's MLP here has mask_estimator_depth hidden layers: one Linear more than BS-Roformer's
         super().__init__(dim, depth, heads, stereo, time_transformer_depth, freq_transformer_depth, n_fft, stft_hop_length,
-                         mask_estimator_depth, mask_estimator_depth + 1)
+                         mask_estimator_depth, mask_estimator_depth + 1, *tables,
+                         match_input_audio_length=match_input_audio_length)
         self.num_bands, self.sample_rate = int(num_bands), int(sample_rate)
-        self.match_input_audio_length = bool(match_input_audio_length)
-        self._tab = None
 
     # ---- weights -------------------------------------------------------------------------------------------------------
     def _dims_in(self):
@@ -113,17 +111,6 @@ class MelBandRoformer(AxialRoformer):
                     out[p + ".norm.g"] = sd[p + ".norm.gamma"].contiguous()
         self._fold_bands(sd, self.num_bands, sd[self._last_norm()], out)
         return out
-
-    def to(self, device):
-        super().to(device)
-        self._tab = None
-        return self
-
-    def _tables(self):
-        """the band tables as device int32 tensors (bins, band_off, cover, cover_off)"""
-        if self._tab is None:
-            self._tab = [torch.from_numpy(t).to(self.device) for t in (self.bins, self.band_off, self.cover, self.cover_off)]
-        return self._tab
 
     @classmethod
     def infer_config(cls, sd, **config):
@@ -190,37 +177,3 @@ class MelBandRoformer(AxialRoformer):
         to DEFAULT_CONFIG's (44.1 kHz, hop 441) and are the caller's to set, as is anything passed in `config`."""
         sd = torch.load(path, map_location="cpu", weights_only=True)
         return cls(**cls.infer_config(sd, **config)).to(device).load_state_dict(sd)
-
-    # ---- forward -------------------------------------------------------------------------------------------------------
-    @torch.no_grad()
-    def forward(self, raw_audio):
-        """raw_audio CUDA [B, S, L] (or [B, L] when mono) -> [B, S, hop * (L // hop)], or [B, S, L] with
-        match_input_audio_length, as the reference's forward"""
-        x = self.check_input(raw_audio)
-        B, S, L = x.shape
-        dev, dim, nb, NB = x.device, self.dim, self.num_bands, self.n_fft // 2 + 1
-        bins, band_off, cover, cover_off = self._tables()
-        n_slots = len(self.bins)
-        cplx = ops.stft(x.view(B * S, L), self.n_fft, self.hop)                     # [B*S, T, NB, 2]
-        T = cplx.shape[1]
-        feat = ops.melband_input(cplx, B, S, band_off, bins, torch.empty((B * T, 2 * S * n_slots), device=dev))
-        x = self._band_split(feat, self.band_off, B * T)
-        del feat
-        cs_t, cs_f = self._rope_table(T), self._rope_table(nb)
-        for i in range(self.depth):
-            for a, n, cs, Lq, geo in ((0, self.t_depth, cs_t, T, (B, T * nb, nb, 1, nb)),
-                                      (1, self.f_depth, cs_f, nb, (B * T, nb, 1, 0, 1))):
-                p = f"layers.{i}.{a}"
-                x = self._transformer(x, p, n, cs, Lq, geo)
-                if p + ".norm.g" in self.bias:
-                    ops.row_rmsnorm(x, self.bias[p + ".norm.g"], out=x)
-        xn = ops.row_l2norm(x).view(B * T, nb * dim)                 # the last Transformer's norm; its gamma is folded
-        del x
-        g = self._mask_estimator(xn, self.band_off, torch.empty((B * T, 2 * S * n_slots), device=dev))
-        del xn
-        mask = ops.melband_mask_avg(g, S, cover_off, cover, torch.empty((B * T, 2 * S * NB), device=dev))
-        del g
-        out = ops.istft(cplx, B, S, self.n_fft, self.hop, mask=mask, length=L if self.match_input_audio_length else None)
-        return out.view(B, S, -1)
-
-    __call__ = forward

@@ -1868,7 +1868,7 @@ class _CeFn(torch.autograd.Function):
         nll = torch.empty(rows, device=dev, dtype=torch.float32)
         flags = torch.empty(rows, device=dev, dtype=torch.uint8)
         out2 = torch.empty(2, device=dev, dtype=torch.float32)
-        _call("evk_ce_fwd_ex", _p(logits), ld, _p(targets), rows, V, topk, ignore, _p(count), T, _p(lse), _p(nll), _p(flags), _p(out2))
+        _call("evk_ce_fwd", _p(logits), ld, _p(targets), rows, V, topk, ignore, _p(count), T, _p(lse), _p(nll), _p(flags), _p(out2))
         ctx.save_for_backward(logits, targets, lse, count)
         ctx.V, ctx.T = V, T
         ctx.mark_non_differentiable(out2)
@@ -1881,7 +1881,7 @@ class _CeFn(torch.autograd.Function):
         V = ctx.V
         gl = gloss.reshape(1).contiguous().float()
         dl = (torch.empty if Vp == V else torch.zeros)(logits.shape, device=logits.device, dtype=torch.float32)
-        _call("evk_ce_bwd_ex", _p(logits), ld, _p(targets), _p(lse), _p(gl), rows, _p(count), ctx.T, _p(dl), Vp, rows, V)
+        _call("evk_ce_bwd", _p(logits), ld, _p(targets), _p(lse), _p(gl), rows, _p(count), ctx.T, _p(dl), Vp, rows, V)
         return dl, None, None, None, None, None
 
 
@@ -1910,7 +1910,7 @@ def attn_decode_dev(cache, n_prev_dev, heads, row, skip=None):
 
 
 def sample_tokens(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, alpha, x_next, q=None, eos_steps=1):
-    """One fused sampling step over the rows of `logits` [B, >= V] (evk_sample_tokens_ex; see include/evk.h for the buffers).
+    """One fused sampling step over the rows of `logits` [B, >= V] (evk_sample_tokens; see include/evk.h for the buffers).
     EOS is excluded at the steps idx < eos_steps (1: infer_panel_batch_infer; 11: infer_panel_naive and prompt-free decoding).
     Everything it reads or writes stays in device memory, so it can be part of a captured CUDA graph."""
     B, D = logits.shape[0], x_next.shape[-1]
@@ -1919,7 +1919,7 @@ def sample_tokens(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, a
     assert logits.stride(-1) == 1 and hist.dtype == torch.int64 and seen.dtype == torch.int32 and fin.dtype == torch.int32
     assert icfg.dtype == torch.int64 and fcfg.dtype == torch.float32 and x_next.is_contiguous() and pe.is_contiguous()
     assert q is None or (q.shape[0] == B and q.stride(-1) == 1)
-    _call("evk_sample_tokens_ex", _p(logits), logits.stride(0), B, V, eos, int(eos_steps), _p(icfg), _p(fcfg), _p(n_dev), _p(q),
+    _call("evk_sample_tokens", _p(logits), logits.stride(0), B, V, eos, int(eos_steps), _p(icfg), _p(fcfg), _p(n_dev), _p(q),
           q.stride(0) if q is not None else 0, _p(hist), hist.stride(0), _p(seen), _p(fin), _p(emb), _p(pe), _p(alpha),
           _p(x_next), D)
 
@@ -1927,7 +1927,7 @@ def sample_tokens(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, a
 def ce_sum_topk(logits, targets, topk=3, ignore_index=1024, V=None, count=None):
     """-> (sum cross-entropy (differentiable), device float32 [2] = (loss, top-k accuracy ignoring ignore_index)).
     V: number of real classes when the last dim of `logits` is zero-padded.  count: None, or an int32 device scalar n for
-    [B, T, Vp] logits: positions t >= n of every row add no loss, no accuracy count and no gradient (evk_ce_fwd_ex)."""
+    [B, T, Vp] logits: positions t >= n of every row add no loss, no accuracy count and no gradient (evk_ce_fwd)."""
     loss, out2 = _CeFn.apply(logits, targets, int(topk), int(ignore_index), int(V or logits.shape[-1]), count)
     return loss, out2
 
@@ -1951,11 +1951,11 @@ class _DpoCeFn(torch.autograd.Function):
             nll = torch.empty(rows, device=dev, dtype=torch.float32)
             flags = torch.empty(rows, device=dev, dtype=torch.uint8)
             o2 = torch.empty(2, device=dev, dtype=torch.float32)
-            _call("evk_ce_fwd_ex", _p(lg), _rows(lg)[2], _p(tg), rows, V, topk, ignore, _p(cn), T, _p(lse), _p(nll), _p(flags), _p(o2))
+            _call("evk_ce_fwd", _p(lg), _rows(lg)[2], _p(tg), rows, V, topk, ignore, _p(cn), T, _p(lse), _p(nll), _p(flags), _p(o2))
             bufs.append((lse, nll, o2))
         out3 = torch.empty(3, device=dev, dtype=torch.float32)
         coef = torch.empty((2, B), device=dev, dtype=torch.float32)
-        _call("evk_dpo_head_ex", _p(bufs[0][1]), Yc, _p(cnt[0]), _p(bufs[1][1]), Yr, _p(cnt[1]), B, ctypes.c_float(beta), _p(out3),
+        _call("evk_dpo_head", _p(bufs[0][1]), Yc, _p(cnt[0]), _p(bufs[1][1]), Yr, _p(cnt[1]), B, ctypes.c_float(beta), _p(out3),
               _p(coef[0]), _p(coef[1]))
         ctx.save_for_backward(lc, tc, bufs[0][0], lr_, tr, bufs[1][0], coef, count)
         ctx.k = (B, Yc, Yr, V)
@@ -1973,7 +1973,7 @@ class _DpoCeFn(torch.autograd.Function):
         for lg, tg, lse, Yn, cf, cn in ((lc, tc, lsec, Yc, gc[0], cnt[0]), (lr_, tr, lser, Yr, gc[1], cnt[1])):
             rows, Vp, ld = _rows(lg)
             dl = (torch.empty if Vp == V else torch.zeros)(lg.shape, device=lg.device, dtype=torch.float32)
-            _call("evk_ce_bwd_ex", _p(lg), ld, _p(tg), _p(lse), _p(cf), Yn, _p(cn), Yn, _p(dl), Vp, rows, V)
+            _call("evk_ce_bwd", _p(lg), ld, _p(tg), _p(lse), _p(cf), Yn, _p(cn), Yn, _p(dl), Vp, rows, V)
             outs.append(dl)
         return outs[0], None, outs[1], None, None, None, None, None, None
 
@@ -1986,7 +1986,7 @@ def _AxpbyFn_scale(coef, g):
 def dpo_ce(logits_c, targets_c, logits_r, targets_r, topk=3, ignore_index=1024, V=None, beta=0.2, count=None):
     """-> (loss_1 + loss_2 (differentiable), device [3] = (loss_1, loss_2, top-k acc)).  count: None, or int32 device [2] =
     (chosen, rejected) counted lengths: positions at or past a branch's count add no loss, accuracy or gradient, and do not
-    enter that branch's log-prob sums (evk_ce_fwd_ex / evk_dpo_head_ex)."""
+    enter that branch's log-prob sums (evk_ce_fwd / evk_dpo_head)."""
     return _DpoCeFn.apply(logits_c, targets_c, logits_r, targets_r, int(topk), int(ignore_index),
                           int(V or logits_c.shape[-1]), float(beta), count)
 
@@ -2068,16 +2068,14 @@ def conv2d_out(n, k, stride, pad, dil):
 
 def conv2d(x: CLView, w, y: CLView, *, k, stride=1, pad=0, dil=1, scale=None, bias=None, act=C2_NONE):
     """y = act(conv2d(x) * scale + bias) (evk_conv2d_fwd): w [N, k, k, C] fp32 contiguous; y must be [B, Ho, Wo, N].
-    pad and dil are ints, or (rows, columns) pairs (evk_conv2d_fwd_hw)."""
+    pad and dil are ints, or (rows, columns) pairs."""
     N = w.shape[0]
     assert w.is_contiguous() and tuple(w.shape) == (N, k, k, x.C) and y.C == N and y.B == x.B, (w.shape, x.C, y.C)
-    hw = isinstance(pad, (tuple, list)) or isinstance(dil, (tuple, list))
     (ph, pw), (dh, dw) = [v if isinstance(v, (tuple, list)) else (v, v) for v in (pad, dil)]
     Ho, Wo = conv2d_out(x.H, k, stride, ph, dh), conv2d_out(x.W, k, stride, pw, dw)
     assert (y.H, y.W) == (Ho, Wo), ((y.H, y.W), (Ho, Wo))
-    geo = ("evk_conv2d_fwd_hw", ph, pw, dh, dw) if hw else ("evk_conv2d_fwd", ph, dh)
-    _call_f(geo[0], 2.0 * x.B * Ho * Wo * N * k * k * x.C, *x.args(), _p(w), _p(scale), _p(bias), *y.args(),
-            x.B, x.H, x.W, x.C, N, k, stride, *geo[1:], act, tag=f"k{k}")
+    _call_f("evk_conv2d_fwd", 2.0 * x.B * Ho * Wo * N * k * k * x.C, *x.args(), _p(w), _p(scale), _p(bias), *y.args(),
+            x.B, x.H, x.W, x.C, N, k, stride, ph, pw, dh, dw, act, tag=f"k{k}")
 
 
 def dwconv3x3(x: CLView, w, y: CLView, dil):
@@ -2139,7 +2137,8 @@ def lstm_bidir(g, w_hh, order="tn"):
 
 
 # ------------------------------------------------------------------------------------------------
-# BS-Roformer (bs_roformer.py): rotary gated attention, band input, row L2 norm, inverse STFT
+# BS-Roformer and Mel-Band Roformer (bs_roformer.py, mel_band_roformer.py): rotary gated attention, band input, row norm,
+# averaged band masks, inverse STFT
 # ------------------------------------------------------------------------------------------------
 def linear_into(x, w: PackedW, y, bias=None, act=ACT_NONE, res=None):
     """y = act(x W^T + bias + res) written into y (no autograd): x [rows, C] and y [rows, N] are 2-D views with unit column
@@ -2162,55 +2161,25 @@ def rope_attn(qkvg, cs, out, heads, L, n_outer, s_outer, n_inner, s_inner, s_tok
     return out
 
 
-def row_l2norm(x, out=None):
-    """x / max(||x||_2, 1e-12) per row of a [rows, C] view (evk_row_l2norm)"""
+def row_norm(x, gamma=None, out=None):
+    """x / max(||x||_2, 1e-12) per row of a [rows, C] view, times sqrt(C) * gamma when gamma is given (evk_row_norm); out may
+    be x"""
     rows, C = x.shape
     assert x.stride(1) == 1
+    assert gamma is None or (gamma.is_contiguous() and gamma.numel() == C and gamma.dtype == torch.float32)
     out = torch.empty((rows, C), device=x.device, dtype=torch.float32) if out is None else out
-    _call("evk_row_l2norm", _p(x), x.stride(0), _p(out), out.stride(0), rows, C)
+    _call("evk_row_norm", _p(x), x.stride(0), _p(gamma), _p(out), out.stride(0), rows, C)
     return out
 
 
-def bs_band_input(cplx, B, S, band_off, out):
-    """evk_bs_band_input: cplx [B*S, T, n_bins, 2] (ops.stft) -> out [B*T, >= 2*S*n_bins] in 'b t (f s c)' order, each band's
-    segment L2-normalised; band_off int32 device [n_bands + 1] bin offsets."""
-    _, T, nb, _ = cplx.shape
-    assert cplx.is_contiguous() and out.stride(1) == 1 and band_off.dtype == torch.int32
-    _call("evk_bs_band_input", _p(cplx), B, S, T, nb, _p(band_off), band_off.numel() - 1, _p(out), out.stride(0))
-    return out
-
-
-def istft(cplx, B, S, n_fft, hop, mask=None, out=None, work=None, length=None):
-    """torch.istft(center=True, Hann(n_fft)) of cplx [B*S, T, n_fft/2+1, 2] (times the complex mask [B*T, (f s c)] when given)
-    -> [B*S, hop*(T-1)] (evk_istft), or [B*S, length] as torch.istft(length=length) (evk_istft_length).  work: scratch of
-    B*S*T*n_fft floats (allocated when None)."""
-    T = cplx.shape[1]
-    assert cplx.is_contiguous() and cplx.shape[2] == n_fft // 2 + 1
-    if out is None:
-        out = torch.empty((B * S, hop * (T - 1) if length is None else length), device=cplx.device, dtype=torch.float32)
-    if work is None:
-        work = torch.empty(B * S * T * n_fft, device=cplx.device, dtype=torch.float32)
-    assert work.numel() >= B * S * T * n_fft and out.stride(1) == 1
-    if mask is not None:
-        assert mask.stride(1) == 1 and mask.shape[0] == B * T
-    ldm = mask.stride(0) if mask is not None else 0
-    if length is None:
-        _call("evk_istft", _p(cplx), _p(mask), ldm, B, S, T, n_fft, hop, _p(work), _p(out), out.stride(0))
-    else:
-        _call("evk_istft_length", _p(cplx), _p(mask), ldm, B, S, T, n_fft, hop, int(length), _p(work), _p(out), out.stride(0))
-    return out
-
-
-# ------------------------------------------------------------------------------------------------
-# Mel-Band Roformer (mel_band_roformer.py): overlapping band input, averaged band masks, RMSNorm with gamma
-# ------------------------------------------------------------------------------------------------
-def melband_input(cplx, B, S, band_off, bins, out):
-    """evk_melband_input: cplx [B*S, T, n_bins, 2] (ops.stft) -> out [B*T, >= 2*S*len(bins)]: band i's bins
-    bins[band_off[i]:band_off[i+1]] in 'b t (f s c)' order, each band's segment L2-normalised; band_off, bins int32 device."""
+def band_input(cplx, B, S, band_off, bins, out):
+    """evk_band_input: cplx [B*S, T, n_bins, 2] (ops.stft) -> out [B*T, >= 2*S*len(bins)]: band i's bins
+    bins[band_off[i]:band_off[i+1]] in 'b t (f s c)' order, each band's segment L2-normalised; band_off, bins int32 device
+    (BS-Roformer's bins: arange(n_bins))."""
     _, T, nb, _ = cplx.shape
     assert cplx.is_contiguous() and out.stride(1) == 1 and band_off.dtype == torch.int32 and bins.dtype == torch.int32
     assert out.shape[0] == B * T and out.shape[1] >= 2 * S * bins.numel()
-    _call("evk_melband_input", _p(cplx), B, S, T, nb, _p(band_off), _p(bins), band_off.numel() - 1, _p(out), out.stride(0))
+    _call("evk_band_input", _p(cplx), B, S, T, nb, _p(band_off), _p(bins), band_off.numel() - 1, _p(out), out.stride(0))
     return out
 
 
@@ -2226,12 +2195,22 @@ def melband_mask_avg(g, S, cover_off, cover, out):
     return out
 
 
-def row_rmsnorm(x, gamma, out=None):
-    """x / max(||x||_2, 1e-12) * sqrt(C) * gamma per row of a [rows, C] view (evk_row_rmsnorm); out may be x"""
-    rows, C = x.shape
-    assert x.stride(1) == 1 and gamma.is_contiguous() and gamma.numel() == C and gamma.dtype == torch.float32
-    out = torch.empty((rows, C), device=x.device, dtype=torch.float32) if out is None else out
-    _call("evk_row_rmsnorm", _p(x), x.stride(0), _p(gamma), _p(out), out.stride(0), rows, C)
+def istft(cplx, B, S, n_fft, hop, mask=None, out=None, work=None, length=None):
+    """torch.istft(center=True, Hann(n_fft)) of cplx [B*S, T, n_fft/2+1, 2] (times the complex mask [B*T, (f s c)] when given)
+    -> [B*S, hop*(T-1)], or [B*S, length] as torch.istft(length=length) (evk_istft).  work: scratch of B*S*T*n_fft floats
+    (allocated when None)."""
+    T = cplx.shape[1]
+    assert cplx.is_contiguous() and cplx.shape[2] == n_fft // 2 + 1
+    if out is None:
+        out = torch.empty((B * S, hop * (T - 1) if length is None else length), device=cplx.device, dtype=torch.float32)
+    if work is None:
+        work = torch.empty(B * S * T * n_fft, device=cplx.device, dtype=torch.float32)
+    assert work.numel() >= B * S * T * n_fft and out.stride(1) == 1
+    if mask is not None:
+        assert mask.stride(1) == 1 and mask.shape[0] == B * T
+    ldm = mask.stride(0) if mask is not None else 0
+    _call("evk_istft", _p(cplx), _p(mask), ldm, B, S, T, n_fft, hop, 0 if length is None else int(length), _p(work), _p(out),
+          out.stride(0))
     return out
 
 
@@ -2431,14 +2410,15 @@ def mdx_add(a: CLView, b: CLView, y: CLView, m: CLView = None):
 # ------------------------------------------------------------------------------------------------
 # Whisper transcription (whisper.py): log-mel front end, decode attention with slot tables, beam step
 # ------------------------------------------------------------------------------------------------
-def whisper_logmel(wav, lens, basis, fb, out=None):
-    """evk_whisper_logmel: wav [B, L] fp32 (row b holds lens[b] 16 kHz samples; lens int32 device [B]), basis [2, 400, 201],
-    fb [201, n_mels] -> [B, 3000, n_mels] normalised log-mel, zero after each clip's lens[b] // 160 frames."""
+def whisper_logmel(wav, lens, T, basis, fb):
+    """evk_whisper_logmel: wav [B, L] fp32 (row b holds lens[b] 16 kHz samples; lens int32 device [B], lens[b] // 160 <= T),
+    basis [2, 400, 201], fb [201, n_mels] -> [B, T, n_mels] normalised log-mel of each whole clip (max over all its frames),
+    zero after its lens[b] // 160 frames.  T = 3000: the encoder's 30 s input."""
     assert wav.dim() == 2 and wav.stride(1) == 1 and lens.dtype == torch.int32 and basis.is_contiguous() and fb.is_contiguous()
     B, M = wav.shape[0], fb.shape[1]
-    out = torch.empty((B, 3000, M), device=wav.device, dtype=torch.float32) if out is None else out
-    assert out.is_contiguous() and out.shape == (B, 3000, M)
-    _call("evk_whisper_logmel", _p(wav), wav.stride(0), _p(lens), B, _p(basis), _p(fb), M, _p(out))
+    out = torch.empty((B, T, M), device=wav.device, dtype=torch.float32)
+    part = torch.empty((B, (T + 255) // 256), device=wav.device, dtype=torch.float32)
+    _call("evk_whisper_logmel", _p(wav), wav.stride(0), _p(lens), B, T, _p(basis), _p(fb), M, _p(part), _p(out))
     return out
 
 
@@ -2490,39 +2470,18 @@ def whisper_first_pass(logits, nospeech, lang_ids, nsp, lang_tok):
           lang_ids.numel(), _p(nsp), _p(lang_tok))
 
 
-def whisper_beam_step(logits, st, beam, lay, length_penalty=1.0):
+def whisper_beam_step(logits, st, beam, lay, length_penalty=1.0, track_lse=False):
     """evk_whisper_beam_step on the decode state `st` (whisper.WhisperModel._state) with token layout `lay` =
-    (eot, notimestamps, ts_begin, max_init_ts, prompt_len, max_length)."""
+    (eot, notimestamps, ts_begin, max_init_ts, prompt_len, max_length).  track_lse: also carry st["run_lse"] / st["fin_lse"],
+    each hypothesis' sum of its processed rows' log-sum-exp (st["row_lse"] is scratch)."""
     clips = logits.shape[0] // beam
     assert st["fin_seq"].stride(1) == st["hist"].stride(0) and st["tab"].stride(0) <= 448
+    lse = [_p(st[k]) if track_lse else None for k in ("row_lse", "run_lse", "fin_lse")]
     _call("evk_whisper_beam_step", _p(logits), logits.stride(0), clips, beam, logits.shape[1], *[int(v) for v in lay],
           _p(st["sup"]), st["sup"].numel(), _p(st["bsup"]), st["bsup"].numel(), _p(st["g"]), ctypes.c_float(length_penalty),
           _p(st["cv"]), _p(st["ci"]), _p(st["score"]), _p(st["hist"]), st["hist"].stride(0), _p(st["tab"]), st["tab"].stride(0),
           _p(st["tok"]), _p(st["parent"]), _p(st["fin_score"]), _p(st["fin_seq"]), _p(st["fin_len"]),
-          _p(st["fin_flag"]), _p(st["unsat"]))
-
-
-def whisper_beam_step_lse(logits, st, beam, lay, length_penalty=1.0):
-    """evk_whisper_beam_step_lse: whisper_beam_step that also carries st["run_lse"] / st["fin_lse"], each hypothesis' sum of
-    its processed rows' log-sum-exp (st["row_lse"] is scratch)."""
-    clips = logits.shape[0] // beam
-    assert st["fin_seq"].stride(1) == st["hist"].stride(0) and st["tab"].stride(0) <= 448
-    _call("evk_whisper_beam_step_lse", _p(logits), logits.stride(0), clips, beam, logits.shape[1], *[int(v) for v in lay],
-          _p(st["sup"]), st["sup"].numel(), _p(st["bsup"]), st["bsup"].numel(), _p(st["g"]), ctypes.c_float(length_penalty),
-          _p(st["cv"]), _p(st["ci"]), _p(st["score"]), _p(st["hist"]), st["hist"].stride(0), _p(st["tab"]), st["tab"].stride(0),
-          _p(st["tok"]), _p(st["parent"]), _p(st["fin_score"]), _p(st["fin_seq"]), _p(st["fin_len"]),
-          _p(st["fin_flag"]), _p(st["unsat"]), _p(st["row_lse"]), _p(st["run_lse"]), _p(st["fin_lse"]))
-
-
-def whisper_logmel_long(wav, lens, T, basis, fb):
-    """evk_whisper_logmel_long: wav [B, L] fp32 (row b holds lens[b] 16 kHz samples; lens int32 device [B]) -> [B, T, n_mels]
-    normalised log-mel of each whole clip (max over all its frames), zero after its lens[b] // 160 frames."""
-    assert wav.dim() == 2 and wav.stride(1) == 1 and lens.dtype == torch.int32 and basis.is_contiguous() and fb.is_contiguous()
-    B, M = wav.shape[0], fb.shape[1]
-    out = torch.empty((B, T, M), device=wav.device, dtype=torch.float32)
-    part = torch.empty((B, (T + 255) // 256), device=wav.device, dtype=torch.float32)
-    _call("evk_whisper_logmel_long", _p(wav), wav.stride(0), _p(lens), B, T, _p(basis), _p(fb), M, _p(part), _p(out))
-    return out
+          _p(st["fin_flag"]), _p(st["unsat"]), *lse)
 
 
 def whisper_window(lm, tab, out=None):

@@ -11,9 +11,9 @@ at most 30 s, long-form (`transcribe_long`: 30 s windows moved by the predicted 
   decoder     one step of all rows: token + learned position, per layer causal self-attention on slot tables
               (evk_whisper_self_kv / evk_whisper_attn), cross-attention, MLP; final LayerNorm; logits from the tied token
               embedding; evk_whisper_beam_step.  The step is captured as a CUDA graph per batch shape and replayed.
-  long-form   evk_whisper_logmel_long: the same log-mel over the whole clip, clamped at the whole clip's max - 8;
-              evk_whisper_window cuts the 3000-frame window at each clip's seek; the windows of several clips are encoded and
-              decoded together as above (evk_whisper_beam_step_lse, which also yields transformers' avg_logprob), and each
+  long-form   evk_whisper_logmel over the whole clip, clamped at the whole clip's max - 8; evk_whisper_window cuts the
+              3000-frame window at each clip's seek; the windows of several clips are encoded and decoded together as above
+              (evk_whisper_beam_step with its log-sum-exp buffers, which also yield transformers' avg_logprob), and each
               clip's seek moves on the host by transformers' _retrieve_segment rules.
 
 Compute is fp32 storage with TF32 tensor-core products in the Linears and the encoder's attention (3xTF32 under
@@ -239,7 +239,7 @@ class WhisperModel(ParamTree):
                 raise ValueError(f"row {b}: {n} samples (a clip takes 201 .. 480000 samples of 16 kHz audio)")
         pk = self._packed()
         ln = torch.tensor(lens, dtype=torch.int32).to(wav.device)
-        return ops.whisper_logmel(wav.float().contiguous(), ln, pk["basis"], pk["fb"])
+        return ops.whisper_logmel(wav.float().contiguous(), ln, N_FRAMES, pk["basis"], pk["fb"])
 
     @torch.no_grad()
     def features_long(self, wav, lens):
@@ -251,7 +251,7 @@ class WhisperModel(ParamTree):
                 raise ValueError(f"row {b}: {n} samples (a clip takes at least 201 samples of 16 kHz audio)")
         pk = self._packed()
         ln = torch.tensor(lens, dtype=torch.int32).to(wav.device)
-        return ops.whisper_logmel_long(wav.float().contiguous(), ln, max(lens) // HOP, pk["basis"], pk["fb"])
+        return ops.whisper_logmel(wav.float().contiguous(), ln, max(lens) // HOP, pk["basis"], pk["fb"])
 
     @torch.no_grad()
     def encode(self, feats):
@@ -336,7 +336,7 @@ class WhisperModel(ParamTree):
         """The decode step (forward of every row, beam step, position + 1) captured once per (clips, beam, max_new_tokens,
         track_lse).  Graphs of one (clips, beam) share one decode state; a batch of another shape replaces that state and its
         graphs rather than adding to the device memory a batch is sized for (cross K/V and slots for every clip).  track_lse:
-        the step is evk_whisper_beam_step_lse, which also carries what transformers' long-form avg_logprob needs."""
+        the beam step also carries what transformers' long-form avg_logprob needs."""
         skey = (clips, beam, str(dev))
         if self.__dict__.get("_gstate") is None or self._gstate[0] != skey:
             self._graphs.clear()
@@ -348,11 +348,10 @@ class WhisperModel(ParamTree):
             return self._graphs[gkey]
         st = self._gstate[1]
         lay = self._layout(3, max_new_tokens)
-        beam_step = ops.whisper_beam_step_lse if track_lse else ops.whisper_beam_step
 
         def step():
             lg = self._forward_rows(st)
-            beam_step(lg, st, beam, lay)
+            ops.whisper_beam_step(lg, st, beam, lay, track_lse=track_lse)
             st["pos"].add_(1)
             st["g"].add_(1)
             return lg

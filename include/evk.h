@@ -453,51 +453,38 @@ int evk_cache_append(const float* row, int32_t ldr, float* cache, int64_t batch_
  * per row b of logits [B][ldl] (V <= 2048 classes, eos = V - 1), in the reference's order: repetition penalty over the row's
  * history (prompt included) -> top-p if top_p < 1 (descending order, cumulative softmax, `cum > top_p` removed, the first kept;
  * on the penalised, un-tempered logits) -> / max(T, 1e-5) -> top-k (values >= the k-th largest kept) -> softmax ->
- * argmax(p / q), q ~ Exp(1).  The step is idx = *n_dev - icfg[2]; at idx 0 EOS is excluded.  The row stops when the token or the
- * argmax of the penalised logits is EOS (fin[b] = (idx, idx - 1)), else when idx + 1 > early_stop (!= -1) or idx == max_steps - 1
- * (fin[b] = (idx, idx)); a row with fin[b][0] >= 0 is left untouched.  Otherwise hist[b][prefix + idx] = token, its bit is set
- * in seen, and x_next[b] = emb[token] + alpha[0] * pe[prefix + idx].
+ * argmax(p / q), q ~ Exp(1).  The step is idx = *n_dev - icfg[2]; at idx < eos_steps (>= 0) EOS is excluded (the batched
+ * decoders pass 1; infer_panel_naive, t2s_model.py:835-836, passes 11, with a prompt or without one).  The row stops when
+ * the token or the argmax of the penalised logits is EOS (fin[b] = (idx, idx - 1)), else when idx + 1 > early_stop (!= -1)
+ * or idx == max_steps - 1 (fin[b] = (idx, idx)); a row with fin[b][0] >= 0 is left untouched.  Otherwise hist[b][prefix +
+ * idx] = token, its bit is set in seen, and x_next[b] = emb[token] + alpha[0] * pe[prefix + idx].
  *   icfg: device int64 [6] = (seed, prefix, n0, top_k >= 1, early_stop, max_steps);  fcfg: device float [3] = (top_p, T, penalty)
  *   q: NULL (counter-based Exp(1) draws keyed by (seed, row, idx, class)) or supplied draws [B][ldq]
  *   hist: int64 [B][ldh];  seen: uint32 [B][(V + 31) / 32] bitmap of the tokens in hist;  fin: int32 [B][2], -1 while running
  *   emb: [V][D], pe: [*][D], x_next: [B][D]. */
-int evk_sample_tokens(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, const int64_t* icfg,
-                      const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist, int32_t ldh,
-                      uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha, float* x_next,
-                      int32_t D, evk_stream_t stream);
-/* The same with EOS excluded at every step idx < eos_steps (>= 0) instead of at step 0 only: evk_sample_tokens is this call with
- * eos_steps = 1.  infer_panel_naive (t2s_model.py:835-836) passes 11, with a prompt or without one (prefix 0). */
-int evk_sample_tokens_ex(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, int32_t eos_steps,
-                         const int64_t* icfg, const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist,
-                         int32_t ldh, uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha,
-                         float* x_next, int32_t D, evk_stream_t stream);
+int evk_sample_tokens(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, int32_t eos_steps,
+                      const int64_t* icfg, const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist,
+                      int32_t ldh, uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha,
+                      float* x_next, int32_t D, evk_stream_t stream);
+/* Cross entropy over rows [B][T] of positions (row r is position r % T).  count: NULL (every row counts; T is then unused), or
+ * a device int32 scalar n: positions t >= n add no loss, no accuracy count (neither valid nor hit) and no gradient (evk_ce_bwd
+ * writes 0 to their logit gradients).  The bound is for batches padded past the collate's length (the stage-1 trainer pads to
+ * a 32-token grid so that a CUDA graph can serve many batches): the reference sums CE over every position of its padded batch
+ * (EOS targets included), so positions added by further padding must not count. */
 int evk_ce_fwd(const float* logits, int32_t ld, const int64_t* targets, int32_t rows, int32_t V, int32_t topk,
-               int64_t ignore_index, float* lse, float* nll, uint8_t* flags, float* out2, evk_stream_t stream);
+               int64_t ignore_index, const int32_t* count, int32_t T, float* lse, float* nll, uint8_t* flags, float* out2,
+               evk_stream_t stream);
 int evk_ce_bwd(const float* logits, int32_t ld, const int64_t* targets, const float* lse, const float* gscale,
-               int32_t rows_per_g /* row r is scaled by gscale[r / rows_per_g]; == rows for one scalar */, float* dl,
-               int32_t lddl, int32_t rows, int32_t V, evk_stream_t stream);
+               int32_t rows_per_g /* row r is scaled by gscale[r / rows_per_g]; == rows for one scalar */, const int32_t* count,
+               int32_t T, float* dl, int32_t lddl, int32_t rows, int32_t V, evk_stream_t stream);
 /* DPO head of Text2SemanticDecoder.forward (t2s_model.py:393-429; utils.py:160-192 with reference_free=True): from the
  * per-token nll of the chosen [B, Yc] and rejected [B, Yr] sequences: out3 = (sum CE of chosen, mean_b -logsigmoid(beta *
- * (logp_chosen_b - logp_rejected_b)), their sum); coef_c/coef_r [B] = d out3[2] / d nll_{c,r}[b][t] (feeds evk_ce_bwd). */
-int evk_dpo_head(const float* nll_c, int32_t Yc, const float* nll_r, int32_t Yr, int32_t B, float beta, float* out3,
-                 float* coef_c, float* coef_r, evk_stream_t stream);
-/* Counted-length bound on the three calls above, for batches padded past the collate's length (the stage-1 trainer pads to
- * a 32-token grid so that a CUDA graph can serve many batches).  The rows are [B][T] positions (row r is position r % T).
- * count: NULL, or a device int32 scalar n: positions t >= n add no loss, no accuracy count (neither valid nor hit) and no
- * gradient (evk_ce_bwd_ex writes 0 to their logit gradients).  count == NULL is exactly evk_ce_fwd / evk_ce_bwd.
- * The bound reproduces the loss at the collate's shape: the reference sums CE over every position of its padded batch (EOS
- * targets included), so positions added by further padding must not count. */
-int evk_ce_fwd_ex(const float* logits, int32_t ld, const int64_t* targets, int32_t rows, int32_t V, int32_t topk,
-                  int64_t ignore_index, const int32_t* count, int32_t T, float* lse, float* nll, uint8_t* flags, float* out2,
-                  evk_stream_t stream);
-int evk_ce_bwd_ex(const float* logits, int32_t ld, const int64_t* targets, const float* lse, const float* gscale,
-                  int32_t rows_per_g, const int32_t* count, int32_t T, float* dl, int32_t lddl, int32_t rows, int32_t V,
-                  evk_stream_t stream);
-/* evk_dpo_head with counted lengths: count_c / count_r NULL, or device int32 scalars; the per-row log-prob sums (and so
- * loss_1) then run over t < min(Yc, *count_c) resp. t < min(Yr, *count_r).  NULL for both is exactly evk_dpo_head.  The
- * stage-1 trainer passes the collate's Y for the chosen branch and max(reject_lens) for the rejected one. */
-int evk_dpo_head_ex(const float* nll_c, int32_t Yc, const int32_t* count_c, const float* nll_r, int32_t Yr,
-                    const int32_t* count_r, int32_t B, float beta, float* out3, float* coef_c, float* coef_r, evk_stream_t stream);
+ * (logp_chosen_b - logp_rejected_b)), their sum); coef_c/coef_r [B] = d out3[2] / d nll_{c,r}[b][t] (feeds evk_ce_bwd).
+ * count_c / count_r: NULL, or device int32 scalars; the per-row log-prob sums (and so loss_1) then run over
+ * t < min(Yc, *count_c) resp. t < min(Yr, *count_r).  The stage-1 trainer passes the collate's Y for the chosen branch and
+ * max(reject_lens) for the rejected one. */
+int evk_dpo_head(const float* nll_c, int32_t Yc, const int32_t* count_c, const float* nll_r, int32_t Yr,
+                 const int32_t* count_r, int32_t B, float beta, float* out3, float* coef_c, float* coef_r, evk_stream_t stream);
 /* Rejected rows of the DPO variant (utils.py:195-232, the repeat branch) from host-drawn spans, capturable in a CUDA graph:
  * row b of y [B][ldy] (int64, padded chosen rows) with span (i0, i1) = spans[b] (int32 [B][2], 0 <= i0 <= i1 <= Yc) becomes
  *   out[b] = y[b][:i0] ++ y[b][i0:i1] ++ y[b][i0:i1] ++ y[b][i1:Yc]  followed by 0 up to Yr   (out: int64 [B][Yr])
@@ -541,21 +528,16 @@ int evk_attn_pad_fwd(const float* q, const float* k, const float* v, int32_t ld,
 enum evk_conv2d_act { EVK_C2_NONE = 0, EVK_C2_RELU = 1, EVK_C2_LRELU = 2 /* slope 0.01 */, EVK_C2_SIGMOID = 3,
                       EVK_C2_GELU = 4 /* exact erf */ };
 /* y = act(conv2d(x, w) * scale[n] + bias[n])  (scale / bias may be null: 1 / 0).  x: [B, H, W, C] (pitch x_pitch >= C,
- * batch stride x_bs); w: [N][k][k][C] (k = 1, 2 or 3); stride 1 or 2, zero padding pad, dilation dil >= 1; y: [B, Ho, Wo, N]
- * (pitch y_pitch >= N, batch stride y_bs), Ho = (H + 2 pad - dil (k - 1) - 1) / stride + 1.  Implicit GEMM with TF32
+ * batch stride x_bs); w: [N][k][k][C] (k = 1, 2 or 3); stride 1 or 2, zero padding and dilation >= 1 per axis (the DeEcho /
+ * DeReverb ASPP: dilation (4, 2), (8, 4), (12, 6)); y: [B, Ho, Wo, N] (pitch y_pitch >= N, batch stride y_bs),
+ * Ho = (H + 2 pad_h - dil_h (k - 1) - 1) / stride + 1, Wo likewise with pad_w, dil_w.  Implicit GEMM with TF32
  * products and fp32 accumulation: wgmma when C, x_pitch and x_bs are multiples of 4 and x, w are 16-byte aligned,
  * mma.sync otherwise and for 3xTF32 under evk_set_precise(1).  No atomics, and every output's sum has one order whatever
  * B is, so results are bit-reproducible and independent of the batch. */
 int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale, const float* bias,
                    float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W, int32_t C, int32_t N, int32_t k,
-                   int32_t stride, int32_t pad, int32_t dil, int32_t act, evk_stream_t stream);
-/* evk_conv2d_fwd with zero padding and dilation per axis (the DeEcho / DeReverb ASPP: dilation (4, 2), (8, 4), (12, 6)):
- * Ho = (H + 2 pad_h - dil_h (k - 1) - 1) / stride + 1, Wo likewise with pad_w, dil_w.  Same kernels, dispatch and
- * guarantees; evk_conv2d_fwd(..., pad, dil, ...) is this call with pad_h = pad_w = pad, dil_h = dil_w = dil. */
-int evk_conv2d_fwd_hw(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale, const float* bias,
-                      float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W, int32_t C, int32_t N,
-                      int32_t k, int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h, int32_t dil_w, int32_t act,
-                      evk_stream_t stream);
+                   int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h, int32_t dil_w, int32_t act,
+                   evk_stream_t stream);
 /* Depthwise 3x3, stride 1, zero padding = dil: y[b,y,x,c] = sum_{i,j} w[c][i][j] x[b, y + (i-1) dil, x + (j-1) dil, c]
  * (fp32 FMA).  w: [C][3][3]. */
 int evk_dwconv3x3_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, float* y, int32_t y_pitch,
@@ -604,28 +586,31 @@ int evk_lstm_bidir_fwd(const float* g, int64_t g_st, int64_t g_sn, const float* 
 int evk_rope_attn_fwd(const float* qkvg, int32_t ld, const float* cs, float* o, int32_t ldo, int32_t H, int32_t L,
                       int32_t n_outer, int64_t s_outer, int32_t n_inner, int64_t s_inner, int64_t s_tok, evk_stream_t stream);
 /* Inverse of evk_stft_fwd's center=True transform with the periodic Hann(n_fft) window: torch.istft(n_fft, hop, n_fft, hann,
- * center=True, normalized=False, onesided=True, length=None) of cplx [B*S*T][n_fft/2+1][2] (rows b*S + s), times mask when
- * given (bs_roformer.py:530-543): bin k of row (b, s), frame t is multiplied by the complex mask at columns
+ * center=True, normalized=False, onesided=True, length=length or None) of cplx [B*S*T][n_fft/2+1][2] (rows b*S + s), times
+ * mask when given (bs_roformer.py:530-543): bin k of row (b, s), frame t is multiplied by the complex mask at columns
  * 2 (k S + s) .. +1 of mask row b*T + t (pitch ld_mask: the mask estimator's 'b t (f s c)' layout).  Per frame a C2R inverse
  * DFT (imaginary parts of bins 0 and n_fft/2 ignored) and the window, written to work [B*S*T][n_fft]; then the overlap-add in
  * frame order, divided by the sum of squared windows, trimmed by n_fft/2 at both ends: out [B*S][ld_out] gets hop*(T-1)
- * samples per row.  n_fft a power of two in [256, 8192], or an even divisor of 61440 (2^12 3 5) in [16, 7680] (the
- * mixed-radix core: the UVR5 VR band sizes 320, 640, 960); T >= 2, hop <= n_fft / 2, B*S <= 65535. */
+ * samples per row when length == 0, else torch.istft's length=length: `length` samples per row, computed by the same
+ * overlap-add (past hop*(T-1) from the frames' tails), 0 < length < hop*(T-1) + n_fft/2; a negative length is EVK_ERR_ARG.
+ * n_fft a power of two in [256, 8192], or an even divisor of 61440 (2^12 3 5) in [16, 7680] (the mixed-radix core: the
+ * UVR5 VR band sizes 320, 640, 960); T >= 2, hop <= n_fft / 2, B*S <= 65535. */
 int evk_istft(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft, int32_t hop,
-              float* work, float* out, int32_t ld_out, evk_stream_t stream);
-/* Band-split operand (bs_roformer.py:481-490 and each band's RMSNorm before its Linear): from evk_stft_fwd's cplx
- * [B*S*T][n_bins][2] (rows b*S + s) to y [B*T][ld_y], row (b, t), column (f S + s) * 2 + c ('b t (f s c)'), with the columns
- * [2 S band_off[i], 2 S band_off[i+1]) of band i divided by max(their L2 norm, 1e-12).  band_off: device int32
- * [n_bands + 1] bin offsets (band_off[n_bands] = n_bins).  S = 1 or 2; 2 S n_bins floats must fit 48 KB. */
-int evk_bs_band_input(const float* cplx, int32_t B, int32_t S, int32_t T, int32_t n_bins, const int32_t* band_off,
-                      int32_t n_bands, float* y, int32_t ldy, evk_stream_t stream);
-/* y[r] = x[r] / max(||x[r]||_2, 1e-12) per row (F.normalize(dim=-1): the RMSNorms, whose gamma * sqrt(dim) the caller folds
- * into the next Linear's weight columns). */
-int evk_row_l2norm(const float* x, int32_t ldx, float* y, int32_t ldy, int64_t rows, int32_t C, evk_stream_t stream);
-/* evk_istft with torch.istft's length=length: out gets `length` samples per row, computed by the same overlap-add (past
- * hop*(T-1) from the frames' tails); 0 < length < hop*(T-1) + n_fft/2. */
-int evk_istft_length(const float* cplx, const float* mask, int32_t ld_mask, int32_t B, int32_t S, int32_t T, int32_t n_fft,
-                     int32_t hop, int32_t length, float* work, float* out, int32_t ld_out, evk_stream_t stream);
+              int32_t length, float* work, float* out, int32_t ld_out, evk_stream_t stream);
+/* Band-split operand (bs_roformer.py:481-490, mel_band_roformer.py:419-425, and each band's RMSNorm before its Linear):
+ * from evk_stft_fwd's cplx [B*S*T][n_bins][2] (rows b*S + s) to y [B*T][ld_y], row (b, t), column (j S + s) * 2 + c for
+ * slot j of the bin table (bin bins[j]; 'b t (f s c)'), with the columns [2 S band_off[i], 2 S band_off[i+1]) of band i
+ * divided by max(their L2 norm, 1e-12).  band_off: device int32 [n_bands + 1]; bins: device int32 [band_off[n_bands]], each
+ * < n_bins (BS-Roformer: the identity table 0 .. n_bins-1).  S = 1 or 2; 2 S n_bins floats must fit 48 KB;
+ * ld_y >= 2 S band_off[n_bands]. */
+int evk_band_input(const float* cplx, int32_t B, int32_t S, int32_t T, int32_t n_bins, const int32_t* band_off,
+                   const int32_t* bins, int32_t n_bands, float* y, int32_t ldy, evk_stream_t stream);
+/* y[r] = x[r] / max(||x[r]||_2, 1e-12) per row when gamma == NULL (F.normalize(dim=-1): the RMSNorms whose gamma * sqrt(dim)
+ * the caller folds into the next Linear's weight columns), else that times sqrt(C) * gamma (RMSNorm with its gamma, the
+ * output norm of each Mel-Band Roformer Transformer; in fp32 in that order; gamma: device [C]).  y may be x (in place,
+ * ldy == ldx). */
+int evk_row_norm(const float* x, int32_t ldx, const float* gamma, float* y, int32_t ldy, int64_t rows, int32_t C,
+                 evk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * UVR5 MDX23C (the TFC-TDF v3 U-Net, mdx23c.py; lib_v5/vr_network/tfc_tdf_v3.py), mdx23c.cu, inference only.  Activations are
@@ -661,26 +646,15 @@ int evk_mdx_add(const float* a, int32_t lda, const float* b, int32_t ldb, const 
                 int64_t P, int32_t C, evk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * Mel-Band Roformer (mel_band_roformer.py; lib_v5/vr_network/mel_band_roformer.py:244-478), mel_roformer.cu.  The bands
+ * Mel-Band Roformer (mel_band_roformer.py; lib_v5/vr_network/mel_band_roformer.py:244-478), roformer.cu.  The bands
  * overlap: band i holds the bins bins[band_off[i] .. band_off[i+1]) (ascending), and a bin may belong to two bands.
  * ------------------------------------------------------------------------------------------ */
-/* Band-split operand (mel_band_roformer.py:419-425 and each band's RMSNorm before its Linear): from evk_stft_fwd's cplx
- * [B*S*T][n_bins][2] (rows b*S + s) to y [B*T][ld_y], row (b, t), column (j S + s) * 2 + c for slot j of the bin table
- * (bin bins[j]), with the columns [2 S band_off[i], 2 S band_off[i+1]) of band i divided by max(their L2 norm, 1e-12).
- * band_off: device int32 [n_bands + 1]; bins: device int32 [band_off[n_bands]], each < n_bins.  S = 1 or 2; 2 S n_bins
- * floats must fit 48 KB; ld_y >= 2 S band_off[n_bands]. */
-int evk_melband_input(const float* cplx, int32_t B, int32_t S, int32_t T, int32_t n_bins, const int32_t* band_off,
-                      const int32_t* bins, int32_t n_bands, float* y, int32_t ldy, evk_stream_t stream);
 /* Averaged mask (mel_band_roformer.py:455-466): g [rows][ldg] holds the mask estimators' complex outputs in the band-split
- * column order of evk_melband_input.  mask [rows][ld_mask] at columns 2 (f S + s) .. +1 (evk_istft's mask layout) gets the
+ * column order of evk_band_input.  mask [rows][ld_mask] at columns 2 (f S + s) .. +1 (evk_istft's mask layout) gets the
  * sum over k in [cover_off[f], cover_off[f+1]) of g's complex pair (cover[k] S + s), summed in that order, divided by the
  * count cover_off[f+1] - cover_off[f] (>= 1).  cover lists the slots of bin f in ascending band order.  No atomics. */
 int evk_melband_mask_avg(const float* g, int32_t ldg, const int32_t* cover_off, const int32_t* cover, int32_t S, int32_t n_bins,
                          int64_t rows, float* mask, int32_t ld_mask, evk_stream_t stream);
-/* y[r] = x[r] / max(||x[r]||_2, 1e-12) * sqrt(C) * gamma per row (RMSNorm with its gamma, the output norm of each
- * Transformer; in fp32 in that order).  gamma: device [C].  y may be x (in place, ldy == ldx). */
-int evk_row_rmsnorm(const float* x, int32_t ldx, const float* gamma, float* y, int32_t ldy, int64_t rows, int32_t C,
-                    evk_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * UVR5 VR front and back end (SeparateVR.separate, uvr5/separate.py:103-196; spec_utils.py), vr_wave.cu.  Frame sizes are
@@ -762,14 +736,15 @@ int evk_fragment_int16(const float* x, const int64_t* frags, const int64_t* dst,
  * Whisper transcription (whisper.py, asr.py), inference only: csrc/whisper.cu.  Token, position and counter arguments
  * named *_dev / pos / gstep are int32 device scalars, so the decode step replays as a CUDA graph.
  * ------------------------------------------------------------------------------------------ */
-/* Whisper's log-mel features of B clips of 16 kHz samples: row b of wav [B][ld_wav] holds lens[b] (int32 device, 201 <= lens[b]
- * <= 480000) samples.  out [B][3000][n_mels]: frame t < lens[b] / 160 of row b is the 400-point periodic-Hann STFT (hop 160,
- * centre reflect padding) as a direct DFT against basis = [400][201] window * cos | [400][201] -window * sin, |X|^2 @ fb
- * ([201][n_mels]), log10(max(., 1e-10)), then max(x, clip max - 8) and (x + 4) / 4 with the max over the clip's own frames;
- * frames from lens[b] / 160 on are 0 (padding in the feature domain).  fp32 FMAs in a fixed order: the same bits alone or in
- * any batch.  n_mels <= 256, B <= 65535. */
-int evk_whisper_logmel(const float* wav, int64_t ld_wav, const int32_t* lens, int32_t B, const float* basis, const float* fb,
-                       int32_t n_mels, float* out, evk_stream_t stream);
+/* Whisper's log-mel features of B whole clips of 16 kHz samples: row b of wav [B][ld_wav] holds lens[b] (int32 device,
+ * lens[b] >= 201, lens[b] / 160 <= T) samples.  out [B][T][n_mels]: frame t < lens[b] / 160 of row b is the 400-point
+ * periodic-Hann STFT (hop 160, centre reflect padding) as a direct DFT against basis = [400][201] window * cos | [400][201]
+ * -window * sin, |X|^2 @ fb ([201][n_mels]), log10(max(., 1e-10)), then max(x, clip max - 8) and (x + 4) / 4 with the max
+ * over all of the clip's own frames; frames from lens[b] / 160 to T are 0 (padding in the feature domain).  The max is taken
+ * per 256 frames into part [B][ceil(T / 256)] and folded in chunk order.  fp32 FMAs in a fixed order: the same bits alone or
+ * in any batch, and for any T.  T = 3000 gives the 30 s input of the encoder.  n_mels <= 256, B <= 65535. */
+int evk_whisper_logmel(const float* wav, int64_t ld_wav, const int32_t* lens, int32_t B, int32_t T, const float* basis,
+                       const float* fb, int32_t n_mels, float* part, float* out, evk_stream_t stream);
 /* x[r] = emb[tok[r]] + pe[*pos] for r < R (rows of d floats, contiguous). */
 int evk_whisper_embed(const int32_t* tok, const float* emb, const float* pe, const int32_t* pos, int32_t R, int32_t d, float* x,
                       evk_stream_t stream);
@@ -809,33 +784,19 @@ int evk_whisper_first_pass(const float* logits, int64_t ld, int32_t R, int32_t V
  * and unsat[clip] becomes 0 when the running beams can no longer beat it; a clip with unsat == 0 is not touched.  hist
  * [rows][ld_hist] (generated tokens) and tab [rows][ld_tab] (slot tables, entries <= plen - 1 + g) of the new rows are
  * gathered from their parents.  The caller advances *gstep.  Everything stays in device memory.  ld_hist, ld_tab <= 448,
- * maxlen - plen <= ld_hist, maxlen <= ld_tab, V <= 262144. */
+ * maxlen - plen <= ld_hist, maxlen <= ld_tab, V <= 262144.
+ * row_lse, run_lse, fin_lse: all null, or all given (anything else is EVK_ERR_ARG) to follow each hypothesis' log-sum-exp of
+ * its processed rows: row_lse [rows] (scratch) gets the log-sum-exp of each row's processed log-probs, run_lse [rows] of the
+ * new rows is their parent's run_lse + row_lse, and fin_lse [clips][beam] moves with the finished set as fin_score does.  For
+ * a finished hypothesis of L tokens, fin_score - fin_lse / L (length_penalty 1) is transformers' long-form avg_logprob: the
+ * mean of log_softmax(processed row)[token].  The caller zeroes run_lse and fin_lse before the first step.  Tokens and
+ * scores do not depend on whether they are given. */
 int evk_whisper_beam_step(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot, int32_t nots,
                           int32_t tsb, int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup, int32_t n_sup,
                           const int32_t* bsup, int32_t n_bsup, const int32_t* gstep, float length_penalty, float* cand_val,
                           int32_t* cand_tok, float* run_score, int32_t* hist, int32_t ld_hist, int32_t* tab, int32_t ld_tab,
                           int32_t* tok, int32_t* parent, float* fin_score, int32_t* fin_seq, int32_t* fin_len, int32_t* fin_flag,
-                          int32_t* unsat, evk_stream_t stream);
-/* evk_whisper_beam_step that also follows each hypothesis' log-sum-exp of its processed rows: row_lse [rows] (scratch) gets
- * the log-sum-exp of each row's processed log-probs, run_lse [rows] of the new rows is their parent's run_lse + row_lse,
- * and fin_lse [clips][beam] moves with the finished set as fin_score does.  For a finished hypothesis of L tokens,
- * fin_score - fin_lse / L (length_penalty 1) is transformers' long-form avg_logprob: the mean of log_softmax(processed
- * row)[token].  The caller zeroes run_lse and fin_lse before the first step.  Tokens and scores are those of
- * evk_whisper_beam_step. */
-int evk_whisper_beam_step_lse(const float* logits, int64_t ld, int32_t clips, int32_t beam, int32_t V, int32_t eot, int32_t nots,
-                              int32_t tsb, int32_t mit, int32_t plen, int32_t maxlen, const int32_t* sup, int32_t n_sup,
-                              const int32_t* bsup, int32_t n_bsup, const int32_t* gstep, float length_penalty, float* cand_val,
-                              int32_t* cand_tok, float* run_score, int32_t* hist, int32_t ld_hist, int32_t* tab, int32_t ld_tab,
-                              int32_t* tok, int32_t* parent, float* fin_score, int32_t* fin_seq, int32_t* fin_len,
-                              int32_t* fin_flag, int32_t* unsat, float* row_lse, float* run_lse, float* fin_lse,
-                              evk_stream_t stream);
-/* evk_whisper_logmel over whole clips of any length: out [B][T][n_mels], frame t < lens[b] / 160 of row b as
- * evk_whisper_logmel computes it (the same code), clamped at the max over all of the clip's frames - 8 and scaled; frames
- * from lens[b] / 160 to T are 0.  The max is taken per 256 frames into part [B][ceil(T / 256)] and folded in chunk order, so
- * a clip's bits do not depend on the batch, and a clip of at most 3000 frames gets the bits of evk_whisper_logmel.
- * lens[b] / 160 <= T, B <= 65535. */
-int evk_whisper_logmel_long(const float* wav, int64_t ld_wav, const int32_t* lens, int32_t B, int32_t T, const float* basis,
-                            const float* fb, int32_t n_mels, float* part, float* out, evk_stream_t stream);
+                          int32_t* unsat, float* row_lse, float* run_lse, float* fin_lse, evk_stream_t stream);
 /* 30 s windows of whole-clip log-mels lm [B][T][n_mels]: output row r < R of out [R][3000][n_mels] is frames
  * [seek, seek + n) of clip row `clip`, zero from n on, with (clip, seek, n) = tab[r][0..2] (int32 device, clip < B,
  * 0 <= seek, n <= 3000).  Frames at or past T read as 0.  n = 0 gives a zero row. */

@@ -162,30 +162,31 @@ def test_istft_output_pitch_and_round_trip(ops):
 
 # ---- band input, row norm, GELU epilogue ------------------------------------------------------------------------------
 @pytest.mark.parametrize("S", [1, 2])
-def test_band_input_vs_float64(ops, S):
+def test_band_input_identity_table_vs_float64(ops, S):
     bands = O.SHIPPED["freqs_per_bands"]
     B, L = 2, 20000
     wav = torch.randn(B * S, L, generator=torch.Generator().manual_seed(S)).to(DEV)
     cplx = ops.stft(wav, 2048, 441)
     T, NB = cplx.shape[1], 1025
     off = torch.tensor(np.concatenate([[0], np.cumsum(bands)]), dtype=torch.int32).to(DEV)
+    bins = torch.arange(NB, dtype=torch.int32, device=DEV)                  # BS-Roformer's identity bin table
     out = torch.full((B * T, 2 * S * NB + 4), 7.0, device=DEV)
-    ops.bs_band_input(cplx, B, S, off, out[:, :2 * S * NB])
+    ops.band_input(cplx, B, S, off, bins, out[:, :2 * S * NB])
     again = out.clone()
-    ops.bs_band_input(cplx, B, S, off, again[:, :2 * S * NB])
+    ops.band_input(cplx, B, S, off, bins, again[:, :2 * S * NB])
     assert torch.equal(out, again) and (out[:, 2 * S * NB:] == 7).all()
     x = cplx.double().cpu().reshape(B, S, T, NB, 2).permute(0, 2, 3, 1, 4).reshape(B * T, -1)
     ref = torch.cat([F.normalize(p, dim=-1) for p in x.split([2 * S * f for f in bands], -1)], -1)
     assert rel(out[:, :2 * S * NB], ref) <= 1e-6
 
 
-def test_row_l2norm_vs_float64(ops):
+def test_row_norm_without_gamma_vs_float64(ops):
     x = torch.randn(1000, 520, generator=torch.Generator().manual_seed(4)).to(DEV)
     x[3] = 0
     out = torch.full((1000, 516), 7.0, device=DEV)
-    ops.row_l2norm(x[:, :512], out=out[:, :512])
+    ops.row_norm(x[:, :512], out=out[:, :512])
     again = torch.full_like(out, 7.0)
-    ops.row_l2norm(x[:, :512], out=again[:, :512])
+    ops.row_norm(x[:, :512], out=again[:, :512])
     assert torch.equal(out, again)                                  # bit-reproducible
     assert (out[:, 512:] == 7).all() and (out[3, :512] == 0).all()
     assert rel(out[:, :512], F.normalize(x[:, :512].double(), dim=-1)) <= 1e-6

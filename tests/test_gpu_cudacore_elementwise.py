@@ -569,7 +569,7 @@ CE_ROWS = [1, 7, 9, 333, 5000]                                       # 1 .. 5000
 
 
 @pytest.mark.parametrize("rows", CE_ROWS)
-def test_ce(ops, rows):
+def test_ce_uncounted(ops, rows):
     """V = 1025 classes in rows of ld = 1028 (NaN padding), logits x 30 (lse needs the max subtracted).  The top-k hit rule:
     a valid row is a hit when FEWER THAN k logits are strictly above the target's.  Targets sit at the row maximum, second
     (inside the top 3), fourth (just outside) and at the ignore index 1024."""
@@ -588,9 +588,9 @@ def test_ce(ops, rows):
         lse, nll = torch.full((rows,), NAN, device=DEV), torch.full((rows,), NAN, device=DEV)
         flags = torch.full((rows,), 255, dtype=torch.uint8, device=DEV)
         out2 = torch.full((2,), NAN, device=DEV)
-        ops._call("evk_ce_fwd", P(lgd), ld, P(tgd), rows, V, k, ignore, P(lse), P(nll), P(flags), P(out2))
+        ops._call("evk_ce_fwd", P(lgd), ld, P(tgd), rows, V, k, ignore, None, 1, P(lse), P(nll), P(flags), P(out2))
         dl = output(rows, V, ld)
-        ops._call("evk_ce_bwd", P(lgd), ld, P(tgd), P(lse), P(gs.to(DEV)), rpg, P(dl), ld, rows, V)
+        ops._call("evk_ce_bwd", P(lgd), ld, P(tgd), P(lse), P(gs.to(DEV)), rpg, None, 1, P(dl), ld, rows, V)
         return [lse.cpu(), nll.cpu(), flags.cpu(), out2.cpu(), body(dl, V, "ce_bwd dlogits")]
 
     lse, nll, flags, out2, dl = twice(run)
@@ -614,7 +614,7 @@ def test_ce(ops, rows):
     check(dl, R.E(gsr) * (p - R.E(onehot)), f"ce_bwd rows={rows} rows_per_g={rpg}")
 
 
-def test_ce_topk_tie_rule(ops):
+def test_ce_uncounted_topk_tie_rule(ops):
     """An exact tie at the k-th place.  The kernel's rule -- hit when fewer than k logits are strictly above the target --
     does not depend on how ties are broken: a target tied for 3rd place is a hit.  The reference's MulticlassAccuracy(
     top_k=3) takes torch.topk's 3 indices, so on such a tie it counts a hit only when topk happens to pick the target;
@@ -626,7 +626,7 @@ def test_ce_topk_tie_rule(ops):
     lgd, tgd = lg.to(DEV), tgt.to(DEV)
     lse, nll = torch.empty(6, device=DEV), torch.empty(6, device=DEV)
     flags, out2 = torch.empty(6, dtype=torch.uint8, device=DEV), torch.empty(2, device=DEV)
-    ops._call("evk_ce_fwd", P(lgd), V, P(tgd), 6, V, k, 1024, P(lse), P(nll), P(flags), P(out2))
+    ops._call("evk_ce_fwd", P(lgd), V, P(tgd), 6, V, k, 1024, None, 1, P(lse), P(nll), P(flags), P(out2))
     hit = (flags.cpu() >> 1) & 1
     assert hit.tolist() == [1, 1, 1, 1, 1, 0]                        # all three tied targets are hits
     ref_hit = (lg.topk(k, -1).indices == tgt[:, None]).any(-1)       # MulticlassAccuracy(top_k=3)'s test, per row
@@ -634,7 +634,7 @@ def test_ce_topk_tie_rule(ops):
     assert int(ref_hit[2:5].sum()) == 1                              # topk keeps one of the three tied columns
 
 
-def test_dpo_head(ops):
+def test_dpo_head_uncounted(ops):
     """z = -beta (A - R) of both signs and |z| >= 20 (both softplus branches, sigmoid saturated); sums of 300 / 280 tokens
     through a 256-thread block_sum."""
     B, Yc, Yr, beta = 4, 300, 280, 0.2
@@ -646,7 +646,7 @@ def test_dpo_head(ops):
 
     def run():
         out3, cc, cr = torch.full((3,), NAN, device=DEV), torch.full((B,), NAN, device=DEV), torch.full((B,), NAN, device=DEV)
-        ops._call("evk_dpo_head", P(nc.to(DEV)), Yc, P(nr.to(DEV)), Yr, B, beta, P(out3), P(cc), P(cr))
+        ops._call("evk_dpo_head", P(nc.to(DEV)), Yc, None, P(nr.to(DEV)), Yr, None, B, beta, P(out3), P(cc), P(cr))
         return [out3.cpu(), cc.cpu(), cr.cpu()]
 
     out3, cc, cr = twice(run)

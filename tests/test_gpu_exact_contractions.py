@@ -6,7 +6,7 @@ predicate, a dropped K block or split, a tap shift into the wrong residue copy o
 changes an output by a whole unit.  A whole-tensor relative-L2 gate cannot see one such output among millions.
 
 Kernels: gemm_tma_kernel (evk_gemm_tf32, the flat Linear path, tap-sum and phased strided convs), conv_wgrad_kernel,
-gconv_tc_kernel, the mma.sync and direct fallbacks, and both kernels of evk_conv2d_fwd[_hw].  Every case asserts from
+gconv_tc_kernel, the mma.sync and direct fallbacks, and both kernels of evk_conv2d_fwd.  Every case asserts from
 the library's dispatch accounting that its flops went to the kernel family it is about.
 """
 import math
@@ -445,7 +445,7 @@ def test_cross_family_bit_identical(ops, exact_mode):
         assert all(torch.equal(results[0], r) for r in results[1:])
 
 
-# ---- evk_conv2d_fwd[_hw] ------------------------------------------------------------------------------------------------
+# ---- evk_conv2d_fwd -----------------------------------------------------------------------------------------------------
 # B, H, W, C, N, k, stride, (dil_h, dil_w), act, (extra input channels, input channel offset), (output offset, extra):
 # every wgmma column-tile boundary, M not a multiple of 128, stride 1 and 2
 CONV2D_N_GRID = [(2, 13, 11, 24, n, 3, 2, (1, 1), a, (4, 0), (0, 3)) for n, a in ((32, 0), (33, 1), (64, 2), (65, 0), (128, 1), (129, 2))]

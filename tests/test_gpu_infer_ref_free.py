@@ -1,5 +1,5 @@
 """GPU tests of prompt-free AR decoding (`pytest -m gpu`): the text-only prompt pass kernels (empty audio part), the sampler's EOS
-window (evk_sample_tokens_ex), Text2SemanticDecoder.infer_panel_naive(prompts=None) and the batched
+window (evk_sample_tokens), Text2SemanticDecoder.infer_panel_naive(prompts=None) and the batched
 infer_panel_naive_batched(prompts=None) against the tokens the reference decoded (tests/golden/infer_ref_free.json) and
 against each other."""
 import json
@@ -185,9 +185,9 @@ class _Sampler:
                                self.alpha, self.x, q=self.q, eos_steps=eos_steps)
         return self.result()
 
-    def plain(self):                                                 # the original entry point, which has no eos_steps
+    def plain(self):                                                 # the entry point called directly with eos_steps = 1
         p = self.ops._p
-        self.ops._call("evk_sample_tokens", p(self.logits), self.logits.stride(0), self.logits.shape[0], V, EOS, p(self.icfg),
+        self.ops._call("evk_sample_tokens", p(self.logits), self.logits.stride(0), self.logits.shape[0], V, EOS, 1, p(self.icfg),
                        p(self.fcfg), p(self.n), p(self.q), self.q.stride(0), p(self.hist), self.hist.stride(0), p(self.seen),
                        p(self.fin), p(self.emb), p(self.pe), p(self.alpha), p(self.x), D)
         return self.result()
@@ -197,7 +197,7 @@ class _Sampler:
         return self.hist[:, self.step].cpu(), self.fin.cpu(), self.x.cpu()
 
 
-def test_sampler_eos_window(ops):
+def test_sampler_eos_steps_window(ops):
     g = torch.Generator().manual_seed(8)
     B = 8
     logits = torch.randn(B, V, generator=g) * 2.5
@@ -210,7 +210,7 @@ def test_sampler_eos_window(ops):
     assert fin[:4].tolist() == [[11, 10]] * 4 and (fin[4:] == -1).all()
     _, fin, _ = _Sampler(ops, logits, 10, q).ex(1)                   # a 1-step window stops them at step 10 already
     assert fin[:4].tolist() == [[10, 9]] * 4
-    for step in (0, 3):                                              # eos_steps = 1 is evk_sample_tokens
+    for step in (0, 3):                                              # eos_steps = 1 is the batched decoders' call
         a, b = _Sampler(ops, logits, step, q).ex(1), _Sampler(ops, logits, step, q).plain()
         assert all(torch.equal(u, v) for u, v in zip(a, b)), step
     with pytest.raises(ValueError, match="eos_steps"):

@@ -1,6 +1,6 @@
-"""GPU tests of the Mel-Band Roformer separator (`pytest -m gpu`): the overlapping band input (evk_melband_input), the averaged
-masks (evk_melband_mask_avg) and the RMSNorm with gamma (evk_row_rmsnorm) element for element against float64 with the
-per-element bounds of tests/cudacore_ref.py, the inverse STFT with an output length (evk_istft_length) against torch.istft,
+"""GPU tests of the Mel-Band Roformer separator (`pytest -m gpu`): the overlapping band input (evk_band_input), the averaged
+masks (evk_melband_mask_avg) and the RMSNorm with gamma (evk_row_norm) element for element against float64 with the
+per-element bounds of tests/cudacore_ref.py, the inverse STFT with an output length (evk_istft) against torch.istft,
 and MelBandRoformer.forward / bs_roformer.demix_track against the outputs the reference computed (tests/golden/mel_roformer.pt,
 pinned by oracle/pin_mel_roformer.py)."""
 import os
@@ -98,7 +98,7 @@ def E_max(a, floor):
 # ---- band input, averaged masks, RMSNorm with gamma ---------------------------------------------------------------------
 @pytest.mark.parametrize("S", [1, 2])
 @pytest.mark.parametrize("sr,n_fft,nb,hop", [(44100, 2048, 60, 441), (48000, 1024, 24, 256)])
-def test_melband_input_elementwise(ops, M, S, sr, n_fft, nb, hop):
+def test_band_input_elementwise(ops, M, S, sr, n_fft, nb, hop):
     bins, band_off, _, _ = M.band_tables(sr, n_fft, nb)
     B, L = 2, 12 * hop + 5
     wav = torch.randn(B * S, L, generator=torch.Generator().manual_seed(S + nb)).to(DEV)
@@ -108,7 +108,7 @@ def test_melband_input_elementwise(ops, M, S, sr, n_fft, nb, hop):
     outs = []
     for _ in range(2):
         out = torch.full((B * T, W + 6), SENTINEL, device=DEV)
-        ops.melband_input(cplx, B, S, doff, dbins, out[:, :W])
+        ops.band_input(cplx, B, S, doff, dbins, out[:, :W])
         outs.append(out.cpu())
     assert torch.equal(outs[0], outs[1]) and (outs[0][:, W:] == SENTINEL).all()
     # float64: the same gather ('b t (f s c)' over the bin table), each band's segment normalised
@@ -117,7 +117,7 @@ def test_melband_input_elementwise(ops, M, S, sr, n_fft, nb, hop):
     got = outs[0][:, :W]
     for i in range(nb):
         c0, c1 = 2 * S * band_off[i], 2 * S * band_off[i + 1]
-        check(got[:, c0:c1], l2norm_rows(R.E(x[:, c0:c1])), f"melband_input band {i} S={S} n_fft={n_fft}")
+        check(got[:, c0:c1], l2norm_rows(R.E(x[:, c0:c1])), f"band_input band {i} S={S} n_fft={n_fft}")
 
 
 @pytest.mark.parametrize("S", [1, 2])
@@ -151,7 +151,7 @@ def test_melband_mask_avg_elementwise(ops, M, S, sr, n_fft, nb):
 
 
 @pytest.mark.parametrize("rows,C,ld", [(1000, 384, 388), (37, 128, 128), (9, 66, 70)])
-def test_row_rmsnorm_elementwise(ops, rows, C, ld):
+def test_row_norm_gamma_elementwise(ops, rows, C, ld):
     gen = torch.Generator().manual_seed(rows + C)
     x = torch.randn(rows, C, generator=gen) * 3.0
     x[3] = 0.0
@@ -162,16 +162,16 @@ def test_row_rmsnorm_elementwise(ops, rows, C, ld):
         xd[:, :C] = x
         xd = xd.to(DEV)
         out = torch.full((rows, ld), SENTINEL, device=DEV)
-        ops.row_rmsnorm(xd[:, :C], gamma.to(DEV), out=out[:, :C])
+        ops.row_norm(xd[:, :C], gamma.to(DEV), out=out[:, :C])
         inplace = xd.clone()
-        ops.row_rmsnorm(inplace[:, :C], gamma.to(DEV), out=inplace[:, :C])
+        ops.row_norm(inplace[:, :C], gamma.to(DEV), out=inplace[:, :C])
         outs.append(out.cpu())
         assert torch.equal(inplace[:, :C].cpu(), out[:, :C].cpu())                  # in place gives the same bits
     assert torch.equal(outs[0], outs[1]) and (outs[0][:, C:] == SENTINEL).all()
     assert (outs[0][3, :C] == 0).all()
     scale = float(np.float32(C ** 0.5))
     ref = l2norm_rows(R.E(x.double())) * scale * R.E(gamma.double())
-    check(outs[0][:, :C], ref, f"row_rmsnorm rows={rows} C={C}")
+    check(outs[0][:, :C], ref, f"row_norm gamma rows={rows} C={C}")
 
 
 @pytest.mark.parametrize("n_fft,hop,S,extra", [(2048, 441, 2, 440), (1024, 441, 1, 17), (1024, 256, 1, 0), (256, 100, 2, 99)])
@@ -187,12 +187,12 @@ def test_istft_length_vs_torch(ops, n_fft, hop, S, extra):
     ops.istft(cplx, B, S, n_fft, hop, mask=mask, out=out[:, :L], length=L)
     assert (out[:, L:] == SENTINEL).all()
     short = ops.istft(cplx, B, S, n_fft, hop, mask=mask)
-    assert torch.equal(short, out[:, :hop * (T - 1)])                 # the first hop*(T-1) samples are evk_istft's
+    assert torch.equal(short, out[:, :hop * (T - 1)])                 # the first hop*(T-1) samples are those of length 0
     X = torch.view_as_complex(cplx.double().cpu().contiguous())
     m = torch.view_as_complex(mask.double().cpu().reshape(B, T, NB, S, 2).contiguous()).permute(0, 3, 1, 2).reshape(B * S, T, NB)
     ref = torch.istft((X * m).transpose(1, 2), n_fft, hop, n_fft, torch.hann_window(n_fft, dtype=torch.float64), length=L)
     e = rel(out[:, :L], ref)
-    print(f"istft_length n_fft={n_fft} hop={hop} S={S} L={L} rel-L2 {e:.3g}")
+    print(f"istft length n_fft={n_fft} hop={hop} S={S} L={L} rel-L2 {e:.3g}")
     assert e <= 2e-6, e
 
 

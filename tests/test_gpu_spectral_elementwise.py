@@ -330,7 +330,7 @@ ISTFT_CASES = [(2048, 441), (256, 64), (320, 80), (640, 160), (960, 240)]
 
 @pytest.mark.parametrize("masked", [False, True])
 @pytest.mark.parametrize("N,hop", ISTFT_CASES, ids=[f"N{a}-hop{b}" for a, b in ISTFT_CASES])
-def test_istft(ops, N, hop, masked):
+def test_istft_untrimmed(ops, N, hop, masked):
     """B = 2, S = 2, T = 12 frames: rows r = b S + s; the mask in the estimator's (b t (f s c)) layout, pitch 2 S NB + 2"""
     B, S_, T, NB = 2, 2, 12, N // 2 + 1
     g = _gen(N + masked)
@@ -344,7 +344,8 @@ def test_istft(ops, N, hop, masked):
 
     def run():
         out = output(B * S_, Lout, Lout + 3)
-        ops._call("evk_istft", P(Xd), P(md) if masked else None, ldm if masked else 0, B, S_, T, N, hop, P(work), P(out), Lout + 3)
+        ops._call("evk_istft", P(Xd), P(md) if masked else None, ldm if masked else 0, B, S_, T, N, hop, 0, P(work), P(out),
+                  Lout + 3)
         return [body(out, Lout, "istft out")]
 
     (got,) = twice(run)

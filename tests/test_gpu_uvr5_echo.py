@@ -1,5 +1,5 @@
 """GPU tests of the UVR5 DeEcho / DeReverb separator (`pytest -m gpu`): the anisotropic 2-D convolution
-(evk_conv2d_fwd_hw) and the bidirectional LSTM recurrence (evk_lstm_bidir_fwd) against float64, their reproducibility and
+(evk_conv2d_fwd) and the bidirectional LSTM recurrence (evk_lstm_bidir_fwd) against float64, their reproducibility and
 batch independence, and CascadedNet.predict / uvr5.inference against the outputs the reference computed
 (tests/golden/uvr5_deecho.pt, pinned by oracle/pin_uvr5_echo.py)."""
 import os

@@ -30,7 +30,7 @@ host back end; and, in a separate profiled call, the device time of the new fron
 The parameter sets are read from tests/golden/uvr5_wave.pt.
 
 --net melroformer measures the Mel-Band Roformer (mel_band_roformer.py, the widely distributed vocal model's configuration
-with seeded weights) the same way on the same mix, with the two new kernel families (evk_melband_input,
+with seeded weights) the same way on the same mix, with the overlapping-band kernel families (evk_band_input,
 evk_melband_mask_avg) split out of the device time, and oracle/mel_roformer_oracle.py's forward as the stock PyTorch arms.
 It skips the rope_attn rates, whose shapes are the BS-Roformer's.
 
@@ -254,7 +254,7 @@ def rope_attn_rates(ops, reps=20):
 
 
 FAMILIES = (("gemm", ("evk_gconv_fwd",)), ("attention", ("evk_rope_attn_fwd",)),
-            ("norms", ("evk_row_l2norm", "evk_bs_band_input")), ("stft_istft", ("evk_stft_fwd", "evk_istft")))
+            ("norms", ("evk_row_norm", "evk_band_input")), ("stft_istft", ("evk_stft_fwd", "evk_istft")))
 
 
 def torch_roformer_demix(P, cfg, mix, half, autocast, forward=BR.forward):
@@ -272,9 +272,9 @@ def torch_roformer_demix(P, cfg, mix, half, autocast, forward=BR.forward):
     return BR.demix_track(net, mix)["vocals"]
 
 
-MEL_FAMILIES = (("gemm", ("evk_gconv_fwd",)), ("attention", ("evk_rope_attn_fwd",)), ("norms", ("evk_row_l2norm", "evk_row_rmsnorm")),
-                ("melband_input", ("evk_melband_input",)), ("melband_mask_avg", ("evk_melband_mask_avg",)),
-                ("stft_istft", ("evk_stft_fwd", "evk_istft", "evk_istft_length")))
+MEL_FAMILIES = (("gemm", ("evk_gconv_fwd",)), ("attention", ("evk_rope_attn_fwd",)), ("norms", ("evk_row_norm",)),
+                ("band_input", ("evk_band_input",)), ("melband_mask_avg", ("evk_melband_mask_avg",)),
+                ("stft_istft", ("evk_stft_fwd", "evk_istft")))
 
 
 def roformer_main(a):
