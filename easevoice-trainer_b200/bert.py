@@ -157,7 +157,7 @@ class BertModel(ParamTree):
         return ids, tt, lens
 
     def _qkv(self, i):
-        """Q, K and V of layer i as one Linear: the three weights concatenated and packed once per parameter version."""
+        """Q, K and V of layer i as one Linear: the three weights concatenated and packed once per weights_key()."""
         key = ("qkv", i)
         if key not in self._active:
             p = f"encoder.layer.{i}.attention.self."
@@ -179,8 +179,7 @@ class BertModel(ParamTree):
         idx = torch.cat([ids.reshape(-1), tt.reshape(-1), pos.reshape(-1), lens]).to(dev)      # one H2D copy
         ids_d, tt_d, pos_d, lens_d = idx[:B * T].view(B, T), idx[B * T:2 * B * T].view(B, T), idx[2 * B * T:3 * B * T].view(B, T), idx[3 * B * T:]
         H, nh, eps = c["hidden_size"], c["num_attention_heads"], c["layer_norm_eps"]
-        self._active, self._memo_pack = self.packed_for_inference(), True
-        try:
+        with self.inference_weights():
             # BertEmbeddings: (word + token type) + position, then LayerNorm
             x = ops.add(ops.embedding(self.P("embeddings.word_embeddings.weight"), ids_d),
                         ops.embedding(self.P("embeddings.token_type_embeddings.weight"), tt_d))
@@ -197,8 +196,6 @@ class BertModel(ParamTree):
                 f = ops.linear(f, self.w(p + "output.dense", need_pb=False), self.b(p + "output.dense"))
                 h = ops.layernorm(h, self.P(p + "output.LayerNorm.weight"), self.P(p + "output.LayerNorm.bias"), res=f, eps=eps)
             return h
-        finally:
-            self._active, self._memo_pack = None, False
 
 
 # ---- phone-level expansion -------------------------------------------------------------------------------------------------

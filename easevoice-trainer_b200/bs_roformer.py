@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from . import lib, ops
+from .weights import check_state_dict, to_device
 
 # SeparateMDXC.get_model_from_config (separate.py:456-490)
 SHIPPED_CONFIG = dict(
@@ -117,21 +118,12 @@ class AxialRoformer:
             # the defaults as stored in the checkpoint's dtype (fp16 checkpoints hold them rounded to half precision)
             if not ok or not torch.allclose(v.float().cpu(), ref, rtol=max(torch.finfo(v.dtype).eps, 1e-5), atol=0):
                 raise ValueError(f"{k}: only the default rotary frequencies (theta 10000) are supported")
-        missing = [k for k in spec if k not in sd]
-        unexpected = [k for k in sd if k not in spec]
-        if missing or unexpected:
-            raise ValueError(f"state_dict does not match {type(self).__name__}: missing {missing[:5]}"
-                             f"{'...' if len(missing) > 5 else ''}, unexpected {unexpected[:5]}{'...' if len(unexpected) > 5 else ''}")
-        for k, shape in spec.items():
-            v = sd[k]
-            if not torch.is_tensor(v) or not v.is_floating_point() or tuple(v.shape) != tuple(shape):
-                raise ValueError(f"{k}: expected a float tensor of shape {tuple(shape)}, got "
-                                 f"{tuple(v.shape) if torch.is_tensor(v) else type(v).__name__}")
+        check_state_dict(sd, spec, type(self).__name__)
         folded = self._fold({k: sd[k].detach().cpu().to(torch.float32) for k in spec})
         # unpacked weights stay on the host (each precision mode packs its own device copy from them); biases (and any
         # other vectors the forward reads) go to the device
         self.host_w = {k[:-2]: v for k, v in folded.items() if k.endswith(".w")}
-        self.bias = {k: v.to(self.device) for k, v in folded.items() if not k.endswith(".w")}
+        self.bias = to_device({k: v for k, v in folded.items() if not k.endswith(".w")}, self.device)
         self._packed = {}
         return self
 
@@ -175,7 +167,7 @@ class AxialRoformer:
     def to(self, device):
         self.device = torch.device(device)
         if self.bias is not None:
-            self.bias = {k: v.to(self.device) for k, v in self.bias.items()}
+            self.bias = to_device(self.bias, self.device)
         self._packed, self._rope, self._tab = {}, {}, None
         return self
 

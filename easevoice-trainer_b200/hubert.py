@@ -121,7 +121,7 @@ class HubertModel(ParamTree):
         return self.conv_lengths(n_samples)[-1]
 
     def _qkv(self, i):
-        """q_proj, k_proj and v_proj of layer i as one Linear: the weights concatenated and packed once per parameter version."""
+        """q_proj, k_proj and v_proj of layer i as one Linear: the weights concatenated and packed once per weights_key()."""
         key = ("qkv", i)
         if key not in self._active:
             p = f"encoder.layers.{i}.attention."
@@ -133,19 +133,16 @@ class HubertModel(ParamTree):
     POS_PIECE = 48           # taps per launch of the positional conv (the descriptor holds EVK_MAX_TAPS = 48 tap offsets)
 
     def _pos_weight(self):
-        """weight_norm(dim=2) folded once per parameter version: w[:, :, k] = g[k] * v[:, :, k] / ||v[:, :, k]||_F.
+        """weight_norm(dim=2) folded once per weights_key(): w[:, :, k] = g[k] * v[:, :, k] / ||v[:, :, k]||_F.
         The k = 128 kernel is packed as ceil(128 / 48) tap pieces (one launch each, chained through the residual input)."""
-        g = self.P("encoder.pos_conv_embed.conv.parametrizations.weight.original0")
-        v = self.P("encoder.pos_conv_embed.conv.parametrizations.weight.original1")
-        key = (int(g._version), int(v._version), str(v.device))
-        c = self.__dict__.get("_posw")
-        if c is None or c[0] != key:
+        def build():
+            g = self.P("encoder.pos_conv_embed.conv.parametrizations.weight.original0")
+            v = self.P("encoder.pos_conv_embed.conv.parametrizations.weight.original1")
             w = v * (g / v.norm(p=2, dim=(0, 1), keepdim=True))
             K = w.shape[2]
             pieces = [(a, min(K, a + self.POS_PIECE)) for a in range(0, K, self.POS_PIECE)]
-            c = (key, [(a, b, ops.pack_weight(w[:, :, a:b].contiguous(), None, need_pb=False)) for a, b in pieces])
-            self.__dict__["_posw"] = c
-        return c[1]
+            return [(a, b, ops.pack_weight(w[:, :, a:b].contiguous(), None, need_pb=False)) for a, b in pieces]
+        return self.cached("pos_weight", build)
 
     def _pos_conv(self, h):
         """HubertPositionalConvEmbedding (modeling_hubert.py): grouped Conv1d(k = 128, pad = 64) + HubertSamePadLayer (drops the
@@ -181,8 +178,7 @@ class HubertModel(ParamTree):
         idx = torch.tensor([f[0] for f in fl] + [f[-1] for f in fl], dtype=torch.int64).to(dev)      # one H2D copy
         n0_d, nt_d = idx[:B].int(), idx[B:].int()
         nt64_d = idx[B:]
-        self._active, self._memo_pack = self.packed_for_inference(), True
-        try:
+        with self.inference_weights():
             # channels-last [B, L, 1], widened to 4 zero-padded channels (16-byte rows) like the discriminators' waveform input
             x = ops.pad_channels(input_values.float().unsqueeze(-1).contiguous(), 4)
             for i, (k, s) in enumerate(zip(c["conv_kernel"], c["conv_stride"])):
@@ -213,8 +209,6 @@ class HubertModel(ParamTree):
                 f = ops.linear(f, self.w(p + "feed_forward.output_dense", need_pb=False), self.b(p + "feed_forward.output_dense"))
                 h = ops.layernorm(h, self.P(p + "final_layer_norm.weight"), self.P(p + "final_layer_norm.bias"), res=f, eps=eps)
             return {"last_hidden_state": h}
-        finally:
-            self._active, self._memo_pack = None, False
 
 
 class CNHubert(torch.nn.Module):

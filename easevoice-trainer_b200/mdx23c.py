@@ -20,6 +20,7 @@ import torch
 
 from . import ops
 from .ops import CLView
+from .weights import check_state_dict, to_device
 
 # The published 8K-FFT InstVoc HQ configuration, written from memory: no checkpoint or YAML of it was at hand to confirm
 # these values.  from_pretrained overrides everything the weights determine.
@@ -148,32 +149,23 @@ class MDX23C:
         """Strict load of the reference's state_dict (fp16 or fp32): a missing or unexpected key or a wrong shape raises
         ValueError.  Conv weights are stored [N, kh, kw, C], transposed-conv weights [2, 2, N, C]."""
         spec = self.state_dict_shapes()
-        sd = dict(sd)
-        missing = [k for k in spec if k not in sd]
-        unexpected = [k for k in sd if k not in spec]
-        if missing or unexpected:
-            raise ValueError(f"state_dict does not match MDX23C: missing {missing[:5]}{'...' if len(missing) > 5 else ''}, "
-                             f"unexpected {unexpected[:5]}{'...' if len(unexpected) > 5 else ''}")
+        check_state_dict(sd, spec, "MDX23C")
         w = {}
-        for k, shape in spec.items():
-            v = sd[k]
-            if not torch.is_tensor(v) or not v.is_floating_point() or tuple(v.shape) != tuple(shape):
-                raise ValueError(f"{k}: expected a float tensor of shape {tuple(shape)}, got "
-                                 f"{tuple(v.shape) if torch.is_tensor(v) else type(v).__name__}")
-            v = v.detach().cpu().to(torch.float32)
+        for k in spec:
+            v = sd[k].detach().cpu().to(torch.float32)
             if ".upscale.conv.2." in k:
                 v = v.permute(2, 3, 1, 0)
             elif v.dim() == 4:
                 v = v.permute(0, 2, 3, 1)
             w[k] = v.contiguous()
         self.host_w = w
-        self.w = {k: v.to(self.device) for k, v in w.items()}
+        self.w = to_device(w, self.device)
         return self
 
     def to(self, device):
         self.device = torch.device(device)
         if self.w is not None:
-            self.w = {k: v.to(self.device) for k, v in self.host_w.items()}
+            self.w = to_device(self.host_w, self.device)
         return self
 
     def eval(self):

@@ -16,7 +16,7 @@ import os
 import torch
 from torch import nn
 
-from . import ops
+from . import lib, ops
 
 D_LANES = max(1, min(6, int(os.environ.get("EVK_D_LANES", "6"))))   # streams the six discriminators are spread over
 D_PRIO = os.environ.get("EVK_D_PRIO", "0") == "1"                    # DiscriminatorS on a high-priority stream (experiment)
@@ -107,18 +107,40 @@ class ParamTree(nn.Module):
             rec.append((key, v, g, need_pb, pad0, pad1, torch.is_grad_enabled() and not self._frozen))
         pw = ops.pack_weight(fz(v), fz(g) if g is not None else None, need_pb, pad0, pad1)
         if act is not None and getattr(self, "_memo_pack", False):
-            act[key] = pw                      # inference: static weights are packed once and kept (see packed_for_inference)
+            act[key] = pw                      # inference: static weights are packed once and kept (see inference_weights)
         return pw
 
+    def weights_key(self):
+        """What packed operands, and CUDA graphs captured with them, depend on: the parameters' and buffers' version counters,
+        the device, and the precise mode (pack_weight rounds to TF32 unless evk_set_precise(1) is on, and a graph replays the
+        kernels of the mode it was captured in)."""
+        # one walk over the modules: parameters() and buffers() together take two to three times as long
+        ver = sum(t._version for m in self.modules() for t in (*m._parameters.values(), *m._buffers.values()) if t is not None)
+        return ver, str(next(self.parameters()).device), lib.load().evk_get_precise()
+
+    def cached(self, name, build):
+        """build()'s result, kept under `name` until weights_key() changes."""
+        key = self.weights_key()
+        cache = self.__dict__.setdefault("_cached", {})
+        if name not in cache or cache[name][0] != key:
+            cache.pop(name, None)              # free the stale value before its replacement is built
+            cache[name] = (key, build())
+        return cache[name][1]
+
     def packed_for_inference(self):
-        """-> dict used as `self._active` during inference loops: every packed weight is produced on first use and reused until
-        a parameter changes (sum of the parameters' version counters)."""
-        ver = sum(int(p._version) for p in self.parameters()) + sum(int(b._version) for b in self.buffers())
-        cache = self.__dict__.get("_infer_pack")
-        if cache is None or cache[0] != ver:
-            cache = (ver, {})
-            self.__dict__["_infer_pack"] = cache
-        return cache[1]
+        """-> the dict inference_weights() hands to w() as `self._active`: the packed weights made during inference, kept until
+        weights_key() changes."""
+        return self.cached("inference", dict)
+
+    @contextlib.contextmanager
+    def inference_weights(self):
+        """Scope of an inference pass: every packed weight w() makes is kept (packed_for_inference) and handed out again by later
+        passes."""
+        self._active, self._memo_pack = self.packed_for_inference(), True
+        try:
+            yield
+        finally:
+            self._active, self._memo_pack = None, False
 
     def b(self, pfx, pad=0):
         if not self.has(pfx + ".bias"):

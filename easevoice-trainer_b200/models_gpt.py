@@ -275,11 +275,12 @@ class Text2SemanticDecoder(ParamTree):
         """Per-layer caches [B, rows, 3 D] and the static buffers / graphs of the batched token step, kept across calls while the
         parameters, B and the capacity allow.  There are two: one for B = 1, its capacity rounded up to 512 rows so that single
         utterances of varying length rarely rebuild it, and one for B > 1, rounded up to 64 rows (a new B frees the previous one
-        first).  Calls with one row and calls with several therefore do not rebuild each other's state."""
-        ver = sum(int(p._version) for p in self.parameters())
+        first).  Calls with one row and calls with several therefore do not rebuild each other's state.  The graphs hold the
+        packed weights and the precise mode's kernels, so a new weights_key() rebuilds the state."""
+        wkey = self.weights_key()
         key, unit = ("_batch_st1", 512) if B == 1 else ("_batch_st", 64)
         st = self.__dict__.get(key)
-        if st is not None and st["ver"] == ver and st["dev"] == dev and st["B"] == B and st["rows"] >= need_rows:
+        if st is not None and st["wkey"] == wkey and st["dev"] == dev and st["B"] == B and st["rows"] >= need_rows:
             return st
         self.__dict__.pop(key, None)
         rows = (need_rows + unit - 1) // unit * unit
@@ -287,7 +288,7 @@ class Text2SemanticDecoder(ParamTree):
 
         def z(*shape, dtype=torch.float32):
             return torch.zeros(shape, device=dev, dtype=dtype)
-        st = dict(ver=ver, dev=dev, B=B, rows=rows, graphs={},
+        st = dict(wkey=wkey, dev=dev, B=B, rows=rows, graphs={},
                   caches=[torch.empty((B, rows, 3 * D), device=dev, dtype=torch.float32) for _ in range(self.num_layers)],
                   n=z(1, dtype=torch.int32), x=z(B, 1, D), logits=z(B, Vp), skip=z(B, 2, dtype=torch.int32),
                   hist=z(B, rows, dtype=torch.int64), seen=z(B, (V + 31) // 32, dtype=torch.int32), fin=z(B, 2, dtype=torch.int32),
@@ -447,39 +448,38 @@ class Text2SemanticDecoder(ParamTree):
         cap = max_steps if early_stop_num == -1 else min(max_steps, early_stop_num + 1)
         was_training = self.training
         self.eval()
-        self._active, self._memo_pack = self.packed_for_inference(), True
         try:
-            xp = torch.zeros((B, max_len), device=dev, dtype=torch.int64)
-            bp = torch.zeros((B, 1024, max_len), device=dev, dtype=torch.float32)
-            for b in range(B):
-                xp[b, :rows[b].shape[0]] = rows[b]
-                bp[b, :, :rows[b].shape[0]] = bert[b]
-            st = self._batch_state(dev, B, L0 + cap + INFER_BATCH_K)
-            Vp = st["logits"].shape[1]
-            head = self.w("ar_predict_layer", pad0=Vp)
-            graph = self._batch_step_graph(st, head, eos_steps)
-            # prompt pass (process_prompt with the padded mask, :596-646; prompt-free: the text alone, :796-803)
-            y = torch.zeros((B, 0), device=dev, dtype=torch.int64) if prompts is None else prompts.to(torch.int64)
-            xe = self._embed_text(xp, bp, False)
-            ye = ops.embedding(self.P("ar_audio_embedding.word_embeddings.weight"), y)
-            h = ops.gpt_embed(xe, ye, self.P("ar_text_position.alpha"), self.P("ar_audio_position.alpha"), st["pe"])
-            xl = torch.tensor(lens, device=dev, dtype=torch.int64)
-            yl = torch.full((B,), Yp, device=dev, dtype=torch.int64)
-            for i in range(self.num_layers):
-                h = self._infer_layer(i, h, st["caches"][i], None, X=max_len, xl=xl, yl=yl)
-            first = xl - 1 if prompts is None else torch.full((B,), L0 - 1, device=dev, dtype=torch.int64)
-            st["logits"].copy_(ops.linear_rows(ops.slice_rows(h, first, 1), head).view(B, Vp))
-            # per-call state of the step graph
-            st["n"].fill_(L0)
-            st["skip"].copy_(torch.tensor([[v, max_len] for v in lens], dtype=torch.int32))
-            st["hist"][:, :Yp].copy_(y)
-            bits = torch.zeros((B, st["seen"].shape[1] * 32), device=dev, dtype=torch.int64).scatter_(1, y, 1)
-            words = (bits.view(B, -1, 32) << torch.arange(32, device=dev, dtype=torch.int64)).sum(-1)
-            st["seen"].copy_(torch.where(words >= 2 ** 31, words - 2 ** 32, words))      # uint32 bit patterns as int32
-            fin = self._run_batch(st, graph, Yp, L0, max_steps, top_k, early_stop_num, top_p, temperature, repetition_penalty, trace)
-            return [st["hist"][b, :Yp + fin[b][0]].clone() for b in range(B)], fin
+            with self.inference_weights():
+                xp = torch.zeros((B, max_len), device=dev, dtype=torch.int64)
+                bp = torch.zeros((B, 1024, max_len), device=dev, dtype=torch.float32)
+                for b in range(B):
+                    xp[b, :rows[b].shape[0]] = rows[b]
+                    bp[b, :, :rows[b].shape[0]] = bert[b]
+                st = self._batch_state(dev, B, L0 + cap + INFER_BATCH_K)
+                Vp = st["logits"].shape[1]
+                head = self.w("ar_predict_layer", pad0=Vp)
+                graph = self._batch_step_graph(st, head, eos_steps)
+                # prompt pass (process_prompt with the padded mask, :596-646; prompt-free: the text alone, :796-803)
+                y = torch.zeros((B, 0), device=dev, dtype=torch.int64) if prompts is None else prompts.to(torch.int64)
+                xe = self._embed_text(xp, bp, False)
+                ye = ops.embedding(self.P("ar_audio_embedding.word_embeddings.weight"), y)
+                h = ops.gpt_embed(xe, ye, self.P("ar_text_position.alpha"), self.P("ar_audio_position.alpha"), st["pe"])
+                xl = torch.tensor(lens, device=dev, dtype=torch.int64)
+                yl = torch.full((B,), Yp, device=dev, dtype=torch.int64)
+                for i in range(self.num_layers):
+                    h = self._infer_layer(i, h, st["caches"][i], None, X=max_len, xl=xl, yl=yl)
+                first = xl - 1 if prompts is None else torch.full((B,), L0 - 1, device=dev, dtype=torch.int64)
+                st["logits"].copy_(ops.linear_rows(ops.slice_rows(h, first, 1), head).view(B, Vp))
+                # per-call state of the step graph
+                st["n"].fill_(L0)
+                st["skip"].copy_(torch.tensor([[v, max_len] for v in lens], dtype=torch.int32))
+                st["hist"][:, :Yp].copy_(y)
+                bits = torch.zeros((B, st["seen"].shape[1] * 32), device=dev, dtype=torch.int64).scatter_(1, y, 1)
+                words = (bits.view(B, -1, 32) << torch.arange(32, device=dev, dtype=torch.int64)).sum(-1)
+                st["seen"].copy_(torch.where(words >= 2 ** 31, words - 2 ** 32, words))      # uint32 bit patterns as int32
+                fin = self._run_batch(st, graph, Yp, L0, max_steps, top_k, early_stop_num, top_p, temperature, repetition_penalty, trace)
+                return [st["hist"][b, :Yp + fin[b][0]].clone() for b in range(B)], fin
         finally:
-            self._active, self._memo_pack = None, False
             self.train(was_training)
 
 def reject_spans(y_lens, Yc, generator=None):

@@ -26,6 +26,7 @@ import torch
 
 from . import ops
 from .ops import CLView
+from .weights import check_state_dict, to_device
 
 # get_nets_model(n_fft, size) parameter sets (nets.py:125-206): band-net width, bridge 2 (nin, nout), full-band net 2
 # width, bridge 3, full-band net 3 width, and whether the ASPP modules carry the two extra dilation-16 branches.
@@ -122,8 +123,7 @@ class _SpecNet:
     def to(self, device):
         self.device = torch.device(device)
         if self.layers is not None:
-            self.layers = {p: {k: (v.to(self.device) if torch.is_tensor(v) else v) for k, v in L.items()}
-                           for p, L in self.layers.items()}
+            self.layers = to_device(self.layers, self.device)
         return self
 
     def eval(self):
@@ -172,15 +172,10 @@ class CascadedASPPNet(_SpecNet):
     # ---- weights -----------------------------------------------------------------------------------------
     def load_state_dict(self, sd):
         """Reference state_dict (fp16 or fp32 storage) -> folded, channels-last fp32 layers on self.device.  Keys ending in
-        num_batches_tracked are ignored; any other missing or unexpected key, or a wrong shape, raises ValueError."""
+        num_batches_tracked are ignored; any other missing or unexpected key, a non-float tensor or a wrong shape raises
+        ValueError."""
         sd = {k: v for k, v in sd.items() if not k.endswith("num_batches_tracked")}
-        want = state_dict_shapes(self.size)
-        missing, unexpected = sorted(set(want) - set(sd)), sorted(set(sd) - set(want))
-        if missing or unexpected:
-            raise ValueError(f"state_dict does not match size {self.size}: missing {missing[:4]}, unexpected {unexpected[:4]}")
-        bad = [k for k, s in want.items() if tuple(sd[k].shape) != tuple(s)]
-        if bad:
-            raise ValueError(f"state_dict shapes do not match size {self.size}: {[(k, tuple(sd[k].shape)) for k in bad[:4]]}")
+        check_state_dict(sd, state_dict_shapes(self.size), f"CascadedASPPNet size {self.size}")
         layers = {}
         for p, (kind, shape) in layer_spec(self.size).items():
             if kind == "conv":
@@ -192,8 +187,7 @@ class CascadedASPPNet(_SpecNet):
                 scale, bias = _fold_bn(sd, p + ".conv.2")
                 layers[p] = dict(dw=sd[p + ".conv.0.weight"].float().reshape(shape[0], 9).contiguous(),
                                  w=_cl_weight(sd[p + ".conv.1.weight"]), scale=scale, bias=bias, k=1)
-        self.layers = {p: {k: (v.to(self.device) if torch.is_tensor(v) else v) for k, v in L.items()}
-                       for p, L in layers.items()}
+        self.layers = to_device(layers, self.device)
         return self
 
     @classmethod
@@ -441,16 +435,11 @@ class CascadedNet(_SpecNet):
 
     def load_state_dict(self, sd):
         """Reference state_dict (fp16 or fp32 storage) -> folded, channels-last fp32 layers on self.device.  Keys ending in
-        num_batches_tracked are ignored; any other missing or unexpected key, or a wrong shape, raises ValueError."""
+        num_batches_tracked are ignored; any other missing or unexpected key, a non-float tensor or a wrong shape raises
+        ValueError."""
         sd = {k: v for k, v in sd.items() if not k.endswith("num_batches_tracked")}
-        want = echo_state_dict_shapes(2 * self.max_bin, self.nout, self.nout_lstm)
-        tag = f"CascadedNet(n_fft={2 * self.max_bin}, nout={self.nout}, nout_lstm={self.nout_lstm})"
-        missing, unexpected = sorted(set(want) - set(sd)), sorted(set(sd) - set(want))
-        if missing or unexpected:
-            raise ValueError(f"state_dict does not match {tag}: missing {missing[:4]}, unexpected {unexpected[:4]}")
-        bad = [k for k, s in want.items() if tuple(sd[k].shape) != tuple(s)]
-        if bad:
-            raise ValueError(f"state_dict shapes do not match {tag}: {[(k, tuple(sd[k].shape)) for k in bad[:4]]}")
+        check_state_dict(sd, echo_state_dict_shapes(2 * self.max_bin, self.nout, self.nout_lstm),
+                         f"CascadedNet(n_fft={2 * self.max_bin}, nout={self.nout}, nout_lstm={self.nout_lstm})")
         place = self._placements()
         layers = {}
         for p, (kind, shape) in echo_layer_spec(2 * self.max_bin, self.nout, self.nout_lstm).items():
@@ -478,8 +467,7 @@ class CascadedNet(_SpecNet):
                 w_d = (sd[p + ".dense.0.weight"].double() * sc[:, None]).float()
                 b_d = ((sd[p + ".dense.0.bias"].double() - mean) * sc + sd[bn + ".bias"].double()).float()
                 layers[p] = dict(w_ih=w_ih.contiguous(), b=b, w_hh=w_hh.contiguous(), w_d=w_d.contiguous(), b_d=b_d)
-        self.layers = {p: {k: (v.to(self.device) if torch.is_tensor(v) else v) for k, v in L.items()}
-                       for p, L in layers.items()}
+        self.layers = to_device(layers, self.device)
         return self
 
     @classmethod

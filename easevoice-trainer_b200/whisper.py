@@ -28,6 +28,7 @@ import torch
 
 from . import ops
 from .models import ParamTree
+from .weights import check_state_dict
 
 N_FFT, HOP, N_FRAMES, N_CTX = 400, 160, 3000, 1500
 MAX_SAMPLES = 30 * 16000
@@ -114,7 +115,6 @@ class WhisperModel(ParamTree):
             raise ValueError("generation config's token layout does not fit the vocabulary")
         for name, shape in self.param_spec(c):
             self._register(name, torch.ones(shape) if name.endswith("layer_norm.weight") else torch.zeros(shape))
-        self._graphs = {}
 
     @staticmethod
     def param_spec(c):
@@ -151,17 +151,11 @@ class WhisperModel(ParamTree):
 
     # ---- loading ----------------------------------------------------------------------------------------------------------
     def load_state_dict(self, sd, strict=True):
-        """Strict: a missing or unexpected key or a wrong shape raises ValueError.  proj_out.weight, when present, must equal
-        the token embedding it is tied to."""
+        """Strict: a missing or unexpected key, a non-float tensor or a wrong shape raises ValueError.  proj_out.weight, when
+        present, must equal the token embedding it is tied to."""
         sd = dict(sd)
         tied = sd.pop("proj_out.weight", None)
-        spec = dict(self.param_spec(self.cfg))
-        miss, extra = sorted(set(spec) - set(sd)), sorted(set(sd) - set(spec))
-        if miss or extra:
-            raise ValueError(f"state_dict mismatch: missing {miss[:8]}, unexpected {extra[:8]}")
-        for k, shape in spec.items():
-            if tuple(sd[k].shape) != tuple(shape):
-                raise ValueError(f"{k}: shape {tuple(sd[k].shape)}, expected {tuple(shape)}")
+        check_state_dict(sd, dict(self.param_spec(self.cfg)), "WhisperModel")
         if tied is not None and not torch.equal(tied.float(), sd["model.decoder.embed_tokens.weight"].float()):
             raise ValueError("proj_out.weight differs from model.decoder.embed_tokens.weight (untied heads are not supported)")
         return super().load_state_dict({k: v.float() for k, v in sd.items()}, strict=True)
@@ -186,11 +180,10 @@ class WhisperModel(ParamTree):
 
     # ---- packed operands --------------------------------------------------------------------------------------------------
     def _packed(self):
-        """Every packed weight, made once per parameter version."""
-        ver = sum(int(p._version) for p in self.parameters())
-        c = self.__dict__.get("_pk")
-        if c is not None and c[0] == ver:
-            return c[1]
+        """Every packed weight, made once per weights_key()."""
+        return self.cached("packed", self._pack)
+
+    def _pack(self):
         cfg, P = self.cfg, self.P
         pk = lambda w: ops.pack_weight(w.detach().contiguous(), None, need_pb=False)   # noqa: E731
         z = lambda n: torch.zeros(n, device=P("model.encoder.conv1.bias").device)     # noqa: E731
@@ -223,7 +216,6 @@ class WhisperModel(ParamTree):
         dev = P("model.encoder.conv1.bias").device
         d["basis"] = torch.tensor(dft_basis(), dtype=torch.float32, device=dev).contiguous()
         d["fb"] = torch.tensor(mel_filters(cfg["num_mel_bins"]), dtype=torch.float32, device=dev).contiguous()
-        self.__dict__["_pk"] = (ver, d)
         return d
 
     def _ln(self, x, name):
@@ -336,16 +328,18 @@ class WhisperModel(ParamTree):
         """The decode step (forward of every row, beam step, position + 1) captured once per (clips, beam, max_new_tokens,
         track_lse).  Graphs of one (clips, beam) share one decode state; a batch of another shape replaces that state and its
         graphs rather than adding to the device memory a batch is sized for (cross K/V and slots for every clip).  track_lse:
-        the beam step also carries what transformers' long-form avg_logprob needs."""
+        the beam step also carries what transformers' long-form avg_logprob needs.  The graphs hold the packed operands and the
+        precise mode's kernels, so they are captured again whenever _packed() is made again."""
+        graphs = self.cached("graphs", dict)
         skey = (clips, beam, str(dev))
         if self.__dict__.get("_gstate") is None or self._gstate[0] != skey:
-            self._graphs.clear()
+            graphs.clear()
             self._gstate = None
             torch.cuda.empty_cache()
             self._gstate = (skey, self._state(clips, beam, dev))
         gkey = (max_new_tokens, track_lse)
-        if gkey in self._graphs:
-            return self._graphs[gkey]
+        if gkey in graphs:
+            return graphs[gkey]
         st = self._gstate[1]
         lay = self._layout(3, max_new_tokens)
 
@@ -364,8 +358,8 @@ class WhisperModel(ParamTree):
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             step()
-        self._graphs[gkey] = (g, st)
-        return self._graphs[gkey]
+        graphs[gkey] = (g, st)
+        return graphs[gkey]
 
     @torch.no_grad()
     def transcribe_features(self, feats, language=None, num_beams=NUM_BEAMS, max_new_tokens=MAX_NEW_TOKENS, check_every=8,

@@ -1595,15 +1595,12 @@ def check_hubert():
             with torch.no_grad():
                 ho.forward(P, wav, m, taps=taps)
             # the feature extractor alone (7 strided convs + GroupNorm + GELU): recomputed through the public pieces
-            net._active, net._memo_pack = net.packed_for_inference(), True
-            try:
+            with net.inference_weights():
                 xx = ops.pad_channels(wav.to(DEV).unsqueeze(-1).contiguous(), 4)
                 for i, (k, st) in enumerate(zip(net.cfg["conv_kernel"], net.cfg["conv_stride"])):
                     xx = ops.conv(xx, net.w(f"feature_extractor.conv_layers.{i}.conv", need_pb=False, pad1=4 if i == 0 else 0), None, stride=st)
                     xx = ops.instnorm_cl(xx, net.P("feature_extractor.conv_layers.0.layer_norm.weight"),
                                          net.P("feature_extractor.conv_layers.0.layer_norm.bias"), 1e-5, gelu_after=True) if i == 0 else ops.gelu(xx)
-            finally:
-                net._active, net._memo_pack = None, False
             out.append(("hubert[l2] feature extractor output vs oracle (rel-L2)", rel(xx, taps["features"]), TOL_NET))
     return out
 

@@ -99,15 +99,11 @@ def test_token_step_rows_are_independent(ops):
 
     def run(cs, xx):
         n = torch.tensor([n_prev], dtype=torch.int32, device=DEV)
-        net._active, net._memo_pack = net.packed_for_inference(), True
-        try:
-            with torch.no_grad():
-                h = xx
-                for i in range(net.num_layers):
-                    h = net._infer_layer(i, h, cs[i], n, skip=skip)
-                return ops.linear_rows(h, net.w("ar_predict_layer", pad0=1028))
-        finally:
-            net._active, net._memo_pack = None, False
+        with net.inference_weights(), torch.no_grad():
+            h = xx
+            for i in range(net.num_layers):
+                h = net._infer_layer(i, h, cs[i], n, skip=skip)
+            return ops.linear_rows(h, net.w("ar_predict_layer", pad0=1028))
     a = run([c.clone() for c in caches], x)
     c2 = [c.clone() for c in caches]
     for c in c2:
