@@ -554,7 +554,7 @@ static int dgrad_polyphase(const evk_gconv_desc* d, const float* wt, int ld_wt, 
                 "gconv_dgrad: memset failed");
   }
   evk_gconv_desc h = {};
-  h.x = d->y; h.y = const_cast<float*>(d->x); h.bias = d->bias;
+  h.x = d->y; h.y = const_cast<float*>(d->x); h.bias = d->bias; h.out_len = d->out_len;     // dX rows >= out_len[b] written as 0
   h.x_sb = d->y_sb; h.w_sq = (long long)s * Cg * ld_wt; h.y_sb = d->x_sb;
   h.ldx = d->ldy; h.ldw = ld_wt; h.ldy = d->ldx;
   h.Z = d->Z * G; h.H = G; h.G = 1; h.C = Ng; h.N = Cg;
@@ -579,11 +579,18 @@ extern "C" int evk_gconv_dgrad(const evk_gconv_desc* d, const float* wt, int32_t
   EVK_REQUIRE(d->H == 1 && d->ldx == d->C && d->x_sb == (long long)d->Tin * d->P * d->C, EVK_ERR_ARG,
               "gconv_dgrad: dX must be a dense [Z][Tin*P][C] tensor, H = 1");
   cudaStream_t st = (cudaStream_t)stream;
-  rc = dgrad_polyphase_ok(d, wt, ld_wt) ? dgrad_polyphase(d, wt, ld_wt, st) : conv_direct_dgrad(d, st);
-  if (rc || !d->in_len) return rc;
-  // the forward reads row t*P + w as zero when t >= in_len[b]: with P*C floats per t, that is a row mask over t
   float* dx = const_cast<float*>(d->x);
   const int ld = d->P * d->C;
+  if (dgrad_polyphase_ok(d, wt, ld_wt)) {
+    rc = dgrad_polyphase(d, wt, ld_wt, st);                  // out_len is applied in the launches' epilogues
+  } else {
+    evk_gconv_desc h = *d;
+    h.out_len = nullptr;                                     // the direct kernel reads out_len as the forward's; masked after
+    rc = conv_direct_dgrad(&h, st);
+    if (!rc && d->out_len) rc = evk_rowmask(dx, ld, dx, ld, d->Z, d->Tin, ld, d->out_len, stream);
+  }
+  if (rc || !d->in_len) return rc;
+  // the forward reads row t*P + w as zero when t >= in_len[b]: with P*C floats per t, that is a row mask over t
   return evk_rowmask(dx, ld, dx, ld, d->Z, d->Tin, ld, d->in_len, stream);
 }
 

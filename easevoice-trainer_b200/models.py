@@ -433,14 +433,20 @@ class SynthesizerTrn(ParamTree):
         stats = ops.linear(y, self.w("enc_p.proj"), self.b("enc_p.proj"), out_len=length)
         return stats
 
-    def _generator(self, z, ge):
-        """Generator.forward, models.py:452-471 + ResBlock1 modules.py:298-311."""
-        x = ops.conv(z, self.w("dec.conv_pre"), self.b("dec.conv_pre"), pad=3)
+    def _generator(self, z, ge, lengths=None):
+        """Generator.forward, models.py:452-471 + ResBlock1 modules.py:298-311.  lengths (inference, int32 device [B], frames
+        of z; z zero past them): rows of different lengths.  Every conv then writes zeros past the row's length at its rate, so
+        every conv reads zeros there, as it reads the zero padding past the end of a row vocoded alone."""
+        lens = lengths
+        x = ops.conv(z, self.w("dec.conv_pre"), self.b("dec.conv_pre"), pad=3, out_len=lens)
         x = ops.add_bvec(x, ops.linear(ge, self.w("dec.cond"), self.b("dec.cond")))
+        if lens is not None:
+            x = ops.rowmask(x, lens)                       # the conditioning vector is added to every row
         nk = len(self.resblock_kernel_sizes)
         for i, (u, k) in enumerate(zip(self.upsample_rates, self.upsample_kernel_sizes)):
             x = ops.lrelu(x, LRELU_SLOPE)
-            x = ops.conv_transpose(x, self.w(f"dec.ups.{i}"), self.b(f"dec.ups.{i}"), stride=u, pad=(k - u) // 2)
+            lens = None if lens is None else lens * u
+            x = ops.conv_transpose(x, self.w(f"dec.ups.{i}"), self.b(f"dec.ups.{i}"), stride=u, pad=(k - u) // 2, out_len=lens)
             xa = ops.lrelu(x, LRELU_SLOPE)                 # shared first activation of the three resblocks
             outs = []
             # the three resblocks of a stage are independent chains of six convolutions; stage 0 is 40 tiles on 132 SMs and
@@ -458,8 +464,9 @@ class SynthesizerTrn(ParamTree):
                     h, ha = x, xa
                     for l, d in enumerate(rd):
                         t = ops.conv(ha, self.w(f"{r}.convs1.{l}"), self.b(f"{r}.convs1.{l}"), pad=(rk * d - d) // 2, dil=d,
-                                     act=ops.ACT_LRELU, slope=LRELU_SLOPE)
-                        h = ops.conv(t, self.w(f"{r}.convs2.{l}"), self.b(f"{r}.convs2.{l}"), pad=(rk - 1) // 2, res=h)
+                                     act=ops.ACT_LRELU, slope=LRELU_SLOPE, out_len=lens)
+                        h = ops.conv(t, self.w(f"{r}.convs2.{l}"), self.b(f"{r}.convs2.{l}"), pad=(rk - 1) // 2, res=h,
+                                     out_len=lens)
                         if l < len(rd) - 1:
                             ha = ops.lrelu(h, LRELU_SLOPE)
                 if st is not None:
@@ -471,7 +478,7 @@ class SynthesizerTrn(ParamTree):
             x = ops.add3(outs[0], outs[1], outs[2], 1.0 / nk, 1.0 / nk, 1.0 / nk)
         x = ops.lrelu(x, 0.01)                             # F.leaky_relu default slope (models.py:467)
         # the single output channel is padded to 4 (zero weights) so that its gradients stay on the tensor-core kernels
-        y4 = ops.conv(x, self.w("dec.conv_post", pad0=4), None, pad=3, act=ops.ACT_TANH)
+        y4 = ops.conv(x, self.w("dec.conv_post", pad0=4), None, pad=3, act=ops.ACT_TANH, out_len=lens)
         return ops.take_channels(y4, 1)
 
     # ---------------------------------------------------------------------------------------------
@@ -646,13 +653,8 @@ class SynthesizerTrn(ParamTree):
         was_training = self.training
         self.eval()
         try:
-            refers = refer if isinstance(refer, (list, tuple)) else [refer]
             dev = codes.device
-            ges = []
-            for r in refers:
-                rl = torch.full((r.shape[0],), r.shape[2], device=dev, dtype=torch.int32)
-                ges.append(self._ref_enc(ops.to_channels_last(r.float(), pad_to=4), rl))
-            ge = ges[0] if len(ges) == 1 else torch.stack(ges, 0).mean(0)
+            ge = self.ref_style(refer)
             B, T = codes.shape[1], codes.shape[2]
             lengths = torch.full((B,), 2 * T, device=dev, dtype=torch.int32)
             text_len = torch.full((B,), text.shape[-1], device=dev, dtype=torch.int32)
@@ -672,6 +674,62 @@ class SynthesizerTrn(ParamTree):
             z = self._flow_reverse(z_p, lengths, ge)
             o = self._generator(ops.rowmask(z, lengths), ge)
             return ops.to_channels_first(o)
+        finally:
+            self.train(was_training)
+
+    @torch.no_grad()
+    def decode_batch(self, codes_list, text_list, ge_rows, noise_scale=0.5, noise=None, noise_keys=None):
+        """decode at speed 1 for several rows of different lengths in one pass (tts.run_many): codes_list[b] int64 [T_b] (the
+        codes of one bucket, its sentences concatenated), text_list[b] int64 [X_b] (their phones), ge_rows [B, 1, 512] (row b's
+        style vector: the mean of _ref_enc over its reference spectrograms, ref_style) -> list of B waveforms [2 T_b * hop].
+        The prior encoder, the flow and the generator take per-row lengths; the generator writes zeros past each row's length at
+        every rate (_generator), so no row reads a neighbour's padding.  noise: None, or a list of [2 T_b, 192] normal draws
+        (tests); without it row b's draws are keyed by noise_keys[b] = (seed, index), so they do not depend on the other rows.
+        speed != 1 is not batched: use decode, one sentence at a time."""
+        was_training = self.training
+        self.eval()
+        try:
+            B, dev, I = len(codes_list), ge_rows.device, self.inter_channels
+            T = [int(c.shape[0]) for c in codes_list]
+            Tm, Xm = max(T), max(int(t.shape[0]) for t in text_list)
+            codes = torch.zeros((B, Tm), dtype=torch.int64, device=dev)
+            text = torch.zeros((B, Xm), dtype=torch.int64, device=dev)
+            for b in range(B):
+                codes[b, :T[b]] = codes_list[b]
+                text[b, :text_list[b].shape[0]] = text_list[b]
+            lengths = torch.tensor([2 * t for t in T], dtype=torch.int32).to(dev)
+            text_len = torch.tensor([int(t.shape[0]) for t in text_list], dtype=torch.int32).to(dev)
+            quantized = ops.embedding(self.P("quantizer.vq.layers.0._codebook.embed"), codes, rep=2)
+            stats = self._enc_p(quantized, lengths, text, text_len, ge_rows)
+            z = torch.zeros((B, 2 * Tm, I), device=dev, dtype=torch.float32)
+            for b in range(B):
+                if noise is not None:
+                    z[b, :2 * T[b]] = noise[b].to(dev, torch.float32)
+                else:
+                    seed, k = noise_keys[b]
+                    state = torch.tensor([int(seed) & (2 ** 63 - 1), int(k) << 40], dtype=torch.int64, device=dev)
+                    z[b, :2 * T[b]] = ops.randn((2 * T[b], I), "decode_batch.noise", device=dev, state=state)
+            z_p = ops.reparam(stats, z * float(noise_scale), lengths)
+            zf = self._flow_reverse(z_p, lengths, ge_rows)
+            o = self._generator(ops.rowmask(zf, lengths), ge_rows, lengths)
+            hop = o.shape[1] // (2 * Tm)
+            return [o[b, :2 * T[b] * hop, 0] for b in range(B)]
+        finally:
+            self.train(was_training)
+
+    @torch.no_grad()
+    def ref_style(self, refer):
+        """decode's style vector: the mean of _ref_enc over the reference spectrograms refer ([1, 1025, Tr] or a list) ->
+        [1, 1, 512]"""
+        was_training = self.training
+        self.eval()
+        try:
+            refers = refer if isinstance(refer, (list, tuple)) else [refer]
+            ges = []
+            for r in refers:
+                rl = torch.full((r.shape[0],), r.shape[2], device=r.device, dtype=torch.int32)
+                ges.append(self._ref_enc(ops.to_channels_last(r.float(), pad_to=4), rl))
+            return ges[0] if len(ges) == 1 else torch.stack(ges, 0).mean(0)
         finally:
             self.train(was_training)
 

@@ -292,13 +292,15 @@ class Text2SemanticDecoder(ParamTree):
                   caches=[torch.empty((B, rows, 3 * D), device=dev, dtype=torch.float32) for _ in range(self.num_layers)],
                   n=z(1, dtype=torch.int32), x=z(B, 1, D), logits=z(B, Vp), skip=z(B, 2, dtype=torch.int32),
                   hist=z(B, rows, dtype=torch.int64), seen=z(B, (V + 31) // 32, dtype=torch.int32), fin=z(B, 2, dtype=torch.int32),
-                  icfg=z(6, dtype=torch.int64), fcfg=z(3), pe=self.pe(rows, dev))
+                  icfg=z(6, dtype=torch.int64), fcfg=z(3), pe=self.pe(rows, dev),
+                  rcfg=z(B, 8, dtype=torch.int64), rfcfg=z(B, 4))                # per-row tables of decode_groups
         self.__dict__[key] = st
         return st
 
     def _batch_step_graph(self, st, head, eos_steps):
         """The step graph of `st` whose sampler excludes EOS at the steps idx < eos_steps (a kernel argument, fixed at capture:
-        1 for infer_panel_batch_infer, 11 for infer_panel_naive and prompt-free decoding), captured on first use."""
+        1 for infer_panel_batch_infer, 11 for infer_panel_naive and prompt-free decoding), captured on first use.  eos_steps
+        "rows": the sampler of decode_groups, which reads every row's configuration from st["rcfg"] / st["rfcfg"]."""
         if eos_steps not in st["graphs"]:
             st["graphs"][eos_steps] = self._capture_batch_step(st, head, eos_steps)
         return st["graphs"][eos_steps]
@@ -310,8 +312,12 @@ class Text2SemanticDecoder(ParamTree):
         a_audio = self.P("ar_audio_position.alpha")
 
         def step():
-            ops.sample_tokens(st["logits"], self.vocab_size, self.EOS, st["icfg"], st["fcfg"], st["n"], st["hist"], st["seen"],
-                              st["fin"], emb, st["pe"], a_audio, st["x"], eos_steps=eos_steps)
+            if eos_steps == "rows":
+                ops.sample_tokens_rows(st["logits"], self.vocab_size, self.EOS, st["rcfg"], st["rfcfg"], st["n"], st["hist"],
+                                       st["seen"], st["fin"], emb, st["pe"], a_audio, st["x"])
+            else:
+                ops.sample_tokens(st["logits"], self.vocab_size, self.EOS, st["icfg"], st["fcfg"], st["n"], st["hist"], st["seen"],
+                                  st["fin"], emb, st["pe"], a_audio, st["x"], eos_steps=eos_steps)
             h = st["x"]
             for i in range(self.num_layers):
                 h = self._infer_layer(i, h, st["caches"][i], st["n"], skip=st["skip"])
@@ -338,11 +344,19 @@ class Text2SemanticDecoder(ParamTree):
         fin as a host list of [stop step, idx] per row.  The noise seed is drawn here, once per call, from torch's CUDA generator."""
         # one row reads the flags after every replay: a short utterance (~40 tokens) would otherwise run up to INFER_BATCH_K - 1
         # steps past its finish, which costs it more than the reads
-        dev, K = st["dev"], (INFER_BATCH_K if st["B"] > 1 and trace is None else 1)
-        st["fin"].fill_(-1)
+        dev = st["dev"]
         st["icfg"][0:1].copy_(torch.randint(0, 2 ** 62, (1,), device=dev, dtype=torch.int64))
         st["icfg"][1:].copy_(torch.tensor([prefix, n0, top_k, early_stop_num, max_steps], dtype=torch.int64))
         st["fcfg"].copy_(torch.tensor([float(top_p), float(temperature), float(repetition_penalty)], dtype=torch.float32))
+        return self._replay(st, graph, trace)
+
+    def _replay(self, st, graph, trace, live=None):
+        """Replay the step graph until every row of `st` has finished -> fin as a host list of [stop step, idx] per row.
+        live: rows live .. B - 1 are padding, finished from the start."""
+        K = INFER_BATCH_K if st["B"] > 1 and trace is None else 1
+        st["fin"].fill_(-1)
+        if live is not None:
+            st["fin"][live:].fill_(0)
         while True:
             for _ in range(K):
                 if trace is not None:
@@ -456,31 +470,119 @@ class Text2SemanticDecoder(ParamTree):
                     xp[b, :rows[b].shape[0]] = rows[b]
                     bp[b, :, :rows[b].shape[0]] = bert[b]
                 st = self._batch_state(dev, B, L0 + cap + INFER_BATCH_K)
-                Vp = st["logits"].shape[1]
-                head = self.w("ar_predict_layer", pad0=Vp)
+                head = self.w("ar_predict_layer", pad0=st["logits"].shape[1])
                 graph = self._batch_step_graph(st, head, eos_steps)
-                # prompt pass (process_prompt with the padded mask, :596-646; prompt-free: the text alone, :796-803)
                 y = torch.zeros((B, 0), device=dev, dtype=torch.int64) if prompts is None else prompts.to(torch.int64)
-                xe = self._embed_text(xp, bp, False)
-                ye = ops.embedding(self.P("ar_audio_embedding.word_embeddings.weight"), y)
-                h = ops.gpt_embed(xe, ye, self.P("ar_text_position.alpha"), self.P("ar_audio_position.alpha"), st["pe"])
-                xl = torch.tensor(lens, device=dev, dtype=torch.int64)
-                yl = torch.full((B,), Yp, device=dev, dtype=torch.int64)
-                for i in range(self.num_layers):
-                    h = self._infer_layer(i, h, st["caches"][i], None, X=max_len, xl=xl, yl=yl)
-                first = xl - 1 if prompts is None else torch.full((B,), L0 - 1, device=dev, dtype=torch.int64)
-                st["logits"].copy_(ops.linear_rows(ops.slice_rows(h, first, 1), head).view(B, Vp))
+                self._prompt_pass(st, head, 0, xp, lens, bp, y, max_len, prompts is not None)
                 # per-call state of the step graph
                 st["n"].fill_(L0)
                 st["skip"].copy_(torch.tensor([[v, max_len] for v in lens], dtype=torch.int32))
-                st["hist"][:, :Yp].copy_(y)
-                bits = torch.zeros((B, st["seen"].shape[1] * 32), device=dev, dtype=torch.int64).scatter_(1, y, 1)
-                words = (bits.view(B, -1, 32) << torch.arange(32, device=dev, dtype=torch.int64)).sum(-1)
-                st["seen"].copy_(torch.where(words >= 2 ** 31, words - 2 ** 32, words))      # uint32 bit patterns as int32
                 fin = self._run_batch(st, graph, Yp, L0, max_steps, top_k, early_stop_num, top_p, temperature, repetition_penalty, trace)
                 return [st["hist"][b, :Yp + fin[b][0]].clone() for b in range(B)], fin
         finally:
             self.train(was_training)
+
+    def _prompt_pass(self, st, head, r0, xp, lens, bp, y, max_len, has_prompt):
+        """Prompt pass of rows r0 .. r0 + B - 1 of `st` (process_prompt with the padded mask, :596-646; prompt-free: the text
+        alone, :796-803): text xp [B, max_len] (bert bp [B, 1024, max_len]; row b's first lens[b] positions are text) then the
+        prompt y [B, Yp], on the training kernels.  Fills cache rows 0 .. max_len + Yp - 1, the first logits (from position
+        max_len + Yp - 1 with a prompt, lens[b] - 1 without), the history's first Yp entries and the seen bitmaps."""
+        B, dev, Vp = xp.shape[0], xp.device, st["logits"].shape[1]
+        Yp = y.shape[1]
+        rows = slice(r0, r0 + B)
+        xe = self._embed_text(xp, bp, False)
+        ye = ops.embedding(self.P("ar_audio_embedding.word_embeddings.weight"), y)
+        h = ops.gpt_embed(xe, ye, self.P("ar_text_position.alpha"), self.P("ar_audio_position.alpha"), st["pe"])
+        xl = torch.tensor(lens, device=dev, dtype=torch.int64)
+        yl = torch.full((B,), Yp, device=dev, dtype=torch.int64)
+        for i in range(self.num_layers):
+            h = self._infer_layer(i, h, st["caches"][i][rows], None, X=max_len, xl=xl, yl=yl)
+        first = torch.full((B,), max_len + Yp - 1, device=dev, dtype=torch.int64) if has_prompt else xl - 1
+        st["logits"][rows].copy_(ops.linear_rows(ops.slice_rows(h, first, 1), head).view(B, Vp))
+        st["hist"][rows, :Yp].copy_(y)
+        bits = torch.zeros((B, st["seen"].shape[1] * 32), device=dev, dtype=torch.int64).scatter_(1, y, 1)
+        words = (bits.view(B, -1, 32) << torch.arange(32, device=dev, dtype=torch.int64)).sum(-1)
+        st["seen"][rows].copy_(torch.where(words >= 2 ** 31, words - 2 ** 32, words))      # uint32 bit patterns as int32
+
+    @torch.no_grad()
+    def decode_groups(self, groups, max_steps=MAX_DECODE_STEPS, trace=None):
+        """Rows of several decoding calls decoded together, each row with its own prompt length and sampling settings
+        (tts.run_many).  groups: list of dicts, one per call that _decode_batch would make, with at most 64 rows in all:
+          rows, lens, bert, max_len  as _decode_batch takes them (list of 1-D phoneme ids, text lengths, [1024, width] features);
+          prompt     1-D int64 device tensor shared by the group's rows, or None (prompt-free);
+          seed       int64 device [1], the noise seed that call would draw;
+          eos_steps, top_k, top_p, temperature, repetition_penalty, early_stop_num  as _decode_batch takes them.
+        -> (ys, fin) as _decode_batch, rows in group order.  Row j of a group samples with its group's seed and key row j, and
+        every part of its computation is the one of that call alone:
+          - each group has its own prompt pass, with its own text width and prompt (_prompt_pass);
+          - the caches then hold, for every row, its text at 0 .. max_len_g - 1 and its prompt right-aligned at L0 - Yp_g .. L0 - 1,
+            L0 = max over groups of max_len_g + Yp_g; the step attention leaves out lens[b] .. L0 - Yp_g - 1 and walks the other keys
+            as one list (evk_attn_decode_dev), so it sums exactly what it sums in the call alone;
+          - the step Linears are row-invariant (ops.linear_rows), and the sampler reads the row's configuration
+            (evk_sample_tokens_rows; the token of step idx is embedded at pe[Yp_g + idx] and stored at hist[Yp_g + idx]).
+        `trace` (a list, tests) receives the raw [B, V] logits of every step."""
+        B = sum(len(g["rows"]) for g in groups)
+        assert 1 <= B <= 64, "decode_groups takes 1 to 64 rows"
+        # the state and its step graph are kept per row count: padding to 8, 16, 32 or 64 rows lets calls with different
+        # mixes of requests share them (padded rows are finished from the start; every step computation is row-invariant)
+        Bp = max(8, 1 << (B - 1).bit_length())
+        dev = groups[0]["bert"][0].device
+        widths = [g["max_len"] + (0 if g["prompt"] is None else g["prompt"].shape[0]) for g in groups]
+        L0 = max(widths)
+        caps = [max_steps if g["early_stop_num"] == -1 else min(max_steps, g["early_stop_num"] + 1) for g in groups]
+        was_training = self.training
+        self.eval()
+        try:
+            with self.inference_weights():
+                st = self._batch_state(dev, Bp, L0 + max(caps) + INFER_BATCH_K)
+                head = self.w("ar_predict_layer", pad0=st["logits"].shape[1])
+                graph = self._batch_step_graph(st, head, "rows")
+                icfg, fcfg, skip, prefixes = row_tables(groups, max_steps)
+                r0 = 0
+                for g, W in zip(groups, widths):
+                    n, ml = len(g["rows"]), g["max_len"]
+                    Yp = 0 if g["prompt"] is None else g["prompt"].shape[0]
+                    xp = torch.zeros((n, ml), device=dev, dtype=torch.int64)
+                    bp = torch.zeros((n, 1024, ml), device=dev, dtype=torch.float32)
+                    for b in range(n):
+                        xp[b, :g["rows"][b].shape[0]] = g["rows"][b]
+                        bp[b, :, :g["rows"][b].shape[0]] = g["bert"][b]
+                    y = (torch.zeros((n, 0), device=dev, dtype=torch.int64) if g["prompt"] is None
+                         else g["prompt"].to(torch.int64).expand(n, -1))
+                    self._prompt_pass(st, head, r0, xp, list(g["lens"]), bp, y, ml, g["prompt"] is not None)
+                    if W < L0 and Yp:                                  # right-align the prompt rows at L0
+                        for c in st["caches"]:
+                            c[r0:r0 + n, L0 - Yp:L0].copy_(c[r0:r0 + n, ml:W].clone())
+                    r0 += n
+                st["rcfg"][:B].copy_(torch.tensor(icfg, dtype=torch.int64))
+                st["rcfg"][:B, 0:1].copy_(torch.cat([g["seed"].reshape(1).expand(len(g["rows"])) for g in groups]).view(B, 1))
+                st["rfcfg"][:B].copy_(torch.tensor(fcfg, dtype=torch.float32))
+                st["skip"][:B].copy_(torch.tensor(skip, dtype=torch.int32))
+                st["skip"][B:].zero_()
+                st["n"].fill_(L0)
+                fin = self._replay(st, graph, trace, live=B)[:B]
+                if trace is not None:
+                    trace[:] = [t[:B] for t in trace]
+                return [st["hist"][b, :prefixes[b] + fin[b][0]].clone() for b in range(B)], fin
+        finally:
+            self.train(was_training)
+
+def row_tables(groups, max_steps):
+    """Host side of decode_groups' per-row state -> (icfg, fcfg, skip, prefixes), one entry per row in group order:
+    icfg (seed placeholder 0, prefix Yp_g, n0 = L0, top_k, early_stop_num, max_steps, eos_steps, key row = the row's index in
+    its group), fcfg (top_p, temperature, repetition_penalty, 0), skip (lens[b], L0 - Yp_g): the keys the row's step attention
+    leaves out, and prefix Yp_g.  L0 = max over groups of max_len + Yp."""
+    yps = [0 if g["prompt"] is None else int(g["prompt"].shape[0]) for g in groups]
+    L0 = max(g["max_len"] + yp for g, yp in zip(groups, yps))
+    icfg, fcfg, skip, prefixes = [], [], [], []
+    for g, Yp in zip(groups, yps):
+        n = len(g["rows"])
+        icfg += [[0, Yp, L0, int(g["top_k"]), int(g["early_stop_num"]), int(max_steps), int(g["eos_steps"]), j] for j in range(n)]
+        fcfg += [[float(g["top_p"]), float(g["temperature"]), float(g["repetition_penalty"]), 0.0]] * n
+        skip += [[int(v), L0 - Yp] for v in g["lens"]]
+        prefixes += [Yp] * n
+    return icfg, fcfg, skip, prefixes
+
 
 def reject_spans(y_lens, Yc, generator=None):
     """The host draw of make_reject_y: per item, sorted(randint(0, Yc, (2,))) -> int32 [B, 2] of spans (i0, i1).  The same

@@ -600,7 +600,7 @@ class _ConvTFn(torch.autograd.Function):
     its forward."""
 
     @staticmethod
-    def forward(ctx, x, pa, pb, bias, cfg):
+    def forward(ctx, x, pa, pb, bias, cfg, out_len=None):
         Q, stride, pad = cfg
         x = _cl(x)
         B, Tin, Cin = x.shape
@@ -608,7 +608,7 @@ class _ConvTFn(torch.autograd.Function):
         Tout = (Tin - 1) * stride - 2 * pad + Q
         y = torch.empty((B, Tout, Cout), device=x.device, dtype=torch.float32)
         _, _, ldx = _rows(x)
-        d = _desc(x=y, w=pa, y=x, bias=bias, x_sb=Tout * Cout, w_sq=Cin * lda, y_sb=Tin * ldx, ldx=Cout, ldw=lda, ldy=ldx, Z=B,
+        d = _desc(x=y, w=pa, y=x, bias=bias, out_len=out_len, x_sb=Tout * Cout, w_sq=Cin * lda, y_sb=Tin * ldx, ldx=Cout, ldw=lda, ldy=ldx, Z=B,
                   C=Cout, N=Cin, Q=Q, Tin=Tout, J=Tin, P=1, is_=stride, os_=1, Tout=Tin, off=[q - pad for q in range(Q)])
         d.wt, d.ld_wt = _p(pb), pb.shape[2]
         _run_desc("evk_gconv_dgrad", d)
@@ -639,11 +639,14 @@ class _ConvTFn(torch.autograd.Function):
         if ctx.needs_input_grad[3]:
             dbias = torch.empty(Cout, device=dy.device, dtype=torch.float32)
             _call("evk_colsum", _p(dy), B * Tout, Cout, Cout, _p(dbias), 0)
-        return dx, dpa, None, dbias, None
+        return dx, dpa, None, dbias, None, None
 
 
-def conv_transpose(x, w: PackedW, bias, *, stride, pad):
-    return _ConvTFn.apply(x, w.pa, w.pb, bias, (w.Q, stride, pad))
+def conv_transpose(x, w: PackedW, bias, *, stride, pad, out_len=None):
+    """ConvTranspose1d.  out_len (inference, int32 device [B]): output rows past out_len[b] are written as zero; x's rows past
+    a row's input length must be zero (evk_gconv_dgrad)."""
+    assert out_len is None or not torch.is_grad_enabled(), "conv_transpose(out_len=...) has no backward"
+    return _ConvTFn.apply(x, w.pa, w.pb, bias, (w.Q, stride, pad), out_len)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1181,9 +1184,10 @@ def dropout(x, p, tag):
     return _DropoutFn.apply(x, p, stream_id(tag))
 
 
-def randn(shape, tag, device=None):
+def randn(shape, tag, device=None, state=None):
+    """standard normal draws keyed by the library's RNG state, or by `state` (int64 device [2] = (seed, offset)) when given"""
     y = torch.empty(shape, device=device or "cuda", dtype=torch.float32)
-    _call("evk_randn", _p(y), y.numel(), _p(rng_state(y.device)), ctypes.c_uint64(stream_id(tag)))
+    _call("evk_randn", _p(y), y.numel(), _p(rng_state(y.device) if state is None else state), ctypes.c_uint64(stream_id(tag)))
     return y
 
 
@@ -1922,6 +1926,18 @@ def sample_tokens(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, a
     _call("evk_sample_tokens", _p(logits), logits.stride(0), B, V, eos, int(eos_steps), _p(icfg), _p(fcfg), _p(n_dev), _p(q),
           q.stride(0) if q is not None else 0, _p(hist), hist.stride(0), _p(seen), _p(fin), _p(emb), _p(pe), _p(alpha),
           _p(x_next), D)
+
+
+def sample_tokens_rows(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, alpha, x_next):
+    """sample_tokens with one configuration per row (evk_sample_tokens_rows): icfg int64 [B, 8] = (seed, prefix, n0, top_k,
+    early_stop, max_steps, eos_steps, key row), fcfg float32 [B, 4] = (top_p, temperature, penalty, unused)."""
+    B, D = logits.shape[0], x_next.shape[-1]
+    assert logits.stride(-1) == 1 and hist.dtype == torch.int64 and seen.dtype == torch.int32 and fin.dtype == torch.int32
+    assert icfg.dtype == torch.int64 and icfg.is_contiguous() and tuple(icfg.shape) == (B, 8)
+    assert fcfg.dtype == torch.float32 and fcfg.is_contiguous() and tuple(fcfg.shape) == (B, 4)
+    assert x_next.is_contiguous() and pe.is_contiguous()
+    _call("evk_sample_tokens_rows", _p(logits), logits.stride(0), B, V, eos, _p(icfg), _p(fcfg), _p(n_dev), _p(hist),
+          hist.stride(0), _p(seen), _p(fin), _p(emb), _p(pe), _p(alpha), _p(x_next), D)
 
 
 def ce_sum_topk(logits, targets, topk=3, ignore_index=1024, V=None, count=None):

@@ -130,7 +130,11 @@ int evk_gconv_wgrad_takes_dyt(const evk_gconv_desc* d);
  *      inner batch.  A strided conv needs taps at consecutive offsets (dilation 1).  When Q < is, dX is zeroed first
  *      (rows of a residue with no tap stay zero, without the bias);
  *   2. otherwise the direct kernel.
- * With d->in_len, rows t*P + w of dX with t >= in_len[b] are zeroed afterwards: the forward read them as zero. */
+ * With d->in_len, rows t*P + w of dX with t >= in_len[b] are zeroed afterwards: the forward read them as zero.
+ * With d->out_len (it bounds dX, the rows this call writes, not the forward's output), rows t*P + w of dX with
+ * t >= out_len[b] are written as zero: by the epilogues of route 1's launches (the length mask of evk_gconv_fwd), after
+ * route 2.  ConvTranspose1d over rows of different lengths passes its output lengths here; its input rows past a row's
+ * length must hold zeros, which they do when they come from launches masked the same way. */
 int evk_gconv_dgrad(const evk_gconv_desc* d, const float* wt, int32_t ld_wt, evk_stream_t stream);
 
 /* out[n] (+)= sum_rows x[row][n]  -- bias gradients */
@@ -466,6 +470,14 @@ int evk_sample_tokens(const float* logits, int32_t ldl, int32_t B, int32_t V, in
                       const int64_t* icfg, const float* fcfg, const int32_t* n_dev, const float* q, int32_t ldq, int64_t* hist,
                       int32_t ldh, uint32_t* seen, int32_t* fin, const float* emb, const float* pe, const float* alpha,
                       float* x_next, int32_t D, evk_stream_t stream);
+/* evk_sample_tokens with one configuration per row (tts.run_many decodes rows of several requests together), no supplied
+ * draws:  icfg: device int64 [B][8], row b = (seed, prefix, n0, top_k >= 1, early_stop, max_steps, eos_steps >= 0, key row);
+ * fcfg: device float [B][4], row b = (top_p, T, penalty, unused).  Row b's Exp(1) draws are keyed by (its seed, its key row,
+ * idx, class) instead of (seed, b, idx, class), so a row samples what it would sample at row `key row` of a batch decoded with
+ * evk_sample_tokens and that seed, whichever rows share the launch. */
+int evk_sample_tokens_rows(const float* logits, int32_t ldl, int32_t B, int32_t V, int32_t eos, const int64_t* icfg,
+                           const float* fcfg, const int32_t* n_dev, int64_t* hist, int32_t ldh, uint32_t* seen, int32_t* fin,
+                           const float* emb, const float* pe, const float* alpha, float* x_next, int32_t D, evk_stream_t stream);
 /* Cross entropy over rows [B][T] of positions (row r is position r % T).  count: NULL (every row counts; T is then unused), or
  * a device int32 scalar n: positions t >= n add no loss, no accuracy count (neither valid nor hit) and no gradient (evk_ce_bwd
  * writes 0 to their logit gradients).  The bound is for batches padded past the collate's length (the stage-1 trainer pads to
