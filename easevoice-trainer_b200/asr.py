@@ -4,7 +4,8 @@
 Differences from the reference, which runs faster-whisper: the model is a local Hugging Face Whisper directory (config.json,
 model.safetensors or pytorch_model.bin, generation_config.json, tokenizer.json), decoding follows transformers' `generate`
 (5 beams, timestamps, at most 224 new tokens per 30 s window) without the temperature-fallback ladder, conditioning on the
-previous window or the VAD filter, and clips are decoded in batches.  Clips of at most 30 s are decoded whole; longer ones
+previous window or the VAD filter, and clips are decoded in batches.  `precision` "float16" and "bfloat16" run every Linear
+on the library's 16-bit kernels (whisper.py); every other compute_type computes in fp32 with TF32 products.  Clips of at most 30 s are decoded whole; longer ones
 follow transformers' long-form generate (30 s windows moved by the predicted timestamps, `WhisperModel.transcribe_long`),
 with the windows of several clips decoded together.  See INTEGRATION.md.
 """
@@ -35,6 +36,14 @@ DEFAULT_MEMORY_BUDGET = 16 << 30
 # share of the budget for a pool of long clips' whole-clip log-mels (fp32 [frames, n_mels]; large-v3: 512 bytes per 10 ms, so
 # 2 GiB of a 16 GiB budget holds about 11.6 hours of audio); the decode batch of long clips takes the rest
 LONG_POOL_SHARE = 1 / 8
+# faster-whisper compute_type values that select the 16-bit Linears.  The others ("float32", "int8*", "default", "auto")
+# are accepted and recorded, and compute in fp32 with TF32 products.
+H16_PRECISIONS = {"float16": torch.float16, "bfloat16": torch.bfloat16}
+
+
+def compute_dtype(precision):
+    """WhisperModel compute type of a compute_type value: torch.float16 / torch.bfloat16, or None (fp32 / TF32)."""
+    return H16_PRECISIONS.get(precision)
 
 
 def read_clip(path, max_seconds=30):
@@ -102,9 +111,11 @@ def long_pools(n16, n_mels, budget=DEFAULT_MEMORY_BUDGET):
 
 class WhisperAsr:
     def __init__(self, model_size: str, language: str, precision: str, model_dir=None, memory_budget=DEFAULT_MEMORY_BUDGET):
-        """model_size and language are validated as the reference does.  precision takes the reference's compute_type values
-        and is recorded only: compute is always fp32 storage with TF32 tensor-core products.  model_dir: the local Hugging
-        Face Whisper directory (default: the directory named model_size)."""
+        """model_size and language are validated as the reference does.  precision takes the reference's compute_type values:
+        "float16" and "bfloat16" run the Linears on the 16-bit kernels (compute_dtype); the others are recorded and compute
+        in fp32 with TF32 tensor-core products.  Cross K/V and the decode slots stay fp32 either way, so the batch size
+        (clips_per_batch) is the same.  model_dir: the local Hugging Face Whisper directory (default: the directory named
+        model_size)."""
         if model_size not in VALID_SIZES:
             raise ValueError(f"Invalid model size: {model_size}")
         if language not in VALID_LANGUAGES:
@@ -121,7 +132,7 @@ class WhisperAsr:
             from tokenizers import Tokenizer
 
             from .whisper import WhisperModel
-            self._loaded = (WhisperModel.from_pretrained(self.model_path, device="cuda"),
+            self._loaded = (WhisperModel.from_pretrained(self.model_path, device="cuda", compute_type=compute_dtype(self.precision)),
                             Tokenizer.from_file(os.path.join(self.model_path, "tokenizer.json")))
         return self._loaded
 

@@ -14,7 +14,7 @@ LIB = os.path.join(HERE, "libevk_sm90.so")
 SOURCES = ["api.cu", "gconv.cu", "gconv_tc.cu", "conv_direct.cu", "mel.cu", "elementwise.cu", "norm_weights.cu", "attention.cu",
            "vq_loss_optim.cu", "flash.cu", "gpt_misc.cu", "gemm_tma.cu", "stft.cu", "pack.cu",
            "sample.cu", "attn64.cu", "conv2d.cu", "lstm.cu", "roformer.cu", "vr_wave.cu", "vq_train.cu", "ssl_prep.cu",
-           "slicer.cu", "mdx23c.cu", "whisper.cu"]
+           "slicer.cu", "mdx23c.cu", "whisper.cu", "linear_h16.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]

@@ -2167,6 +2167,61 @@ def linear_into(x, w: PackedW, y, bias=None, act=ACT_NONE, res=None):
     return y
 
 
+# ---- 16-bit Linears (linear_h16.cu): h(x) . h(W) on fp16 / bf16 tensor cores with fp32 accumulation ------------------
+H16_TYPES = (torch.float16, torch.bfloat16)
+
+
+class PackedH16:
+    """A Linear's weight for the 16-bit kernels: w [N, ldw] fp16 or bf16, ldw = K rounded up to 64, zero past column K."""
+    __slots__ = ("w", "K")
+
+    def __init__(self, w, K):
+        self.w, self.K = w, K
+
+
+def pack_weight_h16(w, dtype):
+    """nn.Linear weight [N, K] -> PackedH16 rounded to `dtype` (torch.float16 or torch.bfloat16) to nearest even, in the
+    layout evk_linear_h16 and evk_linear_rows_h16 read.  A weight that is already exactly 16-bit keeps its bits."""
+    if dtype not in H16_TYPES:
+        raise ValueError(f"16-bit compute type {dtype} (torch.float16 or torch.bfloat16)")
+    N, K = w.shape
+    p = torch.zeros(N, (K + 63) // 64 * 64, dtype=dtype, device=w.device)
+    p[:, :K] = w.detach()
+    return PackedH16(p, K)
+
+
+def _linear_h16(name, x, w: PackedH16, bias, act, res, out):
+    K = x.shape[-1]
+    x2 = x.reshape(-1, K)
+    if x2.stride(1) != 1:
+        x2 = x2.contiguous()
+    rows, N = x2.shape[0], w.w.shape[0]
+    assert K == w.K and x2.dtype == torch.float32 and rows >= 1, (x.shape, w.K, x2.dtype)
+    y = torch.empty(x.shape[:-1] + (N,), device=x.device, dtype=torch.float32) if out is None else out
+    y2 = y.reshape(-1, N) if out is None else out
+    assert y2.shape == (rows, N) and y2.stride(1) == 1, (y2.shape, y2.stride())
+    r2 = None
+    if res is not None:
+        r2 = res.reshape(rows, N)
+        assert r2.stride(1) == 1, r2.stride()
+    _call_f(name, 2.0 * rows * N * K, _p(x2), x2.stride(0), rows, _p(w.w), w.w.shape[1], int(w.w.dtype == torch.bfloat16),
+            _p(bias), _p(r2), r2.stride(0) if r2 is not None else 0, _p(y2), y2.stride(0), N, K, int(act), ctypes.c_float(0.0))
+    return y
+
+
+def linear_h16(x, w: PackedH16, bias=None, act=ACT_NONE, res=None, out=None):
+    """act(h(x) h(W)^T + bias + res) for many rows (evk_linear_h16: the 16-bit wgmma kernel).  x [..., K] fp32 with unit
+    column stride; res shaped like the output; out: a [rows, N] view with unit column stride to write into (column slices of
+    wider buffers), or None.  No gradient."""
+    return _linear_h16("evk_linear_h16", x, w, bias, act, res, out)
+
+
+def linear_rows_h16(x, w: PackedH16, bias=None, act=ACT_NONE, res=None, out=None):
+    """linear_h16 for the few rows of a decode step (evk_linear_rows_h16): any row count, and a row's bits do not depend on
+    how many rows share the launch."""
+    return _linear_h16("evk_linear_rows_h16", x, w, bias, act, res, out)
+
+
 def rope_attn(qkvg, cs, out, heads, L, n_outer, s_outer, n_inner, s_inner, s_tok):
     """evk_rope_attn_fwd: qkvg [rows, ld] token rows [q | k | v | gate logits], cs [L, 32, 2] (cos, sin) -> out [rows, heads*64];
     sequence (u, w) holds rows u*s_outer + w*s_inner + t*s_tok, t < L."""

@@ -17,8 +17,12 @@ at most 30 s, long-form (`transcribe_long`: 30 s windows moved by the predicted 
               clip's seek moves on the host by transformers' _retrieve_segment rules.
 
 Compute is fp32 storage with TF32 tensor-core products in the Linears and the encoder's attention (3xTF32 under
-`evk_set_precise(1)`); the decode attention and the beam step are exact fp32.  Special-token ids come from the generation
-config.  No CPU fallback.
+`evk_set_precise(1)`); the decode attention and the beam step are exact fp32.  With a 16-bit compute type
+(`set_compute_type(torch.float16 / torch.bfloat16)`, faster-whisper's compute_type "float16" / "bfloat16") every Linear
+-- encoder, cross K/V, decode step and head -- runs on the 16-bit kernels instead: weights packed once in 16 bits, activations
+rounded to 16 bits as they are staged, fp32 accumulation and epilogue (evk_linear_h16 for the encoder and the cross K/V
+projection, evk_linear_rows_h16 for the decode step).  Activations, LayerNorm, both attentions, the cross K/V buffer, the
+convs and the beam step stay fp32 as above.  Special-token ids come from the generation config.  No CPU fallback.
 """
 import json
 import os
@@ -111,6 +115,7 @@ class WhisperModel(ParamTree):
         if c["max_source_positions"] != N_CTX or c["num_mel_bins"] % 4:
             raise ValueError("max_source_positions must be 1500 and num_mel_bins a multiple of 4")
         self.cfg, self.gen, self.sp = c, dict(generation_config), special_tokens(generation_config)
+        self.compute_type = None
         if not (self.sp["ts_begin"] + 1501 <= c["vocab_size"] and self.sp["eot"] < self.sp["ts_begin"]):
             raise ValueError("generation config's token layout does not fit the vocabulary")
         for name, shape in self.param_spec(c):
@@ -160,9 +165,22 @@ class WhisperModel(ParamTree):
             raise ValueError("proj_out.weight differs from model.decoder.embed_tokens.weight (untied heads are not supported)")
         return super().load_state_dict({k: v.float() for k, v in sd.items()}, strict=True)
 
+    def set_compute_type(self, dtype):
+        """None: fp32 storage with TF32 products (the default); torch.float16 or torch.bfloat16: every Linear on the 16-bit
+        kernels.  The packed weights and the captured step graphs follow on the next call.  -> self."""
+        if dtype is not None and dtype not in ops.H16_TYPES:
+            raise ValueError(f"compute type {dtype!r} (None, torch.float16 or torch.bfloat16)")
+        self.compute_type = dtype
+        return self
+
+    def weights_key(self):
+        """ParamTree's key and the compute type: a switch repacks the weights and captures the step graphs again."""
+        return super().weights_key() + (str(self.compute_type),)
+
     @classmethod
-    def from_pretrained(cls, path, device="cuda"):
-        """A local Hugging Face directory: config.json, model.safetensors or pytorch_model.bin, generation_config.json."""
+    def from_pretrained(cls, path, device="cuda", compute_type=None):
+        """A local Hugging Face directory: config.json, model.safetensors or pytorch_model.bin, generation_config.json.
+        compute_type: as set_compute_type."""
         for f in ("config.json", "generation_config.json"):
             if not os.path.exists(os.path.join(path, f)):
                 raise FileNotFoundError(os.path.join(path, f))
@@ -176,7 +194,7 @@ class WhisperModel(ParamTree):
         else:
             raise FileNotFoundError(f"no model.safetensors / pytorch_model.bin under {path}")
         net.load_state_dict(sd)
-        return net.to(device).eval()
+        return net.set_compute_type(compute_type).to(device).eval()
 
     # ---- packed operands --------------------------------------------------------------------------------------------------
     def _packed(self):
@@ -184,20 +202,22 @@ class WhisperModel(ParamTree):
         return self.cached("packed", self._pack)
 
     def _pack(self):
-        cfg, P = self.cfg, self.P
-        pk = lambda w: ops.pack_weight(w.detach().contiguous(), None, need_pb=False)   # noqa: E731
+        cfg, P, h16 = self.cfg, self.P, self.compute_type
+        pk32 = lambda w: ops.pack_weight(w.detach().contiguous(), None, need_pb=False)   # noqa: E731
+        # the Linears' operand: the fp32 (TF32) pack, or only the 16-bit one
+        pk = pk32 if h16 is None else lambda w: ops.pack_weight_h16(w, h16)           # noqa: E731
         z = lambda n: torch.zeros(n, device=P("model.encoder.conv1.bias").device)     # noqa: E731
         d = {}
 
-        def lin(name):
-            d[name] = (pk(P(name + ".weight")), P(name + ".bias").detach())
+        def lin(name, pack=pk):
+            d[name] = (pack(P(name + ".weight")), P(name + ".bias").detach())
 
         def qkv(p):
             w = torch.cat([P(p + n + ".weight") for n in ("q_proj", "k_proj", "v_proj")])
             d[p + "qkv"] = (pk(w), torch.cat([P(p + "q_proj.bias"), z(cfg["d_model"]), P(p + "v_proj.bias")]).detach())
 
-        lin("model.encoder.conv1")
-        lin("model.encoder.conv2")
+        lin("model.encoder.conv1", pk32)
+        lin("model.encoder.conv2", pk32)
         for i in range(cfg["encoder_layers"]):
             p = f"model.encoder.layers.{i}."
             qkv(p + "self_attn.")
@@ -220,6 +240,14 @@ class WhisperModel(ParamTree):
 
     def _ln(self, x, name):
         return ops.whisper_layernorm(x, self.P(name + ".weight"), self.P(name + ".bias"), eps=1e-5)
+
+    def _linear(self, x, wb, act=ops.ACT_NONE, res=None, rows=False):
+        """One Linear of the packed (w, b) on the compute type's kernels: TF32 (ops.linear), or 16 bits with the row kernel for
+        the decode step (rows=True) and the wgmma kernel otherwise."""
+        w, b = wb
+        if self.compute_type is None:
+            return ops.linear(x, w, b, act=act, res=res)
+        return (ops.linear_rows_h16 if rows else ops.linear_h16)(x, w, b, act=act, res=res)
 
     # ---- front end and encoder --------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -261,21 +289,21 @@ class WhisperModel(ParamTree):
         H = c["encoder_attention_heads"]
         for i in range(c["encoder_layers"]):
             p = f"model.encoder.layers.{i}."
-            w, b = pk[p + "self_attn.qkv"]
-            a = ops.attention_pad(ops.linear(self._ln(x, p + "self_attn_layer_norm"), w, b), heads=H, lens=lens, scale=0.125)
-            w, b = pk[p + "self_attn.out_proj"]
-            x = ops.linear(a, w, b, res=x)
-            w, b = pk[p + "fc1"]
-            f = ops.linear(self._ln(x, p + "final_layer_norm"), w, b, act=ops.ACT_GELU)
-            w, b = pk[p + "fc2"]
-            x = ops.linear(f, w, b, res=x)
+            qkv = self._linear(self._ln(x, p + "self_attn_layer_norm"), pk[p + "self_attn.qkv"])
+            a = ops.attention_pad(qkv, heads=H, lens=lens, scale=0.125)
+            x = self._linear(a, pk[p + "self_attn.out_proj"], res=x)
+            f = self._linear(self._ln(x, p + "final_layer_norm"), pk[p + "fc1"], act=ops.ACT_GELU)
+            x = self._linear(f, pk[p + "fc2"], res=x)
         return self._ln(x, "model.encoder.layer_norm")
 
     @torch.no_grad()
     def cross_kv(self, enc, out):
         """Writes out [B * 1500, decoder_layers * 2 * d_model]: layer l's K at columns 2 d l, V at 2 d l + d."""
         w, b = self._packed()["cross_kv"]
-        return ops.linear_into(enc.reshape(-1, enc.shape[-1]).contiguous(), w, out, b)
+        x = enc.reshape(-1, enc.shape[-1]).contiguous()
+        if self.compute_type is None:
+            return ops.linear_into(x, w, out, b)
+        return ops.linear_h16(x, w, b, out=out)
 
     # ---- decoding ---------------------------------------------------------------------------------------------------------
     def _state(self, clips, beam, dev):
@@ -301,23 +329,17 @@ class WhisperModel(ParamTree):
                               self.P("model.decoder.embed_positions.weight").detach(), st["pos"], st["x"])
         for i in range(c["decoder_layers"]):
             p = f"model.decoder.layers.{i}."
-            w, b = pk[p + "self_attn.qkv"]
-            qkv = ops.linear(self._ln(x, p + "self_attn_layer_norm"), w, b)
+            qkv = self._linear(self._ln(x, p + "self_attn_layer_norm"), pk[p + "self_attn.qkv"], rows=True)
             pool = st["pool"][:, 2 * d * i:]
             ops.whisper_self_kv(qkv, pool, st["tab"], st["pos"], S)
             a = ops.whisper_attn(qkv, pool, d, H, torch.empty(R, d, device=x.device), tab=st["tab"], pos=st["pos"], n_keys=S)
-            w, b = pk[p + "self_attn.out_proj"]
-            x = ops.linear(a, w, b, res=x)
-            w, b = pk[p + "encoder_attn.q_proj"]
-            q = ops.linear(self._ln(x, p + "encoder_attn_layer_norm"), w, b)
+            x = self._linear(a, pk[p + "self_attn.out_proj"], res=x, rows=True)
+            q = self._linear(self._ln(x, p + "encoder_attn_layer_norm"), pk[p + "encoder_attn.q_proj"], rows=True)
             a = ops.whisper_attn(q, st["ckv"][:, 2 * d * i:], d, H, torch.empty(R, d, device=x.device), n_keys=N_CTX, nq=beam)
-            w, b = pk[p + "encoder_attn.out_proj"]
-            x = ops.linear(a, w, b, res=x)
-            w, b = pk[p + "fc1"]
-            f = ops.linear(self._ln(x, p + "final_layer_norm"), w, b, act=ops.ACT_GELU)
-            w, b = pk[p + "fc2"]
-            x = ops.linear(f, w, b, res=x)
-        return ops.linear(self._ln(x, "model.decoder.layer_norm"), pk["head"])
+            x = self._linear(a, pk[p + "encoder_attn.out_proj"], res=x, rows=True)
+            f = self._linear(self._ln(x, p + "final_layer_norm"), pk[p + "fc1"], act=ops.ACT_GELU, rows=True)
+            x = self._linear(f, pk[p + "fc2"], res=x, rows=True)
+        return self._linear(self._ln(x, "model.decoder.layer_norm"), (pk["head"], None), rows=True)
 
     def _layout(self, plen, max_new_tokens):
         sp = self.sp

@@ -442,6 +442,29 @@ int evk_sinepos_bwd(const float* dy, int32_t ldy, int64_t dy_sb, const float* pe
  * act: EVK_ACT_NONE / RELU / LRELU. */
 int evk_gemv_rows(const float* x, int32_t ldx, int32_t rows, const float* W, int32_t ldw, const float* bias, float* y,
                   int32_t ldy, int32_t N, int32_t C, int32_t act, float slope, evk_stream_t stream);
+/* 16-bit Linears (csrc/linear_h16.cu; Whisper's float16 / bfloat16 compute types).  Numerical contract:
+ *   y[r][n] = act( sum_k h(x[r][k]) * h(W[n][k]) + bias[n] + res[r][n] )
+ * h = round to nearest even to fp16 (bf16 == 0) or bf16 (bf16 != 0): applied to the fp32 activations as they are staged
+ * (cvt.rn; values beyond fp16's range become +-inf as that cast makes them) and to the weight once, when it is packed.
+ * The products are formed on tensor cores and accumulated in fp32; a product of two fp16 or two bf16 values is exact in
+ * fp32, so only the accumulation rounds.  The epilogue (bias, res, act) is fp32, in that order.  evk_set_precise has no
+ * effect here: the operands are already exact.  Each output has one K order whatever `rows` is, so a row's bits never depend
+ * on its neighbours or on how many rows share the launch.
+ * W: the packed weight [N][ldw] 16-bit (fp16 or bf16 bits as selected), ldw % 64 == 0, ldw >= K, columns K .. ldw - 1 zero,
+ * 16-byte aligned (ops.pack_weight_h16).  x [rows][ldx] fp32, ldx >= K (columns past K are never read); y [rows][ldy];
+ * res [rows][ldr] or null; bias [N] or null; act: any evk_act (slope for LRELU).  Both entry points take the same operands.
+ *   evk_linear_rows_h16: the few rows of a decode step, any row count (mma.sync.m16n8k16).  Each CTA streams its slice of W
+ *     once per 128 rows; the K range is split over CTAs by (N, K) alone, and the splits' fp32 partials are added in split
+ *     order (library scratch).
+ *   evk_linear_h16: many rows (wgmma.m64n128k16 from TMA-loaded shared memory): x is first cast to 16 bits in library
+ *     scratch ([rows][K rounded up to 8]).  No K split.  rows <= 65535 * 128.
+ * The two entry points may differ from each other in the last bits of a sum (their K orders differ). */
+int evk_linear_rows_h16(const float* x, int32_t ldx, int32_t rows, const void* w, int32_t ldw, int32_t bf16, const float* bias,
+                        const float* res, int32_t ldr, float* y, int32_t ldy, int32_t N, int32_t K, int32_t act, float slope,
+                        evk_stream_t stream);
+int evk_linear_h16(const float* x, int32_t ldx, int32_t rows, const void* w, int32_t ldw, int32_t bf16, const float* bias,
+                   const float* res, int32_t ldr, float* y, int32_t ldy, int32_t N, int32_t K, int32_t act, float slope,
+                   evk_stream_t stream);
 /* KV-cache attention of one new token -- T2SBlock.decode_next_token (t2s_model.py:203-221), F.scaled_dot_product_attention
  * without mask -- with the position in DEVICE memory, so that a decode step replays as a CUDA graph.  qkv: the in_proj outputs
  * [q | k | v] (3 * H * 32 floats per row, pitch ld, batch stride `batch_stride`) of the positions so far; *n_prev_dev = rows

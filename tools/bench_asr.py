@@ -18,7 +18,12 @@ to end, the device-time split (whole-clip front end, encoder, decode), peak memo
 long-form `generate` (attention_mask, temperature 0, logprob / no-speech thresholds) on the same features, fp32 with TF32 and
 fp16, batched.
 
-Usage:  python tools/bench_asr.py [--clips 256] [--compare-clips 16] [--no-compare]
+--precision float16|bfloat16: the short-form measurement twice for each of the fp32 (TF32) and the 16-bit compute type on
+one model, alternating fp32, 16-bit, fp32, 16-bit in the same process.  Each arm adds the Linears' device time in one profiled
+eager decode step, their share of the step and the floor of that time: the step's Linear weight bytes (shapes below) over
+3.35 TB/s of HBM3.
+
+Usage:  python tools/bench_asr.py [--clips 256] [--compare-clips 16] [--no-compare] [--precision float16|bfloat16]
         python tools/bench_asr.py --long [--clips 8] [--tokens-per-window 120] [--no-compare]
 """
 import argparse
@@ -84,6 +89,15 @@ def encoder_flops(c):
     return conv + c["encoder_layers"] * layer
 
 
+def step_linear_bytes(c, elem):
+    """Weight bytes the decode step's Linears read once each: per layer QKV (3 d^2), out, cross-q, cross-out (d^2 each),
+    fc1 and fc2 (d * ffn each), and the tied head (V * d)."""
+    d, f = c["d_model"], c["decoder_ffn_dim"]
+    return elem * (c["decoder_layers"] * (6 * d * d + 2 * d * f) + c["vocab_size"] * d)
+
+
+HBM_BYTES_PER_S = 3.35e12          # H100 SXM data sheet
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--clips", type=int, default=256)
@@ -93,6 +107,7 @@ def main():
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--long", action="store_true")
     ap.add_argument("--tokens-per-window", type=int, default=120)
+    ap.add_argument("--precision", choices=["float16", "bfloat16"], default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_asr needs a GPU")
@@ -139,7 +154,8 @@ def main():
             timing["decode"] += ev[2].elapsed_time(ev[3])
         return out
 
-    with torch.no_grad():
+    @torch.no_grad()
+    def measure():
         for bt in batches:                                          # warm up: capture the step of every token budget
             run(bt)
         torch.cuda.synchronize()
@@ -166,17 +182,31 @@ def main():
         lg = net._forward_rows(st)
         ops.whisper_beam_step(lg, st, 5, net._layout(3, 224))
         prof = ops.profile_end()
-    step_ms = sum(v["ms"] for v in prof.values())
-    beam_ms = prof.get("evk_whisper_beam_step", {}).get("ms", 0.0)
-    ckv_ms = ckv_ms_batch * len(xs) / len(bt)
-    res = dict(metric="whisper large-v3-shaped transcription audio-seconds/s", card=card(), clips=len(xs),
-               audio_s=sum(secs), tokens_per_second_of_audio=a.tokens_per_second, clips_per_batch=nb,
-               value=sum(secs) / wall, wall_s=wall, peak_mem_gib=peak,
-               device_ms=dict(front_end=timing["front"], encoder=timing["encoder"], cross_kv_est=ckv_ms,
-                              decode_incl_cross_kv=timing["decode"], beam_step_share_of_eager_step=beam_ms / step_ms if step_ms else None,
-                              eager_step_by_call={k: round(v["ms"], 3) for k, v in sorted(prof.items(), key=lambda kv: -kv[1]["ms"])[:8]}),
-               encoder_tflops=encoder_flops(cfg) * len(xs) / (timing["encoder"] * 1e-3) / 1e12,
-               generated_tokens=sum(len(t["tokens"]) for t in toks))
+        step_ms = sum(v["ms"] for v in prof.values())
+        lin_ms = sum(v["ms"] for k, v in prof.items() if k.startswith(("evk_gconv_fwd", "evk_linear")))
+        beam_ms = prof.get("evk_whisper_beam_step", {}).get("ms", 0.0)
+        ckv_ms = ckv_ms_batch * len(xs) / len(bt)
+        elem = 4 if net.compute_type is None else 2
+        return dict(metric="whisper large-v3-shaped transcription audio-seconds/s", card=card(), clips=len(xs),
+                    audio_s=sum(secs), tokens_per_second_of_audio=a.tokens_per_second, clips_per_batch=nb,
+                    value=sum(secs) / wall, wall_s=wall, peak_mem_gib=peak,
+                    device_ms=dict(front_end=timing["front"], encoder=timing["encoder"], cross_kv_est=ckv_ms,
+                                   decode_incl_cross_kv=timing["decode"], beam_step_share_of_eager_step=beam_ms / step_ms if step_ms else None,
+                                   eager_step_by_call={k: round(v["ms"], 3) for k, v in sorted(prof.items(), key=lambda kv: -kv[1]["ms"])[:8]}),
+                    encoder_tflops=encoder_flops(cfg) * len(xs) / (timing["encoder"] * 1e-3) / 1e12,
+                    generated_tokens=sum(len(t["tokens"]) for t in toks), compute_type=str(net.compute_type),
+                    eager_step_ms=step_ms, step_linear_ms=lin_ms, step_linear_share=lin_ms / step_ms if step_ms else None,
+                    step_linear_floor_ms=step_linear_bytes(cfg, elem) / HBM_BYTES_PER_S * 1e3)
+
+    if a.precision is None:
+        res = measure()
+    else:
+        h16 = asr.compute_dtype(a.precision)
+        arms = []
+        for dt in (None, h16, None, h16):
+            net.set_compute_type(dt)
+            arms.append(measure())
+        res = dict(arms[-1], arms=arms)
     if not a.no_compare:
         res["transformers"] = compare(net, cfg, gen, xs[:a.compare_clips], budget[:a.compare_clips], nb, feats_of, dev)
     print(json.dumps(res))
