@@ -1,5 +1,8 @@
 // Stage-1 AR GPT odds and ends: sinusoidal position add (embedding.py:36-81), summed cross-entropy + top-k accuracy
 // (t2s_model.py:486-489), and ScaledAdam (optim.py:123-622) over one flat fp32 arena.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include "evk_common.cuh"
 #include "gemv_route.h"
 
@@ -374,6 +377,102 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const float* __restric
   }
 }
 
+// ---- 16-bit KV cache: append this token's k and v and attend, one launch (evk_attn_decode_h16) -------------------------------
+// Cache rows hold [k | v] (2 * H * 32 16-bit values, pitch ld, batch stride sb), no q.  The CTA of (head h, item b) rounds the
+// head's 32 k and 32 v values of the step's fp32 in_proj row to nearest even, stores them at row *n_dev (its own 64 values only,
+// so CTAs do not depend on each other) and then attends keys 0 .. *n_dev exactly as attn_decode_kernel does: the same key
+// order per thread, fp32 q * scale, fp32 scores, online softmax and P V on the widened (exact) 16-bit k and v.  The cache is
+// read with ordinary loads: the row written above is read back by other threads of the CTA after the barrier.
+template <bool BF16>
+__device__ __forceinline__ float h16_to_f(uint32_t bits) {
+  return BF16 ? __uint_as_float(bits << 16) : __half2float(__ushort_as_half((unsigned short)bits));
+}
+
+template <bool BF16>
+__device__ __forceinline__ void widen8(const uint4 u, float* f) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    f[2 * i] = h16_to_f<BF16>(w[i] & 0xffffu);
+    f[2 * i + 1] = h16_to_f<BF16>(w[i] >> 16);
+  }
+}
+
+template <bool BF16>
+__global__ void __launch_bounds__(128) attn_decode_h16_kernel(const float* __restrict__ row, int ldr, uint16_t* cache, long long sb,
+                                                               int ld, const int* __restrict__ n_dev, const int* __restrict__ skip,
+                                                               int H, float scale, float* __restrict__ out, int ldo) {
+  const int n = *n_dev + 1;                                      // keys 0 .. *n_dev
+  const int h = blockIdx.x, b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int s0 = skip ? skip[2 * b] : n, gap = skip ? skip[2 * b + 1] - s0 : 0;
+  const int D = H * 32;
+  const float* r = row + (long long)b * ldr;
+  uint16_t* base = cache + (long long)b * sb;
+  if (threadIdx.x < 64) {                                        // k of head h (threads 0..31), then its v (32..63)
+    const int part = threadIdx.x >> 5;
+    const float v = r[(1 + part) * D + h * 32 + lane];
+    base[(long long)(n - 1) * ld + part * D + h * 32 + lane] =
+        BF16 ? __bfloat16_as_ushort(__float2bfloat16_rn(v)) : __half_as_ushort(__float2half_rn(v));
+  }
+  float q[32];
+  {
+    const float4* qp = reinterpret_cast<const float4*>(r + h * 32);
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      const float4 t = __ldg(qp + c);
+      q[4 * c] = t.x * scale; q[4 * c + 1] = t.y * scale; q[4 * c + 2] = t.z * scale; q[4 * c + 3] = t.w * scale;
+    }
+  }
+  __syncthreads();                                               // the appended key is visible to every thread of the CTA
+  float m = -INFINITY, l = 0.f, acc[32];
+#pragma unroll
+  for (int c = 0; c < 32; ++c) acc[c] = 0.f;
+  for (int t = threadIdx.x; t < n - gap; t += 128) {
+    const int j = t < s0 ? t : t + gap;
+    const uint4* kp = reinterpret_cast<const uint4*>(base + (long long)j * ld + h * 32);
+    const uint4* vp = reinterpret_cast<const uint4*>(base + (long long)j * ld + D + h * 32);
+    uint4 ku[4], vu[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) ku[c] = kp[c];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) vu[c] = vp[c];
+    float kf[32], vf[32];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) { widen8<BF16>(ku[c], kf + 8 * c); widen8<BF16>(vu[c], vf + 8 * c); }
+    float s = 0.f;
+#pragma unroll
+    for (int c = 0; c < 8; ++c)
+      s = fmaf(q[4 * c], kf[4 * c], fmaf(q[4 * c + 1], kf[4 * c + 1], fmaf(q[4 * c + 2], kf[4 * c + 2], fmaf(q[4 * c + 3], kf[4 * c + 3], s))));
+    const float mn = fmaxf(m, s);
+    const float c0 = expf(m - mn), p = expf(s - mn);             // m = -inf on the first key: c0 = 0
+    l = l * c0 + p;
+#pragma unroll
+    for (int c = 0; c < 32; ++c) acc[c] = fmaf(acc[c], c0, p * vf[c]);
+    m = mn;
+  }
+  __shared__ float sm_m[4], sm_r[4][33];
+  float M = m;
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) M = fmaxf(M, __shfl_xor_sync(0xffffffffu, M, o));
+  if (lane == 0) sm_m[warp] = M;
+  __syncthreads();
+  M = fmaxf(fmaxf(sm_m[0], sm_m[1]), fmaxf(sm_m[2], sm_m[3]));
+  const float f = (m == -INFINITY) ? 0.f : expf(m - M);          // threads without a key contribute nothing
+  l = warp_sum(l * f);
+#pragma unroll
+  for (int c = 0; c < 32; ++c) {
+    const float t = warp_sum(acc[c] * f);
+    if (lane == c) sm_r[warp][c] = t;
+  }
+  if (lane == 0) sm_r[warp][32] = l;
+  __syncthreads();
+  if (warp == 0) {
+    const float Ls = sm_r[0][32] + sm_r[1][32] + sm_r[2][32] + sm_r[3][32];
+    const float A = sm_r[0][lane] + sm_r[1][lane] + sm_r[2][lane] + sm_r[3][lane];
+    out[(long long)b * ldo + h * 32 + lane] = A / Ls;
+  }
+}
+
 // Skinny product of the AR token step:  y[r][n] = act(sum_c x[r][c] * W[n][c] + bias[n]),  R <= 64 rows.
 // A one-row "GEMM" is a stream over the weight matrix (12.6 MB per GPT layer): through the 128-row tensor-core tiles it ran on
 // N/128 = 4..16 CTAs with one barrier round trip per 32 channels (25..100 us per Linear, 9.3 ms per token).  Here KS warps share
@@ -608,6 +707,23 @@ extern "C" int evk_attn_decode_dev(const float* qkv, int64_t batch_stride, int32
   EVK_REQUIRE(ld % 4 == 0 && batch_stride % 4 == 0 && ((uintptr_t)qkv % 16) == 0, EVK_ERR_ARG, "attn_decode_dev: rows must be 16-byte aligned");
   attn_decode_kernel<<<dim3(H, B), 128, 0, st>>>(qkv, batch_stride, ld, n_prev_dev, skip, H, scale, out, ldo);
   return check_launch("attn_decode_dev");
+}
+
+extern "C" int evk_attn_decode_h16(const float* row, int32_t ldr, void* cache, int64_t batch_stride, int32_t ld, int32_t bf16,
+                                   const int32_t* n_prev_dev, const int32_t* skip, int32_t B, int32_t H, float scale, float* out,
+                                   int32_t ldo, cudaStream_t st) {
+  EVK_REQUIRE(row && cache && out && n_prev_dev && B >= 1 && H >= 1, EVK_ERR_ARG, "attn_decode_h16: bad arguments");
+  EVK_REQUIRE(ldr >= 3 * H * 32 && ld >= 2 * H * 32 && ldo >= H * 32, EVK_ERR_ARG,
+              "attn_decode_h16: pitches %d (row) / %d (cache) / %d (out) too small for %d heads of 32", ldr, ld, ldo, H);
+  EVK_REQUIRE(ldr % 4 == 0 && ((uintptr_t)row % 16) == 0 && ld % 8 == 0 && batch_stride % 8 == 0 && ((uintptr_t)cache % 16) == 0,
+              EVK_ERR_ARG, "attn_decode_h16: the fp32 row and the 16-bit cache rows must be 16-byte aligned");
+  if (bf16)
+    attn_decode_h16_kernel<true><<<dim3(H, B), 128, 0, st>>>(row, ldr, static_cast<uint16_t*>(cache), batch_stride, ld, n_prev_dev,
+                                                             skip, H, scale, out, ldo);
+  else
+    attn_decode_h16_kernel<false><<<dim3(H, B), 128, 0, st>>>(row, ldr, static_cast<uint16_t*>(cache), batch_stride, ld, n_prev_dev,
+                                                              skip, H, scale, out, ldo);
+  return check_launch("attn_decode_h16");
 }
 
 extern "C" int evk_cache_append(const float* row, int32_t ldr, float* cache, int64_t batch_stride, int32_t ld, const int32_t* pos_dev,

@@ -13,6 +13,19 @@ Execution is channels-last [B, L, D] fp32 throughout:
 The reference hard-codes dropout 0.1 in the positional embeddings, attention probabilities and the three layer
 dropouts even though configs/gpt.yaml says `dropout: 0` (t2s_model.py:276-293); `layer_dropout` reproduces that
 (default 0.1) and can be set to 0 for parity runs.
+
+AR decoding (the infer_panel* methods and decode_groups) runs in fp32 by default.  set_compute_type(torch.float16 /
+torch.bfloat16) -- the reference's `is_half` -- puts it on 16 bits, with this numerical contract:
+  Linears (bert_proj, in_proj, out_proj, linear1 + ReLU, linear2, head)   y = epi(sum_k h(x_k) h(W_nk)): h rounds to nearest even
+                                                                         to fp16 / bf16, fp32 accumulation and epilogue
+                                                                         (ops.linear_h16 in the prompt pass, ops.linear_rows_h16
+                                                                         in the token step)
+  K/V cache                                                              h of the fp32 in_proj output, stored once ([k | v], no
+                                                                         q: a third of the fp32 cache's bytes) and read by every
+                                                                         later step (ops.attn_decode_h16)
+  prompt-pass attention                                                  the unrounded fp32 qkv, as in fp32 mode
+  q, scores, softmax, P V, LayerNorm, residuals, embeddings, the sampler  fp32
+Training ignores the compute type.
 """
 import math
 
@@ -84,6 +97,34 @@ class Text2SemanticDecoder(ParamTree):
             self._register(p + "norm2.bias", torch.zeros(D))
         self._register("ar_predict_layer.weight", uni((self.vocab_size, D), 1 / math.sqrt(D)))
         self._pe = None
+        self.compute_type = None
+
+    def set_compute_type(self, dtype):
+        """Compute type of AR decoding (every infer_panel* method and decode_groups).  None: fp32 (the default; exact fp32 token
+        step, TF32 prompt pass).  torch.float16 or torch.bfloat16: the decoder's Linears -- bert_proj, in_proj, out_proj,
+        linear1, linear2 and the head -- on the 16-bit kernels (ops.linear_h16 in the prompt pass, ops.linear_rows_h16 in the
+        token step), and a 16-bit K/V cache (ops.attn_decode_h16).  The parameters stay fp32 and state_dict() does not change;
+        the 16-bit packs, the decoding state and its step graphs follow on the next call.  Training (forward, forward_old and
+        DPO) ignores the compute type.  Anything else raises ValueError.  -> self."""
+        if dtype is not None and dtype not in ops.H16_TYPES:
+            raise ValueError(f"compute type {dtype!r} (None, torch.float16 or torch.bfloat16)")
+        if dtype != self.compute_type:
+            self.__dict__.get("_cached", {}).pop("h16", None)           # the 16-bit packs of the previous type are not read again
+        self.compute_type = dtype
+        return self
+
+    def weights_key(self):
+        """ParamTree's key and the compute type: a switch repacks the weights and rebuilds the decoding state and its graphs."""
+        return super().weights_key() + (str(self.compute_type),)
+
+    def _h16(self):
+        """The 16-bit packs of the decoding Linears ({prefix: ops.PackedH16}), made once per weights_key()."""
+        def build():
+            names = ["bert_proj", "ar_predict_layer"] + [f"h.layers.{i}.{n}" for i in range(self.num_layers)
+                                                         for n in ("self_attn.in_proj", "self_attn.out_proj", "linear1", "linear2")]
+            return {n: ops.pack_weight_h16(self.P(n + ("_weight" if n.endswith("in_proj") else ".weight")), self.compute_type)
+                    for n in names}
+        return self.cached("h16", build)
 
     def pe(self, length, device):
         if self._pe is None or self._pe.shape[0] < length or self._pe.device != device:
@@ -131,9 +172,12 @@ class Text2SemanticDecoder(ParamTree):
         Vp = (self.vocab_size + 3) // 4 * 4
         return ops.linear(hy, self.w("ar_predict_layer", pad0=Vp))
 
-    def _embed_text(self, x, bert_feature, bert_channels_last):
+    def _embed_text(self, x, bert_feature, bert_channels_last, h16=None):
+        """h16: None (TF32 bert_proj), or the 16-bit packs of decoding (_h16)."""
         bert_cl = bert_feature if bert_channels_last else ops.to_channels_last(bert_feature)
         xe = ops.embedding(self.P("ar_text_embedding.word_embeddings.weight"), x.to(torch.int64))
+        if h16 is not None:
+            return ops.linear_h16(bert_cl, h16["bert_proj"], self.b("bert_proj"), res=xe)
         return ops.linear(bert_cl, self.w("bert_proj", need_pb=False), self.b("bert_proj"), res=xe)
 
     def forward(self, x, x_lens, y, y_lens, bert_feature, reject=None, bert_channels_last=False, count=None):
@@ -188,21 +232,49 @@ class Text2SemanticDecoder(ParamTree):
         (per-row lengths xl / yl), cache rows 0..L-1 filled (T2SBlock.process_prompt, t2s_model.py:121-185).  Token step (n_dev an
         int32 device scalar, so the step can be a replayed CUDA graph): h [B, 1, D], its in_proj row is appended to the cache at
         *n_dev and attends every cached position (decode_next_token, :187-221); row b leaves out its text padding
-        skip[b, 0] .. skip[b, 1] - 1, and the Linears run on ops.linear_rows (exact fp32 for up to 64 rows)."""
+        skip[b, 0] .. skip[b, 1] - 1, and the Linears run on ops.linear_rows (exact fp32 for up to 64 rows).
+        Under a 16-bit compute type the Linears run on ops.linear_h16 / ops.linear_rows_h16, cache rows hold the 16-bit [k | v]
+        (the prompt pass casts them, round to nearest even; the token step appends and attends in ops.attn_decode_h16), and the
+        prompt pass's attention still reads the fp32 qkv."""
         p = f"h.layers.{i}."
-        H = self.num_head
-        lin = ops.linear if n_dev is None else ops.linear_rows
-        qkv = lin(h, self.w(p + "self_attn.in_proj", suffix="_weight"), self.P(p + "self_attn.in_proj_bias"))
-        if n_dev is None:
-            cache[:, :qkv.shape[1]].copy_(qkv)
-            a = ops.flash_attention(qkv, heads=H, prefix=X, xlen=xl, ylen=yl, p_drop=0.0, tag=f"gpt.infer{i}")
+        H, D = self.num_head, self.model_dim
+        if self.compute_type is None:
+            lin32 = ops.linear if n_dev is None else ops.linear_rows
+
+            def lin(x, name, bias, act=ops.ACT_NONE, suffix=".weight"):
+                return lin32(x, self.w(p + name, suffix=suffix), bias, act=act)
         else:
+            w16, lin16 = self._h16(), ops.linear_h16 if n_dev is None else ops.linear_rows_h16
+
+            def lin(x, name, bias, act=ops.ACT_NONE, suffix=None):
+                return lin16(x, w16[p + name], bias, act=act)
+        qkv = lin(h, "self_attn.in_proj", self.P(p + "self_attn.in_proj_bias"), suffix="_weight")
+        if n_dev is None:
+            cache[:, :qkv.shape[1]].copy_(qkv if self.compute_type is None else qkv[..., D:])
+            a = ops.flash_attention(qkv, heads=H, prefix=X, xlen=xl, ylen=yl, p_drop=0.0, tag=f"gpt.infer{i}")
+        elif self.compute_type is None:
             a = ops.attn_decode_dev(cache, n_dev, H, qkv, skip)
-        a = lin(a, self.w(p + "self_attn.out_proj"), self.b(p + "self_attn.out_proj"))
+        else:
+            a = ops.attn_decode_h16(cache, n_dev, H, qkv, skip)
+        a = lin(a, "self_attn.out_proj", self.b(p + "self_attn.out_proj"))
         h = ops.layernorm(h, self.P(p + "norm1.weight"), self.P(p + "norm1.bias"), res=a)
-        f = lin(h, self.w(p + "linear1"), self.b(p + "linear1"), act=ops.ACT_RELU)
-        f = lin(f, self.w(p + "linear2"), self.b(p + "linear2"))
+        f = lin(h, "linear1", self.b(p + "linear1"), act=ops.ACT_RELU)
+        f = lin(f, "linear2", self.b(p + "linear2"))
         return ops.layernorm(h, self.P(p + "norm2.weight"), self.P(p + "norm2.bias"), res=f)
+
+    def _head(self, st):
+        """The vocabulary projection's packed weight for the logits buffer of `st`: fp32 padded to its width, or 16-bit."""
+        if self.compute_type is None:
+            return self.w("ar_predict_layer", pad0=st["logits"].shape[1])
+        return self._h16()["ar_predict_layer"]
+
+    def _head_into(self, h, head, out):
+        """out [B, Vp] (rows of st["logits"]) = the logits of h [B, 1, D] on the token step's row kernel (16-bit: the V columns
+        are written in place, the padding is left as it is)."""
+        if self.compute_type is None:
+            out.copy_(ops.linear_rows(h, head).view(out.shape))
+        else:
+            ops.linear_rows_h16(h, head, out=out[:, :self.vocab_size])
 
     @torch.no_grad()
     def infer_panel_naive(self, x, x_lens, prompts, bert_feature, top_k=-100, top_p=100, early_stop_num=-1, temperature=1.0,
@@ -272,8 +344,8 @@ class Text2SemanticDecoder(ParamTree):
         return y_list, idx_list
 
     def _batch_state(self, dev, B, need_rows):
-        """Per-layer caches [B, rows, 3 D] and the static buffers / graphs of the batched token step, kept across calls while the
-        parameters, B and the capacity allow.  There are two: one for B = 1, its capacity rounded up to 512 rows so that single
+        """Per-layer caches [B, rows, 3 D] fp32 ([q | k | v]; under a 16-bit compute type [B, rows, 2 D] 16-bit [k | v]) and
+        the static buffers / graphs of the batched token step, kept across calls while the parameters, B and the capacity allow.  There are two: one for B = 1, its capacity rounded up to 512 rows so that single
         utterances of varying length rarely rebuild it, and one for B > 1, rounded up to 64 rows (a new B frees the previous one
         first).  Calls with one row and calls with several therefore do not rebuild each other's state.  The graphs hold the
         packed weights and the precise mode's kernels, so a new weights_key() rebuilds the state."""
@@ -285,11 +357,13 @@ class Text2SemanticDecoder(ParamTree):
         self.__dict__.pop(key, None)
         rows = (need_rows + unit - 1) // unit * unit
         D, V, Vp = self.model_dim, self.vocab_size, (self.vocab_size + 3) // 4 * 4
+        ct = self.compute_type
 
         def z(*shape, dtype=torch.float32):
             return torch.zeros(shape, device=dev, dtype=dtype)
         st = dict(wkey=wkey, dev=dev, B=B, rows=rows, graphs={},
-                  caches=[torch.empty((B, rows, 3 * D), device=dev, dtype=torch.float32) for _ in range(self.num_layers)],
+                  caches=[torch.empty((B, rows, 3 * D if ct is None else 2 * D), device=dev, dtype=ct or torch.float32)
+                          for _ in range(self.num_layers)],
                   n=z(1, dtype=torch.int32), x=z(B, 1, D), logits=z(B, Vp), skip=z(B, 2, dtype=torch.int32),
                   hist=z(B, rows, dtype=torch.int64), seen=z(B, (V + 31) // 32, dtype=torch.int32), fin=z(B, 2, dtype=torch.int32),
                   icfg=z(6, dtype=torch.int64), fcfg=z(3), pe=self.pe(rows, dev),
@@ -321,7 +395,7 @@ class Text2SemanticDecoder(ParamTree):
             h = st["x"]
             for i in range(self.num_layers):
                 h = self._infer_layer(i, h, st["caches"][i], st["n"], skip=st["skip"])
-            st["logits"].copy_(ops.linear_rows(h, head).view(st["logits"].shape))
+            self._head_into(h, head, st["logits"])
             st["n"].add_(1)
         # warm-up and capture with every row marked finished (the sampler is then a no-op) at position 0 with nothing skipped;
         # the caller overwrites all of it before the first replay
@@ -447,7 +521,7 @@ class Text2SemanticDecoder(ParamTree):
             or at idx + 1 > early_stop_num (!= -1) or idx == max_steps - 1 (fin (idx, idx)).
         The caches hold max_len + Yp + min(max_steps, early_stop_num + 1) + INFER_BATCH_K rows of 3 * 512 floats per layer and
         row (_batch_state rounds this up): 24 layers x B x rows x 6 KiB, e.g. 1.4 GiB for B = 16, max_len 120, Yp 150,
-        early_stop_num 300 (640 rows).  Batches of more than 64 rows run in chunks of 64 (the row Linears take 64 rows per
+        early_stop_num 300 (640 rows); under a 16-bit compute type 2 * 512 16-bit values (2 KiB) per layer and row.  Batches of more than 64 rows run in chunks of 64 (the row Linears take 64 rows per
         launch).  `trace` (a list, tests) receives the raw [B, V] logits of every step."""
         B = len(rows)
         if B > 64:
@@ -470,7 +544,7 @@ class Text2SemanticDecoder(ParamTree):
                     xp[b, :rows[b].shape[0]] = rows[b]
                     bp[b, :, :rows[b].shape[0]] = bert[b]
                 st = self._batch_state(dev, B, L0 + cap + INFER_BATCH_K)
-                head = self.w("ar_predict_layer", pad0=st["logits"].shape[1])
+                head = self._head(st)
                 graph = self._batch_step_graph(st, head, eos_steps)
                 y = torch.zeros((B, 0), device=dev, dtype=torch.int64) if prompts is None else prompts.to(torch.int64)
                 self._prompt_pass(st, head, 0, xp, lens, bp, y, max_len, prompts is not None)
@@ -487,10 +561,10 @@ class Text2SemanticDecoder(ParamTree):
         alone, :796-803): text xp [B, max_len] (bert bp [B, 1024, max_len]; row b's first lens[b] positions are text) then the
         prompt y [B, Yp], on the training kernels.  Fills cache rows 0 .. max_len + Yp - 1, the first logits (from position
         max_len + Yp - 1 with a prompt, lens[b] - 1 without), the history's first Yp entries and the seen bitmaps."""
-        B, dev, Vp = xp.shape[0], xp.device, st["logits"].shape[1]
+        B, dev = xp.shape[0], xp.device
         Yp = y.shape[1]
         rows = slice(r0, r0 + B)
-        xe = self._embed_text(xp, bp, False)
+        xe = self._embed_text(xp, bp, False, None if self.compute_type is None else self._h16())
         ye = ops.embedding(self.P("ar_audio_embedding.word_embeddings.weight"), y)
         h = ops.gpt_embed(xe, ye, self.P("ar_text_position.alpha"), self.P("ar_audio_position.alpha"), st["pe"])
         xl = torch.tensor(lens, device=dev, dtype=torch.int64)
@@ -498,7 +572,7 @@ class Text2SemanticDecoder(ParamTree):
         for i in range(self.num_layers):
             h = self._infer_layer(i, h, st["caches"][i][rows], None, X=max_len, xl=xl, yl=yl)
         first = torch.full((B,), max_len + Yp - 1, device=dev, dtype=torch.int64) if has_prompt else xl - 1
-        st["logits"][rows].copy_(ops.linear_rows(ops.slice_rows(h, first, 1), head).view(B, Vp))
+        self._head_into(ops.slice_rows(h, first, 1), head, st["logits"][rows])
         st["hist"][rows, :Yp].copy_(y)
         bits = torch.zeros((B, st["seen"].shape[1] * 32), device=dev, dtype=torch.int64).scatter_(1, y, 1)
         words = (bits.view(B, -1, 32) << torch.arange(32, device=dev, dtype=torch.int64)).sum(-1)
@@ -535,7 +609,7 @@ class Text2SemanticDecoder(ParamTree):
         try:
             with self.inference_weights():
                 st = self._batch_state(dev, Bp, L0 + max(caps) + INFER_BATCH_K)
-                head = self.w("ar_predict_layer", pad0=st["logits"].shape[1])
+                head = self._head(st)
                 graph = self._batch_step_graph(st, head, "rows")
                 icfg, fcfg, skip, prefixes = row_tables(groups, max_steps)
                 r0 = 0

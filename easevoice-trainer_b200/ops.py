@@ -1913,6 +1913,22 @@ def attn_decode_dev(cache, n_prev_dev, heads, row, skip=None):
     return out
 
 
+def attn_decode_h16(cache, n_prev_dev, heads, row, skip=None):
+    """attn_decode_dev on a 16-bit K/V cache [B, rows, 2 * heads * 32] (fp16 or bf16, k then v; evk_attn_decode_h16): the k and v
+    of `row` [B, 1, 3 * heads * 32] fp32 (the step's in_proj output) are rounded to nearest even into cache row *n_prev_dev, and
+    rows 0 .. *n_prev_dev are attended with row's fp32 q.  -> [B, 1, heads * 32] fp32.  One launch, graph-replayable."""
+    assert cache.dim() == 3 and cache.stride(2) == 1 and cache.shape[2] == 2 * heads * 32 and cache.dtype in H16_TYPES
+    assert n_prev_dev.dtype == torch.int32 and row.dtype == torch.float32 and row.shape[-1] == 3 * heads * 32
+    assert skip is None or (skip.dtype == torch.int32 and skip.is_contiguous() and tuple(skip.shape) == (cache.shape[0], 2))
+    B = cache.shape[0]
+    row = row.reshape(B, -1).contiguous()
+    out = torch.empty((B, 1, heads * 32), device=cache.device, dtype=torch.float32)
+    _call("evk_attn_decode_h16", _p(row), row.stride(0), _p(cache), cache.stride(0), cache.stride(1),
+          int(cache.dtype == torch.bfloat16), _p(n_prev_dev), _p(skip), B, heads, ctypes.c_float(1.0 / math.sqrt(32.0)), _p(out),
+          heads * 32)
+    return out
+
+
 def sample_tokens(logits, V, eos, icfg, fcfg, n_dev, hist, seen, fin, emb, pe, alpha, x_next, q=None, eos_steps=1):
     """One fused sampling step over the rows of `logits` [B, >= V] (evk_sample_tokens; see include/evk.h for the buffers).
     EOS is excluded at the steps idx < eos_steps (1: infer_panel_batch_infer; 11: infer_panel_naive and prompt-free decoding).

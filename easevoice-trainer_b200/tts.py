@@ -10,6 +10,7 @@ The caller keeps its `TTS` object, its `TextPreprocessor` (G2P stays on the host
   recovery_order    `recovery_order`
   run               `run`: the whole synthesis generator
   run_many          several `run` requests in one call, their sentences decoded together (Text2SemanticDecoder.decode_groups)
+  enable_half_precision  `enable_half_precision`: AR decoding in 16 bits (or back to fp32); the other models stay fp32
   audio_postprocess `audio_postprocess`: every fragment normalised, placed in sentence order, followed by its silent interval
                     and converted to int16 by one kernel (evk_fragment_int16); the int16 array crosses to the host once
 
@@ -49,6 +50,19 @@ def set_seed(seed):
         torch.backends.cuda.matmul.allow_tf32 = False
         torch.backends.cudnn.allow_tf32 = False
     return seed
+
+
+def enable_half_precision(tts, enable=True, save=True):
+    """`enable_half_precision` (tts.py:317-349) for what this library runs: the stage-1 GPT's AR decoding switches to 16-bit
+    Linears and a 16-bit K/V cache (Text2SemanticDecoder.set_compute_type(torch.float16)), or back to fp32.  The vocoder, BERT
+    and HuBERT stay in fp32 and are not touched.  On a CPU device, enabling does nothing (the reference logs and returns)."""
+    if str(tts.configs.device) == "cpu" and enable:
+        return
+    tts.configs.is_half = enable
+    tts.precision = torch.float16 if enable else torch.float32
+    if save:
+        tts.configs.save_configs()
+    tts.t2s_model.model.set_compute_type(torch.float16 if enable else None)
 
 
 def ref_spec(audio32k, filter_length, sampling_rate, hop_length, win_length, device):

@@ -476,6 +476,19 @@ int evk_attn_decode_dev(const float* qkv, int64_t batch_stride, int32_t ld, cons
                         int32_t B, int32_t H, float scale, float* out, int32_t ldo, evk_stream_t stream);
 int evk_cache_append(const float* row, int32_t ldr, float* cache, int64_t batch_stride, int32_t ld, const int32_t* pos_dev,
                      int32_t B, int32_t W, evk_stream_t stream);
+/* The same token step on a 16-bit K/V cache (the stage-1 GPT's float16 / bfloat16 compute type), one launch per layer in
+ * place of evk_cache_append + evk_attn_decode_dev.  cache: [B][rows][2 * H * 32] 16-bit values, k then v (no q columns), row
+ * pitch ld elements and batch stride batch_stride elements, both multiples of 8, 16-byte aligned; bf16 != 0 selects bf16,
+ * else fp16.  row: this step's in_proj output [B][3 * H * 32] fp32 ([q | k | v]), pitch ldr (a multiple of 4, 16-byte
+ * aligned).  The CTA of (head h, item b) stores h(k) and h(v) of head h at cache row *n_prev_dev (h = round to nearest even,
+ * cvt.rn; it writes only its own head's 64 values) and attends keys 0 .. *n_prev_dev -- the current key with its rounded k
+ * and v -- with the fp32 q block of `row` times `scale` as the query.  Numerical contract: the 16-bit k and v are widened
+ * exactly; scores, the online softmax, its sums and P V are fp32, in evk_attn_decode_dev's order (thread t owns the same keys
+ * whatever B and the padding are), so an item's bits do not depend on the other items of the launch.  skip as for
+ * evk_attn_decode_dev: keys skip[b][0] .. skip[b][1] - 1, and rows past *n_prev_dev, are never read.  out [B][ldo] fp32. */
+int evk_attn_decode_h16(const float* row, int32_t ldr, void* cache, int64_t batch_stride, int32_t ld, int32_t bf16,
+                        const int32_t* n_prev_dev, const int32_t* skip, int32_t B, int32_t H, float scale, float* out, int32_t ldo,
+                        evk_stream_t stream);
 /* Fused token sampler of batched KV-cache decoding (infer_panel_batch_infer, t2s_model.py:563-730; utils.py:109-157), one CTA
  * per row b of logits [B][ldl] (V <= 2048 classes, eos = V - 1), in the reference's order: repetition penalty over the row's
  * history (prompt included) -> top-p if top_p < 1 (descending order, cumulative softmax, `cum > top_p` removed, the first kept;

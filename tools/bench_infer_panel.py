@@ -10,6 +10,9 @@ One JSON line.   python tools/bench_infer_panel.py > gpurun_out/bench_infer_pane
 # infer_panel_naive_batched(prompts=None) for B in {1, 4, 16}, same 120 phonemes / 300 tokens / top_k 15, card name and power limit.
 # --new N: N generated tokens (early_stop_num) instead of 300 in every mode, e.g. 40 for a short sentence, where the steps run
 # past a batch's last finish between two reads of the finished flags weigh the most.
+# --precision float16|bfloat16 (with --batch or --ref-free): the batched numbers for the fp32 and the 16-bit compute type
+# (Text2SemanticDecoder.set_compute_type), alternated twice in one process, each with its peak allocated memory; with --profile
+# DIR, instead only the torch.profiler trace and per-kernel table of one B = 16 call in the 16-bit compute type.
 import json
 import math
 import os
@@ -41,6 +44,7 @@ prompts = torch.randint(0, 1024, (1, Yp), generator=g)
 xd, bd, pd, xl = x.to(dev), bert.to(dev), prompts.to(dev), torch.tensor([X], device=dev)
 BATCH = "--batch" in sys.argv
 REF_FREE = "--ref-free" in sys.argv
+PREC = {"float16": torch.float16, "bfloat16": torch.bfloat16}[sys.argv[sys.argv.index("--precision") + 1]] if "--precision" in sys.argv else None
 
 
 def card_name():
@@ -48,6 +52,22 @@ def card_name():
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                           text=True).stdout.strip().splitlines()
     return card[0] if card else "unknown"
+
+
+def profile_b16(d):
+    """torch.profiler trace and per-kernel table of one B = 16 infer_panel_batch_infer call (40 tokens), after a warm-up"""
+    os.makedirs(d, exist_ok=True)
+    B = 16
+    args = ([xd[0]] * B, torch.full((B,), X), pd.expand(B, -1), [bd[0]] * B)
+    net.infer_panel_batch_infer(*args, top_k=15, top_p=1, early_stop_num=40, temperature=1.0)
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA]) as prof:
+        net.infer_panel_batch_infer(*args, top_k=15, top_p=1, early_stop_num=40, temperature=1.0)
+        torch.cuda.synchronize()
+    tag = "" if net.compute_type is None else "_" + str(net.compute_type).split(".")[-1]
+    prof.export_chrome_trace(os.path.join(d, f"infer_batch_b16{tag}.pt.trace.json"))
+    with open(os.path.join(d, f"infer_batch_b16{tag}_kernels.txt"), "w") as f:
+        f.write(prof.key_averages().table(sort_by="cuda_time_total", row_limit=30))
 
 
 def bench_ref_free():
@@ -75,7 +95,7 @@ def bench_ref_free():
     return single, out
 
 
-if REF_FREE:
+if REF_FREE and PREC is None:
     single, batch = bench_ref_free()
     print(json.dumps(dict(metric="Text2SemanticDecoder.infer_panel_naive_batched(prompts=None) (prompt-free batched KV-cache AR decoding)",
                           unit="semantic-tokens/s", card=card_name(), single_utterance=single, batch=batch,
@@ -99,18 +119,32 @@ def bench_batch():
         gen = [int(y.shape[0]) - Yp for y in ys]
         steps = max(gen) + 1
         out[str(B)] = dict(tokens_per_s=sum(gen) / s, ms_per_step=s / steps * 1e3, generated=sum(gen), steps=steps, seconds=s)
-    if "--profile" in sys.argv:
-        d = sys.argv[sys.argv.index("--profile") + 1]
-        os.makedirs(d, exist_ok=True)
-        B = 16
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA]) as prof:
-            net.infer_panel_batch_infer([xd[0]] * B, torch.full((B,), X), pd.expand(B, -1), [bd[0]] * B, top_k=15, top_p=1,
-                                        early_stop_num=40, temperature=1.0)
-            torch.cuda.synchronize()
-        prof.export_chrome_trace(os.path.join(d, "infer_batch_b16.pt.trace.json"))
-        with open(os.path.join(d, "infer_batch_b16_kernels.txt"), "w") as f:
-            f.write(prof.key_averages().table(sort_by="cuda_time_total", row_limit=30))
+    if "--profile" in sys.argv and PREC is None:
+        profile_b16(sys.argv[sys.argv.index("--profile") + 1])
     return out, card_name()
+
+
+if PREC is not None and (BATCH or REF_FREE):
+    if "--profile" in sys.argv:
+        net.set_compute_type(PREC)
+        profile_b16(sys.argv[sys.argv.index("--profile") + 1])
+        sys.exit(0)
+    card, arms = card_name(), []
+    for dt in (None, PREC, None, PREC):
+        net.set_compute_type(dt)
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        if BATCH:
+            arms.append(dict(compute_type=str(dt), batch=bench_batch()[0]))
+        else:
+            single, batch = bench_ref_free()
+            arms.append(dict(compute_type=str(dt), single_utterance=single, batch=batch))
+        arms[-1]["peak_allocated_gib"] = torch.cuda.max_memory_allocated() / 2 ** 30
+    print(json.dumps(dict(metric="Text2SemanticDecoder " + ("infer_panel_naive_batched(prompts=None)" if REF_FREE else "infer_panel_batch_infer")
+                          + ": fp32 against the 16-bit compute type, alternated", unit="semantic-tokens/s", card=card, arms=arms,
+                          config=dict(layers=24, X=X, prompt=0 if REF_FREE else Yp, early_stop_num=NEW, top_k=15, top_p=1, temperature=1.0),
+                          note="aggregate generated tokens over wall time of one call, prompt pass included; 25 tokens = 1 s of audio")))
+    sys.exit(0)
 
 
 # every warm-up runs at the timed size: it packs the weights, sizes the KV caches and captures the step graph, so that the timed

@@ -8,7 +8,11 @@ events around the wrapped calls; and the assembly (evk_fragment_int16 + one copy
 audio_postprocess (per-fragment max, division, .cpu().numpy(), host concatenation and cast) on the same vocoder outputs,
 alternated in one process.  The card name and power limit are read in the same call.
 
-Usage:  python tools/bench_tts.py [--reps 3]
+--precision float16|bfloat16: every round runs the call once with the fp32 and once with the 16-bit compute type of the
+GPT's AR decoding (Text2SemanticDecoder.set_compute_type, what enable_half_precision selects), alternated; each call also
+reports its peak allocated memory.
+
+Usage:  python tools/bench_tts.py [--reps 3] [--precision float16|bfloat16]
 """
 import argparse
 import json
@@ -111,6 +115,7 @@ def reference_postprocess(audio, sr, batch_index_list, fragment_interval):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--precision", choices=["float16", "bfloat16"], default=None)
     args = ap.parse_args()
     from easevoice_trainer_b200 import lib, tts
     lib.init()
@@ -149,19 +154,25 @@ def main():
     with tempfile.NamedTemporaryFile(suffix=".wav") as f:
         inputs = dict(text="t", text_lang="zh", ref_audio_path=f.name, prompt_text="p", prompt_lang="zh", top_k=15, batch_size=8,
                       seed=7, fragment_interval=0.3)
-        calls = []
-        for rep in range(args.reps + 1):                                    # the first call warms every shape up
-            for v in phases.values():
-                v.clear()
-            caller.reset()
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            sr, wav = next(tts.run(caller, inputs))
-            torch.cuda.synchronize()
-            wall = time.perf_counter() - t0
-            if rep:
-                calls.append(dict(wall_ms=wall * 1e3, samples=int(wav.shape[0]),
-                                  **{k + "_ms": sum(a.elapsed_time(b) for a, b in v) for k, v in phases.items()}))
+        arms = [None] if args.precision is None else [None, getattr(torch, args.precision)]
+        per_arm = {str(dt): [] for dt in arms}
+        for rep in range(args.reps + 1):                                    # the first round warms every shape up
+            for dt in arms:
+                t2s.set_compute_type(dt)
+                for v in phases.values():
+                    v.clear()
+                caller.reset()
+                torch.cuda.synchronize()
+                torch.cuda.reset_peak_memory_stats()
+                t0 = time.perf_counter()
+                sr, wav = next(tts.run(caller, inputs))
+                torch.cuda.synchronize()
+                wall = time.perf_counter() - t0
+                if rep:
+                    per_arm[str(dt)].append(dict(wall_ms=wall * 1e3, samples=int(wav.shape[0]),
+                                                 peak_mem_gib=torch.cuda.max_memory_allocated() / 2 ** 30,
+                                                 **{k + "_ms": sum(a.elapsed_time(b) for a, b in v) for k, v in phases.items()}))
+        calls = per_arm["None"]
     tts.audio_postprocess = post
     audio, (sr, bil, speed, split, interval) = keep["audio"], keep["args"]
     ours, ref = [], []
@@ -176,7 +187,10 @@ def main():
     med = lambda v: float(np.median(v))                                     # noqa: E731
     print(json.dumps({"card": card, "sentences": 20, "fragments": sum(len(x) for x in audio), "audio_s": calls[-1]["samples"] / sr,
                       "calls": calls, "median_wall_ms": med([c["wall_ms"] for c in calls]),
-                      "assembly_ms": med(ours) * 1e3, "reference_host_postprocess_ms": med(ref) * 1e3}))
+                      "assembly_ms": med(ours) * 1e3, "reference_host_postprocess_ms": med(ref) * 1e3,
+                      **({} if args.precision is None else {"arms": {k: dict(calls=v, median_wall_ms=med([c["wall_ms"] for c in v]),
+                                                                            median_ar_ms=med([c["ar_ms"] for c in v]))
+                                                                     for k, v in per_arm.items()}})}))
 
 
 if __name__ == "__main__":

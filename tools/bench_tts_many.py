@@ -9,7 +9,10 @@ decode_batch) and
 int16 assembly (evk_fragment_int16 calls) from CUDA events around the wrapped calls, and the peak allocated memory; and the
 card name and power limit, read in the same call.
 
-Usage:  python tools/bench_tts_many.py [--reps 3]
+--precision float16|bfloat16: run_many alone, with the fp32 and the 16-bit compute type of the GPT's AR decoding
+(Text2SemanticDecoder.set_compute_type) as the two alternated arms instead.
+
+Usage:  python tools/bench_tts_many.py [--reps 3] [--precision float16|bfloat16]
 """
 import argparse
 import json
@@ -74,6 +77,7 @@ class ManyCaller(Caller):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--precision", choices=["float16", "bfloat16"], default=None)
     args = ap.parse_args()
     from easevoice_trainer_b200 import lib, ops, tts
     lib.init()
@@ -121,10 +125,19 @@ def main():
 
         def arm_loop():
             return [next(tts.run(caller, inp)) for inp in inputs]
-        out = {"run_many": [], "run_loop": []}
+        if args.precision is None:
+            arms = (("run_many", arm_many), ("run_loop", arm_loop))
+        else:
+            def typed(dt):
+                def arm():
+                    t2s.set_compute_type(dt)
+                    return arm_many()
+                return arm
+            arms = (("run_many", typed(None)), ("run_many_" + args.precision, typed(getattr(torch, args.precision))))
+        out = {name: [] for name, _ in arms}
         samples = {}
         for rep in range(args.reps + 1):                                    # the first round warms every shape up
-            for name, fn in (("run_many", arm_many), ("run_loop", arm_loop)):
+            for name, fn in arms:
                 for v in phases.values():
                     v.clear()
                 caller.reset()
@@ -142,9 +155,11 @@ def main():
     med = lambda v: float(np.median(v))                                     # noqa: E731
     sent = sum(len(v) for v in caller.text_preprocessor.sent.values())
     print(json.dumps({"card": card, "requests": N_REQ, "sentences": sent, "audio_s": {k: v / 32000 for k, v in samples.items()},
-                      "run_many": out["run_many"], "run_loop": out["run_loop"],
-                      "median_wall_ms": {k: med([c["wall_ms"] for c in v]) for k, v in out.items()},
-                      "speedup": med([c["wall_ms"] for c in out["run_loop"]]) / med([c["wall_ms"] for c in out["run_many"]])}))
+                      **out, "median_wall_ms": {k: med([c["wall_ms"] for c in v]) for k, v in out.items()},
+                      "median_ar_ms": {k: med([c["ar_ms"] for c in v]) for k, v in out.items()},
+                      # run_loop over run_many; with --precision, fp32 over 16-bit
+                      "speedup": (lambda a, b: med([c["wall_ms"] for c in out[a]]) / med([c["wall_ms"] for c in out[b]]))(
+                          *(("run_loop", "run_many") if args.precision is None else ("run_many", arms[1][0])))}))
 
 
 if __name__ == "__main__":
