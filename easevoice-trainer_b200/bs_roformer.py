@@ -8,6 +8,11 @@ are never made.  Every RMSNorm is an L2 normalisation (evk_row_norm without gamm
 folded into the next Linear's weight columns at load; to_gates is appended to to_qkv as extra output rows.  Linears run on the
 TF32 tensor-core GEMM (3xTF32 under evk_set_precise(1)) with GELU, tanh and residual adds in its epilogue.  The complex mask
 multiply is fused into the inverse STFT.  Dropout is the identity.
+
+set_compute_type(torch.float16 / torch.bfloat16) (the reference's is_half) runs every Linear on the 16-bit kernel
+(evk_linear_h16: both operands rounded to 16 bits, fp32 accumulation and epilogue) and the attention on
+evk_rope_attn_fwd_h16 (rotated q, k, v and the probabilities rounded to 16 bits, fp32 softmax and gate).  The STFT, the band
+input, the norms, the GLU, the mask averaging, the inverse STFT, the residual stream and the rotary tables stay fp32.
 """
 import math
 
@@ -73,6 +78,7 @@ class AxialRoformer:
         self.match_input_audio_length = bool(match_input_audio_length)
         self.device = torch.device("cpu")
         self.host_w, self.bias = None, None
+        self.compute_type = None
         self._packed = {}
         self._rope = {}
         self._tab = None
@@ -175,12 +181,33 @@ class AxialRoformer:
         """Inference only already (dropout is the identity): returns self, so `SeparateMDXC.separate`'s model.eval() works."""
         return self
 
+    def set_compute_type(self, dtype):
+        """None: fp32 activations with TF32 products (the default); torch.float16 or torch.bfloat16: every Linear and the
+        attention on the 16-bit kernels.  The weights are packed for the compute type on the next forward.  -> self."""
+        if dtype is not None and dtype not in ops.H16_TYPES:
+            raise ValueError(f"compute type {dtype!r} (None, torch.float16 or torch.bfloat16)")
+        self.compute_type = dtype
+        return self
+
+    def _weights_key(self):
+        """(precise mode, compute type): the TF32 packs depend on evk_set_precise, the 16-bit ones on the dtype only"""
+        return (lib.init().evk_get_precise() if self.compute_type is None else None, str(self.compute_type))
+
     def _weights(self):
-        """PackedW operands per precision mode (the packing rounds to TF32 unless evk_set_precise(1) is on)"""
-        mode = lib.init().evk_get_precise()
-        if mode not in self._packed:
-            self._packed[mode] = {k: ops.pack_weight(v.to(self.device), None, need_pb=False) for k, v in self.host_w.items()}
-        return self._packed[mode]
+        """The Linears' packed weights for _weights_key(): PackedW (rounded to TF32 unless evk_set_precise(1) is on) when the
+        compute type is None, else only PackedH16 of the compute type"""
+        key = self._weights_key()
+        if key not in self._packed:
+            h16 = self.compute_type
+            pk = (lambda w: ops.pack_weight(w, None, need_pb=False)) if h16 is None else (lambda w: ops.pack_weight_h16(w, h16))
+            self._packed[key] = {k: pk(v.to(self.device)) for k, v in self.host_w.items()}
+        return self._packed[key]
+
+    def _linear(self, x, w, out, bias=None, act=ops.ACT_NONE, res=None):
+        """out = act(x W^T + bias + res) on the compute type's kernel: the TF32 GEMM, or evk_linear_h16"""
+        if self.compute_type is None:
+            return ops.linear_into(x, w, out, bias=bias, act=act, res=res)
+        return ops.linear_h16(x, w, bias=bias, act=act, res=res, out=out)
 
     def _rope_table(self, L):
         """[L, 32, 2] (cos, sin) of fp32(p * theta_i), computed in fp32 with accurate cos / sin as rotary_embedding_torch does"""
@@ -222,16 +249,20 @@ class AxialRoformer:
         for j in range(depth):
             q = f"{p}.layers.{j}"
             ops.row_norm(x, out=h)
-            wq = W[q + ".qkvg"]
-            qkvg = ops.linear_into(h, wq, torch.empty((R, wq.D0), device=x.device), bias=sd[q + ".qkvg.b"])
-            a = ops.rope_attn(qkvg, cs, torch.empty((R, D), device=x.device), self.heads, L, *geo)
+            b = sd[q + ".qkvg.b"]
+            qkvg = self._linear(h, W[q + ".qkvg"], torch.empty((R, b.numel()), device=x.device), bias=b)
+            a = torch.empty((R, D), device=x.device)
+            if self.compute_type is None:
+                ops.rope_attn(qkvg, cs, a, self.heads, L, *geo)
+            else:
+                ops.rope_attn_h16(qkvg, cs, a, self.heads, L, *geo, self.compute_type)
             del qkvg
-            x = ops.linear_into(a, W[q + ".out"], torch.empty_like(x), res=x)
+            x = self._linear(a, W[q + ".out"], torch.empty_like(x), res=x)
             del a
             ops.row_norm(x, out=h)
-            f = ops.linear_into(h, W[q + ".ff1"], torch.empty((R, 4 * self.dim), device=x.device), bias=sd[q + ".ff1.b"],
-                                act=ops.ACT_GELU)
-            x = ops.linear_into(f, W[q + ".ff2"], torch.empty_like(x), bias=sd[q + ".ff2.b"], res=x)
+            f = self._linear(h, W[q + ".ff1"], torch.empty((R, 4 * self.dim), device=x.device), bias=sd[q + ".ff1.b"],
+                             act=ops.ACT_GELU)
+            x = self._linear(f, W[q + ".ff2"], torch.empty_like(x), bias=sd[q + ".ff2.b"], res=x)
             del f
         return x
 
@@ -240,8 +271,8 @@ class AxialRoformer:
         W, sd, S, dim, nb = self._weights(), self.bias, self.S, self.dim, len(off) - 1
         h = torch.empty((rows, nb * dim), device=feat.device)
         for i in range(nb):
-            ops.linear_into(feat[:, 2 * S * off[i]:2 * S * off[i + 1]], W[f"band.{i}"], h[:, i * dim:(i + 1) * dim],
-                            bias=sd[f"band.{i}.b"])
+            self._linear(feat[:, 2 * S * off[i]:2 * S * off[i + 1]], W[f"band.{i}"], h[:, i * dim:(i + 1) * dim],
+                         bias=sd[f"band.{i}.b"])
         return h.view(rows * nb, dim)
 
     def _mask_estimator(self, xn, off, out):
@@ -250,10 +281,10 @@ class AxialRoformer:
         for i in range(len(off) - 1):
             hc = xn[:, i * dim:(i + 1) * dim]
             for k in range(self.mask_linears):
-                w = W[f"mask.{i}.{k}"]
+                b = sd[f"mask.{i}.{k}.b"]
                 last = k == self.mask_linears - 1
-                hc = ops.linear_into(hc, w, torch.empty((rows, w.D0), device=xn.device), bias=sd[f"mask.{i}.{k}.b"],
-                                     act=ops.ACT_NONE if last else ops.ACT_TANH)
+                hc = self._linear(hc, W[f"mask.{i}.{k}"], torch.empty((rows, b.numel()), device=xn.device), bias=b,
+                                  act=ops.ACT_NONE if last else ops.ACT_TANH)
             ops.glu_into(hc, out[:, 2 * S * off[i]:2 * S * off[i + 1]])
         return out
 
@@ -344,10 +375,11 @@ class BSRoformer(AxialRoformer):
         return out
 
     @classmethod
-    def from_pretrained(cls, path, device="cuda"):
-        """The SeparateMDXC model (SHIPPED_CONFIG) with the weights of a reference checkpoint file, on `device`."""
+    def from_pretrained(cls, path, device="cuda", compute_type=None):
+        """The SeparateMDXC model (SHIPPED_CONFIG) with the weights of a reference checkpoint file, on `device`.
+        compute_type: as set_compute_type."""
         sd = torch.load(path, map_location="cpu", weights_only=True)
-        return cls(**SHIPPED_CONFIG).to(device).load_state_dict(sd)
+        return cls(**SHIPPED_CONFIG).to(device).load_state_dict(sd).set_compute_type(compute_type)
 
 
 def chunk_plan(n, c=CHUNK, batch=BATCH):

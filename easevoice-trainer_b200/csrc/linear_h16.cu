@@ -12,42 +12,16 @@
 //                        consumer warpgroups of 64 rows, 128-byte swizzle, a ring of 5 stages of 64 K), no K split.
 #include <algorithm>
 
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
-
 #include "wgmma.cuh"
 
 namespace evk {
 namespace {
-
-template <bool BF16>
-__device__ __forceinline__ uint16_t to_h16(float v) {
-  if constexpr (BF16) return __bfloat16_as_ushort(__float2bfloat16_rn(v));
-  else return __half_as_ushort(__float2half_rn(v));
-}
-
-template <bool BF16>
-__device__ __forceinline__ uint32_t to_h16x2(float lo, float hi) {
-  return (uint32_t)to_h16<BF16>(lo) | ((uint32_t)to_h16<BF16>(hi) << 16);
-}
 
 __device__ __forceinline__ float epi(float acc, const float* bias, const float* res, size_t ridx, int n, int act, float slope) {
   float v = acc;
   if (bias) v += bias[n];
   if (res) v += res[ridx];
   return conv_act(v, act, slope);
-}
-
-// d += A * B over K = 16: a0..a3 = A(g, 2t..2t+1), A(g+8, 2t..), A(g, 2t+8..), A(g+8, 2t+8..); b0, b1 = B(2t.., g), B(2t+8.., g)
-// with g = lane / 4, t = lane % 4; d = (g, 2t..2t+1), (g+8, 2t..2t+1).
-template <bool BF16>
-__device__ __forceinline__ void mma16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-  if constexpr (BF16)
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-  else
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
 // ---- row kernel ---------------------------------------------------------------------------------------------------------

@@ -171,9 +171,10 @@ class MelBandRoformer(AxialRoformer):
         return cfg
 
     @classmethod
-    def from_pretrained(cls, path, device="cuda", **config):
+    def from_pretrained(cls, path, device="cuda", compute_type=None, **config):
         """A MelBandRoformer with the weights of a reference checkpoint file, on `device`.  The configuration is inferred
         from the weight shapes (infer_config); sample_rate and stft_hop_length, which the weights do not determine, default
-        to DEFAULT_CONFIG's (44.1 kHz, hop 441) and are the caller's to set, as is anything passed in `config`."""
+        to DEFAULT_CONFIG's (44.1 kHz, hop 441) and are the caller's to set, as is anything passed in `config`.
+        compute_type: as set_compute_type."""
         sd = torch.load(path, map_location="cpu", weights_only=True)
-        return cls(**cls.infer_config(sd, **config)).to(device).load_state_dict(sd)
+        return cls(**cls.infer_config(sd, **config)).to(device).load_state_dict(sd).set_compute_type(compute_type)

@@ -2248,6 +2248,18 @@ def rope_attn(qkvg, cs, out, heads, L, n_outer, s_outer, n_inner, s_inner, s_tok
     return out
 
 
+def rope_attn_h16(qkvg, cs, out, heads, L, n_outer, s_outer, n_inner, s_inner, s_tok, dtype):
+    """rope_attn with 16-bit operands (evk_rope_attn_fwd_h16): rotated q, k, v and the probabilities rounded to `dtype`
+    (torch.float16 or torch.bfloat16), fp32 accumulation, softmax and gate."""
+    if dtype not in H16_TYPES:
+        raise ValueError(f"16-bit compute type {dtype} (torch.float16 or torch.bfloat16)")
+    assert qkvg.dim() == 2 and qkvg.stride(1) == 1 and out.dim() == 2 and out.stride(1) == 1 and cs.is_contiguous()
+    assert cs.shape[0] >= L
+    _call_f("evk_rope_attn_fwd_h16", 4.0 * n_outer * n_inner * heads * L * L * 64, _p(qkvg), qkvg.stride(0), _p(cs), _p(out),
+            out.stride(0), heads, L, n_outer, s_outer, n_inner, s_inner, s_tok, int(dtype == torch.bfloat16))
+    return out
+
+
 def row_norm(x, gamma=None, out=None):
     """x / max(||x||_2, 1e-12) per row of a [rows, C] view, times sqrt(C) * gamma when gamma is given (evk_row_norm); out may
     be x"""

@@ -633,6 +633,18 @@ int evk_lstm_bidir_fwd(const float* g, int64_t g_st, int64_t g_sn, const float* 
  * accumulation (3xTF32 under evk_set_precise(1)); no atomics, bit-reproducible. */
 int evk_rope_attn_fwd(const float* qkvg, int32_t ld, const float* cs, float* o, int32_t ldo, int32_t H, int32_t L,
                       int32_t n_outer, int64_t s_outer, int32_t n_inner, int64_t s_inner, int64_t s_tok, evk_stream_t stream);
+/* The same attention with 16-bit operands (the Roformers' float16 / bfloat16 compute types): the operands, geometry and
+ * strides of evk_rope_attn_fwd, and h = round to nearest even to fp16 (bf16 == 0) or bf16 (bf16 != 0).  Numerical contract:
+ *   q and k are rotated in fp32 with the cs table and the formula above, then rounded with h; v is rounded with h.
+ *   s = h(q_rot) . h(k_rot) on mma.sync.m16n8k16 (products exact, fp32 accumulation), times 1/8.
+ *   The online softmax is fp32 and the same as evk_rope_attn_fwd's (running maxima and sums over 32-key tiles, ex2.approx);
+ *   its sums add the fp32 probabilities p.
+ *   o = (sum_j h(p_j) h(v_j)) / (sum_j p_j) * sigmoid(gate), P . V accumulated in fp32, the gate in fp32.
+ * Values beyond fp16's range become +-inf under h.  No atomics: a sequence's output depends only on that sequence, so it is
+ * bit-identical whatever n_outer / n_inner are.  evk_set_precise has no effect here. */
+int evk_rope_attn_fwd_h16(const float* qkvg, int32_t ld, const float* cs, float* o, int32_t ldo, int32_t H, int32_t L,
+                          int32_t n_outer, int64_t s_outer, int32_t n_inner, int64_t s_inner, int64_t s_tok, int32_t bf16,
+                          evk_stream_t stream);
 /* Inverse of evk_stft_fwd's center=True transform with the periodic Hann(n_fft) window: torch.istft(n_fft, hop, n_fft, hann,
  * center=True, normalized=False, onesided=True, length=length or None) of cplx [B*S*T][n_fft/2+1][2] (rows b*S + s), times
  * mask when given (bs_roformer.py:530-543): bin k of row (b, s), frame t is multiplied by the complex mask at columns

@@ -34,6 +34,10 @@ with seeded weights) the same way on the same mix, with the overlapping-band ker
 evk_melband_mask_avg) split out of the device time, and oracle/mel_roformer_oracle.py's forward as the stock PyTorch arms.
 It skips the rope_attn rates, whose shapes are the BS-Roformer's.
 
+--precision float16 | bfloat16 (with --net roformer or melroformer) adds an arm with that compute type
+(set_compute_type): its demix_track calls alternate with the fp32 arm's, and it gets its own peak memory, device-time split,
+rope_attn rates (evk_rope_attn_fwd_h16) and rel-L2 against the fp32 arm and against the stock PyTorch arms.
+
 --net mdx23c measures MDX23C (mdx23c.py, the 8K-FFT InstVoc configuration with seeded weights) the same way on the same mix
 (31 chunks of 261 120 samples): demix_track wall time and peak memory, the device time of one profiled forward of
 `--max-chunks` chunks split into 3x3 convs, 2x2 down / up convs, TDF Linears, instance norms, STFT / iSTFT and the rest, the
@@ -41,7 +45,7 @@ conv FLOP rate with FLOPs computed from the layer shapes here, and oracle/mdx23c
 restated) as the stock PyTorch arms.
 
 Usage:  python tools/bench_uvr5.py [--net vr|deecho|dereverb|roformer|melroformer|mdx23c] [--wave] [--frames 16538] [--tta 0] [--max-windows 16]
-        [--reps 3]
+        [--reps 3] [--precision float32|float16|bfloat16]
 """
 import argparse
 import json
@@ -230,9 +234,10 @@ def echo_main(a):
     print(json.dumps(res))
 
 
-def rope_attn_rates(ops, reps=20):
-    """TFLOP/s of evk_rope_attn_fwd at the shapes of 4 chunks of the shipped config (801 frames x 62 bands, 8 heads):
-    time axis 248 sequences of 801 tokens, frequency axis 3 204 sequences of 62 tokens (CUDA events over `reps` launches)"""
+def rope_attn_rates(ops, reps=20, dtype=None):
+    """TFLOP/s of evk_rope_attn_fwd (dtype None) or evk_rope_attn_fwd_h16 at the shapes of 4 chunks of the shipped config
+    (801 frames x 62 bands, 8 heads): time axis 248 sequences of 801 tokens, frequency axis 3 204 sequences of 62 tokens
+    (CUDA events over `reps` launches)"""
     B, T, F, H = 4, 801, 62, 8
     ld = 3 * H * 64 + H
     x = torch.randn(B * T * F, ld, device="cuda")
@@ -240,7 +245,10 @@ def rope_attn_rates(ops, reps=20):
     out = {}
     for name, L, geo, nseq in (("time", T, (B, T * F, F, 1, F), B * F), ("freq", F, (B * T, F, 1, 0, 1), B * T)):
         cs = torch.stack(BR.rotary_cos_sin(L), -1).contiguous().cuda()
-        fn = lambda: ops.rope_attn(x, cs, o, H, L, *geo)  # noqa: E731
+        if dtype is None:
+            fn = lambda: ops.rope_attn(x, cs, o, H, L, *geo)  # noqa: E731
+        else:
+            fn = lambda: ops.rope_attn_h16(x, cs, o, H, L, *geo, dtype)  # noqa: E731
         fn()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -253,7 +261,7 @@ def rope_attn_rates(ops, reps=20):
     return out
 
 
-FAMILIES = (("gemm", ("evk_gconv_fwd",)), ("attention", ("evk_rope_attn_fwd",)),
+FAMILIES = (("gemm", ("evk_gconv_fwd", "evk_linear_h16")), ("attention", ("evk_rope_attn_fwd", "evk_rope_attn_fwd_h16")),
             ("norms", ("evk_row_norm", "evk_band_input")), ("stft_istft", ("evk_stft_fwd", "evk_istft")))
 
 
@@ -272,7 +280,8 @@ def torch_roformer_demix(P, cfg, mix, half, autocast, forward=BR.forward):
     return BR.demix_track(net, mix)["vocals"]
 
 
-MEL_FAMILIES = (("gemm", ("evk_gconv_fwd",)), ("attention", ("evk_rope_attn_fwd",)), ("norms", ("evk_row_norm",)),
+MEL_FAMILIES = (("gemm", ("evk_gconv_fwd", "evk_linear_h16")), ("attention", ("evk_rope_attn_fwd", "evk_rope_attn_fwd_h16")),
+                ("norms", ("evk_row_norm",)),
                 ("band_input", ("evk_band_input",)), ("melband_mask_avg", ("evk_melband_mask_avg",)),
                 ("stft_istft", ("evk_stft_fwd", "evk_istft")))
 
@@ -291,28 +300,46 @@ def roformer_main(a):
         model = bs_roformer.BSRoformer(**cfg).to("cuda").load_state_dict(P)
     mix = BR.make_audio(7, (2, 7938000))
     res = dict(gpu=gpu_info(), net=a.net, samples=mix.shape[1], chunks=-(-mix.shape[1] // BR.CHUNK), max_chunks=a.max_chunks)
-    t = time.perf_counter()
-    out = bs_roformer.demix_track(model, mix, "cuda", a.max_chunks)["vocals"]
-    res["evk_first_call_s"] = round(time.perf_counter() - t, 3)
-    torch.cuda.reset_peak_memory_stats()
-    ts = timed(lambda: bs_roformer.demix_track(model, mix, "cuda", a.max_chunks), a.reps)
-    res["evk_s"] = [round(t, 3) for t in ts]
-    res["peak_mem_gib"] = round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)
+    # the fp32 (TF32) arm's results at the top level; a 16-bit arm's under its --precision name.  The arms alternate in the
+    # timed calls, so both see the same card state.
+    arms = [("float32", None, res)]
+    if a.precision != "float32":
+        res[a.precision] = {}
+        arms.append((a.precision, getattr(torch, a.precision), res[a.precision]))
+    outs = {}
+    for name, dt, r in arms:
+        model.set_compute_type(dt)
+        t = time.perf_counter()
+        outs[name] = bs_roformer.demix_track(model, mix, "cuda", a.max_chunks)["vocals"]
+        r["evk_first_call_s"] = round(time.perf_counter() - t, 3)
+        r["evk_s"], r["peak_mem_gib"] = [], 0.0
+    for _ in range(a.reps):
+        for name, dt, r in arms:
+            model.set_compute_type(dt)
+            torch.cuda.reset_peak_memory_stats()
+            r["evk_s"] += [round(t, 3) for t in timed(lambda: bs_roformer.demix_track(model, mix, "cuda", a.max_chunks), 1)]
+            r["peak_mem_gib"] = max(r["peak_mem_gib"], round(torch.cuda.max_memory_allocated() / 2 ** 30, 2))
     batch = mix[:, :a.max_chunks * BR.CHUNK].reshape(2, a.max_chunks, BR.CHUNK).transpose(0, 1).contiguous().cuda()
-    model.forward(batch)
-    ops.profile_begin()
-    model.forward(batch)
-    prof = ops.profile_end()
-    tot = sum(v["ms"] for v in prof.values())
-    fam = {name: round(sum(v["ms"] for k, v in prof.items() if k.split(":")[0] in keys), 2) for name, keys in families}
-    fam["other"] = round(tot - sum(fam.values()), 2)
-    res["forward_ms_by_family"] = fam
-    res["forward_device_ms"] = round(tot, 2)
-    gemm_fl = sum(v["flops"] for k, v in prof.items() if k.split(":")[0] in families[0][1])
-    res["chunk_tflop_gemm"] = round(gemm_fl / a.max_chunks / 1e12, 2)
-    res["gemm_tflops_in_forward"] = round(gemm_fl / fam["gemm"] / 1e9, 1)
-    if a.net == "roformer":
-        res["rope_attn"] = rope_attn_rates(ops)
+    for name, dt, r in arms:
+        model.set_compute_type(dt)
+        model.forward(batch)
+        ops.profile_begin()
+        model.forward(batch)
+        prof = ops.profile_end()
+        tot = sum(v["ms"] for v in prof.values())
+        fam = {n: round(sum(v["ms"] for k, v in prof.items() if k.split(":")[0] in keys), 2) for n, keys in families}
+        fam["other"] = round(tot - sum(fam.values()), 2)
+        r["forward_ms_by_family"] = fam
+        r["forward_device_ms"] = round(tot, 2)
+        gemm_fl = sum(v["flops"] for k, v in prof.items() if k.split(":")[0] in families[0][1])
+        r["chunk_tflop_gemm"] = round(gemm_fl / a.max_chunks / 1e12, 2)
+        r["gemm_tflops_in_forward"] = round(gemm_fl / fam["gemm"] / 1e9, 1)
+        if a.net == "roformer":
+            r["rope_attn"] = rope_attn_rates(ops, dtype=dt)
+    model.set_compute_type(None)
+    out = outs["float32"]
+    if a.precision != "float32":
+        res[a.precision]["rel_l2_vs_evk_float32"] = float(np.linalg.norm(outs[a.precision] - out) / np.linalg.norm(out))
     if not a.skip_torch:
         torch.backends.cudnn.allow_tf32 = True
         small = BR.make_audio(8, (2, BR.CHUNK))
@@ -322,6 +349,8 @@ def roformer_main(a):
         Pd = {k: v.cuda() for k, v in P.items()}
         exact = torch_roformer_demix(Pd, cfg, mix, False, False, forward)
         res["evk_rel_l2_vs_torch_fp32"] = rel(out, exact)
+        if a.precision != "float32":
+            res[a.precision]["rel_l2_vs_torch_fp32"] = rel(outs[a.precision], exact)
         torch.backends.cuda.matmul.allow_tf32 = True
         # (name, weights in fp16, chunks in fp16, autocast): the shipped cfg.is_half path, then fp32 with TF32 allowed
         arms = [("torch_fp16", True, True, True), ("torch_tf32", False, False, False)]
@@ -342,6 +371,8 @@ def roformer_main(a):
             ref = torch_roformer_demix(Pd, cfg, mix, ch, ac, forward)
             res[name + "_rel_l2_vs_evk"] = rel(ref, out)
             res[name + "_rel_l2_vs_torch_fp32"] = rel(ref, exact)
+            if a.precision != "float32":
+                res[a.precision][name + "_rel_l2_vs_evk"] = rel(ref, outs[a.precision])
             del Pd
             torch.cuda.empty_cache()
     print(json.dumps(res))
@@ -521,6 +552,8 @@ def main():
     ap.add_argument("--max-windows", type=int, default=16)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--skip-torch", action="store_true")
+    ap.add_argument("--precision", choices=("float32", "float16", "bfloat16"), default="float32",
+                    help="--net roformer / melroformer: also run this 16-bit compute type, alternating with the fp32 arm")
     ap.add_argument("--wave", action="store_true")
     a = ap.parse_args()
     if a.wave:
