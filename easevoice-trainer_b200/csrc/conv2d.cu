@@ -13,6 +13,9 @@
 //                  ring in the 128-byte-swizzle layout, operands rounded to TF32 in shared memory.
 //                * mma.sync m16n8k8: everything else (the 2-channel first layer, the bridges) and 3xTF32 under
 //                  evk_set_precise(1).  Eight warps of 32 x 32 over 64 columns, a 3-stage cp.async ring.
+//                * conv2d_fwd_h16 (evk_conv2d_fwd_h16, the 16-bit compute types): fp16 / bf16 wgmma with the same tiles,
+//                  the activations gathered as fp32 into registers and rounded on their way to shared memory, the packed
+//                  16-bit weight by cp.async.  Every operand layout, so it has no fallback kernel.
 //                Kernel 1, 2 (the MDX23C 2x2 stride-2 downscale) or 3.
 //                Fused epilogue: y = act(acc * scale[n] + bias[n]).  Every output is summed over K in one fixed order
 //                that does not depend on the pixel's place in the launch, and there are no atomics, so a window gives
@@ -43,6 +46,23 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   if (act == EVK_C2_SIGMOID) return 1.f / (1.f + __expf(-v));
   if (act == EVK_C2_GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
   return v;
+}
+
+// Row geometry of the CTA's BM output pixels m0 .. m0 + BM - 1 (threads 0 .. BM - 1 each set one): the input's batch offset
+// and the top-left input pixel of the pixel's window; rows past M get a row index no tap can bring in bounds (zero rows).
+__device__ __forceinline__ void conv_rows(const ConvArgs& a, int m0, long long* rbase, int* riy, int* rix) {
+  const int tid = threadIdx.x, HWo = a.Ho * a.Wo;
+  if (tid < BM) {
+    const int m = m0 + tid;
+    if (m < a.M) {
+      const int b = m / HWo, r = m - b * HWo, oy = r / a.Wo, ox = r - oy * a.Wo;
+      rbase[tid] = (long long)b * a.x_bs;
+      riy[tid] = oy * a.stride - a.pad_h;
+      rix[tid] = ox * a.stride - a.pad_w;
+    } else {
+      rbase[tid] = 0; riy[tid] = -(1 << 29); rix[tid] = 0;      // never in bounds -> zero rows
+    }
+  }
 }
 
 constexpr int STAGES = 3;
@@ -120,17 +140,7 @@ __global__ void __launch_bounds__(NT, 2) conv2d_fwd_kernel(ConvArgs a) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, gq = lane >> 2, t = lane & 3;
   const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
   const int HWo = a.Ho * a.Wo;
-  if (tid < BM) {
-    const int m = m0 + tid;
-    if (m < a.M) {
-      const int b = m / HWo, r = m - b * HWo, oy = r / a.Wo, ox = r - oy * a.Wo;
-      rbase[tid] = (long long)b * a.x_bs;
-      riy[tid] = oy * a.stride - a.pad_h;
-      rix[tid] = ox * a.stride - a.pad_w;
-    } else {
-      rbase[tid] = 0; riy[tid] = -(1 << 29); rix[tid] = 0;      // never in bounds -> zero rows
-    }
-  }
+  conv_rows(a, m0, rbase, riy, rix);
   __syncthreads();
 
   float acc[2][4][4];
@@ -291,6 +301,31 @@ __device__ __forceinline__ void round_slab_tf32(uint32_t sA, uint32_t sB) {
   }
 }
 
+// Epilogue of a warpgroup's 64 x BNW accumulator tile at output rows m0 .. m0 + 63, columns n0 ..: thread tw holds rows
+// 16 (tw / 32) + (tw % 32) / 4 (+ 8) and columns 8 j + 2 (tw % 4) (+ 1), acc[4 j + 2 h + e]; y = act(acc * scale + bias).
+template <int BNW>
+__device__ __forceinline__ void store_tile_wg(const ConvArgs& a, const float (&acc)[BNW / 2], int m0, int n0, int tw) {
+  const int HWo = a.Ho * a.Wo;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = m0 + 16 * (tw >> 5) + ((tw & 31) >> 2) + 8 * h;
+    if (m >= a.M) continue;
+    const int b = m / HWo, r = m - b * HWo;
+    float* yr = a.y + (long long)b * a.y_bs + (long long)r * a.y_pitch;
+#pragma unroll
+    for (int j = 0; j < BNW / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int n = n0 + 8 * j + 2 * (tw & 3) + e;
+        if (n >= a.N) continue;
+        float v = acc[4 * j + 2 * h + e];
+        if (a.scale) v *= __ldg(a.scale + n);
+        if (a.bias) v += __ldg(a.bias + n);
+        yr[n] = apply_act(v, a.act);
+      }
+  }
+}
+
 template <int BNW>
 __global__ void __launch_bounds__(NT, 1) conv2d_fwd_wgmma_kernel(ConvArgs a) {
   extern __shared__ __align__(16) unsigned char wsm[];
@@ -298,18 +333,7 @@ __global__ void __launch_bounds__(NT, 1) conv2d_fwd_wgmma_kernel(ConvArgs a) {
   __shared__ int riy[BM], rix[BM];
   const int tid = threadIdx.x, wg = tid >> 7, tw = tid & 127;
   const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BNW;
-  const int HWo = a.Ho * a.Wo;
-  if (tid < BM) {
-    const int m = m0 + tid;
-    if (m < a.M) {
-      const int b = m / HWo, r = m - b * HWo, oy = r / a.Wo, ox = r - oy * a.Wo;
-      rbase[tid] = (long long)b * a.x_bs;
-      riy[tid] = oy * a.stride - a.pad_h;
-      rix[tid] = ox * a.stride - a.pad_w;
-    } else {
-      rbase[tid] = 0; riy[tid] = -(1 << 29); rix[tid] = 0;
-    }
-  }
+  conv_rows(a, m0, rbase, riy, rix);
   __syncthreads();
   const uint32_t base = (smem_u32(wsm) + 1023u) & ~1023u;   // swizzle atoms are 1024-byte aligned
   constexpr uint32_t SB = wg_stage_bytes<BNW>();
@@ -346,26 +370,7 @@ __global__ void __launch_bounds__(NT, 1) conv2d_fwd_wgmma_kernel(ConvArgs a) {
     wgmma_wait<0>();
   }
   cp_async_wait<0>();
-
-  // thread tw holds rows 16 (tw / 32) + (tw % 32) / 4 (+ 8) and columns 8 j + 2 (tw % 4) (+ 1): acc[4 j + 2 h + e]
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int m = m0 + wg * 64 + 16 * (tw >> 5) + ((tw & 31) >> 2) + 8 * h;
-    if (m >= a.M) continue;
-    const int b = m / HWo, r = m - b * HWo;
-    float* yr = a.y + (long long)b * a.y_bs + (long long)r * a.y_pitch;
-#pragma unroll
-    for (int j = 0; j < BNW / 8; ++j)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int n = n0 + 8 * j + 2 * (tw & 3) + e;
-        if (n >= a.N) continue;
-        float v = acc[4 * j + 2 * h + e];
-        if (a.scale) v *= __ldg(a.scale + n);
-        if (a.bias) v += __ldg(a.bias + n);
-        yr[n] = apply_act(v, a.act);
-      }
-  }
+  store_tile_wg<BNW>(a, acc, m0 + wg * 64, n0, tw);
 }
 
 template <int BNW>
@@ -381,6 +386,163 @@ int launch_conv_wgmma(const ConvArgs& a, cudaStream_t st) {
   EVK_REQUIRE(grid.y <= 65535, EVK_ERR_ARG, "conv2d: too many output channels");
   conv2d_fwd_wgmma_kernel<BNW><<<grid, NT, wg_smem<BNW>(), st>>>(a);
   return check_launch("conv2d_fwd_wgmma");
+}
+
+// ---- 16-bit path (evk_conv2d_fwd_h16): fp16 / bf16 wgmma, two consumer warpgroups of 64 rows x BNW columns -------------
+// K slabs of 64 16-bit values, one 128-byte swizzle row per pixel and per output channel, in the layout of the TF32 path.
+// The packed weight [N][ldw] streams through a 3-stage cp.async ring.  The activations are gathered as fp32 into registers
+// one slab ahead: while the wgmma of slab kt runs, each thread rounds slab kt + 1 (cvt.rn, to_h16x2) into the free half of
+// a 2-slab ring and issues the loads of slab kt + 2.  No pass over x is made outside the kernel, so any channel count, pitch
+// and offset is read in place: VW = 4 (16-byte loads) when C, x_pitch, x_bs are multiples of 4 and x is 16-byte aligned,
+// VW = 2 (8-byte) for multiples of 2 and 8-byte alignment, else VW = 1.  Thread t stages k columns 4 (t % 16) .. + 3 of rows
+// t / 16 + 16 i.
+constexpr int HK = 64, H_STAGES = 3;
+template <int BNW>
+constexpr int h16_smem() { return 2 * BM * 128 + H_STAGES * BNW * 128 + 1024; }
+
+struct ConvArgsH16 : ConvArgs {
+  const uint16_t* w16;
+  int ldw;
+};
+
+template <int VW>
+__device__ __forceinline__ void gather_h16(const ConvArgs& a, float (&v)[BM / 16][4], int k0, const long long* rbase,
+                                           const int* riy, const int* rix) {
+  const int q = threadIdx.x & 15, rr = threadIdx.x >> 4;
+#pragma unroll
+  for (int s = 0; s < 4 / VW; ++s) {
+    const int k = k0 + 4 * q + s * VW;        // VW consecutive k are VW channels of one tap (C % VW == 0)
+    const bool kin = k < a.Kt;
+    int c = 0, dy = 0, dx = 0;
+    if (kin) {
+      const int tap = k / a.C;
+      c = k - tap * a.C;
+      const int ky = tap / a.k;
+      dy = ky * a.dil_h;
+      dx = (tap - ky * a.k) * a.dil_w;
+    }
+#pragma unroll
+    for (int i = 0; i < BM / 16; ++i) {
+      const int r = rr + 16 * i;
+      const int iy = riy[r] + dy, ix = rix[r] + dx;
+      const bool ok = kin && iy >= 0 && iy < a.H && ix >= 0 && ix < a.W;
+      const float* src = a.x + rbase[r] + (long long)(iy * a.W + ix) * a.x_pitch + c;
+      if constexpr (VW == 4) {
+        const float4 t = ok ? __ldg(reinterpret_cast<const float4*>(src)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        v[i][0] = t.x; v[i][1] = t.y; v[i][2] = t.z; v[i][3] = t.w;
+      } else if constexpr (VW == 2) {
+        const float2 t = ok ? __ldg(reinterpret_cast<const float2*>(src)) : make_float2(0.f, 0.f);
+        v[i][2 * s] = t.x; v[i][2 * s + 1] = t.y;
+      } else {
+        v[i][s] = ok ? __ldg(src) : 0.f;
+      }
+    }
+  }
+}
+
+// h(v) into the A slab at sA: 8 bytes per row, chunk (4 q) / 8 of row r at its swizzled place
+template <bool BF16>
+__device__ __forceinline__ void store_h16(uint32_t sA, const float (&v)[BM / 16][4]) {
+  const int q = threadIdx.x & 15, rr = threadIdx.x >> 4;
+#pragma unroll
+  for (int i = 0; i < BM / 16; ++i) {
+    const int r = rr + 16 * i;
+    const uint32_t addr = sA + r * 128 + (((q >> 1) ^ (r & 7)) << 4) + ((q & 1) << 3);
+    asm volatile("st.shared.v2.b32 [%0], {%1, %2};\n" ::"r"(addr), "r"(to_h16x2<BF16>(v[i][0], v[i][1])),
+                 "r"(to_h16x2<BF16>(v[i][2], v[i][3])) : "memory");
+  }
+}
+
+// weight columns k0 .. k0 + 63 of output channels n0 .. n0 + BNW - 1 (zero past N); k0 + 63 < ldw always
+template <int BNW>
+__device__ __forceinline__ void load_w_h16(const ConvArgsH16& a, uint32_t sB, int k0, int n0) {
+  const int ch = threadIdx.x & 7;
+#pragma unroll
+  for (int r = threadIdx.x >> 3; r < BNW; r += NT / 8) {
+    const int n = n0 + r;
+    const bool ok = n < a.N;
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(sB + r * 128 + ((ch ^ (r & 7)) << 4)),
+                 "l"(ok ? a.w16 + (long long)n * a.ldw + k0 + ch * 8 : a.w16), "r"(ok ? 16 : 0));
+  }
+}
+
+template <int BNW, int VW, bool BF16>
+__global__ void __launch_bounds__(NT, BNW <= 64 ? 2 : 1) conv2d_fwd_h16_kernel(ConvArgsH16 a) {
+  extern __shared__ __align__(16) unsigned char hsm[];
+  __shared__ long long rbase[BM];
+  __shared__ int riy[BM], rix[BM];
+  const int wg = threadIdx.x >> 7, tw = threadIdx.x & 127;
+  const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BNW;
+  conv_rows(a, m0, rbase, riy, rix);
+  __syncthreads();
+  const uint32_t sA = (smem_u32(hsm) + 1023u) & ~1023u, sB = sA + 2 * BM * 128;
+  constexpr uint32_t SA = BM * 128, SB = BNW * 128;
+  float acc[BNW / 2];
+#pragma unroll
+  for (int i = 0; i < BNW / 2; ++i) acc[i] = 0.f;
+
+  const int nk = (a.Kt + HK - 1) / HK;
+#pragma unroll
+  for (int s = 0; s < H_STAGES - 1; ++s) {
+    if (s < nk) load_w_h16<BNW>(a, sB + s * SB, s * HK, n0);
+    cp_async_commit();
+  }
+  float v[BM / 16][4];
+  gather_h16<VW>(a, v, 0, rbase, riy, rix);
+  store_h16<BF16>(sA, v);
+  if (nk > 1) gather_h16<VW>(a, v, HK, rbase, riy, rix);
+  for (int kt = 0; kt < nk; ++kt) {
+    cp_async_wait<H_STAGES - 2>();
+    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+    __syncthreads();                  // A and B of slab kt visible to the tensor core; slab kt - 1 no longer read
+    {
+      const int nx = kt + H_STAGES - 1;
+      if (nx < nk) load_w_h16<BNW>(a, sB + (nx % H_STAGES) * SB, nx * HK, n0);
+      cp_async_commit();
+    }
+    const uint64_t da = wg_desc_sw128(sA + (kt & 1) * SA + wg * 64 * 128), db = wg_desc_sw128(sB + (kt % H_STAGES) * SB);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < HK / 16; ++ks) WgmmaH16<BNW, BF16>::run(acc, da + 2 * ks, db + 2 * ks);   // +32 B per K step
+    wgmma_commit();
+    if (kt + 1 < nk) {                // under the wgmma: round slab kt + 1 into the other half, load slab kt + 2
+      store_h16<BF16>(sA + ((kt + 1) & 1) * SA, v);
+      if (kt + 2 < nk) gather_h16<VW>(a, v, (kt + 2) * HK, rbase, riy, rix);
+    }
+    wgmma_wait<0>();
+  }
+  cp_async_wait<0>();
+  store_tile_wg<BNW>(a, acc, m0 + wg * 64, n0, tw);
+}
+
+template <int BNW, int VW, bool BF16>
+int launch_conv_h16(const ConvArgsH16& a, cudaStream_t st) {
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(conv2d_fwd_h16_kernel<BNW, VW, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         h16_smem<BNW>());
+    EVK_REQUIRE(e == cudaSuccess, EVK_ERR_CUDA, "conv2d_h16: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+    attr = true;
+  }
+  dim3 grid(cdiv(a.M, BM), cdiv(a.N, BNW));
+  EVK_REQUIRE(grid.y <= 65535, EVK_ERR_ARG, "conv2d_h16: too many output channels");
+  conv2d_fwd_h16_kernel<BNW, VW, BF16><<<grid, NT, h16_smem<BNW>(), st>>>(a);
+  return check_launch("conv2d_fwd_h16");
+}
+
+template <int BNW, bool BF16>
+int launch_conv_h16_vw(const ConvArgsH16& a, int vw, cudaStream_t st) {
+  if (vw == 4) return launch_conv_h16<BNW, 4, BF16>(a, st);
+  if (vw == 2) return launch_conv_h16<BNW, 2, BF16>(a, st);
+  return launch_conv_h16<BNW, 1, BF16>(a, st);
+}
+
+template <bool BF16>
+int launch_conv_h16_n(const ConvArgsH16& a, int vw, cudaStream_t st) {
+  if (a.N <= 16) return launch_conv_h16_vw<16, BF16>(a, vw, st);
+  if (a.N <= 32) return launch_conv_h16_vw<32, BF16>(a, vw, st);
+  if (a.N <= 64) return launch_conv_h16_vw<64, BF16>(a, vw, st);
+  return launch_conv_h16_vw<128, BF16>(a, vw, st);
 }
 
 template <bool PR, bool VEC>
@@ -508,10 +670,11 @@ extern int g_precise;
 
 using namespace evk;
 
-extern "C" int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale,
-                              const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W,
-                              int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h,
-                              int32_t dil_w, int32_t act, cudaStream_t st) {
+namespace {
+// The operand checks and the geometry both conv2d entry points share -> a (0 on success)
+int conv_args(ConvArgs& a, const float* x, int32_t x_pitch, int64_t x_bs, const void* w, const float* scale, const float* bias,
+              float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W, int32_t C, int32_t N, int32_t k,
+              int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h, int32_t dil_w, int32_t act) {
   EVK_REQUIRE(x && w && y, EVK_ERR_ARG, "conv2d: null tensor");
   EVK_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && N > 0, EVK_ERR_ARG, "conv2d: bad sizes B=%d H=%d W=%d C=%d N=%d", B, H, W,
               C, N);
@@ -526,9 +689,21 @@ extern "C" int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, con
   const long long M = (long long)B * Ho * Wo, Kt = (long long)k * k * C;
   EVK_REQUIRE(M < (1ll << 31) && Kt < (1ll << 31) && (long long)N * Kt < (1ll << 31) && (long long)H * W < (1 << 30),
               EVK_ERR_ARG, "conv2d: problem too large");
-  ConvArgs a{x, w, scale, bias, y, x_bs, y_bs, x_pitch, y_pitch, B, H, W, C, N, k, stride,
-             pad_h, pad_w, dil_h, dil_w, Ho, Wo, (int)M, (int)Kt, act};
-  dim3 grid(cdiv(M, BM), cdiv(N, BN));
+  a = ConvArgs{x, static_cast<const float*>(w), scale, bias, y, x_bs, y_bs, x_pitch, y_pitch, B, H, W, C, N, k, stride,
+               pad_h, pad_w, dil_h, dil_w, Ho, Wo, (int)M, (int)Kt, act};
+  return 0;
+}
+}  // namespace
+
+extern "C" int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, const float* scale,
+                              const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W,
+                              int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h,
+                              int32_t dil_w, int32_t act, cudaStream_t st) {
+  ConvArgs a;
+  if (int e = conv_args(a, x, x_pitch, x_bs, w, scale, bias, y, y_pitch, y_bs, B, H, W, C, N, k, stride, pad_h, pad_w, dil_h,
+                        dil_w, act))
+    return e;
+  dim3 grid(cdiv(a.M, BM), cdiv(N, BN));
   EVK_REQUIRE(grid.y <= 65535, EVK_ERR_ARG, "conv2d: too many output channels");
   const bool vec = C % 4 == 0 && x_pitch % 4 == 0 && x_bs % 4 == 0 && (uintptr_t)x % 16 == 0 && (uintptr_t)w % 16 == 0;
   // 3xTF32 splits the operands in registers, so it runs on mma.sync; so do operands the 16-byte copies cannot read
@@ -537,6 +712,25 @@ extern "C" int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, con
   if (N <= 32) return launch_conv_wgmma<32>(a, st);
   if (N <= 64) return launch_conv_wgmma<64>(a, st);
   return launch_conv_wgmma<128>(a, st);
+}
+
+extern "C" int evk_conv2d_fwd_h16(const float* x, int32_t x_pitch, int64_t x_bs, const void* w, int32_t ldw, int32_t bf16,
+                                  const float* scale, const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B,
+                                  int32_t H, int32_t W, int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad_h,
+                                  int32_t pad_w, int32_t dil_h, int32_t dil_w, int32_t act, cudaStream_t st) {
+  ConvArgsH16 a;
+  if (int e = conv_args(a, x, x_pitch, x_bs, w, scale, bias, y, y_pitch, y_bs, B, H, W, C, N, k, stride, pad_h, pad_w, dil_h,
+                        dil_w, act))
+    return e;
+  EVK_REQUIRE(ldw % HK == 0 && ldw >= a.Kt && (uintptr_t)w % 16 == 0, EVK_ERR_ARG,
+              "conv2d_h16: packed weight pitch %d (a multiple of 64, at least k*k*C = %d, 16-byte aligned)", ldw, a.Kt);
+  a.w = nullptr;
+  a.w16 = static_cast<const uint16_t*>(w);
+  a.ldw = ldw;
+  const int vw = C % 4 == 0 && x_pitch % 4 == 0 && x_bs % 4 == 0 && (uintptr_t)x % 16 == 0   ? 4
+                 : C % 2 == 0 && x_pitch % 2 == 0 && x_bs % 2 == 0 && (uintptr_t)x % 8 == 0 ? 2
+                                                                                             : 1;
+  return bf16 ? launch_conv_h16_n<true>(a, vw, st) : launch_conv_h16_n<false>(a, vw, st);
 }
 
 extern "C" int evk_dwconv3x3_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, float* y, int32_t y_pitch,

@@ -1,5 +1,5 @@
-// Hopper (sm_90a) warpgroup MMA helpers shared by the tensor-core kernels: TF32 (gemm_tma.cu, gconv_tc.cu) and 16-bit
-// (linear_h16.cu), with the mbarrier / TMA plumbing of the TMA-fed ones.
+// Hopper (sm_90a) warpgroup MMA helpers shared by the tensor-core kernels: TF32 (gemm_tma.cu, gconv_tc.cu, conv2d.cu) and
+// 16-bit (linear_h16.cu, conv2d.cu), with the mbarrier / TMA plumbing of the TMA-fed ones.
 //
 // wgmma.mma_async m64nNk8 f32 += tf32 * tf32: one warpgroup (four consecutive warps, the first warp id a multiple of 4)
 // multiplies a 64 x 8 A tile by an 8 x N B tile, both read from shared memory through matrix descriptors and both K-major
@@ -120,6 +120,66 @@ __device__ __forceinline__ void wgmma_h16_n128(float (&d)[64], uint64_t a, uint6
         : "l"(a), "l"(b), "r"(accum));
   }
 }
+
+// The same instruction with N = 16, 32, 64 or 128 columns, always accumulating into d (the 2-D convolution's column tiles,
+// conv2d.cu): WgmmaH16<N, BF16>::run(d, a, b).
+template <int N, bool BF16>
+struct WgmmaH16;
+template <bool BF16>
+struct WgmmaH16<128, BF16> {
+  static __device__ __forceinline__ void run(float (&d)[64], uint64_t a, uint64_t b) { wgmma_h16_n128<BF16>(d, a, b, 1u); }
+};
+template <bool BF16>
+struct WgmmaH16<16, BF16> {
+  static __device__ __forceinline__ void run(float (&d)[8], uint64_t a, uint64_t b) {
+    if constexpr (BF16)
+      asm volatile(
+          "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+          "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+          : "l"(a), "l"(b));
+    else
+      asm volatile(
+          "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+          "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+          : "l"(a), "l"(b));
+  }
+};
+template <bool BF16>
+struct WgmmaH16<32, BF16> {
+  static __device__ __forceinline__ void run(float (&d)[16], uint64_t a, uint64_t b) {
+    if constexpr (BF16)
+      asm volatile(
+          "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+          "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+          : "l"(a), "l"(b));
+    else
+      asm volatile(
+          "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+          "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+          : "l"(a), "l"(b));
+  }
+};
+template <bool BF16>
+struct WgmmaH16<64, BF16> {
+  static __device__ __forceinline__ void run(float (&d)[32], uint64_t a, uint64_t b) {
+    if constexpr (BF16)
+      asm volatile(
+          "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+          "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+          : "l"(a), "l"(b));
+    else
+      asm volatile(
+          "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+          "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+          : "l"(a), "l"(b));
+  }
+};
 
 // ---- mbarrier and TMA plumbing of the TMA-fed kernels (gemm_tma.cu, linear_h16.cu) ----------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {

@@ -12,6 +12,10 @@ conv into the lower ones.  Every conv and Linear is preceded by InstanceNorm + G
   * the 8192-point STFT and iSTFT: evk_stft_fwd / evk_istft, with evk_mdx_front / evk_mdx_back for cac2cws / cws2cac;
   * the shortcut adds, and the last one's `x * first_conv_out`: evk_mdx_add.
 Every contraction honours evk_set_precise(1) (3xTF32).
+
+set_compute_type(torch.float16 / torch.bfloat16) runs every evk_conv2d_fwd call on evk_conv2d_fwd_h16 instead (the fp32 input
+and the conv weight rounded to 16 bits, fp32 accumulation and epilogue): the 3x3s, the 1x1s, the shortcuts, the 2x2
+downscales and final_conv.  The instance norms, GELU, the TDF Linears, the transposed convs, the STFT and the iSTFT stay fp32.
 """
 import os
 from collections.abc import Mapping
@@ -111,6 +115,8 @@ class MDX23C:
         self.D = 2 * self.S * self.k
         self.device = torch.device("cpu")
         self.w = None
+        self.compute_type = None
+        self._h16 = {}
 
     # ---- weights -------------------------------------------------------------------------------------------------------
     def _tfc_tdf_shapes(self, p, in_c, c, f):
@@ -160,13 +166,39 @@ class MDX23C:
             w[k] = v.contiguous()
         self.host_w = w
         self.w = to_device(w, self.device)
+        self._h16 = {}
         return self
 
     def to(self, device):
         self.device = torch.device(device)
         if self.w is not None:
             self.w = to_device(self.host_w, self.device)
+        self._h16 = {}
         return self
+
+    def set_compute_type(self, dtype):
+        """None: fp32 activations with TF32 products (the default); torch.float16 or torch.bfloat16: every convolution but
+        the transposed ones on evk_conv2d_fwd_h16.  The 16-bit conv weights are packed on first use and kept per compute
+        type.  -> self."""
+        if dtype is not None and dtype not in ops.H16_TYPES:
+            raise ValueError(f"compute type {dtype!r} (None, torch.float16 or torch.bfloat16)")
+        self.compute_type = dtype
+        return self
+
+    def _h16_weights(self):
+        """{key: PackedH16} of every conv weight (4-D, not a transposed conv) for the current 16-bit compute type"""
+        key = str(self.compute_type)
+        if key not in self._h16:
+            self._h16[key] = {k: ops.pack_conv_h16(v, self.compute_type) for k, v in self.w.items()
+                              if v.dim() == 4 and ".upscale." not in k}
+        return self._h16[key]
+
+    def _conv(self, key, x: CLView, y: CLView, k, stride=1, pad=0, act=ops.C2_NONE):
+        """the conv of weight `key` on the compute type's kernel: evk_conv2d_fwd, or evk_conv2d_fwd_h16"""
+        if self.compute_type is None:
+            ops.conv2d(x, self.w[key], y, k=k, stride=stride, pad=pad, act=act)
+        else:
+            ops.conv2d_h16(x, self._h16_weights()[key], y, k=k, stride=stride, pad=pad, act=act)
 
     def eval(self):
         """Inference only already: returns self, so `SeparateMDXC.separate`'s model.eval() works."""
@@ -203,12 +235,12 @@ class MDX23C:
         return out
 
     @classmethod
-    def from_pretrained(cls, path, config=None, device="cuda"):
+    def from_pretrained(cls, path, config=None, device="cuda", compute_type=None):
         """An MDX23C with the weights of a reference checkpoint file, on `device`.  What the weights determine is inferred
         (infer_config); the STFT, chunk and subband settings come from `config` (a mapping, an attribute object or a YAML
-        path) or DEFAULT_CONFIG."""
+        path) or DEFAULT_CONFIG.  compute_type: as set_compute_type."""
         sd = torch.load(path, map_location="cpu", weights_only=True)
-        return cls(cls.infer_config(sd, config)).to(device).load_state_dict(sd)
+        return cls(cls.infer_config(sd, config)).to(device).load_state_dict(sd).set_compute_type(compute_type)
 
     # ---- forward -------------------------------------------------------------------------------------------------------
     def _norm(self, key, x: CLView):
@@ -222,15 +254,15 @@ class MDX23C:
             q = f"{p}.blocks.{j}"
             last = j == self.l - 1
             s = new(W, c)
-            ops.conv2d(x, self.w[q + ".shortcut.weight"], s, k=1)
+            self._conv(q + ".shortcut.weight", x, s, k=1)
             t = new(W, c)
-            ops.conv2d(self._norm(q + ".tfc1.0", x), self.w[q + ".tfc1.2.weight"], t, k=3, pad=1)
+            self._conv(q + ".tfc1.2.weight", self._norm(q + ".tfc1.0", x), t, k=3, pad=1)
             u = new(W // self.bn, c)
             ops.mdx_tdf(self._norm(q + ".tdf.0", t), self.w[q + ".tdf.2.weight"], u)
             ops.mdx_tdf(self._norm(q + ".tdf.3", u), self.w[q + ".tdf.5.weight"], t, res=t)
             del u
             t3 = new(W, c)
-            ops.conv2d(self._norm(q + ".tfc2.0", t), self.w[q + ".tfc2.2.weight"], t3, k=3, pad=1)
+            self._conv(q + ".tfc2.2.weight", self._norm(q + ".tfc2.0", t), t3, k=3, pad=1)
             del t
             y = out if last else new(W, c)
             ops.mdx_add(t3, s, y, mul if last else None)
@@ -266,7 +298,7 @@ class MDX23C:
         mix = ops.mdx_front(cplx, B, S, k, F, CLView(fin, 0, D))
         del cplx
         first = CLView(torch.empty((B, T, F, c), device=dev))
-        ops.conv2d(mix, self.w["first_conv.weight"], first, k=1)
+        self._conv("first_conv.weight", mix, first, k=1)
         x, h, wd, skips = first, T, F, []
         for i in range(self.n):
             cat = torch.empty((B, h, wd, 2 * c), device=dev)
@@ -274,7 +306,7 @@ class MDX23C:
             skips.append(cat)
             p = f"encoder_blocks.{i}.downscale.conv"
             x = CLView(torch.empty((B, h // 2, wd // 2, c + g), device=dev))
-            ops.conv2d(self._norm(p + ".0", enc), self.w[p + ".2.weight"], x, k=2, stride=2)
+            self._conv(p + ".2.weight", self._norm(p + ".0", enc), x, k=2, stride=2)
             c, h, wd = c + g, h // 2, wd // 2
         if self.n == 0:       # the bottleneck is the last block: its output goes straight to final_conv's input
             self._tfc_tdf("bottleneck_block", x, CLView(fin, D, c), first)
@@ -290,10 +322,10 @@ class MDX23C:
             x = self._tfc_tdf(f"decoder_blocks.{i}.tfc_tdf", CLView(cat), out, first if last else None)
             del cat
         h1 = CLView(torch.empty((B, T, F, c), device=dev))
-        ops.conv2d(CLView(fin), self.w["final_conv.0.weight"], h1, k=1, act=ops.C2_GELU)
+        self._conv("final_conv.0.weight", CLView(fin), h1, k=1, act=ops.C2_GELU)
         del fin
         o = CLView(torch.empty((B, T, F, self.nt * D), device=dev))
-        ops.conv2d(h1, self.w["final_conv.2.weight"], o, k=1)
+        self._conv("final_conv.2.weight", h1, o, k=1)
         del h1
         spec = ops.mdx_back(o, self.nt, S, k, NB)
         del o

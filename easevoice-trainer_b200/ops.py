@@ -2110,6 +2110,27 @@ def conv2d(x: CLView, w, y: CLView, *, k, stride=1, pad=0, dil=1, scale=None, bi
             x.B, x.H, x.W, x.C, N, k, stride, ph, pw, dh, dw, act, tag=f"k{k}")
 
 
+def pack_conv_h16(w, dtype):
+    """Conv weight [N, k, k, C] (the layout conv2d takes) -> PackedH16 [N, k*k*C rounded up to 64] rounded to `dtype`
+    (torch.float16 or torch.bfloat16) to nearest even, K = k*k*C, the layout evk_conv2d_fwd_h16 reads.  A weight that is
+    already exactly 16-bit keeps its bits."""
+    assert w.dim() == 4 and w.shape[1] == w.shape[2], w.shape
+    return pack_weight_h16(w.reshape(w.shape[0], -1), dtype)
+
+
+def conv2d_h16(x: CLView, w, y: CLView, *, k, stride=1, pad=0, dil=1, scale=None, bias=None, act=C2_NONE):
+    """conv2d with 16-bit products (evk_conv2d_fwd_h16): h(x) . h(w) accumulated in fp32, then act(acc * scale + bias) in
+    fp32.  w: pack_conv_h16 of the [N, k, k, C] weight; the other arguments as for conv2d."""
+    N = w.w.shape[0]
+    assert w.K == k * k * x.C and y.C == N and y.B == x.B, (w.K, k, x.C, y.C)
+    (ph, pw), (dh, dw) = [v if isinstance(v, (tuple, list)) else (v, v) for v in (pad, dil)]
+    Ho, Wo = conv2d_out(x.H, k, stride, ph, dh), conv2d_out(x.W, k, stride, pw, dw)
+    assert (y.H, y.W) == (Ho, Wo), ((y.H, y.W), (Ho, Wo))
+    _call_f("evk_conv2d_fwd_h16", 2.0 * x.B * Ho * Wo * N * k * k * x.C, *x.args(), _p(w.w), w.w.shape[1],
+            int(w.w.dtype == torch.bfloat16), _p(scale), _p(bias), *y.args(), x.B, x.H, x.W, x.C, N, k, stride, ph, pw, dh, dw,
+            act, tag=f"k{k}")
+
+
 def dwconv3x3(x: CLView, w, y: CLView, dil):
     """depthwise 3x3, stride 1, padding = dil (evk_dwconv3x3_fwd): w [C, 9]"""
     assert w.is_contiguous() and tuple(w.shape) == (x.C, 9) and (y.B, y.H, y.W, y.C) == (x.B, x.H, x.W, x.C)

@@ -13,6 +13,12 @@ once.  Activations are channels-last fp32; a layer writes straight into its slic
     buffer, so cat([x, aux1]) and cat([x, aux1, aux2]) are never built.
 Eval BatchNorm is folded into a per-channel scale and bias of the preceding convolution at load; Dropout is the identity.
 
+set_compute_type(torch.float16 / torch.bfloat16) (the reference's is_half) runs every convolution that evk_conv2d_fwd runs in
+fp32 on evk_conv2d_fwd_h16 instead: the fp32 input and the unscaled conv weight rounded to 16 bits, fp32 accumulation, and
+the BatchNorm scale, bias and activation in the fp32 epilogue.  That is every k, both strides, the dilated ASPP branches,
+the bridges and the LSTM module's 1x1.  The depthwise 3x3s, the bilinear resizes, mean_h, the LSTM's projections and
+recurrence and the mask head stay fp32.
+
 separate_wave runs the whole of SeparateVR.separate (uvr5/separate.py:103-196) from the decoded 44.1 kHz waveform to the two
 output waveforms on the device: the band loop's polyphase resampling, the per-band STFTs written into the combined
 spectrogram, the net, and per output the mask, mirroring, band filters, per-band iSTFTs and the FFT resampling that chains
@@ -119,12 +125,31 @@ class _SpecNet:
         self.offset = offset
         self.device = torch.device("cpu")
         self.layers = None
+        self.compute_type = None
+        self._h16 = {}
 
     def to(self, device):
         self.device = torch.device(device)
         if self.layers is not None:
             self.layers = to_device(self.layers, self.device)
+        self._h16 = {}
         return self
+
+    def set_compute_type(self, dtype):
+        """None: fp32 activations with TF32 products (the default); torch.float16 or torch.bfloat16: every convolution on
+        evk_conv2d_fwd_h16.  The 16-bit conv weights are packed on first use and kept per compute type.  -> self."""
+        if dtype is not None and dtype not in ops.H16_TYPES:
+            raise ValueError(f"compute type {dtype!r} (None, torch.float16 or torch.bfloat16)")
+        self.compute_type = dtype
+        return self
+
+    def _h16_weights(self):
+        """{layer: PackedH16} of every conv weight, unscaled (the BatchNorm scale stays in the fp32 epilogue), for the
+        current 16-bit compute type"""
+        key = str(self.compute_type)
+        if key not in self._h16:
+            self._h16[key] = {p: ops.pack_conv_h16(L["w"], self.compute_type) for p, L in self.layers.items() if "k" in L}
+        return self._h16[key]
 
     def eval(self):
         return self
@@ -157,7 +182,11 @@ class _SpecNet:
         L = self.layers[p]
         k = L["k"]
         pad = tuple(d * (k // 2) for d in dil) if isinstance(dil, tuple) else dil * (k // 2)
-        ops.conv2d(x, L["w"], y, k=k, stride=stride, pad=pad, dil=dil, scale=L["scale"], bias=L["bias"], act=act)
+        if self.compute_type is None:
+            ops.conv2d(x, L["w"], y, k=k, stride=stride, pad=pad, dil=dil, scale=L["scale"], bias=L["bias"], act=act)
+        else:
+            ops.conv2d_h16(x, self._h16_weights()[p], y, k=k, stride=stride, pad=pad, dil=dil, scale=L["scale"],
+                           bias=L["bias"], act=act)
 
 
 class CascadedASPPNet(_SpecNet):
@@ -188,15 +217,16 @@ class CascadedASPPNet(_SpecNet):
                 layers[p] = dict(dw=sd[p + ".conv.0.weight"].float().reshape(shape[0], 9).contiguous(),
                                  w=_cl_weight(sd[p + ".conv.1.weight"]), scale=scale, bias=bias, k=1)
         self.layers = to_device(layers, self.device)
+        self._h16 = {}
         return self
 
     @classmethod
-    def from_pretrained(cls, path, n_fft=1344, device="cuda"):
+    def from_pretrained(cls, path, n_fft=1344, device="cuda", compute_type=None):
         """Load a VR-net .pth (HP2 / HP3 / HP5 ...): the parameter set is read from the weight shapes (band-net width from
         enc1, `enlarge` from the presence of aspp.conv6 / conv7).  Weights that match no get_nets_model set raise
-        ValueError."""
+        ValueError.  compute_type: as set_compute_type."""
         sd = torch.load(path, map_location="cpu", weights_only=True)
-        return cls(n_fft, infer_size(sd)).to(device).load_state_dict(sd)
+        return cls(n_fft, infer_size(sd)).to(device).load_state_dict(sd).set_compute_type(compute_type)
 
     # ---- forward -----------------------------------------------------------------------------------------
     def forward(self, x, aggressiveness=None):
@@ -468,14 +498,16 @@ class CascadedNet(_SpecNet):
                 b_d = ((sd[p + ".dense.0.bias"].double() - mean) * sc + sd[bn + ".bias"].double()).float()
                 layers[p] = dict(w_ih=w_ih.contiguous(), b=b, w_hh=w_hh.contiguous(), w_d=w_d.contiguous(), b_d=b_d)
         self.layers = to_device(layers, self.device)
+        self._h16 = {}
         return self
 
     @classmethod
-    def from_pretrained(cls, path, n_fft=1344, device="cuda"):
+    def from_pretrained(cls, path, n_fft=1344, device="cuda", compute_type=None):
         """Load a DeEcho / DeReverb .pth: nout and nout_lstm are read from the weight shapes (64 for DeReverb, 48 for the
-        DeEcho models).  Weights that do not form a CascadedNet at this n_fft raise ValueError."""
+        DeEcho models).  Weights that do not form a CascadedNet at this n_fft raise ValueError.  compute_type: as
+        set_compute_type."""
         sd = torch.load(path, map_location="cpu", weights_only=True)
-        return cls(n_fft, *infer_echo_config(sd)).to(device).load_state_dict(sd)
+        return cls(n_fft, *infer_echo_config(sd)).to(device).load_state_dict(sd).set_compute_type(compute_type)
 
     # ---- forward -----------------------------------------------------------------------------------------
     def forward(self, x):

@@ -586,6 +586,24 @@ int evk_conv2d_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w
                    float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H, int32_t W, int32_t C, int32_t N, int32_t k,
                    int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h, int32_t dil_w, int32_t act,
                    evk_stream_t stream);
+/* evk_conv2d_fwd with 16-bit products (the VR, DeEcho / DeReverb and MDX23C float16 / bfloat16 compute types): the same
+ * operands, geometry and epilogue, and a packed 16-bit weight.  Numerical contract:
+ *   acc[m][n] = sum_k h(x[m][k]) * h(w[n][k])   over K = k*k*C in evk_conv2d_fwd's order (tap-major, channel-minor),
+ *   y = act(acc * scale[n] + bias[n])
+ * h = round to nearest even to fp16 (bf16 == 0) or bf16 (bf16 != 0): applied to the fp32 activations as they are staged
+ * (cvt.rn; values beyond fp16's range become +-inf as that cast makes them) and to the weight once, when it is packed.  A
+ * product of two 16-bit values is exact in fp32 and the accumulation is fp32; scale and bias stay in the fp32 epilogue
+ * (BatchNorm's scale is not folded into the 16-bit weight, so a weight from an fp16 checkpoint keeps its bits).  No atomics
+ * and no K split: every output is summed in one K order (slabs of 64 in K order) whatever B is, so a window's bits are the
+ * same alone or batched.  evk_set_precise has no effect here.  Any C, pitch and channel offset is read in place (16-, 8- or
+ * 4-byte loads as alignment allows); input channels outside [0, C) of a pixel are never read.
+ * w: [N][ldw] fp16 or bf16 bits, row n = w[n][ky][kx][c] in K order, ldw % 64 == 0, ldw >= k*k*C, columns past k*k*C zero,
+ * 16-byte aligned (ops.pack_conv_h16).  wgmma.m64nNk16 on tiles of 128 output pixels by 16 / 32 / 64 / 128 channels (the
+ * smallest that covers N, 128 for wider layers). */
+int evk_conv2d_fwd_h16(const float* x, int32_t x_pitch, int64_t x_bs, const void* w, int32_t ldw, int32_t bf16,
+                       const float* scale, const float* bias, float* y, int32_t y_pitch, int64_t y_bs, int32_t B, int32_t H,
+                       int32_t W, int32_t C, int32_t N, int32_t k, int32_t stride, int32_t pad_h, int32_t pad_w, int32_t dil_h,
+                       int32_t dil_w, int32_t act, evk_stream_t stream);
 /* Depthwise 3x3, stride 1, zero padding = dil: y[b,y,x,c] = sum_{i,j} w[c][i][j] x[b, y + (i-1) dil, x + (j-1) dil, c]
  * (fp32 FMA).  w: [C][3][3]. */
 int evk_dwconv3x3_fwd(const float* x, int32_t x_pitch, int64_t x_bs, const float* w, float* y, int32_t y_pitch,

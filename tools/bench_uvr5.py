@@ -37,6 +37,11 @@ It skips the rope_attn rates, whose shapes are the BS-Roformer's.
 --precision float16 | bfloat16 (with --net roformer or melroformer) adds an arm with that compute type
 (set_compute_type): its demix_track calls alternate with the fp32 arm's, and it gets its own peak memory, device-time split,
 rope_attn rates (evk_rope_attn_fwd_h16) and rel-L2 against the fp32 arm and against the stock PyTorch arms.
+With --net vr, deecho, dereverb or mdx23c (with or without --wave) it runs the library only, with the fp32 (TF32) arm and the
+16-bit arm alternating call by call on the same input (uvr5.inference on the 16 538-frame spectrogram, demix_track or
+separate_wave on the 3-minute mix): call times, peak memory per arm, the device time of one profiled forward split into the
+convolutions (evk_conv2d_fwd / evk_conv2d_fwd_h16, with their TFLOP/s from the layer shapes) and everything else, the rel-L2
+of the 16-bit output against the fp32 arm's, and whether the 16-bit output is finite.
 
 --net mdx23c measures MDX23C (mdx23c.py, the 8K-FFT InstVoc configuration with seeded weights) the same way on the same mix
 (31 chunks of 261 120 samples): demix_track wall time and peak memory, the device time of one profiled forward of
@@ -543,6 +548,74 @@ def wave_main(a):
     print(json.dumps(res))
 
 
+def h16_main(a):
+    """--precision float16 | bfloat16 with --net vr / deecho / dereverb / mdx23c (and --wave): the fp32 and 16-bit arms of
+    the library alternating in one process"""
+    assert torch.cuda.is_available(), "needs a GPU"
+    from easevoice_trainer_b200 import bs_roformer, lib, mdx23c, ops, uvr5
+    from oracle import uvr5_wave_oracle as W
+    lib.init().evk_set_precise(0)
+    dt = getattr(torch, a.precision)
+    agg = {"value": 0.1, "split_bin": 85, "aggr_correction": None}
+    if a.net == "mdx23c":
+        cfg = MX.config({})
+        net = mdx23c.MDX23C(cfg).to("cuda").load_state_dict(MX.init_params(MX.param_spec(cfg), 321))
+        mix = BR.make_audio(7, (2, 7938000))
+        c = cfg["audio"]["chunk_size"]
+        run = lambda: np.stack(list(bs_roformer.demix_track(net, mix, "cuda", a.max_chunks).values()))  # noqa: E731
+        batch = mix[:, :a.max_chunks * c].reshape(2, a.max_chunks, c).transpose(0, 1).contiguous().cuda()
+        forward = lambda: net.forward(batch)                                                        # noqa: E731
+    else:
+        if a.net == "vr":
+            net = uvr5.get_nets_model(1344).to("cuda").load_state_dict(O.init_params(O.param_spec(61968), 31))
+        else:
+            nout = 48 if a.net == "deecho" else 64
+            net = uvr5.CascadedNet(1344, nout).to("cuda").load_state_dict(E.init_params(E.param_spec(1344, nout), 51))
+        if a.wave:
+            gold = torch.load(os.path.join(ROOT, "tests", "golden", "uvr5_wave.pt"), weights_only=False)
+            param = gold["vr" if a.net == "vr" else "echo"]["param"]
+            mix = W.make_clip(7, 180.0, extra=0)
+            run = lambda: np.stack(uvr5.separate_wave(mix, net, param, 10, bool(a.tta), max_windows=a.max_windows))  # noqa: E731
+        else:
+            spec = O.make_spec(7, 673, a.frames)
+            data = {"window_size": 512, "tta": bool(a.tta)}
+            run = lambda: uvr5.inference(spec, "cuda", net, agg, data, a.max_windows)[0]          # noqa: E731
+        wins = torch.rand(a.max_windows, 2, 673, 512, device="cuda", generator=torch.Generator("cuda").manual_seed(3))
+        forward = lambda: net.predict(wins, agg)                                                  # noqa: E731
+    res = dict(gpu=gpu_info(), net=a.net, wave=bool(a.wave), tta=bool(a.tta), precision=a.precision,
+               max_windows=a.max_windows, max_chunks=a.max_chunks)
+    arms = (("float32", None), (a.precision, dt))
+    outs, times, peak = {}, {n: [] for n, _ in arms}, {}
+    for name, ct in arms:                                 # first calls: packing, allocator growth, module loads
+        net.set_compute_type(ct)
+        outs[name] = run()
+    for _ in range(a.reps):
+        for name, ct in arms:
+            net.set_compute_type(ct)
+            torch.cuda.reset_peak_memory_stats()
+            times[name] += timed(run, 1)
+            peak[name] = max(peak.get(name, 0.0), torch.cuda.max_memory_allocated() / 2 ** 30)
+    for name, ct in arms:
+        net.set_compute_type(ct)
+        forward()
+        ops.profile_begin()
+        forward()
+        prof = ops.profile_end()
+        conv = [v for k, v in prof.items() if k.startswith("evk_conv2d_fwd")]
+        conv_ms, conv_fl = sum(v["ms"] for v in conv), sum(v["flops"] for v in conv)
+        tot = sum(v["ms"] for v in prof.values())
+        res[name] = dict(call_s=[round(t, 3) for t in times[name]], peak_mem_gib=round(peak[name], 2),
+                         forward_device_ms=round(tot, 2), conv_ms=round(conv_ms, 2), other_ms=round(tot - conv_ms, 2),
+                         conv_tflops=round(conv_fl / conv_ms / 1e9, 1),
+                         other_ms_by_family={k: round(v["ms"], 2) for k, v in sorted(prof.items(), key=lambda kv: -kv[1]["ms"])
+                                             if not k.startswith("evk_conv2d_fwd")})
+    ref, got = outs["float32"].astype(np.float64), outs[a.precision].astype(np.float64)
+    res[a.precision]["finite"] = bool(np.isfinite(got).all())
+    res[a.precision]["rel_l2_vs_float32"] = float(np.linalg.norm(got - ref) / np.linalg.norm(ref))
+    net.set_compute_type(None)
+    print(json.dumps(res))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--net", choices=("vr", "deecho", "dereverb", "roformer", "melroformer", "mdx23c"), default="vr")
@@ -553,9 +626,11 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--skip-torch", action="store_true")
     ap.add_argument("--precision", choices=("float32", "float16", "bfloat16"), default="float32",
-                    help="--net roformer / melroformer: also run this 16-bit compute type, alternating with the fp32 arm")
+                    help="also run this 16-bit compute type, alternating with the fp32 arm")
     ap.add_argument("--wave", action="store_true")
     a = ap.parse_args()
+    if a.precision != "float32" and a.net not in ("roformer", "melroformer"):
+        return h16_main(a)
     if a.wave:
         return wave_main(a)
     if a.net in ("roformer", "melroformer"):
